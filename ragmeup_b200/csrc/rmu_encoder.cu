@@ -463,7 +463,7 @@ struct rmu_encoder {
     int tok_cap = 0, seq_cap = 0;
     std::vector<void*> act_allocs;
     SplitOperand X, CTX, X1, FF, QKVP;   // QKVP: q (pre-scaled) | k | v as split planes [T, 3H]
-    float* PRE = nullptr;                 // fp32 pre-LayerNorm rows (hidden sizes the fused GEMM+LN kernel does not cover)
+    float* PRE = nullptr;                 // fp32 pre-LayerNorm rows: projection + bias + residual
     // staging of the *_host entry points: owned by host_mu alone (NOT part of the activation workspace, which a
     // concurrent device-pointer caller may free and re-allocate under mu)
     int *d_ids = nullptr, *d_typ = nullptr, *d_cu = nullptr;
@@ -589,43 +589,26 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
         }
         count_launch();
         RMU_CHECK_LAUNCH();
-        if (gemm_ln_supported(H)) {
-            // attention-output projection + residual + LayerNorm in one kernel (cluster of H / 128 CTAs per row block)
-            GemmLnParams gl{};
-            gl.M = T; gl.N = H; gl.K = H; gl.bias = L.bo; gl.res_hi = e->X.hi; gl.res_lo = e->X.lo;
-            gl.gamma = L.ln1g; gl.beta = L.ln1b; gl.eps = c.ln_eps; gl.out_hi = e->X1.hi; gl.out_lo = e->X1.lo;
-            rc = launch_gemm_ln(e->CTX, L.Wo, gl, e->sms, st);
-            if (rc != RMU_OK) return rc;
-        } else {
-            g = GemmParams{};
-            g.M = T; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE; g.res_hi = e->X.hi; g.res_lo = e->X.lo;
-            rc = launch_gemm(GEMM_BIAS_RESID_F32, e->CTX, L.Wo, g, e->sms, st);
-            if (rc != RMU_OK) return rc;
-            { ProfScope _ps(PROF_LN, st);
-            ln_kernel<<<tok_blocks, wpb * 32, 0, st>>>(e->PRE, T, H, L.ln1g, L.ln1b, c.ln_eps, e->X1.hi, e->X1.lo); }
-            count_launch();
-            RMU_CHECK_LAUNCH();
-        }
+        g = GemmParams{};
+        g.M = T; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE; g.res_hi = e->X.hi; g.res_lo = e->X.lo;
+        rc = launch_gemm(GEMM_BIAS_RESID_F32, e->CTX, L.Wo, g, e->sms, st);
+        if (rc != RMU_OK) return rc;
+        { ProfScope _ps(PROF_LN, st);
+        ln_kernel<<<tok_blocks, wpb * 32, 0, st>>>(e->PRE, T, H, L.ln1g, L.ln1b, c.ln_eps, e->X1.hi, e->X1.lo); }
+        count_launch();
+        RMU_CHECK_LAUNCH();
         g = GemmParams{};
         g.M = T; g.N = F; g.K = H; g.bias = L.b1; g.out_hi = e->FF.hi; g.out_lo = e->FF.lo;
         rc = launch_gemm(GEMM_BIAS_GELU_SPLIT, e->X1, L.W1, g, e->sms, st);
         if (rc != RMU_OK) return rc;
-        if (gemm_ln_supported(H)) {
-            GemmLnParams gl{};
-            gl.M = T; gl.N = H; gl.K = F; gl.bias = L.b2; gl.res_hi = e->X1.hi; gl.res_lo = e->X1.lo;
-            gl.gamma = L.ln2g; gl.beta = L.ln2b; gl.eps = c.ln_eps; gl.out_hi = e->X.hi; gl.out_lo = e->X.lo;
-            rc = launch_gemm_ln(e->FF, L.W2, gl, e->sms, st);
-            if (rc != RMU_OK) return rc;
-        } else {
-            g = GemmParams{};
-            g.M = T; g.N = H; g.K = F; g.bias = L.b2; g.out_f32 = e->PRE; g.res_hi = e->X1.hi; g.res_lo = e->X1.lo;
-            rc = launch_gemm(GEMM_BIAS_RESID_F32, e->FF, L.W2, g, e->sms, st);
-            if (rc != RMU_OK) return rc;
-            { ProfScope _ps(PROF_LN, st);
-            ln_kernel<<<tok_blocks, wpb * 32, 0, st>>>(e->PRE, T, H, L.ln2g, L.ln2b, c.ln_eps, e->X.hi, e->X.lo); }
-            count_launch();
-            RMU_CHECK_LAUNCH();
-        }
+        g = GemmParams{};
+        g.M = T; g.N = H; g.K = F; g.bias = L.b2; g.out_f32 = e->PRE; g.res_hi = e->X1.hi; g.res_lo = e->X1.lo;
+        rc = launch_gemm(GEMM_BIAS_RESID_F32, e->FF, L.W2, g, e->sms, st);
+        if (rc != RMU_OK) return rc;
+        { ProfScope _ps(PROF_LN, st);
+        ln_kernel<<<tok_blocks, wpb * 32, 0, st>>>(e->PRE, T, H, L.ln2g, L.ln2b, c.ln_eps, e->X.hi, e->X.lo); }
+        count_launch();
+        RMU_CHECK_LAUNCH();
     }
     return RMU_OK;
 }

@@ -1,6 +1,3 @@
-#include <algorithm>
-#include <cstdlib>
-
 #include "rmu_gemm.cuh"
 
 namespace rmu {
@@ -19,46 +16,22 @@ static int launch_mode(const SplitOperand& A, const SplitOperand& W, const GemmP
     auto kern = gemm_f16x3_kernel<MODE>;
     // the attribute is per device and the call is cheap: set it on every launch (one process may drive several GPUs)
     RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kGemmSmem)));
+    // output maps of exactly M rows (the TMA store clips the tail of the last row block): 128-row x 128-byte boxes
+    CUtensorMap tOa{}, tOb{};
+    int rc;
+    if (MODE == GEMM_BIAS_F32 || MODE == GEMM_BIAS_RESID_F32) {
+        rc = make_tmap_2d(&tOa, p.out_f32, static_cast<uint64_t>(p.M), static_cast<uint64_t>(p.N),
+                          static_cast<uint64_t>(p.N) * sizeof(float), 32, kGemmBM, 4);
+    } else {
+        const uint64_t pitch = static_cast<uint64_t>(p.N) * sizeof(__half);
+        rc = make_tmap_2d(&tOa, p.out_hi, static_cast<uint64_t>(p.M), static_cast<uint64_t>(p.N), pitch, 64, kGemmBM, 2);
+        if (rc == RMU_OK) rc = make_tmap_2d(&tOb, p.out_lo, static_cast<uint64_t>(p.M), static_cast<uint64_t>(p.N), pitch, 64, kGemmBM, 2);
+    }
+    if (rc != RMU_OK) return rc;
     const int tiles = ((p.M + kGemmBM - 1) / kGemmBM) * (p.N / kGemmBN);
     const int grid = tiles < sms ? tiles : sms;
     ProfScope _ps(PROF_GEMM, st);
-    kern<<<grid, kGemmThreads, kGemmSmem, st>>>(A.map_hi, A.map_lo, W.map_hi, W.map_lo, p);
-    count_launch();
-    RMU_CHECK_LAUNCH();
-    return RMU_OK;
-}
-
-bool gemm_ln_supported(int N) { return N % kGemmBN == 0 && N / kGemmBN <= kLnMaxCL; }
-
-int launch_gemm_ln(const SplitOperand& A, const SplitOperand& W, const GemmLnParams& p, int sms, cudaStream_t st) {
-    if (p.M <= 0) return RMU_OK;
-    if (!gemm_ln_supported(p.N) || p.K % kGemmBK != 0 || A.cols != p.K || W.cols != p.K || W.rows < p.N || A.rows < p.M) {
-        set_error("launch_gemm_ln: shape not supported (N % 128, N <= 1024, K % 64)");
-        return RMU_ERR_UNSUPPORTED;
-    }
-    const int CL = p.N / kGemmBN;
-    RMU_CUDA(cudaFuncSetAttribute(gemm_f16x3_ln_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kLnSmem)));
-    const int m_blks = (p.M + kGemmBM - 1) / kGemmBM;
-    cudaLaunchConfig_t cfg{};
-    cfg.blockDim = dim3(kGemmThreads);
-    cfg.dynamicSmemBytes = kLnSmem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = static_cast<unsigned>(CL);
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    // persistent clusters: only as many as the GPCs hold at once (clusters of CL CTAs with ~209 KB of shared memory each
-    // do not pack sms / CL of them), else a second wave of whole clusters doubles the tail
-    cfg.gridDim = dim3(static_cast<unsigned>(sms / CL * CL));
-    int active = 0;
-    RMU_CUDA(cudaOccupancyMaxActiveClusters(&active, gemm_f16x3_ln_kernel, &cfg));
-    const int clusters = std::max(1, std::min(m_blks, active > 0 ? active : sms / CL));
-    cfg.gridDim = dim3(static_cast<unsigned>(clusters * CL));
-    ProfScope _ps(PROF_GEMM, st);
-    RMU_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16x3_ln_kernel, A.map_hi, A.map_lo, W.map_hi, W.map_lo, p));
+    kern<<<grid, kGemmThreads, kGemmSmem, st>>>(A.map_hi, A.map_lo, W.map_hi, W.map_lo, tOa, tOb, p);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;

@@ -8,10 +8,19 @@
 // SPLIT fp16 PLANES, v = hi + lo with hi = fp16(v), lo = fp16(v - hi) (22 mantissa bits), and each
 // K step issues three wgmma f16 MMAs: hi*hi + lo*hi + hi*lo, fp32 accumulate in registers.
 //
-// Kernel shape: persistent, 1 CTA/SM, 288 threads = two consumer warpgroups (64 rows of the 128-row
-// tile each, 64 fp32 accumulators per thread) + one TMA producer warp.  128x128 output tiles, K blocks
-// of 64 (one 128-byte swizzled row per operand row), 3-stage smem ring (4 planes x 16 KB per stage).
-// The producer runs ahead into the next tile while the consumers write the epilogue of this one.
+// 128x128 output tiles, K blocks of 64 (one 128-byte swizzled row per operand row), 3-stage smem ring
+// (4 planes x 16 KB per stage) filled by TMA.
+//
+// E1 (gemm_f16x3_kernel) is persistent and PING-PONG scheduled: 1 CTA/SM, 384 threads = one producer
+// warpgroup (one elected lane issues the TMA loads, 40 registers per thread) + two consumer warpgroups
+// (232 registers per thread).  Each consumer warpgroup owns a whole tile (128 fp32 accumulators per
+// thread); consecutive tiles of a CTA alternate between the two.  A pair of named barriers hands the
+// tensor cores from one warpgroup to the other once all MMAs of a tile are issued, so one warpgroup
+// issues its MMAs while the other runs its epilogue (bias / GELU / split / residual and the TMA stores);
+// with K = 384 the mainloop is only 6 K blocks, so without the overlap the epilogue stalls the tensor cores.
+// The producer fills the ring in tile order; every consumer warpgroup steps its ring slot and phase past
+// the other warpgroup's K blocks.  The ordering barrier also keeps a warpgroup from waiting on a stage
+// whose barrier is more than one phase behind (the parity test would alias).
 #pragma once
 #include "rmu_common.h"
 #include "rmu_ptx.cuh"
@@ -22,9 +31,14 @@ constexpr int kGemmBM = 128, kGemmBN = 128, kGemmBK = 64;
 constexpr int kGemmStages = 3;
 constexpr int kGemmPlaneBytes = 128 * 128;                 // one plane of a stage: 128 rows x 128 B
 constexpr int kGemmStageBytes = 4 * kGemmPlaneBytes;       // A hi | A lo | W hi | W lo
-constexpr int kGemmConsumerWarps = 8;                      // two warpgroups
-constexpr int kGemmThreads = 32 * kGemmConsumerWarps + 32; // + TMA producer warp
-constexpr size_t kGemmSmem = static_cast<size_t>(kGemmStages) * kGemmStageBytes + 256 + 1024;
+constexpr int kGemmThreads = 3 * 128;                      // E1: producer warpgroup + two consumer warpgroups
+constexpr int kGemmProducerRegs = 40, kGemmConsumerRegs = 232;
+static_assert(128 * kGemmProducerRegs + 256 * kGemmConsumerRegs <= 65536, "register file");
+constexpr int kGemmOrderBar = 1;                           // named barriers 1, 2: "warpgroup w may issue its MMAs"
+constexpr int kGemmEpiBar = 3;                             // named barriers 3, 4: warpgroup w's staging buffer
+constexpr int kGemmStagingBytes = 128 * 128;               // per consumer warpgroup: one 128-row x 128-byte output box
+constexpr size_t kGemmSmem = static_cast<size_t>(kGemmStages) * kGemmStageBytes + 2 * kGemmStagingBytes + 256 + 1024;
+static_assert(kGemmSmem <= 232448, "shared memory budget");
 
 enum GemmMode {
     GEMM_BIAS_F32 = 0,        // out_f32 = acc + bias
@@ -84,276 +98,184 @@ __device__ __forceinline__ void gemm_produce(uint8_t* smem, uint64_t* full, uint
     }
 }
 
-// Consumer warpgroup `wg`: acc[64 x 128] of rows wg * 64 .. + 64 of the tile = sum over K of the three split products.
-// One MMA group stays in flight: the slot of the previous K block is handed back once its group has retired.
-__device__ __forceinline__ void gemm_mainloop(float (&acc)[64], uint8_t* smem, uint64_t* full, uint64_t* empty, int wg,
-                                              int k_blks, int& slot, uint32_t& phase) {
+__device__ __forceinline__ void ring_advance(int& slot, uint32_t& phase, int n) {
+    for (int i = 0; i < n; ++i)
+        if (++slot == kGemmStages) { slot = 0; phase ^= 1; }
+}
+
+// E1 consumer warpgroup: acc0 / acc1 = rows 0..63 / 64..127 of the tile, each the sum over K of the three split
+// products (per element: K steps in order, hi*hi, lo*hi, hi*lo).  One MMA group stays in flight: the slot of the
+// previous K block is handed back (one arrive per warp) once its group has retired.  Returns with the last group still
+// in flight; the caller retires it (wgmma_wait<0>) and hands back the returned slot.
+__device__ __forceinline__ int gemm_mainloop_tile(float (&acc0)[64], float (&acc1)[64], uint8_t* smem, uint64_t* full,
+                                                  uint64_t* empty, int k_blks, int& slot, uint32_t& phase) {
     const unsigned lane = lane_id();
     int prev = -1;
     for (int kb = 0; kb < k_blks; ++kb) {
         mbar_wait(&full[slot], phase);
         const uint32_t sbase = smem_u32(smem + slot * kGemmStageBytes);
-        const uint64_t dAh = wgmma_desc_sw128(sbase + wg * 64 * 128);
-        const uint64_t dAl = wgmma_desc_sw128(sbase + kGemmPlaneBytes + wg * 64 * 128);
+        const uint64_t dAh0 = wgmma_desc_sw128(sbase);
+        const uint64_t dAh1 = wgmma_desc_sw128(sbase + 64 * 128);
+        const uint64_t dAl0 = wgmma_desc_sw128(sbase + kGemmPlaneBytes);
+        const uint64_t dAl1 = wgmma_desc_sw128(sbase + kGemmPlaneBytes + 64 * 128);
         const uint64_t dWh = wgmma_desc_sw128(sbase + 2 * kGemmPlaneBytes);
         const uint64_t dWl = wgmma_desc_sw128(sbase + 3 * kGemmPlaneBytes);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < kGemmBK / 16; ++k) {
             const uint64_t off = static_cast<uint64_t>(k * 2);   // 16 halves = 32 B = 2 x 16 B units
-            wgmma_f16_n128(acc, dAh + off, dWh + off, (kb | k) != 0 ? 1u : 0u);
-            wgmma_f16_n128(acc, dAl + off, dWh + off, 1u);
-            wgmma_f16_n128(acc, dAh + off, dWl + off, 1u);
+            const uint32_t accum = (kb | k) != 0 ? 1u : 0u;
+            wgmma_f16_n128(acc0, dAh0 + off, dWh + off, accum);
+            wgmma_f16_n128(acc1, dAh1 + off, dWh + off, accum);
+            wgmma_f16_n128(acc0, dAl0 + off, dWh + off, 1u);
+            wgmma_f16_n128(acc1, dAl1 + off, dWh + off, 1u);
+            wgmma_f16_n128(acc0, dAh0 + off, dWl + off, 1u);
+            wgmma_f16_n128(acc1, dAh1 + off, dWl + off, 1u);
         }
         wgmma_commit();
         wgmma_wait<1>();
         if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
         prev = slot;
-        if (++slot == kGemmStages) { slot = 0; phase ^= 1; }
+        ring_advance(slot, phase, 1);
     }
-    wgmma_wait<0>();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[prev]);
+    return prev;
 }
 
 // Accumulator layout of wgmma m64nN (f32): thread t of the warpgroup holds rows 16 * (t / 32) + (t % 32) / 4 and + 8,
 // columns 8 j + 2 (t % 4) + {0, 1} for j < N / 8, as d[4 j + 2 h + e] (h = second row, e = second column).
+//
+// Epilogue: the output leaves through the warpgroup's 16 KB staging buffer in four 128-row x 128-byte boxes (split modes:
+// column half x plane; fp32 modes: column quarter), each written to shared memory in the 128-byte swizzle (conflict-free
+// for the accumulator layout) and stored by one TMA bulk store, which writes whole lines and clips the rows past M.
+// Direct 4-byte stores from the accumulator layout cover half a 32-byte sector each and took as long as the mainloop.
 template <int MODE>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_f16x3_kernel(const __grid_constant__ CUtensorMap tAh, const __grid_constant__ CUtensorMap tAl,
                   const __grid_constant__ CUtensorMap tWh, const __grid_constant__ CUtensorMap tWl,
+                  const __grid_constant__ CUtensorMap tOa, const __grid_constant__ CUtensorMap tOb,
                   const GemmParams p) {
+    constexpr bool kF32Out = MODE == GEMM_BIAS_F32 || MODE == GEMM_BIAS_RESID_F32;
+    constexpr int kJB = kF32Out ? 4 : 8;                       // 8-column groups per 128-byte box row
     extern __shared__ uint8_t gemm_smem_raw[];
     // 1024-byte alignment by OFFSET into the shared array (the 128-byte swizzle repeats every 1024 B)
     uint8_t* smem = gemm_smem_raw + ((1024u - (smem_u32(gemm_smem_raw) & 1023u)) & 1023u);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + kGemmStages * kGemmStageBytes);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + kGemmStages * kGemmStageBytes + 2 * kGemmStagingBytes);
     uint64_t* empty = full + kGemmStages;
 
     const int warp = threadIdx.x >> 5;
     const unsigned lane = lane_id();
     if (threadIdx.x == 0) {
-        for (int i = 0; i < kGemmStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kGemmConsumerWarps); }
+        for (int i = 0; i < kGemmStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 4); }   // 4 warps release
         fence_mbar_init();
         prefetch_tmap(&tAh); prefetch_tmap(&tAl); prefetch_tmap(&tWh); prefetch_tmap(&tWl);
+        prefetch_tmap(&tOa);
+        if (!kF32Out) prefetch_tmap(&tOb);
     }
     __syncthreads();
 
     const int n_blks = p.N / kGemmBN;
     const int k_blks = p.K / kGemmBK;
     const int tiles = ((p.M + kGemmBM - 1) / kGemmBM) * n_blks;
+    const int my_tiles = tiles > static_cast<int>(blockIdx.x) ? (tiles - 1 - static_cast<int>(blockIdx.x)) / gridDim.x + 1 : 0;
     int slot = 0;
     uint32_t phase = 0;
 
-    if (warp == kGemmConsumerWarps) {
-        if (elect_one())
-            for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x)
+    if (warp < 4) {
+        setmaxnreg_dec<kGemmProducerRegs>();
+        if (warp == 0 && elect_one())
+            for (int t = 0; t < my_tiles; ++t) {
+                const int tile = blockIdx.x + t * gridDim.x;
                 gemm_produce(smem, full, empty, &tAh, &tAl, &tWh, &tWl, tile / n_blks, tile % n_blks, k_blks, slot, phase);
+            }
         return;
     }
+    setmaxnreg_inc<kGemmConsumerRegs>();
 
-    const int wg = warp >> 2;
-    const int rsub = (warp & 3) * 16 + static_cast<int>(lane >> 2);     // first of this thread's two rows in the 64
-    const int csub = 2 * static_cast<int>(lane & 3);                   // first of its column pairs in every 8 columns
-    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int wg = (warp >> 2) - 1;                                    // consumer warpgroup 0 / 1: local tiles wg, wg + 2, ..
+    const bool store_lead = (threadIdx.x & 127) == 0;                  // issues the warpgroup's TMA stores and waits for them
+    uint8_t* staging = smem + kGemmStages * kGemmStageBytes + wg * kGemmStagingBytes;
+    const uint32_t staging_u32 = smem_u32(staging);
+    const int rsub = (warp & 3) * 16 + static_cast<int>(lane >> 2);     // first of this thread's two rows in each 64
+    const int q4 = static_cast<int>(lane & 3);
+    const int csub = 2 * q4;                                           // first of its column pairs in every 8 columns
+    ring_advance(slot, phase, wg * k_blks);
+    for (int t = wg; t < my_tiles; t += 2) {
+        const int tile = blockIdx.x + t * gridDim.x;
         const int mb = tile / n_blks, nb = tile % n_blks;
-        float acc[64];
-        gemm_mainloop(acc, smem, full, empty, wg, k_blks, slot, phase);
-        // ---- epilogue straight from the accumulator registers: a lane quad writes 8 consecutive columns of a row
-#pragma unroll
-        for (int j = 0; j < kGemmBN / 8; ++j) {
-            const int col = nb * kGemmBN + 8 * j + csub;
-            const float2 bia2 = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-            const float sc = (MODE == GEMM_BIAS_SPLIT_QSCALE && col < p.qcols) ? p.qscale : 1.0f;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int grow = mb * kGemmBM + wg * 64 + rsub + 8 * h;
-                if (grow >= p.M) continue;
-                float2 v = make_float2(acc[4 * j + 2 * h] + bia2.x, acc[4 * j + 2 * h + 1] + bia2.y);
-                const size_t o = static_cast<size_t>(grow) * p.N + col;
-                if (MODE == GEMM_BIAS_GELU_SPLIT) v = make_float2(gelu_erf(v.x), gelu_erf(v.y));
-                if (MODE == GEMM_BIAS_SPLIT_QSCALE) v = make_float2(v.x * sc, v.y * sc);
-                if (MODE == GEMM_BIAS_RESID_F32) {
-                    const float2 rh = __half22float2(*reinterpret_cast<const __half2*>(p.res_hi + o));
-                    const float2 rl = __half22float2(*reinterpret_cast<const __half2*>(p.res_lo + o));
-                    v = make_float2(v.x + (rh.x + rl.x), v.y + (rh.y + rl.y));
-                }
-                if (MODE == GEMM_BIAS_F32 || MODE == GEMM_BIAS_RESID_F32) {
-                    *reinterpret_cast<float2*>(p.out_f32 + o) = v;
-                } else {
-                    __half2 h2, l2;
-                    split_f16x2(v, h2, l2);
-                    *reinterpret_cast<__half2*>(p.out_hi + o) = h2;
-                    *reinterpret_cast<__half2*>(p.out_lo + o) = l2;
-                }
-            }
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// GEMM + bias + residual + LayerNorm -> split planes in ONE kernel (attention-output and FFN-output
-// projections of a post-LN BERT block: transformers BertSelfOutput / BertOutput, modeling_bert.py:287-357).
-//
-// A LayerNorm row spans the whole N = hidden, i.e. CL = N / 128 output tiles.  The CL CTAs of a thread-block
-// CLUSTER take the CL column tiles of the same 128-row block at the same time; every CTA forms (mean, M2) of its 128
-// columns of y = acc + bias + residual per row (per thread over its 32 columns, then over the lane quad that shares
-// the row, Chan's formula), publishes them into the shared memory of all CL CTAs (st.async whose completion bytes are
-// credited to the destination CTA's mbarrier), and each CTA combines the CL partials per row (exact two-pass
-// statistics, no E[x^2] - E[x]^2 cancellation).  y never leaves the registers: compared with GEMM(RESID_F32) +
-// ln_kernel this removes one fp32 write and one fp32 read of [M, N] and a launch per LayerNorm.
-// Double-buffered statistics: a CTA writes buffer b for row block i + 2 only after it has received every peer's
-// partials of block i + 1, which each peer row sends after it has read its block-i statistics.
-// ---------------------------------------------------------------------------------------------------
-struct GemmLnParams {
-    int M, N, K;
-    const float* bias;                            // [N]
-    const __half* res_hi; const __half* res_lo;   // [M, N] residual stream (planes)
-    const float* gamma; const float* beta;        // [N]
-    float eps;
-    __half* out_hi; __half* out_lo;               // [M, N] LayerNorm output (planes)
-};
-
-constexpr int kLnMaxCL = 8;                       // hidden <= 1024 (portable cluster size)
-constexpr size_t kLnStatsBytes = 2ull * kLnMaxCL * kGemmBM * sizeof(float2);
-constexpr size_t kLnSmem = static_cast<size_t>(kGemmStages) * kGemmStageBytes + kLnStatsBytes + 256 + 1024;
-static_assert(kLnSmem <= 232448, "shared memory budget");
-
-static __global__ void __launch_bounds__(kGemmThreads, 1)   // static: only rmu_gemm.cu launches it
-gemm_f16x3_ln_kernel(const __grid_constant__ CUtensorMap tAh, const __grid_constant__ CUtensorMap tAl,
-                     const __grid_constant__ CUtensorMap tWh, const __grid_constant__ CUtensorMap tWl,
-                     const GemmLnParams p) {
-    extern __shared__ uint8_t gemm_smem_raw[];
-    uint8_t* smem = gemm_smem_raw + ((1024u - (smem_u32(gemm_smem_raw) & 1023u)) & 1023u);
-    float2* stats = reinterpret_cast<float2*>(smem + kGemmStages * kGemmStageBytes);        // [2][kLnMaxCL][128]
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + kGemmStages * kGemmStageBytes + kLnStatsBytes);
-    uint64_t* empty = full + kGemmStages;
-    uint64_t* stat_full = empty + kGemmStages;                                                // [2]
-
-    const int warp = threadIdx.x >> 5;
-    const unsigned lane = lane_id();
-    const uint32_t CL = cluster_nctarank();
-    const uint32_t rank = cluster_ctarank();
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < kGemmStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kGemmConsumerWarps); }
-        for (int i = 0; i < 2; ++i) mbar_init(&stat_full[i], 1);   // armed per row block with the bytes of all CL partials
-        fence_mbar_init();
-        prefetch_tmap(&tAh); prefetch_tmap(&tAl); prefetch_tmap(&tWh); prefetch_tmap(&tWl);
-    }
-    cluster_sync_all();                           // every CTA's barriers exist before any remote arrive
-
-    const int m_blks = (p.M + kGemmBM - 1) / kGemmBM;
-    const int k_blks = p.K / kGemmBK;
-    const int cluster_id = blockIdx.x / CL, n_clusters = gridDim.x / CL;
-    const int nb = static_cast<int>(rank);        // this CTA's column tile of every row block
-    int slot = 0;
-    uint32_t phase = 0;
-
-    if (warp == kGemmConsumerWarps) {
-        if (elect_one())
-            for (int mb = cluster_id; mb < m_blks; mb += n_clusters)
-                gemm_produce(smem, full, empty, &tAh, &tAl, &tWh, &tWl, mb, nb, k_blks, slot, phase);
+        float acc[2][64];
+        if (t > 0) bar_sync_named(kGemmOrderBar + wg, 256);           // the other warpgroup has issued tile t - 1
+        const int last = gemm_mainloop_tile(acc[0], acc[1], smem, full, empty, k_blks, slot, phase);
+        // every MMA of this tile is issued: the other warpgroup may queue its own behind them
+        if (t + 1 < my_tiles) bar_arrive_named(kGemmOrderBar + (wg ^ 1), 256);
+        wgmma_wait<0>();
         __syncwarp();
-    } else {
-        const int wg = warp >> 2;
-        const int trow = wg * 64 + (warp & 3) * 16 + static_cast<int>(lane >> 2);   // this thread's first row of the tile
-        const int csub = 2 * static_cast<int>(lane & 3);
-        const bool leader = (lane & 3) == 0;      // the quad leader publishes and reads the row's statistics
-        const float inv_n = 1.0f / static_cast<float>(p.N);
-        int i = 0;
-        for (int mb = cluster_id; mb < m_blks; mb += n_clusters, ++i) {
-            float acc[64];
-            gemm_mainloop(acc, smem, full, empty, wg, k_blks, slot, phase);
-            // ---- y = acc + bias + residual, statistics of this thread's 32 columns of each of its two rows
-            float mean[2], m2[2];
+        if (lane == 0) mbar_arrive(&empty[last]);
+        ring_advance(slot, phase, k_blks);                             // the other warpgroup's tile t + 1
+        // ---- epilogue per column block of 32 (fp32) / 64 (split) columns: values into registers, then one 128-row x
+        // 128-byte box per output plane through the staging buffer
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int grow = mb * kGemmBM + trow + 8 * h;
-                float s = 0.f;
+        for (int c = 0; c < kGemmBN / 8 / kJB; ++c) {
+            uint32_t w[2][2][kJB][2];                                  // [r][h][jj]: fp32 (x, y) or (hi pair, lo pair)
 #pragma unroll
-                for (int j = 0; j < kGemmBN / 8; ++j) {
+            for (int r = 0; r < 2; ++r) {
+#pragma unroll
+                for (int jj = 0; jj < kJB; ++jj) {
+                    const int j = kJB * c + jj;
                     const int col = nb * kGemmBN + 8 * j + csub;
                     const float2 bia2 = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-                    float2 r = make_float2(0.f, 0.f);
-                    if (grow < p.M) {
-                        const size_t o = static_cast<size_t>(grow) * p.N + col;
-                        const float2 rh = __half22float2(*reinterpret_cast<const __half2*>(p.res_hi + o));
-                        const float2 rl = __half22float2(*reinterpret_cast<const __half2*>(p.res_lo + o));
-                        r = make_float2(rh.x + rl.x, rh.y + rl.y);
-                    }
-                    float& y0 = acc[4 * j + 2 * h];
-                    float& y1 = acc[4 * j + 2 * h + 1];
-                    y0 = y0 + bia2.x + r.x;
-                    y1 = y1 + bia2.y + r.y;
-                    s += y0 + y1;
-                }
-                float mu = s * (1.0f / 32.0f), q = 0.f;
+                    const float sc = (MODE == GEMM_BIAS_SPLIT_QSCALE && col < p.qcols) ? p.qscale : 1.0f;
 #pragma unroll
-                for (int j = 0; j < kGemmBN / 8; ++j) {
-                    const float d0 = acc[4 * j + 2 * h] - mu, d1 = acc[4 * j + 2 * h + 1] - mu;
-                    q = fmaf(d0, d0, fmaf(d1, d1, q));
-                }
-                // merge over the four lanes of the quad (equal counts: 32, then 64 columns)
-#pragma unroll
-                for (int o = 1, n = 32; o < 4; o <<= 1, n <<= 1) {
-                    const float mo = __shfl_xor_sync(0xffffffffu, mu, o), qo = __shfl_xor_sync(0xffffffffu, q, o);
-                    const float d = mo - mu;
-                    q = q + qo + d * d * (0.5f * static_cast<float>(n));
-                    mu = 0.5f * (mu + mo);
-                }
-                mean[h] = mu;
-                m2[h] = q;
-            }
-            // ---- exchange (mean, M2) of (row, rank) with every CTA of the cluster
-            const int sbuf = i & 1;
-            const uint32_t use = static_cast<uint32_t>(i >> 1);
-            if (threadIdx.x == 0) mbar_arrive_expect_tx(&stat_full[sbuf], static_cast<uint32_t>(CL * kGemmBM * sizeof(float2)));
-            if (leader) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    float2* my = stats + (static_cast<size_t>(sbuf) * kLnMaxCL + rank) * kGemmBM + trow + 8 * h;
-                    for (uint32_t c = 0; c < CL; ++c) st_async_cluster_f2(my, &stat_full[sbuf], c, make_float2(mean[h], m2[h]));
-                }
-            }
-            mbar_wait(&stat_full[sbuf], use & 1);
-            float rmean[2], rstd[2];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                float mu = 0.f, M2 = 0.f;
-                if (leader) {
-                    const float2* st = stats + static_cast<size_t>(sbuf) * kLnMaxCL * kGemmBM + trow + 8 * h;
-                    for (uint32_t c = 0; c < CL; ++c) mu += st[c * kGemmBM].x;
-                    mu /= static_cast<float>(CL);
-                    for (uint32_t c = 0; c < CL; ++c) {
-                        const float2 s2 = st[c * kGemmBM];
-                        const float d = s2.x - mu;
-                        M2 += s2.y + static_cast<float>(kGemmBN) * d * d;
+                    for (int h = 0; h < 2; ++h) {
+                        const int grow = mb * kGemmBM + r * 64 + rsub + 8 * h;
+                        float2 v = make_float2(acc[r][4 * j + 2 * h] + bia2.x, acc[r][4 * j + 2 * h + 1] + bia2.y);
+                        if (MODE == GEMM_BIAS_GELU_SPLIT) v = make_float2(gelu_erf(v.x), gelu_erf(v.y));
+                        if (MODE == GEMM_BIAS_SPLIT_QSCALE) v = make_float2(v.x * sc, v.y * sc);
+                        if (MODE == GEMM_BIAS_RESID_F32 && grow < p.M) {
+                            const size_t o = static_cast<size_t>(grow) * p.N + col;
+                            const float2 rh = __half22float2(*reinterpret_cast<const __half2*>(p.res_hi + o));
+                            const float2 rl = __half22float2(*reinterpret_cast<const __half2*>(p.res_lo + o));
+                            v = make_float2(v.x + (rh.x + rl.x), v.y + (rh.y + rl.y));
+                        }
+                        if (kF32Out) {
+                            w[r][h][jj][0] = __float_as_uint(v.x);
+                            w[r][h][jj][1] = __float_as_uint(v.y);
+                        } else {
+                            __half2 h2, l2;
+                            split_f16x2(v, h2, l2);
+                            w[r][h][jj][0] = *reinterpret_cast<const uint32_t*>(&h2);
+                            w[r][h][jj][1] = *reinterpret_cast<const uint32_t*>(&l2);
+                        }
                     }
                 }
-                rmean[h] = __shfl_sync(0xffffffffu, mu, lane & ~3u);
-                rstd[h] = 1.0f / sqrtf(__shfl_sync(0xffffffffu, M2, lane & ~3u) * inv_n + p.eps);
             }
-            // ---- normalise, gamma / beta, split, plane stores
 #pragma unroll
-            for (int j = 0; j < kGemmBN / 8; ++j) {
-                const int col = nb * kGemmBN + 8 * j + csub;
-                const float2 g2 = __ldg(reinterpret_cast<const float2*>(p.gamma + col));
-                const float2 b2 = __ldg(reinterpret_cast<const float2*>(p.beta + col));
+            for (int pl = 0; pl < (kF32Out ? 1 : 2); ++pl) {
+                if (store_lead) bulk_wait_read<0>();                  // the previous box has left the staging buffer
+                bar_sync_named(kGemmEpiBar + wg, 128);
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int grow = mb * kGemmBM + trow + 8 * h;
-                    if (grow >= p.M) continue;
-                    const float2 v = make_float2(fmaf((acc[4 * j + 2 * h] - rmean[h]) * rstd[h], g2.x, b2.x),
-                                                 fmaf((acc[4 * j + 2 * h + 1] - rmean[h]) * rstd[h], g2.y, b2.y));
-                    __half2 h2, l2;
-                    split_f16x2(v, h2, l2);
-                    const size_t o = static_cast<size_t>(grow) * p.N + col;
-                    *reinterpret_cast<__half2*>(p.out_hi + o) = h2;
-                    *reinterpret_cast<__half2*>(p.out_lo + o) = l2;
+                for (int r = 0; r < 2; ++r) {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = r * 64 + rsub + 8 * h;
+                        const uint32_t rbase = staging_u32 + row * 128;   // 16-byte chunk k of the row lives at k ^ (row & 7)
+                        const int sw = row & 7;
+#pragma unroll
+                        for (int jj = 0; jj < kJB; ++jj) {
+                            if (kF32Out) st_shared_v2(rbase + (((2 * jj + (q4 >> 1)) ^ sw) << 4) + 8 * (q4 & 1), w[r][h][jj][0], w[r][h][jj][1]);
+                            else st_shared_b32(rbase + ((jj ^ sw) << 4) + 4 * q4, w[r][h][jj][pl]);
+                        }
+                    }
+                }
+                fence_proxy_async_smem();                              // generic-proxy writes -> visible to the TMA store
+                bar_sync_named(kGemmEpiBar + wg, 128);
+                if (store_lead) {
+                    tma_store_2d(pl ? &tOb : &tOa, staging, nb * kGemmBN + 8 * kJB * c, mb * kGemmBM);
+                    bulk_commit();
                 }
             }
         }
     }
-    cluster_sync_all();                           // no CTA leaves while a peer could still address its shared memory
+    if (store_lead) bulk_wait<0>();                                    // the stores have completed before the CTA retires
 }
 
 // A K-major fp16 operand carried as two planes, with the TMA maps of both (box {64 halves, 128 rows}, SWIZZLE_128B)
@@ -368,8 +290,5 @@ struct SplitOperand {
 int make_split_operand(SplitOperand* op, __half* hi, __half* lo, int64_t rows, int cols);
 // C = A * W^T with the epilogue `mode`; A rows used = p.M (<= A.rows)
 int launch_gemm(int mode, const SplitOperand& A, const SplitOperand& W, const GemmParams& p, int sms, cudaStream_t st);
-// fused GEMM + bias + residual + LayerNorm -> planes; N = 128 * CL with CL <= 8 (gemm_ln_supported)
-bool gemm_ln_supported(int N);
-int launch_gemm_ln(const SplitOperand& A, const SplitOperand& W, const GemmLnParams& p, int sms, cudaStream_t st);
 
 }  // namespace rmu

@@ -1,6 +1,6 @@
 // Thin inline-PTX wrappers for the sm_90a features the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with operands in shared memory and the
-// accumulator in registers), plus the wgmma shared-memory descriptor encoding.
+// mbarrier, TMA (cp.async.bulk.tensor loads and stores), named barriers, setmaxnreg, wgmma (warpgroup MMA with operands
+// in shared memory and the accumulator in registers), plus the wgmma shared-memory descriptor encoding.
 // Everything here is hand-written for sm_90a; there is no other target.
 #pragma once
 #include <cuda_runtime.h>
@@ -80,10 +80,39 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, in
         "l"(policy)
         : "memory");
 }
+// 2-D tiled tensor store: the box at `smem_src` (written in the map's swizzle) goes to global memory, rows and columns
+// past the tensor's extent are clipped.  Tracked by the issuing thread's bulk async-groups.
+__device__ __forceinline__ void tma_store_2d(const void* tmap, const void* smem_src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still READ their shared-memory source (the buffer may be rewritten)
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's bulk groups are incomplete (their global writes included)
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_v2(uint32_t addr, uint32_t x, uint32_t y) {
+    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(x), "r"(y) : "memory");
+}
 // named barriers over a subset of the CTA's warps
 __device__ __forceinline__ void bar_sync_named(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// signal a named barrier without waiting on it (the waiting side uses bar_sync_named with the same count)
+__device__ __forceinline__ void bar_arrive_named(int id, int nthreads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+// per-thread register budget of the calling warpgroup (all 128 threads execute it; N is a multiple of 8 in [24, 256])
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 // barrier + OR-reduction of a predicate over the participating threads
 __device__ __forceinline__ bool bar_red_or_named(int id, int nthreads, bool pred) {
     uint32_t r;
@@ -96,34 +125,6 @@ __device__ __forceinline__ bool bar_red_or_named(int id, int nthreads, bool pred
         : "r"(id), "r"(nthreads), "r"(static_cast<uint32_t>(pred))
         : "memory");
     return r != 0;
-}
-
-// ---------------------------------------------------------------- clusters
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ uint32_t cluster_nctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
-    return r;
-}
-// every thread of every CTA of the cluster
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// 8-byte asynchronous store into CTA `cta`'s shared memory whose completion is credited (8 bytes of transaction
-// count) to the mbarrier at `bar`'s offset in THAT CTA: data and signal travel together (the waiter sees the data once
-// the barrier phase completes, as with TMA)
-__device__ __forceinline__ void st_async_cluster_f2(float2* p, uint64_t* bar, uint32_t cta, float2 v) {
-    asm volatile(
-        "{\n\t.reg .b32 ra, rb;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %2;\n\t"
-        "mapa.shared::cluster.u32 rb, %1, %2;\n\t"
-        "st.async.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [ra], {%3, %4}, [rb];\n\t}"
-        ::"r"(smem_u32(p)), "r"(smem_u32(bar)), "r"(cta), "f"(v.x), "f"(v.y)
-        : "memory");
 }
 
 // ---------------------------------------------------------------- wgmma
