@@ -189,6 +189,33 @@ int rmu_encoder_classify_host(rmu_encoder* enc, const int32_t* ids_h, const int3
                               const int32_t* cu_seqlens_h, int B, int total_tokens, int max_seqlen, float* out_h,
                               void* stream);
 
+/* ------------------------------------------------------------------ kernel-level test entry points,
+ * not part of the product path.  Each runs ONE encoder kernel through the launcher the encoder itself uses, on
+ * split fp16 planes the caller owns (v = hi + lo, hi = fp16(v), lo = fp16(v - hi); planes are fp16 bit patterns,
+ * row-major, device pointers); they allocate nothing.  Shapes the kernels do not take return RMU_ERR_UNSUPPORTED
+ * before any CUDA call.  For tests that compare each kernel with a high-precision reference. */
+#define RMU_GEMM_BIAS_F32 0           /* out_f32 = A W^T + bias                                         */
+#define RMU_GEMM_BIAS_GELU_SPLIT 1    /* out planes = split(gelu_erf(A W^T + bias))                     */
+#define RMU_GEMM_BIAS_RESID_F32 2     /* out_f32 = A W^T + bias + (res_hi + res_lo)                     */
+#define RMU_GEMM_BIAS_SPLIT_QSCALE 3  /* out planes = split((A W^T + bias) * (col < qcols ? qscale : 1)) */
+
+/* For tests: E1 on A [a_rows, K] (rows M..a_rows are read by the TMA loads but never reach the output) and
+ * W [N, K]; bias [N], res [M, N], out [M, N].  N % 128 == 0, K % 64 == 0, a_rows >= M.  max_ctas caps the
+ * persistent grid (0 = the device's SM count), so a small problem can put many tiles through one CTA. */
+int rmu_debug_gemm(int mode, const uint16_t* a_hi, const uint16_t* a_lo, int64_t a_rows, const uint16_t* w_hi,
+                   const uint16_t* w_lo, int M, int N, int K, const float* bias, const uint16_t* res_hi,
+                   const uint16_t* res_lo, int qcols, float qscale, int max_ctas, float* out_f32, uint16_t* out_hi,
+                   uint16_t* out_lo, void* stream);
+/* For tests: E2 on the QKV planes [T, 3H] of a ragged batch (q | k | v, q pre-scaled by log2(e) / sqrt(d_h) as the
+ * QKV epilogue leaves it), cu_seqlens [B+1] int32 -> ctx planes [T, H].  d_h = H / heads is 32 or 64; warps is 10,
+ * or 5 with d_h = 32. */
+int rmu_debug_attention(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu_seqlens, int B, int H,
+                        int heads, int max_seqlen, int warps, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream);
+/* For tests: E3 ln_kernel, LayerNorm of pre [T, H] fp32 (biased variance, eps inside the sqrt) -> planes [T, H].
+ * H % 128 == 0, H <= 1024. */
+int rmu_debug_layernorm(const float* pre, int T, int H, const float* gamma, const float* beta, float eps,
+                        uint16_t* out_hi, uint16_t* out_lo, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

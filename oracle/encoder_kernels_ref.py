@@ -1,0 +1,106 @@
+"""Oracle: float64 references of the encoder kernels one at a time, on the split fp16 planes they read.
+TEST INFRASTRUCTURE ONLY (see ``oracle/__init__.py``).
+
+The encoder carries every activation and weight as two fp16 planes, v = hi + lo with hi = fp16_rn(v) and
+lo = fp16_rn(v - hi) (``csrc/rmu_gemm.cuh``).  Each reference below takes the planes the kernel actually read and
+evaluates hi + lo in float64 (torch, on whichever device the inputs live), so what is left between kernel and
+reference is the kernel's own arithmetic:
+
+* ``gemm_ref``: E1 ``gemm_f16x3_kernel``, sum_k (ah wh + al wh + ah wl) and the four epilogues;
+* ``attention_ref``: E2 ``attention_planes_kernel``, base-2 softmax over the keys of the same sequence;
+* ``layernorm_ref``: E3 ``ln_kernel``, two-pass LayerNorm, biased variance, eps inside the square root.
+"""
+from __future__ import annotations
+
+import math
+
+import numpy as np
+import torch
+
+# mode ids of rmu_debug_gemm (include/ragmeup_b200.h)
+GEMM_BIAS_F32, GEMM_BIAS_GELU_SPLIT, GEMM_BIAS_RESID_F32, GEMM_BIAS_SPLIT_QSCALE = 0, 1, 2, 3
+
+
+def split_f16(v) -> tuple[np.ndarray, np.ndarray]:
+    """float32 v -> (hi, lo) fp16 planes as the kernels make them: hi = fp16_rn(v), lo = fp16_rn(v - hi).
+    v - hi is exact in float32; below |v| ~ 0.125 lo is an fp16 subnormal."""
+    v = np.asarray(v, dtype=np.float32)
+    hi = v.astype(np.float16)
+    lo = (v - hi.astype(np.float32)).astype(np.float16)
+    return hi, lo
+
+
+def ulp_f16(hi) -> np.ndarray:
+    """float64 spacing of the fp16 grid at |hi| (2^-24 in the subnormal range); lo of a correct split is at most
+    half of it"""
+    _, e = np.frexp(np.asarray(hi, np.float64))          # |hi| in [2^(e-1), 2^e)
+    return np.exp2(np.maximum(e - 11, -24).astype(np.float64))
+
+
+def join(hi, lo) -> np.ndarray:
+    """hi + lo in float64"""
+    return np.asarray(hi, np.float64) + np.asarray(lo, np.float64)
+
+
+def _f64(x) -> torch.Tensor:
+    """planes / fp32 arrays (numpy or torch, any device) -> float64 torch tensor on the same device"""
+    return x.to(torch.float64) if isinstance(x, torch.Tensor) else torch.from_numpy(np.asarray(x, np.float64))
+
+
+def gemm_ref(mode: int, a_hi, a_lo, w_hi, w_lo, bias, res_hi=None, res_lo=None, qcols: int = 0,
+             qscale: float = 1.0) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """E1 on A [M, K] and W [N, K] planes.  Returns (out, x, S): out [M, N] float64 after the epilogue of `mode`,
+    x = the pre-epilogue sum + bias (GELU's argument), and S_ij = sum_k |a_ik w_jk| for the error bound."""
+    ah, al, wh, wl = _f64(a_hi), _f64(a_lo), _f64(w_hi), _f64(w_lo)
+    acc = ah @ wh.T + al @ wh.T + ah @ wl.T          # the three products the kernel issues (no lo * lo)
+    S = (ah + al).abs() @ (wh + wl).abs().T
+    x = acc + _f64(bias)[None, :]
+    if mode == GEMM_BIAS_F32:
+        out = x
+    elif mode == GEMM_BIAS_GELU_SPLIT:
+        out = 0.5 * x * (1.0 + torch.special.erf(x / math.sqrt(2.0)))
+    elif mode == GEMM_BIAS_RESID_F32:
+        out = x + (_f64(res_hi) + _f64(res_lo))
+    elif mode == GEMM_BIAS_SPLIT_QSCALE:
+        sc = torch.ones(x.shape[1], dtype=torch.float64, device=x.device)
+        sc[:qcols] = float(np.float32(qscale))
+        out = x * sc[None, :]
+    else:
+        raise ValueError(mode)
+    return out, x, S
+
+
+def attention_ref(qkv_hi, qkv_lo, cu, heads: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """E2 on the QKV planes [T, 3H] (q | k | v, q pre-scaled by log2(e) / sqrt(d_h)) of the ragged batch `cu`.
+    Per sequence and head: s = q k^T, p = 2^(s - max s), ctx = p V / sum p, over that sequence's keys only.
+    Returns (ctx [T, H], A [T, heads]) with A = max over the row's keys of sum_d |q_d k_d|, the magnitude the
+    kernel's score rounding scales with."""
+    qkv = _f64(qkv_hi) + _f64(qkv_lo)
+    T, H3 = qkv.shape
+    H = H3 // 3
+    dh = H // heads
+    ctx = torch.zeros((T, H), dtype=torch.float64, device=qkv.device)
+    A = torch.zeros((T, heads), dtype=torch.float64, device=qkv.device)
+    cu = [int(c) for c in cu]
+    for b in range(len(cu) - 1):
+        t0, t1 = cu[b], cu[b + 1]
+        if t1 == t0:
+            continue
+        x = qkv[t0:t1].view(t1 - t0, 3, heads, dh).transpose(0, 2)      # [heads, 3, S, dh]
+        q, k, v = x[:, 0], x[:, 1], x[:, 2]
+        s = q @ k.transpose(1, 2)
+        p = torch.exp2(s - s.amax(2, keepdim=True))
+        ctx[t0:t1] = ((p @ v) / p.sum(2, keepdim=True)).transpose(0, 1).reshape(t1 - t0, H)
+        A[t0:t1] = (q.abs() @ k.abs().transpose(1, 2)).amax(2).T
+    return ctx, A
+
+
+def layernorm_ref(x, gamma, beta, eps: float) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """E3 on fp32 rows x [T, H]: two-pass mean / biased variance in float64, eps (as the fp32 the kernel gets) inside
+    the square root.  Returns (y, xhat, sigma) with sigma = sqrt(var + eps) per row."""
+    x = _f64(x)
+    mu = x.mean(1, keepdim=True)
+    var = ((x - mu) ** 2).mean(1, keepdim=True)
+    sigma = torch.sqrt(var + float(np.float32(eps)))
+    xhat = (x - mu) / sigma
+    return xhat * _f64(gamma)[None, :] + _f64(beta)[None, :], xhat, sigma

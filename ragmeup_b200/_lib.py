@@ -84,6 +84,13 @@ SIGNATURES = {
                                          C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "rmu_encoder_classify_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                             C.c_void_p, C.c_void_p]),
+    "rmu_debug_gemm": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                 C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_void_p,
+                                 C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_layernorm": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
+                                      C.c_void_p, C.c_void_p]),
 }
 
 

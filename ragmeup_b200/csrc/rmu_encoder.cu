@@ -442,6 +442,38 @@ __global__ void join_planes_kernel(const __half* __restrict__ hi, const __half* 
     if (i < n) out[i] = __half2float(hi[i]) + __half2float(lo[i]);
 }
 
+// E2 on the QKV planes [T, 3H] (q pre-scaled by log2(e) / sqrt(d_h)) of a ragged batch -> ctx planes [T, H].
+// warps = 10 (160-row CTAs), or 5 (80-row CTAs, four per SM) with d_h = 32.
+static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const int* cu, int B, int H, int heads,
+                            int max_seqlen, int warps, __half* ctx_hi, __half* ctx_lo, cudaStream_t st) {
+    const int DH = H / heads;
+    if (!(warps == kAttWarps || (warps == 5 && DH == 32))) { set_error("attention: warps must be 10, or 5 with head_dim 32"); return RMU_ERR_ARG; }
+    ProfScope _ps(PROF_ATTN, st);
+    dim3 pg(static_cast<unsigned>(heads), static_cast<unsigned>(B), static_cast<unsigned>((max_seqlen + warps * 16 - 1) / (warps * 16)));
+    // keys resident per CTA: the whole (longest) sequence when it fits, else super-blocks of kKeySB
+    const int ksb = std::min(kKeySB, (max_seqlen + 31) / 32 * 32);
+    const size_t smem_max = 4 * sizeof(__half) * static_cast<size_t>(kKeySB) * (DH + 8);
+    const size_t smem = 4 * sizeof(__half) * static_cast<size_t>(ksb) * (DH + 8);
+    auto kern = DH == 32 ? (warps == 5 ? attention_planes_kernel<32, 4, 5> : attention_planes_kernel<32, 2>)
+                         : attention_planes_kernel<64, 1>;   // d_h = 64 needs > 96 registers
+    RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
+    kern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, cu, H, ksb, ctx_hi, ctx_lo);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// E3 ln_kernel: LayerNorm of T fp32 rows of H -> split planes.  8 warps (tokens) per block.
+static int launch_layernorm(const float* pre, int T, int H, const float* g, const float* b, float eps, __half* hi,
+                            __half* lo, cudaStream_t st) {
+    constexpr int wpb = 8;
+    ProfScope _ps(PROF_LN, st);
+    ln_kernel<<<static_cast<unsigned>((T + wpb - 1) / wpb), wpb * 32, 0, st>>>(pre, T, H, g, b, eps, hi, lo);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
 }  // namespace rmu
 
 using namespace rmu;
@@ -571,32 +603,17 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
         g.out_hi = e->QKVP.hi; g.out_lo = e->QKVP.lo; g.qcols = H; g.qscale = scale * 1.4426950408889634f;
         rc = launch_gemm(GEMM_BIAS_SPLIT_QSCALE, e->X, L.Wqkv, g, e->sms, st);
         if (rc != RMU_OK) return rc;
-        {
-            ProfScope _ps(PROF_ATTN, st);
-            // RMU_ATTN_WARPS = 5: 80-row CTAs, four per SM (same warps/SM, K/V staged twice per 147-token sequence)
-            static const int nw_env = [] { const char* e = getenv("RMU_ATTN_WARPS"); return e ? atoi(e) : kAttWarps; }();
-            const int nw = (nw_env == 5 && DH == 32) ? 5 : kAttWarps;
-            dim3 pg(static_cast<unsigned>(c.heads), static_cast<unsigned>(B),
-                    static_cast<unsigned>((max_seqlen + nw * 16 - 1) / (nw * 16)));
-            // keys resident per CTA: the whole (longest) sequence when it fits, else super-blocks of kKeySB
-            const int ksb = std::min(kKeySB, (max_seqlen + 31) / 32 * 32);
-            const size_t smem_max = 4 * sizeof(__half) * static_cast<size_t>(kKeySB) * (DH + 8);
-            const size_t smem = 4 * sizeof(__half) * static_cast<size_t>(ksb) * (DH + 8);
-            auto kern = DH == 32 ? (nw == 5 ? attention_planes_kernel<32, 4, 5> : attention_planes_kernel<32, 2>)
-                                 : attention_planes_kernel<64, 1>;   // d_h = 64 needs > 96 registers
-            RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
-            kern<<<pg, nw * 32, smem, st>>>(e->QKVP.hi, e->QKVP.lo, cu, H, ksb, e->CTX.hi, e->CTX.lo);
-        }
-        count_launch();
-        RMU_CHECK_LAUNCH();
+        // RMU_ATTN_WARPS = 5: 80-row CTAs, four per SM (same warps/SM, K/V staged twice per 147-token sequence)
+        static const int nw_env = [] { const char* e = getenv("RMU_ATTN_WARPS"); return e ? atoi(e) : kAttWarps; }();
+        rc = launch_attention(e->QKVP.hi, e->QKVP.lo, cu, B, H, c.heads, max_seqlen, (nw_env == 5 && DH == 32) ? 5 : kAttWarps,
+                              e->CTX.hi, e->CTX.lo, st);
+        if (rc != RMU_OK) return rc;
         g = GemmParams{};
         g.M = T; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE; g.res_hi = e->X.hi; g.res_lo = e->X.lo;
         rc = launch_gemm(GEMM_BIAS_RESID_F32, e->CTX, L.Wo, g, e->sms, st);
         if (rc != RMU_OK) return rc;
-        { ProfScope _ps(PROF_LN, st);
-        ln_kernel<<<tok_blocks, wpb * 32, 0, st>>>(e->PRE, T, H, L.ln1g, L.ln1b, c.ln_eps, e->X1.hi, e->X1.lo); }
-        count_launch();
-        RMU_CHECK_LAUNCH();
+        rc = launch_layernorm(e->PRE, T, H, L.ln1g, L.ln1b, c.ln_eps, e->X1.hi, e->X1.lo, st);
+        if (rc != RMU_OK) return rc;
         g = GemmParams{};
         g.M = T; g.N = F; g.K = H; g.bias = L.b1; g.out_hi = e->FF.hi; g.out_lo = e->FF.lo;
         rc = launch_gemm(GEMM_BIAS_GELU_SPLIT, e->X1, L.W1, g, e->sms, st);
@@ -605,10 +622,8 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
         g.M = T; g.N = H; g.K = F; g.bias = L.b2; g.out_f32 = e->PRE; g.res_hi = e->X1.hi; g.res_lo = e->X1.lo;
         rc = launch_gemm(GEMM_BIAS_RESID_F32, e->FF, L.W2, g, e->sms, st);
         if (rc != RMU_OK) return rc;
-        { ProfScope _ps(PROF_LN, st);
-        ln_kernel<<<tok_blocks, wpb * 32, 0, st>>>(e->PRE, T, H, L.ln2g, L.ln2b, c.ln_eps, e->X.hi, e->X.lo); }
-        count_launch();
-        RMU_CHECK_LAUNCH();
+        rc = launch_layernorm(e->PRE, T, H, L.ln2g, L.ln2b, c.ln_eps, e->X.hi, e->X.lo, st);
+        if (rc != RMU_OK) return rc;
     }
     return RMU_OK;
 }
@@ -797,6 +812,36 @@ int rmu_encoder_classify_host(rmu_encoder* e, const int32_t* ids_h, const int32_
     RMU_CUDA(cudaMemcpyAsync(out_h, e->d_out, static_cast<size_t>(B) * e->cfg.num_labels * sizeof(float), cudaMemcpyDeviceToHost, st));
     RMU_CUDA(cudaStreamSynchronize(st));
     return RMU_OK;
+}
+
+// ---- kernel-level test entry points: the launchers run_encoder uses, on caller-owned planes
+int rmu_debug_attention(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu, int B, int H, int heads,
+                        int max_seqlen, int warps, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream) {
+    if (!qkv_hi || !qkv_lo || !cu || !ctx_hi || !ctx_lo || B <= 0 || heads <= 0 || H <= 0 || max_seqlen <= 0) {
+        set_error("rmu_debug_attention: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H % heads != 0 || (H / heads != 32 && H / heads != 64)) {
+        set_error("rmu_debug_attention: head_dim must be 32 or 64");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_attention(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), cu, B, H,
+                            heads, max_seqlen, warps, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
+                            static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_layernorm(const float* pre, int T, int H, const float* gamma, const float* beta, float eps,
+                        uint16_t* out_hi, uint16_t* out_lo, void* stream) {
+    if (!pre || !gamma || !beta || !out_hi || !out_lo || T <= 0 || H <= 0) {
+        set_error("rmu_debug_layernorm: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H % 128 != 0 || H > 32 * kMaxPerLane) {
+        set_error("rmu_debug_layernorm: hidden must be a multiple of 128, at most 1024");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_layernorm(pre, T, H, gamma, beta, eps, reinterpret_cast<__half*>(out_hi), reinterpret_cast<__half*>(out_lo),
+                            static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -53,4 +53,43 @@ int launch_gemm(int mode, const SplitOperand& A, const SplitOperand& W, const Ge
     return RMU_ERR_ARG;
 }
 
+static_assert(RMU_GEMM_BIAS_F32 == GEMM_BIAS_F32 && RMU_GEMM_BIAS_GELU_SPLIT == GEMM_BIAS_GELU_SPLIT &&
+              RMU_GEMM_BIAS_RESID_F32 == GEMM_BIAS_RESID_F32 && RMU_GEMM_BIAS_SPLIT_QSCALE == GEMM_BIAS_SPLIT_QSCALE,
+              "the C ABI mode ids are the kernel's");
+
 }  // namespace rmu
+
+using namespace rmu;
+
+extern "C" int rmu_debug_gemm(int mode, const uint16_t* a_hi, const uint16_t* a_lo, int64_t a_rows, const uint16_t* w_hi,
+                              const uint16_t* w_lo, int M, int N, int K, const float* bias, const uint16_t* res_hi,
+                              const uint16_t* res_lo, int qcols, float qscale, int max_ctas, float* out_f32,
+                              uint16_t* out_hi, uint16_t* out_lo, void* stream) {
+    const bool f32_out = mode == GEMM_BIAS_F32 || mode == GEMM_BIAS_RESID_F32;
+    if (mode < GEMM_BIAS_F32 || mode > GEMM_BIAS_SPLIT_QSCALE || !a_hi || !a_lo || !w_hi || !w_lo || !bias ||
+        (f32_out ? !out_f32 : (!out_hi || !out_lo)) || (mode == GEMM_BIAS_RESID_F32 && (!res_hi || !res_lo)) ||
+        M <= 0 || N <= 0 || K <= 0 || max_ctas < 0) {
+        set_error("rmu_debug_gemm: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (N % kGemmBN != 0 || K % kGemmBK != 0 || a_rows < M) {
+        set_error("rmu_debug_gemm: shape not supported (N % 128, K % 64, a_rows >= M)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    SplitOperand A, W;
+    int rc = make_split_operand(&A, const_cast<__half*>(reinterpret_cast<const __half*>(a_hi)),
+                                const_cast<__half*>(reinterpret_cast<const __half*>(a_lo)), a_rows, K);
+    if (rc == RMU_OK)
+        rc = make_split_operand(&W, const_cast<__half*>(reinterpret_cast<const __half*>(w_hi)),
+                                const_cast<__half*>(reinterpret_cast<const __half*>(w_lo)), N, K);
+    if (rc != RMU_OK) return rc;
+    GemmParams p{};
+    p.M = M; p.N = N; p.K = K; p.bias = bias;
+    p.out_f32 = out_f32;
+    p.out_hi = reinterpret_cast<__half*>(out_hi); p.out_lo = reinterpret_cast<__half*>(out_lo);
+    p.res_hi = reinterpret_cast<const __half*>(res_hi); p.res_lo = reinterpret_cast<const __half*>(res_lo);
+    p.qcols = qcols; p.qscale = qscale;
+    const int sms = max_ctas > 0 ? max_ctas : device_sm_count();
+    if (sms <= 0) { set_error("rmu_debug_gemm: no CUDA device"); return RMU_ERR_CUDA; }
+    return launch_gemm(mode, A, W, p, sms, static_cast<cudaStream_t>(stream));
+}

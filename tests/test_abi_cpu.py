@@ -45,6 +45,48 @@ def test_loader_signatures_cover_header(built_lib):
     assert isinstance(_lib.launch_count(), int)
 
 
+def test_kernel_test_entry_points_reject_before_any_cuda_call(built_lib):
+    """rmu_debug_*: shapes the kernels do not take are refused before a tensor map is encoded or a kernel launched,
+    so these run without a device; the pointers are never dereferenced"""
+    from ragmeup_b200 import _lib
+    l = _lib.lib()
+    p = 1 << 20                                    # stand-in device address, never touched
+
+    def gemm(mode=0, a_rows=256, M=200, N=256, K=128, **kw):
+        a = dict(res=p, out_f32=p, out_hi=p, out_lo=p, max_ctas=0)
+        a.update(kw)
+        return l.rmu_debug_gemm(mode, p, p, a_rows, p, p, M, N, K, p, a["res"], a["res"], 0, 1.0, a["max_ctas"],
+                                a["out_f32"], a["out_hi"], a["out_lo"], None)
+
+    for mode in range(4):
+        assert gemm(mode, N=192) == -3                      # N % 128
+        assert gemm(mode, N=64) == -3
+        assert gemm(mode, K=96) == -3                       # K % 64
+        assert gemm(mode, K=32) == -3
+        assert gemm(mode, a_rows=199) == -3                 # A's tensor map must cover M rows
+    assert gemm(4) == -1 and gemm(-1) == -1                 # mode
+    assert gemm(0, M=0) == -1 and gemm(0, K=0) == -1 and gemm(0, max_ctas=-1) == -1
+    assert gemm(0, out_f32=None) == -1 and gemm(2, res=None) == -1
+    assert gemm(1, out_hi=None) == -1 and gemm(3, out_lo=None) == -1
+    assert gemm(0, N=100) == -3 and b"shape not supported" in l.rmu_last_error()
+
+    def attn(B=2, H=384, heads=12, max_seqlen=64, warps=10, cu=p):
+        return l.rmu_debug_attention(p, p, cu, B, H, heads, max_seqlen, warps, p, p, None)
+
+    assert attn(H=384, heads=8) == -3                       # d_h = 48
+    assert attn(H=384, heads=4) == -3                       # d_h = 96
+    assert attn(H=100, heads=3) == -3
+    assert attn(H=768, heads=12, warps=5) == -1             # the 5-warp variant is d_h = 32 only
+    assert attn(warps=7) == -1 and attn(warps=0) == -1
+    assert attn(B=0) == -1 and attn(max_seqlen=0) == -1 and attn(cu=None) == -1
+
+    def ln(T=9, H=384):
+        return l.rmu_debug_layernorm(p, T, H, p, p, 1e-12, p, p, None)
+
+    assert ln(H=320) == -3 and ln(H=1152) == -3 and ln(H=96) == -3
+    assert ln(T=0) == -1
+
+
 def test_product_fails_loudly_without_cuda(built_lib):
     import torch
     if torch.cuda.is_available():

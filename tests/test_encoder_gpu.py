@@ -84,3 +84,44 @@ def test_ragged_batch_vs_oracle_long_sequences(cuda):
     for b in (1, 3):
         one = enc.classify_tokens(ids[cu[b]:cu[b + 1]], typ[cu[b]:cu[b + 1]], np.array([0, lens[b]], np.int32), lens[b]).cpu()
         assert float((one[0] - lg[b]).abs().max()) < 1e-5
+
+
+def _oracle_hidden(w, cfg, ids, typ, lens):
+    cu = np.r_[0, np.cumsum(lens)]
+    S = max(lens)
+    I = np.zeros((len(lens), S), np.int64); M = np.zeros_like(I); T = np.zeros_like(I)
+    for b, n in enumerate(lens):
+        I[b, :n] = ids[cu[b]:cu[b + 1]]; T[b, :n] = typ[cu[b]:cu[b + 1]]; M[b, :n] = 1
+    with torch.no_grad():
+        h = bert_ref.bert_encoder_forward(w, bert_ref.BertCfg(**asdict(cfg)), torch.from_numpy(I), torch.from_numpy(M),
+                                          torch.from_numpy(T))
+    return h, torch.from_numpy(M)
+
+
+@pytest.mark.parametrize("preset,lens", [
+    # d_h = 64, K = 768 and 3072; 160-row blocks past the first, the 256-key super-block, a 1-token sequence
+    ("bge-base-en-v1.5", [512, 300, 257, 161, 33, 1]),
+    # K = 128 and 256 with 9 000 tokens: 213 QKV and 142 FFN-in tiles on 132 SMs, so both consumer warpgroups of a
+    # CTA run and the ring starts a tile at every slot
+    ("tiny", [int(n) for n in np.random.default_rng(11).integers(110, 129, 75)]),
+])
+def test_encoder_matches_oracle_at_scale(cuda, preset, lens):
+    from ragmeup_b200.encoder import BertEncoder
+    cfg = BertConfig(**asdict(PRESETS[preset][0]))
+    w = synthetic_bert_weights(cfg, seed=21, scale=1.0)
+    enc = BertEncoder(cfg, w, with_head=False)
+    rng = np.random.default_rng(12)
+    ids = np.concatenate([np.r_[101, rng.integers(104, cfg.vocab_size, max(n - 2, 0)), 102][:n] for n in lens]).astype(np.int32)
+    typ = np.concatenate([np.r_[np.zeros(n // 2, np.int32), np.ones(n - n // 2, np.int32)] for n in lens])
+    cu = np.r_[0, np.cumsum(lens)].astype(np.int32)
+    href, mask = _oracle_hidden(w, cfg, ids, typ, lens)
+    h = enc.hidden_tokens(ids, typ, cu, max(lens)).cpu()
+    flat = torch.cat([href[b, :n] for b, n in enumerate(lens)])
+    herr = float((h - flat).abs().max())
+    for mode in ("mean", "cls"):
+        e = enc.embed_tokens(ids, typ, cu, max(lens), mode, True).cpu()
+        want = bert_ref.l2_normalize(bert_ref.pool(href, mask, mode))
+        eerr = float((e - want).abs().max())
+        print(f"\n{preset} T={cu[-1]}: hidden max err {herr:.3g}, {mode} embedding max err {eerr:.3g}")
+        assert eerr < TOL
+    assert herr < 5e-3          # the hidden-state bound of test_embeddings_match_hf_golden
