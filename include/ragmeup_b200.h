@@ -87,7 +87,10 @@ int rmu_index_search(rmu_index* idx, const float* queries, int nq, int k, int64_
 /* same, HOST buffers in and out (H2D + D2H inside the call, synchronises `stream`) */
 int rmu_index_search_host(rmu_index* idx, const float* queries_h, int nq, int k, int64_t id_offset, int mode,
                           float* out_scores_h, int64_t* out_ids_h, void* stream);
-/* diagnostics: raw TF32 accumulators of the first 256 rows (one CTA-pair tile) for nq <= 64 queries, out [64, 256] */
+/* For tests: raw TF32 accumulators of the scan's first 256 rows (tiles 0 and 1, one per CTA) -> out [nq, 256] device
+ * fp32 (rows past size() are written as 0).  dim % 4 == 0 and nq <= the scan's query block at this dim (64 up to
+ * dim 384, 32 up to 768, 16 up to 1536); queries [nq, dim] device fp32, 16-byte aligned.  Shapes outside that, an
+ * empty index or a null pointer return RMU_ERR_ARG before any CUDA call. */
 int rmu_debug_scan_tile(rmu_index* idx, const float* queries, int nq, float* out, void* stream);
 /* rows[n] (int64, local row numbers) -> out [n, dim]; feeds MMR (langchain-milvus fetches the
  * fetch_k stored vectors the same way after col.search) */

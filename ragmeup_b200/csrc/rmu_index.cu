@@ -1053,10 +1053,11 @@ int rmu_index_search(rmu_index* idx, const float* queries, int nq, int k, int64_
     return RMU_OK;
 }
 
-// diagnostics: raw TF32 accumulators of the first 256 rows (tiles 0 and 1), out [nq <= 64, 256] device fp32
+// diagnostics: raw TF32 accumulators of the first 256 rows (tiles 0 and 1), out [nq, 256] device fp32, for any dim the
+// scan takes and nq up to its query block at that dim.  Every argument is checked before the first CUDA call.
 int rmu_debug_scan_tile(rmu_index* idx, const float* queries, int nq, float* out, void* stream) {
-    if (!idx || !queries || !out || nq <= 0 || nq > 64 || idx->n <= 0 || idx->dim % 4 != 0 || idx->dim > 384 ||
-        (reinterpret_cast<uintptr_t>(queries) & 15) != 0) {
+    if (!idx || !queries || !out || nq <= 0 || nq > kScanMaxQ || (reinterpret_cast<uintptr_t>(queries) & 15) != 0 ||
+        idx->n <= 0 || idx->dim % 4 != 0 || scan_block_cap(idx->dim) < nq) {
         set_error("rmu_debug_scan_tile: bad argument");
         return RMU_ERR_ARG;
     }
@@ -1068,7 +1069,7 @@ int rmu_debug_scan_tile(rmu_index* idx, const float* queries, int nq, float* out
     if (rc != RMU_OK) return rc;
     rc = ensure_corpus_tmap(idx);
     if (rc != RMU_OK) return rc;
-    ScanGeom geo = scan_geometry(idx->dim, 64);
+    ScanGeom geo = scan_geometry(idx->dim, kScanMaxQ);
     CUtensorMap tq;
     rc = make_tmap_2d(&tq, queries, static_cast<uint64_t>(nq), static_cast<uint64_t>(idx->dim),
                       static_cast<uint64_t>(idx->dim) * sizeof(float), 32, static_cast<uint32_t>(geo.nq), 4);

@@ -86,6 +86,17 @@ def test_kernel_test_entry_points_reject_before_any_cuda_call(built_lib):
     assert ln(H=320) == -3 and ln(H=1152) == -3 and ln(H=96) == -3
     assert ln(T=0) == -1
 
+    # the scan tile needs an index handle, which needs a device: what is checked here is refused before the handle is
+    # read (the dim / nq / empty-index refusals are in tests/test_index_kernels_gpu.py)
+    def tile(h=None, q=p, nq=16, out=p):
+        return l.rmu_debug_scan_tile(h, q, nq, out, None)
+
+    assert tile() == -1 and b"rmu_debug_scan_tile" in l.rmu_last_error()
+    fake = ctypes.c_void_p(p)                               # never dereferenced: every call below is refused first
+    assert tile(fake, q=None) == -1 and tile(fake, out=None) == -1
+    assert tile(fake, nq=0) == -1 and tile(fake, nq=-3) == -1 and tile(fake, nq=65) == -1
+    assert tile(fake, q=p + 4) == -1 and tile(fake, q=p + 8) == -1     # queries must be 16-byte aligned (TMA)
+
 
 def test_product_fails_loudly_without_cuda(built_lib):
     import torch
