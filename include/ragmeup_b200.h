@@ -108,13 +108,15 @@ int rmu_topk_merge_strided(const float* scores, const int64_t* ids, int64_t rank
 /* greedy maximal-marginal-relevance re-selection (langchain `maximal_marginal_relevance`,
  * used by as_retriever(search_type="mmr"), server/RAGHelper.py:497-499,533-535):
  * q [nq, dim], cand [nq, fetch_k, dim], n_cand[nq] valid candidates, out_sel [nq, k] int32
- * positions into the candidate list (-1 padded). */
+ * positions into the candidate list (-1 padded).  lambda_mult is a double, as the Python float langchain multiplies
+ * with: rounding 0.3 to float moves it by 1.2e-8, which is enough to flip a near-tie. */
 int rmu_mmr_select(const float* q, const float* cand, const int32_t* n_cand, int nq, int fetch_k, int dim,
-                   int k, float lambda_mult, int32_t* out_sel, void* stream);
+                   int k, double lambda_mult, int32_t* out_sel, void* stream);
 
 /* cosine DISTANCE (1 - cosine similarity) between consecutive rows of x [n, dim] -> out [n - 1] (device, float64):
  * the sentence-to-sentence distances of langchain_experimental's SemanticChunker, which the reference builds at
- * server/RAGHelper.py:329-341 and runs through text_splitter.split_documents (:368) (SURVEY.md §8 f4). */
+ * server/RAGHelper.py:329-341 and runs through text_splitter.split_documents (:368) (SURVEY.md §8 f4).  A zero row has
+ * similarity 0 (cosine_similarity maps NaN and +-inf to 0), so its distances are exactly 1. */
 int rmu_adjacent_cosine_distance(const float* x, int64_t n, int dim, double* out, void* stream);
 
 /* ------------------------------------------------------------------ BM25 sparse leg (SURVEY.md §8 f2)
@@ -134,7 +136,7 @@ int64_t rmu_bm25_size(const rmu_bm25* h);
 int64_t rmu_bm25_terms(const rmu_bm25* h);
 /* Q queries: terms of query i are q_terms[q_ptr[i] .. q_ptr[i+1]) (term ids in query order, repeats
  * kept); out_scores [Q, k] float64, out_ids [Q, k] int64 document numbers, -1 padded when the corpus
- * has fewer than k documents.  1 <= k <= 256.  Device pointers: */
+ * has fewer than k documents.  1 <= k <= 256; any Q >= 1 (batches past 65 535 queries run in chunks).  Device pointers: */
 int rmu_bm25_search(rmu_bm25* h, const int32_t* q_ptr, const int32_t* q_terms, int Q, int k, double* out_scores,
                     int64_t* out_ids, void* stream);
 /* the same with HOST buffers (copies + synchronise inside the call) */
@@ -218,6 +220,16 @@ int rmu_debug_attention(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const in
  * H % 128 == 0, H <= 1024. */
 int rmu_debug_layernorm(const float* pre, int T, int H, const float* gamma, const float* beta, float eps,
                         uint16_t* out_hi, uint16_t* out_lo, void* stream);
+/* For tests: the BM25 select stage alone (bm25_select_kernel rounds, through the launcher rmu_bm25_search uses) on
+ * caller-owned candidate lists: scores [Q, m] float64 and idx [Q, m] int32 document numbers (-1 = absent), each row
+ * ascending in document number among its present entries, as stage 1 leaves them.  Scores hold no NaN and no -0.0 (the
+ * scorer makes neither: every cell starts at +0.0, and +0.0 + -0.0 = +0.0).  Writes the top k of each row to out_scores
+ * [Q, k] float64 and out_ids [Q, k] int64, score descending, equal scores by larger document number, -1 padded.
+ * ws_scores and ws_idx are the ping-pong workspace, ws_elems elements each, at least 2 * Q * ceil(m / 4096) * k.  Null
+ * pointers, Q < 1, m < 1 or a smaller workspace return RMU_ERR_ARG, and k outside 1..256 or Q > 65 535
+ * RMU_ERR_UNSUPPORTED, before any CUDA call.  Allocates nothing. */
+int rmu_debug_bm25_select(const double* scores, const int32_t* idx, int Q, int m, int k, double* ws_scores,
+                          int32_t* ws_idx, int64_t ws_elems, double* out_scores, int64_t* out_ids, void* stream);
 
 #ifdef __cplusplus
 }

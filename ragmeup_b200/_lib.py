@@ -55,7 +55,7 @@ SIGNATURES = {
     "rmu_topk_merge_strided": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_adjacent_cosine_distance": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
-    "rmu_mmr_select": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+    "rmu_mmr_select": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double,
                                  C.c_void_p, C.c_void_p]),
     "rmu_bm25_create": (C.c_int, [C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_double, C.POINTER(C.c_void_p)]),
@@ -91,6 +91,8 @@ SIGNATURES = {
                                       C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_layernorm": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
                                       C.c_void_p, C.c_void_p]),
+    "rmu_debug_bm25_select": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                        C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 

@@ -28,6 +28,7 @@ constexpr int kBmThreads = 256;
 constexpr int kBmPer = kBmDocs / kBmThreads;   // consecutive items per thread in the order-preserving compaction
 constexpr int kBmTermBatch = 256;   // query terms whose range bounds are resident at a time
 constexpr int kBmMaxK = 256;
+constexpr int kBmMaxQ = 65535;      // queries per launch: the query index is blockIdx.y
 
 // order-preserving map double -> u64 (larger score = larger key); 0 is reserved for "absent"
 __device__ __forceinline__ uint64_t f64_key(double v) {
@@ -298,35 +299,50 @@ static int bm_upload(T** dst, const T* src_h, size_t n) {
     return RMU_OK;
 }
 
+// Select rounds over candidate lists in[Q, m] (ascending document order, index -1 = absent) down to the sorted top k in
+// out_scores / out_ids [Q, k].  Round r writes ws_s[r & 1] / ws_i[r & 1], each of Q * ceil(m / 4096) * k elements; every
+// round but the last hands its output to the next as input.  Q <= kBmMaxQ.
+static int bm25_select_rounds(const double* in_s, const int32_t* in_i, int Q, int m, int k, double* const ws_s[2],
+                              int32_t* const ws_i[2], double* out_scores, int64_t* out_ids, cudaStream_t st) {
+    for (int r = 0;; ++r) {
+        const int blocks = (m + kBmDocs - 1) / kBmDocs;
+        const int final_round = blocks == 1;
+        bm25_select_kernel<<<dim3(static_cast<unsigned>(blocks), static_cast<unsigned>(Q)), kBmThreads, 0, st>>>(
+            in_s, in_i, m, k, final_round, ws_s[r & 1], ws_i[r & 1], out_scores, reinterpret_cast<long long*>(out_ids));
+        count_launch();
+        RMU_CHECK_LAUNCH();
+        if (final_round) return RMU_OK;
+        in_s = ws_s[r & 1];
+        in_i = ws_i[r & 1];
+        m = blocks * k;
+    }
+}
+
 static int bm25_search_locked(rmu_bm25* h, const int32_t* q_ptr, const int32_t* q_terms, int Q, int k, double* out_scores,
                               int64_t* out_ids, cudaStream_t st) {
     const int nblk = static_cast<int>((h->n_docs + kBmDocs - 1) / kBmDocs);
-    const size_t need = static_cast<size_t>(Q) * nblk * k;
+    // the query index is gridDim.y (at most 65 535): larger batches run in chunks, each reusing the candidate buffers
+    const size_t need = static_cast<size_t>(std::min(Q, kBmMaxQ)) * nblk * k;
     for (int i = 0; i < 2; ++i) {
         int rc = h->cs[i].ensure(need * sizeof(double));
         if (rc == RMU_OK) rc = h->ci[i].ensure(need * sizeof(int32_t));
         if (rc != RMU_OK) return rc;
     }
-    {
-        ProfScope _ps(PROF_MISC, st);
-        bm25_score_kernel<<<dim3(static_cast<unsigned>(nblk), static_cast<unsigned>(Q)), kBmThreads, 0, st>>>(
-            h->post_ptr, h->post_doc, h->post_tf, h->den, h->idf, h->k1p1, h->n_docs, q_ptr, q_terms, k, h->cs[0].as<double>(),
-            h->ci[0].as<int32_t>());
+    // stage 1 writes buffer 0; the rounds then go 0 -> 1 -> 0 -> ...
+    double* const ws_s[2] = {h->cs[1].as<double>(), h->cs[0].as<double>()};
+    int32_t* const ws_i[2] = {h->ci[1].as<int32_t>(), h->ci[0].as<int32_t>()};
+    ProfScope _ps(PROF_MISC, st);
+    for (int q0 = 0; q0 < Q; q0 += kBmMaxQ) {
+        const int qc = std::min(kBmMaxQ, Q - q0);
+        bm25_score_kernel<<<dim3(static_cast<unsigned>(nblk), static_cast<unsigned>(qc)), kBmThreads, 0, st>>>(
+            h->post_ptr, h->post_doc, h->post_tf, h->den, h->idf, h->k1p1, h->n_docs, q_ptr + q0, q_terms, k,
+            h->cs[0].as<double>(), h->ci[0].as<int32_t>());
         count_launch();
         RMU_CHECK_LAUNCH();
-        int m = nblk * k, cur = 0;
-        for (;;) {
-            const int blocks = (m + kBmDocs - 1) / kBmDocs;
-            const int final_round = blocks == 1;
-            bm25_select_kernel<<<dim3(static_cast<unsigned>(blocks), static_cast<unsigned>(Q)), kBmThreads, 0, st>>>(
-                h->cs[cur].as<double>(), h->ci[cur].as<int32_t>(), m, k, final_round, h->cs[cur ^ 1].as<double>(),
-                h->ci[cur ^ 1].as<int32_t>(), out_scores, reinterpret_cast<long long*>(out_ids));
-            count_launch();
-            RMU_CHECK_LAUNCH();
-            if (final_round) break;
-            m = blocks * k;
-            cur ^= 1;
-        }
+        const size_t o = static_cast<size_t>(q0) * k;
+        const int rc = bm25_select_rounds(h->cs[0].as<double>(), h->ci[0].as<int32_t>(), qc, nblk * k, k, ws_s, ws_i,
+                                          out_scores + o, out_ids + o, st);
+        if (rc != RMU_OK) return rc;
     }
     return RMU_OK;
 }
@@ -412,6 +428,27 @@ int rmu_bm25_search_host(rmu_bm25* h, const int32_t* q_ptr_h, const int32_t* q_t
     RMU_CUDA(cudaMemcpyAsync(out_ids_h, h->out_i.p, static_cast<size_t>(Q) * k * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     RMU_CUDA(cudaStreamSynchronize(st));
     return RMU_OK;
+}
+
+/* For tests: the select rounds alone on caller-owned candidate lists (see the header) */
+int rmu_debug_bm25_select(const double* scores, const int32_t* idx, int Q, int m, int k, double* ws_scores,
+                          int32_t* ws_idx, int64_t ws_elems, double* out_scores, int64_t* out_ids, void* stream) {
+    if (!scores || !idx || !ws_scores || !ws_idx || !out_scores || !out_ids || Q < 1 || m < 1) {
+        set_error("rmu_debug_bm25_select: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (k < 1 || k > kBmMaxK || Q > kBmMaxQ) {
+        set_error("rmu_debug_bm25_select: k must be in [1, 256] and Q at most 65535");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    const int64_t half = static_cast<int64_t>(Q) * ((m + kBmDocs - 1) / kBmDocs) * k;
+    if (ws_elems < 2 * half) {
+        set_error("rmu_debug_bm25_select: workspace needs 2 * Q * ceil(m / 4096) * k elements");
+        return RMU_ERR_ARG;
+    }
+    double* const ws_s[2] = {ws_scores, ws_scores + half};
+    int32_t* const ws_i[2] = {ws_idx, ws_idx + half};
+    return bm25_select_rounds(scores, idx, Q, m, k, ws_s, ws_i, out_scores, out_ids, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -532,7 +532,11 @@ __global__ void adjacent_cosine_kernel(const float* __restrict__ x, long long pa
         na += __shfl_xor_sync(0xffffffffu, na, o);
         nb += __shfl_xor_sync(0xffffffffu, nb, o);
     }
-    if (lane == 0) out[pair] = 1.0 - dot / (sqrt(na) * sqrt(nb));
+    if (lane == 0) {
+        double c = dot / (sqrt(na) * sqrt(nb));
+        if (isnan(c) || isinf(c)) c = 0.0;      // cosine_similarity's rule: a zero row has similarity 0, distance 1
+        out[pair] = 1.0 - c;
+    }
 }
 
 // =====================================================================================================
@@ -1177,7 +1181,7 @@ int rmu_adjacent_cosine_distance(const float* x, int64_t n, int dim, double* out
 }
 
 int rmu_mmr_select(const float* q, const float* cand, const int32_t* n_cand, int nq, int fetch_k, int dim, int k,
-                   float lambda_mult, int32_t* out_sel, void* stream) {
+                   double lambda_mult, int32_t* out_sel, void* stream) {
     if (!q || !cand || !out_sel || nq < 0 || fetch_k <= 0 || fetch_k > 64 || dim <= 0 || k <= 0) {
         set_error("rmu_mmr_select: bad argument (fetch_k must be in 1..64)");
         return RMU_ERR_ARG;
@@ -1185,7 +1189,7 @@ int rmu_mmr_select(const float* q, const float* cand, const int32_t* n_cand, int
     if (nq == 0) return RMU_OK;
     const size_t smem = sizeof(double) * (3 * static_cast<size_t>(fetch_k) + static_cast<size_t>(fetch_k) * fetch_k);
     mmr_kernel<<<nq, 128, smem, static_cast<cudaStream_t>(stream)>>>(q, cand, n_cand, fetch_k, dim, k,
-                                                                     static_cast<double>(lambda_mult), out_sel);
+                                                                     lambda_mult, out_sel);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;

@@ -27,7 +27,8 @@ def test_header_declares_the_path():
     syms = declared_symbols()
     for must in ("rmu_index_create", "rmu_index_add", "rmu_index_search", "rmu_index_search_host", "rmu_topk_merge",
                  "rmu_mmr_select", "rmu_index_gather", "rmu_encoder_create", "rmu_encoder_embed",
-                 "rmu_encoder_classify", "rmu_encoder_embed_host", "rmu_encoder_classify_host", "rmu_last_error"):
+                 "rmu_encoder_classify", "rmu_encoder_embed_host", "rmu_encoder_classify_host", "rmu_last_error",
+                 "rmu_debug_bm25_select"):
         assert must in syms
 
 
@@ -96,6 +97,22 @@ def test_kernel_test_entry_points_reject_before_any_cuda_call(built_lib):
     assert tile(fake, q=None) == -1 and tile(fake, out=None) == -1
     assert tile(fake, nq=0) == -1 and tile(fake, nq=-3) == -1 and tile(fake, nq=65) == -1
     assert tile(fake, q=p + 4) == -1 and tile(fake, q=p + 8) == -1     # queries must be 16-byte aligned (TMA)
+
+    # the BM25 select stage on caller-owned candidate lists: workspace 2 * Q * ceil(m / 4096) * k elements
+    def bsel(Q=3, m=5000, k=10, ws_elems=2 * 3 * 2 * 10, **kw):
+        a = dict(scores=p, idx=p, ws_s=p, ws_i=p, out_s=p, out_i=p)
+        a.update(kw)
+        return l.rmu_debug_bm25_select(a["scores"], a["idx"], Q, m, k, a["ws_s"], a["ws_i"], ws_elems, a["out_s"],
+                                       a["out_i"], None)
+
+    assert bsel(k=0) == -3 and bsel(k=257) == -3 and bsel(k=-1) == -3
+    assert bsel(Q=65536, ws_elems=1 << 40) == -3 and b"rmu_debug_bm25_select" in l.rmu_last_error()
+    assert bsel(Q=0) == -1 and bsel(Q=-2) == -1 and bsel(m=0) == -1 and bsel(m=-4096) == -1
+    for name in ("scores", "idx", "ws_s", "ws_i", "out_s", "out_i"):
+        assert bsel(**{name: None}) == -1, name
+    assert bsel(ws_elems=2 * 3 * 2 * 10 - 1) == -1                      # one element short
+    assert bsel(m=4096, ws_elems=2 * 3 * 10 - 1) == -1 and bsel(m=4097, ws_elems=2 * 3 * 2 * 10 - 1) == -1
+    assert bsel(Q=65535, m=1, k=256, ws_elems=2 * 65535 * 256 - 1) == -1
 
 
 def test_product_fails_loudly_without_cuda(built_lib):
