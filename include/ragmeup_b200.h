@@ -69,6 +69,13 @@ int rmu_index_add(rmu_index* idx, const float* vecs, int64_t n, int src_is_host,
 /* overwrite existing rows in place (PGVector's upsert-on-id, langchain-postgres add_embeddings): rows[n] int64 local row
  * numbers and vecs [n, dim] fp32, both DEVICE pointers; rows outside [0, size) are ignored */
 int rmu_index_set_rows(rmu_index* idx, const int64_t* rows, const float* vecs, int64_t n, void* stream);
+/* delete rows (a vector store's delete by id / by expression): rows_h[n] int64 local row numbers, a HOST array, in any
+ * order, duplicates allowed (taken as a set).  The surviving rows close up in place on the device, keeping their order,
+ * and their statistics are recomputed: afterwards the index equals a fresh one built by adding the survivors in order.
+ * Capacity is kept.  A null rows_h with n > 0, n < 0 or a row outside [0, size) returns RMU_ERR_ARG before any CUDA
+ * call, with the index untouched; n = 0 launches nothing.  Waits for all work on the device (like a growing add), so
+ * nothing enqueued earlier reads rows while they move. */
+int rmu_index_remove(rmu_index* idx, const int64_t* rows_h, int64_t n, void* stream);
 int64_t rmu_index_size(const rmu_index* idx);
 int rmu_index_dim(const rmu_index* idx);
 int rmu_index_metric(const rmu_index* idx);

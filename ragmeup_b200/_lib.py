@@ -39,6 +39,7 @@ SIGNATURES = {
     "rmu_index_reserve": (C.c_int, [C.c_void_p, C.c_int64]),
     "rmu_index_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "rmu_index_set_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "rmu_index_remove": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "rmu_index_size": (C.c_int64, [C.c_void_p]),
     "rmu_index_dim": (C.c_int, [C.c_void_p]),
     "rmu_index_metric": (C.c_int, [C.c_void_p]),

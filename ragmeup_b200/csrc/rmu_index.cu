@@ -20,10 +20,14 @@
 #include <mutex>
 #include <vector>
 
+#include <cooperative_groups.h>
+
 #include "rmu_common.h"
 #include "rmu_ptx.cuh"
 
 namespace rmu {
+
+namespace cg = cooperative_groups;
 
 // =====================================================================================================
 // exact fp32 metric — ONE definition, used by the finalize re-score and by the exact scan, so both
@@ -172,6 +176,116 @@ __global__ void set_rows_kernel(float* __restrict__ x, const long long* __restri
         if (metric == RMU_METRIC_L2) rbias[r] = -0.5f * s;
         atomicMax(max_norm_bits, __float_as_uint(nrm));
         atomicMax(max_dev_bits, __float_as_uint(fabsf(s - 1.0f)));
+    }
+}
+
+// =====================================================================================================
+// in-place stable compaction of the corpus (rmu_index_remove)
+//
+// Removing the sorted rows del[0..m) moves every surviving row i > del[0] to i - #{del < i}.  The survivors between
+// del[j] and del[j+1] (del[m] = n) form run j: destination rows [a[j], a[j+1]) with a[j] = del[j] - j, source =
+// destination + (j + 1) rows.  The runs tile the destination rows [a[0], n') without gaps (a[m] = n'), so the moved data
+// is the float range [a[0]·D, n'·D) of the corpus.  It is cut into chunks of kCompactChunk floats: a chunk's destination
+// is contiguous and its source is one contiguous piece per run it meets.
+//
+// Ordering.  A destination is never above its source and the mapping is monotone, so any source that chunk c's
+// destination [lo_c, hi_c) overwrites belongs to a chunk <= c (a source s in [lo_c, hi_c) goes to d(s) <= s < hi_c).
+// The grid works in rounds: CTA b takes chunk r·G + b in round r, and each round is  load -> grid barrier -> store.
+// After the barrier of round r every chunk of rounds <= r has finished loading, which covers every source a store of
+// round r overwrites.  The loads of round r + 1 read sources at or above their own destinations, all of which lie above
+// every destination of round r, so they are issued before round r's stores and overlap them.  Progress: the kernel is
+// launched cooperatively, so all G CTAs are resident and the grid barrier cannot wait on a CTA that never runs; a grid
+// that would not fit is refused at launch instead.
+//
+// D % 4 == 0: every piece and every chunk is 16-byte aligned.  One thread per piece issues a 1-D bulk copy global ->
+// shared onto the buffer's mbarrier, and one bulk copy shared -> global writes the chunk back; two buffers alternate by
+// round.  Other D: the threads copy float by float through one buffer, and rounds do not overlap.
+// Each moved row is read once and written once.  Only x moves: the caller recomputes the row statistics afterwards.
+// =====================================================================================================
+constexpr int kCompactThreads = 256;
+constexpr int kCompactChunk = 24576;      // floats per chunk (96 KB); with two buffers one CTA fills an SM's shared memory
+
+// the run of destination row r: the largest j in [jlo, jhi] with a[j] <= r (a is nondecreasing and a[jlo] <= r)
+__device__ __forceinline__ long long compact_run(const long long* __restrict__ a, long long jlo, long long jhi, long long r) {
+    while (jlo < jhi) {
+        const long long mid = (jlo + jhi + 1) >> 1;
+        if (a[mid] <= r) jlo = mid; else jhi = mid - 1;
+    }
+    return jlo;
+}
+
+template <bool BULK>
+__global__ void __launch_bounds__(kCompactThreads) compact_rows_kernel(float* x, const long long* __restrict__ a, long long m,
+                                                                       int D, long long nchunks) {
+    extern __shared__ __align__(128) float cbuf[];     // [BULK ? 2 : 1][kCompactChunk]
+    __shared__ __align__(8) uint64_t bar[2];
+    __shared__ long long s_j[2];
+    cg::grid_group grid = cg::this_grid();
+    const int tid = threadIdx.x;
+    const long long lo0 = a[0] * D, end = a[m] * D;
+    const long long G = gridDim.x, b = blockIdx.x;
+    const long long rounds = (nchunks + G - 1) / G;
+    // runs met by the chunk [lo, hi): [s_j[0], s_j[1]]
+    auto runs_of = [&](long long lo, long long hi) {
+        if (tid == 0) {
+            s_j[0] = compact_run(a, 0, m - 1, lo / D);
+            s_j[1] = compact_run(a, s_j[0], m - 1, (hi - 1) / D);
+        }
+    };
+    if constexpr (BULK) {
+        if (tid == 0) { mbar_init(&bar[0], 1); mbar_init(&bar[1], 1); fence_mbar_init(); }
+        __syncthreads();
+        // chunk c -> buffer buf: thread 0 arms the barrier with the chunk's bytes, then every thread issues pieces
+        auto load = [&](long long c, int buf) {
+            const long long lo = lo0 + c * kCompactChunk, hi = min(lo + kCompactChunk, end);
+            runs_of(lo, hi);
+            if (tid == 0) {
+                bulk_wait_read<0>();                   // the store that last read this buffer is done with it
+                mbar_arrive_expect_tx(&bar[buf], static_cast<uint32_t>(hi - lo) * 4u);
+            }
+            __syncthreads();
+            const long long jlo = s_j[0], jhi = s_j[1];
+            float* dst = cbuf + buf * kCompactChunk;
+            for (long long j = jlo + tid; j <= jhi; j += blockDim.x) {
+                const long long plo = max(a[j] * D, lo), phi = min(a[j + 1] * D, hi);
+                if (phi > plo) bulk_load_1d(dst + (plo - lo), x + plo + (j + 1) * D, static_cast<uint32_t>(phi - plo) * 4u, &bar[buf]);
+            }
+        };
+        if (b < nchunks) load(b, 0);
+        for (long long r = 0; r < rounds; ++r) {
+            const long long c = r * G + b;
+            const int buf = static_cast<int>(r & 1);
+            if (tid == 0 && c < nchunks) mbar_wait(&bar[buf], static_cast<uint32_t>((r >> 1) & 1));
+            grid.sync();
+            if (tid == 0) fence_proxy_async_global();
+            if (c + G < nchunks) load(c + G, buf ^ 1);
+            if (tid == 0 && c < nchunks) {
+                const long long lo = lo0 + c * kCompactChunk, hi = min(lo + kCompactChunk, end);
+                bulk_store_1d(x + lo, cbuf + buf * kCompactChunk, static_cast<uint32_t>(hi - lo) * 4u);
+                bulk_commit();
+            }
+        }
+        if (tid == 0) bulk_wait<0>();
+    } else {
+        for (long long r = 0; r < rounds; ++r) {
+            const long long c = r * G + b;
+            const long long lo = lo0 + c * kCompactChunk, hi = min(lo + kCompactChunk, end);
+            __syncthreads();
+            if (c < nchunks) {
+                runs_of(lo, hi);
+                __syncthreads();
+                const long long jlo = s_j[0], jhi = s_j[1];
+                long long j = jlo;
+                for (long long e = lo + tid; e < hi; e += blockDim.x) {
+                    const long long row = e / D;
+                    if (row < a[j] || row >= a[j + 1]) j = compact_run(a, jlo, jhi, row);
+                    cbuf[e - lo] = x[e + (j + 1) * D];
+                }
+            }
+            grid.sync();
+            if (c < nchunks)
+                for (long long e = lo + tid; e < hi; e += blockDim.x) x[e] = cbuf[e - lo];
+        }
     }
 }
 
@@ -848,6 +962,65 @@ int rmu_index_clear(rmu_index* idx) {
     idx->n = 0;
     idx->tmap_rows = -1;
     RMU_CUDA(cudaMemset(idx->max_norm_bits, 0, 2 * sizeof(unsigned)));
+    return RMU_OK;
+}
+
+int rmu_index_remove(rmu_index* idx, const int64_t* rows_h, int64_t n, void* stream) {
+    if (!idx || n < 0 || (n > 0 && !rows_h)) { set_error("rmu_index_remove: bad argument"); return RMU_ERR_ARG; }
+    if (n == 0) return RMU_OK;
+    std::lock_guard<std::mutex> g(idx->mu);
+    const int64_t size = idx->n;
+    for (int64_t i = 0; i < n; ++i)
+        if (rows_h[i] < 0 || rows_h[i] >= size) { set_error("rmu_index_remove: row outside [0, size)"); return RMU_ERR_ARG; }
+    std::vector<int64_t> del(rows_h, rows_h + n);
+    std::sort(del.begin(), del.end());
+    del.erase(std::unique(del.begin(), del.end()), del.end());
+    const int64_t m = static_cast<int64_t>(del.size());
+    const int64_t kept = size - m;
+    const int D = idx->dim;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // work enqueued earlier on any stream (searches, gathers) must not read rows while they move
+    RMU_CUDA(cudaDeviceSynchronize());
+    idx->tmap_rows = -1;
+    RMU_CUDA(cudaMemsetAsync(idx->max_norm_bits, 0, 2 * sizeof(unsigned), st));
+    if (kept == 0) { idx->n = 0; return RMU_OK; }            // what rmu_index_clear leaves
+
+    // runs of survivors: destination rows [a[j], a[j+1]) come from `j + 1` rows further up
+    std::vector<long long> a(static_cast<size_t>(m) + 1);
+    for (int64_t j = 0; j < m; ++j) a[j] = del[j] - j;
+    a[m] = kept;
+    const long long moved = (kept - a[0]) * static_cast<long long>(D);   // floats that change place
+    if (moved > 0) {
+        int rc = ensure_ws(idx, a.size() * sizeof(long long));
+        if (rc != RMU_OK) return rc;
+        long long* d_a = static_cast<long long*>(idx->ws);
+        RMU_CUDA(cudaMemcpyAsync(d_a, a.data(), a.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+        const bool bulk = D % 4 == 0;
+        const void* kern = bulk ? reinterpret_cast<const void*>(compact_rows_kernel<true>)
+                                : reinterpret_cast<const void*>(compact_rows_kernel<false>);
+        const size_t smem = sizeof(float) * kCompactChunk * (bulk ? 2 : 1);
+        RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+        int per_sm = 0;
+        RMU_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kCompactThreads, smem));
+        if (per_sm < 1) { set_error("rmu_index_remove: the compaction kernel does not fit an SM"); return RMU_ERR_UNSUPPORTED; }
+        long long nchunks = (moved + kCompactChunk - 1) / kCompactChunk;
+        const unsigned grid = static_cast<unsigned>(std::min<long long>(nchunks, static_cast<long long>(per_sm) * idx->sms));
+        float* xp = idx->x;
+        long long mm = m;
+        int dim = D;
+        void* args[] = {&xp, &d_a, &mm, &dim, &nchunks};
+        RMU_CUDA(cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(kCompactThreads), args, smem, st));
+        count_launch();
+        RMU_CHECK_LAUNCH();
+    }
+    // statistics exactly as a fresh add of the surviving rows computes them
+    const int wpb = 8;
+    row_stats_kernel<<<static_cast<unsigned>((kept + wpb - 1) / wpb), wpb * 32, 0, st>>>(
+        idx->x, 0, kept, D, idx->metric, idx->rscale, idx->rbias, idx->max_norm_bits, idx->max_norm_bits + 1);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    idx->n = kept;
+    RMU_CUDA(cudaEventRecord(idx->ws_done, st));              // the run table lives in the shared scratch
     return RMU_OK;
 }
 

@@ -87,6 +87,22 @@ __device__ __forceinline__ void tma_store_2d(const void* tmap, const void* smem_
                  ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
                  : "memory");
 }
+// 1-D bulk copy global -> shared of `bytes` (multiple of 16; both addresses 16-byte aligned), credited to `bar`
+__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
+                 : "memory");
+}
+// 1-D bulk copy shared -> global (same alignment rules), tracked by the issuing thread's bulk async-groups
+__device__ __forceinline__ void bulk_store_1d(void* gdst, const void* smem_src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+                 ::"l"(reinterpret_cast<uint64_t>(gdst)), "r"(smem_u32(smem_src)), "r"(bytes)
+                 : "memory");
+}
+// order this thread's generic-proxy global accesses with its later async-proxy (bulk copy) ones
+__device__ __forceinline__ void fence_proxy_async_global() {
+    asm volatile("fence.proxy.async.global;" ::: "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // at most N of this thread's bulk groups still READ their shared-memory source (the buffer may be rewritten)
 template <int N>

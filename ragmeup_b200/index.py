@@ -97,6 +97,17 @@ class FlatIndex:
             r.record_stream(torch.cuda.current_stream())
             v.record_stream(torch.cuda.current_stream())
 
+    def remove(self, rows) -> None:
+        """Delete rows (ints, numpy or a tensor of local row numbers; any order, duplicates allowed).  The survivors
+        close up in place and keep their order, so row numbers above a removed row shift down.  Runs on the current
+        stream; raises ``RmuError`` (index untouched) for a row outside ``[0, len)``."""
+        if hasattr(rows, "detach"):
+            rows = rows.detach().cpu().numpy()
+        r = np.ascontiguousarray(np.asarray(rows, dtype=np.int64).reshape(-1))
+        with self.torch.cuda.device(self.device):
+            _lib.check(_lib.lib().rmu_index_remove(self._h, r.ctypes.data if r.size else None, r.size, _lib.stream_ptr()),
+                       "rmu_index_remove")
+
     def search(self, queries, k: int, id_offset: int = 0, mode: int = MODE_AUTO,
                want_stats: bool = False, out=None) -> Tuple["object", "object"]:
         """queries CUDA fp32 [nq, dim] -> (scores fp32 [nq, k], ids int64 [nq, k]) on the device.

@@ -10,6 +10,8 @@ from __future__ import annotations
 
 from typing import Any, Callable, Optional, Tuple
 
+import numpy as np
+
 
 class ShardedFlatIndex:
     def __init__(self, local_index: Any, group: Any = None, merge_fn: Optional[Callable] = None):
@@ -26,8 +28,12 @@ class ShardedFlatIndex:
             merge_fn = topk_merge
         self.merge_fn = merge_fn
         self._xkey, self._x = None, None
-        self._batches = []          # sizes of the batches passed to add(), in order (identical on every rank)
         self._preloaded = len(local_index)   # rows that were in the shard before the first add()
+        self._batches = []          # sizes of the batches passed to add(), in order (identical on every rank)
+        # what remove() took out, identical on every rank: per shard, the removed rows numbered among every row ever
+        # added to that shard (sorted), and their positions in the order the batches were added (sorted, all shards)
+        self._gone = [np.zeros(0, np.int64) for _ in range(self.world)]
+        self._gone_pos = np.zeros(0, np.int64)
         self.offset = 0
         self.total = len(local_index)
         self._sizes = [len(local_index)]
@@ -66,25 +72,73 @@ class ShardedFlatIndex:
             self.total = sum(self._sizes)
         return lo, hi
 
+    def _layout(self):
+        """per batch b and rank r: the first row of the batch the rank kept, where it starts in the rank's rows as if
+        nothing were removed, and where the batch starts in the order the batches were added"""
+        R = self.world
+        nb = np.asarray(self._batches, np.int64)
+        r = np.arange(R, dtype=np.int64)[:, None]
+        first = r * nb // R                                                                        # [R, nb]
+        local_start = np.concatenate([np.zeros((R, 1), np.int64), np.cumsum((r + 1) * nb // R - first, 1)], 1)
+        batch_start = np.concatenate([[0], np.cumsum(nb)])
+        return first, local_start, batch_start
+
+    def _positions(self, r: int, local, layout):
+        """current local rows of shard r -> their positions in the order the batches were added, removed rows counted"""
+        first, local_start, batch_start = layout
+        gone = self._gone[r]
+        # the l-th surviving row is row l + #{removed rows before it} of everything the shard was given
+        o = local + np.searchsorted(gone - np.arange(gone.size), local, side="right") if gone.size else local
+        b = np.searchsorted(local_start[r], o, side="right") - 1
+        return o, batch_start[b] + first[r, b] + (o - local_start[r, b])
+
+    def remove(self, global_ids) -> int:
+        """Every rank is handed the same merged ids (shard offset + local row, as :meth:`search` returns them; any order,
+        duplicates allowed) and removes those that fall in its shard.  Each rank derives every shard's new size from the
+        list, so offsets stay in step without a collective.  Raises ``ValueError`` on every rank, removing nothing, for
+        an id outside ``[0, total)``.  Returns the number of rows this rank removed."""
+        g = np.unique(np.asarray(global_ids.cpu() if hasattr(global_ids, "cpu") else global_ids, dtype=np.int64).reshape(-1))
+        if self._sizes is None or len(self._sizes) != self.world:
+            self.sync_offsets()
+        if g.size and (g[0] < 0 or g[-1] >= self.total):
+            raise ValueError(f"ids must lie in [0, {self.total})")
+        starts = np.concatenate([[0], np.cumsum(self._sizes)])
+        cuts = np.searchsorted(g, starts)
+        mine = g[cuts[self.rank]:cuts[self.rank + 1]] - starts[self.rank]
+        if mine.size:
+            self.index.remove(mine)
+        if not self._preloaded and g.size:
+            layout = self._layout()
+            found = [self._positions(r, g[cuts[r]:cuts[r + 1]] - starts[r], layout) for r in range(self.world)]
+            for r, (o, _) in enumerate(found):
+                self._gone[r] = np.union1d(self._gone[r], o)
+            self._gone_pos = np.union1d(self._gone_pos, np.concatenate([pos for _, pos in found]))
+        self._sizes = [s - int(cuts[r + 1] - cuts[r]) for r, s in enumerate(self._sizes)]
+        self.offset = sum(self._sizes[: self.rank])
+        self.total = sum(self._sizes)
+        return int(mine.size)
+
     def to_insertion_order(self, ids):
-        """merged global ids (shard offset + local row) -> position of the row in the order the batches were added
-        (what an unsharded store would have called it); -1 stays -1.  Only for shards filled through :meth:`add`."""
-        import numpy as np
+        """merged global ids (shard offset + local row) -> position of the row among the surviving rows in the order the
+        batches were added (what an unsharded store given the same adds and removes would call it); -1 stays -1.
+        Only for shards filled through :meth:`add`."""
         if self._preloaded:
             raise ValueError("to_insertion_order needs shards that were filled through add() only")
         g = np.asarray(ids.cpu() if hasattr(ids, "cpu") else ids, dtype=np.int64)
-        R = self.world
-        sizes = np.array([[(r + 1) * n // R - r * n // R for n in self._batches] for r in range(R)], dtype=np.int64)   # [R, nb]
-        local_start = np.concatenate([np.zeros((R, 1), np.int64), np.cumsum(sizes, 1)], 1)                             # [R, nb + 1]
-        offsets = np.concatenate([[0], np.cumsum(local_start[:, -1])])                                                 # [R + 1]
-        batch_start = np.concatenate([[0], np.cumsum(self._batches)])
+        layout = self._layout()
+        sizes = layout[1][:, -1] - np.array([gone.size for gone in self._gone], np.int64)
+        offsets = np.concatenate([[0], np.cumsum(sizes)])
         out = np.full(g.shape, -1, np.int64)
         ok = g >= 0
-        r = np.searchsorted(offsets, g[ok], side="right") - 1
-        local = g[ok] - offsets[r]
-        b = np.array([np.searchsorted(local_start[ri], li, side="right") - 1 for ri, li in zip(r, local)], dtype=np.int64)
-        first_kept = np.array([ri * self._batches[bi] // R for ri, bi in zip(r, b)], dtype=np.int64)
-        out[ok] = batch_start[b] + first_kept + (local - local_start[r, b])
+        gk = g[ok]
+        res = np.empty(gk.shape, np.int64)
+        rk = np.searchsorted(offsets, gk, side="right") - 1
+        for r in range(self.world):
+            sel = rk == r
+            if sel.any():
+                _, pos = self._positions(r, gk[sel] - offsets[r], layout)
+                res[sel] = pos - np.searchsorted(self._gone_pos, pos)      # removed rows before it do not count
+        out[ok] = res
         return out
 
     def _exchange_buffers(self, Q: int, k: int, device):

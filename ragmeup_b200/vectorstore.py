@@ -22,18 +22,20 @@ host.  All distance arithmetic runs in ``csrc/rmu_index.cu``.
 Persistence (``vector_store_uri`` reuse, ``server/.env.template:33``, ``vector_store_initial_load``
 ``server/RAGHelper.py:406-434``): the reference's stores keep their rows across process restarts (a
 milvus-lite file at ``connection_args["uri"]`` / a Postgres database).  Here a collection with a storage
-directory appends one segment file per ``add_*`` call (vectors + ids + texts + metadata) and reloads the
-segments when it is constructed again, unless ``drop_old`` is set, which deletes them.  ``Milvus``:
+directory appends one segment file per ``add_*`` call (vectors + ids + texts + metadata) and one per ``delete``
+(the removed positions), and replays the segments in order when it is constructed again, unless ``drop_old`` is set, which deletes them.  ``Milvus``:
 directory ``<uri>.b200/<collection_name>``; ``PGVector``: ``$RMU_STORE_DIR/<collection_name>`` when that
 variable is set, otherwise the collection only lives in GPU memory (said once on stderr).
 """
 from __future__ import annotations
 
+import ast
 import atexit
 import glob
 import json
 import os
 import queue
+import re
 import shutil
 import sys
 import threading
@@ -98,6 +100,8 @@ class B200VectorStore:
         self._texts: List[str] = []
         self._metas: List[Dict[str, Any]] = []
         self._row_of: Dict[str, int] = {}
+        self._added = 0             # rows ever inserted: default ids count them, so a deletion never makes one repeat
+        self._generation = 0        # bumped by every removal: row numbers from an older generation name other documents
         self._lock = threading.RLock()
         self._storage_dir = storage_dir
         self._segments = 0
@@ -164,6 +168,7 @@ class B200VectorStore:
                     self._texts[r], self._metas[r] = texts[j], dict(metadatas[j])
         if new:
             index.add(vectors if len(new) == n else vectors[new])
+            self._added += len(new)
             for j in new:
                 self._row_of[ids[j]] = len(self._pks)
                 self._pks.append(ids[j])
@@ -181,7 +186,7 @@ class B200VectorStore:
         metas = [dict(m) for m in (metadatas or [{} for _ in range(n)])]
         texts = list(texts)
         with self._lock:                                    # default ids, rows and the host tables move together
-            pks = [str(len(self._pks) + i) for i in range(n)] if ids is None else [str(i) for i in ids]
+            pks = [str(self._added + i) for i in range(n)] if ids is None else [str(i) for i in ids]
             self._insert_locked(vectors, texts, metas, pks)
             if self._storage_dir is not None:
                 seg = self._segments
@@ -211,12 +216,63 @@ class B200VectorStore:
         metas = [d.metadata for d in documents]
         return self.add_texts(texts, metas, ids=ids, **kwargs)
 
+    # ------------------------------------------------------------------ delete
+    def _remove_locked(self, rows: Sequence[int]) -> int:
+        """remove rows (positions, any order) from the index and the host tables in one pass; ``self._lock`` held"""
+        drop = set(int(r) for r in rows)
+        if not drop:
+            return 0
+        self.index.remove(sorted(drop))
+        keep = [r for r in range(len(self._pks)) if r not in drop]
+        self._pks = [self._pks[r] for r in keep]
+        self._texts = [self._texts[r] for r in keep]
+        self._metas = [self._metas[r] for r in keep]
+        self._row_of = {pk: r for r, pk in enumerate(self._pks)}    # a repeated pk maps to its last row, as after adds
+        self._generation += 1
+        return len(drop)
+
+    def _delete_rows(self, match) -> int:
+        """remove every row r with ``match(r)``; persisted as the removed positions, through the segment writer"""
+        with self._lock:
+            rows = [r for r in range(len(self._pks)) if match(r)]
+            if not rows:
+                return 0
+            self._remove_locked(rows)
+            if self._storage_dir is not None:
+                seg = self._segments
+                self._segments += 1
+                if self._sync_writes:
+                    self._write_segment(seg, None, [], [], [], deleted=rows)
+                else:
+                    self._enqueue_segment(seg, None, [], [], [], deleted=rows)
+        return len(rows)
+
+    def _delete_by_ids(self, ids: Iterable[Any]) -> int:
+        want = set(str(i) for i in ids)
+        return self._delete_rows(lambda r: self._pks[r] in want)
+
+    def delete(self, ids: Optional[Sequence[Any]] = None, expr: Optional[str] = None, **_: Any) -> "DeleteResult":
+        """``langchain_milvus.Milvus.delete`` (``PGVector`` narrows it to ids): every row whose pk is in ``ids`` (then
+        ``expr`` is ignored, as langchain-milvus does), or every row ``expr`` matches.  ``expr`` takes the forms the reference writes,
+        ``<field> == "<string>"`` and ``<field> in ["a", ...]``, where the field is ``pk`` or a metadata key
+        (``db.delete(expr='source == "<path>"')`` removes a file's chunks).  Any other expression raises ``ValueError``
+        and deletes nothing.  The result's ``delete_count`` is the number of rows removed."""
+        if ids is not None and len(ids) > 0:
+            return DeleteResult(self._delete_by_ids(ids))
+        if not isinstance(expr, str):
+            raise ValueError("Either ids list or expr string must be provided.")
+        field, values = parse_delete_expr(expr)
+        if field == self.id_field:
+            return DeleteResult(self._delete_by_ids(values))
+        return DeleteResult(self._delete_rows(lambda r: self._metas[r].get(field, _NO_VALUE) in values))
+
     # ------------------------------------------------------------------ persistence: one segment per add call
     # Segments are written by one background thread per store, in insertion order: the device->host copy of the vectors,
     # the JSON table and the file write (together as long as the GPU work of a 1000-document batch) stay off the ingest
     # loop.  ``flush()`` waits for everything queued so far and re-raises a writer error; it runs at interpreter exit, in
     # ``save`` and before segments are re-read.  RMU_STORE_SYNC=1 writes inside ``add_*`` instead.
-    def _enqueue_segment(self, seg: int, vectors, texts, metas, pks) -> None:
+    def _enqueue_segment(self, seg: int, vectors, texts, metas, pks, deleted: Optional[List[int]] = None,
+                         added: Optional[int] = None) -> None:
         if self._writer is None:
             self._queue = queue.Queue(maxsize=8)             # bounds the vectors kept alive for the writer
             self._writer = threading.Thread(target=self._writer_loop, name="rmu-segment-writer", daemon=True)
@@ -224,7 +280,7 @@ class B200VectorStore:
             atexit.register(self.flush)
         if self._writer_error is not None:
             self.flush()
-        self._queue.put((seg, vectors, list(texts), [dict(m) for m in metas], list(pks)))
+        self._queue.put((seg, vectors, list(texts), [dict(m) for m in metas], list(pks), deleted, added))
 
     def _writer_loop(self) -> None:
         while True:
@@ -247,10 +303,21 @@ class B200VectorStore:
             e, self._writer_error = self._writer_error, None
             raise RuntimeError(f"segment writer failed: {e!r}") from e
 
-    def _write_segment(self, seg: int, vectors, texts, metas, pks) -> None:
+    def _write_segment(self, seg: int, vectors, texts, metas, pks, deleted: Optional[List[int]] = None,
+                       added: Optional[int] = None) -> None:
+        """an add segment; with ``deleted`` a deletion record: the positions removed, as they were at that moment (pks
+        would not do: Milvus keeps repeated pks, and an expression may match only some of those rows); with ``added``
+        the default-id counter carried over from an export"""
         os.makedirs(self._storage_dir, exist_ok=True)
-        vec = vectors if isinstance(vectors, np.ndarray) else vectors.detach().float().cpu().numpy()
-        table = np.frombuffer(json.dumps({"pks": pks, "texts": texts, "metas": metas}).encode(), dtype=np.uint8)
+        if added is not None:
+            vec = np.zeros((0, 0), np.float32)
+            table = np.frombuffer(json.dumps({"added": int(added)}).encode(), dtype=np.uint8)
+        elif deleted is not None:
+            vec = np.zeros((0, 0), np.float32)
+            table = np.frombuffer(json.dumps({"deleted": [int(r) for r in deleted]}).encode(), dtype=np.uint8)
+        else:
+            vec = vectors if isinstance(vectors, np.ndarray) else vectors.detach().float().cpu().numpy()
+            table = np.frombuffer(json.dumps({"pks": pks, "texts": texts, "metas": metas}).encode(), dtype=np.uint8)
         path = os.path.join(self._storage_dir, f"seg_{seg:08d}.npz")
         tmp = path + ".tmp.npz"
         np.savez(tmp, vectors=np.ascontiguousarray(vec, dtype=np.float32), metric=self.metric, table=table)
@@ -264,7 +331,13 @@ class B200VectorStore:
             if str(z["metric"]) != self.metric:
                 raise ValueError(f"{f} was written by a {z['metric']} collection, this store is {self.metric}")
             table = json.loads(bytes(z["table"]).decode())
-            if z["vectors"].size:
+            if "deleted" in table:                          # replayed in order: positions refer to the rows at that point
+                with self._lock:
+                    self._remove_locked(table["deleted"])
+            elif "added" in table:
+                with self._lock:
+                    self._added = max(self._added, int(table["added"]))
+            elif z["vectors"].size:
                 with self._lock:
                     self._insert_locked(np.ascontiguousarray(z["vectors"]), table["texts"], table["metas"], table["pks"])
         self._segments = len(files)
@@ -275,14 +348,16 @@ class B200VectorStore:
         return (1.0 - scores) if self.metric == "cosine" else scores
 
     def search_tensor(self, queries, k: int):
-        """CUDA fp32 [Q, D] -> (scores [Q,k], rows int64 [Q,k]) on the device; rows index insertion order."""
+        """CUDA fp32 [Q, D] -> (scores [Q,k], rows int64 [Q,k]) on the device; rows index insertion order.  A delete
+        renumbers the rows above the first one it removes: a caller that may race with one holds ``self._lock``."""
         if self.index is None:
             raise _lib.RmuError("the collection is empty")
         s, i = self.index.search(queries, k)
         return self._score_out(s), i
 
     def mmr_tensor(self, queries, k: int = 4, fetch_k: int = 20, lambda_mult: float = 0.5):
-        """CUDA fp32 [Q, D] -> rows int64 [Q, k] in MMR order (-1 padded), all on the device."""
+        """CUDA fp32 [Q, D] -> rows int64 [Q, k] in MMR order (-1 padded), all on the device (rows as in
+        :meth:`search_tensor`)."""
         if self.index is None:
             raise _lib.RmuError("the collection is empty")
         torch = self.index.torch
@@ -307,25 +382,39 @@ class B200VectorStore:
                 return [self._doc(r) for r in rows if r >= 0]
             return [(self._doc(r), float(sc)) for sc, r in zip(scores, rows) if r >= 0]
 
+    def _search_docs(self, run, with_scores: bool):
+        """``run()`` searches the device -> (rows, scores) of query 0 as lists -> documents.  The search runs outside the
+        lock, so that searches do not wait for each other's host work.  A delete that lands between the search and the
+        mapping renumbers the rows, so then the search runs again under the lock, where no delete can interleave."""
+        gen = self._generation
+        rows, scores = run()
+        with self._lock:
+            if gen != self._generation:
+                rows, scores = run()
+            return self._docs(rows, scores if with_scores else None)
+
     def _embed_query_tensor(self, query: str):
         torch = _lib.require_cuda()
         if hasattr(self.embedding_func, "encode_tensor"):
             return self.embedding_func.encode_tensor([query])
         return torch.tensor([self.embedding_func.embed_query(query)], dtype=torch.float32, device="cuda")
 
+    def _top_rows(self, q, k: int):
+        s, i = self.search_tensor(q, k)
+        return i[0].tolist(), s[0].tolist()
+
     def similarity_search_with_score_by_vector(self, embedding: List[float], k: int = 4, **_: Any) -> List[Tuple[Document, float]]:
         if self.index is None or len(self) == 0:
             return []
         torch = self.index.torch
         q = torch.as_tensor(np.asarray(embedding, dtype=np.float32)[None], device=self.index.device)
-        s, i = self.search_tensor(q, k)
-        return self._docs(i[0].tolist(), s[0].tolist())
+        return self._search_docs(lambda: self._top_rows(q, k), True)
 
     def similarity_search_with_score(self, query: str, k: int = 4, **kw: Any) -> List[Tuple[Document, float]]:
         if self.index is None or len(self) == 0:
             return []
-        s, i = self.search_tensor(self._embed_query_tensor(query), k)
-        return self._docs(i[0].tolist(), s[0].tolist())
+        q = self._embed_query_tensor(query)
+        return self._search_docs(lambda: self._top_rows(q, k), True)
 
     def similarity_search(self, query: str, k: int = 4, **kw: Any) -> List[Document]:
         return [d for d, _ in self.similarity_search_with_score(query, k, **kw)]
@@ -351,13 +440,14 @@ class B200VectorStore:
             return []
         torch = self.index.torch
         q = torch.as_tensor(np.asarray(embedding, dtype=np.float32)[None], device=self.index.device)
-        return self._docs(self.mmr_tensor(q, k, fetch_k, lambda_mult)[0].tolist())
+        return self._search_docs(lambda: (self.mmr_tensor(q, k, fetch_k, lambda_mult)[0].tolist(), None), False)
 
     def max_marginal_relevance_search(self, query: str, k: int = 4, fetch_k: int = 20, lambda_mult: float = 0.5,
                                       **_: Any) -> List[Document]:
         if self.index is None or len(self) == 0:
             return []
-        return self._docs(self.mmr_tensor(self._embed_query_tensor(query), k, fetch_k, lambda_mult)[0].tolist())
+        q = self._embed_query_tensor(query)
+        return self._search_docs(lambda: (self.mmr_tensor(q, k, fetch_k, lambda_mult)[0].tolist(), None), False)
 
     def as_retriever(self, **kwargs: Any) -> B200Retriever:
         return B200Retriever(self, kwargs.get("search_type", "similarity"), kwargs.get("search_kwargs"))
@@ -368,7 +458,7 @@ class B200VectorStore:
         self.flush()
         with self._lock:
             vec = self.index.data().cpu().numpy() if self.index is not None else np.zeros((0, 0), np.float32)
-            table = json.dumps({"pks": self._pks, "texts": self._texts, "metas": self._metas}).encode()
+            table = json.dumps({"pks": self._pks, "texts": self._texts, "metas": self._metas, "added": self._added}).encode()
         np.savez(path, vectors=vec, metric=self.metric, table=np.frombuffer(table, dtype=np.uint8))
 
     @classmethod
@@ -380,7 +470,22 @@ class B200VectorStore:
         table = json.loads(bytes(z["table"]).decode())
         if z["vectors"].size:
             store.add_embeddings(np.ascontiguousarray(z["vectors"]), table["texts"], table["metas"], table["pks"])
+        store._restore_added(int(table.get("added", 0)))
         return store
+
+    def _restore_added(self, added: int) -> None:
+        """default ids keep counting past rows deleted before an export; a storage directory records the counter too"""
+        with self._lock:
+            if added <= self._added:
+                return
+            self._added = added
+            if self._storage_dir is not None:
+                seg = self._segments
+                self._segments += 1
+                if self._sync_writes:
+                    self._write_segment(seg, None, [], [], [], added=added)
+                else:
+                    self._enqueue_segment(seg, None, [], [], [], added=added)
 
 
 class Milvus(B200VectorStore):
@@ -401,6 +506,38 @@ class Milvus(B200VectorStore):
             storage = os.path.join(str(uri) + ".b200", collection_name)
         super().__init__(embedding_function, metric="l2", collection_name=collection_name, device=device,
                          storage_dir=storage, drop_old=drop_old)
+
+
+class DeleteResult:
+    """what ``pymilvus`` ``Collection.delete`` returns, as far as the reference reads it (``delete_count``)"""
+
+    def __init__(self, delete_count: int):
+        self.delete_count = int(delete_count)
+
+    def __repr__(self) -> str:
+        return f"(delete count: {self.delete_count})"
+
+
+_NO_VALUE = object()
+_EXPR = re.compile(r"^\s*([A-Za-z_][A-Za-z0-9_]*)\s*(==|\bin\b)\s*(.+?)\s*$", re.S)
+
+
+def parse_delete_expr(expr: str) -> Tuple[str, List[str]]:
+    """``<field> == "<string>"`` / ``<field> in ["a", ...]`` (quoted strings, single or double quotes) ->
+    (field, [values]); anything else raises ``ValueError``."""
+    m = _EXPR.match(expr)
+    if m is None:
+        raise ValueError(f"unsupported delete expression {expr!r}: use <field> == \"<string>\" or <field> in [\"a\", ...]")
+    field, op, rhs = m.groups()
+    try:
+        value = ast.literal_eval(rhs)
+    except (ValueError, SyntaxError):
+        value = None
+    if op == "==" and isinstance(value, str) and rhs[0] in "'\"":
+        return field, [value]
+    if op == "in" and isinstance(value, list) and rhs[0] == "[" and all(isinstance(v, str) for v in value):
+        return field, list(value)
+    raise ValueError(f"unsupported delete expression {expr!r}: use <field> == \"<string>\" or <field> in [\"a\", ...]")
 
 
 _warned_memory_only = False
@@ -426,3 +563,8 @@ class PGVector(B200VectorStore):
             _warned_memory_only = True
         super().__init__(embeddings, metric="cosine", collection_name=collection_name, device=device,
                          storage_dir=os.path.join(root, collection_name) if root else None, drop_old=pre_delete_collection)
+
+    def delete(self, ids: Optional[Sequence[Any]] = None, collection_only: bool = False, **_: Any) -> None:
+        """``langchain_postgres.PGVector.delete``: removes the row of each id; unknown ids are ignored."""
+        if ids:
+            self._delete_by_ids(ids)
