@@ -16,7 +16,6 @@
 //              does not take) run the exact fp32 CUDA-core scan.
 // The ids and scores returned are therefore those of an exact fp32 brute-force search.
 #include <algorithm>
-#include <cstdlib>
 #include <mutex>
 #include <vector>
 
@@ -30,45 +29,10 @@ namespace rmu {
 namespace cg = cooperative_groups;
 
 // =====================================================================================================
-// exact fp32 metric — ONE definition, used by the finalize re-score and by the exact scan, so both
-// paths return bit-identical scores.  Fixed summation order: four interleaved fmaf chains.
+// exact fp32 metric of QT queries against one row (the row is read once for all of them).  Fixed summation order:
+// four interleaved fmaf chains per (query, row), combined as (a0 + a1) + (a2 + a3).  exact_metric_quad (rmu_scan.cuh)
+// spreads the same chains over four lanes, so the exact scan and the re-scores return bit-identical scores.
 // =====================================================================================================
-__device__ __forceinline__ float exact_metric(const float* __restrict__ q, const float* __restrict__ x, int D,
-                                              int metric, float qnorm) {
-    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-    float n0 = 0.f, n1 = 0.f, n2 = 0.f, n3 = 0.f;
-    const int D4 = D & ~3;
-    if (metric == RMU_METRIC_L2) {
-        for (int d = 0; d < D4; d += 4) {
-            float e0 = q[d] - x[d], e1 = q[d + 1] - x[d + 1], e2 = q[d + 2] - x[d + 2], e3 = q[d + 3] - x[d + 3];
-            a0 = fmaf(e0, e0, a0); a1 = fmaf(e1, e1, a1); a2 = fmaf(e2, e2, a2); a3 = fmaf(e3, e3, a3);
-        }
-        for (int d = D4; d < D; ++d) { float e = q[d] - x[d]; a0 = fmaf(e, e, a0); }
-        return (a0 + a1) + (a2 + a3);
-    }
-    if (metric == RMU_METRIC_IP) {
-        for (int d = 0; d < D4; d += 4) {
-            a0 = fmaf(q[d], x[d], a0); a1 = fmaf(q[d + 1], x[d + 1], a1);
-            a2 = fmaf(q[d + 2], x[d + 2], a2); a3 = fmaf(q[d + 3], x[d + 3], a3);
-        }
-        for (int d = D4; d < D; ++d) a0 = fmaf(q[d], x[d], a0);
-        return (a0 + a1) + (a2 + a3);
-    }
-    // cosine
-    for (int d = 0; d < D4; d += 4) {
-        float x0 = x[d], x1 = x[d + 1], x2 = x[d + 2], x3 = x[d + 3];
-        a0 = fmaf(q[d], x0, a0); a1 = fmaf(q[d + 1], x1, a1); a2 = fmaf(q[d + 2], x2, a2); a3 = fmaf(q[d + 3], x3, a3);
-        n0 = fmaf(x0, x0, n0); n1 = fmaf(x1, x1, n1); n2 = fmaf(x2, x2, n2); n3 = fmaf(x3, x3, n3);
-    }
-    for (int d = D4; d < D; ++d) { a0 = fmaf(q[d], x[d], a0); n0 = fmaf(x[d], x[d], n0); }
-    float ip = (a0 + a1) + (a2 + a3);
-    float xn = sqrtf((n0 + n1) + (n2 + n3));
-    float den = qnorm * xn;
-    return den > 0.f ? ip / den : 0.f;
-}
-
-// The same arithmetic as exact_metric (same four fmaf chains per (query,row), so bit-identical results)
-// for QT queries at once: the row is read once for all of them.
 template <int QT>
 __device__ __forceinline__ void exact_metric_multi(const float* __restrict__ qs /*[QT][D]*/, const float* __restrict__ x,
                                                    int D, int metric, const float* __restrict__ qnorm, float (&out)[QT]) {
@@ -135,8 +99,20 @@ __device__ __forceinline__ float block_sum(float v, float* red /*[32]*/) {
 }
 
 // =====================================================================================================
-// per-row statistics at insert time: cosine scale 1/||x||, L2 bias -0.5||x||^2, running max ||x||
+// per-row statistics: cosine scale 1/||x||, L2 bias -0.5||x||^2, running max ||x|| and max | ||x||^2 - 1 |
 // =====================================================================================================
+// the statistics of row r from s = ||x||^2 (warp-strided fmaf sum), written by one thread.  Every path that writes
+// rows (add, upsert, remove) goes through here, so the scan and the certificate see the same numbers whichever wrote them.
+__device__ __forceinline__ void write_row_stats(long long r, float s, int metric, float* __restrict__ rscale,
+                                                float* __restrict__ rbias, unsigned* __restrict__ max_norm_bits,
+                                                unsigned* __restrict__ max_dev_bits) {
+    const float nrm = sqrtf(s);
+    if (metric == RMU_METRIC_COSINE) rscale[r] = nrm > 0.f ? 1.f / nrm : 0.f;
+    if (metric == RMU_METRIC_L2) rbias[r] = -0.5f * s;
+    atomicMax(max_norm_bits, __float_as_uint(nrm));  // non-negative floats order like uints
+    atomicMax(max_dev_bits, __float_as_uint(fabsf(s - 1.0f)));   // how far from unit norm the corpus gets
+}
+
 __global__ void row_stats_kernel(const float* __restrict__ x, long long row0, long long n, int D, int metric,
                                  float* __restrict__ rscale, float* __restrict__ rbias, unsigned* __restrict__ max_norm_bits,
                                  unsigned* __restrict__ max_dev_bits) {
@@ -147,13 +123,7 @@ __global__ void row_stats_kernel(const float* __restrict__ x, long long row0, lo
     float s = 0.f;
     for (int d = lane_id(); d < D; d += 32) s = fmaf(p[d], p[d], s);
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane_id() == 0) {
-        float nrm = sqrtf(s);
-        if (metric == RMU_METRIC_COSINE) rscale[row0 + r] = nrm > 0.f ? 1.f / nrm : 0.f;
-        if (metric == RMU_METRIC_L2) rbias[row0 + r] = -0.5f * s;
-        atomicMax(max_norm_bits, __float_as_uint(nrm));  // non-negative floats order like uints
-        atomicMax(max_dev_bits, __float_as_uint(fabsf(s - 1.0f)));   // how far from unit norm the corpus gets
-    }
+    if (lane_id() == 0) write_row_stats(row0 + r, s, metric, rscale, rbias, max_norm_bits, max_dev_bits);
 }
 
 // overwrite existing rows (upsert of a vector store): one warp per row copies the vector and refreshes its statistics
@@ -170,13 +140,7 @@ __global__ void set_rows_kernel(float* __restrict__ x, const long long* __restri
     float s = 0.f;
     for (int d = lane_id(); d < D; d += 32) { const float v = src[d]; dst[d] = v; s = fmaf(v, v, s); }
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane_id() == 0) {
-        const float nrm = sqrtf(s);
-        if (metric == RMU_METRIC_COSINE) rscale[r] = nrm > 0.f ? 1.f / nrm : 0.f;
-        if (metric == RMU_METRIC_L2) rbias[r] = -0.5f * s;
-        atomicMax(max_norm_bits, __float_as_uint(nrm));
-        atomicMax(max_dev_bits, __float_as_uint(fabsf(s - 1.0f)));
-    }
+    if (lane_id() == 0) write_row_stats(r, s, metric, rscale, rbias, max_norm_bits, max_dev_bits);
 }
 
 // =====================================================================================================
@@ -417,9 +381,10 @@ __global__ void __launch_bounds__(256) exact_scan_kernel(const ExactParams p) {
     }
 }
 
-// threads of the selection kernels (select_tau, finalize): their 8 radix passes over nlists * len keys are latency-bound,
-// one CTA per query
+// threads of the selection kernels (finalize, K2, the pool re-score): their 8 radix passes over nlists * len keys are
+// latency-bound, one CTA per query
 constexpr int kSelThreads = 512;
+constexpr int kSel2Max = 1024;                   // keys a selection kernel collects, sorts (and re-scores), at most
 
 // Block-wide radix select (8 bits per pass, most significant first) over passes [pass0, pass1): after pass 8 the
 // state holds the ksel-th largest non-zero key among load_key(0..total); after pass 4 its 32 score bits (the low
@@ -473,15 +438,55 @@ __device__ __forceinline__ unsigned long long block_radix_select(LoadKey load_ke
     return *s_remaining < 0 ? 1ull : *s_prefix;
 }
 
+// the non-zero keys >= T among load_key(0..total) into sel[0 .. kSel2Max), in no particular order; returns how many there
+// were (more than kSel2Max were not stored).  All threads call.
+template <typename LoadKey>
+__device__ __forceinline__ int block_collect(LoadKey load_key, long long total, unsigned long long T, unsigned long long* sel,
+                                             int* s_cnt) {
+    if (threadIdx.x == 0) *s_cnt = 0;
+    __syncthreads();
+    for (long long idx = threadIdx.x; idx < total; idx += blockDim.x) {
+        const unsigned long long key = load_key(idx);
+        if (key != 0ull && key >= T) { const int pos = atomicAdd(s_cnt, 1); if (pos < kSel2Max) sel[pos] = key; }
+    }
+    __syncthreads();
+    return *s_cnt;
+}
+
+// sort sel[0 .. n) descending (n <= kSel2Max), zero padded to a power of two >= 32.  All threads call.
+__device__ __forceinline__ void block_sort_desc(unsigned long long* sel, int n) {
+    int m2 = 32;
+    while (m2 < n) m2 <<= 1;
+    for (int i = n + threadIdx.x; i < m2; i += blockDim.x) sel[i] = 0ull;
+    block_bitonic_desc(sel, m2);
+}
+
+// row qg of the outputs [*, k] from the descending keys sel[0 .. n): scores in the metric's sign, ids id_offset + row;
+// past n missing results (score -inf, +inf for L2; id -1)
+__device__ __forceinline__ void write_topk(const unsigned long long* sel, int n, int qg, int k, int metric, long long id_offset,
+                                           float* out_scores, long long* out_ids) {
+    const float missing = metric == RMU_METRIC_L2 ? INFINITY : -INFINITY;
+    for (int j = threadIdx.x; j < k; j += blockDim.x) {
+        float s = missing;
+        long long id = -1;
+        if (j < n) {
+            const float rk = key_score(sel[j]);
+            s = metric == RMU_METRIC_L2 ? -rk : rk;
+            id = id_offset + key_row(sel[j]);
+        }
+        out_scores[static_cast<long long>(qg) * k + j] = s;
+        out_ids[static_cast<long long>(qg) * k + j] = id;
+    }
+}
+
 // =====================================================================================================
-// (3b) merge of the exact scan's per-chunk lists: select the best `ksel` keys, sort, write the top-k
+// (3b) merge of the exact scan's per-chunk lists: select the best `len` keys, sort, write the top-k
 // =====================================================================================================
 struct FinalizeParams {
     const unsigned long long* lists;   // [nlists][nq_total][len] exact keys, sorted per chunk, zero padded
     int nlists;        // lists per query
     int qstride;       // queries per list block
-    int len;           // entries per list, pow2
-    int ksel;          // keys to keep (<= 1024)
+    int len;           // entries per list and keys kept, pow2 <= kSel2Max
     int metric;
     const int* qmap;   // blockIdx.x -> query through qmap (nullable: identity)
     const int* nsel;   // number of valid blockIdx.x (nullable: all)
@@ -491,7 +496,7 @@ struct FinalizeParams {
 };
 
 __global__ void __launch_bounds__(kSelThreads) finalize_kernel(const FinalizeParams p) {
-    __shared__ unsigned long long cand[1024];
+    __shared__ unsigned long long cand[kSel2Max];
     __shared__ int hist[256];
     __shared__ int s_ncand;
     __shared__ unsigned long long s_prefix;
@@ -500,43 +505,18 @@ __global__ void __launch_bounds__(kSelThreads) finalize_kernel(const FinalizePar
     const int f = blockIdx.x;
     if (p.nsel != nullptr && f >= *p.nsel) return;
     const int qg = p.qmap ? p.qmap[f] : f;
-    const int tid = threadIdx.x;
 
-    const long long total = static_cast<long long>(p.nlists) * p.len;
     const int len_shift = __ffs(p.len) - 1;
+    const long long total = static_cast<long long>(p.nlists) << len_shift;
     auto load_key = [&](long long idx) -> unsigned long long {
         const long long l = idx >> len_shift;
         const int e = static_cast<int>(idx & (p.len - 1));
         return p.lists[(l * p.qstride + f) * p.len + e];
     };
-    const unsigned long long T = block_radix_select(load_key, total, p.ksel, hist, &s_prefix, &s_remaining, &s_ties);
-    if (tid == 0) s_ncand = 0;
-    __syncthreads();
-    for (long long idx = tid; idx < total; idx += blockDim.x) {
-        const unsigned long long key = load_key(idx);
-        if (key != 0ull && key >= T) {
-            const int pos = atomicAdd(&s_ncand, 1);
-            if (pos < 1024) cand[pos] = key;
-        }
-    }
-    __syncthreads();
-    const int ncand = min(s_ncand, p.ksel);
-    for (int c = ncand + tid; c < 1024; c += blockDim.x) cand[c] = 0ull;
-    int n2 = 32;
-    while (n2 < ncand) n2 <<= 1;
-    block_bitonic_desc(cand, n2);
-    const float missing = p.metric == RMU_METRIC_L2 ? INFINITY : -INFINITY;
-    for (int j = tid; j < p.k; j += blockDim.x) {
-        float s = missing;
-        long long id = -1;
-        if (j < ncand) {
-            const float rk = key_score(cand[j]);
-            s = p.metric == RMU_METRIC_L2 ? -rk : rk;
-            id = p.id_offset + key_row(cand[j]);
-        }
-        p.out_scores[static_cast<long long>(qg) * p.k + j] = s;
-        p.out_ids[static_cast<long long>(qg) * p.k + j] = id;
-    }
+    const unsigned long long T = block_radix_select(load_key, total, p.len, hist, &s_prefix, &s_remaining, &s_ties);
+    const int ncand = min(block_collect(load_key, total, T, cand, &s_ncand), p.len);
+    block_sort_desc(cand, ncand);
+    write_topk(cand, ncand, qg, p.k, p.metric, p.id_offset, p.out_scores, p.out_ids);
 }
 
 #include "rmu_scan.cuh"
@@ -665,7 +645,6 @@ __global__ void __launch_bounds__(128) mmr_kernel(const float* __restrict__ q, c
     double* norms = sim_q + fetch_k;       // [fetch_k]
     double* simmat = norms + fetch_k;      // [fetch_k * fetch_k]
     double* best_sel = simmat + fetch_k * fetch_k;  // [fetch_k] running max similarity to the selected set
-    __shared__ int s_sel[1];
     const int qi = blockIdx.x;
     const int n = n_cand ? min(n_cand[qi], fetch_k) : fetch_k;
     const float* qv = q + static_cast<long long>(qi) * dim;
@@ -732,7 +711,6 @@ __global__ void __launch_bounds__(128) mmr_kernel(const float* __restrict__ q, c
             for (int i = 0; i < n; ++i) best_sel[i] = fmax(best_sel[i], simmat[i * fetch_k + add]);
         }
         for (int j = nsel; j < k; ++j) out_sel[static_cast<long long>(qi) * k + j] = -1;
-        s_sel[0] = nsel;
     }
 }
 
@@ -790,13 +768,9 @@ struct ScanGeom { int nq, nstages; size_t smem; };
 constexpr int kPass2MaxQ = 256;         // flagged queries the second pass takes per search (more stay flagged)
 constexpr int kPass2PoolCap = 16384;    // rows a flagged query may collect; more -> the exact scan answers
 
-static int env_int(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }
-static int scan_kd() { static const int v = env_int("RMU_SCAN_KD", 2) == 1 ? 1 : 2; return v; }          // boxes per stage
-static int scan_stages_cap() { static const int v = env_int("RMU_SCAN_STAGES", 0); return v; }           // study: cap the ring
-
-template <int NQ, int KD>
+template <int NQ>
 static int scan_launch_t(const CUtensorMap& tx, const CUtensorMap& tq, const ScanParams& p, int grid, size_t smem, cudaStream_t st) {
-    auto kern = scan_rows_kernel<NQ, KD>;
+    auto kern = scan_rows_kernel<NQ>;
     // per device and cheap: set on every launch (a process may drive several GPUs); always the device maximum, so that
     // concurrent callers on other handles never lower it under a launch that needs more
     RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
@@ -807,18 +781,8 @@ static int scan_launch_t(const CUtensorMap& tx, const CUtensorMap& tq, const Sca
     return RMU_OK;
 }
 
-static int scan_dispatch(const ScanGeom& g, const CUtensorMap& tx, const CUtensorMap& tq, const ScanParams& p, int grid, cudaStream_t st) {
-    const int kd = scan_kd();
-#define RMU_SCAN_CASE(NQ)                                                                                        \
-    if (g.nq == NQ) return kd == 2 ? scan_launch_t<NQ, 2>(tx, tq, p, grid, g.smem, st) : scan_launch_t<NQ, 1>(tx, tq, p, grid, g.smem, st);
-    RMU_SCAN_CASE(64) RMU_SCAN_CASE(32) RMU_SCAN_CASE(16)
-#undef RMU_SCAN_CASE
-    set_error("scan: unsupported geometry");
-    return RMU_ERR_UNSUPPORTED;
-}
-
 // K blocks of the resident query operand: dim in 32-float blocks, padded to whole pipeline stages
-static int scan_qblocks(int dim) { const int kd = scan_kd(); return ((dim + 31) / 32 + kd - 1) / kd * kd; }
+static int scan_qblocks(int dim) { return ((dim + 31) / 32 + kScanKD - 1) / kScanKD * kScanKD; }
 
 // largest query block (MMA N) whose resident operand fits shared memory at this dimension; 0: dim too large (> 1536)
 static int scan_block_cap(int dim) {
@@ -837,13 +801,38 @@ static ScanGeom scan_geometry(int dim, int rem) {
     int nq = 16;
     while (nq < cap && nq < rem) nq <<= 1;
     const size_t qop = static_cast<size_t>(KB) * nq * 128;
-    const size_t stage = static_cast<size_t>(scan_kd()) * kBoxBytes;
+    const size_t stage = static_cast<size_t>(kScanKD) * kBoxBytes;
     const size_t budget = 227 * 1024 - 1024 - kScanStateBytes - qop;
     g.nq = nq;
     g.nstages = static_cast<int>(std::min<size_t>(budget / stage, kScanMaxStages));
-    if (scan_stages_cap() > 0) g.nstages = std::min(g.nstages, scan_stages_cap());
     g.smem = 1024 + qop + static_cast<size_t>(g.nstages) * stage + kScanStateBytes;
     return g;
+}
+
+// One scan launch on `grid` CTAs over the first `ntiles` tiles of the corpus: the `nq` queries at q (rows of dim floats,
+// 16-byte aligned) in a query block of geo.nq.  The caller sets in `sp` what differs between the first pass, the second
+// pass and the diagnostic tile (metric, lists, exchange groups, pool, dbg); the rest is set here, and every launch takes
+// a fresh exchange epoch.  idx->mu held, corpus tensor map current.
+static int scan_launch(rmu_index* idx, const ScanGeom& geo, const float* q, int nq, int grid, int ntiles, ScanParams& sp,
+                       cudaStream_t st) {
+    const int D = idx->dim;
+    CUtensorMap tq;
+    int rc = make_tmap_2d(&tq, q, static_cast<uint64_t>(nq), static_cast<uint64_t>(D), static_cast<uint64_t>(D) * sizeof(float),
+                          32, static_cast<uint32_t>(geo.nq), 4);
+    if (rc != RMU_OK) return rc;
+    sp.nq = nq; sp.dim = D; sp.n = idx->n; sp.ntiles = ntiles; sp.nstages = geo.nstages;
+    sp.rscale = idx->rscale; sp.rbias = idx->rbias; sp.stats_bits = idx->max_norm_bits; sp.gmax = idx->gmax;
+    sp.epoch = ++idx->epoch;
+    if (idx->epoch == 0xFFFFFFFFu) {                     // epoch wrap: start over from clean tags
+        RMU_CUDA(cudaMemsetAsync(idx->gmax, 0, sizeof(unsigned long long) * 256 * kGroupsMax, st));
+        idx->epoch = 0;
+        sp.epoch = ++idx->epoch;
+    }
+    if (geo.nq == 64) return scan_launch_t<64>(idx->tmap, tq, sp, grid, geo.smem, st);
+    if (geo.nq == 32) return scan_launch_t<32>(idx->tmap, tq, sp, grid, geo.smem, st);
+    if (geo.nq == 16) return scan_launch_t<16>(idx->tmap, tq, sp, grid, geo.smem, st);
+    set_error("scan: unsupported geometry");
+    return RMU_ERR_UNSUPPORTED;
 }
 
 extern "C" {
@@ -1100,28 +1089,16 @@ int rmu_index_search(rmu_index* idx, const float* queries, int nq, int k, int64_
         rc = ensure_corpus_tmap(idx);
         if (rc != RMU_OK) return rc;
         const int ntiles = static_cast<int>((N + kTileRows - 1) / kTileRows);
+        const int grid = std::min(idx->sms, ntiles);       // one CTA per SM
         for (int q0 = 0; q0 < nq;) {
             const ScanGeom geo = scan_geometry(D, nq - q0);
             const int nql = std::min(nq - q0, geo.nq);
-            const int grid = std::min(idx->sms, ntiles);   // one CTA per SM
             const float* qbase = queries + static_cast<size_t>(q0) * D;
-            CUtensorMap tq;
-            rc = make_tmap_2d(&tq, qbase, static_cast<uint64_t>(nql), static_cast<uint64_t>(D),
-                              static_cast<uint64_t>(D) * sizeof(float), 32, static_cast<uint32_t>(geo.nq), 4);
-            if (rc != RMU_OK) return rc;
             ScanParams sp{};
-            sp.nq = nql; sp.dim = D; sp.n = N; sp.ntiles = ntiles; sp.nstages = geo.nstages; sp.metric = idx->metric;
-            sp.rscale = idx->rscale; sp.rbias = idx->rbias; sp.stats_bits = idx->max_norm_bits;
-            sp.lists = d_scan; sp.counts = d_cnt; sp.floors = d_floor; sp.gmax = idx->gmax;
-            sp.epoch = ++idx->epoch;
-            if (idx->epoch == 0xFFFFFFFFu) {                 // epoch wrap: start over from clean tags
-                RMU_CUDA(cudaMemsetAsync(idx->gmax, 0, sizeof(unsigned long long) * 256 * kGroupsMax, st));
-                idx->epoch = 0;
-                sp.epoch = ++idx->epoch;
-            }
+            sp.metric = idx->metric; sp.lists = d_scan; sp.counts = d_cnt; sp.floors = d_floor;
             sp.groups = keep / kPubRank;                      // 16 * groups >= keep rows score >= the exchanged threshold
             if (grid < 2 * sp.groups) sp.groups = 0;          // small grids: lists are cut only by their own floors
-            rc = scan_dispatch(geo, idx->tmap, tq, sp, grid, st);
+            rc = scan_launch(idx, geo, qbase, nql, grid, ntiles, sp, st);
             if (rc != RMU_OK) return rc;
             ++scan_launches;
             SelectParams fp{};
@@ -1134,7 +1111,7 @@ int rmu_index_search(rmu_index* idx, const float* queries, int nq, int k, int64_
             const size_t sel_smem = sizeof(unsigned long long) * kSel2Cap + static_cast<size_t>(D) * sizeof(float);
             RMU_CUDA(cudaFuncSetAttribute(select_rescore_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
             { ProfScope _ps(PROF_FINALIZE, st);
-            select_rescore_kernel<<<nql, kSel2Threads, sel_smem, st>>>(fp); }
+            select_rescore_kernel<<<nql, kSelThreads, sel_smem, st>>>(fp); }
             count_launch();
             RMU_CHECK_LAUNCH();
             q0 += nql;
@@ -1153,27 +1130,20 @@ int rmu_index_search(rmu_index* idx, const float* queries, int nq, int k, int64_
             for (int j0 = 0; j0 < p2max;) {
                 const ScanGeom geo = scan_geometry(D, p2max - j0);
                 const int nql = std::min(p2max - j0, geo.nq);
-                const int grid = std::min(idx->sms, ntiles);
-                CUtensorMap tq;
-                rc = make_tmap_2d(&tq, d_qbuf + static_cast<size_t>(j0) * D, static_cast<uint64_t>(nql), static_cast<uint64_t>(D),
-                                  static_cast<uint64_t>(D) * sizeof(float), 32, static_cast<uint32_t>(geo.nq), 4);
-                if (rc != RMU_OK) return rc;
-                ScanParams sp{};
-                sp.nq = nql; sp.dim = D; sp.n = N; sp.ntiles = ntiles; sp.nstages = geo.nstages; sp.metric = idx->metric;
-                sp.rscale = idx->rscale; sp.rbias = idx->rbias; sp.stats_bits = idx->max_norm_bits;
-                sp.lists = d_scan; sp.counts = d_cnt; sp.floors = d_floor; sp.gmax = idx->gmax; sp.epoch = idx->epoch; sp.groups = 0;
+                ScanParams sp{};                              // pool mode: no lists, no exchange
+                sp.metric = idx->metric;
                 sp.fixed_tau = d_taub + j0; sp.pool = d_pool + static_cast<size_t>(j0) * kPass2PoolCap; sp.pool_cnt = d_pcnt + j0;
                 sp.pool_cap = kPass2PoolCap; sp.nq_dev = d_nsel; sp.q_off = j0;
-                rc = scan_dispatch(geo, idx->tmap, tq, sp, grid, st);
+                rc = scan_launch(idx, geo, d_qbuf + static_cast<size_t>(j0) * D, nql, grid, ntiles, sp, st);
                 if (rc != RMU_OK) return rc;
                 j0 += nql;
             }
             PoolParams pp{};
-            pp.pool = d_pool; pp.pool_cnt = d_pcnt; pp.pool_cap = kPass2PoolCap; pp.qmap = d_qmap; pp.nsel = d_nsel; pp.max_slots = p2max;
+            pp.pool = d_pool; pp.pool_cnt = d_pcnt; pp.pool_cap = kPass2PoolCap; pp.qmap = d_qmap; pp.nsel = d_nsel;
             pp.x = idx->x; pp.dim = D; pp.metric = idx->metric; pp.q = queries; pp.k = k; pp.id_offset = id_offset;
             pp.out_scores = out_scores; pp.out_ids = reinterpret_cast<long long*>(out_ids); pp.flags = d_flags;
             { ProfScope _ps(PROF_FINALIZE, st);
-            pool_rescore_kernel<<<p2max, kSel2Threads, static_cast<size_t>(D) * sizeof(float), st>>>(pp); }
+            pool_rescore_kernel<<<p2max, kSelThreads, static_cast<size_t>(D) * sizeof(float), st>>>(pp); }
             count_launch();
             RMU_CHECK_LAUNCH();
             compact_flags_kernel<<<1, 32, 0, st>>>(d_flags, nq, d_qmap2, d_nsel2);
@@ -1184,7 +1154,7 @@ int rmu_index_search(rmu_index* idx, const float* queries, int nq, int k, int64_
 
     if (!tensor_ok || mode == RMU_SEARCH_AUTO) {
         FinalizeParams fp{};
-        fp.lists = d_exact; fp.qstride = nq; fp.len = keepx; fp.ksel = keepx; fp.metric = idx->metric;
+        fp.lists = d_exact; fp.qstride = nq; fp.len = keepx; fp.metric = idx->metric;
         fp.k = k; fp.id_offset = id_offset;
         fp.out_scores = out_scores; fp.out_ids = reinterpret_cast<long long*>(out_ids);
         if (N > 0) {
@@ -1246,20 +1216,13 @@ int rmu_debug_scan_tile(rmu_index* idx, const float* queries, int nq, float* out
     if (rc != RMU_OK) return rc;
     rc = ensure_corpus_tmap(idx);
     if (rc != RMU_OK) return rc;
-    ScanGeom geo = scan_geometry(idx->dim, kScanMaxQ);
-    CUtensorMap tq;
-    rc = make_tmap_2d(&tq, queries, static_cast<uint64_t>(nq), static_cast<uint64_t>(idx->dim),
-                      static_cast<uint64_t>(idx->dim) * sizeof(float), 32, static_cast<uint32_t>(geo.nq), 4);
-    if (rc != RMU_OK) return rc;
     ScanParams sp{};
-    sp.nq = nq; sp.dim = idx->dim; sp.n = idx->n; sp.ntiles = 2; sp.nstages = geo.nstages; sp.metric = RMU_METRIC_IP;
-    sp.stats_bits = idx->max_norm_bits;
+    sp.metric = RMU_METRIC_IP;
     sp.lists = static_cast<unsigned long long*>(idx->ws);
     sp.counts = reinterpret_cast<int*>(static_cast<uint8_t*>(idx->ws) + lists);
     sp.floors = reinterpret_cast<float*>(sp.counts + 128);
-    sp.gmax = idx->gmax; sp.epoch = ++idx->epoch; sp.groups = 0;
     sp.dbg = out;
-    rc = scan_dispatch(geo, idx->tmap, tq, sp, 2, st);
+    rc = scan_launch(idx, scan_geometry(idx->dim, kScanMaxQ), queries, nq, 2, 2, sp, st);
     RMU_CUDA(cudaEventRecord(idx->ws_done, st));
     return rc;
 }

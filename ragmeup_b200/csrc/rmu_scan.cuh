@@ -1,5 +1,6 @@
 // Coarse top-k scan of the flat index (sm_90a) and its selection kernel.  Included by rmu_index.cu inside
-// namespace rmu, after exact_metric / block_bitonic_desc / block_radix_select / warp_bitonic_desc.
+// namespace rmu, after block_sum / warp_bitonic_desc / block_radix_select and the top-k tail (block_collect,
+// block_sort_desc, write_topk).
 //
 // Stands behind the reference's brute-force search (col.search of the retriever built at
 // server/RAGHelper.py:497-499; Milvus-lite FLAT / pgvector sequential scan on the CPU).
@@ -38,6 +39,7 @@ constexpr int kPubRank = 16;                     // the published key of a list:
 constexpr int kGroupsMax = 16;                   // gmax row length; KSEL <= 16 * kPubRank = 256
 constexpr int kScanStateBytes = 2048;            // mbarriers + per-query state behind the ring
 constexpr int kScanQOpMax = 96 * 1024;           // shared memory the resident query operand may take
+constexpr int kScanKD = 2;                       // boxes (128-byte K blocks) per pipeline stage
 constexpr int kScanMaxStages = 16;
 constexpr int kScanMaxQ = 64;                    // queries per launch (MMA N)
 
@@ -99,9 +101,10 @@ __device__ __forceinline__ void scan_mma(float (&acc)[NQ / 2], uint64_t a, uint6
 }
 
 // Accumulator element d[4 j + 2 h + e] of a thread is (row rsub + 8 h of its warpgroup's 64, query 8 j + 2 (lane % 4) + e).
-template <int NQ, int KD>
+template <int NQ>
 __global__ void __launch_bounds__(kScanThreads, 1)
 scan_rows_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_q, const ScanParams p) {
+    constexpr int KD = kScanKD;
     constexpr int STAGE_BYTES = KD * kBoxBytes;
     constexpr int QBLK_BYTES = NQ * 128;                 // one K block of the query operand
     constexpr int NACC = NQ / 2;
@@ -309,9 +312,7 @@ scan_rows_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
 // selection: union of the (cluster, query) lists -> best KSEL coarse candidates -> exact fp32 re-score ->
 // sort -> top-k + certificate.  One CTA per query.
 // =====================================================================================================
-constexpr int kSel2Threads = 512;
 constexpr int kSel2Cap = 16384;                  // candidates gathered into shared memory (128 KB); more -> radix select over the lists
-constexpr int kSel2Max = 1024;                   // coarse candidates re-scored exactly, at most
 
 struct SelectParams {
     const unsigned long long* lists; const int* counts; const float* floors; const unsigned long long* gmax;
@@ -328,9 +329,9 @@ struct SelectParams {
     float* tau2;               // [nq] per query: the coarse-key threshold a second pass must use when the query is flagged
 };
 
-// exact_metric with the four fmaf chains of one (query, row) pair spread over the four lanes of a quad (lane & 3 = chain):
-// every chain sees the same elements in the same order and the partial sums are combined as (a0 + a1) + (a2 + a3), so the
-// result is bit-identical to exact_metric.  All four lanes return the value.
+// exact_metric_multi with the four fmaf chains of one (query, row) pair spread over the four lanes of a quad (lane & 3 =
+// chain): every chain sees the same elements in the same order and the partial sums are combined as (a0 + a1) + (a2 + a3),
+// so the result is bit-identical to exact_metric_multi's.  All four lanes return the value.
 __device__ __forceinline__ float exact_metric_quad(const float* __restrict__ q, const float* __restrict__ x, int D, int metric,
                                                    float qnorm) {
     const int c = static_cast<int>(lane_id() & 3u);
@@ -362,7 +363,36 @@ __device__ __forceinline__ float exact_metric_quad(const float* __restrict__ q, 
     return den > 0.f ? s / den : 0.f;
 }
 
-__global__ void __launch_bounds__(kSel2Threads) select_rescore_kernel(const SelectParams p) {
+// copy query q [dim] to shared memory and return ||q||, summed in the order of exact_scan_kernel (256 threads, stride 256,
+// then block_sum) so that the cosine scores of the re-scores and of the exact scan are bit-identical.  All threads call.
+__device__ __forceinline__ float stage_query(const float* __restrict__ q, int dim, float* qs, float* red /*[32]*/) {
+    float part = 0.f;
+    if (threadIdx.x < 256) {
+        for (int d = threadIdx.x; d < dim; d += 256) {
+            const float v = q[d];
+            qs[d] = v;
+            part = fmaf(v, v, part);
+        }
+    }
+    return sqrtf(block_sum(part, red));
+}
+
+// exact re-score in place of keys[0 .. n): coarse key -> exact key of the same row, a quad of lanes per candidate (the
+// same arithmetic as the exact scan: bit-identical scores).  All threads call.
+__device__ __forceinline__ void rescore_keys(unsigned long long* keys, int n, const float* qs, float qnorm, const float* x, int dim,
+                                             int metric) {
+    const int tid = threadIdx.x;
+    for (int c0 = 0; c0 < n; c0 += kSelThreads / 4) {
+        const int c = c0 + (tid >> 2);
+        const bool live = c < n;
+        const uint32_t row = live ? key_row(keys[c]) : 0u;
+        const float v = exact_metric_quad(qs, x + static_cast<long long>(row) * dim, dim, metric, qnorm);
+        __syncwarp();
+        if (live && (tid & 3) == 0) keys[c] = make_key(metric_to_rank(v, metric), row);
+    }
+}
+
+__global__ void __launch_bounds__(kSelThreads) select_rescore_kernel(const SelectParams p) {
     __shared__ unsigned long long sel[kSel2Max];
     __shared__ int hist[256];
     __shared__ float red[32];
@@ -378,17 +408,7 @@ __global__ void __launch_bounds__(kSel2Threads) select_rescore_kernel(const Sele
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
 
-    // ||q|| in the summation order of exact_scan_kernel (256 threads, stride 256), so that cosine scores of the
-    // two paths are bit-identical
-    float part = 0.f;
-    if (tid < 256) {
-        for (int d = tid; d < p.dim; d += 256) {
-            const float v = p.q[static_cast<long long>(f) * p.dim + d];
-            qs[d] = v;
-            part = fmaf(v, v, part);
-        }
-    }
-    const float qnorm = sqrtf(block_sum(part, red));
+    const float qnorm = stage_query(p.q + static_cast<long long>(f) * p.dim, p.dim, qs, red);
 
     // ---- what the scan may have rejected: everything <= tau (exchange) or <= a list's floor (cuts)
     if (tid == 0) {
@@ -402,7 +422,6 @@ __global__ void __launch_bounds__(kSel2Threads) select_rescore_kernel(const Sele
         }
         s_tau = tg;
         s_n = 0;
-        s_nsel = 0;
     }
     float fl = -INFINITY;
     for (int c = tid; c < p.ncl; c += blockDim.x) fl = fmaxf(fl, p.floors[c * p.qb + f]);
@@ -411,13 +430,13 @@ __global__ void __launch_bounds__(kSel2Threads) select_rescore_kernel(const Sele
     if (lane == 0) red[warp] = fl;
     __syncthreads();
     fl = red[0];
-    for (int w = 1; w < kSel2Threads / 32; ++w) fl = fmaxf(fl, red[w]);
+    for (int w = 1; w < kSelThreads / 32; ++w) fl = fmaxf(fl, red[w]);
     const float tau = s_tau;
     float bound = fmaxf(tau, fl);                // coarse upper bound of every row that is in no list
     __syncthreads();
 
     // ---- gather the entries above tau (two lists per warp step: the count loads of both are in flight together)
-    for (int c = 2 * warp; c < p.ncl; c += 2 * (kSel2Threads / 32)) {
+    for (int c = 2 * warp; c < p.ncl; c += 2 * (kSelThreads / 32)) {
         const int n0 = p.counts[c * p.qb + f];
         const int n1 = c + 1 < p.ncl ? p.counts[(c + 1) * p.qb + f] : 0;
         const unsigned long long* b0 = p.lists + static_cast<size_t>(c * p.qb + f) * kListCap;
@@ -442,11 +461,7 @@ __global__ void __launch_bounds__(kSel2Threads) select_rescore_kernel(const Sele
         if (n <= kSel2Cap) {
             auto load_key = [&](long long idx) -> unsigned long long { return cand[idx]; };
             T = block_radix_select(load_key, n, p.ksel, hist, &s_prefix, &s_remaining, &s_ties);
-            __syncthreads();
-            for (int i = tid; i < n; i += blockDim.x) {
-                const unsigned long long key = cand[i];
-                if (key >= T) { const int pos = atomicAdd(&s_nsel, 1); if (pos < kSel2Max) sel[pos] = key; }
-            }
+            ncand = block_collect(load_key, n, T, sel, &s_nsel);
         } else {
             const long long total = static_cast<long long>(p.ncl) * kListCap;
             auto load_key = [&](long long idx) -> unsigned long long {
@@ -456,47 +471,17 @@ __global__ void __launch_bounds__(kSel2Threads) select_rescore_kernel(const Sele
                 return key_score(key) > tau ? key : 0ull;
             };
             T = block_radix_select(load_key, total, p.ksel, hist, &s_prefix, &s_remaining, &s_ties);
-            __syncthreads();
-            for (long long idx = tid; idx < total; idx += blockDim.x) {
-                const unsigned long long key = load_key(idx);
-                if (key != 0ull && key >= T) { const int pos = atomicAdd(&s_nsel, 1); if (pos < kSel2Max) sel[pos] = key; }
-            }
+            ncand = block_collect(load_key, total, T, sel, &s_nsel);
         }
-        __syncthreads();
-        ncand = min(s_nsel, p.ksel);
+        ncand = min(ncand, p.ksel);
         bound = fmaxf(bound, key_score(T));      // list entries that were not selected are below T
     }
     __syncthreads();
 
-    // ---- exact re-score, a quad of lanes per candidate (the same arithmetic as the exact scan: bit-identical scores)
-    for (int c0 = 0; c0 < ncand; c0 += kSel2Threads / 4) {
-        const int c = c0 + (tid >> 2);
-        const bool live = c < ncand;
-        const uint32_t row = live ? key_row(sel[c]) : 0u;
-        const float v = exact_metric_quad(qs, p.x + static_cast<long long>(row) * p.dim, p.dim, p.metric, qnorm);
-        __syncwarp();
-        if (live && (tid & 3) == 0) sel[c] = make_key(metric_to_rank(v, p.metric), row);
-    }
-    int m2 = 32;
-    while (m2 < ncand) m2 <<= 1;
-    __syncthreads();
-    for (int i = ncand + tid; i < m2; i += blockDim.x) sel[i] = 0ull;
-    block_bitonic_desc(sel, m2);
-
-    // ---- outputs
+    rescore_keys(sel, ncand, qs, qnorm, p.x, p.dim, p.metric);
+    block_sort_desc(sel, ncand);
     const int qg = p.q0 + f;
-    const float missing = p.metric == RMU_METRIC_L2 ? INFINITY : -INFINITY;
-    for (int j = tid; j < p.k; j += blockDim.x) {
-        float s = missing;
-        long long id = -1;
-        if (j < ncand) {
-            const float rk = key_score(sel[j]);
-            s = p.metric == RMU_METRIC_L2 ? -rk : rk;
-            id = p.id_offset + key_row(sel[j]);
-        }
-        p.out_scores[static_cast<long long>(qg) * p.k + j] = s;
-        p.out_ids[static_cast<long long>(qg) * p.k + j] = id;
-    }
+    write_topk(sel, ncand, qg, p.k, p.metric, p.id_offset, p.out_scores, p.out_ids);
     // ---- certificate: every row outside the candidate set has coarse key <= bound; its exact key is at
     //      most eps above.  The k-th exact candidate must beat that strictly.
     if (tid == 0 && p.flags != nullptr) {
@@ -540,7 +525,7 @@ __global__ void pool_prepare_kernel(const float* __restrict__ q, const int* __re
 
 struct PoolParams {
     unsigned long long* pool; const int* pool_cnt; int pool_cap;
-    const int* qmap; const int* nsel; int max_slots;   // flagged queries beyond max_slots stay flagged
+    const int* qmap; const int* nsel;   // the grid has a block per slot: flagged queries beyond it stay flagged
     const float* x; int dim; int metric;
     const float* q;            // all queries [nq, dim]
     int k; long long id_offset;
@@ -549,7 +534,7 @@ struct PoolParams {
 
 // block j: every row of the pool (a superset of the rows whose exact score can reach the k-th) is re-scored exactly in
 // place, the best k are selected; the result is the exact top-k.  A pool that overflowed leaves the query flagged.
-__global__ void __launch_bounds__(kSel2Threads) pool_rescore_kernel(const PoolParams p) {
+__global__ void __launch_bounds__(kSelThreads) pool_rescore_kernel(const PoolParams p) {
     __shared__ unsigned long long sel[kSel2Max];
     __shared__ int hist[256];
     __shared__ float red[32];
@@ -560,54 +545,16 @@ __global__ void __launch_bounds__(kSel2Threads) pool_rescore_kernel(const PoolPa
     const int j = blockIdx.x;
     if (j >= *p.nsel) return;
     const int qg = p.qmap[j];
-    const int tid = threadIdx.x;
-    if (j >= p.max_slots) return;                // never scanned: stays flagged
     const int n = p.pool_cnt[j];
     if (n > p.pool_cap) return;                  // overflow: stays flagged, the exact scan answers
-    float part = 0.f;
-    if (tid < 256) {
-        for (int d = tid; d < p.dim; d += 256) {
-            const float v = p.q[static_cast<size_t>(qg) * p.dim + d];
-            pqs[d] = v;
-            part = fmaf(v, v, part);
-        }
-    }
-    const float qnorm = sqrtf(block_sum(part, red));
-    if (tid == 0) s_nsel = 0;
+    const float qnorm = stage_query(p.q + static_cast<size_t>(qg) * p.dim, p.dim, pqs, red);
     unsigned long long* pool = p.pool + static_cast<size_t>(j) * p.pool_cap;
-    for (int c0 = 0; c0 < n; c0 += kSel2Threads / 4) {
-        const int c = c0 + (tid >> 2);
-        const bool live = c < n;
-        const uint32_t row = live ? key_row(pool[c]) : 0u;
-        const float v = exact_metric_quad(pqs, p.x + static_cast<long long>(row) * p.dim, p.dim, p.metric, qnorm);
-        __syncwarp();
-        if (live && (tid & 3) == 0) pool[c] = make_key(metric_to_rank(v, p.metric), row);
-    }
+    rescore_keys(pool, n, pqs, qnorm, p.x, p.dim, p.metric);
     __syncthreads();
     auto load_key = [&](long long idx) -> unsigned long long { return pool[idx]; };
     const unsigned long long T = block_radix_select(load_key, n, p.k, hist, &s_prefix, &s_remaining, &s_ties);
-    __syncthreads();
-    for (int i = tid; i < n; i += blockDim.x) {
-        const unsigned long long key = pool[i];
-        if (key >= T) { const int pos = atomicAdd(&s_nsel, 1); if (pos < kSel2Max) sel[pos] = key; }
-    }
-    __syncthreads();
-    const int ncand = min(s_nsel, p.k);
-    int m2 = 32;
-    while (m2 < min(s_nsel, kSel2Max)) m2 <<= 1;
-    for (int i = min(s_nsel, kSel2Max) + tid; i < m2; i += blockDim.x) sel[i] = 0ull;
-    block_bitonic_desc(sel, m2);
-    const float missing = p.metric == RMU_METRIC_L2 ? INFINITY : -INFINITY;
-    for (int jj = tid; jj < p.k; jj += blockDim.x) {
-        float sc = missing;
-        long long id = -1;
-        if (jj < ncand) {
-            const float rk = key_score(sel[jj]);
-            sc = p.metric == RMU_METRIC_L2 ? -rk : rk;
-            id = p.id_offset + key_row(sel[jj]);
-        }
-        p.out_scores[static_cast<long long>(qg) * p.k + jj] = sc;
-        p.out_ids[static_cast<long long>(qg) * p.k + jj] = id;
-    }
-    if (tid == 0) p.flags[qg] = 0;               // answered exactly
+    const int nsel = block_collect(load_key, n, T, sel, &s_nsel);
+    block_sort_desc(sel, min(nsel, kSel2Max));   // everything collected is sorted, the best k are written
+    write_topk(sel, min(nsel, p.k), qg, p.k, p.metric, p.id_offset, p.out_scores, p.out_ids);
+    if (threadIdx.x == 0) p.flags[qg] = 0;       // answered exactly
 }

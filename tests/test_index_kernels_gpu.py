@@ -7,7 +7,6 @@ references are oracle/flat_kernels_ref.py (pinned on the CPU by tests/test_flat_
 Error unit u = 2^-24.  Each bound's constant is derived next to it; the measured worst ratios are printed (-s) and
 recorded in DESIGN.md section 2."""
 import math
-import os
 
 import numpy as np
 import pytest
@@ -35,21 +34,13 @@ def _modes():
 
 def _block_cap(D):
     """queries per K1 launch at dim D (scan_block_cap): the resident operand, ceil(D / 32) K blocks padded to whole stages
-    of KD blocks (KD = 2, or 1 when RMU_SCAN_KD=1, as the library reads it) of NQ x 128 bytes each, must fit 96 KB;
-    0 = D goes to K3"""
-    kd = 1 if os.environ.get("RMU_SCAN_KD") is not None and _atoi(os.environ["RMU_SCAN_KD"]) == 1 else 2
+    of KD = 2 blocks of NQ x 128 bytes each, must fit 96 KB; 0 = D goes to K3"""
+    kd = 2
     kb = ((D + 31) // 32 + kd - 1) // kd * kd
     cap = 64
     while cap >= 16 and kb * cap * 128 > 96 * 1024:
         cap //= 2
     return cap if cap >= 16 else 0
-
-
-def _atoi(v):
-    """C atoi: the leading integer of the string, 0 when there is none"""
-    import re
-    m = re.match(r"\s*[+-]?\d+", v)
-    return int(m.group()) if m else 0
 
 
 def _index(x, metric):
