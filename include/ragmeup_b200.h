@@ -174,7 +174,10 @@ typedef struct rmu_bert_config {
 typedef struct rmu_encoder rmu_encoder;
 
 /* weights_h: host fp32 arrays in the canonical order documented in ragmeup_b200/encoder.py
- * (HuggingFace BertModel tensor order; pooler + classifier last when has_head). */
+ * (HuggingFace BertModel tensor order; pooler + classifier last when has_head).  The GEMM weights (query, key, value,
+ * attention output, intermediate, output) are held as split fp16 planes, which cannot hold |w| >= 65520: such an
+ * element (infinities included) returns RMU_ERR_UNSUPPORTED before any CUDA call.  Embedding tables, biases, LayerNorm
+ * parameters and the pooler / classifier stay fp32 and are not limited. */
 int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* weights_h, int n_weights, int has_head,
                        rmu_encoder** out);
 void rmu_encoder_destroy(rmu_encoder* enc);
@@ -182,12 +185,18 @@ void rmu_encoder_destroy(rmu_encoder* enc);
 #define RMU_POOL_MEAN 0
 #define RMU_POOL_CLS 1
 
-/* ragged batch: ids/type_ids [total_tokens] int32, cu_seqlens [B+1] int32 (all device).
- * out [B, hidden] fp32 sentence embeddings. */
+/* ragged batch: ids/type_ids [total_tokens] int32, cu_seqlens [B+1] int32 (all device); type_ids may be null (all 0).
+ * max_seqlen must be at least the longest sequence in cu_seqlens; only max_seqlen itself is checked against
+ * max_position_embeddings (cu_seqlens is on the device).  Out-of-range inputs are clamped on the device, where
+ * HuggingFace raises an IndexError: token ids into [0, vocab_size), type ids into [0, type_vocab), and positions past
+ * max_position_embeddings - 1 take that last row.  An empty sequence (cu_seqlens[b + 1] == cu_seqlens[b]) is allowed.
+ * These rules hold for every rmu_encoder_* entry point below.
+ * out [B, hidden] fp32 sentence embeddings; an empty sequence gets a zero vector. */
 int rmu_encoder_embed(rmu_encoder* enc, const int32_t* ids, const int32_t* type_ids, const int32_t* cu_seqlens,
                       int B, int total_tokens, int max_seqlen, int pool_mode, int normalize, float* out,
                       void* stream);
-/* cross-encoder logits: out [B, num_labels] fp32 (raw logits; activation is the caller's) */
+/* cross-encoder logits: out [B, num_labels] fp32 (raw logits; activation is the caller's).  An empty sequence has a
+ * zero CLS hidden state: its logits are W_c tanh(b_p) + b_c. */
 int rmu_encoder_classify(rmu_encoder* enc, const int32_t* ids, const int32_t* type_ids, const int32_t* cu_seqlens,
                          int B, int total_tokens, int max_seqlen, float* out, void* stream);
 /* last hidden state [total_tokens, hidden] fp32 (tests / provenance) */
@@ -227,6 +236,27 @@ int rmu_debug_attention(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const in
  * H % 128 == 0, H <= 1024. */
 int rmu_debug_layernorm(const float* pre, int T, int H, const float* gamma, const float* beta, float eps,
                         uint16_t* out_hi, uint16_t* out_lo, void* stream);
+/* For tests: E3 embed_ln_kernel on fp32 tables word [vocab, H], pos [max_pos, H], typ [type_vocab, H], ids / type_ids
+ * [T] int32 (type_ids null = all 0) and cu_seqlens [B+1] -> LayerNorm(word + typ + pos) planes [T, H], clamping ids,
+ * type ids and positions as rmu_encoder_embed does.  H % 128 == 0, H <= 1024; null pointers (but type_ids) and B, T,
+ * vocab, max_pos or type_vocab < 1 return RMU_ERR_ARG. */
+int rmu_debug_embed_ln(const int32_t* ids, const int32_t* type_ids, const int32_t* cu_seqlens, int B, int T, int H,
+                       int vocab, int max_pos, int type_vocab, const float* word, const float* pos, const float* typ,
+                       const float* gamma, const float* beta, float eps, uint16_t* out_hi, uint16_t* out_lo, void* stream);
+/* For tests: E4 pool_kernel, RMU_POOL_MEAN or RMU_POOL_CLS of planes [T, H] per sequence of cu_seqlens [B+1], then
+ * x / max(||x||, 1e-12) when normalize -> out [B, H] fp32 (an empty sequence gives zeros).  1 <= H <= 1024. */
+int rmu_debug_pool(const uint16_t* hi, const uint16_t* lo, const int32_t* cu_seqlens, int B, int H, int pool_mode,
+                   int normalize, float* out, void* stream);
+/* For tests: E4 cls_head_kernel on planes [T, H] and cu_seqlens [B+1] (h_cls = row cu_seqlens[b], 0 for an empty
+ * sequence), pooler pw [H, H] / pb [H], classifier cw [num_labels, H] / cb [num_labels] fp32 -> out [B, num_labels]
+ * = cw tanh(pw h_cls + pb) + cb.  1 <= H <= 1024. */
+int rmu_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const int32_t* cu_seqlens, int B, int H, int num_labels,
+                       const float* pw, const float* pb, const float* cw, const float* cb, float* out, void* stream);
+/* For tests: n fp32 values -> (hi, lo) planes, as every GEMM weight is uploaded; and hi + lo -> n fp32 values, as
+ * rmu_encoder_hidden returns the last hidden state.  n < 0 or a null pointer return RMU_ERR_ARG; n = 0 launches
+ * nothing. */
+int rmu_debug_split_planes(const float* src, int64_t n, uint16_t* hi, uint16_t* lo, void* stream);
+int rmu_debug_join_planes(const uint16_t* hi, const uint16_t* lo, int64_t n, float* out, void* stream);
 /* For tests: the BM25 select stage alone (bm25_select_kernel rounds, through the launcher rmu_bm25_search uses) on
  * caller-owned candidate lists: scores [Q, m] float64 and idx [Q, m] int32 document numbers (-1 = absent), each row
  * ascending in document number among its present entries, as stage 1 leaves them.  Scores hold no NaN and no -0.0 (the

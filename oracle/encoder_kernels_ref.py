@@ -8,7 +8,12 @@ reference is the kernel's own arithmetic:
 
 * ``gemm_ref``: E1 ``gemm_f16x3_kernel``, sum_k (ah wh + al wh + ah wl) and the four epilogues;
 * ``attention_ref``: E2 ``attention_planes_kernel``, base-2 softmax over the keys of the same sequence;
-* ``layernorm_ref``: E3 ``ln_kernel``, two-pass LayerNorm, biased variance, eps inside the square root.
+* ``layernorm_ref``: E3 ``ln_kernel``, two-pass LayerNorm, biased variance, eps inside the square root;
+* ``embed_ln_ref``: E3 ``embed_ln_kernel``, word + token-type + position rows (clamped as the kernel clamps), then
+  ``layernorm_ref``;
+* ``pool_ref``: E4 ``pool_kernel``, mean or CLS pooling and the optional L2 normalisation (sentence-transformers
+  Pooling + Normalize);
+* ``cls_head_ref``: E4 ``cls_head_kernel``, BertPooler tanh(W_p h_cls + b_p) and the classifier.
 """
 from __future__ import annotations
 
@@ -104,3 +109,70 @@ def layernorm_ref(x, gamma, beta, eps: float) -> tuple[torch.Tensor, torch.Tenso
     sigma = torch.sqrt(var + float(np.float32(eps)))
     xhat = (x - mu) / sigma
     return xhat * _f64(gamma)[None, :] + _f64(beta)[None, :], xhat, sigma
+
+
+def _long(x, device) -> torch.Tensor:
+    return (x if isinstance(x, torch.Tensor) else torch.from_numpy(np.asarray(x))).to(device=device, dtype=torch.int64)
+
+
+def embed_ln_ref(ids, type_ids, cu, word, pos, typ, gamma, beta, eps: float):
+    """E3 ``embed_ln_kernel`` on the fp32 tables word [vocab, H], pos [max_pos, H], typ [type_vocab, H] for the ragged
+    batch `cu` (type_ids None = all 0).  Token ids are clamped into [0, vocab), type ids into [0, type_vocab) and
+    positions (the token's offset in its sequence) to max_pos - 1, as the kernel does.  x = word + typ + pos in float64,
+    then ``layernorm_ref``.  Returns (y, xhat, sigma, M) with M [T, 1] = max_d (|word_d| + |typ_d| + |pos_d|), the
+    magnitude the kernel's fp32 three-term sum rounds against."""
+    w = _f64(word)
+    dev = w.device
+    cu = _long(cu, dev)
+    T = int(cu[-1])
+    lens = cu[1:] - cu[:-1]
+    p = torch.arange(T, device=dev) - torch.repeat_interleave(cu[:-1], lens)
+    p = p.clamp(max=int(pos.shape[0]) - 1)
+    i = _long(ids, dev).clamp(0, int(word.shape[0]) - 1)
+    ty = torch.zeros(T, dtype=torch.int64, device=dev) if type_ids is None else \
+        _long(type_ids, dev).clamp(0, int(typ.shape[0]) - 1)
+    a, c, e = w[i], _f64(typ).to(dev)[ty], _f64(pos).to(dev)[p]
+    y, xhat, sigma = layernorm_ref(a + c + e, gamma, beta, eps)
+    return y, xhat, sigma, (a.abs() + c.abs() + e.abs()).amax(1, keepdim=True)
+
+
+def pool_ref(hi, lo, cu, mode: int, normalize: bool):
+    """E4 ``pool_kernel`` on planes [T, H] of the ragged batch `cu`: mode 0 = mean (sum / max(S, 1e-9), so an empty
+    sequence gives 0), mode 1 = CLS (row cu[b], 0 for an empty sequence); then x / max(||x||, 1e-12) when normalize.
+    Only rows the kernel reads are read.  Returns (out [B, H], m [B, H] before normalisation, P [B, H]) with
+    P = sum over the sequence of |x_td| (mean) or 0 (CLS, an exact copy): the magnitude the fp32 sum rounds against."""
+    x = _f64(hi) + _f64(lo)
+    cu = [int(c) for c in cu]
+    B, H = len(cu) - 1, x.shape[1]
+    m = torch.zeros((B, H), dtype=torch.float64, device=x.device)
+    P = torch.zeros_like(m)
+    for b in range(B):
+        t0, t1 = cu[b], cu[b + 1]
+        if t1 == t0:
+            continue
+        if mode == 1:
+            m[b] = x[t0]
+        else:
+            m[b] = x[t0:t1].sum(0) / (t1 - t0)
+            P[b] = x[t0:t1].abs().sum(0)
+    out = m / m.norm(dim=1, keepdim=True).clamp(min=1e-12) if normalize else m
+    return out, m, P
+
+
+def cls_head_ref(hi, lo, cu, pw, pb, cw, cb):
+    """E4 ``cls_head_kernel`` on planes [T, H] of the ragged batch `cu`: h = row cu[b] (0 for an empty sequence),
+    z = pw h + pb, pooled = tanh(z), logits = cw pooled + cb, in float64.  Returns (logits [B, L], z [B, H], pooled,
+    A [B, H], C [B, L]) with A_bj = sum_d |pw_jd h_d| and C_bc = sum_j |cw_cj pooled_j|, the magnitudes the two dot
+    products round against."""
+    x = _f64(hi) + _f64(lo)
+    cu = [int(c) for c in cu]
+    B, H = len(cu) - 1, x.shape[1]
+    h = torch.zeros((B, H), dtype=torch.float64, device=x.device)
+    for b in range(B):
+        if cu[b + 1] > cu[b]:
+            h[b] = x[cu[b]]
+    W, Wc = _f64(pw).to(x.device), _f64(cw).to(x.device)
+    z = h @ W.T + _f64(pb).to(x.device)[None, :]
+    pooled = torch.tanh(z)
+    logits = pooled @ Wc.T + _f64(cb).to(x.device)[None, :]
+    return logits, z, pooled, h.abs() @ W.abs().T, pooled.abs() @ Wc.abs().T

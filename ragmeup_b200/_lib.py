@@ -92,6 +92,15 @@ SIGNATURES = {
                                       C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_layernorm": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
                                       C.c_void_p, C.c_void_p]),
+    "rmu_debug_embed_ln": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                     C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float,
+                                     C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_pool": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                 C.c_void_p]),
+    "rmu_debug_cls_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_split_planes": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_join_planes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "rmu_debug_bm25_select": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                         C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
 }

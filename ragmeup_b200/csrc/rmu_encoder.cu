@@ -13,6 +13,7 @@
 // Activations between kernels are split fp16 planes (see rmu_gemm.cuh); LayerNorm, softmax, GELU,
 // residual adds, pooling and the classifier head are fp32.
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <mutex>
 #include <vector>
@@ -406,7 +407,8 @@ __global__ void __launch_bounds__(256) pool_kernel(const __half* __restrict__ hi
     for (int d = threadIdx.x; d < H; d += blockDim.x, ++nv) out[static_cast<size_t>(b) * H + d] = vals[nv] * inv;
 }
 
-// BertPooler (tanh(W_p h_cls + b_p)) + classifier -> logits [B, num_labels]
+// BertPooler (tanh(W_p h_cls + b_p)) + classifier -> logits [B, num_labels].  An empty sequence has h_cls = 0 (its row
+// cu[b] belongs to the next sequence, or lies past T).
 __global__ void __launch_bounds__(256) cls_head_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo,
                                                        const int* __restrict__ cu, int H, int num_labels,
                                                        const float* __restrict__ pw, const float* __restrict__ pb,
@@ -416,8 +418,9 @@ __global__ void __launch_bounds__(256) cls_head_kernel(const __half* __restrict_
     float* hcls = sh;
     float* pooled = sh + H;
     const int b = blockIdx.x;
-    const size_t o = static_cast<size_t>(cu[b]) * H;
-    for (int d = threadIdx.x; d < H; d += blockDim.x) hcls[d] = __half2float(hi[o + d]) + __half2float(lo[o + d]);
+    const int t0 = cu[b], S = cu[b + 1] - t0;
+    const size_t o = static_cast<size_t>(t0) * H;
+    for (int d = threadIdx.x; d < H; d += blockDim.x) hcls[d] = S > 0 ? __half2float(hi[o + d]) + __half2float(lo[o + d]) : 0.f;
     __syncthreads();
     const int warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
     for (int j = warp; j < H; j += nw) {
@@ -469,6 +472,58 @@ static int launch_layernorm(const float* pre, int T, int H, const float* g, cons
     constexpr int wpb = 8;
     ProfScope _ps(PROF_LN, st);
     ln_kernel<<<static_cast<unsigned>((T + wpb - 1) / wpb), wpb * 32, 0, st>>>(pre, T, H, g, b, eps, hi, lo);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// E3 embed_ln_kernel: word + token-type + position rows of T tokens of a ragged batch -> LayerNorm -> planes [T, H].
+// 8 warps (tokens) per block.
+static int launch_embed_ln(const int* ids, const int* type_ids, const int* cu, int B, int T, int H, int vocab, int max_pos,
+                           int type_vocab, const float* word, const float* pos, const float* typ, const float* g,
+                           const float* b, float eps, __half* hi, __half* lo, cudaStream_t st) {
+    constexpr int wpb = 8;
+    ProfScope _ps(PROF_EMBED, st);
+    embed_ln_kernel<<<static_cast<unsigned>((T + wpb - 1) / wpb), wpb * 32, 0, st>>>(ids, type_ids, cu, B, T, H, vocab, max_pos,
+                                                                                     type_vocab, word, pos, typ, g, b, eps, hi, lo);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// E4 pool_kernel: one 256-thread block per sequence -> out [B, H] (H <= 1024: four columns per thread)
+static int launch_pool(const __half* hi, const __half* lo, const int* cu, int B, int H, int mode, int normalize, float* out,
+                       cudaStream_t st) {
+    ProfScope _ps(PROF_POOL_HEAD, st);
+    pool_kernel<<<B, 256, 0, st>>>(hi, lo, cu, H, mode, normalize, out);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// E4 cls_head_kernel: one 256-thread block per sequence, h_cls and the pooled vector in shared memory -> out [B, num_labels]
+static int launch_cls_head(const __half* hi, const __half* lo, const int* cu, int B, int H, int num_labels, const float* pw,
+                           const float* pb, const float* cw, const float* cb, float* out, cudaStream_t st) {
+    ProfScope _ps(PROF_POOL_HEAD, st);
+    cls_head_kernel<<<B, 256, 2 * H * sizeof(float), st>>>(hi, lo, cu, H, num_labels, pw, pb, cw, cb, out);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// n fp32 values -> (hi, lo) planes; n = 0 launches nothing
+static int launch_split_planes(const float* src, size_t n, __half* hi, __half* lo, cudaStream_t st) {
+    if (n == 0) return RMU_OK;
+    split_planes_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(src, hi, lo, n);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// hi + lo -> n fp32 values; n = 0 launches nothing
+static int launch_join_planes(const __half* hi, const __half* lo, size_t n, float* out, cudaStream_t st) {
+    if (n == 0) return RMU_OK;
+    join_planes_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(hi, lo, out, n);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
@@ -534,10 +589,10 @@ static int upload_split(rmu_encoder* e, SplitOperand* op, const std::vector<cons
     int rc = dev_alloc(e->allocs, &hi, n);
     if (rc == RMU_OK) rc = dev_alloc(e->allocs, &lo, n);
     if (rc != RMU_OK) { cudaFree(tmp); return rc; }
-    split_planes_kernel<<<static_cast<unsigned>((n + 255) / 256), 256>>>(tmp, hi, lo, n);
-    count_launch();
+    rc = launch_split_planes(tmp, n, hi, lo, nullptr);
     cudaError_t err = cudaDeviceSynchronize();
     cudaFree(tmp);
+    if (rc != RMU_OK) return rc;
     if (err != cudaSuccess) { set_error(std::string("split_planes: ") + cudaGetErrorString(err)); return RMU_ERR_CUDA; }
     return make_split_operand(op, hi, lo, static_cast<int64_t>(rows), cols);
 }
@@ -586,13 +641,9 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
     int rc = ensure_tokens(e, T, B);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace is shared by all callers
-    const int wpb = 8;
-    const unsigned tok_blocks = static_cast<unsigned>((T + wpb - 1) / wpb);
-    { ProfScope _ps(PROF_EMBED, st);
-    embed_ln_kernel<<<tok_blocks, wpb * 32, 0, st>>>(ids, type_ids, cu, B, T, H, c.vocab_size, c.max_pos, c.type_vocab,
-                                                     e->word, e->pos, e->typ, e->eg, e->eb, c.ln_eps, e->X.hi, e->X.lo); }
-    count_launch();
-    RMU_CHECK_LAUNCH();
+    rc = launch_embed_ln(ids, type_ids, cu, B, T, H, c.vocab_size, c.max_pos, c.type_vocab, e->word, e->pos, e->typ, e->eg,
+                         e->eb, c.ln_eps, e->X.hi, e->X.lo, st);
+    if (rc != RMU_OK) return rc;
     const float scale = 1.0f / sqrtf(static_cast<float>(DH));
     for (int l = 0; l < c.layers; ++l) {
         EncLayer& L = e->layers[l];
@@ -644,6 +695,23 @@ int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* w, int n_
         (H / cfg->heads != 32 && H / cfg->heads != 64)) {
         set_error("rmu_encoder_create: unsupported shape (hidden/ffn multiples of 128, hidden <= 1024, head_dim 32 or 64)");
         return RMU_ERR_UNSUPPORTED;
+    }
+    // the GEMM weights travel as fp16 planes: |w| >= 65520 rounds hi to inf and turns every output it touches into NaN
+    for (int l = 0; l < L; ++l) {
+        static const char* const kName[] = {"query", "key", "value", "attention output", "intermediate", "output"};
+        const int slot[] = {0, 2, 4, 6, 10, 12};                  // weight offsets within the layer's 16 tensors
+        const size_t count[] = {size_t(H) * H, size_t(H) * H, size_t(H) * H, size_t(H) * H, size_t(F) * H, size_t(H) * F};
+        for (int k = 0; k < 6; ++k) {
+            const float* p = w[5 + 16 * l + slot[k]];
+            if (!p) { set_error("rmu_encoder_create: null weight tensor"); return RMU_ERR_ARG; }
+            for (size_t j = 0; j < count[k]; ++j) {
+                if (std::fabs(p[j]) >= 65520.0f) {
+                    set_error("rmu_encoder_create: layer " + std::to_string(l) + " " + kName[k] + " weight [" + std::to_string(j) +
+                              "] = " + std::to_string(p[j]) + " is outside the split fp16 planes' range (|w| < 65520)");
+                    return RMU_ERR_UNSUPPORTED;
+                }
+            }
+        }
     }
     rmu_encoder* e = new rmu_encoder();
     e->cfg = *cfg;
@@ -719,10 +787,8 @@ int rmu_encoder_embed(rmu_encoder* e, const int32_t* ids, const int32_t* type_id
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, st);
     if (rc != RMU_OK) return rc;
-    ProfScope _ps(PROF_POOL_HEAD, st);
-    pool_kernel<<<B, 256, 0, st>>>(e->X.hi, e->X.lo, cu, e->cfg.hidden, pool_mode, normalize, out);
-    count_launch();
-    RMU_CHECK_LAUNCH();
+    rc = launch_pool(e->X.hi, e->X.lo, cu, B, e->cfg.hidden, pool_mode, normalize, out, st);
+    if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
 }
@@ -736,12 +802,8 @@ int rmu_encoder_classify(rmu_encoder* e, const int32_t* ids, const int32_t* type
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, st);
     if (rc != RMU_OK) return rc;
-    const int H = e->cfg.hidden;
-    ProfScope _ps(PROF_POOL_HEAD, st);
-    cls_head_kernel<<<B, 256, 2 * H * sizeof(float), st>>>(e->X.hi, e->X.lo, cu, H, e->cfg.num_labels, e->pw, e->pb,
-                                                            e->cw, e->cb, out);
-    count_launch();
-    RMU_CHECK_LAUNCH();
+    rc = launch_cls_head(e->X.hi, e->X.lo, cu, B, e->cfg.hidden, e->cfg.num_labels, e->pw, e->pb, e->cw, e->cb, out, st);
+    if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
 }
@@ -754,10 +816,8 @@ int rmu_encoder_hidden(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, st);
     if (rc != RMU_OK) return rc;
-    const size_t n = static_cast<size_t>(T) * e->cfg.hidden;
-    join_planes_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(e->X.hi, e->X.lo, out, n);
-    count_launch();
-    RMU_CHECK_LAUNCH();
+    rc = launch_join_planes(e->X.hi, e->X.lo, static_cast<size_t>(T) * e->cfg.hidden, out, st);
+    if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
 }
@@ -842,6 +902,68 @@ int rmu_debug_layernorm(const float* pre, int T, int H, const float* gamma, cons
     }
     return launch_layernorm(pre, T, H, gamma, beta, eps, reinterpret_cast<__half*>(out_hi), reinterpret_cast<__half*>(out_lo),
                             static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_embed_ln(const int32_t* ids, const int32_t* type_ids, const int32_t* cu, int B, int T, int H, int vocab,
+                       int max_pos, int type_vocab, const float* word, const float* pos, const float* typ,
+                       const float* gamma, const float* beta, float eps, uint16_t* out_hi, uint16_t* out_lo, void* stream) {
+    if (!ids || !cu || !word || !pos || !typ || !gamma || !beta || !out_hi || !out_lo || B <= 0 || T <= 0 || H <= 0 ||
+        vocab <= 0 || max_pos <= 0 || type_vocab <= 0) {
+        set_error("rmu_debug_embed_ln: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H % 128 != 0 || H > 32 * kMaxPerLane) {
+        set_error("rmu_debug_embed_ln: hidden must be a multiple of 128, at most 1024");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_embed_ln(ids, type_ids, cu, B, T, H, vocab, max_pos, type_vocab, word, pos, typ, gamma, beta, eps,
+                           reinterpret_cast<__half*>(out_hi), reinterpret_cast<__half*>(out_lo), static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_pool(const uint16_t* hi, const uint16_t* lo, const int32_t* cu, int B, int H, int pool_mode, int normalize,
+                   float* out, void* stream) {
+    if (!hi || !lo || !cu || !out || B <= 0 || H <= 0 || (pool_mode != RMU_POOL_MEAN && pool_mode != RMU_POOL_CLS)) {
+        set_error("rmu_debug_pool: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H > 1024) {
+        set_error("rmu_debug_pool: hidden must be at most 1024");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_pool(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), cu, B, H, pool_mode, normalize,
+                       out, static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const int32_t* cu, int B, int H, int num_labels,
+                       const float* pw, const float* pb, const float* cw, const float* cb, float* out, void* stream) {
+    if (!hi || !lo || !cu || !pw || !pb || !cw || !cb || !out || B <= 0 || H <= 0 || num_labels <= 0) {
+        set_error("rmu_debug_cls_head: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H > 1024) {
+        set_error("rmu_debug_cls_head: hidden must be at most 1024");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_cls_head(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), cu, B, H, num_labels, pw,
+                           pb, cw, cb, out, static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_split_planes(const float* src, int64_t n, uint16_t* hi, uint16_t* lo, void* stream) {
+    if (!src || !hi || !lo || n < 0) {
+        set_error("rmu_debug_split_planes: bad argument");
+        return RMU_ERR_ARG;
+    }
+    return launch_split_planes(src, static_cast<size_t>(n), reinterpret_cast<__half*>(hi), reinterpret_cast<__half*>(lo),
+                               static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_join_planes(const uint16_t* hi, const uint16_t* lo, int64_t n, float* out, void* stream) {
+    if (!hi || !lo || !out || n < 0) {
+        set_error("rmu_debug_join_planes: bad argument");
+        return RMU_ERR_ARG;
+    }
+    return launch_join_planes(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), static_cast<size_t>(n),
+                              out, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -4,6 +4,7 @@ import ctypes
 import os
 import re
 
+import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -87,6 +88,44 @@ def test_kernel_test_entry_points_reject_before_any_cuda_call(built_lib):
     assert ln(H=320) == -3 and ln(H=1152) == -3 and ln(H=96) == -3
     assert ln(T=0) == -1
 
+    def emb(B=2, T=9, H=384, vocab=30522, max_pos=512, type_vocab=2, **kw):
+        a = dict(ids=p, typ=p, cu=p, word=p, pos=p, ttab=p, g=p, b=p, oh=p, ol=p)
+        a.update(kw)
+        return l.rmu_debug_embed_ln(a["ids"], a["typ"], a["cu"], B, T, H, vocab, max_pos, type_vocab, a["word"], a["pos"],
+                                    a["ttab"], a["g"], a["b"], 1e-12, a["oh"], a["ol"], None)
+
+    assert emb(H=320) == -3 and emb(H=1152) == -3 and emb(H=96) == -3 and b"rmu_debug_embed_ln" in l.rmu_last_error()
+    for name in ("ids", "cu", "word", "pos", "ttab", "g", "b", "oh", "ol"):
+        assert emb(**{name: None}) == -1, name
+    for name in ("B", "T", "vocab", "max_pos", "type_vocab"):
+        assert emb(**{name: 0}) == -1 and emb(**{name: -1}) == -1, name
+    assert emb(H=0) == -1
+
+    def pool(B=2, H=384, mode=0, hi=p, lo=p, cu=p, out=p):
+        return l.rmu_debug_pool(hi, lo, cu, B, H, mode, 1, out, None)
+
+    assert pool(H=1025) == -3 and pool(H=2048) == -3 and b"rmu_debug_pool" in l.rmu_last_error()
+    assert pool(mode=2) == -1 and pool(mode=-1) == -1 and pool(B=0) == -1 and pool(H=0) == -1
+    assert pool(hi=None) == -1 and pool(lo=None) == -1 and pool(cu=None) == -1 and pool(out=None) == -1
+
+    def head(B=2, H=384, L=1, **kw):
+        a = dict(hi=p, lo=p, cu=p, pw=p, pb=p, cw=p, cb=p, out=p)
+        a.update(kw)
+        return l.rmu_debug_cls_head(a["hi"], a["lo"], a["cu"], B, H, L, a["pw"], a["pb"], a["cw"], a["cb"], a["out"], None)
+
+    assert head(H=1025) == -3 and b"rmu_debug_cls_head" in l.rmu_last_error()
+    assert head(B=0) == -1 and head(H=0) == -1 and head(L=0) == -1 and head(L=-2) == -1
+    for name in ("hi", "lo", "cu", "pw", "pb", "cw", "cb", "out"):
+        assert head(**{name: None}) == -1, name
+
+    assert l.rmu_debug_split_planes(p, -1, p, p, None) == -1 and l.rmu_debug_join_planes(p, p, -1, p, None) == -1
+    assert l.rmu_debug_split_planes(None, 8, p, p, None) == -1 and l.rmu_debug_split_planes(p, 8, None, p, None) == -1
+    assert l.rmu_debug_split_planes(p, 8, p, None, None) == -1 and l.rmu_debug_join_planes(None, p, 8, p, None) == -1
+    assert l.rmu_debug_join_planes(p, None, 8, p, None) == -1 and l.rmu_debug_join_planes(p, p, 8, None, None) == -1
+    n0 = _lib.launch_count()                                # n = 0: nothing to launch, so no device is needed
+    assert l.rmu_debug_split_planes(p, 0, p, p, None) == 0 and l.rmu_debug_join_planes(p, p, 0, p, None) == 0
+    assert _lib.launch_count() == n0
+
     # the scan tile needs an index handle, which needs a device: what is checked here is refused before the handle is
     # read (the dim / nq / empty-index refusals are in tests/test_index_kernels_gpu.py)
     def tile(h=None, q=p, nq=16, out=p):
@@ -113,6 +152,43 @@ def test_kernel_test_entry_points_reject_before_any_cuda_call(built_lib):
     assert bsel(ws_elems=2 * 3 * 2 * 10 - 1) == -1                      # one element short
     assert bsel(m=4096, ws_elems=2 * 3 * 10 - 1) == -1 and bsel(m=4097, ws_elems=2 * 3 * 2 * 10 - 1) == -1
     assert bsel(Q=65535, m=1, k=256, ws_elems=2 * 65535 * 256 - 1) == -1
+
+
+def test_encoder_create_refuses_weights_the_split_planes_cannot_hold(built_lib):
+    """GEMM weights travel as fp16 planes, and fp16 rounds |w| >= 65520 to inf: rmu_encoder_create refuses such a
+    weight on the host, before any CUDA call.  Tables, biases, LayerNorm parameters and the head stay fp32."""
+    from ragmeup_b200 import _lib
+    from ragmeup_b200.weights import PRESETS, synthetic_bert_weights, weight_names
+    l = _lib.lib()
+    cfg = PRESETS["tiny"][0]
+    names = [n for n, _ in weight_names(cfg, True)]
+    base = synthetic_bert_weights(cfg, seed=0, with_head=True)
+
+    def create(name, idx, value):
+        w = {k: v.copy() for k, v in base.items()}
+        w[name].reshape(-1)[idx] = value
+        arrs = [np.ascontiguousarray(w[n]) for n in names]
+        ptrs = (ctypes.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
+        cc = _lib.BertConfigC(cfg.vocab_size, cfg.hidden, cfg.layers, cfg.heads, cfg.ffn, cfg.max_pos, cfg.type_vocab,
+                              cfg.num_labels, cfg.ln_eps)
+        h = ctypes.c_void_p()
+        rc = l.rmu_encoder_create(ctypes.byref(cc), ptrs, len(arrs), 1, ctypes.byref(h))
+        if rc == 0:
+            l.rmu_encoder_destroy(h)
+        return rc
+
+    for name in ("encoder.layer.1.intermediate.dense.weight", "encoder.layer.0.attention.self.query.weight",
+                 "encoder.layer.0.attention.self.value.weight", "encoder.layer.1.attention.output.dense.weight",
+                 "encoder.layer.0.output.dense.weight", "encoder.layer.1.attention.self.key.weight"):
+        for v in (7e4, -7e4, 65520.0, np.inf, -np.inf):
+            assert create(name, 37, v) == -3, (name, v)
+        assert b"65520" in l.rmu_last_error()
+        # 65 519 (and 65 519.996, which rounds hi to 65 504) pass the check: without a device the next step fails
+        for v in (65519.0, float(np.nextafter(np.float32(65520), np.float32(0))), -65519.0):
+            assert create(name, 37, v) in (0, -2), (name, v)
+    for name in ("embeddings.word_embeddings.weight", "encoder.layer.0.attention.self.query.bias",
+                 "encoder.layer.0.output.LayerNorm.weight", "pooler.dense.weight", "classifier.weight"):
+        assert create(name, 0, 7e4) in (0, -2), name
 
 
 def test_product_fails_loudly_without_cuda(built_lib):
