@@ -179,8 +179,15 @@ __device__ __forceinline__ float fast_exp2(float x) {   // ex2.approx: 2 ulp, ex
 // to 3 CTAs / 64 registers spills in the key loop and measured 541 us instead of 352 us per layer call).
 // Grid = (heads, sequences, row blocks): the heads of one sequence run together, so the 64-byte (d_h = 32)
 // K / V row segments of neighbouring heads are fetched from DRAM as whole lines.
-template <int DH, int MINB, int NW = kAttWarps>      // NW warps = 16 * NW query rows per CTA
+//
+// CLS = true: query row 0 of each sequence only, for the last layer when only the CLS rows leave the encoder.  Q comes
+// from row b of the compact planes cls_q [B, H], the context goes to row b of ctx [B, H] (zeros for an empty sequence),
+// grid z = 1.  Warp 0 runs the same code as warp 0 of the full kernel with query rows 1..15 zero; the MMA rows and the
+// softmax rows are independent, so row 0 comes out bit-identical.  The other NW - 1 warps only help stage K / V.
+template <int DH, int MINB, int NW = kAttWarps, bool CLS = false>      // NW warps = 16 * NW query rows per CTA
 __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const __half* __restrict__ ph, const __half* __restrict__ pl,
+                                                                          const __half* __restrict__ cls_q_hi,
+                                                                          const __half* __restrict__ cls_q_lo,
                                                                           const int* __restrict__ cu, int H, int ksb,
                                                                           __half* __restrict__ ctx_hi, __half* __restrict__ ctx_lo) {
     constexpr int KSTR = DH + 8;
@@ -194,14 +201,26 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
 
     const int b = blockIdx.y, h = blockIdx.x;
     const int t0 = cu[b], S = cu[b + 1] - t0;
+    if (CLS && S <= 0) {
+        for (int c = threadIdx.x; c < DH; c += blockDim.x) {
+            ctx_hi[static_cast<size_t>(b) * H + h * DH + c] = __ushort_as_half(0);
+            ctx_lo[static_cast<size_t>(b) * H + h * DH + c] = __ushort_as_half(0);
+        }
+        return;
+    }
     const int rbase = blockIdx.z * (NW * 16);
     if (rbase >= S) return;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
     const size_t ld = static_cast<size_t>(3) * H;
-    const __half* qh_base = ph + static_cast<size_t>(t0) * ld + h * DH;
-    const __half* ql_base = pl + static_cast<size_t>(t0) * ld + h * DH;
+    // query rows: the sequence's rows of the QKV planes, or (CLS) its one row of the compact Q planes; the context rows
+    // start at the same row index, of the [T, H] or the [B, H] output
+    const size_t qld = CLS ? static_cast<size_t>(H) : ld;
+    const int qrows = CLS ? 1 : S;
+    const int orow = CLS ? b : t0;
+    const __half* qh_base = CLS ? cls_q_hi + static_cast<size_t>(b) * H + h * DH : ph + static_cast<size_t>(t0) * ld + h * DH;
+    const __half* ql_base = CLS ? cls_q_lo + static_cast<size_t>(b) * H + h * DH : pl + static_cast<size_t>(t0) * ld + h * DH;
     const int r0 = rbase + warp * 16;
-    const bool warp_live = r0 < S;
+    const bool warp_live = r0 < qrows;
 
     uint32_t qh[KS][4], ql[KS][4];
     {
@@ -210,17 +229,17 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
         for (int ks = 0; ks < KS; ++ks) {
 #pragma unroll
             for (int i = 0; i < 4; ++i) { qh[ks][i] = 0u; ql[ks][i] = 0u; }
-            if (warp_live && ra < S) {
-                qh[ks][0] = *reinterpret_cast<const uint32_t*>(qh_base + ra * ld + ks * 16 + 2 * t);
-                ql[ks][0] = *reinterpret_cast<const uint32_t*>(ql_base + ra * ld + ks * 16 + 2 * t);
-                qh[ks][2] = *reinterpret_cast<const uint32_t*>(qh_base + ra * ld + ks * 16 + 2 * t + 8);
-                ql[ks][2] = *reinterpret_cast<const uint32_t*>(ql_base + ra * ld + ks * 16 + 2 * t + 8);
+            if (warp_live && ra < qrows) {
+                qh[ks][0] = *reinterpret_cast<const uint32_t*>(qh_base + ra * qld + ks * 16 + 2 * t);
+                ql[ks][0] = *reinterpret_cast<const uint32_t*>(ql_base + ra * qld + ks * 16 + 2 * t);
+                qh[ks][2] = *reinterpret_cast<const uint32_t*>(qh_base + ra * qld + ks * 16 + 2 * t + 8);
+                ql[ks][2] = *reinterpret_cast<const uint32_t*>(ql_base + ra * qld + ks * 16 + 2 * t + 8);
             }
-            if (warp_live && rb < S) {
-                qh[ks][1] = *reinterpret_cast<const uint32_t*>(qh_base + rb * ld + ks * 16 + 2 * t);
-                ql[ks][1] = *reinterpret_cast<const uint32_t*>(ql_base + rb * ld + ks * 16 + 2 * t);
-                qh[ks][3] = *reinterpret_cast<const uint32_t*>(qh_base + rb * ld + ks * 16 + 2 * t + 8);
-                ql[ks][3] = *reinterpret_cast<const uint32_t*>(ql_base + rb * ld + ks * 16 + 2 * t + 8);
+            if (warp_live && rb < qrows) {
+                qh[ks][1] = *reinterpret_cast<const uint32_t*>(qh_base + rb * qld + ks * 16 + 2 * t);
+                ql[ks][1] = *reinterpret_cast<const uint32_t*>(ql_base + rb * qld + ks * 16 + 2 * t);
+                qh[ks][3] = *reinterpret_cast<const uint32_t*>(qh_base + rb * qld + ks * 16 + 2 * t + 8);
+                ql[ks][3] = *reinterpret_cast<const uint32_t*>(ql_base + rb * qld + ks * 16 + 2 * t + 8);
             }
         }
     }
@@ -360,33 +379,35 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
     for (int n = 0; n < NT; ++n) {
         const int col = h * DH + n * 8 + 2 * t;
         uint32_t hi, lo;
-        if (ra < S) {
+        if (ra < qrows) {
             split_pack(oacc[n][0] * i0, oacc[n][1] * i0, hi, lo);
-            *reinterpret_cast<uint32_t*>(ctx_hi + static_cast<size_t>(t0 + ra) * H + col) = hi;
-            *reinterpret_cast<uint32_t*>(ctx_lo + static_cast<size_t>(t0 + ra) * H + col) = lo;
+            *reinterpret_cast<uint32_t*>(ctx_hi + static_cast<size_t>(orow + ra) * H + col) = hi;
+            *reinterpret_cast<uint32_t*>(ctx_lo + static_cast<size_t>(orow + ra) * H + col) = lo;
         }
-        if (rb < S) {
+        if (rb < qrows) {
             split_pack(oacc[n][2] * i1, oacc[n][3] * i1, hi, lo);
-            *reinterpret_cast<uint32_t*>(ctx_hi + static_cast<size_t>(t0 + rb) * H + col) = hi;
-            *reinterpret_cast<uint32_t*>(ctx_lo + static_cast<size_t>(t0 + rb) * H + col) = lo;
+            *reinterpret_cast<uint32_t*>(ctx_hi + static_cast<size_t>(orow + rb) * H + col) = hi;
+            *reinterpret_cast<uint32_t*>(ctx_lo + static_cast<size_t>(orow + rb) * H + col) = lo;
         }
     }
 }
 
-// sentence-transformers Pooling (mean | cls) + optional Normalize -> out [B, H]
+// sentence-transformers Pooling (mean | cls) + optional Normalize -> out [B, H].  compact (CLS only): the planes hold the
+// CLS rows alone, [B, H], and sequence b's is row b instead of row cu[b].
 __global__ void __launch_bounds__(256) pool_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo,
-                                                   const int* __restrict__ cu, int H, int mode, int normalize,
+                                                   const int* __restrict__ cu, int H, int mode, int normalize, int compact,
                                                    float* __restrict__ out) {
     __shared__ float red[32];
     const int b = blockIdx.x;
     const int t0 = cu[b], S = cu[b + 1] - t0;
+    const size_t cls_row = compact ? b : t0;
     float ss = 0.f;
     float vals[4];   // H <= 1024 with 256 threads
     int nv = 0;
     for (int d = threadIdx.x; d < H; d += blockDim.x, ++nv) {
         float v = 0.f;
         if (mode == RMU_POOL_CLS) {
-            if (S > 0) v = __half2float(hi[static_cast<size_t>(t0) * H + d]) + __half2float(lo[static_cast<size_t>(t0) * H + d]);
+            if (S > 0) v = __half2float(hi[cls_row * H + d]) + __half2float(lo[cls_row * H + d]);
         } else {
             for (int t = 0; t < S; ++t) {
                 const size_t o = static_cast<size_t>(t0 + t) * H + d;
@@ -408,9 +429,9 @@ __global__ void __launch_bounds__(256) pool_kernel(const __half* __restrict__ hi
 }
 
 // BertPooler (tanh(W_p h_cls + b_p)) + classifier -> logits [B, num_labels].  An empty sequence has h_cls = 0 (its row
-// cu[b] belongs to the next sequence, or lies past T).
+// cu[b] belongs to the next sequence, or lies past T).  compact: h_cls of sequence b is row b of [B, H] planes.
 __global__ void __launch_bounds__(256) cls_head_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo,
-                                                       const int* __restrict__ cu, int H, int num_labels,
+                                                       const int* __restrict__ cu, int H, int num_labels, int compact,
                                                        const float* __restrict__ pw, const float* __restrict__ pb,
                                                        const float* __restrict__ cw, const float* __restrict__ cb,
                                                        float* __restrict__ out) {
@@ -419,7 +440,7 @@ __global__ void __launch_bounds__(256) cls_head_kernel(const __half* __restrict_
     float* pooled = sh + H;
     const int b = blockIdx.x;
     const int t0 = cu[b], S = cu[b + 1] - t0;
-    const size_t o = static_cast<size_t>(t0) * H;
+    const size_t o = static_cast<size_t>(compact ? b : t0) * H;
     for (int d = threadIdx.x; d < H; d += blockDim.x) hcls[d] = S > 0 ? __half2float(hi[o + d]) + __half2float(lo[o + d]) : 0.f;
     __syncthreads();
     const int warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -440,27 +461,57 @@ __global__ void __launch_bounds__(256) cls_head_kernel(const __half* __restrict_
     }
 }
 
+// row cu[b] of [T, H] planes -> row b of [B, H] planes, bit for bit (zeros for an empty sequence).  H % 8 == 0.
+__global__ void gather_cls_rows_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, const int* __restrict__ cu,
+                                       int H, __half* __restrict__ out_hi, __half* __restrict__ out_lo) {
+    const int b = blockIdx.x;
+    const int t0 = cu[b];
+    const bool empty = cu[b + 1] == t0;
+    const uint4* sh = reinterpret_cast<const uint4*>(hi + static_cast<size_t>(t0) * H);
+    const uint4* sl = reinterpret_cast<const uint4*>(lo + static_cast<size_t>(t0) * H);
+    uint4* dh = reinterpret_cast<uint4*>(out_hi + static_cast<size_t>(b) * H);
+    uint4* dl = reinterpret_cast<uint4*>(out_lo + static_cast<size_t>(b) * H);
+    for (int i = threadIdx.x; i < H / 8; i += blockDim.x) {
+        uint4 vh = make_uint4(0, 0, 0, 0), vl = vh;
+        if (!empty) { vh = sh[i]; vl = sl[i]; }
+        dh[i] = vh;
+        dl[i] = vl;
+    }
+}
+
 __global__ void join_planes_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, float* __restrict__ out, size_t n) {
     size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i < n) out[i] = __half2float(hi[i]) + __half2float(lo[i]);
 }
 
+// CLS-only attention: one CTA per (sequence, head) holds the whole K / V staging buffer (51 KB at d_h = 32 and 147
+// tokens, so four CTAs per SM).  The kernel is bound by that latency-bound copy, not by the one query row: with one warp
+// per CTA only four warps per SM would issue it, so four warps stage and warp 0 computes.
+constexpr int kClsAttWarps = 4;
+
 // E2 on the QKV planes [T, 3H] (q pre-scaled by log2(e) / sqrt(d_h)) of a ragged batch -> ctx planes [T, H].
 // warps = 10 (160-row CTAs), or 5 (80-row CTAs, four per SM) with d_h = 32.
-static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const int* cu, int B, int H, int heads,
-                            int max_seqlen, int warps, __half* ctx_hi, __half* ctx_lo, cudaStream_t st) {
+// cls_q_hi / cls_q_lo non-null: query row 0 of each sequence only, q from those compact planes [B, H] -> ctx [B, H]
+// (the K / V columns of the QKV planes are read as above; their Q columns are not); `warps` is ignored.
+static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __half* cls_q_hi, const __half* cls_q_lo,
+                            const int* cu, int B, int H, int heads, int max_seqlen, int warps, __half* ctx_hi,
+                            __half* ctx_lo, cudaStream_t st) {
     const int DH = H / heads;
-    if (!(warps == kAttWarps || (warps == 5 && DH == 32))) { set_error("attention: warps must be 10, or 5 with head_dim 32"); return RMU_ERR_ARG; }
+    const bool cls = cls_q_hi != nullptr;
+    if (cls) warps = kClsAttWarps;
+    else if (!(warps == kAttWarps || (warps == 5 && DH == 32))) { set_error("attention: warps must be 10, or 5 with head_dim 32"); return RMU_ERR_ARG; }
     ProfScope _ps(PROF_ATTN, st);
-    dim3 pg(static_cast<unsigned>(heads), static_cast<unsigned>(B), static_cast<unsigned>((max_seqlen + warps * 16 - 1) / (warps * 16)));
+    const unsigned zblocks = cls ? 1u : static_cast<unsigned>((max_seqlen + warps * 16 - 1) / (warps * 16));
+    dim3 pg(static_cast<unsigned>(heads), static_cast<unsigned>(B), zblocks);
     // keys resident per CTA: the whole (longest) sequence when it fits, else super-blocks of kKeySB
     const int ksb = std::min(kKeySB, (max_seqlen + 31) / 32 * 32);
     const size_t smem_max = 4 * sizeof(__half) * static_cast<size_t>(kKeySB) * (DH + 8);
     const size_t smem = 4 * sizeof(__half) * static_cast<size_t>(ksb) * (DH + 8);
-    auto kern = DH == 32 ? (warps == 5 ? attention_planes_kernel<32, 4, 5> : attention_planes_kernel<32, 2>)
+    auto kern = cls ? (DH == 32 ? attention_planes_kernel<32, 4, kClsAttWarps, true> : attention_planes_kernel<64, 2, kClsAttWarps, true>)
+              : DH == 32 ? (warps == 5 ? attention_planes_kernel<32, 4, 5> : attention_planes_kernel<32, 2>)
                          : attention_planes_kernel<64, 1>;   // d_h = 64 needs > 96 registers
     RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
-    kern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, cu, H, ksb, ctx_hi, ctx_lo);
+    kern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, cls_q_hi, cls_q_lo, cu, H, ksb, ctx_hi, ctx_lo);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
@@ -492,20 +543,30 @@ static int launch_embed_ln(const int* ids, const int* type_ids, const int* cu, i
 }
 
 // E4 pool_kernel: one 256-thread block per sequence -> out [B, H] (H <= 1024: four columns per thread)
-static int launch_pool(const __half* hi, const __half* lo, const int* cu, int B, int H, int mode, int normalize, float* out,
-                       cudaStream_t st) {
+static int launch_pool(const __half* hi, const __half* lo, const int* cu, int B, int H, int mode, int normalize, bool compact,
+                       float* out, cudaStream_t st) {
     ProfScope _ps(PROF_POOL_HEAD, st);
-    pool_kernel<<<B, 256, 0, st>>>(hi, lo, cu, H, mode, normalize, out);
+    pool_kernel<<<B, 256, 0, st>>>(hi, lo, cu, H, mode, normalize, compact ? 1 : 0, out);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
 }
 
 // E4 cls_head_kernel: one 256-thread block per sequence, h_cls and the pooled vector in shared memory -> out [B, num_labels]
-static int launch_cls_head(const __half* hi, const __half* lo, const int* cu, int B, int H, int num_labels, const float* pw,
-                           const float* pb, const float* cw, const float* cb, float* out, cudaStream_t st) {
+static int launch_cls_head(const __half* hi, const __half* lo, const int* cu, int B, int H, int num_labels, bool compact,
+                           const float* pw, const float* pb, const float* cw, const float* cb, float* out, cudaStream_t st) {
     ProfScope _ps(PROF_POOL_HEAD, st);
-    cls_head_kernel<<<B, 256, 2 * H * sizeof(float), st>>>(hi, lo, cu, H, num_labels, pw, pb, cw, cb, out);
+    cls_head_kernel<<<B, 256, 2 * H * sizeof(float), st>>>(hi, lo, cu, H, num_labels, compact ? 1 : 0, pw, pb, cw, cb, out);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// row cu[b] of the hidden-state planes [T, H] -> compact planes [B, H]: one 128-thread block per sequence
+static int launch_gather_cls_rows(const __half* hi, const __half* lo, const int* cu, int B, int H, __half* out_hi,
+                                  __half* out_lo, cudaStream_t st) {
+    ProfScope _ps(PROF_MISC, st);
+    gather_cls_rows_kernel<<<B, 128, 0, st>>>(hi, lo, cu, H, out_hi, out_lo);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
@@ -545,12 +606,16 @@ struct rmu_encoder {
     std::vector<void*> allocs;
     float *word = nullptr, *pos = nullptr, *typ = nullptr, *eg = nullptr, *eb = nullptr;
     std::vector<EncLayer> layers;
+    SplitOperand last_wq, last_wkv;       // views of the last layer's Wqkv: rows 0..H (q) and H..3H (k | v)
     float *pw = nullptr, *pb = nullptr, *cw = nullptr, *cb = nullptr;
     // activations
     int tok_cap = 0, seq_cap = 0;
     std::vector<void*> act_allocs;
     SplitOperand X, CTX, X1, FF, QKVP;   // QKVP: q (pre-scaled) | k | v as split planes [T, 3H]
     float* PRE = nullptr;                 // fp32 pre-LayerNorm rows: projection + bias + residual
+    // the last layer on the CLS rows (run_last_layer_cls): row b = sequence b, [seq_cap, .]; X_cls ends as their hidden state
+    SplitOperand X_cls, Q_cls, CTX_cls, X1_cls, FF_cls;
+    float* PRE_cls = nullptr;
     // staging of the *_host entry points: owned by host_mu alone (NOT part of the activation workspace, which a
     // concurrent device-pointer caller may free and re-allocate under mu)
     int *d_ids = nullptr, *d_typ = nullptr, *d_cu = nullptr;
@@ -611,30 +676,78 @@ static int ensure_tokens(rmu_encoder* e, int T, int B) {
     int cap = std::max(T, 1024);
     cap = (cap + 127) / 128 * 128;
     const int scap = std::max(B + 1, 1024);
-    auto planes = [&](SplitOperand* op, int cols) -> int {
+    auto planes = [&](SplitOperand* op, int rows, int cols) -> int {
         __half *hi = nullptr, *lo = nullptr;
-        int rc = dev_alloc(e->act_allocs, &hi, static_cast<size_t>(cap) * cols);
-        if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &lo, static_cast<size_t>(cap) * cols);
+        int rc = dev_alloc(e->act_allocs, &hi, static_cast<size_t>(rows) * cols);
+        if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &lo, static_cast<size_t>(rows) * cols);
         if (rc != RMU_OK) return rc;
-        RMU_CUDA(cudaMemset(hi, 0, static_cast<size_t>(cap) * cols * sizeof(__half)));
-        RMU_CUDA(cudaMemset(lo, 0, static_cast<size_t>(cap) * cols * sizeof(__half)));
-        return make_split_operand(op, hi, lo, cap, cols);
+        RMU_CUDA(cudaMemset(hi, 0, static_cast<size_t>(rows) * cols * sizeof(__half)));
+        RMU_CUDA(cudaMemset(lo, 0, static_cast<size_t>(rows) * cols * sizeof(__half)));
+        return make_split_operand(op, hi, lo, rows, cols);
     };
-    int rc = planes(&e->X, H);
-    if (rc == RMU_OK) rc = planes(&e->CTX, H);
-    if (rc == RMU_OK) rc = planes(&e->X1, H);
-    if (rc == RMU_OK) rc = planes(&e->FF, F);
-    if (rc == RMU_OK) rc = planes(&e->QKVP, 3 * H);
+    int rc = planes(&e->X, cap, H);
+    if (rc == RMU_OK) rc = planes(&e->CTX, cap, H);
+    if (rc == RMU_OK) rc = planes(&e->X1, cap, H);
+    if (rc == RMU_OK) rc = planes(&e->FF, cap, F);
+    if (rc == RMU_OK) rc = planes(&e->QKVP, cap, 3 * H);
     if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->PRE, static_cast<size_t>(cap) * H);
+    // one row per sequence: B exceeds T when sequences are empty
+    if (rc == RMU_OK) rc = planes(&e->X_cls, scap, H);
+    if (rc == RMU_OK) rc = planes(&e->Q_cls, scap, H);
+    if (rc == RMU_OK) rc = planes(&e->CTX_cls, scap, H);
+    if (rc == RMU_OK) rc = planes(&e->X1_cls, scap, H);
+    if (rc == RMU_OK) rc = planes(&e->FF_cls, scap, F);
+    if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->PRE_cls, static_cast<size_t>(scap) * H);
     if (rc != RMU_OK) { free_acts(e); return rc; }
     e->tok_cap = cap;
     e->seq_cap = scap;
     return RMU_OK;
 }
 
-// the encoder stack: leaves the last hidden state in e->X (split planes)
+// The last layer when only the CLS rows leave the encoder (classifier head, CLS pooling).  The CLS query attends to
+// every key, so K and V are projected for all T rows, into the k | v columns of QKVP; everything else runs on row cu[b]
+// of each sequence alone, gathered into row b of the compact planes, and leaves that row's hidden state in e->X_cls.
+// Every kernel computes a row from that row's inputs alone with a fixed per-element order (E1 whatever the grid, E2 row 0
+// whatever the other query rows, ln_kernel one warp per row), so those rows are bit-identical to the full layer's.
+static int run_last_layer_cls(rmu_encoder* e, const EncLayer& L, const int32_t* cu, int B, int T, int max_seqlen,
+                              float qscale, cudaStream_t st) {
+    const rmu_bert_config& c = e->cfg;
+    const int H = c.hidden, F = c.ffn;
+    GemmParams g{};
+    g.M = T; g.N = 2 * H; g.K = H; g.bias = L.bqkv + H;
+    g.out_hi = e->QKVP.hi + H; g.out_lo = e->QKVP.lo + H; g.out_ld = 3 * H; g.qcols = 0; g.qscale = 1.0f;
+    int rc = launch_gemm(GEMM_BIAS_SPLIT_QSCALE, e->X, e->last_wkv, g, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    rc = launch_gather_cls_rows(e->X.hi, e->X.lo, cu, B, H, e->X_cls.hi, e->X_cls.lo, st);
+    if (rc != RMU_OK) return rc;
+    g = GemmParams{};
+    g.M = B; g.N = H; g.K = H; g.bias = L.bqkv; g.out_hi = e->Q_cls.hi; g.out_lo = e->Q_cls.lo; g.qcols = H; g.qscale = qscale;
+    rc = launch_gemm(GEMM_BIAS_SPLIT_QSCALE, e->X_cls, e->last_wq, g, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    rc = launch_attention(e->QKVP.hi, e->QKVP.lo, e->Q_cls.hi, e->Q_cls.lo, cu, B, H, c.heads, max_seqlen, 0, e->CTX_cls.hi,
+                          e->CTX_cls.lo, st);
+    if (rc != RMU_OK) return rc;
+    g = GemmParams{};
+    g.M = B; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE_cls; g.res_hi = e->X_cls.hi; g.res_lo = e->X_cls.lo;
+    rc = launch_gemm(GEMM_BIAS_RESID_F32, e->CTX_cls, L.Wo, g, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    rc = launch_layernorm(e->PRE_cls, B, H, L.ln1g, L.ln1b, c.ln_eps, e->X1_cls.hi, e->X1_cls.lo, st);
+    if (rc != RMU_OK) return rc;
+    g = GemmParams{};
+    g.M = B; g.N = F; g.K = H; g.bias = L.b1; g.out_hi = e->FF_cls.hi; g.out_lo = e->FF_cls.lo;
+    rc = launch_gemm(GEMM_BIAS_GELU_SPLIT, e->X1_cls, L.W1, g, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    g = GemmParams{};
+    g.M = B; g.N = H; g.K = F; g.bias = L.b2; g.out_f32 = e->PRE_cls; g.res_hi = e->X1_cls.hi; g.res_lo = e->X1_cls.lo;
+    rc = launch_gemm(GEMM_BIAS_RESID_F32, e->FF_cls, L.W2, g, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    return launch_layernorm(e->PRE_cls, B, H, L.ln2g, L.ln2b, c.ln_eps, e->X_cls.hi, e->X_cls.lo, st);
+}
+
+// the encoder stack: leaves the last hidden state in e->X (split planes), or with cls_only that of the CLS rows alone in
+// e->X_cls (row b = sequence b; e->X then holds the input of the last layer)
 static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_ids, const int32_t* cu, int B, int T,
-                       int max_seqlen, cudaStream_t st) {
+                       int max_seqlen, bool cls_only, cudaStream_t st) {
     const rmu_bert_config& c = e->cfg;
     const int H = c.hidden, F = c.ffn, DH = H / c.heads;
     if (max_seqlen > c.max_pos) { set_error("sequence longer than max_position_embeddings"); return RMU_ERR_ARG; }
@@ -645,19 +758,22 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
                          e->eb, c.ln_eps, e->X.hi, e->X.lo, st);
     if (rc != RMU_OK) return rc;
     const float scale = 1.0f / sqrtf(static_cast<float>(DH));
+    // q (scaled by 1/sqrt(dh)), k, v leave the GEMM as split fp16 planes: attention does no conversions
+    // (the softmax runs in base 2: q also carries log2(e))
+    const float qscale = scale * 1.4426950408889634f;
+    if (cls_only && c.layers == 0) return launch_gather_cls_rows(e->X.hi, e->X.lo, cu, B, H, e->X_cls.hi, e->X_cls.lo, st);
     for (int l = 0; l < c.layers; ++l) {
         EncLayer& L = e->layers[l];
+        if (cls_only && l == c.layers - 1) return run_last_layer_cls(e, L, cu, B, T, max_seqlen, qscale, st);
         GemmParams g{};
         g.M = T; g.N = 3 * H; g.K = H; g.bias = L.bqkv;
-        // q (scaled by 1/sqrt(dh)), k, v leave the GEMM as split fp16 planes: attention does no conversions
-        // (the softmax runs in base 2: q also carries log2(e))
-        g.out_hi = e->QKVP.hi; g.out_lo = e->QKVP.lo; g.qcols = H; g.qscale = scale * 1.4426950408889634f;
+        g.out_hi = e->QKVP.hi; g.out_lo = e->QKVP.lo; g.qcols = H; g.qscale = qscale;
         rc = launch_gemm(GEMM_BIAS_SPLIT_QSCALE, e->X, L.Wqkv, g, e->sms, st);
         if (rc != RMU_OK) return rc;
         // RMU_ATTN_WARPS = 5: 80-row CTAs, four per SM (same warps/SM, K/V staged twice per 147-token sequence)
         static const int nw_env = [] { const char* e = getenv("RMU_ATTN_WARPS"); return e ? atoi(e) : kAttWarps; }();
-        rc = launch_attention(e->QKVP.hi, e->QKVP.lo, cu, B, H, c.heads, max_seqlen, (nw_env == 5 && DH == 32) ? 5 : kAttWarps,
-                              e->CTX.hi, e->CTX.lo, st);
+        rc = launch_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, H, c.heads, max_seqlen,
+                              (nw_env == 5 && DH == 32) ? 5 : kAttWarps, e->CTX.hi, e->CTX.lo, st);
         if (rc != RMU_OK) return rc;
         g = GemmParams{};
         g.M = T; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE; g.res_hi = e->X.hi; g.res_lo = e->X.lo;
@@ -757,6 +873,12 @@ int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* w, int n_
         up(&Ly.ln2g, H);
         up(&Ly.ln2b, H);
     }
+    if (rc == RMU_OK && L > 0) {
+        const SplitOperand& W = e->layers[L - 1].Wqkv;
+        const size_t kv = static_cast<size_t>(H) * H;
+        rc = make_split_operand(&e->last_wq, W.hi, W.lo, H, H);
+        if (rc == RMU_OK) rc = make_split_operand(&e->last_wkv, W.hi + kv, W.lo + kv, 2 * H, H);
+    }
     if (has_head) {
         up(&e->pw, static_cast<size_t>(H) * H);
         up(&e->pb, H);
@@ -785,9 +907,11 @@ int rmu_encoder_embed(rmu_encoder* e, const int32_t* ids, const int32_t* type_id
     if (pool_mode != RMU_POOL_MEAN && pool_mode != RMU_POOL_CLS) { set_error("bad pool_mode"); return RMU_ERR_ARG; }
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, st);
+    const bool cls = pool_mode == RMU_POOL_CLS;
+    rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, cls, st);
     if (rc != RMU_OK) return rc;
-    rc = launch_pool(e->X.hi, e->X.lo, cu, B, e->cfg.hidden, pool_mode, normalize, out, st);
+    const SplitOperand& h = cls ? e->X_cls : e->X;
+    rc = launch_pool(h.hi, h.lo, cu, B, e->cfg.hidden, pool_mode, normalize, cls, out, st);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
@@ -800,9 +924,10 @@ int rmu_encoder_classify(rmu_encoder* e, const int32_t* ids, const int32_t* type
     if (!e->has_head) { set_error("rmu_encoder_classify: encoder was created without a classification head"); return RMU_ERR_ARG; }
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, st);
+    rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, true, st);
     if (rc != RMU_OK) return rc;
-    rc = launch_cls_head(e->X.hi, e->X.lo, cu, B, e->cfg.hidden, e->cfg.num_labels, e->pw, e->pb, e->cw, e->cb, out, st);
+    rc = launch_cls_head(e->X_cls.hi, e->X_cls.lo, cu, B, e->cfg.hidden, e->cfg.num_labels, true, e->pw, e->pb, e->cw, e->cb,
+                         out, st);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
@@ -814,7 +939,7 @@ int rmu_encoder_hidden(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
     if (rc != RMU_OK) return rc;
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, st);
+    rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, false, st);
     if (rc != RMU_OK) return rc;
     rc = launch_join_planes(e->X.hi, e->X.lo, static_cast<size_t>(T) * e->cfg.hidden, out, st);
     if (rc != RMU_OK) return rc;
@@ -885,8 +1010,8 @@ int rmu_debug_attention(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const in
         set_error("rmu_debug_attention: head_dim must be 32 or 64");
         return RMU_ERR_UNSUPPORTED;
     }
-    return launch_attention(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), cu, B, H,
-                            heads, max_seqlen, warps, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
+    return launch_attention(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), nullptr, nullptr,
+                            cu, B, H, heads, max_seqlen, warps, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
                             static_cast<cudaStream_t>(stream));
 }
 
@@ -931,7 +1056,7 @@ int rmu_debug_pool(const uint16_t* hi, const uint16_t* lo, const int32_t* cu, in
         return RMU_ERR_UNSUPPORTED;
     }
     return launch_pool(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), cu, B, H, pool_mode, normalize,
-                       out, static_cast<cudaStream_t>(stream));
+                       false, out, static_cast<cudaStream_t>(stream));
 }
 
 int rmu_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const int32_t* cu, int B, int H, int num_labels,
@@ -944,8 +1069,8 @@ int rmu_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const int32_t* cu
         set_error("rmu_debug_cls_head: hidden must be at most 1024");
         return RMU_ERR_UNSUPPORTED;
     }
-    return launch_cls_head(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), cu, B, H, num_labels, pw,
-                           pb, cw, cb, out, static_cast<cudaStream_t>(stream));
+    return launch_cls_head(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), cu, B, H, num_labels,
+                           false, pw, pb, cw, cb, out, static_cast<cudaStream_t>(stream));
 }
 
 int rmu_debug_split_planes(const float* src, int64_t n, uint16_t* hi, uint16_t* lo, void* stream) {

@@ -18,12 +18,13 @@ static int launch_mode(const SplitOperand& A, const SplitOperand& W, const GemmP
     RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kGemmSmem)));
     // output maps of exactly M rows (the TMA store clips the tail of the last row block): 128-row x 128-byte boxes
     CUtensorMap tOa{}, tOb{};
+    const uint64_t ld = static_cast<uint64_t>(p.out_ld ? p.out_ld : p.N);
     int rc;
     if (MODE == GEMM_BIAS_F32 || MODE == GEMM_BIAS_RESID_F32) {
-        rc = make_tmap_2d(&tOa, p.out_f32, static_cast<uint64_t>(p.M), static_cast<uint64_t>(p.N),
-                          static_cast<uint64_t>(p.N) * sizeof(float), 32, kGemmBM, 4);
+        rc = make_tmap_2d(&tOa, p.out_f32, static_cast<uint64_t>(p.M), static_cast<uint64_t>(p.N), ld * sizeof(float), 32,
+                          kGemmBM, 4);
     } else {
-        const uint64_t pitch = static_cast<uint64_t>(p.N) * sizeof(__half);
+        const uint64_t pitch = ld * sizeof(__half);
         rc = make_tmap_2d(&tOa, p.out_hi, static_cast<uint64_t>(p.M), static_cast<uint64_t>(p.N), pitch, 64, kGemmBM, 2);
         if (rc == RMU_OK) rc = make_tmap_2d(&tOb, p.out_lo, static_cast<uint64_t>(p.M), static_cast<uint64_t>(p.N), pitch, 64, kGemmBM, 2);
     }
@@ -39,7 +40,8 @@ static int launch_mode(const SplitOperand& A, const SplitOperand& W, const GemmP
 
 int launch_gemm(int mode, const SplitOperand& A, const SplitOperand& W, const GemmParams& p, int sms, cudaStream_t st) {
     if (p.M <= 0) return RMU_OK;
-    if (p.N % kGemmBN != 0 || p.K % kGemmBK != 0 || A.cols != p.K || W.cols != p.K || W.rows < p.N || A.rows < p.M) {
+    if (p.N % kGemmBN != 0 || p.K % kGemmBK != 0 || A.cols != p.K || W.cols != p.K || W.rows < p.N || A.rows < p.M ||
+        (p.out_ld != 0 && p.out_ld < p.N)) {
         set_error("launch_gemm: shape not supported (N % 128, K % 64)");
         return RMU_ERR_UNSUPPORTED;
     }

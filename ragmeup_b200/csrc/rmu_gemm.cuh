@@ -54,6 +54,7 @@ struct GemmParams {
     __half* out_hi; __half* out_lo;       // [M, N]
     const __half* res_hi; const __half* res_lo;  // [M, N]
     int qcols; float qscale;              // GEMM_BIAS_SPLIT_QSCALE
+    int out_ld;                           // row pitch of out_f32 / out_hi / out_lo in elements (0 = N)
 };
 
 __device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {
