@@ -189,8 +189,10 @@ void rmu_encoder_destroy(rmu_encoder* enc);
  * max_seqlen must be at least the longest sequence in cu_seqlens; only max_seqlen itself is checked against
  * max_position_embeddings (cu_seqlens is on the device).  Out-of-range inputs are clamped on the device, where
  * HuggingFace raises an IndexError: token ids into [0, vocab_size), type ids into [0, type_vocab), and positions past
- * max_position_embeddings - 1 take that last row.  An empty sequence (cu_seqlens[b + 1] == cu_seqlens[b]) is allowed.
- * These rules hold for every rmu_encoder_* entry point below.
+ * max_position_embeddings - 1 take that last row.  An empty sequence (cu_seqlens[b + 1] == cu_seqlens[b]) is allowed,
+ * but a batch must hold at least one token: B < 1 or total_tokens < 1 (a batch of empty sequences only) returns
+ * RMU_ERR_ARG before any CUDA call.  B has no upper limit besides int and device memory (attention runs batches of more
+ * than 65 535 sequences in slices).  These rules hold for every rmu_encoder_* entry point below.
  * out [B, hidden] fp32 sentence embeddings; an empty sequence gets a zero vector. */
 int rmu_encoder_embed(rmu_encoder* enc, const int32_t* ids, const int32_t* type_ids, const int32_t* cu_seqlens,
                       int B, int total_tokens, int max_seqlen, int pool_mode, int normalize, float* out,

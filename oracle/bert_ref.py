@@ -43,10 +43,10 @@ class BertCfg:
     num_labels: int = 1
 
 
-def _t(w) -> torch.Tensor:
+def _t(w, device=None) -> torch.Tensor:
     if isinstance(w, torch.Tensor):
-        return w.detach().to(torch.float32).cpu()
-    return torch.from_numpy(np.ascontiguousarray(w, dtype=np.float32))
+        return w.detach().to(device=device or "cpu", dtype=torch.float32)
+    return torch.from_numpy(np.ascontiguousarray(w, dtype=np.float32)).to(device or "cpu")
 
 
 def _layer_norm(x: torch.Tensor, g: torch.Tensor, b: torch.Tensor, eps: float) -> torch.Tensor:
@@ -62,41 +62,46 @@ def _gelu_erf(x: torch.Tensor) -> torch.Tensor:
 def bert_encoder_forward(w: Dict[str, object], cfg: BertCfg, input_ids: torch.Tensor,
                          attention_mask: torch.Tensor,
                          token_type_ids: Optional[torch.Tensor] = None,
-                         matmul=None) -> torch.Tensor:
+                         matmul=None, device=None) -> torch.Tensor:
     """[B,S] ids/mask/type -> last hidden state [B,S,H], fp32, padded computation
     (additive mask = finfo.min on padded keys, exactly the HF eager path).
 
     ``matmul(x, W)`` computes ``x @ W.T``; tests swap it to emulate reduced
-    precision when sizing tolerances."""
+    precision when sizing tolerances.  ``device`` (default the CPU) is where the
+    forward runs; the result stays there."""
     mm = matmul or (lambda x, W: x @ W.t())
+    dev = device or "cpu"
+    tw = lambda a: _t(a, dev)  # noqa: E731
+    input_ids, attention_mask = input_ids.to(dev), attention_mask.to(dev)
     B, S = input_ids.shape
     H, nh = cfg.hidden, cfg.heads
     dh = H // nh
     if token_type_ids is None:
         token_type_ids = torch.zeros_like(input_ids)
-    pos = torch.arange(S)
-    x = (_t(w["embeddings.word_embeddings.weight"])[input_ids]
-         + _t(w["embeddings.token_type_embeddings.weight"])[token_type_ids]
-         + _t(w["embeddings.position_embeddings.weight"])[pos][None])
-    x = _layer_norm(x, _t(w["embeddings.LayerNorm.weight"]), _t(w["embeddings.LayerNorm.bias"]), cfg.ln_eps)
+    token_type_ids = token_type_ids.to(dev)
+    pos = torch.arange(S, device=dev)
+    x = (tw(w["embeddings.word_embeddings.weight"])[input_ids]
+         + tw(w["embeddings.token_type_embeddings.weight"])[token_type_ids]
+         + tw(w["embeddings.position_embeddings.weight"])[pos][None])
+    x = _layer_norm(x, tw(w["embeddings.LayerNorm.weight"]), tw(w["embeddings.LayerNorm.bias"]), cfg.ln_eps)
     add_mask = (1.0 - attention_mask.to(torch.float32))[:, None, None, :] * torch.finfo(torch.float32).min
     for l in range(cfg.layers):
         p = f"encoder.layer.{l}."
-        q = mm(x, _t(w[p + "attention.self.query.weight"])) + _t(w[p + "attention.self.query.bias"])
-        k = mm(x, _t(w[p + "attention.self.key.weight"])) + _t(w[p + "attention.self.key.bias"])
-        v = mm(x, _t(w[p + "attention.self.value.weight"])) + _t(w[p + "attention.self.value.bias"])
+        q = mm(x, tw(w[p + "attention.self.query.weight"])) + tw(w[p + "attention.self.query.bias"])
+        k = mm(x, tw(w[p + "attention.self.key.weight"])) + tw(w[p + "attention.self.key.bias"])
+        v = mm(x, tw(w[p + "attention.self.value.weight"])) + tw(w[p + "attention.self.value.bias"])
         q = q.view(B, S, nh, dh).transpose(1, 2)
         k = k.view(B, S, nh, dh).transpose(1, 2)
         v = v.view(B, S, nh, dh).transpose(1, 2)
         att = torch.matmul(q, k.transpose(2, 3)) * (dh ** -0.5) + add_mask
         att = torch.softmax(att, dim=-1)
         ctx = torch.matmul(att, v).transpose(1, 2).reshape(B, S, H)
-        o = mm(ctx, _t(w[p + "attention.output.dense.weight"])) + _t(w[p + "attention.output.dense.bias"])
-        x = _layer_norm(o + x, _t(w[p + "attention.output.LayerNorm.weight"]),
-                        _t(w[p + "attention.output.LayerNorm.bias"]), cfg.ln_eps)
-        f = _gelu_erf(mm(x, _t(w[p + "intermediate.dense.weight"])) + _t(w[p + "intermediate.dense.bias"]))
-        o = mm(f, _t(w[p + "output.dense.weight"])) + _t(w[p + "output.dense.bias"])
-        x = _layer_norm(o + x, _t(w[p + "output.LayerNorm.weight"]), _t(w[p + "output.LayerNorm.bias"]), cfg.ln_eps)
+        o = mm(ctx, tw(w[p + "attention.output.dense.weight"])) + tw(w[p + "attention.output.dense.bias"])
+        x = _layer_norm(o + x, tw(w[p + "attention.output.LayerNorm.weight"]),
+                        tw(w[p + "attention.output.LayerNorm.bias"]), cfg.ln_eps)
+        f = _gelu_erf(mm(x, tw(w[p + "intermediate.dense.weight"])) + tw(w[p + "intermediate.dense.bias"]))
+        o = mm(f, tw(w[p + "output.dense.weight"])) + tw(w[p + "output.dense.bias"])
+        x = _layer_norm(o + x, tw(w[p + "output.LayerNorm.weight"]), tw(w[p + "output.LayerNorm.bias"]), cfg.ln_eps)
     return x
 
 
@@ -116,9 +121,10 @@ def l2_normalize(x: torch.Tensor) -> torch.Tensor:
 
 
 def classifier_head(w: Dict[str, object], hidden: torch.Tensor) -> torch.Tensor:
-    """BertForSequenceClassification head: pooler tanh + classifier -> [B, num_labels]."""
-    pooled = torch.tanh(hidden[:, 0] @ _t(w["pooler.dense.weight"]).t() + _t(w["pooler.dense.bias"]))
-    return pooled @ _t(w["classifier.weight"]).t() + _t(w["classifier.bias"])
+    """BertForSequenceClassification head: pooler tanh + classifier -> [B, num_labels], on hidden's device."""
+    dev = hidden.device
+    pooled = torch.tanh(hidden[:, 0] @ _t(w["pooler.dense.weight"], dev).t() + _t(w["pooler.dense.bias"], dev))
+    return pooled @ _t(w["classifier.weight"], dev).t() + _t(w["classifier.bias"], dev)
 
 
 # --------------------------------------------------------------------------- host-side batching rules

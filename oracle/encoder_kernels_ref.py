@@ -14,6 +14,9 @@ reference is the kernel's own arithmetic:
 * ``pool_ref``: E4 ``pool_kernel``, mean or CLS pooling and the optional L2 normalisation (sentence-transformers
   Pooling + Normalize);
 * ``cls_head_ref``: E4 ``cls_head_kernel``, BertPooler tanh(W_p h_cls + b_p) and the classifier.
+
+``encoder_stack_ref`` composes them into the whole encoder in float64, with the GEMM weights either as the fp32
+tensors or as hi + lo of the split planes ``rmu_encoder_create`` uploads (``split_weight``).
 """
 from __future__ import annotations
 
@@ -176,3 +179,63 @@ def cls_head_ref(hi, lo, cu, pw, pb, cw, cb):
     pooled = torch.tanh(z)
     logits = pooled @ Wc.T + _f64(cb).to(x.device)[None, :]
     return logits, z, pooled, h.abs() @ W.abs().T, pooled.abs() @ Wc.abs().T
+
+
+# the six GEMM weights of a layer, which rmu_encoder_create uploads as split planes
+GEMM_WEIGHTS = ("attention.self.query.weight", "attention.self.key.weight", "attention.self.value.weight",
+                "attention.output.dense.weight", "intermediate.dense.weight", "output.dense.weight")
+
+
+def split_weight(w) -> torch.Tensor:
+    """fp32 weight (numpy or torch, any device) -> hi + lo of its split planes in float64, on the same device.  For
+    |w| < 2^-14 * 2^11 ~ 0.125 the lo plane is an fp16 subnormal, so a weight keeps max(2^-22 |w|, 2^-25) of error
+    instead of 2^-22 |w|."""
+    t = (w if isinstance(w, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(w, np.float32))).to(torch.float32)
+    hi = t.half()
+    return hi.double() + (t - hi.float()).half().double()
+
+
+def encoder_stack_ref(w, cfg, ids, type_ids, cu, weights: str = "fp32", device=None) -> dict:
+    """The whole encoder in float64 on the ragged batch (ids [T], type_ids [T] or None = all 0, cu [B + 1]), with the
+    kernels' documented rules: ids, type ids and positions clamped (``embed_ln_ref``), an empty sequence embeds as
+    zeros and scores W_c tanh(b_p) + b_c (``pool_ref``, ``cls_head_ref``).  ``w`` is the weight dict of
+    ``ragmeup_b200.weights.weight_names``; cfg anything with hidden, heads, layers and ln_eps.  weights = "fp32" takes the
+    GEMM weights as given, "split" as hi + lo of their split planes (``split_weight``).  Runs in torch on ``device``
+    (default the CPU).  Returns {"hidden": [T, H], "mean" / "cls" / "mean_norm" / "cls_norm": [B, H], and "logits":
+    [B, num_labels] when w holds the head}, float64 on ``device``."""
+    if weights not in ("fp32", "split"):
+        raise ValueError(weights)
+    dev = torch.device(device or "cpu")
+    W = lambda name: (split_weight(w[name]) if weights == "split" else _f64(w[name])).to(dev)  # noqa: E731
+    V = lambda name: _f64(w[name]).to(dev)                                                        # noqa: E731
+    cu_l = [int(c) for c in cu]
+    H, heads, eps = cfg.hidden, cfg.heads, float(cfg.ln_eps)
+    x = embed_ln_ref(_long(ids, dev), None if type_ids is None else _long(type_ids, dev), _long(cu_l, dev),
+                     V("embeddings.word_embeddings.weight"), V("embeddings.position_embeddings.weight"),
+                     V("embeddings.token_type_embeddings.weight"), V("embeddings.LayerNorm.weight"),
+                     V("embeddings.LayerNorm.bias"), eps)[0]
+    qs = math.log2(math.e) / math.sqrt(H // heads)        # the exact scale attention_ref's base-2 softmax expects
+    z = torch.zeros_like
+    for l in range(cfg.layers):
+        p = f"encoder.layer.{l}."
+        wqkv = torch.cat([W(p + "attention.self." + n + ".weight") for n in ("query", "key", "value")])
+        bqkv = torch.cat([V(p + "attention.self." + n + ".bias") for n in ("query", "key", "value")])
+        qkv = gemm_ref(GEMM_BIAS_F32, x, z(x), wqkv, z(wqkv), bqkv)[0]
+        qkv[:, :H] *= qs
+        ctx = attention_ref(qkv, z(qkv), cu_l, heads)[0]
+        wo = W(p + "attention.output.dense.weight")
+        o = gemm_ref(GEMM_BIAS_RESID_F32, ctx, z(ctx), wo, z(wo), V(p + "attention.output.dense.bias"), x, z(x))[0]
+        x1 = layernorm_ref(o, V(p + "attention.output.LayerNorm.weight"), V(p + "attention.output.LayerNorm.bias"), eps)[0]
+        w1 = W(p + "intermediate.dense.weight")
+        f = gemm_ref(GEMM_BIAS_GELU_SPLIT, x1, z(x1), w1, z(w1), V(p + "intermediate.dense.bias"))[0]
+        w2 = W(p + "output.dense.weight")
+        o = gemm_ref(GEMM_BIAS_RESID_F32, f, z(f), w2, z(w2), V(p + "output.dense.bias"), x1, z(x1))[0]
+        x = layernorm_ref(o, V(p + "output.LayerNorm.weight"), V(p + "output.LayerNorm.bias"), eps)[0]
+    out = {"hidden": x}
+    for mode, name in ((0, "mean"), (1, "cls")):
+        out[name] = pool_ref(x, z(x), cu_l, mode, False)[0]
+        out[name + "_norm"] = pool_ref(x, z(x), cu_l, mode, True)[0]
+    if "pooler.dense.weight" in w:
+        out["logits"] = cls_head_ref(x, z(x), cu_l, V("pooler.dense.weight"), V("pooler.dense.bias"),
+                                     V("classifier.weight"), V("classifier.bias"))[0]
+    return out

@@ -493,6 +493,10 @@ constexpr int kClsAttWarps = 4;
 // warps = 10 (160-row CTAs), or 5 (80-row CTAs, four per SM) with d_h = 32.
 // cls_q_hi / cls_q_lo non-null: query row 0 of each sequence only, q from those compact planes [B, H] -> ctx [B, H]
 // (the K / V columns of the QKV planes are read as above; their Q columns are not); `warps` is ignored.
+// The sequence index is gridDim.y, at most 65 535: a larger batch runs in slices of 65 535 sequences, each launch with
+// cu (and in CLS mode the compact Q and context rows) offset by the slice start.  Within a slice the grid and the
+// kernel are those of one launch, so the heads of a sequence still run together and every row is computed the same.
+constexpr int kMaxGridY = 65535;
 static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __half* cls_q_hi, const __half* cls_q_lo,
                             const int* cu, int B, int H, int heads, int max_seqlen, int warps, __half* ctx_hi,
                             __half* ctx_lo, cudaStream_t st) {
@@ -502,7 +506,6 @@ static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __
     else if (!(warps == kAttWarps || (warps == 5 && DH == 32))) { set_error("attention: warps must be 10, or 5 with head_dim 32"); return RMU_ERR_ARG; }
     ProfScope _ps(PROF_ATTN, st);
     const unsigned zblocks = cls ? 1u : static_cast<unsigned>((max_seqlen + warps * 16 - 1) / (warps * 16));
-    dim3 pg(static_cast<unsigned>(heads), static_cast<unsigned>(B), zblocks);
     // keys resident per CTA: the whole (longest) sequence when it fits, else super-blocks of kKeySB
     const int ksb = std::min(kKeySB, (max_seqlen + 31) / 32 * 32);
     const size_t smem_max = 4 * sizeof(__half) * static_cast<size_t>(kKeySB) * (DH + 8);
@@ -511,9 +514,16 @@ static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __
               : DH == 32 ? (warps == 5 ? attention_planes_kernel<32, 4, 5> : attention_planes_kernel<32, 2>)
                          : attention_planes_kernel<64, 1>;   // d_h = 64 needs > 96 registers
     RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
-    kern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, cls_q_hi, cls_q_lo, cu, H, ksb, ctx_hi, ctx_lo);
-    count_launch();
-    RMU_CHECK_LAUNCH();
+    for (int s0 = 0; s0 < B; s0 += kMaxGridY) {
+        const int nb = std::min(kMaxGridY, B - s0);
+        // full mode addresses Q and the context by token (cu[b] is absolute), CLS mode by sequence
+        const size_t roff = cls ? static_cast<size_t>(s0) * H : 0;
+        dim3 pg(static_cast<unsigned>(heads), static_cast<unsigned>(nb), zblocks);
+        kern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, cls ? cls_q_hi + roff : nullptr, cls ? cls_q_lo + roff : nullptr,
+                                           cu + s0, H, ksb, ctx_hi + roff, ctx_lo + roff);
+        count_launch();
+        RMU_CHECK_LAUNCH();
+    }
     return RMU_OK;
 }
 

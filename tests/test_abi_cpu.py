@@ -191,6 +191,22 @@ def test_encoder_create_refuses_weights_the_split_planes_cannot_hold(built_lib):
         assert create(name, 0, 7e4) in (0, -2), name
 
 
+def test_encoder_refuses_a_batch_without_tokens(built_lib):
+    """Empty sequences are allowed, but a batch of empty sequences only (total_tokens = 0), or no sequence at all, is
+    refused with RMU_ERR_ARG before the handle is read or any CUDA call is made (include/ragmeup_b200.h)"""
+    from ragmeup_b200 import _lib
+    l = _lib.lib()
+    p = 1 << 20
+    fake = ctypes.c_void_p(p)                               # never dereferenced: every call below is refused first
+    for B, T in ((3, 0), (1, 0), (0, 0), (0, 5), (-1, 5), (3, -1)):
+        assert l.rmu_encoder_embed(fake, p, None, p, B, T, 1, 0, 1, p, None) == -1, (B, T)
+        assert l.rmu_encoder_classify(fake, p, None, p, B, T, 1, p, None) == -1, (B, T)
+        assert l.rmu_encoder_hidden(fake, p, p, p, B, T, 1, p, None) == -1, (B, T)
+        assert l.rmu_encoder_embed_host(fake, p, None, p, B, T, 1, 1, 0, p, None) == -1, (B, T)
+        assert l.rmu_encoder_classify_host(fake, p, p, p, B, T, 1, p, None) == -1, (B, T)
+    assert b"encoder" in l.rmu_last_error()
+
+
 def test_product_fails_loudly_without_cuda(built_lib):
     import torch
     if torch.cuda.is_available():

@@ -108,6 +108,11 @@ GEMM_CASES = [
     (3, 127, 384, 128, 1.0, 1.0, 0, (2, 0)),              # q-scale on no column
     (3, 127, 384, 128, 1.0, 1.0, 384, (2, 0)),            # q-scale on every column
     (3, 130, 384, 320, 1.0, 1.0, 128, (1, 0)),            # q-scale boundary at a tile edge, 5 K blocks
+    (3, 1000, 3072, 1024, 1.0, 0.02, 1024, (3, 0)),       # QKV of H = 1024 (bge-large): N = 3072, 16 K blocks
+    (1, 1000, 4096, 1024, 1.0, 0.02, 0, (3, 0)),          # FFN-in of H = 1024: N = 4096
+    (2, 1000, 1024, 4096, 1.0, 0.02, 0, (1, 0)),          # FFN-out of H = 1024: K = 4096, 64 K blocks
+    (3, 300, 2688, 896, 1.0, 0.02, 896, (2, 0)),          # QKV of H = 896: 21 tiles wide, 14 K blocks
+    (1, 300, 2688, 896, 1.0, 0.02, 0, (2, 0)),            # FFN-in of H = 896, F = 2688
 ]
 
 
@@ -239,6 +244,9 @@ ATT_CASES = [
     (384, 12, "random", [257], 257, (10, 5)),           # one key past the first super-block
     (768, 12, "random", [256], 256, (10,)),
     (768, 12, "random", [257], 257, (10,)),
+    (1024, 16, "random", LENS, None, (10,)),            # bge-large: d_h = 64 at the largest H
+    (1024, 32, "random", LENS, None, (10, 5)),          # d_h = 32 at the largest H
+    (128, 2, "random", LENS, None, (10,)),              # d_h = 64 at the smallest H
 ]
 
 
@@ -310,7 +318,7 @@ def _ln_rows(rng, T, H):
     return x, const
 
 
-@pytest.mark.parametrize("H", [128, 384, 768, 1024])
+@pytest.mark.parametrize("H", [128, 384, 768, 896, 1024])
 @pytest.mark.parametrize("T", [1, 7, 9, 1001])
 @pytest.mark.parametrize("eps", [1e-12, 1e-5])
 def test_layernorm_matches_float64(cuda, H, T, eps):
@@ -406,7 +414,7 @@ def _same(a, b):
 
 
 # H = 128 ... 1024: per_lane 4 to 32, every branch of the kernel's unrolled loops; T not a multiple of 8 tokens per block
-EMB_CASES = [(H, batch) for H in (128, 256, 384, 640, 768, 1024) for batch in ("T=1", "T=7", "T=9", "T=4097")] + \
+EMB_CASES = [(H, batch) for H in (128, 256, 384, 640, 768, 896, 1024) for batch in ("T=1", "T=7", "T=9", "T=4097")] + \
     [(128, "B=70000"), (768, "B=70000")]
 
 

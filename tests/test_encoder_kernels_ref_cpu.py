@@ -1,12 +1,15 @@
 """CPU: the float64 per-kernel references (oracle/encoder_kernels_ref.py) against independent restatements, so that
 tests/test_encoder_kernels_gpu.py judges the kernels against something that is itself pinned."""
 import math
+from dataclasses import asdict
 
 import numpy as np
+import pytest
 import torch
 
 from oracle import bert_ref
 from oracle import encoder_kernels_ref as ref
+from ragmeup_b200.weights import PRESETS, BertConfig, synthetic_bert_weights
 
 
 def test_split_emulation_matches_torch_half():
@@ -207,3 +210,179 @@ def test_cls_head_reference_agrees_with_bert_ref():
     assert (np.abs(z) > 20).all() and np.array_equal(np.abs(pooled), np.ones_like(pooled))
     sgn = np.sign(pb).astype(np.float64)
     assert np.allclose(logits, np.broadcast_to(args[2].astype(np.float64) @ sgn + args[3], logits.shape), rtol=0, atol=1e-12)
+
+
+# ------------------------------------------------------------------------------------------- the whole stack
+def _ragged(ids, mask, typ):
+    lens = mask.sum(1)
+    cu = np.r_[0, np.cumsum(lens)]
+    return (np.concatenate([ids[b, :n] for b, n in enumerate(lens)]), np.concatenate([typ[b, :n] for b, n in enumerate(lens)]),
+            cu)
+
+
+@pytest.mark.parametrize("preset,seed,scale", [("tiny", 0, 1.0), ("all-MiniLM-L6-v2", 1, 4.0)])
+def test_stack_reference_matches_bert_ref_and_the_hf_goldens(golden_dir, preset, seed, scale):
+    """float64 forward on the fp32 weights: within the oracle's own tolerances (tests/test_oracle_golden.py) of the HF
+    goldens, and of bert_ref's padded fp32 forward"""
+    g = np.load(f"{golden_dir}/encoder.npz")
+    key = f"enc_{preset}_{seed}_{scale}"
+    cfg = BertConfig(**asdict(PRESETS[preset][0]))
+    w = synthetic_bert_weights(cfg, seed=seed, scale=scale)
+    I, M, Ty = (g[key + s].astype(np.int64) for s in ("_ids", "_mask", "_typ"))
+    ids, typ, cu = _ragged(I, M, Ty)
+    out = {k: v.numpy() for k, v in ref.encoder_stack_ref(w, cfg, ids, typ, cu).items()}
+    tol = 2e-5 if scale == 1.0 else 2e-4
+    assert np.abs(out["mean_norm"] - g[key + "_mean"]).max() < tol
+    assert np.abs(out["cls_norm"] - g[key + "_cls"]).max() < tol
+    assert np.abs(out["hidden"][cu[:-1]] - g[key + "_h_first"]).max() < 50 * tol
+    assert np.abs(out["hidden"][cu[1:] - 1] - g[key + "_h_last"]).max() < 50 * tol
+    with torch.no_grad():
+        h = bert_ref.bert_encoder_forward(w, bert_ref.BertCfg(**asdict(cfg)), *(torch.from_numpy(a) for a in (I, M, Ty)))
+        mean = bert_ref.pool(h, torch.from_numpy(M), "mean")
+    flat = torch.cat([h[b, :n] for b, n in enumerate(M.sum(1))]).double().numpy()
+    assert np.abs(out["hidden"] - flat).max() < 1e-4
+    assert np.abs(out["mean"] - mean.double().numpy()).max() < 1e-5
+    assert np.abs(out["mean_norm"] - bert_ref.l2_normalize(mean).double().numpy()).max() < 1e-5
+
+
+@pytest.mark.parametrize("preset,seed,scale", [("tiny", 3, 4.0), ("ms-marco-MiniLM-L-6-v2", 0, 1.0)])
+def test_stack_reference_logits_match_the_hf_goldens(golden_dir, preset, seed, scale):
+    g = np.load(f"{golden_dir}/cross_encoder.npz")
+    key = f"ce_{preset}_{seed}_{scale}"
+    cfg = BertConfig(**asdict(PRESETS[preset][0]))
+    w = synthetic_bert_weights(cfg, seed=seed, with_head=True, scale=scale)
+    ids, typ, cu = _ragged(*(g[key + s].astype(np.int64) for s in ("_ids", "_mask", "_typ")))
+    logits = ref.encoder_stack_ref(w, cfg, ids, typ, cu)["logits"].numpy()
+    assert np.abs(logits - g[key + "_logits"]).max() < (2e-5 if scale == 1.0 else 5e-4)
+
+
+def _small_cfg(layers, **kw):
+    a = dict(vocab_size=60, hidden=128, layers=layers, heads=2, ffn=256, max_pos=16, type_vocab=2, num_labels=3)
+    a.update(kw)
+    return BertConfig(**a)
+
+
+def test_stack_reference_layer_by_layer():
+    """Layer l of the stack is the per-kernel references applied to layer l - 1's output in the encoder's order (QKV with
+    q scaled by log2(e) / sqrt(d_h), attention, output projection + residual, LayerNorm, GELU FFN + residual, LayerNorm),
+    and bert_ref's fp32 forward truncated to l layers agrees to fp32 accuracy.  Empty sequences first, in the middle and
+    last; ids, type ids and positions out of range are clamped."""
+    cfg = _small_cfg(3)
+    w = synthetic_bert_weights(cfg, seed=11, with_head=True, scale=4.0)
+    rng = np.random.default_rng(12)
+    lens = [0, 5, 16, 0, 1, 9, 0]
+    cu = np.r_[0, np.cumsum(lens)]
+    T = int(cu[-1])
+    ids = rng.integers(0, cfg.vocab_size, T)
+    typ = rng.integers(0, 2, T)
+    ids[3], ids[7], typ[4], typ[8] = -4, cfg.vocab_size + 2, -1, 5
+    H, dh = cfg.hidden, cfg.hidden // cfg.heads
+    V = lambda n: torch.from_numpy(w[n].astype(np.float64))  # noqa: E731
+    prev = None
+    for L in range(cfg.layers + 1):
+        c = BertConfig(**{**asdict(cfg), "layers": L})
+        got = ref.encoder_stack_ref(w, c, ids, typ, cu)
+        if L == 0:
+            want = ref.embed_ln_ref(ids, typ, cu, *(w["embeddings." + n] for n in (
+                "word_embeddings.weight", "position_embeddings.weight", "token_type_embeddings.weight",
+                "LayerNorm.weight", "LayerNorm.bias")), cfg.ln_eps)[0]
+        else:
+            p = f"encoder.layer.{L - 1}."
+            x = prev
+            q = x @ V(p + "attention.self.query.weight").T + V(p + "attention.self.query.bias")
+            k = x @ V(p + "attention.self.key.weight").T + V(p + "attention.self.key.bias")
+            v = x @ V(p + "attention.self.value.weight").T + V(p + "attention.self.value.bias")
+            qkv = torch.cat([q * (math.log2(math.e) / math.sqrt(dh)), k, v], 1)
+            ctx = ref.attention_ref(qkv, torch.zeros_like(qkv), cu, cfg.heads)[0]
+            o = ctx @ V(p + "attention.output.dense.weight").T + V(p + "attention.output.dense.bias") + x
+            x1 = ref.layernorm_ref(o, w[p + "attention.output.LayerNorm.weight"], w[p + "attention.output.LayerNorm.bias"],
+                                   cfg.ln_eps)[0]
+            f = bert_ref._gelu_erf(x1 @ V(p + "intermediate.dense.weight").T + V(p + "intermediate.dense.bias"))
+            o = f @ V(p + "output.dense.weight").T + V(p + "output.dense.bias") + x1
+            want = ref.layernorm_ref(o, w[p + "output.LayerNorm.weight"], w[p + "output.LayerNorm.bias"], cfg.ln_eps)[0]
+        assert torch.allclose(got["hidden"], want, rtol=0, atol=1e-12), f"layer {L}"
+        prev = got["hidden"]
+        # bert_ref in fp32, padded, on the clamped inputs (it indexes the tables directly)
+        S = max(lens)
+        I = np.zeros((len(lens), S), np.int64); M = np.zeros_like(I); Ty = np.zeros_like(I)
+        for b, n in enumerate(lens):
+            I[b, :n] = np.clip(ids[cu[b]:cu[b + 1]], 0, cfg.vocab_size - 1)
+            Ty[b, :n] = np.clip(typ[cu[b]:cu[b + 1]], 0, 1)
+            M[b, :n] = 1
+        with torch.no_grad():
+            h = bert_ref.bert_encoder_forward(w, bert_ref.BertCfg(**asdict(c)), *(torch.from_numpy(a) for a in (I, M, Ty)))
+        flat = torch.cat([h[b, :n] for b, n in enumerate(lens)]).double()
+        assert (got["hidden"] - flat).abs().max() < 2e-5, f"layer {L} vs bert_ref"
+    # the outputs of the last layer: pooling and head rules, empty sequences included
+    empty = np.diff(cu) == 0
+    for name in ("mean", "cls", "mean_norm", "cls_norm"):
+        assert (got[name][torch.from_numpy(empty)] == 0).all()
+    e = np.tanh(w["pooler.dense.bias"].astype(np.float64)) @ w["classifier.weight"].T.astype(np.float64) + w["classifier.bias"]
+    assert np.allclose(got["logits"].numpy()[empty], e, rtol=0, atol=1e-14)
+    assert torch.equal(got["cls"][torch.from_numpy(~empty)], got["hidden"][torch.from_numpy(cu[:-1][~empty])])
+
+
+def test_stack_reference_on_split_weights_is_the_forward_on_hi_plus_lo():
+    """weights="split" is exactly the fp32 forward on fp32(hi + lo) (hi + lo has at most 22 significant bits, so it is
+    an fp32 value), and only the GEMM weights are split"""
+    cfg = _small_cfg(2)
+    w = synthetic_bert_weights(cfg, seed=13, with_head=True, scale=1.0)
+    ws = dict(w)
+    for name in w:
+        if name.endswith(ref.GEMM_WEIGHTS):
+            hi, lo = ref.split_f16(w[name])
+            joined = ref.join(hi, lo)
+            assert np.array_equal(joined.astype(np.float32).astype(np.float64), joined)
+            ws[name] = joined.astype(np.float32)
+            assert np.array_equal(ref.split_weight(w[name]).numpy(), joined)
+    assert sum(n.endswith(ref.GEMM_WEIGHTS) for n in w) == 6 * cfg.layers
+    rng = np.random.default_rng(14)
+    # a subnormal lo plane: |w| ~ 0.02 keeps its error under max(2^-22 |w|, 2^-25); most weights exceed 2^-22 |w|
+    x = (0.02 * rng.standard_normal(100000)).astype(np.float32)
+    err = np.abs(ref.split_weight(x).numpy() - x.astype(np.float64))
+    assert (err <= np.maximum(2.0 ** -22 * np.abs(x), 2.0 ** -25)).all()
+    assert (err > 2.0 ** -22 * np.abs(x)).mean() > 0.5
+    lens = [3, 0, 16, 7]
+    cu = np.r_[0, np.cumsum(lens)]
+    ids = rng.integers(0, cfg.vocab_size, cu[-1])
+    a = ref.encoder_stack_ref(w, cfg, ids, None, cu, weights="split")
+    b = ref.encoder_stack_ref(ws, cfg, ids, None, cu, weights="fp32")
+    for k in a:
+        assert torch.equal(a[k], b[k]), k
+
+
+# What the split weights cost, measured (float64 forward on hi + lo against the float64 forward on the fp32 weights,
+# synthetic weights, 4 sequences of 96 tokens), beside what a plain fp32 forward (bert_ref) costs against the same
+# float64 result: (hidden max, hidden rms, normalised mean-embedding max) for each.  Pinned within a factor of 1.5 either
+# way: the representation costs up to ~1.7x fp32's hidden-state error and ~7x its error on normalised embeddings.
+REP_COST = {
+    ("all-MiniLM-L6-v2", 1.0): ((2.95e-6, 5.89e-7, 1.19e-7), (3.59e-6, 3.14e-7, 6.09e-8)),
+    ("all-MiniLM-L6-v2", 4.0): ((3.31e-6, 9.14e-7, 1.67e-7), (3.66e-6, 6.81e-7, 6.80e-8)),
+    ("bge-base-en-v1.5", 1.0): ((8.80e-6, 1.67e-6, 2.16e-7), (5.10e-6, 6.41e-7, 3.09e-8)),
+}
+
+
+@pytest.mark.parametrize("preset,scale", list(REP_COST))
+def test_split_weight_representation_cost(preset, scale):
+    cfg = BertConfig(**asdict(PRESETS[preset][0]))
+    w = synthetic_bert_weights(cfg, seed=3, scale=scale)
+    rng = np.random.default_rng(5)
+    lens = [96] * 4
+    ids = rng.integers(104, cfg.vocab_size, sum(lens))
+    cu = np.r_[0, np.cumsum(lens)]
+    a = ref.encoder_stack_ref(w, cfg, ids, None, cu, "fp32")
+    b = ref.encoder_stack_ref(w, cfg, ids, None, cu, "split")
+    I = torch.from_numpy(ids.reshape(4, 96))
+    with torch.no_grad():
+        h = bert_ref.bert_encoder_forward(w, bert_ref.BertCfg(**asdict(cfg)), I, torch.ones_like(I))
+        e32 = bert_ref.l2_normalize(h.mean(1)).double()
+    h32 = h.reshape(-1, cfg.hidden).double()
+
+    def costs(h_, e_):
+        d = (h_ - a["hidden"]).abs()
+        return float(d.max()), float(d.pow(2).mean().sqrt()), float((e_ - a["mean_norm"]).abs().max())
+
+    for what, got, want in (("split", costs(b["hidden"], b["mean_norm"]), REP_COST[preset, scale][0]),
+                            ("fp32", costs(h32, e32), REP_COST[preset, scale][1])):
+        for g_, w_, name in zip(got, want, ("hidden max", "hidden rms", "embedding max")):
+            assert w_ / 1.5 <= g_ <= 1.5 * w_, f"{what} {name}: {g_:.3g}, pinned {w_:.3g}"
