@@ -8,6 +8,8 @@
     from langchain_postgres.vectorstores import PGVector                     RAGHelper.py:29
     from langchain_community.cross_encoders import HuggingFaceCrossEncoder   RAGHelper.py:12
     from ScoredCrossEncoderReranker import ScoredCrossEncoderReranker        RAGHelper.py:33
+    from langchain.retrievers.document_compressors import FlashrankRerank   RAGHelper.py:11
+        (also langchain_community.document_compressors[.flashrank_rerank])
     from langchain_community.retrievers import BM25Retriever                 RAGHelper.py:24
     from langchain.retrievers import ContextualCompressionRetriever, EnsembleRetriever   RAGHelper.py:10
     from langchain_experimental.text_splitter import SemanticChunker        RAGHelper.py:27
@@ -20,6 +22,7 @@ LangChain (this build image) the plain classes are registered.
 """
 from __future__ import annotations
 
+import importlib
 import sys
 import types
 from typing import Any, Dict, Optional
@@ -45,13 +48,14 @@ def build_classes() -> Dict[str, Any]:
     """The drop-in classes, re-based on LangChain's ABCs when LangChain is importable."""
     from .cross_encoder import HuggingFaceCrossEncoder
     from .embeddings import HuggingFaceEmbeddings
+    from .flashrank import FlashrankRerank
     from .reranker import ScoredCrossEncoderReranker
     from .retrievers import BM25Retriever, ContextualCompressionRetriever, EnsembleRetriever
     from .vectorstore import Milvus, PGVector
 
     out = dict(HuggingFaceEmbeddings=HuggingFaceEmbeddings, HuggingFaceCrossEncoder=HuggingFaceCrossEncoder,
-               ScoredCrossEncoderReranker=ScoredCrossEncoderReranker, Milvus=Milvus, PGVector=PGVector,
-               BM25Retriever=BM25Retriever, EnsembleRetriever=EnsembleRetriever,
+               ScoredCrossEncoderReranker=ScoredCrossEncoderReranker, FlashrankRerank=FlashrankRerank,
+               Milvus=Milvus, PGVector=PGVector, BM25Retriever=BM25Retriever, EnsembleRetriever=EnsembleRetriever,
                ContextualCompressionRetriever=ContextualCompressionRetriever)
     try:  # pragma: no cover - LangChain is not present in the build image
         from langchain_core.embeddings import Embeddings
@@ -81,6 +85,28 @@ def build_classes() -> Dict[str, Any]:
             scores = self.model.score([(query, d.page_content) for d in documents])
             ranked = sorted(zip(documents, scores), key=lambda ds: ds[1], reverse=True)
             return [copy_document(d, {**d.metadata, "relevance_score": s}) for d, s in ranked[: self.top_n]]
+
+    from . import flashrank as fr
+
+    class LCFlashrankRerank(BaseDocumentCompressor):  # type: ignore[misc]
+        """pydantic form of flashrank.FlashrankRerank (langchain-community 0.2.10's fields) [3P-recall]."""
+        client: Any = None
+        top_n: int = 3
+        score_threshold: float = 0.0
+        model: Optional[str] = None
+        prefix_metadata: str = ""
+        model_config = ConfigDict(arbitrary_types_allowed=True, extra="forbid")
+
+        def __init__(self, **data: Any):
+            super().__init__(**data)            # refuses unknown fields before any model is loaded
+            if self.client is None:
+                self.client = fr.Ranker(model_name=self.model or fr.DEFAULT_MODEL_NAME)
+
+        def compress_documents(self, documents, query, callbacks=None):
+            return fr.compress(self.client, documents, query, self.top_n, self.score_threshold, self.prefix_metadata)
+
+        async def acompress_documents(self, documents, query, callbacks=None):
+            return self.compress_documents(documents, query, callbacks)
 
     from langchain_core.retrievers import BaseRetriever
     from .bm25 import BM25Index
@@ -123,9 +149,10 @@ def build_classes() -> Dict[str, Any]:
     except Exception:
         pass
     LCReranker.__name__ = "ScoredCrossEncoderReranker"
+    LCFlashrankRerank.__name__ = "FlashrankRerank"
     LCEmbeddings.__name__ = "HuggingFaceEmbeddings"
     out.update(HuggingFaceEmbeddings=LCEmbeddings, Milvus=_vs(Milvus), PGVector=_vs(PGVector),
-               ScoredCrossEncoderReranker=LCReranker)
+               ScoredCrossEncoderReranker=LCReranker, FlashrankRerank=LCFlashrankRerank)
     return out
 
 
@@ -161,6 +188,15 @@ def install() -> Dict[str, Any]:
     except Exception:
         _module("langchain.retrievers", EnsembleRetriever=c["EnsembleRetriever"],
                 ContextualCompressionRetriever=c["ContextualCompressionRetriever"])
+    # the default reranker (RAGHelper.py:11,480).  langchain 0.2 resolves FlashrankRerank through a module
+    # __getattr__; an attribute set on the real module takes precedence over it
+    for name in ("langchain.retrievers.document_compressors", "langchain_community.document_compressors",
+                 "langchain_community.document_compressors.flashrank_rerank"):
+        try:
+            mod = importlib.import_module(name)  # pragma: no cover - LangChain is not present in the build image
+            mod.FlashrankRerank = c["FlashrankRerank"]  # type: ignore[attr-defined]  # pragma: no cover
+        except Exception:
+            _module(name, FlashrankRerank=c["FlashrankRerank"])
     # the semantic text splitter (server/RAGHelper.py:27,329-341): device embeddings + adjacent-distance kernel
     from .chunker import SemanticChunker
     c["SemanticChunker"] = SemanticChunker

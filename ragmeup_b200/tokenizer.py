@@ -48,8 +48,11 @@ def synthetic_vocab(size: int = 30522, seed: int = 7) -> Dict[str, int]:
         vocab["##" + ch] = i
         i += 1
     rng = np.random.default_rng(seed)
+    # words of up to 3 syllables give about 56 000 entries; larger vocabularies (the 105 879 of multilingual BERT)
+    # take words of up to 4.  Vocabularies of BERT's usual 30 522 and smaller are unchanged.
+    syllables = 4 if size > 50000 else 3
     while i < size:
-        n = int(rng.integers(1, 4))
+        n = int(rng.integers(1, syllables + 1))
         word = "".join(_SYL[int(j)] for j in rng.integers(0, len(_SYL), n))
         if rng.random() < 0.25:
             word = "##" + word

@@ -65,6 +65,20 @@ PRESETS: Dict[str, Tuple[BertConfig, str, int]] = {
     "GIST-small-Embedding-v0": (BertConfig(hidden=384, layers=12, heads=12, ffn=1536), "cls", 512),
     # tiny shapes for unit tests
     "tiny": (BertConfig(vocab_size=1000, hidden=128, layers=2, heads=4, ffn=256, max_pos=128), "mean", 64),
+    # the BERT rerankers FlashRank ships (FLASHRANK_MODELS)
+    "ms-marco-MultiBERT-L-12": (BertConfig(vocab_size=105879, hidden=768, layers=12, heads=12, ffn=3072, num_labels=2),
+                                "cls", 512),
+    "ms-marco-TinyBERT-L-2-v2": (BertConfig(hidden=128, layers=2, heads=2, ffn=512, num_labels=1), "cls", 512),
+    "ms-marco-MiniLM-L-12-v2": (BertConfig(hidden=384, layers=12, heads=12, ffn=1536, num_labels=1), "cls", 512),
+}
+
+# FlashRank's model names -> the public HuggingFace checkpoints its ONNX files were exported from [3P-recall: flashrank
+# 0.2.x; the mapping is recalled, not read, and is unverified].  Only the BERT cross-encoders are here: FlashRank's T5
+# (rank-T5-flan) and listwise LLM (rank_zephyr_7b_v1_full) models are not BERT encoders.
+FLASHRANK_MODELS: Dict[str, str] = {
+    "ms-marco-MultiBERT-L-12": "amberoad/bert-multilingual-passage-reranking-msmarco",
+    "ms-marco-TinyBERT-L-2-v2": "cross-encoder/ms-marco-TinyBERT-L-2-v2",
+    "ms-marco-MiniLM-L-12-v2": "cross-encoder/ms-marco-MiniLM-L-12-v2",
 }
 
 
@@ -126,15 +140,27 @@ def _read_json(path: str) -> Optional[dict]:
     return None
 
 
+def _load_tensors(path: str) -> Dict[str, np.ndarray]:
+    """``model.safetensors``, or for snapshots that ship only the older format (the multilingual MS MARCO reranker
+    behind FlashRank's default) ``pytorch_model.bin``, read with ``weights_only=True`` so no pickled code runs."""
+    st = os.path.join(path, "model.safetensors")
+    pt = os.path.join(path, "pytorch_model.bin")
+    if not os.path.exists(st) and os.path.exists(pt):
+        import torch
+        sd = torch.load(pt, weights_only=True, map_location="cpu")
+        return {k: v.detach().to(torch.float32).numpy() for k, v in sd.items() if v.is_floating_point()}
+    from safetensors.numpy import load_file
+    return load_file(st)
+
+
 def load_hf_snapshot(path: str, with_head: bool):
     """Read a local HF / sentence-transformers snapshot.  Returns
     (config, weights, pooling, normalize, max_seq_length, activation)."""
-    from safetensors.numpy import load_file
     cfgd = _read_json(os.path.join(path, "config.json"))
     if cfgd is None:
         raise FileNotFoundError(f"{path}: no config.json")
     cfg = BertConfig.from_hf(cfgd)
-    raw = load_file(os.path.join(path, "model.safetensors"))
+    raw = _load_tensors(path)
     w: Dict[str, np.ndarray] = {}
     for k, v in raw.items():
         k2 = k[5:] if k.startswith("bert.") else k
@@ -195,3 +221,41 @@ def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] 
     raise FileNotFoundError(
         f"model {model_name!r} not found locally (no network in this deployment): point "
         f"RAGMEUP_MODEL_DIR at a directory holding its HuggingFace snapshot, or use 'synthetic:<preset>'")
+
+
+def resolve_flashrank(model_name: str, cache_folder: Optional[str] = None, max_length: int = 512):
+    """FlashRank model name -> (cfg, weights with the classifier head, max_length, vocab_source).
+
+    A snapshot is looked up under ``cache_folder`` and ``$RAGMEUP_MODEL_DIR`` by either name: the FlashRank name or
+    the HuggingFace id of FLASHRANK_MODELS (``<root>/<org>/<name>`` or ``<root>/<name>``).  ``synthetic:<preset>``
+    names work as in ``resolve_model``.  ``num_labels`` is the classifier's row count; a config that states another
+    count is refused.  ``max_length`` is FlashRank's truncation [3P-recall]: ``min(model_max_length of
+    tokenizer_config.json, max_length)``, or ``min(max_position_embeddings, max_length)`` without that file or key."""
+    if model_name.startswith("synthetic:"):
+        cfg, w, _pool, _norm, _len, _act, src = resolve_model(model_name, with_head=True)
+        return cfg, w, min(cfg.max_pos, int(max_length)), src
+    if model_name not in FLASHRANK_MODELS:
+        raise ValueError(f"FlashRank model {model_name!r} is not supported here: the BERT cross-encoders "
+                         f"{sorted(FLASHRANK_MODELS)} are (or 'synthetic:<preset>')")
+    hf = FLASHRANK_MODELS[model_name]
+    names = [model_name, hf, hf.split("/")[-1]]
+    roots = [r for r in (cache_folder, os.environ.get("RAGMEUP_MODEL_DIR")) if r]
+    path = next((os.path.join(r, n) for r in roots for n in names if os.path.isdir(os.path.join(r, n))), None)
+    if path is None:
+        raise FileNotFoundError(
+            f"FlashRank model {model_name!r} not found locally (no network in this deployment): put the HuggingFace "
+            f"snapshot of {hf!r} at <dir>/{model_name} or <dir>/{hf}, with <dir> = RAGMEUP_MODEL_DIR or cache_folder "
+            f"(searched: {roots or 'none set'})")
+    cfgd = _read_json(os.path.join(path, "config.json")) or {}
+    cfg, w, *_ = load_hf_snapshot(path, with_head=True)
+    rows = int(w["classifier.weight"].shape[0])
+    stated = len(cfgd["id2label"]) if "id2label" in cfgd else cfgd.get("num_labels")
+    if stated is not None and int(stated) != rows:
+        raise ValueError(f"{path}: the classifier has {rows} rows but config.json states {stated} labels")
+    cfg.num_labels = rows
+    tc = _read_json(os.path.join(path, "tokenizer_config.json")) or {}
+    if tc.get("model_max_length") is not None:
+        max_len = min(int(tc["model_max_length"]), int(max_length))
+    else:
+        max_len = min(cfg.max_pos, int(max_length))
+    return cfg, w, min(max_len, cfg.max_pos), path     # the model has no positions past max_pos
