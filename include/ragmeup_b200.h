@@ -166,18 +166,30 @@ int rmu_bm25_csr_free(rmu_bm25_csr* c);
  * Stands behind HuggingFaceEmbeddings.embed_documents/embed_query (sentence-transformers
  * encode -> BertModel -> Pooling -> Normalize) and HuggingFaceCrossEncoder.score
  * (CrossEncoder.predict -> BertForSequenceClassification). */
+/* position_mode: how a token's row of the position table is chosen */
+#define RMU_POS_ABSOLUTE 0   /* BERT: the token's offset j in its sequence                                          */
+#define RMU_POS_OFFSET 1     /* MPNet / RoBERTa (padding index 1): a token of id 1 takes row 1, any other token row
+                              * 2 + j - (tokens of id 1 before it); sequences may hold max_pos - 2 tokens             */
+
+/* The two trailing fields are zero for BERT.  MPNet sets position_mode = RMU_POS_OFFSET and rel_buckets = 32: every
+ * attention score gets bias[bucket(key - query), head] of a [32, heads] table shared by all layers (transformers'
+ * MPNet relative_position_bucket, 32 buckets, max distance 128). */
 typedef struct rmu_bert_config {
     int32_t vocab_size, hidden, layers, heads, ffn, max_pos, type_vocab, num_labels;
     float ln_eps;
+    int32_t position_mode, rel_buckets;
 } rmu_bert_config;
 
 typedef struct rmu_encoder rmu_encoder;
 
 /* weights_h: host fp32 arrays in the canonical order documented in ragmeup_b200/encoder.py
- * (HuggingFace BertModel tensor order; pooler + classifier last when has_head).  The GEMM weights (query, key, value,
+ * (HuggingFace BertModel tensor order; pooler + classifier when has_head; then, when rel_buckets = 32, the relative
+ * attention bias [32, heads] last).  The GEMM weights (query, key, value,
  * attention output, intermediate, output) are held as split fp16 planes, which cannot hold |w| >= 65520: such an
  * element (infinities included) returns RMU_ERR_UNSUPPORTED before any CUDA call.  Embedding tables, biases, LayerNorm
- * parameters and the pooler / classifier stay fp32 and are not limited. */
+ * parameters and the pooler / classifier stay fp32 and are not limited.  A position_mode other than 0 or 1 or a
+ * rel_buckets other than 0 or 32 returns RMU_ERR_UNSUPPORTED, and a weight count that does not match (the bias table
+ * included) or a null bias table RMU_ERR_ARG, before any CUDA call. */
 int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* weights_h, int n_weights, int has_head,
                        rmu_encoder** out);
 void rmu_encoder_destroy(rmu_encoder* enc);
@@ -187,7 +199,8 @@ void rmu_encoder_destroy(rmu_encoder* enc);
 
 /* ragged batch: ids/type_ids [total_tokens] int32, cu_seqlens [B+1] int32 (all device); type_ids may be null (all 0).
  * max_seqlen must be at least the longest sequence in cu_seqlens; only max_seqlen itself is checked against
- * max_position_embeddings (cu_seqlens is on the device).  Out-of-range inputs are clamped on the device, where
+ * max_position_embeddings (max_seqlen + 2 <= max_pos with RMU_POS_OFFSET; cu_seqlens is on the device).  Out-of-range
+ * inputs are clamped on the device, where
  * HuggingFace raises an IndexError: token ids into [0, vocab_size), type ids into [0, type_vocab), and positions past
  * max_position_embeddings - 1 take that last row.  An empty sequence (cu_seqlens[b + 1] == cu_seqlens[b]) is allowed,
  * but a batch must hold at least one token: B < 1 or total_tokens < 1 (a batch of empty sequences only) returns
@@ -245,6 +258,22 @@ int rmu_debug_layernorm(const float* pre, int T, int H, const float* gamma, cons
 int rmu_debug_embed_ln(const int32_t* ids, const int32_t* type_ids, const int32_t* cu_seqlens, int B, int T, int H,
                        int vocab, int max_pos, int type_vocab, const float* word, const float* pos, const float* typ,
                        const float* gamma, const float* beta, float eps, uint16_t* out_hi, uint16_t* out_lo, void* stream);
+/* For tests: the same with the position rule pos_mode (RMU_POS_ABSOLUTE is rmu_debug_embed_ln; RMU_POS_OFFSET compares
+ * the raw ids with 1, then clamps positions to max_pos - 1).  Another pos_mode returns RMU_ERR_ARG. */
+int rmu_debug_embed_ln_pos(const int32_t* ids, const int32_t* type_ids, const int32_t* cu_seqlens, int B, int T, int H,
+                           int vocab, int max_pos, int type_vocab, const float* word, const float* pos, const float* typ,
+                           const float* gamma, const float* beta, float eps, int pos_mode, uint16_t* out_hi,
+                           uint16_t* out_lo, void* stream);
+/* Host only, no GPU work: the attention bias table rmu_encoder_create builds from bias_h [buckets, heads] fp32 ->
+ * table_h [heads, 255] fp32, entry (h, r + 127) = bias_h[bucket(r), h] * log2(e) for r = key - query in [-127, 127]
+ * (every |r| >= 127 falls in the last bucket of its side).  buckets other than 32 return RMU_ERR_UNSUPPORTED. */
+int rmu_relative_bias_table(const float* bias_h, int buckets, int heads, float* table_h);
+/* For tests: E2 with the relative bias, rel_table [heads, 255] fp32 on the device (rmu_relative_bias_table's layout),
+ * 10 warps.  cls_q_hi / cls_q_lo null: every query row, ctx [T, H]; non-null: the compact Q planes [B, H] of query row 0
+ * of each sequence (the last layer's CLS-only mode), ctx [B, H]. */
+int rmu_debug_attention_bias(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const uint16_t* cls_q_hi,
+                             const uint16_t* cls_q_lo, const int32_t* cu_seqlens, int B, int H, int heads, int max_seqlen,
+                             const float* rel_table, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream);
 /* For tests: E4 pool_kernel, RMU_POOL_MEAN or RMU_POOL_CLS of planes [T, H] per sequence of cu_seqlens [B+1], then
  * x / max(||x||, 1e-12) when normalize -> out [B, H] fp32 (an empty sequence gives zeros).  1 <= H <= 1024. */
 int rmu_debug_pool(const uint16_t* hi, const uint16_t* lo, const int32_t* cu_seqlens, int B, int H, int pool_mode,

@@ -23,7 +23,7 @@ class RmuError(RuntimeError):
 class BertConfigC(C.Structure):
     _fields_ = [("vocab_size", C.c_int32), ("hidden", C.c_int32), ("layers", C.c_int32), ("heads", C.c_int32),
                 ("ffn", C.c_int32), ("max_pos", C.c_int32), ("type_vocab", C.c_int32), ("num_labels", C.c_int32),
-                ("ln_eps", C.c_float)]
+                ("ln_eps", C.c_float), ("position_mode", C.c_int32), ("rel_buckets", C.c_int32)]
 
 
 # name -> (restype, argtypes); mirrors include/ragmeup_b200.h
@@ -95,6 +95,12 @@ SIGNATURES = {
     "rmu_debug_embed_ln": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float,
                                      C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_embed_ln_pos": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                         C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float,
+                                         C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_relative_bias_table": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "rmu_debug_attention_bias": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                           C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_pool": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                  C.c_void_p]),
     "rmu_debug_cls_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

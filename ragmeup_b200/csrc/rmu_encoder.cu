@@ -75,6 +75,11 @@ __device__ __forceinline__ void warp_layernorm_store(float (&v)[kMaxPerLane], in
 }
 
 // word + position + token-type embedding sum -> LayerNorm -> split planes.  One warp per token.
+// POS = RMU_POS_OFFSET (MPNet, RoBERTa): HF's create_position_ids_from_input_ids with padding_idx 1, i.e. a token of
+// id 1 takes position 1 and any other token at offset j takes 2 + j - (tokens of id 1 before it).  The warp counts those
+// with one ballot per 32 tokens of the prefix.  POS = RMU_POS_ABSOLUTE (BERT) is position j.
+constexpr int kPadId = 1;
+template <int POS>
 __global__ void embed_ln_kernel(const int* __restrict__ ids, const int* __restrict__ type_ids,
                                 const int* __restrict__ cu, int B, int T, int H, int vocab, int max_pos, int type_vocab,
                                 const float* __restrict__ word, const float* __restrict__ pos,
@@ -89,6 +94,15 @@ __global__ void embed_ln_kernel(const int* __restrict__ ids, const int* __restri
         if (cu[mid] <= t) lo_b = mid; else hi_b = mid;
     }
     int p = t - cu[lo_b];
+    if constexpr (POS == RMU_POS_OFFSET) {
+        const int* seq = ids + cu[lo_b];
+        int pads = 0;
+        for (int k0 = 0; k0 < p; k0 += 32) {
+            const int k = k0 + static_cast<int>(lane_id());
+            pads += __popc(__ballot_sync(0xffffffffu, k < p && seq[k] == kPadId));
+        }
+        p = ids[t] == kPadId ? kPadId : p + kPadId + 1 - pads;
+    }
     p = p < max_pos ? p : max_pos - 1;
     int id = ids[t];
     id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
@@ -184,12 +198,21 @@ __device__ __forceinline__ float fast_exp2(float x) {   // ex2.approx: 2 ulp, ex
 // from row b of the compact planes cls_q [B, H], the context goes to row b of ctx [B, H] (zeros for an empty sequence),
 // grid z = 1.  Warp 0 runs the same code as warp 0 of the full kernel with query rows 1..15 zero; the MMA rows and the
 // softmax rows are independent, so row 0 comes out bit-identical.  The other NW - 1 warps only help stage K / V.
-template <int DH, int MINB, int NW = kAttWarps, bool CLS = false>      // NW warps = 16 * NW query rows per CTA
+//
+// RelBias = const float* (MPNet): the kernel takes one more parameter, rel_bias, and score(i, j) +=
+// rel_bias[h][clamp(j - i, -127, 127) + 127], a [heads, kRelSpan] fp32 table already multiplied by log2(e)
+// (build_relative_bias_table), with i and j the query and key rows within the sequence.  The CTA's head row of the
+// table sits in shared memory behind the V planes.  With the pack empty (BERT) the parameter list and the code are
+// those of the kernel without the bias: one more kernel parameter alone changes ptxas's register allocation.
+constexpr int kRelMax = 127;                  // |j - i| >= 127 all fall in MPNet's last bucket (distance >= 91)
+constexpr int kRelSpan = 2 * kRelMax + 1;
+template <int DH, int MINB, int NW = kAttWarps, bool CLS = false, typename... RelBias>  // NW warps = 16 * NW query rows per CTA
 __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const __half* __restrict__ ph, const __half* __restrict__ pl,
                                                                           const __half* __restrict__ cls_q_hi,
                                                                           const __half* __restrict__ cls_q_lo,
                                                                           const int* __restrict__ cu, int H, int ksb,
-                                                                          __half* __restrict__ ctx_hi, __half* __restrict__ ctx_lo) {
+                                                                          __half* __restrict__ ctx_hi, __half* __restrict__ ctx_lo,
+                                                                          RelBias... rel_bias) {
     constexpr int KSTR = DH + 8;
     constexpr int KS = DH / 16;
     constexpr int NT = DH / 8;
@@ -221,6 +244,11 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
     const __half* ql_base = CLS ? cls_q_lo + static_cast<size_t>(b) * H + h * DH : pl + static_cast<size_t>(t0) * ld + h * DH;
     const int r0 = rbase + warp * 16;
     const bool warp_live = r0 < qrows;
+    if constexpr (sizeof...(RelBias) == 1) {   // this head's biases, visible after the first __syncthreads of the key loop
+        const float* tab = (rel_bias, ...);
+        float* relb = reinterpret_cast<float*>(Vl + ksb * KSTR);
+        for (int e = threadIdx.x; e < kRelSpan; e += blockDim.x) relb[e] = tab[h * kRelSpan + e];
+    }
 
     uint32_t qh[KS][4], ql[KS][4];
     {
@@ -295,6 +323,21 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
                 for (int n = 0; n < 4; ++n) if (n < 2 || full_blk) mma16816(sacc[n], ql[ks], bh[n]);
 #pragma unroll
                 for (int n = 0; n < 4; ++n) if (n < 2 || full_blk) mma16816(sacc[n], qh[ks], bl[n]);
+            }
+            if constexpr (sizeof...(RelBias) == 1) {
+                // fragment (n, c): key sb0 + kb0 + n * 8 + 2t + (c & 1), query row r0 + g (c < 2) or r0 + g + 8; keys past
+                // the sequence end read a clamped entry and are masked below
+                const float* relb = reinterpret_cast<const float*>(Vl + ksb * KSTR);
+                const int ja = sb0 + kb0 + 2 * t - (CLS ? 0 : r0 + g);
+                const int jb = CLS ? ja : ja - 8;
+#pragma unroll
+                for (int n = 0; n < 4; ++n) {
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        sacc[n][c] += relb[min(max(ja + n * 8 + c, -kRelMax), kRelMax) + kRelMax];
+                        sacc[n][2 + c] += relb[min(max(jb + n * 8 + c, -kRelMax), kRelMax) + kRelMax];
+                    }
+                }
             }
             float bm0 = -INFINITY, bm1 = -INFINITY;
             if (kb0 + 32 > nk) {                     // only the last key block holds keys past the sequence end
@@ -496,31 +539,47 @@ constexpr int kClsAttWarps = 4;
 // The sequence index is gridDim.y, at most 65 535: a larger batch runs in slices of 65 535 sequences, each launch with
 // cu (and in CLS mode the compact Q and context rows) offset by the slice start.  Within a slice the grid and the
 // kernel are those of one launch, so the heads of a sequence still run together and every row is computed the same.
+// rel_bias non-null: the [heads, kRelSpan] table of build_relative_bias_table is added to every score (warps must be 10).
 constexpr int kMaxGridY = 65535;
 static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __half* cls_q_hi, const __half* cls_q_lo,
                             const int* cu, int B, int H, int heads, int max_seqlen, int warps, __half* ctx_hi,
-                            __half* ctx_lo, cudaStream_t st) {
+                            __half* ctx_lo, cudaStream_t st, const float* rel_bias = nullptr) {
     const int DH = H / heads;
     const bool cls = cls_q_hi != nullptr;
+    const bool bias = rel_bias != nullptr;
     if (cls) warps = kClsAttWarps;
-    else if (!(warps == kAttWarps || (warps == 5 && DH == 32))) { set_error("attention: warps must be 10, or 5 with head_dim 32"); return RMU_ERR_ARG; }
+    else if (!(warps == kAttWarps || (warps == 5 && DH == 32 && !bias))) {
+        set_error("attention: warps must be 10, or 5 with head_dim 32 and no relative bias");
+        return RMU_ERR_ARG;
+    }
     ProfScope _ps(PROF_ATTN, st);
     const unsigned zblocks = cls ? 1u : static_cast<unsigned>((max_seqlen + warps * 16 - 1) / (warps * 16));
     // keys resident per CTA: the whole (longest) sequence when it fits, else super-blocks of kKeySB
     const int ksb = std::min(kKeySB, (max_seqlen + 31) / 32 * 32);
-    const size_t smem_max = 4 * sizeof(__half) * static_cast<size_t>(kKeySB) * (DH + 8);
-    const size_t smem = 4 * sizeof(__half) * static_cast<size_t>(ksb) * (DH + 8);
+    const size_t tab = bias ? kRelSpan * sizeof(float) : 0;
+    const size_t smem_max = 4 * sizeof(__half) * static_cast<size_t>(kKeySB) * (DH + 8) + tab;
+    const size_t smem = 4 * sizeof(__half) * static_cast<size_t>(ksb) * (DH + 8) + tab;
     auto kern = cls ? (DH == 32 ? attention_planes_kernel<32, 4, kClsAttWarps, true> : attention_planes_kernel<64, 2, kClsAttWarps, true>)
               : DH == 32 ? (warps == 5 ? attention_planes_kernel<32, 4, 5> : attention_planes_kernel<32, 2>)
                          : attention_planes_kernel<64, 1>;   // d_h = 64 needs > 96 registers
-    RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
+    using Tab = const float*;
+    auto bkern = cls ? (DH == 32 ? attention_planes_kernel<32, 4, kClsAttWarps, true, Tab>
+                                 : attention_planes_kernel<64, 2, kClsAttWarps, true, Tab>)
+                     : (DH == 32 ? attention_planes_kernel<32, 2, kAttWarps, false, Tab>
+                                 : attention_planes_kernel<64, 1, kAttWarps, false, Tab>);
+    if (bias) RMU_CUDA(cudaFuncSetAttribute(bkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
+    else RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
     for (int s0 = 0; s0 < B; s0 += kMaxGridY) {
         const int nb = std::min(kMaxGridY, B - s0);
         // full mode addresses Q and the context by token (cu[b] is absolute), CLS mode by sequence
         const size_t roff = cls ? static_cast<size_t>(s0) * H : 0;
         dim3 pg(static_cast<unsigned>(heads), static_cast<unsigned>(nb), zblocks);
-        kern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, cls ? cls_q_hi + roff : nullptr, cls ? cls_q_lo + roff : nullptr,
-                                           cu + s0, H, ksb, ctx_hi + roff, ctx_lo + roff);
+        if (bias)
+            bkern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, cls ? cls_q_hi + roff : nullptr, cls ? cls_q_lo + roff : nullptr,
+                                                cu + s0, H, ksb, ctx_hi + roff, ctx_lo + roff, rel_bias);
+        else
+            kern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, cls ? cls_q_hi + roff : nullptr, cls ? cls_q_lo + roff : nullptr,
+                                               cu + s0, H, ksb, ctx_hi + roff, ctx_lo + roff);
         count_launch();
         RMU_CHECK_LAUNCH();
     }
@@ -539,14 +598,15 @@ static int launch_layernorm(const float* pre, int T, int H, const float* g, cons
 }
 
 // E3 embed_ln_kernel: word + token-type + position rows of T tokens of a ragged batch -> LayerNorm -> planes [T, H].
-// 8 warps (tokens) per block.
+// 8 warps (tokens) per block.  pos_mode: RMU_POS_ABSOLUTE or RMU_POS_OFFSET.
 static int launch_embed_ln(const int* ids, const int* type_ids, const int* cu, int B, int T, int H, int vocab, int max_pos,
                            int type_vocab, const float* word, const float* pos, const float* typ, const float* g,
-                           const float* b, float eps, __half* hi, __half* lo, cudaStream_t st) {
+                           const float* b, float eps, __half* hi, __half* lo, cudaStream_t st, int pos_mode = RMU_POS_ABSOLUTE) {
     constexpr int wpb = 8;
     ProfScope _ps(PROF_EMBED, st);
-    embed_ln_kernel<<<static_cast<unsigned>((T + wpb - 1) / wpb), wpb * 32, 0, st>>>(ids, type_ids, cu, B, T, H, vocab, max_pos,
-                                                                                     type_vocab, word, pos, typ, g, b, eps, hi, lo);
+    auto kern = pos_mode == RMU_POS_OFFSET ? embed_ln_kernel<RMU_POS_OFFSET> : embed_ln_kernel<RMU_POS_ABSOLUTE>;
+    kern<<<static_cast<unsigned>((T + wpb - 1) / wpb), wpb * 32, 0, st>>>(ids, type_ids, cu, B, T, H, vocab, max_pos,
+                                                                          type_vocab, word, pos, typ, g, b, eps, hi, lo);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
@@ -600,6 +660,26 @@ static int launch_join_planes(const __half* hi, const __half* lo, size_t n, floa
     return RMU_OK;
 }
 
+// MPNet's relative_position_bucket (transformers MPNetEncoder, num_buckets 32, max_distance 128) of rel = key - query:
+// keys after the query take buckets 16..31, keys before it 0..15; distances below 8 are exact, larger ones log-spaced
+// (the float32 log and the truncation of torch's version) and saturate at bucket 15 from distance 91 on.
+static int relative_bucket(int rel) {
+    constexpr int kHalf = 16, kExact = 8;
+    const int n = rel < 0 ? -rel : rel;
+    const int base = rel > 0 ? kHalf : 0;
+    if (n < kExact) return base + n;
+    const int large = kExact + static_cast<int>(logf(static_cast<float>(n) / kExact) / logf(16.0f) * (kHalf - kExact));
+    return base + std::min(large, kHalf - 1);
+}
+
+// bias [32, heads] (the checkpoint's relative_attention_bias.weight) -> out [heads, kRelSpan]: entry (h, r + kRelMax) is
+// bias[bucket(r), h] * log2(e) for r = key - query in [-kRelMax, kRelMax], in the log2 units of the attention scores
+static void build_relative_bias_table(const float* bias, int heads, float* out) {
+    for (int h = 0; h < heads; ++h)
+        for (int r = -kRelMax; r <= kRelMax; ++r)
+            out[static_cast<size_t>(h) * kRelSpan + r + kRelMax] = bias[relative_bucket(r) * heads + h] * 1.4426950408889634f;
+}
+
 }  // namespace rmu
 
 using namespace rmu;
@@ -615,6 +695,7 @@ struct rmu_encoder {
     int has_head = 0, sms = 0, device = 0;
     std::vector<void*> allocs;
     float *word = nullptr, *pos = nullptr, *typ = nullptr, *eg = nullptr, *eb = nullptr;
+    float* rel = nullptr;                 // rel_buckets = 32: [heads, kRelSpan] attention bias table, else null
     std::vector<EncLayer> layers;
     SplitOperand last_wq, last_wkv;       // views of the last layer's Wqkv: rows 0..H (q) and H..3H (k | v)
     float *pw = nullptr, *pb = nullptr, *cw = nullptr, *cb = nullptr;
@@ -735,7 +816,7 @@ static int run_last_layer_cls(rmu_encoder* e, const EncLayer& L, const int32_t* 
     rc = launch_gemm(GEMM_BIAS_SPLIT_QSCALE, e->X_cls, e->last_wq, g, e->sms, st);
     if (rc != RMU_OK) return rc;
     rc = launch_attention(e->QKVP.hi, e->QKVP.lo, e->Q_cls.hi, e->Q_cls.lo, cu, B, H, c.heads, max_seqlen, 0, e->CTX_cls.hi,
-                          e->CTX_cls.lo, st);
+                          e->CTX_cls.lo, st, e->rel);
     if (rc != RMU_OK) return rc;
     g = GemmParams{};
     g.M = B; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE_cls; g.res_hi = e->X_cls.hi; g.res_lo = e->X_cls.lo;
@@ -760,12 +841,18 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
                        int max_seqlen, bool cls_only, cudaStream_t st) {
     const rmu_bert_config& c = e->cfg;
     const int H = c.hidden, F = c.ffn, DH = H / c.heads;
-    if (max_seqlen > c.max_pos) { set_error("sequence longer than max_position_embeddings"); return RMU_ERR_ARG; }
+    // the last position a sequence can reach is its length - 1 plus the offset (2 with padding-offset positions)
+    const int pos_offset = c.position_mode == RMU_POS_OFFSET ? kPadId + 1 : 0;
+    if (max_seqlen + pos_offset > c.max_pos) {
+        set_error(pos_offset ? "sequence longer than max_position_embeddings - 2 (positions start after the padding index)"
+                             : "sequence longer than max_position_embeddings");
+        return RMU_ERR_ARG;
+    }
     int rc = ensure_tokens(e, T, B);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace is shared by all callers
     rc = launch_embed_ln(ids, type_ids, cu, B, T, H, c.vocab_size, c.max_pos, c.type_vocab, e->word, e->pos, e->typ, e->eg,
-                         e->eb, c.ln_eps, e->X.hi, e->X.lo, st);
+                         e->eb, c.ln_eps, e->X.hi, e->X.lo, st, c.position_mode);
     if (rc != RMU_OK) return rc;
     const float scale = 1.0f / sqrtf(static_cast<float>(DH));
     // q (scaled by 1/sqrt(dh)), k, v leave the GEMM as split fp16 planes: attention does no conversions
@@ -783,7 +870,7 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
         // RMU_ATTN_WARPS = 5: 80-row CTAs, four per SM (same warps/SM, K/V staged twice per 147-token sequence)
         static const int nw_env = [] { const char* e = getenv("RMU_ATTN_WARPS"); return e ? atoi(e) : kAttWarps; }();
         rc = launch_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, H, c.heads, max_seqlen,
-                              (nw_env == 5 && DH == 32) ? 5 : kAttWarps, e->CTX.hi, e->CTX.lo, st);
+                              (nw_env == 5 && DH == 32 && !e->rel) ? 5 : kAttWarps, e->CTX.hi, e->CTX.lo, st, e->rel);
         if (rc != RMU_OK) return rc;
         g = GemmParams{};
         g.M = T; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE; g.res_hi = e->X.hi; g.res_lo = e->X.lo;
@@ -815,8 +902,18 @@ extern "C" {
 int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* w, int n_weights, int has_head, rmu_encoder** out) {
     if (!cfg || !w || !out) { set_error("rmu_encoder_create: bad argument"); return RMU_ERR_ARG; }
     const int H = cfg->hidden, F = cfg->ffn, L = cfg->layers;
-    const int expect = 5 + 16 * L + (has_head ? 4 : 0);
+    if (cfg->position_mode != RMU_POS_ABSOLUTE && cfg->position_mode != RMU_POS_OFFSET) {
+        set_error("rmu_encoder_create: position_mode must be RMU_POS_ABSOLUTE (0) or RMU_POS_OFFSET (1)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (cfg->rel_buckets != 0 && cfg->rel_buckets != 32) {
+        set_error("rmu_encoder_create: rel_buckets must be 0 (no relative position bias) or 32 (MPNet)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    const bool rel = cfg->rel_buckets == 32;
+    const int expect = 5 + 16 * L + (has_head ? 4 : 0) + (rel ? 1 : 0);
     if (n_weights != expect) { set_error("rmu_encoder_create: expected " + std::to_string(expect) + " weight tensors"); return RMU_ERR_ARG; }
+    if (rel && !w[expect - 1]) { set_error("rmu_encoder_create: null relative attention bias"); return RMU_ERR_ARG; }
     if (H % 128 != 0 || F % 128 != 0 || H > 1024 || cfg->heads <= 0 || H % cfg->heads != 0 ||
         (H / cfg->heads != 32 && H / cfg->heads != 64)) {
         set_error("rmu_encoder_create: unsupported shape (hidden/ffn multiples of 128, hidden <= 1024, head_dim 32 or 64)");
@@ -894,6 +991,11 @@ int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* w, int n_
         up(&e->pb, H);
         up(&e->cw, static_cast<size_t>(cfg->num_labels) * H);
         up(&e->cb, cfg->num_labels);
+    }
+    if (rel && rc == RMU_OK) {
+        std::vector<float> tab(static_cast<size_t>(cfg->heads) * kRelSpan);
+        build_relative_bias_table(w[i], cfg->heads, tab.data());
+        rc = upload(e, &e->rel, tab.data(), tab.size());
     }
     if (rc != RMU_OK) { rmu_encoder_destroy(e); return rc; }
     *out = e;
@@ -1053,6 +1155,53 @@ int rmu_debug_embed_ln(const int32_t* ids, const int32_t* type_ids, const int32_
     }
     return launch_embed_ln(ids, type_ids, cu, B, T, H, vocab, max_pos, type_vocab, word, pos, typ, gamma, beta, eps,
                            reinterpret_cast<__half*>(out_hi), reinterpret_cast<__half*>(out_lo), static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_embed_ln_pos(const int32_t* ids, const int32_t* type_ids, const int32_t* cu, int B, int T, int H, int vocab,
+                           int max_pos, int type_vocab, const float* word, const float* pos, const float* typ,
+                           const float* gamma, const float* beta, float eps, int pos_mode, uint16_t* out_hi,
+                           uint16_t* out_lo, void* stream) {
+    if (pos_mode != RMU_POS_ABSOLUTE && pos_mode != RMU_POS_OFFSET) {
+        set_error("rmu_debug_embed_ln_pos: pos_mode must be RMU_POS_ABSOLUTE or RMU_POS_OFFSET");
+        return RMU_ERR_ARG;
+    }
+    if (!ids || !cu || !word || !pos || !typ || !gamma || !beta || !out_hi || !out_lo || B <= 0 || T <= 0 || H <= 0 ||
+        vocab <= 0 || max_pos <= 0 || type_vocab <= 0) {
+        set_error("rmu_debug_embed_ln_pos: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H % 128 != 0 || H > 32 * kMaxPerLane) {
+        set_error("rmu_debug_embed_ln_pos: hidden must be a multiple of 128, at most 1024");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_embed_ln(ids, type_ids, cu, B, T, H, vocab, max_pos, type_vocab, word, pos, typ, gamma, beta, eps,
+                           reinterpret_cast<__half*>(out_hi), reinterpret_cast<__half*>(out_lo), static_cast<cudaStream_t>(stream),
+                           pos_mode);
+}
+
+int rmu_relative_bias_table(const float* bias_h, int buckets, int heads, float* table_h) {
+    if (!bias_h || !table_h || heads <= 0) { set_error("rmu_relative_bias_table: bad argument"); return RMU_ERR_ARG; }
+    if (buckets != 32) { set_error("rmu_relative_bias_table: buckets must be 32"); return RMU_ERR_UNSUPPORTED; }
+    build_relative_bias_table(bias_h, heads, table_h);
+    return RMU_OK;
+}
+
+int rmu_debug_attention_bias(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const uint16_t* cls_q_hi, const uint16_t* cls_q_lo,
+                             const int32_t* cu, int B, int H, int heads, int max_seqlen, const float* rel_table,
+                             uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream) {
+    if (!qkv_hi || !qkv_lo || !cu || !rel_table || !ctx_hi || !ctx_lo || (!cls_q_hi) != (!cls_q_lo) || B <= 0 ||
+        heads <= 0 || H <= 0 || max_seqlen <= 0) {
+        set_error("rmu_debug_attention_bias: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H % heads != 0 || (H / heads != 32 && H / heads != 64)) {
+        set_error("rmu_debug_attention_bias: head_dim must be 32 or 64");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_attention(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo),
+                            reinterpret_cast<const __half*>(cls_q_hi), reinterpret_cast<const __half*>(cls_q_lo), cu, B, H,
+                            heads, max_seqlen, kAttWarps, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
+                            static_cast<cudaStream_t>(stream), rel_table);
 }
 
 int rmu_debug_pool(const uint16_t* hi, const uint16_t* lo, const int32_t* cu, int B, int H, int pool_mode, int normalize,

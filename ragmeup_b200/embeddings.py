@@ -56,7 +56,7 @@ class HuggingFaceEmbeddings:
         # sentence-transformers applies the model's own Normalize module; encode_kwargs can force it
         self.normalize = bool(normalize or self.encode_kwargs.get("normalize_embeddings", False))
         self.max_seq_length = int(max_len)
-        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size)
+        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, mpnet=cfg.position_mode == 1)
         self._ragged = RaggedTokenizer(self.tokenizer, self.max_seq_length)
         self.client = BertEncoder(cfg, w, with_head=False, device=device)
 

@@ -2,7 +2,8 @@
 
 Weights go to the library in the canonical order of ``weights.weight_names`` (HuggingFace
 ``BertModel`` tensor order: embeddings, then per layer q/k/v/attention-output/LayerNorm/
-intermediate/output/LayerNorm, then pooler + classifier when a head is present).
+intermediate/output/LayerNorm, then pooler + classifier when a head is present, then MPNet's
+relative attention bias [32, heads] when the config has one).
 """
 from __future__ import annotations
 
@@ -34,7 +35,7 @@ class BertEncoder:
             arrs.append(a)
         ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
         cc = _lib.BertConfigC(cfg.vocab_size, cfg.hidden, cfg.layers, cfg.heads, cfg.ffn, cfg.max_pos, cfg.type_vocab,
-                              cfg.num_labels, cfg.ln_eps)
+                              cfg.num_labels, cfg.ln_eps, cfg.position_mode, cfg.rel_buckets)
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().rmu_encoder_create(C.byref(cc), ptrs, len(arrs), int(self.with_head), C.byref(self._h)),

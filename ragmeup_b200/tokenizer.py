@@ -74,10 +74,35 @@ def build_wordpiece(vocab: Dict[str, int], lowercase: bool = True) -> Tokenizer:
     return tok
 
 
-def load_tokenizer(source: Optional[str], vocab_size: int = 30522) -> Tokenizer:
-    """``source`` = snapshot dir (tokenizer.json or vocab.txt) or None -> synthetic vocab."""
+MPNET_SPECIALS = ("<s>", "<pad>", "</s>", "<unk>")    # ids 0..3; "<mask>" is the last id
+
+
+def synthetic_mpnet_vocab(size: int = 30527) -> Dict[str, int]:
+    """MPNet's id layout: <s>=0, <pad>=1, </s>=2, <unk>=3, then the BERT vocabulary of ``synthetic_vocab(size - 5)``
+    shifted by 4 ([UNK] at 104), then <mask>."""
+    vocab = {t: i for i, t in enumerate(MPNET_SPECIALS)}
+    for t, i in synthetic_vocab(size - 5).items():
+        vocab[t] = i + 4
+    vocab["<mask>"] = size - 1
+    return vocab
+
+
+def build_mpnet_wordpiece(vocab: Dict[str, int]) -> Tokenizer:
+    """MPNet's tokenizer: BERT normalisation and WordPiece, RoBERTa's templates ``<s> A </s>`` and
+    ``<s> A </s> </s> B </s>`` (type ids 0), and the specials as added tokens, so a literal "<pad>" in a text is id 1."""
+    tok = build_wordpiece(vocab)
+    tok.post_processor = processors.RobertaProcessing(sep=("</s>", vocab["</s>"]), cls=("<s>", vocab["<s>"]),
+                                                      trim_offsets=False, add_prefix_space=False)
+    tok.add_special_tokens([*MPNET_SPECIALS, "<mask>"])
+    return tok
+
+
+def load_tokenizer(source: Optional[str], vocab_size: int = 30522, mpnet: bool = False) -> Tokenizer:
+    """``source`` = snapshot dir (tokenizer.json or vocab.txt) or None -> synthetic vocab; ``mpnet`` selects MPNet's
+    vocabulary layout and templates where the snapshot has no tokenizer.json."""
+    build = build_mpnet_wordpiece if mpnet else build_wordpiece
     if source is None:
-        return build_wordpiece(synthetic_vocab(vocab_size))
+        return build(synthetic_mpnet_vocab(vocab_size) if mpnet else synthetic_vocab(vocab_size))
     tj = os.path.join(source, "tokenizer.json")
     if os.path.exists(tj):
         return Tokenizer.from_file(tj)
@@ -85,7 +110,7 @@ def load_tokenizer(source: Optional[str], vocab_size: int = 30522) -> Tokenizer:
     if os.path.exists(vt):
         with open(vt, encoding="utf-8") as f:
             vocab = {line.rstrip("\n"): i for i, line in enumerate(f)}
-        return build_wordpiece(vocab)
+        return build(vocab)
     raise FileNotFoundError(f"{source}: neither tokenizer.json nor vocab.txt")
 
 

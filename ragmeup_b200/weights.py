@@ -21,7 +21,7 @@ from __future__ import annotations
 import json
 import os
 from dataclasses import dataclass, asdict
-from typing import Dict, Optional, Tuple
+from typing import ClassVar, Dict, Optional, Tuple
 
 import numpy as np
 
@@ -37,10 +37,18 @@ class BertConfig:
     type_vocab: int = 2
     ln_eps: float = 1e-12
     num_labels: int = 1
+    # BERT: positions 0..S-1, no relative bias (class constants, so asdict() of a BERT config keeps its nine fields)
+    position_mode: ClassVar[int] = 0
+    rel_buckets: ClassVar[int] = 0
 
     @property
     def head_dim(self) -> int:
         return self.hidden // self.heads
+
+    @property
+    def position_offset(self) -> int:
+        """first position row a token can take: a sequence may hold max_pos - position_offset tokens"""
+        return 2 if self.position_mode == 1 else 0
 
     @staticmethod
     def from_hf(d: dict) -> "BertConfig":
@@ -54,6 +62,31 @@ class BertConfig:
             max_pos=d["max_position_embeddings"], type_vocab=d.get("type_vocab_size", 2),
             ln_eps=d.get("layer_norm_eps", 1e-12),
             num_labels=len(d["id2label"]) if "id2label" in d else d.get("num_labels", 1))
+
+
+@dataclass
+class MPNetConfig(BertConfig):
+    """MPNet (transformers ``MPNetModel``): BERT's post-LN encoder with RoBERTa-style positions (padding index 1:
+    positions start at 2, a token of id 1 takes position 1) and a relative position bias [32, heads] shared by every
+    layer.  It has no token-type table; the encoder gets a zero [1, H] one, and (w + 0) + p == w + p exactly."""
+    vocab_size: int = 30527
+    max_pos: int = 514
+    type_vocab: int = 1
+    ln_eps: float = 1e-5
+    position_mode: int = 1
+    rel_buckets: int = 32
+
+    @staticmethod
+    def from_hf(d: dict) -> "MPNetConfig":
+        if d.get("hidden_act", "gelu") != "gelu":
+            raise ValueError(f"only erf-GELU MPNet encoders are supported, got {d.get('hidden_act')}")
+        nb = int(d.get("relative_attention_num_buckets", 32))
+        if nb < 32:
+            raise ValueError(f"MPNet with relative_attention_num_buckets = {nb} is not supported: transformers' MPNet "
+                             f"always looks up 32 buckets")
+        return MPNetConfig(vocab_size=d["vocab_size"], hidden=d["hidden_size"], layers=d["num_hidden_layers"],
+                           heads=d["num_attention_heads"], ffn=d["intermediate_size"],
+                           max_pos=d["max_position_embeddings"], ln_eps=d.get("layer_norm_eps", 1e-12))
 
 
 # shapes of the models BASELINE.json / .env.template name (SURVEY.md §2.2 table)
@@ -70,7 +103,14 @@ PRESETS: Dict[str, Tuple[BertConfig, str, int]] = {
                                 "cls", 512),
     "ms-marco-TinyBERT-L-2-v2": (BertConfig(hidden=128, layers=2, heads=2, ffn=512, num_labels=1), "cls", 512),
     "ms-marco-MiniLM-L-12-v2": (BertConfig(hidden=384, layers=12, heads=12, ffn=1536, num_labels=1), "cls", 512),
+    # MPNet sentence embedders (HuggingFaceEmbeddings' default model; Normalize follows the preset's own pipeline)
+    "all-mpnet-base-v2": (MPNetConfig(hidden=768, layers=12, heads=12, ffn=3072), "mean", 384),
+    "multi-qa-mpnet-base-dot-v1": (MPNetConfig(hidden=768, layers=12, heads=12, ffn=3072), "cls", 512),
+    "tiny-mpnet": (MPNetConfig(vocab_size=1000, hidden=128, layers=2, heads=4, ffn=256, max_pos=130), "mean", 64),
 }
+
+# presets whose sentence-transformers pipeline has no Normalize module
+UNNORMALIZED_PRESETS = {"multi-qa-mpnet-base-dot-v1"}
 
 # FlashRank's model names -> the public HuggingFace checkpoints its ONNX files were exported from [3P-recall: flashrank
 # 0.2.x; the mapping is recalled, not read, and is unverified].  Only the BERT cross-encoders are here: FlashRank's T5
@@ -108,7 +148,32 @@ def weight_names(cfg: BertConfig, with_head: bool):
             ("pooler.dense.weight", (H, H)), ("pooler.dense.bias", (H,)),
             ("classifier.weight", (cfg.num_labels, H)), ("classifier.bias", (cfg.num_labels,)),
         ]
+    if cfg.rel_buckets:
+        names.append((REL_BIAS, (cfg.rel_buckets, cfg.heads)))
     return names
+
+
+REL_BIAS = "encoder.relative_attention_bias.weight"
+# MPNet checkpoint names -> the BERT names above (the embeddings and the FFN blocks have BERT's names already)
+_MPNET_RENAME = (("attention.attn.q.", "attention.self.query."), ("attention.attn.k.", "attention.self.key."),
+                 ("attention.attn.v.", "attention.self.value."), ("attention.attn.o.", "attention.output.dense."),
+                 ("attention.LayerNorm.", "attention.output.LayerNorm."))
+
+
+def mpnet_to_canonical(raw: Dict[str, np.ndarray], cfg: MPNetConfig) -> Dict[str, np.ndarray]:
+    """MPNet tensors (bare or under ``mpnet.``) -> the canonical names of ``weight_names``: q/k/v/o and the attention
+    LayerNorm renamed, a zero [1, H] token-type table, and rows 0..31 of the relative bias (transformers looks up 32
+    buckets whatever the table holds)."""
+    w: Dict[str, np.ndarray] = {}
+    for k, v in raw.items():
+        k = k[6:] if k.startswith("mpnet.") else k
+        for a, b in _MPNET_RENAME:
+            k = k.replace(a, b)
+        w[k] = np.ascontiguousarray(v, dtype=np.float32)
+    w["embeddings.token_type_embeddings.weight"] = np.zeros((1, cfg.hidden), np.float32)
+    if REL_BIAS in w:
+        w[REL_BIAS] = np.ascontiguousarray(w[REL_BIAS][:cfg.rel_buckets])
+    return w
 
 
 def synthetic_bert_weights(cfg: BertConfig, seed: int = 0, with_head: bool = False,
@@ -119,7 +184,11 @@ def synthetic_bert_weights(cfg: BertConfig, seed: int = 0, with_head: bool = Fal
     rng = np.random.default_rng(seed)
     out: Dict[str, np.ndarray] = {}
     for name, shape in weight_names(cfg, with_head):
-        if name.endswith("LayerNorm.weight"):
+        if name == REL_BIAS:                       # a few units across buckets, as trained MPNet biases spread
+            a = rng.standard_normal(shape)
+        elif name == "embeddings.token_type_embeddings.weight" and cfg.position_mode:
+            a = np.zeros(shape)                    # MPNet has no token types
+        elif name.endswith("LayerNorm.weight"):
             a = 1.0 + 0.1 * rng.standard_normal(shape)
         elif name.endswith("LayerNorm.bias"):
             a = 0.05 * rng.standard_normal(shape)
@@ -159,17 +228,23 @@ def load_hf_snapshot(path: str, with_head: bool):
     cfgd = _read_json(os.path.join(path, "config.json"))
     if cfgd is None:
         raise FileNotFoundError(f"{path}: no config.json")
-    cfg = BertConfig.from_hf(cfgd)
+    mpnet = cfgd.get("model_type") == "mpnet"
+    if mpnet and with_head:
+        raise ValueError(f"{path}: MPNet cross-encoders are not supported (MPNet runs as a sentence embedder only)")
+    cfg = MPNetConfig.from_hf(cfgd) if mpnet else BertConfig.from_hf(cfgd)
     raw = _load_tensors(path)
-    w: Dict[str, np.ndarray] = {}
-    for k, v in raw.items():
-        k2 = k[5:] if k.startswith("bert.") else k
-        w[k2] = np.ascontiguousarray(v, dtype=np.float32)
+    if mpnet:
+        w = mpnet_to_canonical(raw, cfg)
+    else:
+        w: Dict[str, np.ndarray] = {}
+        for k, v in raw.items():
+            k2 = k[5:] if k.startswith("bert.") else k
+            w[k2] = np.ascontiguousarray(v, dtype=np.float32)
     need = [n for n, _ in weight_names(cfg, with_head)]
     missing = [n for n in need if n not in w]
     if missing:
         raise KeyError(f"{path}: missing tensors {missing[:4]}...")
-    pooling, normalize, max_len = "mean", False, min(cfg.max_pos, 512)
+    pooling, normalize, max_len = "mean", False, min(cfg.max_pos - cfg.position_offset, 512)
     mods = _read_json(os.path.join(path, "modules.json")) or []
     for m in mods:
         if m.get("type", "").endswith("Pooling"):
@@ -208,9 +283,11 @@ def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] 
         if preset not in PRESETS:
             raise ValueError(f"unknown synthetic preset {preset!r}; have {sorted(PRESETS)}")
         cfg, pooling, max_len = PRESETS[preset]
-        cfg = BertConfig(**asdict(cfg))
+        if cfg.position_mode and with_head:
+            raise ValueError(f"synthetic preset {preset!r} is MPNet: MPNet cross-encoders are not supported")
+        cfg = type(cfg)(**asdict(cfg))
         w = synthetic_bert_weights(cfg, seed=seed, with_head=with_head, scale=scale)
-        return cfg, w, pooling, True, max_len, "identity", None
+        return cfg, w, pooling, preset not in UNNORMALIZED_PRESETS, max_len, "identity", None
     cands = [model_name]
     for root in (cache_folder, os.environ.get("RAGMEUP_MODEL_DIR")):
         if root:
