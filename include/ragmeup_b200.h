@@ -168,8 +168,9 @@ int rmu_bm25_csr_free(rmu_bm25_csr* c);
  * (CrossEncoder.predict -> BertForSequenceClassification). */
 /* position_mode: how a token's row of the position table is chosen */
 #define RMU_POS_ABSOLUTE 0   /* BERT: the token's offset j in its sequence                                          */
-#define RMU_POS_OFFSET 1     /* MPNet / RoBERTa (padding index 1): a token of id 1 takes row 1, any other token row
-                              * 2 + j - (tokens of id 1 before it); sequences may hold max_pos - 2 tokens             */
+#define RMU_POS_OFFSET 1     /* MPNet, RoBERTa and XLM-RoBERTa (padding index 1): a token of id 1 takes row 1, any
+                              * other token row 2 + j - (tokens of id 1 before it); sequences may hold max_pos - 2
+                              * tokens (512 for the 514-row tables, 8192 for bge-m3's 8194 rows)                      */
 
 /* The two trailing fields are zero for BERT.  MPNet sets position_mode = RMU_POS_OFFSET and rel_buckets = 32: every
  * attention score gets bias[bucket(key - query), head] of a [32, heads] table shared by all layers (transformers'

@@ -5,7 +5,9 @@ constructs it (``server/RAGHelper.py:483-486``): ``HuggingFaceCrossEncoder(model
 ``.score(text_pairs) -> float32 array [n]``.  Host side mirrors sentence-transformers 2.6.1
 ``CrossEncoder.predict`` (strip, pair tokenisation ``[CLS] q [SEP] d [SEP]`` with token types 0/1,
 truncation=longest_first to 512, input order kept, default activation from the model config;
-SURVEY Appendix A.5/A.6).  Arithmetic: ``csrc/rmu_encoder.cu``.
+SURVEY Appendix A.5/A.6).  XLM-R / RoBERTa rerankers (the bge rerankers, this class's default model) pair as
+``<s> q </s> </s> d </s>`` with no token types and truncate to ``min(model_max_length, max_pos - 2)``.
+Arithmetic: ``csrc/rmu_encoder.cu``.
 """
 from __future__ import annotations
 
@@ -16,7 +18,7 @@ import numpy as np
 from .embeddings import _check_device
 from .encoder import MAX_TOKENS_PER_CALL, BertEncoder
 from .tokenizer import PairAssembler, RaggedTokenizer, load_tokenizer, pipelined
-from .weights import resolve_model
+from .weights import XLMRConfig, resolve_model
 
 PIPE_PAIRS = 512      # pairs per pipelined chunk of a bulk score() call (one 100-pair rerank is a single chunk)
 
@@ -39,10 +41,13 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
         self.config = cfg
         self.max_length = min(int(max_len), cfg.max_pos)
         self.activation = activation
-        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size)
+        xlmr = isinstance(cfg, XLMRConfig)
+        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, xlmr=xlmr)
         self._ragged = RaggedTokenizer(self.tokenizer, self.max_length)
-        # pair batches assembled from cached per-text WordPiece ids (identical to self._ragged(a, b); tests/test_host_logic.py)
+        # pair batches assembled from cached per-text ids (identical to self._ragged(a, b); tests/test_host_logic.py)
         self._pairs = PairAssembler(self.tokenizer, self.max_length)
+        # XLM-R / RoBERTa take no token types (their tokenizers return none): a null pointer, all zeros
+        self._types = not xlmr
         self.client = BertEncoder(cfg, w, with_head=True, device=device)
 
     def _post(self, logits: np.ndarray) -> np.ndarray:
@@ -59,7 +64,7 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
         # bulk calls: pairs in chunks, WordPiece of chunk i+1 overlapped with the device scoring of chunk i
         chunks = [pairs[s:s + PIPE_PAIRS] for s in range(0, len(pairs), PIPE_PAIRS)]
         outs = pipelined(chunks, lambda c: self._pairs([p[0].strip() for p in c], [p[1].strip() for p in c]),
-                         lambda t: self.client.classify_host(*t))
+                         lambda t: self.client.classify_host(t[0], t[1] if self._types else None, t[2]))
         return self._post(outs[0] if len(outs) == 1 else np.concatenate(outs, 0))
 
     def score_tensor(self, text_pairs: Sequence[Tuple[str, str]]):
@@ -75,7 +80,8 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
         for s, e in BertEncoder._chunks(cu, MAX_TOKENS_PER_CALL):
             t0, t1 = int(cu[s]), int(cu[e])
             sub_cu = (cu[s:e + 1] - cu[s]).astype(np.int32)
-            outs.append(self.client.classify_tokens(ids[t0:t1], typ[t0:t1], sub_cu, int(np.max(np.diff(sub_cu)))))
+            outs.append(self.client.classify_tokens(ids[t0:t1], typ[t0:t1] if self._types else None, sub_cu,
+                                                    int(np.max(np.diff(sub_cu)))))
         logits = outs[0] if len(outs) == 1 else torch.cat(outs, 0)
         if self.activation == "sigmoid":
             logits = torch.sigmoid(logits)

@@ -21,7 +21,7 @@ import numpy as np
 from . import _lib
 from .encoder import MAX_TOKENS_PER_CALL, BertEncoder
 from .tokenizer import RaggedTokenizer, load_tokenizer, pipelined
-from .weights import resolve_model
+from .weights import MPNetConfig, XLMRConfig, resolve_model
 
 PIPE_TEXTS = 1000     # texts per pipelined chunk of a bulk embed_documents() call
 
@@ -56,8 +56,10 @@ class HuggingFaceEmbeddings:
         # sentence-transformers applies the model's own Normalize module; encode_kwargs can force it
         self.normalize = bool(normalize or self.encode_kwargs.get("normalize_embeddings", False))
         self.max_seq_length = int(max_len)
-        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, mpnet=cfg.position_mode == 1)
+        xlmr = isinstance(cfg, XLMRConfig)
+        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, mpnet=isinstance(cfg, MPNetConfig), xlmr=xlmr)
         self._ragged = RaggedTokenizer(self.tokenizer, self.max_seq_length)
+        self._types = not xlmr         # XLM-R / RoBERTa take no token types: a null pointer, all zeros
         self.client = BertEncoder(cfg, w, with_head=False, device=device)
 
     # -- tensor fast path (additional to the reference surface)
@@ -72,8 +74,8 @@ class HuggingFaceEmbeddings:
         for s, e in BertEncoder._chunks(cu, MAX_TOKENS_PER_CALL):
             t0, t1 = int(cu[s]), int(cu[e])
             sub_cu = (cu[s:e + 1] - cu[s]).astype(np.int32)
-            outs.append(self.client.embed_tokens(ids[t0:t1], typ[t0:t1], sub_cu, int(np.max(np.diff(sub_cu))),
-                                                 self.pooling, self.normalize))
+            outs.append(self.client.embed_tokens(ids[t0:t1], typ[t0:t1] if self._types else None, sub_cu,
+                                                 int(np.max(np.diff(sub_cu))), self.pooling, self.normalize))
         return outs[0] if len(outs) == 1 else torch.cat(outs, 0)
 
     def _encode_host(self, texts: List[str]) -> np.ndarray:
@@ -82,7 +84,8 @@ class HuggingFaceEmbeddings:
         texts = [t.replace("\n", " ").strip() for t in texts]
         # bulk calls: WordPiece of chunk i+1 overlapped with the device encode of chunk i
         chunks = [texts[s:s + PIPE_TEXTS] for s in range(0, len(texts), PIPE_TEXTS)]
-        outs = pipelined(chunks, self._ragged, lambda t: self.client.embed_host(t[0], t[1], t[2], self.pooling, self.normalize))
+        outs = pipelined(chunks, self._ragged, lambda t: self.client.embed_host(t[0], t[1] if self._types else None, t[2],
+                                                                                  self.pooling, self.normalize))
         return outs[0] if len(outs) == 1 else np.concatenate(outs, 0)
 
     # -- the reference surface

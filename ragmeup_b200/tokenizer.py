@@ -11,6 +11,7 @@ batches into the ragged ``cu_seqlens`` layout the CUDA encoder consumes
 """
 from __future__ import annotations
 
+import functools
 import os
 import threading
 from concurrent.futures import ThreadPoolExecutor
@@ -97,15 +98,71 @@ def build_mpnet_wordpiece(vocab: Dict[str, int]) -> Tokenizer:
     return tok
 
 
-def load_tokenizer(source: Optional[str], vocab_size: int = 30522, mpnet: bool = False) -> Tokenizer:
+XLMR_SPECIALS = MPNET_SPECIALS                         # <s>=0, <pad>=1, </s>=2, <unk>=3; "<mask>" is the last id
+_LETTERS = "abcdefghijklmnopqrstuvwxyz0123456789.,;:!?'\"()-"
+
+
+@functools.lru_cache(maxsize=4)
+def synthetic_xlmr_pieces(size: int = 250002, seed: int = 11) -> Tuple[Tuple[str, float], ...]:
+    """A seeded SentencePiece Unigram vocabulary of ``size`` pieces in XLM-R's id layout: the four specials, "▁", every
+    letter, digit and punctuation mark with and without the "▁" word-start mark, then distinct pseudo-words of one to
+    four syllables (about half of them word-initial), then <mask>.  Scores are negative log-probabilities that favour
+    short pieces, so a word splits into few pieces."""
+    assert size >= 400
+    pieces = [(t, 0.0) for t in XLMR_SPECIALS] + [("▁", -3.0)]
+    pieces += [(p + c, -8.0) for c in _LETTERS for p in ("▁", "")]
+    seen = {p for p, _ in pieces}
+    rng = np.random.default_rng(seed)
+    need = size - 1 - len(pieces)
+    while need > 0:
+        m = 2 * need + 64
+        n = rng.integers(1, 5, m)
+        syl = rng.integers(0, len(_SYL), (m, 4))
+        mark = rng.random(m) < 0.5
+        score = -(n + rng.random(m))
+        for k in range(m):
+            w = ("▁" if mark[k] else "") + "".join(_SYL[j] for j in syl[k, :n[k]])
+            if w not in seen:
+                seen.add(w)
+                pieces.append((w, float(score[k])))
+                need -= 1
+                if need == 0:
+                    break
+    pieces.append(("<mask>", 0.0))
+    return tuple(pieces)
+
+
+def build_xlmr_unigram(pieces: Sequence[Tuple[str, float]]) -> Tokenizer:
+    """XLM-R's tokenizer shape: Unigram over ``pieces``, Metaspace pre-tokenisation, templates ``<s> A </s>`` and
+    ``<s> A </s> </s> B </s>`` (type ids 0), and the specials as added tokens, so a literal "<pad>" is id 1."""
+    tok = Tokenizer(models.Unigram(list(pieces), unk_id=3, byte_fallback=False))
+    tok.pre_tokenizer = pre_tokenizers.Metaspace(replacement="▁", prepend_scheme="always")
+    tok.post_processor = processors.TemplateProcessing(
+        single="<s> $A </s>", pair="<s> $A </s> </s> $B </s>", special_tokens=[("<s>", 0), ("</s>", 2)])
+    tok.decoder = decoders.Metaspace(replacement="▁", prepend_scheme="always")
+    tok.add_special_tokens([*XLMR_SPECIALS, "<mask>"])
+    return tok
+
+
+def load_tokenizer(source: Optional[str], vocab_size: int = 30522, mpnet: bool = False, xlmr: bool = False) -> Tokenizer:
     """``source`` = snapshot dir (tokenizer.json or vocab.txt) or None -> synthetic vocab; ``mpnet`` selects MPNet's
-    vocabulary layout and templates where the snapshot has no tokenizer.json."""
+    vocabulary layout and templates where the snapshot has no tokenizer.json.  ``xlmr`` (XLM-R / RoBERTa): a snapshot
+    must have tokenizer.json (SentencePiece Unigram or byte-level BPE, read by ``tokenizers``); None -> the synthetic
+    Unigram vocabulary."""
+    if xlmr and source is None:
+        return build_xlmr_unigram(synthetic_xlmr_pieces(vocab_size))
     build = build_mpnet_wordpiece if mpnet else build_wordpiece
     if source is None:
         return build(synthetic_mpnet_vocab(vocab_size) if mpnet else synthetic_vocab(vocab_size))
     tj = os.path.join(source, "tokenizer.json")
     if os.path.exists(tj):
         return Tokenizer.from_file(tj)
+    if xlmr:
+        why = (f"{source}: XLM-R / RoBERTa snapshots need tokenizer.json (the sentencepiece package is not a "
+               f"dependency; saving the tokenizer with transformers' fast tokenizer writes it)")
+        if os.path.exists(os.path.join(source, "sentencepiece.bpe.model")):
+            raise ValueError(why + ", and this one has only sentencepiece.bpe.model")
+        raise FileNotFoundError(why)
     vt = os.path.join(source, "vocab.txt")
     if os.path.exists(vt):
         with open(vt, encoding="utf-8") as f:
@@ -202,27 +259,46 @@ def pipelined(chunks: Sequence, tokenize, run) -> List:
 
 
 class PairAssembler:
-    """(text_a, text_b) pairs -> the ragged ``[CLS] a [SEP] b [SEP]`` batch of ``RaggedTokenizer(a, b)``, built from
-    PER-TEXT WordPiece ids that are cached.  A reranker scores the same documents against many queries (and the same
-    query against many documents): with the cache only unseen texts reach the tokeniser.
+    """(text_a, text_b) pairs -> the ragged batch of ``RaggedTokenizer(a, b)`` (``[CLS] a [SEP] b [SEP]`` for BERT,
+    ``<s> a </s> </s> b </s>`` for XLM-R / RoBERTa), built from PER-TEXT ids that are cached.  A reranker scores the
+    same documents against many queries (and the same query against many documents): with the cache only unseen texts
+    reach the tokeniser.
 
-    Equality with pair tokenisation rests on two facts checked in tests/test_host_logic.py: BERT normalisation and
-    pre-tokenisation act on each segment separately, and `truncation="longest_first"` in HF `tokenizers` is the closed
-    form below (shorter side n1, longer n2: n2 = max(n1, B - n1); if still too long n1 = B // 2, n2 = n1 + B % 2), with
-    B = max_length minus the three special tokens."""
+    The special tokens around and between the two texts, and their token types, are the tokenizer's own pair template,
+    read once from the post-processor's output on a probe pair.  Equality with pair tokenisation rests on two facts
+    checked in tests/test_host_logic.py and tests/test_xlmr_cpu.py: normalisation and pre-tokenisation act on each
+    segment separately, and `truncation="longest_first"` in HF `tokenizers` is the closed form below (shorter side n1,
+    longer n2: n2 = max(n1, B - n1); if still too long n1 = B // 2, n2 = n1 + B % 2), with B = max_length minus the
+    template's special tokens (three for BERT, four for RoBERTa)."""
 
     def __init__(self, tok: Tokenizer, max_length: int, max_entries: int = 1 << 18):
         self.max_length = int(max_length)
         self._tok = Tokenizer.from_str(tok.to_str())
         self._tok.no_truncation()
         self._tok.no_padding()
-        self._cls = tok.token_to_id("[CLS]")
-        self._sep = tok.token_to_id("[SEP]")
-        if self._cls is None or self._sep is None:
-            raise ValueError("PairAssembler needs a BERT vocabulary with [CLS] and [SEP]")
+        self._pre, self._mid, self._post, self._type_a, self._type_b = self._template(self._tok)
         self._cache: Dict[str, np.ndarray] = {}
         self._max_entries = int(max_entries)
         self._lock = threading.Lock()
+
+    @staticmethod
+    def _template(tok: Tokenizer):
+        """the pair template as (ids before a, ids between a and b, ids after b, type of [pre, a, mid], type of
+        [b, post]) from the post-processor's output on the pair ("a", "b")"""
+        e = tok.encode("a", "b")
+        seq, ids, typ = e.sequence_ids, np.asarray(e.ids, dtype=np.int32), e.type_ids
+        ia = [i for i, s in enumerate(seq) if s == 0]
+        ib = [i for i, s in enumerate(seq) if s == 1]
+        if not ia or not ib or ia != list(range(ia[0], ia[-1] + 1)) or ib != list(range(ib[0], ib[-1] + 1)) \
+                or ia[-1] >= ib[0]:
+            raise ValueError("PairAssembler: the tokenizer's pair template is not <specials> a <specials> b <specials>")
+        a0, a1, b0, b1 = ia[0], ia[-1] + 1, ib[0], ib[-1] + 1
+        if any(seq[i] is not None for i in (*range(a0), *range(a1, b0), *range(b1, len(seq)))):
+            raise ValueError("PairAssembler: the pair template interleaves text and special tokens")
+        ta, tb = typ[a0], typ[b0]
+        if any(t != ta for t in typ[:b0]) or any(t != tb for t in typ[b0:]):
+            raise ValueError("PairAssembler: the pair template's token types are not one run for a, one for b")
+        return ids[:a0], ids[a1:b0], ids[b1:], int(ta), int(tb)
 
     def _ids(self, texts: Sequence[str]) -> List[np.ndarray]:
         got: Dict[str, np.ndarray] = {}
@@ -246,7 +322,8 @@ class PairAssembler:
         ia, ib = self._ids(list(texts_a)), self._ids(list(texts_b))
         la = np.fromiter(map(len, ia), dtype=np.int64, count=len(ia))
         lb = np.fromiter(map(len, ib), dtype=np.int64, count=len(ib))
-        budget = self.max_length - 3
+        pre, mid, post = self._pre, self._mid, self._post
+        budget = self.max_length - (len(pre) + len(mid) + len(post))
         swap = la > lb
         n1, n2 = np.where(swap, lb, la), np.where(swap, la, lb)
         over = la + lb > budget
@@ -257,15 +334,14 @@ class PairAssembler:
         na = np.where(over, np.where(swap, n2t, n1t), la)
         nb = np.where(over, np.where(swap, n1t, n2t), lb)
         cu = np.zeros(len(ia) + 1, dtype=np.int32)
-        np.cumsum(na + nb + 3, out=cu[1:])
-        cls = np.asarray([self._cls], dtype=np.int32)
-        sep = np.asarray([self._sep], dtype=np.int32)
+        np.cumsum(na + nb + (len(pre) + len(mid) + len(post)), out=cu[1:])
         pieces = []
         for a, b, x, y in zip(ia, ib, na, nb):
-            pieces += (cls, a[:x], sep, b[:y], sep)
+            pieces += (pre, a[:x], mid, b[:y], post)
         ids = np.concatenate(pieces) if pieces else np.zeros(0, dtype=np.int32)
-        typ = np.zeros(int(cu[-1]), dtype=np.int32)
-        starts = cu[:-1] + na.astype(np.int32) + 2                 # first token of segment b
-        for s0, e0 in zip(starts, cu[1:]):
-            typ[s0:e0] = 1
+        if self._type_a == self._type_b:
+            typ = np.full(int(cu[-1]), self._type_a, dtype=np.int32)
+        else:                                                      # one run of type_a, then one of type_b per pair
+            runs = np.stack([na + (len(pre) + len(mid)), nb + len(post)], 1).ravel()
+            typ = np.repeat(np.tile(np.asarray([self._type_a, self._type_b], np.int32), len(ia)), runs)
         return ids, typ, cu

@@ -89,6 +89,41 @@ class MPNetConfig(BertConfig):
                            max_pos=d["max_position_embeddings"], ln_eps=d.get("layer_norm_eps", 1e-12))
 
 
+@dataclass
+class XLMRConfig(BertConfig):
+    """XLM-RoBERTa and RoBERTa (transformers ``XLMRobertaModel`` / ``RobertaModel``): BERT's post-LN encoder with
+    MPNet's padding-offset positions (padding index 1) and no relative bias.  The [1, H] token-type table is a trained
+    row, added to every token (the tokenizers return no token types).  The classification head
+    (``RobertaClassificationHead``: dense, tanh, out_proj on token 0) is BERT's pooler + classifier."""
+    vocab_size: int = 250002
+    max_pos: int = 514
+    type_vocab: int = 1
+    ln_eps: float = 1e-5
+    position_mode: int = 1
+    rel_buckets: int = 0
+
+    @staticmethod
+    def from_hf(d: dict) -> "XLMRConfig":
+        kind = d.get("model_type", "xlm-roberta")
+        if int(d.get("pad_token_id", 1)) != 1:
+            raise ValueError(f"{kind} with pad_token_id = {d['pad_token_id']} is not supported: the encoder's position "
+                             f"rule has the padding index fixed at 1")
+        if d.get("position_embedding_type", "absolute") != "absolute":
+            raise ValueError(f"{kind}: only absolute position embeddings are supported, got "
+                             f"{d['position_embedding_type']!r}")
+        if d.get("hidden_act", "gelu") != "gelu":
+            raise ValueError(f"only erf-GELU {kind} encoders are supported, got {d.get('hidden_act')}")
+        return XLMRConfig(vocab_size=d["vocab_size"], hidden=d["hidden_size"], layers=d["num_hidden_layers"],
+                          heads=d["num_attention_heads"], ffn=d["intermediate_size"],
+                          max_pos=d["max_position_embeddings"], type_vocab=d.get("type_vocab_size", 1),
+                          ln_eps=d.get("layer_norm_eps", 1e-5),
+                          num_labels=len(d["id2label"]) if "id2label" in d else d.get("num_labels", 1))
+
+
+# config.json model_type -> how the snapshot is read; a config without model_type is read as BERT
+MODEL_TYPES = ("bert", "mpnet", "roberta", "xlm-roberta")
+
+
 # shapes of the models BASELINE.json / .env.template name (SURVEY.md §2.2 table)
 PRESETS: Dict[str, Tuple[BertConfig, str, int]] = {
     # name: (config, pooling, max_seq_length)
@@ -107,10 +142,19 @@ PRESETS: Dict[str, Tuple[BertConfig, str, int]] = {
     "all-mpnet-base-v2": (MPNetConfig(hidden=768, layers=12, heads=12, ffn=3072), "mean", 384),
     "multi-qa-mpnet-base-dot-v1": (MPNetConfig(hidden=768, layers=12, heads=12, ffn=3072), "cls", 512),
     "tiny-mpnet": (MPNetConfig(vocab_size=1000, hidden=128, layers=2, heads=4, ffn=256, max_pos=130), "mean", 64),
+    # XLM-R: the bge rerankers (HuggingFaceCrossEncoder's default model) and the multilingual embedders
+    "bge-reranker-base": (XLMRConfig(hidden=768, layers=12, heads=12, ffn=3072), "cls", 512),
+    "bge-reranker-v2-m3": (XLMRConfig(hidden=1024, layers=24, heads=16, ffn=4096, max_pos=8194), "cls", 8192),
+    "multilingual-e5-small": (XLMRConfig(vocab_size=250037, hidden=384, layers=12, heads=12, ffn=1536), "mean", 512),
+    "multilingual-e5-base": (XLMRConfig(hidden=768, layers=12, heads=12, ffn=3072), "mean", 512),
+    "bge-m3": (XLMRConfig(hidden=1024, layers=24, heads=16, ffn=4096, max_pos=8194), "cls", 8192),
+    "paraphrase-multilingual-mpnet-base-v2": (XLMRConfig(hidden=768, layers=12, heads=12, ffn=3072), "mean", 128),
+    "tiny-xlmr": (XLMRConfig(vocab_size=2000, hidden=128, layers=2, heads=4, ffn=256, max_pos=130), "mean", 64),
+    "tiny-xlmr-long": (XLMRConfig(vocab_size=2000, hidden=128, layers=2, heads=4, ffn=256, max_pos=8194), "cls", 8192),
 }
 
 # presets whose sentence-transformers pipeline has no Normalize module
-UNNORMALIZED_PRESETS = {"multi-qa-mpnet-base-dot-v1"}
+UNNORMALIZED_PRESETS = {"multi-qa-mpnet-base-dot-v1", "paraphrase-multilingual-mpnet-base-v2"}
 
 # FlashRank's model names -> the public HuggingFace checkpoints its ONNX files were exported from [3P-recall: flashrank
 # 0.2.x; the mapping is recalled, not read, and is unverified].  Only the BERT cross-encoders are here: FlashRank's T5
@@ -176,6 +220,24 @@ def mpnet_to_canonical(raw: Dict[str, np.ndarray], cfg: MPNetConfig) -> Dict[str
     return w
 
 
+def xlmr_to_canonical(raw: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
+    """XLM-R / RoBERTa tensors (bare, as ``XLMRobertaModel.save_pretrained`` writes them, or under ``roberta.``, as the
+    sequence-classification model does) -> the canonical names of ``weight_names``.  The classification head's
+    ``classifier.dense`` is the pooler and ``classifier.out_proj`` the classifier; a bare ``pooler.*`` (the embedder's
+    unused BertPooler) is dropped, so it never stands in for a head."""
+    w: Dict[str, np.ndarray] = {}
+    for k, v in raw.items():
+        if k.startswith("pooler."):
+            continue
+        k = k[8:] if k.startswith("roberta.") else k
+        if k.startswith("classifier.dense."):
+            k = "pooler.dense." + k[17:]
+        elif k.startswith("classifier.out_proj."):
+            k = "classifier." + k[20:]
+        w[k] = np.ascontiguousarray(v, dtype=np.float32)
+    return w
+
+
 def synthetic_bert_weights(cfg: BertConfig, seed: int = 0, with_head: bool = False,
                            scale: float = 1.0) -> Dict[str, np.ndarray]:
     """Seeded random weights.  ``scale=1`` is BERT's init (N(0, 0.02)) with small
@@ -186,8 +248,8 @@ def synthetic_bert_weights(cfg: BertConfig, seed: int = 0, with_head: bool = Fal
     for name, shape in weight_names(cfg, with_head):
         if name == REL_BIAS:                       # a few units across buckets, as trained MPNet biases spread
             a = rng.standard_normal(shape)
-        elif name == "embeddings.token_type_embeddings.weight" and cfg.position_mode:
-            a = np.zeros(shape)                    # MPNet has no token types
+        elif name == "embeddings.token_type_embeddings.weight" and isinstance(cfg, MPNetConfig):
+            a = np.zeros(shape)                    # MPNet has no token types (XLM-R's one row is trained)
         elif name.endswith("LayerNorm.weight"):
             a = 1.0 + 0.1 * rng.standard_normal(shape)
         elif name.endswith("LayerNorm.bias"):
@@ -228,13 +290,18 @@ def load_hf_snapshot(path: str, with_head: bool):
     cfgd = _read_json(os.path.join(path, "config.json"))
     if cfgd is None:
         raise FileNotFoundError(f"{path}: no config.json")
-    mpnet = cfgd.get("model_type") == "mpnet"
+    kind = cfgd.get("model_type", "bert")
+    if kind not in MODEL_TYPES:
+        raise ValueError(f"{path}: model_type {kind!r} is not supported; the encoder runs {', '.join(MODEL_TYPES)}")
+    mpnet, xlmr = kind == "mpnet", kind in ("roberta", "xlm-roberta")
     if mpnet and with_head:
         raise ValueError(f"{path}: MPNet cross-encoders are not supported (MPNet runs as a sentence embedder only)")
-    cfg = MPNetConfig.from_hf(cfgd) if mpnet else BertConfig.from_hf(cfgd)
+    cfg = MPNetConfig.from_hf(cfgd) if mpnet else XLMRConfig.from_hf(cfgd) if xlmr else BertConfig.from_hf(cfgd)
     raw = _load_tensors(path)
     if mpnet:
         w = mpnet_to_canonical(raw, cfg)
+    elif xlmr:
+        w = xlmr_to_canonical(raw)
     else:
         w: Dict[str, np.ndarray] = {}
         for k, v in raw.items():
@@ -245,6 +312,13 @@ def load_hf_snapshot(path: str, with_head: bool):
     if missing:
         raise KeyError(f"{path}: missing tensors {missing[:4]}...")
     pooling, normalize, max_len = "mean", False, min(cfg.max_pos - cfg.position_offset, 512)
+    if xlmr:
+        # CrossEncoder passes max_length=None, so the tokenizer's model_max_length applies [3P-recall]; positions end
+        # at max_pos - 2 tokens either way (8192 for bge-m3 and bge-reranker-v2-m3)
+        max_len = cfg.max_pos - cfg.position_offset
+        tc = _read_json(os.path.join(path, "tokenizer_config.json")) or {}
+        if tc.get("model_max_length") is not None:
+            max_len = min(int(tc["model_max_length"]), max_len)
     mods = _read_json(os.path.join(path, "modules.json")) or []
     for m in mods:
         if m.get("type", "").endswith("Pooling"):
@@ -283,11 +357,13 @@ def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] 
         if preset not in PRESETS:
             raise ValueError(f"unknown synthetic preset {preset!r}; have {sorted(PRESETS)}")
         cfg, pooling, max_len = PRESETS[preset]
-        if cfg.position_mode and with_head:
+        if isinstance(cfg, MPNetConfig) and with_head:
             raise ValueError(f"synthetic preset {preset!r} is MPNet: MPNet cross-encoders are not supported")
         cfg = type(cfg)(**asdict(cfg))
         w = synthetic_bert_weights(cfg, seed=seed, with_head=with_head, scale=scale)
-        return cfg, w, pooling, preset not in UNNORMALIZED_PRESETS, max_len, "identity", None
+        # an XLM-R preset scores as its checkpoint does: one label, no sbert_ce_default_activation_function -> sigmoid
+        act = "sigmoid" if with_head and isinstance(cfg, XLMRConfig) and cfg.num_labels == 1 else "identity"
+        return cfg, w, pooling, preset not in UNNORMALIZED_PRESETS, max_len, act, None
     cands = [model_name]
     for root in (cache_folder, os.environ.get("RAGMEUP_MODEL_DIR")):
         if root:
@@ -300,6 +376,12 @@ def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] 
         f"RAGMEUP_MODEL_DIR at a directory holding its HuggingFace snapshot, or use 'synthetic:<preset>'")
 
 
+def _refuse_xlmr_flashrank(cfg: BertConfig, where: str) -> None:
+    if isinstance(cfg, XLMRConfig):
+        raise ValueError(f"{where}: an XLM-R / RoBERTa model is not a FlashRank model (FlashRank's rerankers are BERT "
+                         f"checkpoints); use HuggingFaceCrossEncoder for it")
+
+
 def resolve_flashrank(model_name: str, cache_folder: Optional[str] = None, max_length: int = 512):
     """FlashRank model name -> (cfg, weights with the classifier head, max_length, vocab_source).
 
@@ -310,6 +392,7 @@ def resolve_flashrank(model_name: str, cache_folder: Optional[str] = None, max_l
     tokenizer_config.json, max_length)``, or ``min(max_position_embeddings, max_length)`` without that file or key."""
     if model_name.startswith("synthetic:"):
         cfg, w, _pool, _norm, _len, _act, src = resolve_model(model_name, with_head=True)
+        _refuse_xlmr_flashrank(cfg, model_name)
         return cfg, w, min(cfg.max_pos, int(max_length)), src
     if model_name not in FLASHRANK_MODELS:
         raise ValueError(f"FlashRank model {model_name!r} is not supported here: the BERT cross-encoders "
@@ -325,6 +408,7 @@ def resolve_flashrank(model_name: str, cache_folder: Optional[str] = None, max_l
             f"(searched: {roots or 'none set'})")
     cfgd = _read_json(os.path.join(path, "config.json")) or {}
     cfg, w, *_ = load_hf_snapshot(path, with_head=True)
+    _refuse_xlmr_flashrank(cfg, path)
     rows = int(w["classifier.weight"].shape[0])
     stated = len(cfgd["id2label"]) if "id2label" in cfgd else cfgd.get("num_labels")
     if stated is not None and int(stated) != rows:
