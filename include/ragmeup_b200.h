@@ -226,6 +226,43 @@ int rmu_encoder_classify_host(rmu_encoder* enc, const int32_t* ids_h, const int3
                               const int32_t* cu_seqlens_h, int B, int total_tokens, int max_seqlen, float* out_h,
                               void* stream);
 
+/* ------------------------------------------------------------------ ColBERT late interaction
+ * Stands behind HuggingFaceCrossEncoder.score on a ColBERT checkpoint (the reference README's `rerank_model`
+ * colbert-ir/colbertv2.0): every query and document token gets a unit vector, linear(h) / max(||linear(h)||, 1e-12)
+ * of the last hidden state h, and a (query, document) pair scores sum over the query's tokens of the maximum dot product
+ * with the document's kept tokens (MaxSim).
+ *
+ * cfg and weights_h as rmu_encoder_create with has_head = 0; linear_h [dim, hidden] host fp32 (ColBERT's `linear`, no
+ * bias), held as split fp16 planes like the GEMM weights: |w| >= 65520 returns RMU_ERR_UNSUPPORTED before any CUDA call,
+ * as does a dim above 128 that is not a multiple of 128, or rel_buckets != 0.  Token ids only: ColBERT sends no token
+ * types. */
+typedef struct rmu_colbert rmu_colbert;
+int rmu_colbert_create(const rmu_bert_config* cfg, const float* const* weights_h, int n_weights, const float* linear_h,
+                       int dim, rmu_colbert** out);
+void rmu_colbert_destroy(rmu_colbert* cb);
+int rmu_colbert_dim(const rmu_colbert* cb);
+/* token vectors of a ragged batch (the rules of rmu_encoder_embed) -> out [total_tokens, dim] fp32.  nkeys [B] int32
+ * (nullable): the attention keys of sequence b are its first min(max(nkeys[b], 1), S_b) tokens in every layer, while
+ * every token is a query row (ColBERT's [MASK] query padding, attend_to_mask_tokens = false).  keep [total_tokens] uint8
+ * (nullable = all kept): a token with keep 0 gets a zero vector.  All device pointers. */
+int rmu_colbert_vectors(rmu_colbert* cb, const int32_t* ids, const int32_t* cu_seqlens, const int32_t* nkeys,
+                        const uint8_t* keep, int B, int total_tokens, int max_seqlen, float* out, void* stream);
+/* MaxSim: q [*, dim] query token vectors with q_cu, d [*, dim] document token vectors with d_cu and d_keep (nullable =
+ * all kept; a token with keep 0 is skipped, never a candidate for the maximum); pair p scores query pair_q[p] against
+ * document pair_d[p] -> out [n_pairs] fp32.  Each pair is computed in a fixed order from its own token lists, so its
+ * score does not depend on the other pairs of the call.  A document without a kept token scores -inf.  Indices must be
+ * in range (device arrays, not checked); n_pairs = 0 launches nothing.  All device pointers. */
+int rmu_colbert_maxsim(const float* q, const int32_t* q_cu, const float* d, const int32_t* d_cu, const uint8_t* d_keep,
+                       int dim, const int32_t* pair_q, const int32_t* pair_d, int n_pairs, float* out, void* stream);
+/* the whole score from HOST buffers: the query batch (q_nkeys_h nullable) in one run, the documents in runs of at most
+ * max_tokens_per_batch tokens (a longer document runs alone), then MaxSim over the pairs -> out_h [n_pairs].  Pair
+ * indices out of range, cu arrays that do not start at 0, end at the token count or decrease, and a document without a
+ * kept token return RMU_ERR_ARG before any CUDA call.  Synchronises `stream`. */
+int rmu_colbert_score_host(rmu_colbert* cb, const int32_t* q_ids_h, const int32_t* q_cu_h, const int32_t* q_nkeys_h, int nq,
+                           int q_tokens, const int32_t* d_ids_h, const int32_t* d_cu_h, const uint8_t* d_keep_h, int nd,
+                           int d_tokens, const int32_t* pair_q_h, const int32_t* pair_d_h, int n_pairs,
+                           int max_tokens_per_batch, float* out_h, void* stream);
+
 /* ------------------------------------------------------------------ kernel-level test entry points,
  * not part of the product path.  Each runs ONE encoder kernel through the launcher the encoder itself uses, on
  * split fp16 planes the caller owns (v = hi + lo, hi = fp16(v), lo = fp16(v - hi); planes are fp16 bit patterns,
@@ -248,6 +285,11 @@ int rmu_debug_gemm(int mode, const uint16_t* a_hi, const uint16_t* a_lo, int64_t
  * or 5 with d_h = 32. */
 int rmu_debug_attention(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu_seqlens, int B, int H,
                         int heads, int max_seqlen, int warps, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream);
+/* For tests: E2 with a key limit per sequence, as rmu_colbert_vectors runs it: nkeys [B] int32 on the device, sequence
+ * b's keys are its first min(max(nkeys[b], 1), S_b) rows and every row is a query.  warps as rmu_debug_attention. */
+int rmu_debug_attention_keys(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu_seqlens, const int32_t* nkeys,
+                             int B, int H, int heads, int max_seqlen, int warps, uint16_t* ctx_hi, uint16_t* ctx_lo,
+                             void* stream);
 /* For tests: E3 ln_kernel, LayerNorm of pre [T, H] fp32 (biased variance, eps inside the sqrt) -> planes [T, H].
  * H % 128 == 0, H <= 1024. */
 int rmu_debug_layernorm(const float* pre, int T, int H, const float* gamma, const float* beta, float eps,

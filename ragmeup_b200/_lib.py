@@ -85,6 +85,19 @@ SIGNATURES = {
                                          C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "rmu_encoder_classify_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                             C.c_void_p, C.c_void_p]),
+    "rmu_colbert_create": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(C.c_void_p), C.c_int, C.c_void_p, C.c_int,
+                                     C.POINTER(C.c_void_p)]),
+    "rmu_colbert_destroy": (None, [C.c_void_p]),
+    "rmu_colbert_dim": (C.c_int, [C.c_void_p]),
+    "rmu_colbert_vectors": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                      C.c_int, C.c_void_p, C.c_void_p]),
+    "rmu_colbert_maxsim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                     C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "rmu_colbert_score_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                         C.c_int, C.c_void_p, C.c_void_p]),
+    "rmu_debug_attention_keys": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                           C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_gemm": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                  C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -7,6 +7,9 @@ constructs it (``server/RAGHelper.py:483-486``): ``HuggingFaceCrossEncoder(model
 truncation=longest_first to 512, input order kept, default activation from the model config;
 SURVEY Appendix A.5/A.6).  XLM-R / RoBERTa rerankers (the bge rerankers, this class's default model) pair as
 ``<s> q </s> </s> d </s>`` with no token types and truncate to ``min(model_max_length, max_pos - 2)``.
+A ColBERT checkpoint (colbert-ir/colbertv2.0, the reference README's accuracy pick) scores by late interaction instead:
+``score`` returns raw MaxSim scores (``colbert.ColBERTScorer``), where the reference's CrossEncoder would put an
+untrained classification head on the checkpoint (INTEGRATION.md).
 Arithmetic: ``csrc/rmu_encoder.cu``.
 """
 from __future__ import annotations
@@ -18,7 +21,7 @@ import numpy as np
 from .embeddings import _check_device
 from .encoder import MAX_TOKENS_PER_CALL, BertEncoder
 from .tokenizer import PairAssembler, RaggedTokenizer, load_tokenizer, pipelined
-from .weights import XLMRConfig, resolve_model
+from .weights import XLMRConfig, resolve_colbert, resolve_model
 
 PIPE_PAIRS = 512      # pairs per pipelined chunk of a bulk score() call (one 100-pair rerank is a single chunk)
 
@@ -36,6 +39,18 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
         self.model_name = model_name
         self.model_kwargs = dict(model_kwargs or {})
         device = _check_device(self.model_kwargs)
+        self.colbert = None
+        cb = resolve_colbert(model_name, cache_folder=cache_folder)
+        if cb is not None:
+            from .colbert import ColBERTScorer
+            cfg, w, linear, spec, vocab_src = cb
+            self.config = cfg
+            self.colbert = ColBERTScorer(cfg, w, linear, spec, load_tokenizer(vocab_src, cfg.vocab_size), device=device)
+            self.tokenizer = self.colbert.tokenizer
+            self.max_length = spec.doc_maxlen
+            self.activation = "identity"
+            self.client = self.colbert
+            return
         cfg, w, _pool, _norm, max_len, activation, vocab_src = resolve_model(model_name, with_head=True,
                                                                              cache_folder=cache_folder)
         self.config = cfg
@@ -57,6 +72,8 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
         return np.ascontiguousarray(logits[:, 0] if self.config.num_labels == 1 else logits[:, 1], dtype=np.float32)
 
     def score(self, text_pairs: Sequence[Tuple[str, str]]) -> np.ndarray:
+        if self.colbert is not None:
+            return self.colbert.score(text_pairs)
         pairs = list(text_pairs)
         if len(pairs) == 0:
             # sentence-transformers 2.6.1 raises on an empty list (SURVEY §3.4); keep the behaviour
@@ -69,6 +86,8 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
 
     def score_tensor(self, text_pairs: Sequence[Tuple[str, str]]):
         """same scores as a CUDA fp32 tensor [n] (stays on the device)."""
+        if self.colbert is not None:
+            return self.colbert.score_tensor(text_pairs)
         torch = self.client.torch
         pairs = list(text_pairs)
         if len(pairs) == 0:

@@ -16,6 +16,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <mutex>
+#include <type_traits>
 #include <vector>
 
 #include "rmu_gemm.cuh"
@@ -204,6 +205,15 @@ __device__ __forceinline__ float fast_exp2(float x) {   // ex2.approx: 2 ulp, ex
 // (build_relative_bias_table), with i and j the query and key rows within the sequence.  The CTA's head row of the
 // table sits in shared memory behind the V planes.  With the pack empty (BERT) the parameter list and the code are
 // those of the kernel without the bias: one more kernel parameter alone changes ptxas's register allocation.
+//
+// RelBias = KeyLimit (ColBERT queries): the kernel takes nkeys, and sequence b's keys stop at row
+// min(max(nkeys[b], 1), S_b) of the sequence.  Every query row still runs; keys at or past the limit are never staged and
+// are masked like keys past the sequence end, so with nkeys[b] = S_b the arithmetic is the kernel's without the limit.
+struct KeyLimit {
+    const int* __restrict__ n;                // [B] keys per sequence, offset by the slice start like cu
+};
+template <typename... P> constexpr bool kHasBias = (std::is_same_v<P, const float*> || ...);
+template <typename... P> constexpr bool kHasKeyLimit = (std::is_same_v<P, KeyLimit> || ...);
 constexpr int kRelMax = 127;                  // |j - i| >= 127 all fall in MPNet's last bucket (distance >= 91)
 constexpr int kRelSpan = 2 * kRelMax + 1;
 template <int DH, int MINB, int NW = kAttWarps, bool CLS = false, typename... RelBias>  // NW warps = 16 * NW query rows per CTA
@@ -244,7 +254,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
     const __half* ql_base = CLS ? cls_q_lo + static_cast<size_t>(b) * H + h * DH : pl + static_cast<size_t>(t0) * ld + h * DH;
     const int r0 = rbase + warp * 16;
     const bool warp_live = r0 < qrows;
-    if constexpr (sizeof...(RelBias) == 1) {   // this head's biases, visible after the first __syncthreads of the key loop
+    if constexpr (kHasBias<RelBias...>) {      // this head's biases, visible after the first __syncthreads of the key loop
         const float* tab = (rel_bias, ...);
         float* relb = reinterpret_cast<float*>(Vl + ksb * KSTR);
         for (int e = threadIdx.x; e < kRelSpan; e += blockDim.x) relb[e] = tab[h * kRelSpan + e];
@@ -276,8 +286,15 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
     for (int n = 0; n < NT; ++n) oacc[n][0] = oacc[n][1] = oacc[n][2] = oacc[n][3] = 0.f;
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
 
-    for (int sb0 = 0; sb0 < S; sb0 += ksb) {
-        const int nk = min(ksb, S - sb0);
+    // (declared here, next to the key loop: with the block further up, the instantiations without a key limit got
+    // another register allocation)
+    int SK = S;                                    // keys of this sequence
+    if constexpr (kHasKeyLimit<RelBias...>) {
+        const KeyLimit lim = (rel_bias, ...);
+        SK = min(max(lim.n[b], 1), S);
+    }
+    for (int sb0 = 0; sb0 < SK; sb0 += ksb) {
+        const int nk = min(ksb, SK - sb0);
         const int nk16 = (nk + 15) & ~15;
         __syncthreads();
         for (int e = threadIdx.x; e < nk16 * (DH / 8); e += blockDim.x) {
@@ -324,7 +341,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
 #pragma unroll
                 for (int n = 0; n < 4; ++n) if (n < 2 || full_blk) mma16816(sacc[n], qh[ks], bl[n]);
             }
-            if constexpr (sizeof...(RelBias) == 1) {
+            if constexpr (kHasBias<RelBias...>) {
                 // fragment (n, c): key sb0 + kb0 + n * 8 + 2t + (c & 1), query row r0 + g (c < 2) or r0 + g + 8; keys past
                 // the sequence end read a clamped entry and are masked below
                 const float* relb = reinterpret_cast<const float*>(Vl + ksb * KSTR);
@@ -540,13 +557,18 @@ constexpr int kClsAttWarps = 4;
 // cu (and in CLS mode the compact Q and context rows) offset by the slice start.  Within a slice the grid and the
 // kernel are those of one launch, so the heads of a sequence still run together and every row is computed the same.
 // rel_bias non-null: the [heads, kRelSpan] table of build_relative_bias_table is added to every score (warps must be 10).
+// nkeys non-null ([B] int32, full mode without a bias): sequence b attends to its first min(max(nkeys[b], 1), S_b) rows.
 constexpr int kMaxGridY = 65535;
 static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __half* cls_q_hi, const __half* cls_q_lo,
                             const int* cu, int B, int H, int heads, int max_seqlen, int warps, __half* ctx_hi,
-                            __half* ctx_lo, cudaStream_t st, const float* rel_bias = nullptr) {
+                            __half* ctx_lo, cudaStream_t st, const float* rel_bias = nullptr, const int* nkeys = nullptr) {
     const int DH = H / heads;
     const bool cls = cls_q_hi != nullptr;
     const bool bias = rel_bias != nullptr;
+    if (nkeys && (cls || bias)) {
+        set_error("attention: a key limit runs on every query row and without a relative bias");
+        return RMU_ERR_ARG;
+    }
     if (cls) warps = kClsAttWarps;
     else if (!(warps == kAttWarps || (warps == 5 && DH == 32 && !bias))) {
         set_error("attention: warps must be 10, or 5 with head_dim 32 and no relative bias");
@@ -567,14 +589,21 @@ static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __
                                  : attention_planes_kernel<64, 2, kClsAttWarps, true, Tab>)
                      : (DH == 32 ? attention_planes_kernel<32, 2, kAttWarps, false, Tab>
                                  : attention_planes_kernel<64, 1, kAttWarps, false, Tab>);
+    auto lkern = DH == 32 ? (warps == 5 ? attention_planes_kernel<32, 4, 5, false, KeyLimit>
+                                        : attention_planes_kernel<32, 2, kAttWarps, false, KeyLimit>)
+                          : attention_planes_kernel<64, 1, kAttWarps, false, KeyLimit>;
     if (bias) RMU_CUDA(cudaFuncSetAttribute(bkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
+    else if (nkeys) RMU_CUDA(cudaFuncSetAttribute(lkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
     else RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
     for (int s0 = 0; s0 < B; s0 += kMaxGridY) {
         const int nb = std::min(kMaxGridY, B - s0);
         // full mode addresses Q and the context by token (cu[b] is absolute), CLS mode by sequence
         const size_t roff = cls ? static_cast<size_t>(s0) * H : 0;
         dim3 pg(static_cast<unsigned>(heads), static_cast<unsigned>(nb), zblocks);
-        if (bias)
+        if (nkeys)
+            lkern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, nullptr, nullptr, cu + s0, H, ksb, ctx_hi, ctx_lo,
+                                                KeyLimit{nkeys + s0});
+        else if (bias)
             bkern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, cls ? cls_q_hi + roff : nullptr, cls ? cls_q_lo + roff : nullptr,
                                                 cu + s0, H, ksb, ctx_hi + roff, ctx_lo + roff, rel_bias);
         else
@@ -678,6 +707,84 @@ static void build_relative_bias_table(const float* bias, int heads, float* out) 
     for (int h = 0; h < heads; ++h)
         for (int r = -kRelMax; r <= kRelMax; ++r)
             out[static_cast<size_t>(h) * kRelSpan + r + kRelMax] = bias[relative_bucket(r) * heads + h] * 1.4426950408889634f;
+}
+
+// ---------------------------------------------------------------------------------------------------- ColBERT
+// C1 colbert_normalize_kernel: fp32 projections proj [T, ld] (ColBERT's `linear`, columns dim..ld zero padding) -> unit
+// token vectors out [T, dim] = x / max(||x||, 1e-12) (F.normalize).  keep [T] (null = all kept): a dropped token (the
+// punctuation skiplist) is written as zeros; MaxSim skips it by the same mask.  One warp per token.
+__global__ void colbert_normalize_kernel(const float* __restrict__ proj, int T, int ld, int dim, const uint8_t* __restrict__ keep,
+                                         float* __restrict__ out) {
+    const int t = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (t >= T) return;
+    const int lane = static_cast<int>(lane_id());
+    const float* row = proj + static_cast<size_t>(t) * ld;
+    float ss = 0.f;
+    for (int c = lane; c < dim; c += 32) ss = fmaf(row[c], row[c], ss);
+    for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    const float nrm = fmaxf(sqrtf(ss), 1e-12f);
+    const bool kept = keep == nullptr || keep[t] != 0;
+    float* dst = out + static_cast<size_t>(t) * dim;
+    for (int c = lane; c < dim; c += 32) dst[c] = kept ? row[c] / nrm : 0.f;
+}
+
+// C2 colbert_maxsim_kernel: one CTA per (query, document) pair -> out[p] = sum over the query's tokens i of
+// max over the document's kept tokens j of q_i . d_j.  A dot product is one thread's fmaf chain over the dims in order;
+// warp w takes query tokens w, w + kMaxSimWarps, ... and adds their maxima in that order; thread 0 adds the warps' sums
+// in warp order.  So a pair's score depends on its two token lists alone, not on the batch or the grid.  A document
+// without a kept token has max -inf (callers refuse that case: [CLS], the marker and [SEP] are always kept).
+constexpr int kMaxSimWarps = 8;
+__global__ void __launch_bounds__(kMaxSimWarps * 32) colbert_maxsim_kernel(
+        const float* __restrict__ q, const int* __restrict__ q_cu, const float* __restrict__ d, const int* __restrict__ d_cu,
+        const uint8_t* __restrict__ d_keep, int dim, const int* __restrict__ pair_q, const int* __restrict__ pair_d,
+        float* __restrict__ out) {
+    __shared__ float part[kMaxSimWarps];
+    const int p = blockIdx.x;
+    const int qi = pair_q[p], di = pair_d[p];
+    const int q0 = q_cu[qi], nq = q_cu[qi + 1] - q0, d0 = d_cu[di], nd = d_cu[di + 1] - d0;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float acc = 0.f;
+    for (int i = warp; i < nq; i += kMaxSimWarps) {
+        const float* qv = q + static_cast<size_t>(q0 + i) * dim;
+        float m = -INFINITY;
+        for (int j = lane; j < nd; j += 32) {
+            if (d_keep != nullptr && d_keep[d0 + j] == 0) continue;
+            const float* dv = d + static_cast<size_t>(d0 + j) * dim;
+            float s = 0.f;
+            for (int c = 0; c < dim; ++c) s = fmaf(__ldg(qv + c), __ldg(dv + c), s);
+            m = fmaxf(m, s);
+        }
+        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+        acc += m;
+    }
+    if (lane == 0) part[warp] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float s = 0.f;
+        for (int w = 0; w < kMaxSimWarps; ++w) s += part[w];
+        out[p] = s;
+    }
+}
+
+static int launch_colbert_normalize(const float* proj, int T, int ld, int dim, const uint8_t* keep, float* out, cudaStream_t st) {
+    constexpr int wpb = 8;
+    ProfScope _ps(PROF_POOL_HEAD, st);
+    colbert_normalize_kernel<<<static_cast<unsigned>((T + wpb - 1) / wpb), wpb * 32, 0, st>>>(proj, T, ld, dim, keep, out);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// n_pairs = 0 launches nothing
+static int launch_colbert_maxsim(const float* q, const int* q_cu, const float* d, const int* d_cu, const uint8_t* d_keep,
+                                 int dim, const int* pair_q, const int* pair_d, int n_pairs, float* out, cudaStream_t st) {
+    if (n_pairs == 0) return RMU_OK;
+    ProfScope _ps(PROF_POOL_HEAD, st);
+    colbert_maxsim_kernel<<<static_cast<unsigned>(n_pairs), kMaxSimWarps * 32, 0, st>>>(q, q_cu, d, d_cu, d_keep, dim, pair_q,
+                                                                                      pair_d, out);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
 }
 
 }  // namespace rmu
@@ -836,9 +943,10 @@ static int run_last_layer_cls(rmu_encoder* e, const EncLayer& L, const int32_t* 
 }
 
 // the encoder stack: leaves the last hidden state in e->X (split planes), or with cls_only that of the CLS rows alone in
-// e->X_cls (row b = sequence b; e->X then holds the input of the last layer)
+// e->X_cls (row b = sequence b; e->X then holds the input of the last layer).  nkeys ([B] device int32, not with
+// cls_only): every layer's attention keys of sequence b stop at row nkeys[b] (ColBERT's [MASK] query padding).
 static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_ids, const int32_t* cu, int B, int T,
-                       int max_seqlen, bool cls_only, cudaStream_t st) {
+                       int max_seqlen, bool cls_only, cudaStream_t st, const int32_t* nkeys = nullptr) {
     const rmu_bert_config& c = e->cfg;
     const int H = c.hidden, F = c.ffn, DH = H / c.heads;
     // the last position a sequence can reach is its length - 1 plus the offset (2 with padding-offset positions)
@@ -870,7 +978,8 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
         // RMU_ATTN_WARPS = 5: 80-row CTAs, four per SM (same warps/SM, K/V staged twice per 147-token sequence)
         static const int nw_env = [] { const char* e = getenv("RMU_ATTN_WARPS"); return e ? atoi(e) : kAttWarps; }();
         rc = launch_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, H, c.heads, max_seqlen,
-                              (nw_env == 5 && DH == 32 && !e->rel) ? 5 : kAttWarps, e->CTX.hi, e->CTX.lo, st, e->rel);
+                              (nw_env == 5 && DH == 32 && !e->rel) ? 5 : kAttWarps, e->CTX.hi, e->CTX.lo, st, e->rel,
+                              nkeys);
         if (rc != RMU_OK) return rc;
         g = GemmParams{};
         g.M = T; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE; g.res_hi = e->X.hi; g.res_lo = e->X.lo;
@@ -1109,6 +1218,240 @@ int rmu_encoder_classify_host(rmu_encoder* e, const int32_t* ids_h, const int32_
     RMU_CUDA(cudaMemcpyAsync(out_h, e->d_out, static_cast<size_t>(B) * e->cfg.num_labels * sizeof(float), cudaMemcpyDeviceToHost, st));
     RMU_CUDA(cudaStreamSynchronize(st));
     return RMU_OK;
+}
+
+}  // extern "C"
+
+// ---- ColBERT: the encoder without a head, `linear` on the last hidden state, per-token normalisation, MaxSim
+struct DevBuf {
+    void* p = nullptr;
+    size_t cap = 0;
+};
+
+struct rmu_colbert {
+    rmu_encoder* enc = nullptr;
+    int dim = 0, dpad = 0;                // dpad: dim rounded up to E1's 128-column tile (zero rows of `linear`)
+    SplitOperand lin;                     // linear [dpad, H] as split planes (allocations owned by enc)
+    float* zero_bias = nullptr;           // [dpad]
+    float* proj = nullptr;                // [proj_cap, dpad] fp32 projections: workspace, used under enc->mu
+    int proj_cap = 0;
+    // staging of rmu_colbert_score_host, owned by host_mu
+    DevBuf s_qids, s_qcu, s_qnk, s_dids, s_dcu, s_dkeep, s_qv, s_dv, s_pq, s_pd, s_out;
+    std::mutex host_mu;
+};
+
+// grow a staging buffer; the caller holds host_mu and the previous score_host call has synchronised its stream
+static int grow(DevBuf& b, size_t bytes) {
+    if (bytes <= b.cap) return RMU_OK;
+    cudaFree(b.p);
+    b.p = nullptr;
+    b.cap = 0;
+    const size_t cap = std::max<size_t>(bytes + bytes / 2, 4096);
+    RMU_CUDA(cudaMalloc(&b.p, cap));
+    b.cap = cap;
+    return RMU_OK;
+}
+
+// token vectors of a ragged batch -> out [T, dim]: the encoder (keys limited by nkeys when given), E1 mode 0 with
+// `linear` and a zero bias on the last hidden state's split planes -> proj fp32, then C1
+static int colbert_vectors(rmu_colbert* cb, const int32_t* ids, const int32_t* cu, const int32_t* nkeys, const uint8_t* keep,
+                           int B, int T, int max_seqlen, float* out, cudaStream_t st) {
+    rmu_encoder* e = cb->enc;
+    std::lock_guard<std::mutex> g(e->mu);
+    if (T > cb->proj_cap) {
+        RMU_CUDA(cudaDeviceSynchronize());
+        cudaFree(cb->proj);
+        cb->proj = nullptr;
+        cb->proj_cap = 0;
+        const int cap = (std::max(T, 1024) + 127) / 128 * 128;
+        RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&cb->proj), static_cast<size_t>(cap) * cb->dpad * sizeof(float)));
+        cb->proj_cap = cap;
+    }
+    int rc = run_encoder(e, ids, nullptr, cu, B, T, max_seqlen, false, st, nkeys);
+    if (rc != RMU_OK) return rc;
+    GemmParams g2{};
+    g2.M = T; g2.N = cb->dpad; g2.K = e->cfg.hidden; g2.bias = cb->zero_bias; g2.out_f32 = cb->proj;
+    rc = launch_gemm(GEMM_BIAS_F32, e->X, cb->lin, g2, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    rc = launch_colbert_normalize(cb->proj, T, cb->dpad, cb->dim, keep, out, st);
+    if (rc != RMU_OK) return rc;
+    RMU_CUDA(cudaEventRecord(e->ws_done, st));
+    return RMU_OK;
+}
+
+extern "C" {
+
+int rmu_colbert_create(const rmu_bert_config* cfg, const float* const* w, int n_weights, const float* linear_h, int dim,
+                       rmu_colbert** out) {
+    if (!cfg || !w || !linear_h || !out || dim <= 0 || cfg->hidden <= 0) {
+        set_error("rmu_colbert_create: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (dim > 128 && dim % 128 != 0) {
+        set_error("rmu_colbert_create: dim must be at most 128 or a multiple of 128");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (cfg->rel_buckets != 0) {
+        set_error("rmu_colbert_create: a relative attention bias is not supported with ColBERT's key limit");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    const int H = cfg->hidden;
+    const size_t n = static_cast<size_t>(dim) * H;
+    for (size_t j = 0; j < n; ++j) {
+        if (std::fabs(linear_h[j]) >= 65520.0f) {
+            set_error("rmu_colbert_create: linear weight [" + std::to_string(j) + "] = " + std::to_string(linear_h[j]) +
+                      " is outside the split fp16 planes' range (|w| < 65520)");
+            return RMU_ERR_UNSUPPORTED;
+        }
+    }
+    rmu_encoder* enc = nullptr;
+    int rc = rmu_encoder_create(cfg, w, n_weights, 0, &enc);
+    if (rc != RMU_OK) return rc;
+    rmu_colbert* cb = new rmu_colbert();
+    cb->enc = enc;
+    cb->dim = dim;
+    cb->dpad = (dim + 127) / 128 * 128;
+    std::vector<float> pad(static_cast<size_t>(cb->dpad) * H, 0.f);
+    std::copy(linear_h, linear_h + n, pad.begin());
+    rc = upload_split(enc, &cb->lin, {pad.data()}, cb->dpad, H);
+    std::vector<float> zeros(cb->dpad, 0.f);
+    if (rc == RMU_OK) rc = upload(enc, &cb->zero_bias, zeros.data(), zeros.size());
+    if (rc != RMU_OK) { rmu_colbert_destroy(cb); return rc; }
+    *out = cb;
+    return RMU_OK;
+}
+
+void rmu_colbert_destroy(rmu_colbert* cb) {
+    if (!cb) return;
+    cudaDeviceSynchronize();
+    cudaFree(cb->proj);
+    for (DevBuf* b : {&cb->s_qids, &cb->s_qcu, &cb->s_qnk, &cb->s_dids, &cb->s_dcu, &cb->s_dkeep, &cb->s_qv, &cb->s_dv,
+                      &cb->s_pq, &cb->s_pd, &cb->s_out})
+        cudaFree(b->p);
+    rmu_encoder_destroy(cb->enc);
+    delete cb;
+}
+
+int rmu_colbert_dim(const rmu_colbert* cb) { return cb ? cb->dim : 0; }
+
+int rmu_colbert_vectors(rmu_colbert* cb, const int32_t* ids, const int32_t* cu, const int32_t* nkeys, const uint8_t* keep,
+                        int B, int T, int max_seqlen, float* out, void* stream) {
+    int rc = check_batch(cb ? cb->enc : nullptr, ids, cu, B, T, out);
+    if (rc != RMU_OK) return rc;
+    return colbert_vectors(cb, ids, cu, nkeys, keep, B, T, max_seqlen, out, static_cast<cudaStream_t>(stream));
+}
+
+int rmu_colbert_maxsim(const float* q, const int32_t* q_cu, const float* d, const int32_t* d_cu, const uint8_t* d_keep,
+                       int dim, const int32_t* pair_q, const int32_t* pair_d, int n_pairs, float* out, void* stream) {
+    if (!q || !q_cu || !d || !d_cu || dim <= 0 || n_pairs < 0 || (n_pairs > 0 && (!pair_q || !pair_d || !out))) {
+        set_error("rmu_colbert_maxsim: bad argument");
+        return RMU_ERR_ARG;
+    }
+    return launch_colbert_maxsim(q, q_cu, d, d_cu, d_keep, dim, pair_q, pair_d, n_pairs, out, static_cast<cudaStream_t>(stream));
+}
+
+int rmu_colbert_score_host(rmu_colbert* cb, const int32_t* q_ids_h, const int32_t* q_cu_h, const int32_t* q_nkeys_h, int nq,
+                           int q_tokens, const int32_t* d_ids_h, const int32_t* d_cu_h, const uint8_t* d_keep_h, int nd,
+                           int d_tokens, const int32_t* pair_q_h, const int32_t* pair_d_h, int n_pairs,
+                           int max_tokens_per_batch, float* out_h, void* stream) {
+    if (!cb || !q_ids_h || !q_cu_h || !d_ids_h || !d_cu_h || !pair_q_h || !pair_d_h || !out_h || nq <= 0 || q_tokens <= 0 ||
+        nd <= 0 || d_tokens <= 0 || n_pairs <= 0 || max_tokens_per_batch <= 0 || q_cu_h[0] != 0 || q_cu_h[nq] != q_tokens ||
+        d_cu_h[0] != 0 || d_cu_h[nd] != d_tokens) {
+        set_error("rmu_colbert_score_host: bad argument");
+        return RMU_ERR_ARG;
+    }
+    for (int p = 0; p < n_pairs; ++p) {
+        if (pair_q_h[p] < 0 || pair_q_h[p] >= nq || pair_d_h[p] < 0 || pair_d_h[p] >= nd) {
+            set_error("rmu_colbert_score_host: pair index out of range");
+            return RMU_ERR_ARG;
+        }
+    }
+    int q_max = 0;
+    for (int b = 0; b < nq; ++b) {
+        if (q_cu_h[b + 1] < q_cu_h[b]) { set_error("rmu_colbert_score_host: q_cu must be non-decreasing"); return RMU_ERR_ARG; }
+        q_max = std::max(q_max, q_cu_h[b + 1] - q_cu_h[b]);
+    }
+    for (int b = 0; b < nd; ++b) {
+        const int t0 = d_cu_h[b], t1 = d_cu_h[b + 1];
+        if (t1 < t0) { set_error("rmu_colbert_score_host: d_cu must be non-decreasing"); return RMU_ERR_ARG; }
+        bool any = false;
+        for (int t = t0; t < t1 && !any; ++t) any = d_keep_h == nullptr || d_keep_h[t] != 0;
+        if (!any) { set_error("rmu_colbert_score_host: a document has no kept token"); return RMU_ERR_ARG; }
+    }
+    // document runs of at most max_tokens_per_batch tokens (a longer document runs alone), each with its own cu from 0
+    std::vector<int> run_start{0}, run_cu;
+    for (int s = 0; s < nd;) {
+        int e = s + 1;
+        while (e < nd && d_cu_h[e + 1] - d_cu_h[s] <= max_tokens_per_batch) ++e;
+        for (int b = s; b <= e; ++b) run_cu.push_back(d_cu_h[b] - d_cu_h[s]);
+        run_start.push_back(e);
+        s = e;
+    }
+    const int dim = cb->dim;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    std::lock_guard<std::mutex> hg(cb->host_mu);
+    int rc = RMU_OK;
+    const size_t i4 = sizeof(int32_t);
+    for (auto& [buf, bytes] : std::initializer_list<std::pair<DevBuf*, size_t>>{
+             {&cb->s_qids, q_tokens * i4}, {&cb->s_qcu, (nq + 1) * i4}, {&cb->s_qnk, nq * i4}, {&cb->s_dids, d_tokens * i4},
+             {&cb->s_dcu, (run_cu.size() + nd + 1) * i4}, {&cb->s_dkeep, static_cast<size_t>(d_tokens)},
+             {&cb->s_qv, static_cast<size_t>(q_tokens) * dim * sizeof(float)},
+             {&cb->s_dv, static_cast<size_t>(d_tokens) * dim * sizeof(float)}, {&cb->s_pq, n_pairs * i4},
+             {&cb->s_pd, n_pairs * i4}, {&cb->s_out, n_pairs * sizeof(float)}}) {
+        if (rc == RMU_OK) rc = grow(*buf, bytes);
+    }
+    if (rc != RMU_OK) return rc;
+    auto* qids = static_cast<int32_t*>(cb->s_qids.p);
+    auto* qcu = static_cast<int32_t*>(cb->s_qcu.p);
+    auto* qnk = static_cast<int32_t*>(cb->s_qnk.p);
+    auto* dids = static_cast<int32_t*>(cb->s_dids.p);
+    auto* dcu = static_cast<int32_t*>(cb->s_dcu.p);         // [nd + 1] absolute, then the runs' own cu arrays
+    auto* dkeep = static_cast<uint8_t*>(cb->s_dkeep.p);
+    auto* qv = static_cast<float*>(cb->s_qv.p);
+    auto* dv = static_cast<float*>(cb->s_dv.p);
+    RMU_CUDA(cudaMemcpyAsync(qids, q_ids_h, q_tokens * i4, cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(qcu, q_cu_h, (nq + 1) * i4, cudaMemcpyHostToDevice, st));
+    if (q_nkeys_h) RMU_CUDA(cudaMemcpyAsync(qnk, q_nkeys_h, nq * i4, cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(dids, d_ids_h, d_tokens * i4, cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(dcu, d_cu_h, (nd + 1) * i4, cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(dcu + nd + 1, run_cu.data(), run_cu.size() * i4, cudaMemcpyHostToDevice, st));
+    if (d_keep_h) RMU_CUDA(cudaMemcpyAsync(dkeep, d_keep_h, d_tokens, cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(cb->s_pq.p, pair_q_h, n_pairs * i4, cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(cb->s_pd.p, pair_d_h, n_pairs * i4, cudaMemcpyHostToDevice, st));
+    rc = colbert_vectors(cb, qids, qcu, q_nkeys_h ? qnk : nullptr, nullptr, nq, q_tokens, q_max, qv, st);
+    size_t cu_off = nd + 1;
+    for (size_t r = 0; r + 1 < run_start.size() && rc == RMU_OK; ++r) {
+        const int s = run_start[r], e = run_start[r + 1];
+        const int t0 = d_cu_h[s], t1 = d_cu_h[e];
+        int mx = 0;
+        for (int b = s; b < e; ++b) mx = std::max(mx, d_cu_h[b + 1] - d_cu_h[b]);
+        if (t1 > t0)
+            rc = colbert_vectors(cb, dids + t0, dcu + cu_off, nullptr, d_keep_h ? dkeep + t0 : nullptr, e - s, t1 - t0, mx,
+                                 dv + static_cast<size_t>(t0) * dim, st);
+        cu_off += e - s + 1;
+    }
+    if (rc == RMU_OK)
+        rc = launch_colbert_maxsim(qv, qcu, dv, dcu, d_keep_h ? dkeep : nullptr, dim, static_cast<int32_t*>(cb->s_pq.p),
+                                   static_cast<int32_t*>(cb->s_pd.p), n_pairs, static_cast<float*>(cb->s_out.p), st);
+    if (rc != RMU_OK) { cudaStreamSynchronize(st); return rc; }
+    RMU_CUDA(cudaMemcpyAsync(out_h, cb->s_out.p, n_pairs * sizeof(float), cudaMemcpyDeviceToHost, st));
+    RMU_CUDA(cudaStreamSynchronize(st));
+    return RMU_OK;
+}
+
+int rmu_debug_attention_keys(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu, const int32_t* nkeys, int B,
+                             int H, int heads, int max_seqlen, int warps, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream) {
+    if (!qkv_hi || !qkv_lo || !cu || !nkeys || !ctx_hi || !ctx_lo || B <= 0 || heads <= 0 || H <= 0 || max_seqlen <= 0) {
+        set_error("rmu_debug_attention_keys: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H % heads != 0 || (H / heads != 32 && H / heads != 64)) {
+        set_error("rmu_debug_attention_keys: head_dim must be 32 or 64");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_attention(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), nullptr, nullptr,
+                            cu, B, H, heads, max_seqlen, warps, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
+                            static_cast<cudaStream_t>(stream), nullptr, nkeys);
 }
 
 // ---- kernel-level test entry points: the launchers run_encoder uses, on caller-owned planes

@@ -376,6 +376,128 @@ def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] 
         f"RAGMEUP_MODEL_DIR at a directory holding its HuggingFace snapshot, or use 'synthetic:<preset>'")
 
 
+@dataclass
+class ColBERTSpec:
+    """ColBERT's scoring settings.  The defaults are colbert-ai's ``ColBERTConfig`` defaults [3P-recall: colbert-ai
+    0.2.x, not installed here]: query_maxlen 32, doc_maxlen 220, dim 128, markers [unused0] / [unused1],
+    attend_to_mask_tokens False, mask_punctuation True, cosine similarity.  A snapshot's ``artifact.metadata`` overrides
+    them."""
+    dim: int = 128
+    query_maxlen: int = 32
+    doc_maxlen: int = 220
+    query_token: str = "[unused0]"
+    doc_token: str = "[unused1]"
+    attend_to_mask_tokens: bool = False
+    mask_punctuation: bool = True
+    similarity: str = "cosine"
+
+
+# synthetic ColBERT checkpoints: (config, spec).  colbertv2.0 is BERT-base with dim 128, query_maxlen 32 and
+# doc_maxlen 180, the values of colbert-ir/colbertv2.0's artifact.metadata [3P-recall].  tiny-colbert has dim = H = 128,
+# so a transposed `linear` has the right shape and must be caught by the numbers.
+COLBERT_PRESETS: Dict[str, Tuple[BertConfig, ColBERTSpec]] = {
+    "colbertv2.0": (BertConfig(hidden=768, layers=12, heads=12, ffn=3072), ColBERTSpec(doc_maxlen=180)),
+    "tiny-colbert": (BertConfig(vocab_size=1000, hidden=128, layers=2, heads=4, ffn=256, max_pos=128),
+                     ColBERTSpec(query_maxlen=16, doc_maxlen=64)),
+}
+
+
+def colbert_spec(meta: Optional[dict], dim: int) -> ColBERTSpec:
+    """``artifact.metadata`` (or None) + the rows of ``linear.weight`` -> ColBERTSpec; refuses what the encoder does
+    not compute: a similarity other than cosine, attend_to_mask_tokens, a dim that disagrees with the weight, and a dim
+    above 128 that is not a multiple of 128 (the projection runs on 128-column tiles)."""
+    meta = meta or {}
+    s = ColBERTSpec(dim=int(dim))
+    for key, field in (("query_maxlen", "query_maxlen"), ("doc_maxlen", "doc_maxlen"), ("query_token_id", "query_token"),
+                       ("doc_token_id", "doc_token"), ("attend_to_mask_tokens", "attend_to_mask_tokens"),
+                       ("mask_punctuation", "mask_punctuation"), ("similarity", "similarity")):
+        if meta.get(key) is not None:
+            setattr(s, field, type(getattr(s, field))(meta[key]))
+    if meta.get("dim") is not None and int(meta["dim"]) != s.dim:
+        raise ValueError(f"ColBERT: artifact.metadata states dim {meta['dim']} but linear.weight has {s.dim} rows")
+    if s.similarity != "cosine":
+        raise ValueError(f"ColBERT similarity {s.similarity!r} is not supported (cosine only)")
+    if s.attend_to_mask_tokens:
+        raise ValueError("ColBERT with attend_to_mask_tokens = true is not supported: the query's [MASK] padding "
+                         "attends to the real tokens only")
+    if s.dim > 128 and s.dim % 128:
+        raise ValueError(f"ColBERT dim {s.dim} is not supported: at most 128, or a multiple of 128")
+    return s
+
+
+def _tensor_names(path: str):
+    st = os.path.join(path, "model.safetensors")
+    if os.path.exists(st):
+        from safetensors import safe_open
+        with safe_open(st, framework="numpy") as f:
+            return set(f.keys())
+    return set(_load_tensors(path))
+
+
+def is_colbert_snapshot(path: str) -> bool:
+    """``architectures`` names HF_ColBERT, or the tensors hold ``linear.weight`` and no classifier"""
+    cfgd = _read_json(os.path.join(path, "config.json")) or {}
+    if "HF_ColBERT" in (cfgd.get("architectures") or []):
+        return True
+    names = _tensor_names(path)
+    return "linear.weight" in names and not any(n.startswith(("classifier.", "bert.classifier.")) for n in names)
+
+
+def load_colbert_snapshot(path: str):
+    """ColBERT snapshot -> (BertConfig, BERT weights without a head, linear [dim, H] fp32, ColBERTSpec).  The encoder is
+    read under ``bert.`` (or bare); only BERT checkpoints are taken (``model_type`` bert)."""
+    cfgd = _read_json(os.path.join(path, "config.json")) or {}
+    kind = cfgd.get("model_type", "bert")
+    if kind != "bert":
+        raise ValueError(f"{path}: a ColBERT checkpoint of model_type {kind!r} is not supported (BERT only)")
+    cfg = BertConfig.from_hf(cfgd)
+    raw = _load_tensors(path)
+    w = {(k[5:] if k.startswith("bert.") else k): np.ascontiguousarray(v, dtype=np.float32) for k, v in raw.items()}
+    missing = [n for n, _ in weight_names(cfg, False) if n not in w]
+    if missing or "linear.weight" not in w:
+        raise KeyError(f"{path}: missing tensors {(missing or ['linear.weight'])[:4]}...")
+    lin = w["linear.weight"]
+    if lin.ndim != 2 or lin.shape[1] != cfg.hidden:
+        raise ValueError(f"{path}: linear.weight has shape {lin.shape}, expected [dim, {cfg.hidden}]")
+    spec = colbert_spec(_read_json(os.path.join(path, "artifact.metadata")), lin.shape[0])
+    return cfg, {n: w[n] for n, _ in weight_names(cfg, False)}, np.ascontiguousarray(lin), spec
+
+
+def synthetic_colbert(preset: str, seed: int = 0, scale: float = 1.0):
+    """seeded ColBERT weights of a COLBERT_PRESETS shape -> (cfg, weights, linear [dim, H], spec); ``linear`` is
+    N(0, 0.02 * scale) like the other projections"""
+    cfg, spec = COLBERT_PRESETS[preset]
+    cfg = BertConfig(**asdict(cfg))
+    w = synthetic_bert_weights(cfg, seed=seed, with_head=False, scale=scale)
+    rng = np.random.default_rng(seed + 7919)
+    lin = (0.02 * scale * rng.standard_normal((spec.dim, cfg.hidden))).astype(np.float32)
+    return cfg, w, lin, ColBERTSpec(**asdict(spec))
+
+
+def resolve_colbert(model_name: str, cache_folder: Optional[str] = None):
+    """model id -> (cfg, weights, linear, spec, vocab_source) when it names a ColBERT checkpoint (``synthetic:`` one of
+    COLBERT_PRESETS, or a snapshot found as in ``resolve_model``), else None.  A snapshot whose model_type is not one
+    of MODEL_TYPES is left to ``resolve_model``, which refuses it."""
+    if model_name.startswith("synthetic:"):
+        parts = model_name.split(":")
+        if parts[1] not in COLBERT_PRESETS:
+            return None
+        seed = int(parts[2]) if len(parts) > 2 else 0
+        scale = float(parts[3]) if len(parts) > 3 else 1.0
+        return (*synthetic_colbert(parts[1], seed, scale), None)
+    cands = [model_name]
+    for root in (cache_folder, os.environ.get("RAGMEUP_MODEL_DIR")):
+        if root:
+            cands += [os.path.join(root, model_name), os.path.join(root, model_name.split("/")[-1])]
+    for c in cands:
+        if os.path.isdir(c):
+            cfgd = _read_json(os.path.join(c, "config.json"))
+            if cfgd is None or cfgd.get("model_type", "bert") not in MODEL_TYPES or not is_colbert_snapshot(c):
+                return None
+            return (*load_colbert_snapshot(c), c)
+    return None
+
+
 def _refuse_xlmr_flashrank(cfg: BertConfig, where: str) -> None:
     if isinstance(cfg, XLMRConfig):
         raise ValueError(f"{where}: an XLM-R / RoBERTa model is not a FlashRank model (FlashRank's rerankers are BERT "
