@@ -172,25 +172,31 @@ int rmu_bm25_csr_free(rmu_bm25_csr* c);
                               * other token row 2 + j - (tokens of id 1 before it); sequences may hold max_pos - 2
                               * tokens (512 for the 514-row tables, 8192 for bge-m3's 8194 rows)                      */
 
-/* The two trailing fields are zero for BERT.  MPNet sets position_mode = RMU_POS_OFFSET and rel_buckets = 32: every
+/* The three trailing fields are zero for BERT.  MPNet sets position_mode = RMU_POS_OFFSET and rel_buckets = 32: every
  * attention score gets bias[bucket(key - query), head] of a [32, heads] table shared by all layers (transformers'
- * MPNet relative_position_bucket, 32 buckets, max distance 128). */
+ * MPNet relative_position_bucket, 32 buckets, max distance 128).  X-MOD (XLM-R with one language adapter per layer, post-LN,
+ * the adapter after the layer's output LayerNorm, which it reuses) sets adapter_dim = A, the bottleneck width: with
+ * LN = the layer's output LayerNorm and y = W2 ffn + b2 + x1, the layer's output is LN(D2 gelu(D1 LN(y) + d1) + d2 + LN(y))
+ * instead of LN(y).  adapter_dim 0 is no adapter. */
 typedef struct rmu_bert_config {
     int32_t vocab_size, hidden, layers, heads, ffn, max_pos, type_vocab, num_labels;
     float ln_eps;
     int32_t position_mode, rel_buckets;
+    int32_t adapter_dim;
 } rmu_bert_config;
 
 typedef struct rmu_encoder rmu_encoder;
 
 /* weights_h: host fp32 arrays in the canonical order documented in ragmeup_b200/encoder.py
  * (HuggingFace BertModel tensor order; pooler + classifier when has_head; then, when rel_buckets = 32, the relative
- * attention bias [32, heads] last).  The GEMM weights (query, key, value,
- * attention output, intermediate, output) are held as split fp16 planes, which cannot hold |w| >= 65520: such an
- * element (infinities included) returns RMU_ERR_UNSUPPORTED before any CUDA call.  Embedding tables, biases, LayerNorm
- * parameters and the pooler / classifier stay fp32 and are not limited.  A position_mode other than 0 or 1 or a
- * rel_buckets other than 0 or 32 returns RMU_ERR_UNSUPPORTED, and a weight count that does not match (the bias table
- * included) or a null bias table RMU_ERR_ARG, before any CUDA call. */
+ * attention bias [32, heads]; then, when adapter_dim = A > 0, the adapters last, layer by layer: dense1.weight [A, H],
+ * dense1.bias [A], dense2.weight [H, A], dense2.bias [H], so every other tensor keeps its index).  The GEMM weights
+ * (query, key, value, attention output, intermediate, output, adapter dense1 and dense2) are held as split fp16 planes,
+ * which cannot hold |w| >= 65520: such an element (infinities included) returns RMU_ERR_UNSUPPORTED before any CUDA
+ * call.  Embedding tables, biases, LayerNorm parameters and the pooler / classifier stay fp32 and are not limited.  A
+ * position_mode other than 0 or 1, a rel_buckets other than 0 or 32, or an adapter_dim that is negative, not a multiple
+ * of 128 or larger than ffn returns RMU_ERR_UNSUPPORTED, and a weight count that does not match (the bias table and the
+ * adapters included), a null bias table or a null adapter tensor RMU_ERR_ARG, before any CUDA call. */
 int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* weights_h, int n_weights, int has_head,
                        rmu_encoder** out);
 void rmu_encoder_destroy(rmu_encoder* enc);
@@ -232,7 +238,8 @@ int rmu_encoder_classify_host(rmu_encoder* enc, const int32_t* ids_h, const int3
  * of the last hidden state h, and a (query, document) pair scores sum over the query's tokens of the maximum dot product
  * with the document's kept tokens (MaxSim).
  *
- * cfg and weights_h as rmu_encoder_create with has_head = 0; linear_h [dim, hidden] host fp32 (ColBERT's `linear`, no
+ * cfg and weights_h as rmu_encoder_create with has_head = 0 (an X-MOD backbone, colbert-xm, brings its adapters at
+ * the end of weights_h and gets rmu_encoder_create's adapter_dim checks and error codes); linear_h [dim, hidden] host fp32 (ColBERT's `linear`, no
  * bias), held as split fp16 planes like the GEMM weights: |w| >= 65520 returns RMU_ERR_UNSUPPORTED before any CUDA call,
  * as does a dim above 128 that is not a multiple of 128, or rel_buckets != 0.  Token ids only: ColBERT sends no token
  * types. */

@@ -23,7 +23,14 @@ class RmuError(RuntimeError):
 class BertConfigC(C.Structure):
     _fields_ = [("vocab_size", C.c_int32), ("hidden", C.c_int32), ("layers", C.c_int32), ("heads", C.c_int32),
                 ("ffn", C.c_int32), ("max_pos", C.c_int32), ("type_vocab", C.c_int32), ("num_labels", C.c_int32),
-                ("ln_eps", C.c_float), ("position_mode", C.c_int32), ("rel_buckets", C.c_int32)]
+                ("ln_eps", C.c_float), ("position_mode", C.c_int32), ("rel_buckets", C.c_int32),
+                ("adapter_dim", C.c_int32)]
+
+
+def bert_config_c(cfg) -> BertConfigC:
+    """weights.BertConfig (or a subclass) -> the C struct; adapter_dim is 0 for every family but X-MOD"""
+    return BertConfigC(cfg.vocab_size, cfg.hidden, cfg.layers, cfg.heads, cfg.ffn, cfg.max_pos, cfg.type_vocab,
+                       cfg.num_labels, cfg.ln_eps, cfg.position_mode, cfg.rel_buckets, cfg.adapter_dim)
 
 
 # name -> (restype, argtypes); mirrors include/ragmeup_b200.h

@@ -10,6 +10,10 @@ The reference README names ``colbert-ir/colbertv2.0`` as the accuracy pick for `
   (``nkeys`` = the real tokens), and all ``query_maxlen`` vectors are kept;
 * a document is ``". " + text`` truncated to ``doc_maxlen`` with position 1 the document marker; tokens whose id is the
   first id of a ``string.punctuation`` character (or the padding id) are dropped from scoring;
+* on a SentencePiece vocabulary (XLM-R and X-MOD backbones, colbert-xm) the specials are the tokenizer's own: <s>,
+  </s>, <mask> and <pad> (id 1) stand for [CLS], [SEP], [MASK] and [PAD], and a marker token the vocabulary lacks is
+  <unk>.  The punctuation skiplist keeps its rule, so with Metaspace pre-tokenisation it can hold "▁" (the first piece
+  of a mark the vocabulary has no "▁"-piece for), and a lone "▁" is dropped from documents, as colbert-ai does;
 * token vectors are ``normalize(linear(h))``; a pair scores sum over query tokens of the max dot product with the
   document's kept tokens.
 """
@@ -38,11 +42,20 @@ class ColBERTTokenizer:
         self._tok.no_truncation()
         self._tok.no_padding()
         tid = self._tok.token_to_id
-        self.cls, self.sep, self.mask, self.pad = tid("[CLS]"), tid("[SEP]"), tid("[MASK]"), tid("[PAD]")
-        self.q_marker, self.d_marker = tid(spec.query_token), tid(spec.doc_token)
-        if None in (self.cls, self.sep, self.mask, self.pad, self.q_marker, self.d_marker):
-            raise ValueError("ColBERT: the tokenizer lacks [CLS], [SEP], [MASK], [PAD] or a marker token "
-                             f"({spec.query_token}, {spec.doc_token})")
+        if tid("[CLS]") is not None:
+            self.cls, self.sep, self.mask, self.pad = tid("[CLS]"), tid("[SEP]"), tid("[MASK]"), tid("[PAD]")
+            self.q_marker, self.d_marker = tid(spec.query_token), tid(spec.doc_token)
+            if None in (self.cls, self.sep, self.mask, self.pad, self.q_marker, self.d_marker):
+                raise ValueError("ColBERT: the tokenizer lacks [CLS], [SEP], [MASK], [PAD] or a marker token "
+                                 f"({spec.query_token}, {spec.doc_token})")
+        else:
+            # a SentencePiece vocabulary (XLM-R, X-MOD): the tokenizer's own specials; a marker the vocabulary lacks
+            # is <unk>, what convert_tokens_to_ids returns for it
+            self.cls, self.sep, self.mask, self.pad, unk = tid("<s>"), tid("</s>"), tid("<mask>"), tid("<pad>"), tid("<unk>")
+            if None in (self.cls, self.sep, self.mask, self.pad, unk):
+                raise ValueError("ColBERT: the tokenizer has neither [CLS], [SEP], [MASK], [PAD] nor <s>, </s>, <mask>, "
+                                 "<pad>, <unk>")
+            self.q_marker, self.d_marker = (unk if t is None else t for t in (tid(spec.query_token), tid(spec.doc_token)))
         skip = set()
         if spec.mask_punctuation:
             for e in self._tok.encode_batch(list(string.punctuation), add_special_tokens=False):
@@ -112,8 +125,7 @@ class ColBERTScorer:
         if self._linear.shape != (spec.dim, cfg.hidden):
             raise ValueError(f"linear.weight: expected shape {(spec.dim, cfg.hidden)}, got {self._linear.shape}")
         ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
-        cc = _lib.BertConfigC(cfg.vocab_size, cfg.hidden, cfg.layers, cfg.heads, cfg.ffn, cfg.max_pos, cfg.type_vocab,
-                              cfg.num_labels, cfg.ln_eps, cfg.position_mode, cfg.rel_buckets)
+        cc = _lib.bert_config_c(cfg)
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().rmu_colbert_create(C.byref(cc), ptrs, len(arrs), self._linear.ctypes.data, spec.dim,

@@ -9,7 +9,8 @@ SURVEY Appendix A.5/A.6).  XLM-R / RoBERTa rerankers (the bge rerankers, this cl
 ``<s> q </s> </s> d </s>`` with no token types and truncate to ``min(model_max_length, max_pos - 2)``.
 A ColBERT checkpoint (colbert-ir/colbertv2.0, the reference README's accuracy pick) scores by late interaction instead:
 ``score`` returns raw MaxSim scores (``colbert.ColBERTScorer``), where the reference's CrossEncoder would put an
-untrained classification head on the checkpoint (INTEGRATION.md).
+untrained classification head on the checkpoint (INTEGRATION.md).  ColBERT-XM (antoinelouis/colbert-xm, the README's
+multilingual pick) is ColBERT on an X-MOD backbone and runs one language, chosen as ``weights.select_language`` says.
 Arithmetic: ``csrc/rmu_encoder.cu``.
 """
 from __future__ import annotations
@@ -45,7 +46,8 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
             from .colbert import ColBERTScorer
             cfg, w, linear, spec, vocab_src = cb
             self.config = cfg
-            self.colbert = ColBERTScorer(cfg, w, linear, spec, load_tokenizer(vocab_src, cfg.vocab_size), device=device)
+            tok = load_tokenizer(vocab_src, cfg.vocab_size, xlmr=isinstance(cfg, XLMRConfig))
+            self.colbert = ColBERTScorer(cfg, w, linear, spec, tok, device=device)
             self.tokenizer = self.colbert.tokenizer
             self.max_length = spec.doc_maxlen
             self.activation = "identity"

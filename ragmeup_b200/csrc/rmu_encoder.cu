@@ -795,6 +795,8 @@ struct EncLayer {
     SplitOperand Wqkv, Wo, W1, W2;
     float *bqkv = nullptr, *bo = nullptr, *b1 = nullptr, *b2 = nullptr;
     float *ln1g = nullptr, *ln1b = nullptr, *ln2g = nullptr, *ln2b = nullptr;
+    SplitOperand D1, D2;                  // adapter_dim > 0: X-MOD's language adapter, dense1 [A, H] and dense2 [H, A]
+    float *d1 = nullptr, *d2 = nullptr;
 };
 
 struct rmu_encoder {
@@ -814,6 +816,7 @@ struct rmu_encoder {
     // the last layer on the CLS rows (run_last_layer_cls): row b = sequence b, [seq_cap, .]; X_cls ends as their hidden state
     SplitOperand X_cls, Q_cls, CTX_cls, X1_cls, FF_cls;
     float* PRE_cls = nullptr;
+    SplitOperand FFA, FFA_cls;            // adapter_dim > 0: the FF / FF_cls planes seen as [rows, adapter_dim]
     // staging of the *_host entry points: owned by host_mu alone (NOT part of the activation workspace, which a
     // concurrent device-pointer caller may free and re-allocate under mu)
     int *d_ids = nullptr, *d_typ = nullptr, *d_cu = nullptr;
@@ -896,10 +899,33 @@ static int ensure_tokens(rmu_encoder* e, int T, int B) {
     if (rc == RMU_OK) rc = planes(&e->X1_cls, scap, H);
     if (rc == RMU_OK) rc = planes(&e->FF_cls, scap, F);
     if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->PRE_cls, static_cast<size_t>(scap) * H);
+    // the adapter's bottleneck activations reuse the FF planes (adapter_dim <= ffn)
+    const int A = e->cfg.adapter_dim;
+    if (rc == RMU_OK && A > 0) rc = make_split_operand(&e->FFA, e->FF.hi, e->FF.lo, cap, A);
+    if (rc == RMU_OK && A > 0) rc = make_split_operand(&e->FFA_cls, e->FF_cls.hi, e->FF_cls.lo, scap, A);
     if (rc != RMU_OK) { free_acts(e); return rc; }
     e->tok_cap = cap;
     e->seq_cap = scap;
     return RMU_OK;
+}
+
+// X-MOD's language adapter (adapter_dim > 0), between the FFN output and the layer's last LayerNorm.  pre [M, H] holds
+// y = W2 ffn + b2 + x1 on entry and z on exit: h = LN2(y) goes into the x1 planes (free once the FFN-out GEMM has read
+// its residual), then z = D2 gelu(D1 h + d1) + d2 + h through the ffa planes; the caller applies LN2 to z, the same
+// gamma and beta again (adapter_reuse_layer_norm).  Every step computes a row from that row alone.
+static int run_adapter(rmu_encoder* e, const EncLayer& L, int M, float* pre, const SplitOperand& x1, const SplitOperand& ffa,
+                       cudaStream_t st) {
+    const rmu_bert_config& c = e->cfg;
+    const int H = c.hidden, A = c.adapter_dim;
+    int rc = launch_layernorm(pre, M, H, L.ln2g, L.ln2b, c.ln_eps, x1.hi, x1.lo, st);
+    if (rc != RMU_OK) return rc;
+    GemmParams g{};
+    g.M = M; g.N = A; g.K = H; g.bias = L.d1; g.out_hi = ffa.hi; g.out_lo = ffa.lo;
+    rc = launch_gemm(GEMM_BIAS_GELU_SPLIT, x1, L.D1, g, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    g = GemmParams{};
+    g.M = M; g.N = H; g.K = A; g.bias = L.d2; g.out_f32 = pre; g.res_hi = x1.hi; g.res_lo = x1.lo;
+    return launch_gemm(GEMM_BIAS_RESID_F32, ffa, L.D2, g, e->sms, st);
 }
 
 // The last layer when only the CLS rows leave the encoder (classifier head, CLS pooling).  The CLS query attends to
@@ -939,6 +965,10 @@ static int run_last_layer_cls(rmu_encoder* e, const EncLayer& L, const int32_t* 
     g.M = B; g.N = H; g.K = F; g.bias = L.b2; g.out_f32 = e->PRE_cls; g.res_hi = e->X1_cls.hi; g.res_lo = e->X1_cls.lo;
     rc = launch_gemm(GEMM_BIAS_RESID_F32, e->FF_cls, L.W2, g, e->sms, st);
     if (rc != RMU_OK) return rc;
+    if (c.adapter_dim > 0) {
+        rc = run_adapter(e, L, B, e->PRE_cls, e->X1_cls, e->FFA_cls, st);
+        if (rc != RMU_OK) return rc;
+    }
     return launch_layernorm(e->PRE_cls, B, H, L.ln2g, L.ln2b, c.ln_eps, e->X_cls.hi, e->X_cls.lo, st);
 }
 
@@ -995,6 +1025,10 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
         g.M = T; g.N = H; g.K = F; g.bias = L.b2; g.out_f32 = e->PRE; g.res_hi = e->X1.hi; g.res_lo = e->X1.lo;
         rc = launch_gemm(GEMM_BIAS_RESID_F32, e->FF, L.W2, g, e->sms, st);
         if (rc != RMU_OK) return rc;
+        if (c.adapter_dim > 0) {
+            rc = run_adapter(e, L, T, e->PRE, e->X1, e->FFA, st);
+            if (rc != RMU_OK) return rc;
+        }
         rc = launch_layernorm(e->PRE, T, H, L.ln2g, L.ln2b, c.ln_eps, e->X.hi, e->X.lo, st);
         if (rc != RMU_OK) return rc;
     }
@@ -1019,10 +1053,18 @@ int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* w, int n_
         set_error("rmu_encoder_create: rel_buckets must be 0 (no relative position bias) or 32 (MPNet)");
         return RMU_ERR_UNSUPPORTED;
     }
+    const int A = cfg->adapter_dim;
+    if (A < 0 || A % 128 != 0 || A > F) {
+        set_error("rmu_encoder_create: adapter_dim must be 0 (no adapter) or a multiple of 128 no larger than ffn");
+        return RMU_ERR_UNSUPPORTED;
+    }
     const bool rel = cfg->rel_buckets == 32;
-    const int expect = 5 + 16 * L + (has_head ? 4 : 0) + (rel ? 1 : 0);
+    const int adapter0 = 5 + 16 * L + (has_head ? 4 : 0) + (rel ? 1 : 0);   // the adapter tensors come last
+    const int expect = adapter0 + (A > 0 ? 4 * L : 0);
     if (n_weights != expect) { set_error("rmu_encoder_create: expected " + std::to_string(expect) + " weight tensors"); return RMU_ERR_ARG; }
-    if (rel && !w[expect - 1]) { set_error("rmu_encoder_create: null relative attention bias"); return RMU_ERR_ARG; }
+    if (rel && !w[adapter0 - 1]) { set_error("rmu_encoder_create: null relative attention bias"); return RMU_ERR_ARG; }
+    for (int j = adapter0; j < expect; ++j)
+        if (!w[j]) { set_error("rmu_encoder_create: null adapter tensor"); return RMU_ERR_ARG; }
     if (H % 128 != 0 || F % 128 != 0 || H > 1024 || cfg->heads <= 0 || H % cfg->heads != 0 ||
         (H / cfg->heads != 32 && H / cfg->heads != 64)) {
         set_error("rmu_encoder_create: unsupported shape (hidden/ffn multiples of 128, hidden <= 1024, head_dim 32 or 64)");
@@ -1040,6 +1082,19 @@ int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* w, int n_
                 if (std::fabs(p[j]) >= 65520.0f) {
                     set_error("rmu_encoder_create: layer " + std::to_string(l) + " " + kName[k] + " weight [" + std::to_string(j) +
                               "] = " + std::to_string(p[j]) + " is outside the split fp16 planes' range (|w| < 65520)");
+                    return RMU_ERR_UNSUPPORTED;
+                }
+            }
+        }
+    }
+    for (int l = 0; l < L && A > 0; ++l) {
+        for (int k = 0; k < 2; ++k) {                             // dense1 [A, H] and dense2 [H, A]
+            const float* p = w[adapter0 + 4 * l + 2 * k];
+            for (size_t j = 0; j < static_cast<size_t>(A) * H; ++j) {
+                if (std::fabs(p[j]) >= 65520.0f) {
+                    set_error("rmu_encoder_create: layer " + std::to_string(l) + " adapter dense" + std::to_string(k + 1) +
+                              " weight [" + std::to_string(j) + "] = " + std::to_string(p[j]) +
+                              " is outside the split fp16 planes' range (|w| < 65520)");
                     return RMU_ERR_UNSUPPORTED;
                 }
             }
@@ -1105,6 +1160,16 @@ int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* w, int n_
         std::vector<float> tab(static_cast<size_t>(cfg->heads) * kRelSpan);
         build_relative_bias_table(w[i], cfg->heads, tab.data());
         rc = upload(e, &e->rel, tab.data(), tab.size());
+    }
+    i = adapter0;
+    for (int l = 0; l < L && A > 0 && rc == RMU_OK; ++l) {
+        EncLayer& Ly = e->layers[l];
+        rc = upload_split(e, &Ly.D1, {w[i]}, A, H);
+        ++i;
+        up(&Ly.d1, A);
+        if (rc == RMU_OK) rc = upload_split(e, &Ly.D2, {w[i]}, H, A);
+        ++i;
+        up(&Ly.d2, H);
     }
     if (rc != RMU_OK) { rmu_encoder_destroy(e); return rc; }
     *out = e;

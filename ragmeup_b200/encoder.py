@@ -3,7 +3,8 @@
 Weights go to the library in the canonical order of ``weights.weight_names`` (HuggingFace
 ``BertModel`` tensor order: embeddings, then per layer q/k/v/attention-output/LayerNorm/
 intermediate/output/LayerNorm, then pooler + classifier when a head is present, then MPNet's
-relative attention bias [32, heads] when the config has one).
+relative attention bias [32, heads] when the config has one, then X-MOD's language adapter of every layer, for the
+config's one language, when it has ``adapter_dim > 0``).
 """
 from __future__ import annotations
 
@@ -34,8 +35,7 @@ class BertEncoder:
                 raise ValueError(f"{name}: expected shape {shape}, got {a.shape}")
             arrs.append(a)
         ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
-        cc = _lib.BertConfigC(cfg.vocab_size, cfg.hidden, cfg.layers, cfg.heads, cfg.ffn, cfg.max_pos, cfg.type_vocab,
-                              cfg.num_labels, cfg.ln_eps, cfg.position_mode, cfg.rel_buckets)
+        cc = _lib.bert_config_c(cfg)
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().rmu_encoder_create(C.byref(cc), ptrs, len(arrs), int(self.with_head), C.byref(self._h)),

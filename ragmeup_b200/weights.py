@@ -37,9 +37,11 @@ class BertConfig:
     type_vocab: int = 2
     ln_eps: float = 1e-12
     num_labels: int = 1
-    # BERT: positions 0..S-1, no relative bias (class constants, so asdict() of a BERT config keeps its nine fields)
+    # BERT: positions 0..S-1, no relative bias, no language adapter (class constants, so asdict() of a BERT config keeps
+    # its nine fields)
     position_mode: ClassVar[int] = 0
     rel_buckets: ClassVar[int] = 0
+    adapter_dim: ClassVar[int] = 0
 
     @property
     def head_dim(self) -> int:
@@ -120,8 +122,64 @@ class XLMRConfig(BertConfig):
                           num_labels=len(d["id2label"]) if "id2label" in d else d.get("num_labels", 1))
 
 
+XMOD_LANGUAGE_ENV = "RMU_XMOD_LANGUAGE"
+SYNTHETIC_LANGUAGES = ("en_XX", "de_DE", "fr_XX")
+
+
+def select_language(languages, default: Optional[str], where: str) -> str:
+    """The X-MOD language an encoder runs: ``$RMU_XMOD_LANGUAGE`` when set, else ``default`` (config.json's
+    ``default_language``).  No language at all, or one that is not in ``languages``, is a ValueError, as transformers'
+    ``XmodModel.forward`` raises one without ``lang_ids`` or a default language: such a checkpoint is refused like a
+    ``model_type`` the encoder does not run."""
+    lang = os.environ.get(XMOD_LANGUAGE_ENV) or default
+    if lang is None:
+        raise ValueError(f"{where}: model_type 'xmod' is not supported without an input language: config.json sets no "
+                         f"default_language; set {XMOD_LANGUAGE_ENV} to one of {list(languages)}")
+    if lang not in languages:
+        raise ValueError(f"{where}: model_type 'xmod' is not supported in language {lang!r}: it is not one of the "
+                         f"checkpoint's languages {list(languages)}")
+    return lang
+
+
+def xmod_languages(d: dict) -> Tuple[str, ...]:
+    """config.json's ``languages``, in adapter order (transformers' XmodConfig default: en_XX alone)"""
+    return tuple(str(x) for x in d.get("languages", ("en_XX",)))
+
+
+@dataclass
+class XmodConfig(XLMRConfig):
+    """X-MOD (transformers ``XmodModel``): XLM-R with a bottleneck adapter per language in every layer, after the
+    feed-forward output.  With the flags of ``facebook/xmod-base`` (post-LN, ``adapter_reuse_layer_norm``,
+    ``ln_before_adapter``, no adapter LayerNorm) a layer ends ``h = LN(y); out = LN(D2 gelu(D1 h + d1) + d2 + h)`` with
+    the layer's own output LayerNorm both times.  One encoder runs one language, ``language``, of ``languages`` (the
+    order of ``config.languages``); only that language's adapters are read and uploaded."""
+    adapter_dim: int = 384
+    languages: Tuple[str, ...] = SYNTHETIC_LANGUAGES
+    language: str = SYNTHETIC_LANGUAGES[0]
+
+    @staticmethod
+    def from_hf(d: dict, where: str = "xmod") -> "XmodConfig":
+        for key, default, want in (("pre_norm", False, False), ("adapter_layer_norm", False, False),
+                                   ("adapter_reuse_layer_norm", True, True), ("ln_before_adapter", True, True)):
+            if bool(d.get(key, default)) != want:
+                raise ValueError(f"xmod with {key} = {d.get(key)} is not supported: the encoder runs X-MOD with "
+                                 f"pre_norm false, adapter_layer_norm false, adapter_reuse_layer_norm true and "
+                                 f"ln_before_adapter true (facebook/xmod-base's flags)")
+        H, r = int(d["hidden_size"]), int(d.get("adapter_reduction_factor", 2))
+        if r <= 0 or H % r:
+            raise ValueError(f"xmod: hidden_size {H} is not divisible by adapter_reduction_factor {r}")
+        base = XLMRConfig.from_hf({**d, "model_type": "xmod"})
+        languages = xmod_languages(d)
+        lang = select_language(languages, d.get("default_language"), where)
+        return XmodConfig(**asdict(base), adapter_dim=H // r, languages=languages, language=lang)
+
+
+def adapter_prefix(layer: int, language: str) -> str:
+    return f"encoder.layer.{layer}.output.adapter_modules.{language}."
+
+
 # config.json model_type -> how the snapshot is read; a config without model_type is read as BERT
-MODEL_TYPES = ("bert", "mpnet", "roberta", "xlm-roberta")
+MODEL_TYPES = ("bert", "mpnet", "roberta", "xlm-roberta", "xmod")
 
 
 # shapes of the models BASELINE.json / .env.template name (SURVEY.md §2.2 table)
@@ -151,6 +209,10 @@ PRESETS: Dict[str, Tuple[BertConfig, str, int]] = {
     "paraphrase-multilingual-mpnet-base-v2": (XLMRConfig(hidden=768, layers=12, heads=12, ffn=3072), "mean", 128),
     "tiny-xlmr": (XLMRConfig(vocab_size=2000, hidden=128, layers=2, heads=4, ffn=256, max_pos=130), "mean", 64),
     "tiny-xlmr-long": (XLMRConfig(vocab_size=2000, hidden=128, layers=2, heads=4, ffn=256, max_pos=8194), "cls", 8192),
+    # X-MOD: XLM-R base with one adapter per language (adapter_reduction_factor 2); the preset's language is its default
+    "xmod-base": (XmodConfig(hidden=768, layers=12, heads=12, ffn=3072, adapter_dim=384), "mean", 512),
+    "tiny-xmod": (XmodConfig(vocab_size=2000, hidden=256, layers=2, heads=4, ffn=512, max_pos=130, adapter_dim=128),
+                  "mean", 64),
 }
 
 # presets whose sentence-transformers pipeline has no Normalize module
@@ -194,7 +256,18 @@ def weight_names(cfg: BertConfig, with_head: bool):
         ]
     if cfg.rel_buckets:
         names.append((REL_BIAS, (cfg.rel_buckets, cfg.heads)))
+    if cfg.adapter_dim:
+        for l in range(cfg.layers):
+            names += adapter_names(cfg, l, cfg.language)
     return names
+
+
+def adapter_names(cfg: BertConfig, layer: int, language: str):
+    """the four tensors of one X-MOD adapter, in the order rmu_encoder_create takes them"""
+    H, A = cfg.hidden, cfg.adapter_dim
+    p = adapter_prefix(layer, language)
+    return [(p + "dense1.weight", (A, H)), (p + "dense1.bias", (A,)), (p + "dense2.weight", (H, A)),
+            (p + "dense2.bias", (H,))]
 
 
 REL_BIAS = "encoder.relative_attention_bias.weight"
@@ -242,11 +315,17 @@ def synthetic_bert_weights(cfg: BertConfig, seed: int = 0, with_head: bool = Fal
                            scale: float = 1.0) -> Dict[str, np.ndarray]:
     """Seeded random weights.  ``scale=1`` is BERT's init (N(0, 0.02)) with small
     random biases and LayerNorm gains near 1; ``scale>1`` widens the linear
-    weights to a "trained-like" regime (saturating softmax, logits of order 10)."""
+    weights to a "trained-like" regime (saturating softmax, logits of order 10).  An X-MOD config gets an adapter set for
+    every one of its languages, drawn after the rest from a second stream, so the other tensors are those of the XLM-R
+    config of the same shape and seed."""
     rng = np.random.default_rng(seed)
     out: Dict[str, np.ndarray] = {}
-    for name, shape in weight_names(cfg, with_head):
-        if name == REL_BIAS:                       # a few units across buckets, as trained MPNet biases spread
+    names = [(n, s, rng) for n, s in weight_names(cfg, with_head) if ".adapter_modules." not in n]
+    if cfg.adapter_dim:
+        rng2 = np.random.default_rng(seed + 104729)
+        names += [(n, s, rng2) for lang in cfg.languages for l in range(cfg.layers) for n, s in adapter_names(cfg, l, lang)]
+    for name, shape, rng in names:
+        if name == REL_BIAS:                     # a few units across buckets, as trained MPNet biases spread
             a = rng.standard_normal(shape)
         elif name == "embeddings.token_type_embeddings.weight" and isinstance(cfg, MPNetConfig):
             a = np.zeros(shape)                    # MPNet has no token types (XLM-R's one row is trained)
@@ -271,17 +350,30 @@ def _read_json(path: str) -> Optional[dict]:
     return None
 
 
-def _load_tensors(path: str) -> Dict[str, np.ndarray]:
+def _load_tensors(path: str, keep=None) -> Dict[str, np.ndarray]:
     """``model.safetensors``, or for snapshots that ship only the older format (the multilingual MS MARCO reranker
-    behind FlashRank's default) ``pytorch_model.bin``, read with ``weights_only=True`` so no pickled code runs."""
+    behind FlashRank's default) ``pytorch_model.bin``, read with ``weights_only=True`` so no pickled code runs.
+    ``keep(name)`` (optional) selects tensors: from safetensors only those are read; a pickle is read whole and
+    filtered."""
     st = os.path.join(path, "model.safetensors")
     pt = os.path.join(path, "pytorch_model.bin")
     if not os.path.exists(st) and os.path.exists(pt):
         import torch
         sd = torch.load(pt, weights_only=True, map_location="cpu")
-        return {k: v.detach().to(torch.float32).numpy() for k, v in sd.items() if v.is_floating_point()}
-    from safetensors.numpy import load_file
-    return load_file(st)
+        return {k: v.detach().to(torch.float32).numpy() for k, v in sd.items()
+                if v.is_floating_point() and (keep is None or keep(k))}
+    if keep is None:
+        from safetensors.numpy import load_file
+        return load_file(st)
+    from safetensors import safe_open
+    with safe_open(st, framework="numpy") as f:
+        return {k: f.get_tensor(k) for k in f.keys() if keep(k)}
+
+
+def _xmod_keep(language: str):
+    """tensor filter of an X-MOD snapshot: everything but the adapters of the other languages"""
+    mine = f".adapter_modules.{language}."
+    return lambda name: ".adapter_modules." not in name or mine in name
 
 
 def load_hf_snapshot(path: str, with_head: bool):
@@ -293,11 +385,14 @@ def load_hf_snapshot(path: str, with_head: bool):
     kind = cfgd.get("model_type", "bert")
     if kind not in MODEL_TYPES:
         raise ValueError(f"{path}: model_type {kind!r} is not supported; the encoder runs {', '.join(MODEL_TYPES)}")
-    mpnet, xlmr = kind == "mpnet", kind in ("roberta", "xlm-roberta")
+    mpnet, xlmr = kind == "mpnet", kind in ("roberta", "xlm-roberta", "xmod")
     if mpnet and with_head:
         raise ValueError(f"{path}: MPNet cross-encoders are not supported (MPNet runs as a sentence embedder only)")
-    cfg = MPNetConfig.from_hf(cfgd) if mpnet else XLMRConfig.from_hf(cfgd) if xlmr else BertConfig.from_hf(cfgd)
-    raw = _load_tensors(path)
+    if kind == "xmod":
+        cfg = XmodConfig.from_hf(cfgd, path)
+    else:
+        cfg = MPNetConfig.from_hf(cfgd) if mpnet else XLMRConfig.from_hf(cfgd) if xlmr else BertConfig.from_hf(cfgd)
+    raw = _load_tensors(path, _xmod_keep(cfg.language) if cfg.adapter_dim else None)
     if mpnet:
         w = mpnet_to_canonical(raw, cfg)
     elif xlmr:
@@ -360,6 +455,8 @@ def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] 
         if isinstance(cfg, MPNetConfig) and with_head:
             raise ValueError(f"synthetic preset {preset!r} is MPNet: MPNet cross-encoders are not supported")
         cfg = type(cfg)(**asdict(cfg))
+        if isinstance(cfg, XmodConfig):
+            cfg.language = select_language(cfg.languages, cfg.language, model_name)
         w = synthetic_bert_weights(cfg, seed=seed, with_head=with_head, scale=scale)
         # an XLM-R preset scores as its checkpoint does: one label, no sbert_ce_default_activation_function -> sigmoid
         act = "sigmoid" if with_head and isinstance(cfg, XLMRConfig) and cfg.num_labels == 1 else "identity"
@@ -399,6 +496,12 @@ COLBERT_PRESETS: Dict[str, Tuple[BertConfig, ColBERTSpec]] = {
     "colbertv2.0": (BertConfig(hidden=768, layers=12, heads=12, ffn=3072), ColBERTSpec(doc_maxlen=180)),
     "tiny-colbert": (BertConfig(vocab_size=1000, hidden=128, layers=2, heads=4, ffn=256, max_pos=128),
                      ColBERTSpec(query_maxlen=16, doc_maxlen=64)),
+    # antoinelouis/colbert-xm, the reference README's multilingual pick: an xmod-base backbone with colbert-ai's default
+    # dim and lengths [3P-recall: its artifact.metadata is not read here]; [unused0] / [unused1] are not in XLM-R's
+    # vocabulary, so both markers are <unk>
+    "colbert-xm": (XmodConfig(hidden=768, layers=12, heads=12, ffn=3072, adapter_dim=384), ColBERTSpec()),
+    "tiny-colbert-xm": (XmodConfig(vocab_size=2000, hidden=256, layers=2, heads=4, ffn=512, max_pos=130, adapter_dim=128),
+                        ColBERTSpec(query_maxlen=16, doc_maxlen=64)),
 }
 
 
@@ -444,15 +547,25 @@ def is_colbert_snapshot(path: str) -> bool:
 
 
 def load_colbert_snapshot(path: str):
-    """ColBERT snapshot -> (BertConfig, BERT weights without a head, linear [dim, H] fp32, ColBERTSpec).  The encoder is
-    read under ``bert.`` (or bare); only BERT checkpoints are taken (``model_type`` bert)."""
+    """ColBERT snapshot -> (config, encoder weights without a head, linear [dim, H] fp32, ColBERTSpec).  BERT encoders
+    are read under ``bert.`` (or bare); XLM-R, RoBERTa and X-MOD ones under ``roberta.`` (or bare), the base-model prefix
+    of transformers' classes for them, which colbert-ai's HF_ColBERT is assumed to keep [3P-recall: colbert-xm's tensor
+    names are not read here].  An X-MOD backbone reads only its selected language's adapters.  MPNet is refused."""
     cfgd = _read_json(os.path.join(path, "config.json")) or {}
     kind = cfgd.get("model_type", "bert")
-    if kind != "bert":
-        raise ValueError(f"{path}: a ColBERT checkpoint of model_type {kind!r} is not supported (BERT only)")
-    cfg = BertConfig.from_hf(cfgd)
-    raw = _load_tensors(path)
-    w = {(k[5:] if k.startswith("bert.") else k): np.ascontiguousarray(v, dtype=np.float32) for k, v in raw.items()}
+    if kind not in ("bert", "xlm-roberta", "roberta", "xmod"):
+        raise ValueError(f"{path}: a ColBERT checkpoint of model_type {kind!r} is not supported (bert, xlm-roberta, "
+                         f"roberta and xmod are)")
+    if kind == "bert":
+        cfg = BertConfig.from_hf(cfgd)
+        raw = _load_tensors(path)
+        w = {(k[5:] if k.startswith("bert.") else k): np.ascontiguousarray(v, dtype=np.float32) for k, v in raw.items()}
+    else:
+        if any(n.startswith("bert.") for n in _tensor_names(path)):
+            raise ValueError(f"{path}: a ColBERT checkpoint of model_type {kind!r} holds its encoder under 'bert.'; "
+                             f"that prefix is read for BERT only (model_type bert), so the snapshot contradicts itself")
+        cfg = XmodConfig.from_hf(cfgd, path) if kind == "xmod" else XLMRConfig.from_hf(cfgd)
+        w = xlmr_to_canonical(_load_tensors(path, _xmod_keep(cfg.language) if cfg.adapter_dim else None))
     missing = [n for n, _ in weight_names(cfg, False) if n not in w]
     if missing or "linear.weight" not in w:
         raise KeyError(f"{path}: missing tensors {(missing or ['linear.weight'])[:4]}...")
@@ -467,7 +580,9 @@ def synthetic_colbert(preset: str, seed: int = 0, scale: float = 1.0):
     """seeded ColBERT weights of a COLBERT_PRESETS shape -> (cfg, weights, linear [dim, H], spec); ``linear`` is
     N(0, 0.02 * scale) like the other projections"""
     cfg, spec = COLBERT_PRESETS[preset]
-    cfg = BertConfig(**asdict(cfg))
+    cfg = type(cfg)(**asdict(cfg))
+    if isinstance(cfg, XmodConfig):
+        cfg.language = select_language(cfg.languages, cfg.language, f"synthetic:{preset}")
     w = synthetic_bert_weights(cfg, seed=seed, with_head=False, scale=scale)
     rng = np.random.default_rng(seed + 7919)
     lin = (0.02 * scale * rng.standard_normal((spec.dim, cfg.hidden))).astype(np.float32)
@@ -477,7 +592,8 @@ def synthetic_colbert(preset: str, seed: int = 0, scale: float = 1.0):
 def resolve_colbert(model_name: str, cache_folder: Optional[str] = None):
     """model id -> (cfg, weights, linear, spec, vocab_source) when it names a ColBERT checkpoint (``synthetic:`` one of
     COLBERT_PRESETS, or a snapshot found as in ``resolve_model``), else None.  A snapshot whose model_type is not one
-    of MODEL_TYPES is left to ``resolve_model``, which refuses it."""
+    of MODEL_TYPES, and an X-MOD one without a language it can run (``select_language``), is left to
+    ``resolve_model``, which refuses it with the same error as any other model of that type."""
     if model_name.startswith("synthetic:"):
         parts = model_name.split(":")
         if parts[1] not in COLBERT_PRESETS:
@@ -494,13 +610,19 @@ def resolve_colbert(model_name: str, cache_folder: Optional[str] = None):
             cfgd = _read_json(os.path.join(c, "config.json"))
             if cfgd is None or cfgd.get("model_type", "bert") not in MODEL_TYPES or not is_colbert_snapshot(c):
                 return None
+            if cfgd.get("model_type") == "xmod":
+                try:
+                    select_language(xmod_languages(cfgd), cfgd.get("default_language"), c)
+                except ValueError:
+                    return None
             return (*load_colbert_snapshot(c), c)
     return None
 
 
 def _refuse_xlmr_flashrank(cfg: BertConfig, where: str) -> None:
     if isinstance(cfg, XLMRConfig):
-        raise ValueError(f"{where}: an XLM-R / RoBERTa model is not a FlashRank model (FlashRank's rerankers are BERT "
+        kind = "an X-MOD" if isinstance(cfg, XmodConfig) else "an XLM-R / RoBERTa"
+        raise ValueError(f"{where}: {kind} model is not a FlashRank model (FlashRank's rerankers are BERT "
                          f"checkpoints); use HuggingFaceCrossEncoder for it")
 
 
