@@ -185,20 +185,44 @@ typedef struct rmu_bert_config {
     int32_t adapter_dim;
 } rmu_bert_config;
 
+/* What rmu_encoder_create_ex adds, all zero for every model but DeBERTa.  These fields travel in their own struct,
+ * not at the end of rmu_bert_config, so that struct keeps its size and layout for callers built against it, and
+ * rmu_encoder_create keeps its signature.
+ * DeBERTa-v2 / v3 (disentangled attention, share_att_key, pos_att_type c2p | p2c) sets position_buckets = s > 0 and
+ * max_relative_positions = the max_position of transformers' make_log_bucket_position (config.max_relative_positions, or
+ * max_position_embeddings when that is < 1), with zero position and token-type tables (DeBERTa-v3 adds neither).  With
+ * R = LN_rel(rel_embeddings[0:2s]) and, per layer, PQ = Wq R + bq, PK = Wk R + bk split by head like Q and K, every
+ * attention score is (Q_i.K_j + Q_i.PK[c] + K_j.PQ[c]) / sqrt(3 d_h), c = clamp(s + bucket(i - j), 0, 2s - 1).
+ * Sequences may hold max_pos tokens; d_h must be 64, and rel_buckets and adapter_dim 0.  head_act selects the
+ * activation between the pooler and the classifier: RMU_HEAD_TANH (BERT's pooler, 0) or RMU_HEAD_GELU (DeBERTa's
+ * ContextPooler, erf-GELU). */
+#define RMU_HEAD_TANH 0
+#define RMU_HEAD_GELU 1
+typedef struct rmu_encoder_ext {
+    int32_t position_buckets, max_relative_positions, head_act;
+} rmu_encoder_ext;
+
 typedef struct rmu_encoder rmu_encoder;
 
 /* weights_h: host fp32 arrays in the canonical order documented in ragmeup_b200/encoder.py
  * (HuggingFace BertModel tensor order; pooler + classifier when has_head; then, when rel_buckets = 32, the relative
  * attention bias [32, heads]; then, when adapter_dim = A > 0, the adapters last, layer by layer: dense1.weight [A, H],
- * dense1.bias [A], dense2.weight [H, A], dense2.bias [H], so every other tensor keeps its index).  The GEMM weights
+ * dense1.bias [A], dense2.weight [H, A], dense2.bias [H], so every other tensor keeps its index; then, when
+ * position_buckets = s > 0, rel_embeddings [2s, H] and LN_rel's weight [H] and bias [H]).  The GEMM weights
  * (query, key, value, attention output, intermediate, output, adapter dense1 and dense2) are held as split fp16 planes,
  * which cannot hold |w| >= 65520: such an element (infinities included) returns RMU_ERR_UNSUPPORTED before any CUDA
  * call.  Embedding tables, biases, LayerNorm parameters and the pooler / classifier stay fp32 and are not limited.  A
  * position_mode other than 0 or 1, a rel_buckets other than 0 or 32, or an adapter_dim that is negative, not a multiple
  * of 128 or larger than ffn returns RMU_ERR_UNSUPPORTED, and a weight count that does not match (the bias table and the
- * adapters included), a null bias table or a null adapter tensor RMU_ERR_ARG, before any CUDA call. */
+ * adapters included), a null bias table or a null adapter tensor RMU_ERR_ARG, before any CUDA call.  So do, with
+ * RMU_ERR_UNSUPPORTED: a head_act other than 0 or 1; position_buckets < 0; position_buckets = 0 with
+ * max_relative_positions != 0; position_buckets > 0 with max_relative_positions < s / 2 + 2, s > 4096, d_h != 64,
+ * rel_buckets or adapter_dim != 0; and, with RMU_ERR_ARG, a null relative embedding or LN_rel tensor (these for
+ * rmu_encoder_create_ex; rmu_encoder_create is rmu_encoder_create_ex with ext = NULL, all zero). */
 int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* weights_h, int n_weights, int has_head,
                        rmu_encoder** out);
+int rmu_encoder_create_ex(const rmu_bert_config* cfg, const rmu_encoder_ext* ext, const float* const* weights_h,
+                          int n_weights, int has_head, rmu_encoder** out);
 void rmu_encoder_destroy(rmu_encoder* enc);
 
 #define RMU_POOL_MEAN 0
@@ -324,6 +348,24 @@ int rmu_relative_bias_table(const float* bias_h, int buckets, int heads, float* 
 int rmu_debug_attention_bias(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const uint16_t* cls_q_hi,
                              const uint16_t* cls_q_lo, const int32_t* cu_seqlens, int B, int H, int heads, int max_seqlen,
                              const float* rel_table, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream);
+/* Host only, no GPU work: DeBERTa's relative position buckets, out_h[r + n - 1] = make_log_bucket_position(r,
+ * buckets, max_position) for r in [-(n - 1), n - 1], in torch's float32 arithmetic, as rmu_encoder_create builds them.
+ * buckets < 2, max_position < buckets / 2 + 2 or n < 1 return RMU_ERR_UNSUPPORTED / RMU_ERR_ARG. */
+int rmu_log_bucket_table(int buckets, int max_position, int n, int32_t* out_h);
+/* For tests: E2 with DeBERTa's disentangled position terms, as the encoder runs it: the terms C2P (query rows against
+ * PK) and P2C (every key against PQ') into ws, then E2 adding C2P[i, c] + P2C[j, c] to each score.  qkv planes [T, 3H]
+ * with q pre-scaled by log2(e) / sqrt(3 d_h); pos planes [2s, 2H] = PQ' | PK, PQ' pre-scaled like q; cidx_h (HOST)
+ * [2 max_seqlen - 1] int32, entry r + max_seqlen - 1 = clamp(s + bucket(r), 0, 2s - 1), non-decreasing in r; it is
+ * copied into the tail of ws.  cls_q null: every query row, ctx [T, H]; non-null: the compact Q planes [B, H] of query
+ * row 0 of each sequence, ctx [B, H].  ws (device fp32) holds (qrows + T) heads W + 2 max_seqlen - 1 elements, qrows = B
+ * (CLS) or T and W = cidx_h[last] - cidx_h[0] + 1.  d_h must be 64; a smaller ws, a cidx_h that decreases, is negative
+ * or reaches row 2 position_buckets of the pos planes, null pointers or bad sizes return RMU_ERR_ARG before any CUDA
+ * call. */
+int rmu_debug_attention_disentangled(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const uint16_t* cls_q_hi,
+                                     const uint16_t* cls_q_lo, const int32_t* cu_seqlens, int B, int T, int H, int heads,
+                                     int max_seqlen, const uint16_t* pos_hi, const uint16_t* pos_lo, int position_buckets,
+                                     const int32_t* cidx_h, float* ws, int64_t ws_elems, uint16_t* ctx_hi, uint16_t* ctx_lo,
+                                     void* stream);
 /* For tests: E4 pool_kernel, RMU_POOL_MEAN or RMU_POOL_CLS of planes [T, H] per sequence of cu_seqlens [B+1], then
  * x / max(||x||, 1e-12) when normalize -> out [B, H] fp32 (an empty sequence gives zeros).  1 <= H <= 1024. */
 int rmu_debug_pool(const uint16_t* hi, const uint16_t* lo, const int32_t* cu_seqlens, int B, int H, int pool_mode,
@@ -333,6 +375,16 @@ int rmu_debug_pool(const uint16_t* hi, const uint16_t* lo, const int32_t* cu_seq
  * = cw tanh(pw h_cls + pb) + cb.  1 <= H <= 1024. */
 int rmu_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const int32_t* cu_seqlens, int B, int H, int num_labels,
                        const float* pw, const float* pb, const float* cw, const float* cb, float* out, void* stream);
+/* For tests: copies layer `layer`'s PQ' | PK planes [2s, 2H] of a DeBERTa encoder (position_buckets = s > 0), as
+ * rmu_encoder_create_ex computed them, into hi / lo (device, 2s * 2H fp16 each).  Another encoder or layer returns
+ * RMU_ERR_ARG. */
+int rmu_debug_encoder_position_planes(const rmu_encoder* enc, int layer, uint16_t* hi, uint16_t* lo, void* stream);
+/* For tests: the same with the activation between pooler and classifier, head_act RMU_HEAD_TANH (rmu_debug_cls_head) or
+ * RMU_HEAD_GELU (DeBERTa's ContextPooler, erf-GELU), as rmu_encoder_create_ex's ext->head_act selects it.  Another
+ * head_act returns RMU_ERR_ARG. */
+int rmu_debug_cls_head_act(const uint16_t* hi, const uint16_t* lo, const int32_t* cu_seqlens, int B, int H, int num_labels,
+                           const float* pw, const float* pb, const float* cw, const float* cb, int head_act, float* out,
+                           void* stream);
 /* For tests: n fp32 values -> (hi, lo) planes, as every GEMM weight is uploaded; and hi + lo -> n fp32 values, as
  * rmu_encoder_hidden returns the last hidden state.  n < 0 or a null pointer return RMU_ERR_ARG; n = 0 launches
  * nothing. */

@@ -27,10 +27,19 @@ class BertConfigC(C.Structure):
                 ("adapter_dim", C.c_int32)]
 
 
+class EncoderExtC(C.Structure):
+    _fields_ = [("position_buckets", C.c_int32), ("max_relative_positions", C.c_int32), ("head_act", C.c_int32)]
+
+
 def bert_config_c(cfg) -> BertConfigC:
     """weights.BertConfig (or a subclass) -> the C struct; adapter_dim is 0 for every family but X-MOD"""
     return BertConfigC(cfg.vocab_size, cfg.hidden, cfg.layers, cfg.heads, cfg.ffn, cfg.max_pos, cfg.type_vocab,
                        cfg.num_labels, cfg.ln_eps, cfg.position_mode, cfg.rel_buckets, cfg.adapter_dim)
+
+
+def encoder_ext_c(cfg) -> EncoderExtC:
+    """rmu_encoder_create_ex's extra fields: DeBERTa-v2's buckets and head activation, zero for every other family"""
+    return EncoderExtC(cfg.position_buckets, cfg.max_relative_positions, cfg.head_act)
 
 
 # name -> (restype, argtypes); mirrors include/ragmeup_b200.h
@@ -81,6 +90,8 @@ SIGNATURES = {
     "rmu_bm25_csr_free": (C.c_int, [C.c_void_p]),
     "rmu_encoder_create": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(C.c_void_p), C.c_int, C.c_int,
                                      C.POINTER(C.c_void_p)]),
+    "rmu_encoder_create_ex": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(EncoderExtC), C.POINTER(C.c_void_p), C.c_int,
+                                        C.c_int, C.POINTER(C.c_void_p)]),
     "rmu_encoder_destroy": (None, [C.c_void_p]),
     "rmu_encoder_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_void_p, C.c_void_p]),
@@ -121,6 +132,13 @@ SIGNATURES = {
     "rmu_relative_bias_table": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "rmu_debug_attention_bias": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                            C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_log_bucket_table": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "rmu_debug_attention_disentangled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                                   C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                                   C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_encoder_position_planes": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_cls_head_act": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "rmu_debug_pool": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                  C.c_void_p]),
     "rmu_debug_cls_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

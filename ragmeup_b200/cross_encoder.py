@@ -6,7 +6,10 @@ constructs it (``server/RAGHelper.py:483-486``): ``HuggingFaceCrossEncoder(model
 ``CrossEncoder.predict`` (strip, pair tokenisation ``[CLS] q [SEP] d [SEP]`` with token types 0/1,
 truncation=longest_first to 512, input order kept, default activation from the model config;
 SURVEY Appendix A.5/A.6).  XLM-R / RoBERTa rerankers (the bge rerankers, this class's default model) pair as
-``<s> q </s> </s> d </s>`` with no token types and truncate to ``min(model_max_length, max_pos - 2)``.
+``<s> q </s> </s> d </s>`` with no token types and truncate to ``min(model_max_length, max_pos - 2)``.  DeBERTa-v2 / v3
+rerankers (mxbai-rerank-*-v1) pair as ``[CLS] q [SEP] d [SEP]`` and send no token types (the model has none); they
+truncate to ``min(model_max_length, max_position_embeddings)`` and run in calls of at most ``deberta_tokens_per_call``
+tokens, which bounds the attention position terms' workspace.
 A ColBERT checkpoint (colbert-ir/colbertv2.0, the reference README's accuracy pick) scores by late interaction instead:
 ``score`` returns raw MaxSim scores (``colbert.ColBERTScorer``), where the reference's CrossEncoder would put an
 untrained classification head on the checkpoint (INTEGRATION.md).  ColBERT-XM (antoinelouis/colbert-xm, the README's
@@ -20,9 +23,9 @@ from typing import Any, Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from .embeddings import _check_device
-from .encoder import MAX_TOKENS_PER_CALL, BertEncoder
+from .encoder import BertEncoder
 from .tokenizer import PairAssembler, RaggedTokenizer, load_tokenizer, pipelined
-from .weights import XLMRConfig, resolve_colbert, resolve_model
+from .weights import DebertaConfig, XLMRConfig, resolve_colbert, resolve_model
 
 PIPE_PAIRS = 512      # pairs per pipelined chunk of a bulk score() call (one 100-pair rerank is a single chunk)
 
@@ -58,14 +61,16 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
         self.config = cfg
         self.max_length = min(int(max_len), cfg.max_pos)
         self.activation = activation
-        xlmr = isinstance(cfg, XLMRConfig)
-        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, xlmr=xlmr)
+        xlmr, deberta = isinstance(cfg, XLMRConfig), isinstance(cfg, DebertaConfig)
+        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, xlmr=xlmr, deberta=deberta)
         self._ragged = RaggedTokenizer(self.tokenizer, self.max_length)
         # pair batches assembled from cached per-text ids (identical to self._ragged(a, b); tests/test_host_logic.py)
         self._pairs = PairAssembler(self.tokenizer, self.max_length)
-        # XLM-R / RoBERTa take no token types (their tokenizers return none): a null pointer, all zeros
-        self._types = not xlmr
+        # XLM-R / RoBERTa take no token types (their tokenizers return none), and DeBERTa-v3 has no token-type table:
+        # a null pointer, all zeros
+        self._types = not (xlmr or deberta)
         self.client = BertEncoder(cfg, w, with_head=True, device=device)
+        self._max_tokens = self.client.max_tokens_per_call
 
     def _post(self, logits: np.ndarray) -> np.ndarray:
         if self.activation == "sigmoid":
@@ -98,7 +103,7 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
         b = [p[1].strip() for p in pairs]
         ids, typ, cu = self._pairs(a, b)
         outs = []
-        for s, e in BertEncoder._chunks(cu, MAX_TOKENS_PER_CALL):
+        for s, e in BertEncoder._chunks(cu, self._max_tokens):
             t0, t1 = int(cu[s]), int(cu[e])
             sub_cu = (cu[s:e + 1] - cu[s]).astype(np.int32)
             outs.append(self.client.classify_tokens(ids[t0:t1], typ[t0:t1] if self._types else None, sub_cu,

@@ -212,8 +212,19 @@ __device__ __forceinline__ float fast_exp2(float x) {   // ex2.approx: 2 ulp, ex
 struct KeyLimit {
     const int* __restrict__ n;                // [B] keys per sequence, offset by the slice start like cu
 };
+// RelBias = Disentangled (DeBERTa-v2): score(i, j) += C2P[qrow, h, c] + P2C[t0 + j, h, c] with c = cidx[i - j + rmax] - c0,
+// the position terms of launch_position_terms, already in the log2 units of the scores.  qrow is t0 + i, or (CLS) row b
+// of the compact C2P rows.  Reads of query rows and keys past the sequence end are clamped into it; those scores are
+// discarded or masked as without the terms.
+struct Disentangled {
+    const float* __restrict__ c2p;            // [rows, heads, W]: the query rows (tokens, or CLS rows offset by the slice)
+    const float* __restrict__ p2c;            // [T, heads, W]: every key row
+    const int* __restrict__ cidx;             // [2 rmax + 1]: clamp(s + bucket(r), 0, 2s - 1) at r + rmax, r = i - j
+    int rmax, c0, W;
+};
 template <typename... P> constexpr bool kHasBias = (std::is_same_v<P, const float*> || ...);
 template <typename... P> constexpr bool kHasKeyLimit = (std::is_same_v<P, KeyLimit> || ...);
+template <typename... P> constexpr bool kHasDis = (std::is_same_v<P, Disentangled> || ...);
 constexpr int kRelMax = 127;                  // |j - i| >= 127 all fall in MPNet's last bucket (distance >= 91)
 constexpr int kRelSpan = 2 * kRelMax + 1;
 template <int DH, int MINB, int NW = kAttWarps, bool CLS = false, typename... RelBias>  // NW warps = 16 * NW query rows per CTA
@@ -356,6 +367,24 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
                     }
                 }
             }
+            if constexpr (kHasDis<RelBias...>) {
+                const Disentangled dis = (rel_bias, ...);
+                const size_t rs = static_cast<size_t>(gridDim.x) * dis.W;     // heads * W floats per row
+                const int ia = CLS ? 0 : min(r0 + g, S - 1), ib = CLS ? 0 : min(r0 + g + 8, S - 1);
+                const float* c2a = dis.c2p + static_cast<size_t>(CLS ? b : t0 + ia) * rs + h * dis.W - dis.c0;
+                const float* c2b = dis.c2p + static_cast<size_t>(CLS ? b : t0 + ib) * rs + h * dis.W - dis.c0;
+#pragma unroll
+                for (int n = 0; n < 4; ++n) {
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const int j = min(sb0 + kb0 + n * 8 + 2 * t + c, S - 1);
+                        const float* p2 = dis.p2c + static_cast<size_t>(t0 + j) * rs + h * dis.W - dis.c0;
+                        const int ca = __ldg(dis.cidx + ia - j + dis.rmax), cb = __ldg(dis.cidx + ib - j + dis.rmax);
+                        sacc[n][c] += __ldg(c2a + ca) + __ldg(p2 + ca);
+                        sacc[n][2 + c] += __ldg(c2b + cb) + __ldg(p2 + cb);
+                    }
+                }
+            }
             float bm0 = -INFINITY, bm1 = -INFINITY;
             if (kb0 + 32 > nk) {                     // only the last key block holds keys past the sequence end
 #pragma unroll
@@ -488,13 +517,14 @@ __global__ void __launch_bounds__(256) pool_kernel(const __half* __restrict__ hi
     for (int d = threadIdx.x; d < H; d += blockDim.x, ++nv) out[static_cast<size_t>(b) * H + d] = vals[nv] * inv;
 }
 
-// BertPooler (tanh(W_p h_cls + b_p)) + classifier -> logits [B, num_labels].  An empty sequence has h_cls = 0 (its row
+// BertPooler (tanh(W_p h_cls + b_p)) + classifier -> logits [B, num_labels]; head_act RMU_HEAD_GELU: DeBERTa's ContextPooler,
+// erf-GELU in place of tanh.  An empty sequence has h_cls = 0 (its row
 // cu[b] belongs to the next sequence, or lies past T).  compact: h_cls of sequence b is row b of [B, H] planes.
 __global__ void __launch_bounds__(256) cls_head_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo,
                                                        const int* __restrict__ cu, int H, int num_labels, int compact,
                                                        const float* __restrict__ pw, const float* __restrict__ pb,
                                                        const float* __restrict__ cw, const float* __restrict__ cb,
-                                                       float* __restrict__ out) {
+                                                       int head_act, float* __restrict__ out) {
     extern __shared__ float sh[];   // h[H], pooled[H]
     float* hcls = sh;
     float* pooled = sh + H;
@@ -509,7 +539,10 @@ __global__ void __launch_bounds__(256) cls_head_kernel(const __half* __restrict_
         float s = 0.f;
         for (int d = lane_id(); d < H; d += 32) s = fmaf(wr[d], hcls[d], s);
         for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-        if (lane_id() == 0) pooled[j] = tanhf(s + pb[j]);
+        if (lane_id() == 0) {
+            const float x = s + pb[j];
+            pooled[j] = head_act == RMU_HEAD_GELU ? gelu_erf(x) : tanhf(x);
+        }
     }
     __syncthreads();
     for (int c = warp; c < num_labels; c += nw) {
@@ -558,15 +591,22 @@ constexpr int kClsAttWarps = 4;
 // kernel are those of one launch, so the heads of a sequence still run together and every row is computed the same.
 // rel_bias non-null: the [heads, kRelSpan] table of build_relative_bias_table is added to every score (warps must be 10).
 // nkeys non-null ([B] int32, full mode without a bias): sequence b attends to its first min(max(nkeys[b], 1), S_b) rows.
+// dis non-null (DeBERTa-v2, d_h = 64, neither a bias nor a key limit): the position terms of launch_position_terms are
+// added to every score (warps must be 10); in CLS mode its c2p rows are the compact CLS rows, offset here per slice.
 constexpr int kMaxGridY = 65535;
 static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __half* cls_q_hi, const __half* cls_q_lo,
                             const int* cu, int B, int H, int heads, int max_seqlen, int warps, __half* ctx_hi,
-                            __half* ctx_lo, cudaStream_t st, const float* rel_bias = nullptr, const int* nkeys = nullptr) {
+                            __half* ctx_lo, cudaStream_t st, const float* rel_bias = nullptr, const int* nkeys = nullptr,
+                            const Disentangled* dis = nullptr) {
     const int DH = H / heads;
     const bool cls = cls_q_hi != nullptr;
     const bool bias = rel_bias != nullptr;
     if (nkeys && (cls || bias)) {
         set_error("attention: a key limit runs on every query row and without a relative bias");
+        return RMU_ERR_ARG;
+    }
+    if (dis && (bias || nkeys || DH != 64 || (!cls && warps != kAttWarps))) {
+        set_error("attention: the disentangled position terms run with head_dim 64 and 10 warps, without a bias or key limit");
         return RMU_ERR_ARG;
     }
     if (cls) warps = kClsAttWarps;
@@ -592,7 +632,10 @@ static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __
     auto lkern = DH == 32 ? (warps == 5 ? attention_planes_kernel<32, 4, 5, false, KeyLimit>
                                         : attention_planes_kernel<32, 2, kAttWarps, false, KeyLimit>)
                           : attention_planes_kernel<64, 1, kAttWarps, false, KeyLimit>;
-    if (bias) RMU_CUDA(cudaFuncSetAttribute(bkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
+    auto dkern = cls ? attention_planes_kernel<64, 2, kClsAttWarps, true, Disentangled>
+                     : attention_planes_kernel<64, 1, kAttWarps, false, Disentangled>;
+    if (dis) RMU_CUDA(cudaFuncSetAttribute(dkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
+    else if (bias) RMU_CUDA(cudaFuncSetAttribute(bkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
     else if (nkeys) RMU_CUDA(cudaFuncSetAttribute(lkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
     else RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
     for (int s0 = 0; s0 < B; s0 += kMaxGridY) {
@@ -600,7 +643,12 @@ static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __
         // full mode addresses Q and the context by token (cu[b] is absolute), CLS mode by sequence
         const size_t roff = cls ? static_cast<size_t>(s0) * H : 0;
         dim3 pg(static_cast<unsigned>(heads), static_cast<unsigned>(nb), zblocks);
-        if (nkeys)
+        if (dis) {
+            Disentangled d = *dis;
+            if (cls) d.c2p += static_cast<size_t>(s0) * heads * d.W;
+            dkern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, cls ? cls_q_hi + roff : nullptr, cls ? cls_q_lo + roff : nullptr,
+                                                cu + s0, H, ksb, ctx_hi + roff, ctx_lo + roff, d);
+        } else if (nkeys)
             lkern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, nullptr, nullptr, cu + s0, H, ksb, ctx_hi, ctx_lo,
                                                 KeyLimit{nkeys + s0});
         else if (bias)
@@ -653,9 +701,11 @@ static int launch_pool(const __half* hi, const __half* lo, const int* cu, int B,
 
 // E4 cls_head_kernel: one 256-thread block per sequence, h_cls and the pooled vector in shared memory -> out [B, num_labels]
 static int launch_cls_head(const __half* hi, const __half* lo, const int* cu, int B, int H, int num_labels, bool compact,
-                           const float* pw, const float* pb, const float* cw, const float* cb, float* out, cudaStream_t st) {
+                           const float* pw, const float* pb, const float* cw, const float* cb, float* out, cudaStream_t st,
+                           int head_act = RMU_HEAD_TANH) {
     ProfScope _ps(PROF_POOL_HEAD, st);
-    cls_head_kernel<<<B, 256, 2 * H * sizeof(float), st>>>(hi, lo, cu, H, num_labels, compact ? 1 : 0, pw, pb, cw, cb, out);
+    cls_head_kernel<<<B, 256, 2 * H * sizeof(float), st>>>(hi, lo, cu, H, num_labels, compact ? 1 : 0, pw, pb, cw, cb,
+                                                           head_act, out);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
@@ -707,6 +757,142 @@ static void build_relative_bias_table(const float* bias, int heads, float* out) 
     for (int h = 0; h < heads; ++h)
         for (int r = -kRelMax; r <= kRelMax; ++r)
             out[static_cast<size_t>(h) * kRelSpan + r + kRelMax] = bias[relative_bucket(r) * heads + h] * 1.4426950408889634f;
+}
+
+// ---------------------------------------------------------------------------------------------------- DeBERTa-v2
+// transformers' make_log_bucket_position(r, s, max_position) in its float32 arithmetic: r itself for |r| <= s / 2, else
+// sign(r) (ceil(log(|r| / mid) / log((max_position - 1) / mid) (mid - 1)) + mid).  Built on the host only: a ceil
+// boundary can flip with a device logf.
+static int log_bucket(int r, int s, int max_position) {
+    const int mid = s / 2;
+    const int a = r < 0 ? -r : r;
+    if (a <= mid) return r;
+    const float lp = ceilf(logf(static_cast<float>(a) / static_cast<float>(mid)) /
+                           logf(static_cast<float>(static_cast<double>(max_position - 1) / mid)) * static_cast<float>(mid - 1)) +
+                     static_cast<float>(mid);
+    return r < 0 ? -static_cast<int>(lp) : static_cast<int>(lp);
+}
+
+// the row of the relative embeddings query i uses for key j: cidx[r + rmax] = clamp(s + bucket(r), 0, 2s - 1), r = i - j
+// in [-rmax, rmax].  It is non-decreasing in r (bucket is).
+static void build_position_index(int s, int max_position, int rmax, int* cidx) {
+    for (int r = -rmax; r <= rmax; ++r) cidx[r + rmax] = std::min(std::max(s + log_bucket(r, s, max_position), 0), 2 * s - 1);
+}
+
+// P1 position_terms_kernel: out[r, h, w] = a_r,h . p_(c0 + w),h over the head's DH columns, fp32 (hi + lo of both operands
+// joined), for r < rows and w < W.  a: split planes with row pitch a_ld (the Q or K columns of the QKV planes, or the
+// compact CLS Q planes); p: the PQ' | PK planes [2s, 2H], pitch p_ld, starting at the wanted half.  A CTA computes 32
+// rows x 64 relative positions of one head; a thread two rows x four positions, each an fmaf chain over d in order.
+constexpr int kPosRows = 32, kPosCols = 64;
+template <int DH>
+__global__ void __launch_bounds__(256) position_terms_kernel(const __half* __restrict__ a_hi, const __half* __restrict__ a_lo,
+                                                             size_t a_ld, int rows, const __half* __restrict__ p_hi,
+                                                             const __half* __restrict__ p_lo, size_t p_ld, int c0, int W,
+                                                             float* __restrict__ out) {
+    __shared__ float As[kPosRows][DH + 1];
+    __shared__ float Ps[kPosCols][DH + 1];
+    const int h = blockIdx.z, heads = gridDim.z;
+    const int r0 = blockIdx.y * kPosRows, w0 = blockIdx.x * kPosCols;
+    for (int e = threadIdx.x; e < kPosRows * DH; e += blockDim.x) {
+        const int r = e / DH, d = e % DH;
+        float v = 0.f;
+        if (r0 + r < rows) {
+            const size_t o = static_cast<size_t>(r0 + r) * a_ld + h * DH + d;
+            v = __half2float(a_hi[o]) + __half2float(a_lo[o]);
+        }
+        As[r][d] = v;
+    }
+    for (int e = threadIdx.x; e < kPosCols * DH; e += blockDim.x) {
+        const int w = e / DH, d = e % DH;
+        float v = 0.f;
+        if (w0 + w < W) {
+            const size_t o = static_cast<size_t>(c0 + w0 + w) * p_ld + h * DH + d;
+            v = __half2float(p_hi[o]) + __half2float(p_lo[o]);
+        }
+        Ps[w][d] = v;
+    }
+    __syncthreads();
+    const int tr = threadIdx.x >> 4, tc = threadIdx.x & 15;     // rows tr, tr + 16; positions tc + 16 k
+    float acc[2][4] = {};
+#pragma unroll 8
+    for (int d = 0; d < DH; ++d) {
+        const float x0 = As[tr][d], x1 = As[tr + 16][d];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const float p = Ps[tc + 16 * k][d];
+            acc[0][k] = fmaf(x0, p, acc[0][k]);
+            acc[1][k] = fmaf(x1, p, acc[1][k]);
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int r = r0 + tr + 16 * i;
+        if (r >= rows) continue;
+        float* o = out + (static_cast<size_t>(r) * heads + h) * W + w0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            if (w0 + tc + 16 * k < W) o[tc + 16 * k] = acc[i][k];
+    }
+}
+
+// P1 on `rows` rows of a (row pitch a_ld) against the p half (PK for C2P, PQ' for P2C) -> out [rows, heads, W].
+// rows = 0 launches nothing.
+static int launch_position_terms(const __half* a_hi, const __half* a_lo, size_t a_ld, int rows, const __half* p_hi,
+                                 const __half* p_lo, size_t p_ld, int heads, int DH, int c0, int W, float* out,
+                                 cudaStream_t st) {
+    if (rows == 0) return RMU_OK;
+    if (DH != 64 || (rows + kPosRows - 1) / kPosRows > kMaxGridY) {
+        set_error("position terms: head_dim must be 64 and a call at most 65535 * 32 rows");
+        return RMU_ERR_ARG;
+    }
+    ProfScope _ps(PROF_ATTN, st);
+    dim3 grid(static_cast<unsigned>((W + kPosCols - 1) / kPosCols), static_cast<unsigned>((rows + kPosRows - 1) / kPosRows),
+              static_cast<unsigned>(heads));
+    position_terms_kernel<64><<<grid, 256, 0, st>>>(a_hi, a_lo, a_ld, rows, p_hi, p_lo, p_ld, c0, W, out);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// The relative positions a call with sequences of at most max_seqlen tokens reaches: c0 and W of cidx over
+// |r| <= max_seqlen - 1 (cidx spans [-rmax, rmax], rmax >= max_seqlen - 1).
+static void position_window(const int* cidx_h, int rmax, int max_seqlen, int* c0, int* W) {
+    const int m = std::max(std::min(max_seqlen - 1, rmax), 0);
+    *c0 = cidx_h[rmax - m];
+    *W = cidx_h[rmax + m] - *c0 + 1;
+}
+
+// E2 with DeBERTa's position terms on caller-owned planes: P1 twice into ws (C2P of the query rows, P2C of every key),
+// then E2 with the Disentangled pack.  pos planes [2s, 2H] = PQ' | PK; cidx_d (device) / cidx_h (host) from
+// build_position_index with rmax.  cls_q non-null: the compact Q planes [B, H] of the CLS rows.  ws holds
+// (qrows + T) heads W floats, qrows = B (CLS) or T.
+static int run_disentangled_attention(const __half* qkv_hi, const __half* qkv_lo, const __half* cls_q_hi,
+                                      const __half* cls_q_lo, const int* cu, int B, int T, int H, int heads, int max_seqlen,
+                                      const __half* pos_hi, const __half* pos_lo, const int* cidx_d, const int* cidx_h,
+                                      int rmax, float* ws, __half* ctx_hi, __half* ctx_lo, cudaStream_t st) {
+    const int DH = H / heads;
+    const bool cls = cls_q_hi != nullptr;
+    int c0 = 0, W = 0;
+    position_window(cidx_h, rmax, max_seqlen, &c0, &W);
+    const int qrows = cls ? B : T;
+    float* c2p = ws;
+    float* p2c = ws + static_cast<size_t>(qrows) * heads * W;
+    const size_t ld3 = static_cast<size_t>(3) * H, p_ld = static_cast<size_t>(2) * H;
+    int rc = cls ? launch_position_terms(cls_q_hi, cls_q_lo, H, B, pos_hi + H, pos_lo + H, p_ld, heads, DH, c0, W, c2p, st)
+                 : launch_position_terms(qkv_hi, qkv_lo, ld3, T, pos_hi + H, pos_lo + H, p_ld, heads, DH, c0, W, c2p, st);
+    if (rc != RMU_OK) return rc;
+    rc = launch_position_terms(qkv_hi + H, qkv_lo + H, ld3, T, pos_hi, pos_lo, p_ld, heads, DH, c0, W, p2c, st);
+    if (rc != RMU_OK) return rc;
+    const Disentangled dis{c2p, p2c, cidx_d, rmax, c0, W};
+    return launch_attention(qkv_hi, qkv_lo, cls_q_hi, cls_q_lo, cu, B, H, heads, max_seqlen, kAttWarps, ctx_hi, ctx_lo, st,
+                            nullptr, nullptr, &dis);
+}
+
+// floats of run_disentangled_attention's workspace
+static size_t position_ws_floats(const int* cidx_h, int rmax, int max_seqlen, int qrows, int T, int heads) {
+    int c0 = 0, W = 0;
+    position_window(cidx_h, rmax, max_seqlen, &c0, &W);
+    return (static_cast<size_t>(qrows) + T) * heads * W;
 }
 
 // ---------------------------------------------------------------------------------------------------- ColBERT
@@ -797,10 +983,12 @@ struct EncLayer {
     float *ln1g = nullptr, *ln1b = nullptr, *ln2g = nullptr, *ln2b = nullptr;
     SplitOperand D1, D2;                  // adapter_dim > 0: X-MOD's language adapter, dense1 [A, H] and dense2 [H, A]
     float *d1 = nullptr, *d2 = nullptr;
+    __half *pos_hi = nullptr, *pos_lo = nullptr;   // position_buckets > 0: PQ' | PK planes [2s, 2H] of the layer
 };
 
 struct rmu_encoder {
     rmu_bert_config cfg{};
+    rmu_encoder_ext ext{};                // DeBERTa's fields, zero for every other model
     int has_head = 0, sms = 0, device = 0;
     std::vector<void*> allocs;
     float *word = nullptr, *pos = nullptr, *typ = nullptr, *eg = nullptr, *eb = nullptr;
@@ -817,6 +1005,12 @@ struct rmu_encoder {
     SplitOperand X_cls, Q_cls, CTX_cls, X1_cls, FF_cls;
     float* PRE_cls = nullptr;
     SplitOperand FFA, FFA_cls;            // adapter_dim > 0: the FF / FF_cls planes seen as [rows, adapter_dim]
+    // position_buckets > 0 (DeBERTa): cidx over |i - j| <= max_pos - 1 (host copy and device table), and the position
+    // terms' workspace, grown under mu
+    std::vector<int> cidx_h;
+    int* cidx = nullptr;
+    float* pos_ws = nullptr;
+    size_t pos_ws_cap = 0;
     // staging of the *_host entry points: owned by host_mu alone (NOT part of the activation workspace, which a
     // concurrent device-pointer caller may free and re-allocate under mu)
     int *d_ids = nullptr, *d_typ = nullptr, *d_cu = nullptr;
@@ -867,6 +1061,23 @@ static void free_acts(rmu_encoder* e) {
     for (void* p : e->act_allocs) cudaFree(p);
     e->act_allocs.clear();
     e->tok_cap = 0;
+    cudaFree(e->pos_ws);
+    e->pos_ws = nullptr;
+    e->pos_ws_cap = 0;
+}
+
+// DeBERTa: the position terms' workspace for a call (qrows query rows, T keys), grown to fit
+static int ensure_position_ws(rmu_encoder* e, int qrows, int T, int max_seqlen) {
+    const int rmax = e->cfg.max_pos - 1;
+    const size_t need = position_ws_floats(e->cidx_h.data(), rmax, max_seqlen, qrows, T, e->cfg.heads);
+    if (need <= e->pos_ws_cap) return RMU_OK;
+    RMU_CUDA(cudaDeviceSynchronize());
+    cudaFree(e->pos_ws);
+    e->pos_ws = nullptr;
+    e->pos_ws_cap = 0;
+    RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->pos_ws), need * sizeof(float)));
+    e->pos_ws_cap = need;
+    return RMU_OK;
 }
 
 static int ensure_tokens(rmu_encoder* e, int T, int B) {
@@ -948,8 +1159,16 @@ static int run_last_layer_cls(rmu_encoder* e, const EncLayer& L, const int32_t* 
     g.M = B; g.N = H; g.K = H; g.bias = L.bqkv; g.out_hi = e->Q_cls.hi; g.out_lo = e->Q_cls.lo; g.qcols = H; g.qscale = qscale;
     rc = launch_gemm(GEMM_BIAS_SPLIT_QSCALE, e->X_cls, e->last_wq, g, e->sms, st);
     if (rc != RMU_OK) return rc;
-    rc = launch_attention(e->QKVP.hi, e->QKVP.lo, e->Q_cls.hi, e->Q_cls.lo, cu, B, H, c.heads, max_seqlen, 0, e->CTX_cls.hi,
-                          e->CTX_cls.lo, st, e->rel);
+    if (e->ext.position_buckets > 0) {
+        rc = ensure_position_ws(e, B, T, max_seqlen);
+        if (rc == RMU_OK)
+            rc = run_disentangled_attention(e->QKVP.hi, e->QKVP.lo, e->Q_cls.hi, e->Q_cls.lo, cu, B, T, H, c.heads, max_seqlen,
+                                            L.pos_hi, L.pos_lo, e->cidx, e->cidx_h.data(), c.max_pos - 1, e->pos_ws,
+                                            e->CTX_cls.hi, e->CTX_cls.lo, st);
+    } else {
+        rc = launch_attention(e->QKVP.hi, e->QKVP.lo, e->Q_cls.hi, e->Q_cls.lo, cu, B, H, c.heads, max_seqlen, 0, e->CTX_cls.hi,
+                              e->CTX_cls.lo, st, e->rel);
+    }
     if (rc != RMU_OK) return rc;
     g = GemmParams{};
     g.M = B; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE_cls; g.res_hi = e->X_cls.hi; g.res_lo = e->X_cls.lo;
@@ -992,9 +1211,9 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
     rc = launch_embed_ln(ids, type_ids, cu, B, T, H, c.vocab_size, c.max_pos, c.type_vocab, e->word, e->pos, e->typ, e->eg,
                          e->eb, c.ln_eps, e->X.hi, e->X.lo, st, c.position_mode);
     if (rc != RMU_OK) return rc;
-    const float scale = 1.0f / sqrtf(static_cast<float>(DH));
-    // q (scaled by 1/sqrt(dh)), k, v leave the GEMM as split fp16 planes: attention does no conversions
-    // (the softmax runs in base 2: q also carries log2(e))
+    // q (scaled by 1/sqrt(dh), DeBERTa's three score terms by 1/sqrt(3 dh)), k, v leave the GEMM as split fp16 planes:
+    // attention does no conversions (the softmax runs in base 2: q also carries log2(e))
+    const float scale = 1.0f / sqrtf(static_cast<float>(e->ext.position_buckets > 0 ? 3 * DH : DH));
     const float qscale = scale * 1.4426950408889634f;
     if (cls_only && c.layers == 0) return launch_gather_cls_rows(e->X.hi, e->X.lo, cu, B, H, e->X_cls.hi, e->X_cls.lo, st);
     for (int l = 0; l < c.layers; ++l) {
@@ -1007,9 +1226,17 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
         if (rc != RMU_OK) return rc;
         // RMU_ATTN_WARPS = 5: 80-row CTAs, four per SM (same warps/SM, K/V staged twice per 147-token sequence)
         static const int nw_env = [] { const char* e = getenv("RMU_ATTN_WARPS"); return e ? atoi(e) : kAttWarps; }();
-        rc = launch_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, H, c.heads, max_seqlen,
-                              (nw_env == 5 && DH == 32 && !e->rel) ? 5 : kAttWarps, e->CTX.hi, e->CTX.lo, st, e->rel,
-                              nkeys);
+        if (e->ext.position_buckets > 0) {
+            rc = ensure_position_ws(e, T, T, max_seqlen);
+            if (rc == RMU_OK)
+                rc = run_disentangled_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, T, H, c.heads, max_seqlen,
+                                                L.pos_hi, L.pos_lo, e->cidx, e->cidx_h.data(), c.max_pos - 1, e->pos_ws,
+                                                e->CTX.hi, e->CTX.lo, st);
+        } else {
+            rc = launch_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, H, c.heads, max_seqlen,
+                                  (nw_env == 5 && DH == 32 && !e->rel) ? 5 : kAttWarps, e->CTX.hi, e->CTX.lo, st, e->rel,
+                                  nkeys);
+        }
         if (rc != RMU_OK) return rc;
         g = GemmParams{};
         g.M = T; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE; g.res_hi = e->X.hi; g.res_lo = e->X.lo;
@@ -1043,7 +1270,13 @@ static int check_batch(const rmu_encoder* e, const void* ids, const void* cu, in
 extern "C" {
 
 int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* w, int n_weights, int has_head, rmu_encoder** out) {
+    return rmu_encoder_create_ex(cfg, nullptr, w, n_weights, has_head, out);
+}
+
+int rmu_encoder_create_ex(const rmu_bert_config* cfg, const rmu_encoder_ext* ext_in, const float* const* w, int n_weights,
+                          int has_head, rmu_encoder** out) {
     if (!cfg || !w || !out) { set_error("rmu_encoder_create: bad argument"); return RMU_ERR_ARG; }
+    const rmu_encoder_ext ext = ext_in ? *ext_in : rmu_encoder_ext{};
     const int H = cfg->hidden, F = cfg->ffn, L = cfg->layers;
     if (cfg->position_mode != RMU_POS_ABSOLUTE && cfg->position_mode != RMU_POS_OFFSET) {
         set_error("rmu_encoder_create: position_mode must be RMU_POS_ABSOLUTE (0) or RMU_POS_OFFSET (1)");
@@ -1058,13 +1291,35 @@ int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* w, int n_
         set_error("rmu_encoder_create: adapter_dim must be 0 (no adapter) or a multiple of 128 no larger than ffn");
         return RMU_ERR_UNSUPPORTED;
     }
+    if (ext.head_act != RMU_HEAD_TANH && ext.head_act != RMU_HEAD_GELU) {
+        set_error("rmu_encoder_create: head_act must be RMU_HEAD_TANH (0) or RMU_HEAD_GELU (1)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    const int PB = ext.position_buckets, MRP = ext.max_relative_positions;
+    if (PB < 0 || (PB == 0 && MRP != 0) || PB > 4096) {
+        set_error("rmu_encoder_create: position_buckets must be 0 (with max_relative_positions 0) or 1..4096");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (PB > 0 && (PB < 2 || MRP < PB / 2 + 2)) {
+        set_error("rmu_encoder_create: position_buckets needs at least 2 buckets and max_relative_positions >= "
+                  "position_buckets / 2 + 2");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (PB > 0 && (cfg->rel_buckets != 0 || A != 0 || cfg->heads <= 0 || H % cfg->heads != 0 || H / cfg->heads != 64)) {
+        set_error("rmu_encoder_create: disentangled attention (position_buckets > 0) runs with head_dim 64, without "
+                  "rel_buckets or an adapter");
+        return RMU_ERR_UNSUPPORTED;
+    }
     const bool rel = cfg->rel_buckets == 32;
     const int adapter0 = 5 + 16 * L + (has_head ? 4 : 0) + (rel ? 1 : 0);   // the adapter tensors come last
-    const int expect = adapter0 + (A > 0 ? 4 * L : 0);
+    const int pos0 = adapter0 + (A > 0 ? 4 * L : 0);                           // then DeBERTa's relative embeddings
+    const int expect = pos0 + (PB > 0 ? 3 : 0);
     if (n_weights != expect) { set_error("rmu_encoder_create: expected " + std::to_string(expect) + " weight tensors"); return RMU_ERR_ARG; }
     if (rel && !w[adapter0 - 1]) { set_error("rmu_encoder_create: null relative attention bias"); return RMU_ERR_ARG; }
-    for (int j = adapter0; j < expect; ++j)
+    for (int j = adapter0; j < pos0; ++j)
         if (!w[j]) { set_error("rmu_encoder_create: null adapter tensor"); return RMU_ERR_ARG; }
+    for (int j = pos0; j < expect; ++j)
+        if (!w[j]) { set_error("rmu_encoder_create: null relative embedding or LN_rel tensor"); return RMU_ERR_ARG; }
     if (H % 128 != 0 || F % 128 != 0 || H > 1024 || cfg->heads <= 0 || H % cfg->heads != 0 ||
         (H / cfg->heads != 32 && H / cfg->heads != 64)) {
         set_error("rmu_encoder_create: unsupported shape (hidden/ffn multiples of 128, hidden <= 1024, head_dim 32 or 64)");
@@ -1102,6 +1357,7 @@ int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* w, int n_
     }
     rmu_encoder* e = new rmu_encoder();
     e->cfg = *cfg;
+    e->ext = ext;
     e->has_head = has_head;
     if (cudaGetDevice(&e->device) != cudaSuccess || (e->sms = device_sm_count()) <= 0 ||
         cudaEventCreateWithFlags(&e->ws_done, cudaEventDisableTiming) != cudaSuccess) {
@@ -1171,6 +1427,46 @@ int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* w, int n_
         ++i;
         up(&Ly.d2, H);
     }
+    if (PB > 0 && rc == RMU_OK) {
+        // R = LN_rel(rel_embeddings) once; per layer PQ' | PK = split((R [Wq; Wk]^T + [bq; bk]) * (col < H ? qscale : 1)),
+        // the QKV epilogue's arithmetic on R, with q's scale log2(e) / sqrt(3 d_h)
+        const int R2 = 2 * PB;
+        float *rel_f = nullptr, *lng = nullptr, *lnb = nullptr;
+        i = pos0;
+        up(&rel_f, static_cast<size_t>(R2) * H);
+        up(&lng, H);
+        up(&lnb, H);
+        SplitOperand Rp;
+        __half *rh = nullptr, *rl = nullptr;
+        if (rc == RMU_OK) rc = dev_alloc(e->allocs, &rh, static_cast<size_t>(R2) * H);
+        if (rc == RMU_OK) rc = dev_alloc(e->allocs, &rl, static_cast<size_t>(R2) * H);
+        if (rc == RMU_OK) rc = launch_layernorm(rel_f, R2, H, lng, lnb, cfg->ln_eps, rh, rl, nullptr);
+        if (rc == RMU_OK) rc = make_split_operand(&Rp, rh, rl, R2, H);
+        const float qs = 1.4426950408889634f / sqrtf(static_cast<float>(3 * (H / cfg->heads)));
+        for (int l = 0; l < L && rc == RMU_OK; ++l) {
+            EncLayer& Ly = e->layers[l];
+            SplitOperand wqk;
+            rc = make_split_operand(&wqk, Ly.Wqkv.hi, Ly.Wqkv.lo, 2 * H, H);
+            if (rc == RMU_OK) rc = dev_alloc(e->allocs, &Ly.pos_hi, static_cast<size_t>(R2) * 2 * H);
+            if (rc == RMU_OK) rc = dev_alloc(e->allocs, &Ly.pos_lo, static_cast<size_t>(R2) * 2 * H);
+            if (rc != RMU_OK) break;
+            GemmParams g{};
+            g.M = R2; g.N = 2 * H; g.K = H; g.bias = Ly.bqkv; g.out_hi = Ly.pos_hi; g.out_lo = Ly.pos_lo; g.qcols = H; g.qscale = qs;
+            rc = launch_gemm(GEMM_BIAS_SPLIT_QSCALE, Rp, wqk, g, e->sms, nullptr);
+        }
+        if (rc == RMU_OK) {
+            const int rmax = cfg->max_pos - 1;
+            e->cidx_h.resize(2 * static_cast<size_t>(rmax) + 1);
+            build_position_index(PB, MRP, rmax, e->cidx_h.data());
+            rc = dev_alloc(e->allocs, &e->cidx, e->cidx_h.size());
+            if (rc == RMU_OK)
+                RMU_CUDA(cudaMemcpy(e->cidx, e->cidx_h.data(), e->cidx_h.size() * sizeof(int), cudaMemcpyHostToDevice));
+        }
+        if (rc == RMU_OK) {
+            const cudaError_t err = cudaDeviceSynchronize();
+            if (err != cudaSuccess) { set_error(std::string("rmu_encoder_create: ") + cudaGetErrorString(err)); rc = RMU_ERR_CUDA; }
+        }
+    }
     if (rc != RMU_OK) { rmu_encoder_destroy(e); return rc; }
     *out = e;
     return RMU_OK;
@@ -1213,7 +1509,7 @@ int rmu_encoder_classify(rmu_encoder* e, const int32_t* ids, const int32_t* type
     rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, true, st);
     if (rc != RMU_OK) return rc;
     rc = launch_cls_head(e->X_cls.hi, e->X_cls.lo, cu, B, e->cfg.hidden, e->cfg.num_labels, true, e->pw, e->pb, e->cw, e->cb,
-                         out, st);
+                         out, st, e->ext.head_act);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
@@ -1612,6 +1908,58 @@ int rmu_debug_attention_bias(const uint16_t* qkv_hi, const uint16_t* qkv_lo, con
                             static_cast<cudaStream_t>(stream), rel_table);
 }
 
+int rmu_log_bucket_table(int buckets, int max_position, int n, int32_t* out_h) {
+    if (!out_h || n < 1) { set_error("rmu_log_bucket_table: bad argument"); return RMU_ERR_ARG; }
+    if (buckets < 2 || max_position < buckets / 2 + 2) {
+        set_error("rmu_log_bucket_table: buckets must be at least 2 and max_position at least buckets / 2 + 2");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    for (int r = -(n - 1); r <= n - 1; ++r) out_h[r + n - 1] = log_bucket(r, buckets, max_position);
+    return RMU_OK;
+}
+
+int rmu_debug_attention_disentangled(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const uint16_t* cls_q_hi,
+                                     const uint16_t* cls_q_lo, const int32_t* cu, int B, int T, int H, int heads,
+                                     int max_seqlen, const uint16_t* pos_hi, const uint16_t* pos_lo, int position_buckets,
+                                     const int32_t* cidx_h, float* ws, int64_t ws_elems, uint16_t* ctx_hi, uint16_t* ctx_lo,
+                                     void* stream) {
+    if (!qkv_hi || !qkv_lo || !cu || !pos_hi || !pos_lo || !cidx_h || !ws || !ctx_hi || !ctx_lo ||
+        (!cls_q_hi) != (!cls_q_lo) || B <= 0 || T <= 0 || heads <= 0 || H <= 0 || max_seqlen <= 0 || ws_elems < 0 ||
+        position_buckets <= 0) {
+        set_error("rmu_debug_attention_disentangled: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H % heads != 0 || H / heads != 64) {
+        set_error("rmu_debug_attention_disentangled: head_dim must be 64");
+        return RMU_ERR_ARG;
+    }
+    const int rmax = max_seqlen - 1;
+    // P1 reads rows cidx_h[0] .. cidx_h[2 rmax] of the pos planes, which hold 2 position_buckets rows
+    for (int k = 0; k < 2 * rmax; ++k)
+        if (cidx_h[k + 1] < cidx_h[k] || cidx_h[k] < 0) {
+            set_error("rmu_debug_attention_disentangled: cidx must be non-negative and non-decreasing");
+            return RMU_ERR_ARG;
+        }
+    if (cidx_h[2 * rmax] >= 2 * position_buckets) {
+        set_error("rmu_debug_attention_disentangled: cidx reaches past the 2 * position_buckets rows of the pos planes");
+        return RMU_ERR_ARG;
+    }
+    const bool cls = cls_q_hi != nullptr;
+    const size_t terms = position_ws_floats(cidx_h, rmax, max_seqlen, cls ? B : T, T, heads);
+    if (static_cast<size_t>(ws_elems) < terms + 2 * static_cast<size_t>(rmax) + 1) {
+        set_error("rmu_debug_attention_disentangled: workspace too small");
+        return RMU_ERR_ARG;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int* cidx_d = reinterpret_cast<int*>(ws + terms);
+    RMU_CUDA(cudaMemcpyAsync(cidx_d, cidx_h, (2 * static_cast<size_t>(rmax) + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+    return run_disentangled_attention(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo),
+                                      reinterpret_cast<const __half*>(cls_q_hi), reinterpret_cast<const __half*>(cls_q_lo), cu,
+                                      B, T, H, heads, max_seqlen, reinterpret_cast<const __half*>(pos_hi),
+                                      reinterpret_cast<const __half*>(pos_lo), cidx_d, cidx_h, rmax, ws,
+                                      reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo), st);
+}
+
 int rmu_debug_pool(const uint16_t* hi, const uint16_t* lo, const int32_t* cu, int B, int H, int pool_mode, int normalize,
                    float* out, void* stream) {
     if (!hi || !lo || !cu || !out || B <= 0 || H <= 0 || (pool_mode != RMU_POOL_MEAN && pool_mode != RMU_POOL_CLS)) {
@@ -1638,6 +1986,35 @@ int rmu_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const int32_t* cu
     }
     return launch_cls_head(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), cu, B, H, num_labels,
                            false, pw, pb, cw, cb, out, static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_encoder_position_planes(const rmu_encoder* e, int layer, uint16_t* hi, uint16_t* lo, void* stream) {
+    if (!e || !hi || !lo || e->ext.position_buckets <= 0 || layer < 0 || layer >= e->cfg.layers) {
+        set_error("rmu_debug_encoder_position_planes: bad argument (an encoder with position_buckets > 0 and a layer of it)");
+        return RMU_ERR_ARG;
+    }
+    const EncLayer& L = e->layers[layer];
+    const size_t n = static_cast<size_t>(2) * e->ext.position_buckets * 2 * e->cfg.hidden * sizeof(__half);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    RMU_CUDA(cudaMemcpyAsync(hi, L.pos_hi, n, cudaMemcpyDeviceToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(lo, L.pos_lo, n, cudaMemcpyDeviceToDevice, st));
+    return RMU_OK;
+}
+
+int rmu_debug_cls_head_act(const uint16_t* hi, const uint16_t* lo, const int32_t* cu, int B, int H, int num_labels,
+                           const float* pw, const float* pb, const float* cw, const float* cb, int head_act, float* out,
+                           void* stream) {
+    if (!hi || !lo || !cu || !pw || !pb || !cw || !cb || !out || B <= 0 || H <= 0 || num_labels <= 0 ||
+        (head_act != RMU_HEAD_TANH && head_act != RMU_HEAD_GELU)) {
+        set_error("rmu_debug_cls_head_act: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H > 1024) {
+        set_error("rmu_debug_cls_head_act: hidden must be at most 1024");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_cls_head(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), cu, B, H, num_labels,
+                           false, pw, pb, cw, cb, out, static_cast<cudaStream_t>(stream), head_act);
 }
 
 int rmu_debug_split_planes(const float* src, int64_t n, uint16_t* hi, uint16_t* lo, void* stream) {

@@ -4,7 +4,8 @@ Weights go to the library in the canonical order of ``weights.weight_names`` (Hu
 ``BertModel`` tensor order: embeddings, then per layer q/k/v/attention-output/LayerNorm/
 intermediate/output/LayerNorm, then pooler + classifier when a head is present, then MPNet's
 relative attention bias [32, heads] when the config has one, then X-MOD's language adapter of every layer, for the
-config's one language, when it has ``adapter_dim > 0``).
+config's one language, when it has ``adapter_dim > 0``, then DeBERTa's relative embeddings and LN_rel when it has
+``position_buckets > 0``).
 """
 from __future__ import annotations
 
@@ -18,6 +19,16 @@ from .weights import BertConfig, weight_names
 
 POOL = {"mean": 0, "cls": 1}
 MAX_TOKENS_PER_CALL = 131072    # bounds the activation workspace (~19 KB/token for MiniLM shapes => ~2.5 GB)
+POSITION_WS_BYTES = 1 << 30     # DeBERTa: bound of the attention position terms' workspace, 2 T heads W fp32 per call
+
+
+def deberta_tokens_per_call(cfg: BertConfig) -> int:
+    """tokens per encoder call that keep DeBERTa's position terms (C2P and P2C, heads x W floats per token each, W at
+    most 2s relative positions) within POSITION_WS_BYTES; MAX_TOKENS_PER_CALL for every other model"""
+    if not cfg.position_buckets:
+        return MAX_TOKENS_PER_CALL
+    per_token = 2 * cfg.heads * 2 * cfg.position_buckets * 4
+    return max(1, min(MAX_TOKENS_PER_CALL, POSITION_WS_BYTES // per_token))
 
 
 class BertEncoder:
@@ -27,6 +38,7 @@ class BertEncoder:
         self.cfg = cfg
         self.with_head = bool(with_head)
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
+        self.max_tokens_per_call = deberta_tokens_per_call(cfg)
         names = weight_names(cfg, with_head)
         arrs = []
         for name, shape in names:
@@ -38,8 +50,13 @@ class BertEncoder:
         cc = _lib.bert_config_c(cfg)
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().rmu_encoder_create(C.byref(cc), ptrs, len(arrs), int(self.with_head), C.byref(self._h)),
-                       "rmu_encoder_create")
+            if cfg.position_buckets or cfg.head_act:
+                ext = _lib.encoder_ext_c(cfg)
+                _lib.check(_lib.lib().rmu_encoder_create_ex(C.byref(cc), C.byref(ext), ptrs, len(arrs), int(self.with_head),
+                                                            C.byref(self._h)), "rmu_encoder_create_ex")
+            else:
+                _lib.check(_lib.lib().rmu_encoder_create(C.byref(cc), ptrs, len(arrs), int(self.with_head),
+                                                         C.byref(self._h)), "rmu_encoder_create")
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -122,7 +139,7 @@ class BertEncoder:
         typ = None if type_ids is None else np.ascontiguousarray(type_ids, dtype=np.int32)
         cu = np.ascontiguousarray(cu, dtype=np.int32)
         with self.torch.cuda.device(self.device):
-            for s, e in self._chunks(cu, MAX_TOKENS_PER_CALL):
+            for s, e in self._chunks(cu, self.max_tokens_per_call):
                 t0, t1 = int(cu[s]), int(cu[e])
                 sub_cu = np.ascontiguousarray(cu[s:e + 1] - cu[s], dtype=np.int32)
                 sub_ids = ids[t0:t1]
@@ -143,7 +160,7 @@ class BertEncoder:
         typ = None if type_ids is None else np.ascontiguousarray(type_ids, dtype=np.int32)
         cu = np.ascontiguousarray(cu, dtype=np.int32)
         with self.torch.cuda.device(self.device):
-            for s, e in self._chunks(cu, MAX_TOKENS_PER_CALL):
+            for s, e in self._chunks(cu, self.max_tokens_per_call):
                 t0, t1 = int(cu[s]), int(cu[e])
                 sub_cu = np.ascontiguousarray(cu[s:e + 1] - cu[s], dtype=np.int32)
                 sub_ids = ids[t0:t1]

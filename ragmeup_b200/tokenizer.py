@@ -144,11 +144,48 @@ def build_xlmr_unigram(pieces: Sequence[Tuple[str, float]]) -> Tokenizer:
     return tok
 
 
-def load_tokenizer(source: Optional[str], vocab_size: int = 30522, mpnet: bool = False, xlmr: bool = False) -> Tokenizer:
+DEBERTA_SPECIALS = ("[PAD]", "[CLS]", "[SEP]", "[UNK]")   # ids 0..3; "[MASK]" is the last id
+
+
+def synthetic_deberta_pieces(size: int = 128100) -> Tuple[Tuple[str, float], ...]:
+    """DeBERTa-v3's id layout ([PAD]=0, [CLS]=1, [SEP]=2, [UNK]=3, [MASK] last) over the pieces of
+    ``synthetic_xlmr_pieces(size)``"""
+    pieces = list(synthetic_xlmr_pieces(size))
+    pieces[:4] = [(t, 0.0) for t in DEBERTA_SPECIALS]
+    pieces[-1] = ("[MASK]", 0.0)
+    return tuple(pieces)
+
+
+def build_deberta_unigram(pieces: Sequence[Tuple[str, float]]) -> Tokenizer:
+    """DeBERTa-v3's tokenizer shape (``DebertaV2TokenizerFast``'s tokenizer.json): Unigram over ``pieces``, Metaspace
+    with ``prepend_scheme="first"``, templates ``[CLS] A [SEP]`` and ``[CLS] A [SEP] B [SEP]`` with type ids 0 / 1, and
+    the specials as added tokens."""
+    tok = Tokenizer(models.Unigram(list(pieces), unk_id=3, byte_fallback=False))
+    tok.pre_tokenizer = pre_tokenizers.Metaspace(replacement="▁", prepend_scheme="first")
+    tok.post_processor = processors.TemplateProcessing(
+        single="[CLS] $A [SEP]", pair="[CLS] $A [SEP] $B:1 [SEP]:1", special_tokens=[("[CLS]", 1), ("[SEP]", 2)])
+    tok.decoder = decoders.Metaspace(replacement="▁", prepend_scheme="first")
+    tok.add_special_tokens([*DEBERTA_SPECIALS, "[MASK]"])
+    return tok
+
+
+def load_tokenizer(source: Optional[str], vocab_size: int = 30522, mpnet: bool = False, xlmr: bool = False,
+                   deberta: bool = False) -> Tokenizer:
     """``source`` = snapshot dir (tokenizer.json or vocab.txt) or None -> synthetic vocab; ``mpnet`` selects MPNet's
-    vocabulary layout and templates where the snapshot has no tokenizer.json.  ``xlmr`` (XLM-R / RoBERTa): a snapshot
-    must have tokenizer.json (SentencePiece Unigram or byte-level BPE, read by ``tokenizers``); None -> the synthetic
-    Unigram vocabulary."""
+    vocabulary layout and templates where the snapshot has no tokenizer.json.  ``xlmr`` (XLM-R / RoBERTa) and
+    ``deberta`` (DeBERTa-v2 / v3): a snapshot must have tokenizer.json (read by ``tokenizers``); None -> the synthetic
+    Unigram vocabulary of that family."""
+    if deberta:
+        if source is None:
+            return build_deberta_unigram(synthetic_deberta_pieces(vocab_size))
+        tj = os.path.join(source, "tokenizer.json")
+        if os.path.exists(tj):
+            return Tokenizer.from_file(tj)
+        why = (f"{source}: DeBERTa-v2 snapshots need tokenizer.json (the sentencepiece package is not a dependency; "
+               f"saving the tokenizer with transformers' fast tokenizer writes it)")
+        if os.path.exists(os.path.join(source, "spm.model")):
+            raise ValueError(why + ", and this one has only spm.model")
+        raise FileNotFoundError(why)
     if xlmr and source is None:
         return build_xlmr_unigram(synthetic_xlmr_pieces(vocab_size))
     build = build_mpnet_wordpiece if mpnet else build_wordpiece

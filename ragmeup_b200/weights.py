@@ -42,6 +42,10 @@ class BertConfig:
     position_mode: ClassVar[int] = 0
     rel_buckets: ClassVar[int] = 0
     adapter_dim: ClassVar[int] = 0
+    # no disentangled attention, BERT's tanh pooler
+    position_buckets: ClassVar[int] = 0
+    max_relative_positions: ClassVar[int] = 0
+    head_act: ClassVar[int] = 0
 
     @property
     def head_dim(self) -> int:
@@ -174,12 +178,90 @@ class XmodConfig(XLMRConfig):
         return XmodConfig(**asdict(base), adapter_dim=H // r, languages=languages, language=lang)
 
 
+@dataclass
+class DebertaConfig(BertConfig):
+    """DeBERTa-v2 / v3 (transformers ``DebertaV2Model``; mxbai-rerank-*-v1, cross-encoder/nli-deberta-v3-*): BERT's
+    post-LN encoder with disentangled attention and no absolute positions or token types.  Every score adds
+    ``Q_i . PK[c] + K_j . PQ[c]``, with ``PQ`` / ``PK`` the layer's own query / key projections (biases included) of
+    ``R = LN_rel(rel_embeddings[0:2s])`` and ``c = clamp(s + bucket(i - j), 0, 2s - 1)``, and the three terms share the
+    scale ``1 / sqrt(3 d_h)``.  The encoder gets zero position [max_pos, H] and token-type [1, H] tables:
+    ``(w + 0) + 0 == w`` exactly.  The head is ContextPooler (erf-GELU) + classifier."""
+    vocab_size: int = 128100
+    max_pos: int = 512
+    type_vocab: int = 1
+    ln_eps: float = 1e-7
+    position_buckets: int = 256
+    max_relative_positions: int = 512
+    head_act: int = 1
+
+    @staticmethod
+    def from_hf(d: dict) -> "DebertaConfig":
+        """config.json of a ``deberta-v2`` checkpoint -> DebertaConfig; refuses, naming the field, what the encoder does
+        not compute"""
+        def refuse(field, why):
+            raise ValueError(f"deberta-v2 with {field} = {d.get(field)!r} is not supported: {why}")
+        if not d.get("relative_attention", False):
+            refuse("relative_attention", "the encoder runs DeBERTa with relative (disentangled) attention only")
+        if int(d.get("position_buckets", -1)) <= 0:
+            refuse("position_buckets", "the encoder runs log-bucketed relative positions (position_buckets > 0) only")
+        if not d.get("share_att_key", False):
+            refuse("share_att_key", "the position projections are the layer's own query / key projections")
+        pat = d.get("pos_att_type") or []
+        pat = pat.split("|") if isinstance(pat, str) else list(pat)
+        if sorted(x.strip().lower() for x in pat) != ["c2p", "p2c"]:
+            refuse("pos_att_type", "the encoder computes exactly the c2p and p2c terms")
+        if "layer_norm" not in [x.strip() for x in str(d.get("norm_rel_ebd", "none")).lower().split("|")]:
+            refuse("norm_rel_ebd", "the relative embeddings must pass the encoder's LayerNorm (layer_norm)")
+        if d.get("position_biased_input", True):
+            refuse("position_biased_input", "DeBERTa-v3 adds no absolute positions")
+        if int(d.get("type_vocab_size", 0)) > 0:
+            refuse("type_vocab_size", "DeBERTa-v3 has no token types")
+        if int(d.get("conv_kernel_size", 0)) > 0:
+            refuse("conv_kernel_size", "the ConvLayer of deberta-v2-xlarge is not computed")
+        H = int(d["hidden_size"])
+        if int(d.get("embedding_size", H)) != H:
+            refuse("embedding_size", f"it must equal hidden_size {H} (no embed_proj)")
+        for key in ("hidden_act", "pooler_hidden_act"):
+            if d.get(key, "gelu") != "gelu":
+                refuse(key, "only erf-GELU is computed")
+        max_pos = int(d.get("max_position_embeddings", 512))
+        mrp = int(d.get("max_relative_positions", -1))
+        return DebertaConfig(vocab_size=d["vocab_size"], hidden=H, layers=d["num_hidden_layers"],
+                             heads=d["num_attention_heads"], ffn=d["intermediate_size"], max_pos=max_pos,
+                             ln_eps=d.get("layer_norm_eps", 1e-7),
+                             num_labels=len(d["id2label"]) if "id2label" in d else d.get("num_labels", 1),
+                             position_buckets=int(d["position_buckets"]),
+                             max_relative_positions=mrp if mrp >= 1 else max_pos)
+
+
+REL_EMB = "encoder.rel_embeddings.weight"
+REL_LN = ("encoder.LayerNorm.weight", "encoder.LayerNorm.bias")
+
+
+def deberta_to_canonical(raw: Dict[str, np.ndarray], cfg: DebertaConfig) -> Dict[str, np.ndarray]:
+    """DeBERTa-v2 tensors (bare, or under ``deberta.`` as the sequence-classification model saves them) -> the
+    canonical names of ``weight_names``: ``query_proj`` / ``key_proj`` / ``value_proj`` -> ``query`` / ``key`` /
+    ``value``, zero position and token-type tables, rows 0..2s of ``rel_embeddings``; ``pooler.dense`` and
+    ``classifier`` keep their names."""
+    w: Dict[str, np.ndarray] = {}
+    for k, v in raw.items():
+        k = k[8:] if k.startswith("deberta.") else k
+        for a in ("query", "key", "value"):
+            k = k.replace(f"attention.self.{a}_proj.", f"attention.self.{a}.")
+        w[k] = np.ascontiguousarray(v, dtype=np.float32)
+    w["embeddings.position_embeddings.weight"] = np.zeros((cfg.max_pos, cfg.hidden), np.float32)
+    w["embeddings.token_type_embeddings.weight"] = np.zeros((1, cfg.hidden), np.float32)
+    if REL_EMB in w:
+        w[REL_EMB] = np.ascontiguousarray(w[REL_EMB][:2 * cfg.position_buckets])
+    return w
+
+
 def adapter_prefix(layer: int, language: str) -> str:
     return f"encoder.layer.{layer}.output.adapter_modules.{language}."
 
 
 # config.json model_type -> how the snapshot is read; a config without model_type is read as BERT
-MODEL_TYPES = ("bert", "mpnet", "roberta", "xlm-roberta", "xmod")
+MODEL_TYPES = ("bert", "mpnet", "roberta", "xlm-roberta", "xmod", "deberta-v2")
 
 
 # shapes of the models BASELINE.json / .env.template name (SURVEY.md §2.2 table)
@@ -213,6 +295,11 @@ PRESETS: Dict[str, Tuple[BertConfig, str, int]] = {
     "xmod-base": (XmodConfig(hidden=768, layers=12, heads=12, ffn=3072, adapter_dim=384), "mean", 512),
     "tiny-xmod": (XmodConfig(vocab_size=2000, hidden=256, layers=2, heads=4, ffn=512, max_pos=130, adapter_dim=128),
                   "mean", 64),
+    # DeBERTa-v3 rerankers (mixedbread-ai/mxbai-rerank-*-v1): position_buckets 256, max_position_embeddings 512
+    "mxbai-rerank-xsmall-v1": (DebertaConfig(hidden=384, layers=12, heads=6, ffn=1536), "cls", 512),
+    "mxbai-rerank-base-v1": (DebertaConfig(hidden=768, layers=12, heads=12, ffn=3072), "cls", 512),
+    "mxbai-rerank-large-v1": (DebertaConfig(hidden=1024, layers=24, heads=16, ffn=4096), "cls", 512),
+    "tiny-deberta": (DebertaConfig(vocab_size=2000, hidden=128, layers=2, heads=2, ffn=256), "cls", 512),
 }
 
 # presets whose sentence-transformers pipeline has no Normalize module
@@ -259,6 +346,8 @@ def weight_names(cfg: BertConfig, with_head: bool):
     if cfg.adapter_dim:
         for l in range(cfg.layers):
             names += adapter_names(cfg, l, cfg.language)
+    if cfg.position_buckets:
+        names += [(REL_EMB, (2 * cfg.position_buckets, H)), (REL_LN[0], (H,)), (REL_LN[1], (H,))]
     return names
 
 
@@ -327,8 +416,10 @@ def synthetic_bert_weights(cfg: BertConfig, seed: int = 0, with_head: bool = Fal
     for name, shape, rng in names:
         if name == REL_BIAS:                     # a few units across buckets, as trained MPNet biases spread
             a = rng.standard_normal(shape)
-        elif name == "embeddings.token_type_embeddings.weight" and isinstance(cfg, MPNetConfig):
-            a = np.zeros(shape)                    # MPNet has no token types (XLM-R's one row is trained)
+        elif name == "embeddings.token_type_embeddings.weight" and isinstance(cfg, (MPNetConfig, DebertaConfig)):
+            a = np.zeros(shape)                    # MPNet and DeBERTa have no token types (XLM-R's one row is trained)
+        elif name == "embeddings.position_embeddings.weight" and isinstance(cfg, DebertaConfig):
+            a = np.zeros(shape)                    # nor absolute positions (position_biased_input false)
         elif name.endswith("LayerNorm.weight"):
             a = 1.0 + 0.1 * rng.standard_normal(shape)
         elif name.endswith("LayerNorm.bias"):
@@ -385,16 +476,22 @@ def load_hf_snapshot(path: str, with_head: bool):
     kind = cfgd.get("model_type", "bert")
     if kind not in MODEL_TYPES:
         raise ValueError(f"{path}: model_type {kind!r} is not supported; the encoder runs {', '.join(MODEL_TYPES)}")
-    mpnet, xlmr = kind == "mpnet", kind in ("roberta", "xlm-roberta", "xmod")
+    mpnet, xlmr, deberta = kind == "mpnet", kind in ("roberta", "xlm-roberta", "xmod"), kind == "deberta-v2"
     if mpnet and with_head:
         raise ValueError(f"{path}: MPNet cross-encoders are not supported (MPNet runs as a sentence embedder only)")
+    if deberta and not with_head:
+        raise ValueError(f"{path}: model_type 'deberta-v2' runs as a cross-encoder (reranker) only, not as an embedder")
     if kind == "xmod":
         cfg = XmodConfig.from_hf(cfgd, path)
+    elif deberta:
+        cfg = DebertaConfig.from_hf(cfgd)
     else:
         cfg = MPNetConfig.from_hf(cfgd) if mpnet else XLMRConfig.from_hf(cfgd) if xlmr else BertConfig.from_hf(cfgd)
     raw = _load_tensors(path, _xmod_keep(cfg.language) if cfg.adapter_dim else None)
     if mpnet:
         w = mpnet_to_canonical(raw, cfg)
+    elif deberta:
+        w = deberta_to_canonical(raw, cfg)
     elif xlmr:
         w = xlmr_to_canonical(raw)
     else:
@@ -407,6 +504,12 @@ def load_hf_snapshot(path: str, with_head: bool):
     if missing:
         raise KeyError(f"{path}: missing tensors {missing[:4]}...")
     pooling, normalize, max_len = "mean", False, min(cfg.max_pos - cfg.position_offset, 512)
+    if deberta:
+        # CrossEncoder passes max_length=None: the tokenizer's model_max_length, within max_position_embeddings
+        max_len = cfg.max_pos
+        tc = _read_json(os.path.join(path, "tokenizer_config.json")) or {}
+        if tc.get("model_max_length") is not None:
+            max_len = min(int(tc["model_max_length"]), max_len)
     if xlmr:
         # CrossEncoder passes max_length=None, so the tokenizer's model_max_length applies [3P-recall]; positions end
         # at max_pos - 2 tokens either way (8192 for bge-m3 and bge-reranker-v2-m3)
@@ -454,12 +557,14 @@ def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] 
         cfg, pooling, max_len = PRESETS[preset]
         if isinstance(cfg, MPNetConfig) and with_head:
             raise ValueError(f"synthetic preset {preset!r} is MPNet: MPNet cross-encoders are not supported")
+        if isinstance(cfg, DebertaConfig) and not with_head:
+            raise ValueError(f"synthetic preset {preset!r}: model_type 'deberta-v2' runs as a cross-encoder only")
         cfg = type(cfg)(**asdict(cfg))
         if isinstance(cfg, XmodConfig):
             cfg.language = select_language(cfg.languages, cfg.language, model_name)
         w = synthetic_bert_weights(cfg, seed=seed, with_head=with_head, scale=scale)
         # an XLM-R preset scores as its checkpoint does: one label, no sbert_ce_default_activation_function -> sigmoid
-        act = "sigmoid" if with_head and isinstance(cfg, XLMRConfig) and cfg.num_labels == 1 else "identity"
+        act = "sigmoid" if with_head and isinstance(cfg, (XLMRConfig, DebertaConfig)) and cfg.num_labels == 1 else "identity"
         return cfg, w, pooling, preset not in UNNORMALIZED_PRESETS, max_len, act, None
     cands = [model_name]
     for root in (cache_folder, os.environ.get("RAGMEUP_MODEL_DIR")):
@@ -553,6 +658,9 @@ def load_colbert_snapshot(path: str):
     names are not read here].  An X-MOD backbone reads only its selected language's adapters.  MPNet is refused."""
     cfgd = _read_json(os.path.join(path, "config.json")) or {}
     kind = cfgd.get("model_type", "bert")
+    if kind == "deberta-v2":
+        raise ValueError(f"{path}: a ColBERT checkpoint of model_type 'deberta-v2' is not supported: DeBERTa runs as a "
+                         f"cross-encoder only")
     if kind not in ("bert", "xlm-roberta", "roberta", "xmod"):
         raise ValueError(f"{path}: a ColBERT checkpoint of model_type {kind!r} is not supported (bert, xlm-roberta, "
                          f"roberta and xmod are)")
@@ -620,6 +728,9 @@ def resolve_colbert(model_name: str, cache_folder: Optional[str] = None):
 
 
 def _refuse_xlmr_flashrank(cfg: BertConfig, where: str) -> None:
+    if isinstance(cfg, DebertaConfig):
+        raise ValueError(f"{where}: a DeBERTa-v2 (model_type 'deberta-v2') model is not a FlashRank model (FlashRank's "
+                         f"rerankers are BERT checkpoints); use HuggingFaceCrossEncoder for it")
     if isinstance(cfg, XLMRConfig):
         kind = "an X-MOD" if isinstance(cfg, XmodConfig) else "an XLM-R / RoBERTa"
         raise ValueError(f"{where}: {kind} model is not a FlashRank model (FlashRank's rerankers are BERT "
