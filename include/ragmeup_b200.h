@@ -223,6 +223,42 @@ int rmu_encoder_create(const rmu_bert_config* cfg, const float* const* weights_h
                        rmu_encoder** out);
 int rmu_encoder_create_ex(const rmu_bert_config* cfg, const rmu_encoder_ext* ext, const float* const* weights_h,
                           int n_weights, int has_head, rmu_encoder** out);
+
+/* ModernBERT (transformers ModernBertModel / ModernBertForSequenceClassification, model_type "modernbert"): a pre-LN
+ * encoder with rotary positions, a GeGLU feed-forward and sliding-window attention on the local layers.  With x the
+ * fp32 residual stream:
+ *   x = LN_emb(tok_embeddings[id]);  per layer l:  a = (l == 0 ? x : LN_a(x));  x += Wo attn(rope(Wqkv a)) + bo;
+ *   x += Wo2 (gelu(Wi_in m + bi_in) * (Wi_gate m + bi_gate)) + bo2 with m = LN_m(x);  hidden = LN_final(x).
+ * Wqkv [3H, H] holds q | k | v; q and k are rotated per head (x'[c] = x[c] cos - x[c + d/2] sin, x'[c + d/2] =
+ * x[c + d/2] cos + x[c] sin) with the cos / sin of the token's position within its sequence, taken from the global tables
+ * on layers with half_window 0 and from the local tables otherwise.  A layer with half_window w > 0 lets query i see key
+ * j iff |i - j| <= w.  The head (has_head): logits = classifier(LN_head(gelu(dense(p)))) with p the final hidden state's
+ * CLS row or mean over the sequence (`pooling`).  Every GELU is erf-GELU.  Absent biases and LayerNorm shifts are
+ * passed as zero arrays.
+ *
+ * weights_h (host fp32), in this order: tok_embeddings [V, H], embedding norm weight [H], bias [H]; per layer:
+ * attn_norm weight [H] and bias [H] (layer 0: not read, may be NULL), Wqkv [3H, H], bqkv [3H], attention Wo [H, H],
+ * bo [H], mlp_norm weight [H] and bias [H], Wi [2F, H] (rows 0..F the GELU input, F..2F the gate), bi [2F], mlp Wo
+ * [H, F], bo2 [H]; final_norm weight [H] and bias [H]; with has_head: head dense weight [H, H], bias [H], head norm
+ * weight [H], bias [H], classifier weight [num_labels, H], bias [num_labels]; then the rope tables cos_global,
+ * sin_global, cos_local, sin_local, each [max_pos, d_h / 2] (row p, column i = cos / sin of p * inv_freq[i], as the
+ * model computes them in float32).  3 + 12 layers + 2 (+ 6) + 4 tensors.
+ * cfg: vocab_size, hidden, layers, heads, ffn (= intermediate_size F), max_pos, num_labels and ln_eps (norm_eps) are
+ * read; type_vocab is not (token types are ignored).  Refused before any CUDA call: position_mode, rel_buckets or
+ * adapter_dim != 0, d_h other than 32 or 64, hidden not a multiple of 128 or above 1024, F % 64 != 0 and a head_form
+ * other than RMU_MB_HEAD_DENSE_GELU_LN (RMU_ERR_UNSUPPORTED); a negative half-window, a pooling other than CLS or mean,
+ * rope_rows != max_pos, rope_half != d_h / 2, a wrong tensor count or a null tensor (RMU_ERR_ARG); a GEMM weight with
+ * |w| >= 65520 (RMU_ERR_UNSUPPORTED).  Sequences may hold max_pos tokens.  The embed / classify / hidden entry points
+ * take such an encoder as any other; every layer runs on every row. */
+#define RMU_MB_HEAD_DENSE_GELU_LN 0
+typedef struct rmu_modernbert_ext {
+    const int32_t* half_window_h;   /* [layers] host: 0 = global attention, w > 0 = sliding window |i - j| <= w */
+    int32_t pooling;                /* the classifier's pooling: RMU_POOL_CLS or RMU_POOL_MEAN */
+    int32_t head_form;              /* RMU_MB_HEAD_DENSE_GELU_LN */
+    int32_t rope_rows, rope_half;   /* shape of each rope table: max_pos, d_h / 2 */
+} rmu_modernbert_ext;
+int rmu_encoder_create_modernbert(const rmu_bert_config* cfg, const rmu_modernbert_ext* mb, const float* const* weights_h,
+                                  int n_weights, int has_head, rmu_encoder** out);
 void rmu_encoder_destroy(rmu_encoder* enc);
 
 #define RMU_POOL_MEAN 0
@@ -303,6 +339,10 @@ int rmu_colbert_score_host(rmu_colbert* cb, const int32_t* q_ids_h, const int32_
 #define RMU_GEMM_BIAS_GELU_SPLIT 1    /* out planes = split(gelu_erf(A W^T + bias))                     */
 #define RMU_GEMM_BIAS_RESID_F32 2     /* out_f32 = A W^T + bias + (res_hi + res_lo)                     */
 #define RMU_GEMM_BIAS_SPLIT_QSCALE 3  /* out planes = split((A W^T + bias) * (col < qcols ? qscale : 1)) */
+#define RMU_GEMM_BIAS_SPLIT_ROPE 4    /* mode 3 with columns < 2 qcols (q, k) rotated per head at pos[row]      */
+#define RMU_GEMM_BIAS_GEGLU_SPLIT 5   /* W in 128-row blocks of 64 input | 64 gate rows: out planes [M, N / 2] =
+                                       * split(gelu_erf(in + b_in) * (gate + b_gate))                           */
+#define RMU_GEMM_BIAS_RESF32_F32 6    /* out_f32 = A W^T + bias + res_f32 (res_f32 may equal out_f32)            */
 
 /* For tests: E1 on A [a_rows, K] (rows M..a_rows are read by the TMA loads but never reach the output) and
  * W [N, K]; bias [N], res [M, N], out [M, N].  N % 128 == 0, K % 64 == 0, a_rows >= M.  max_ctas caps the
@@ -311,6 +351,24 @@ int rmu_debug_gemm(int mode, const uint16_t* a_hi, const uint16_t* a_lo, int64_t
                    const uint16_t* w_lo, int M, int N, int K, const float* bias, const uint16_t* res_hi,
                    const uint16_t* res_lo, int qcols, float qscale, int max_ctas, float* out_f32, uint16_t* out_hi,
                    uint16_t* out_lo, void* stream);
+/* For tests: E1 in the ModernBERT modes 4, 5 and 6, shapes as rmu_debug_gemm.  Mode 4: pos [M] int32 (device) is each
+ * row's position, clamped into the rope_cos / rope_sin tables [rope_rows, head_dim / 2] (device fp32); qcols (= H) is a
+ * multiple of 64 and of head_dim (32 or 64); out planes [M, N].  Mode 5: W as the mode describes it, out planes
+ * [M, N / 2].  Mode 6: res_f32 [M, N], out_f32 [M, N], which may be the same array.  Another mode returns RMU_ERR_ARG. */
+int rmu_debug_gemm_ex(int mode, const uint16_t* a_hi, const uint16_t* a_lo, int64_t a_rows, const uint16_t* w_hi,
+                      const uint16_t* w_lo, int M, int N, int K, const float* bias, const float* res_f32, int qcols,
+                      float qscale, const int32_t* pos, const float* rope_cos, const float* rope_sin, int rope_rows,
+                      int head_dim, int max_ctas, float* out_f32, uint16_t* out_hi, uint16_t* out_lo, void* stream);
+/* For tests: E2 with ModernBERT's sliding window, as a local layer runs it: key j is visible to query i iff
+ * |i - j| <= window (window > 0), 10 warps, every query row; otherwise as rmu_debug_attention.  With window >= the
+ * longest sequence - 1 the output equals rmu_debug_attention's bit for bit. */
+int rmu_debug_attention_window(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu_seqlens, int B, int H,
+                               int heads, int max_seqlen, int window, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream);
+/* For tests: ModernBERT's head on pooled rows [B, H] (device fp32): out [B, num_labels] = cw LN(gelu_erf(dense_w p +
+ * dense_b)) + cb, LN with norm_w, norm_b and eps.  1 <= H <= 1024. */
+int rmu_debug_modernbert_head(const float* pooled, int B, int H, int num_labels, const float* dense_w, const float* dense_b,
+                              const float* norm_w, const float* norm_b, float eps, const float* cw, const float* cb,
+                              float* out, void* stream);
 /* For tests: E2 on the QKV planes [T, 3H] of a ragged batch (q | k | v, q pre-scaled by log2(e) / sqrt(d_h) as the
  * QKV epilogue leaves it), cu_seqlens [B+1] int32 -> ctx planes [T, H].  d_h = H / heads is 32 or 64; warps is 10,
  * or 5 with d_h = 32. */

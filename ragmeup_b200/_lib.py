@@ -31,6 +31,11 @@ class EncoderExtC(C.Structure):
     _fields_ = [("position_buckets", C.c_int32), ("max_relative_positions", C.c_int32), ("head_act", C.c_int32)]
 
 
+class ModernBertExtC(C.Structure):
+    _fields_ = [("half_window_h", C.c_void_p), ("pooling", C.c_int32), ("head_form", C.c_int32), ("rope_rows", C.c_int32),
+                ("rope_half", C.c_int32)]
+
+
 def bert_config_c(cfg) -> BertConfigC:
     """weights.BertConfig (or a subclass) -> the C struct; adapter_dim is 0 for every family but X-MOD"""
     return BertConfigC(cfg.vocab_size, cfg.hidden, cfg.layers, cfg.heads, cfg.ffn, cfg.max_pos, cfg.type_vocab,
@@ -92,6 +97,8 @@ SIGNATURES = {
                                      C.POINTER(C.c_void_p)]),
     "rmu_encoder_create_ex": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(EncoderExtC), C.POINTER(C.c_void_p), C.c_int,
                                         C.c_int, C.POINTER(C.c_void_p)]),
+    "rmu_encoder_create_modernbert": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(ModernBertExtC), C.POINTER(C.c_void_p),
+                                                C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "rmu_encoder_destroy": (None, [C.c_void_p]),
     "rmu_encoder_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_void_p, C.c_void_p]),
@@ -143,6 +150,14 @@ SIGNATURES = {
                                  C.c_void_p]),
     "rmu_debug_cls_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_gemm_ex": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                    C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p]),
+    "rmu_debug_attention_window": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                             C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_modernbert_head": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_split_planes": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_join_planes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "rmu_debug_bm25_select": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

@@ -9,7 +9,9 @@ SURVEY Appendix A.5/A.6).  XLM-R / RoBERTa rerankers (the bge rerankers, this cl
 ``<s> q </s> </s> d </s>`` with no token types and truncate to ``min(model_max_length, max_pos - 2)``.  DeBERTa-v2 / v3
 rerankers (mxbai-rerank-*-v1) pair as ``[CLS] q [SEP] d [SEP]`` and send no token types (the model has none); they
 truncate to ``min(model_max_length, max_position_embeddings)`` and run in calls of at most ``deberta_tokens_per_call``
-tokens, which bounds the attention position terms' workspace.
+tokens, which bounds the attention position terms' workspace.  ModernBERT rerankers (gte-reranker-modernbert-base) pair
+the same way, send no token types and truncate to ``min(model_max_length, max_position_embeddings)`` (8192); their head
+pools by ``classifier_pooling`` (CLS or mean).
 A ColBERT checkpoint (colbert-ir/colbertv2.0, the reference README's accuracy pick) scores by late interaction instead:
 ``score`` returns raw MaxSim scores (``colbert.ColBERTScorer``), where the reference's CrossEncoder would put an
 untrained classification head on the checkpoint (INTEGRATION.md).  ColBERT-XM (antoinelouis/colbert-xm, the README's
@@ -25,7 +27,7 @@ import numpy as np
 from .embeddings import _check_device
 from .encoder import BertEncoder
 from .tokenizer import PairAssembler, RaggedTokenizer, load_tokenizer, pipelined
-from .weights import DebertaConfig, XLMRConfig, resolve_colbert, resolve_model
+from .weights import DebertaConfig, ModernBertConfig, XLMRConfig, resolve_colbert, resolve_model
 
 PIPE_PAIRS = 512      # pairs per pipelined chunk of a bulk score() call (one 100-pair rerank is a single chunk)
 
@@ -62,13 +64,14 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
         self.max_length = min(int(max_len), cfg.max_pos)
         self.activation = activation
         xlmr, deberta = isinstance(cfg, XLMRConfig), isinstance(cfg, DebertaConfig)
-        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, xlmr=xlmr, deberta=deberta)
+        modern = isinstance(cfg, ModernBertConfig)
+        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, xlmr=xlmr, deberta=deberta, modernbert=modern)
         self._ragged = RaggedTokenizer(self.tokenizer, self.max_length)
         # pair batches assembled from cached per-text ids (identical to self._ragged(a, b); tests/test_host_logic.py)
         self._pairs = PairAssembler(self.tokenizer, self.max_length)
-        # XLM-R / RoBERTa take no token types (their tokenizers return none), and DeBERTa-v3 has no token-type table:
-        # a null pointer, all zeros
-        self._types = not (xlmr or deberta)
+        # XLM-R / RoBERTa take no token types (their tokenizers return none), and DeBERTa-v3 and ModernBERT have no
+        # token-type table: a null pointer, all zeros
+        self._types = not (xlmr or deberta or modern)
         self.client = BertEncoder(cfg, w, with_head=True, device=device)
         self._max_tokens = self.client.max_tokens_per_call
 

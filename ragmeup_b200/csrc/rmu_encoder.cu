@@ -222,9 +222,19 @@ struct Disentangled {
     const int* __restrict__ cidx;             // [2 rmax + 1]: clamp(s + bucket(r), 0, 2s - 1) at r + rmax, r = i - j
     int rmax, c0, W;
 };
+// RelBias = Window (ModernBERT's local layers, full mode): key j is visible to query i iff |i - j| <= w.  A CTA stages
+// only the keys [max(0, rbase - w), min(S, rbase + 16 NW + w)), a warp skips the 32-key blocks outside its rows' windows,
+// and the remaining scores outside the window are masked to -inf.  A row can then meet a block whose keys are all masked
+// before any visible key: its running max is still -inf, and exp2(-inf - -inf) would be NaN, so (as FlashAttention
+// does) the exponent base is 0 while the max is -inf.  With w >= S - 1 the staged keys, their order and every score are
+// those of the kernel without the pack, so the output is bit-identical to it.
+struct Window {
+    int w;
+};
 template <typename... P> constexpr bool kHasBias = (std::is_same_v<P, const float*> || ...);
 template <typename... P> constexpr bool kHasKeyLimit = (std::is_same_v<P, KeyLimit> || ...);
 template <typename... P> constexpr bool kHasDis = (std::is_same_v<P, Disentangled> || ...);
+template <typename... P> constexpr bool kHasWindow = (std::is_same_v<P, Window> || ...);
 constexpr int kRelMax = 127;                  // |j - i| >= 127 all fall in MPNet's last bucket (distance >= 91)
 constexpr int kRelSpan = 2 * kRelMax + 1;
 template <int DH, int MINB, int NW = kAttWarps, bool CLS = false, typename... RelBias>  // NW warps = 16 * NW query rows per CTA
@@ -304,7 +314,13 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
         const KeyLimit lim = (rel_bias, ...);
         SK = min(max(lim.n[b], 1), S);
     }
-    for (int sb0 = 0; sb0 < SK; sb0 += ksb) {
+    int K0 = 0;                                    // first key staged
+    if constexpr (kHasWindow<RelBias...>) {
+        const Window win = (rel_bias, ...);
+        K0 = max(0, rbase - win.w);
+        SK = min(S, rbase + NW * 16 + win.w);
+    }
+    for (int sb0 = K0; sb0 < SK; sb0 += ksb) {
         const int nk = min(ksb, SK - sb0);
         const int nk16 = (nk + 15) & ~15;
         __syncthreads();
@@ -326,6 +342,11 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
         __syncthreads();
         if (!warp_live) continue;
         for (int kb0 = 0; kb0 < nk16; kb0 += 32) {
+            if constexpr (kHasWindow<RelBias...>) {    // every key of the block outside every row's window: no change
+                const Window win = (rel_bias, ...);
+                const int j0 = sb0 + kb0;
+                if (j0 + 31 < r0 - win.w || j0 > r0 + 15 + win.w) continue;
+            }
             float sacc[4][4];
 #pragma unroll
             for (int n = 0; n < 4; ++n) sacc[n][0] = sacc[n][1] = sacc[n][2] = sacc[n][3] = 0.f;
@@ -385,6 +406,19 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
                     }
                 }
             }
+            if constexpr (kHasWindow<RelBias...>) {
+                const Window win = (rel_bias, ...);
+                const int ia = r0 + g, ib = r0 + g + 8;
+#pragma unroll
+                for (int n = 0; n < 4; ++n) {
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const int j = sb0 + kb0 + n * 8 + 2 * t + c;
+                        if (abs(ia - j) > win.w) sacc[n][c] = -INFINITY;
+                        if (abs(ib - j) > win.w) sacc[n][2 + c] = -INFINITY;
+                    }
+                }
+            }
             float bm0 = -INFINITY, bm1 = -INFINITY;
             if (kb0 + 32 > nk) {                     // only the last key block holds keys past the sequence end
 #pragma unroll
@@ -404,13 +438,16 @@ __global__ void __launch_bounds__(NW * 32, MINB) attention_planes_kernel(const _
             bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 1));
             bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 2));
             const float mn0 = fmaxf(m0, bm0), mn1 = fmaxf(m1, bm1);
-            const float c0 = fast_exp2(m0 - mn0), c1 = fast_exp2(m1 - mn1);   // scores are pre-scaled by log2(e)
+            // exponent base: the running max, or 0 while a windowed row has seen masked keys only (see Window)
+            const float ms0 = kHasWindow<RelBias...> && mn0 == -INFINITY ? 0.f : mn0;
+            const float ms1 = kHasWindow<RelBias...> && mn1 == -INFINITY ? 0.f : mn1;
+            const float c0 = fast_exp2(m0 - ms0), c1 = fast_exp2(m1 - ms1);   // scores are pre-scaled by log2(e)
             m0 = mn0; m1 = mn1;
             float ps0 = 0.f, ps1 = 0.f;
 #pragma unroll
             for (int n = 0; n < 4; ++n) {
-                sacc[n][0] = fast_exp2(sacc[n][0] - mn0); sacc[n][1] = fast_exp2(sacc[n][1] - mn0);
-                sacc[n][2] = fast_exp2(sacc[n][2] - mn1); sacc[n][3] = fast_exp2(sacc[n][3] - mn1);
+                sacc[n][0] = fast_exp2(sacc[n][0] - ms0); sacc[n][1] = fast_exp2(sacc[n][1] - ms0);
+                sacc[n][2] = fast_exp2(sacc[n][2] - ms1); sacc[n][3] = fast_exp2(sacc[n][3] - ms1);
                 ps0 += sacc[n][0] + sacc[n][1];
                 ps1 += sacc[n][2] + sacc[n][3];
             }
@@ -554,6 +591,69 @@ __global__ void __launch_bounds__(256) cls_head_kernel(const __half* __restrict_
     }
 }
 
+// ModernBERT's head (ModernBertPredictionHead + classifier) on pooled rows p [B, H] fp32 (pool_kernel's CLS or mean, not
+// normalised) -> out [B, num_labels] = cw LN(gelu_erf(dw p + db)) + cb, LN with gain ng and shift nb (zeros without
+// norm_bias).  One 256-thread block per row; the dense layer's outputs are one warp's fmaf chain each, the LayerNorm's
+// mean and variance block reductions in a fixed order.
+__global__ void __launch_bounds__(256) mb_head_kernel(const float* __restrict__ pooled, int H, int num_labels,
+                                                      const float* __restrict__ dw, const float* __restrict__ db,
+                                                      const float* __restrict__ ng, const float* __restrict__ nb, float eps,
+                                                      const float* __restrict__ cw, const float* __restrict__ cb,
+                                                      float* __restrict__ out) {
+    extern __shared__ float sh[];   // p[H], y[H]
+    __shared__ float red[32];
+    float* pr = sh;
+    float* y = sh + H;
+    const int b = blockIdx.x;
+    for (int d = threadIdx.x; d < H; d += blockDim.x) pr[d] = pooled[static_cast<size_t>(b) * H + d];
+    __syncthreads();
+    const int warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    for (int j = warp; j < H; j += nw) {
+        const float* wr = dw + static_cast<size_t>(j) * H;
+        float s = 0.f;
+        for (int d = lane_id(); d < H; d += 32) s = fmaf(wr[d], pr[d], s);
+        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+        if (lane_id() == 0) y[j] = gelu_erf(s + db[j]);
+    }
+    __syncthreads();
+    auto block_sum = [&](float v) {
+        for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+        if (lane_id() == 0) red[warp] = v;
+        __syncthreads();
+        float t = 0.f;
+        for (int i = 0; i < nw; ++i) t += red[i];
+        __syncthreads();
+        return t;
+    };
+    float s = 0.f;
+    for (int d = threadIdx.x; d < H; d += blockDim.x) s += y[d];
+    const float mean = block_sum(s) / static_cast<float>(H);
+    float q = 0.f;
+    for (int d = threadIdx.x; d < H; d += blockDim.x) { const float e = y[d] - mean; q = fmaf(e, e, q); }
+    const float rstd = 1.0f / sqrtf(block_sum(q) / static_cast<float>(H) + eps);
+    for (int d = threadIdx.x; d < H; d += blockDim.x) y[d] = (y[d] - mean) * rstd * ng[d] + nb[d];
+    __syncthreads();
+    for (int c = warp; c < num_labels; c += nw) {
+        const float* wr = cw + static_cast<size_t>(c) * H;
+        float t = 0.f;
+        for (int d = lane_id(); d < H; d += 32) t = fmaf(wr[d], y[d], t);
+        for (int off = 16; off > 0; off >>= 1) t += __shfl_xor_sync(0xffffffffu, t, off);
+        if (lane_id() == 0) out[static_cast<size_t>(b) * num_labels + c] = t + cb[c];
+    }
+}
+
+// pos[t] = t - cu[b] for token t of sequence b: each row's position within its sequence (the rotary epilogue's input)
+__global__ void seq_positions_kernel(const int* __restrict__ cu, int B, int T, int* __restrict__ pos) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= T) return;
+    int lo_b = 0, hi_b = B;
+    while (hi_b - lo_b > 1) {
+        const int mid = (lo_b + hi_b) >> 1;
+        if (cu[mid] <= t) lo_b = mid; else hi_b = mid;
+    }
+    pos[t] = t - cu[lo_b];
+}
+
 // row cu[b] of [T, H] planes -> row b of [B, H] planes, bit for bit (zeros for an empty sequence).  H % 8 == 0.
 __global__ void gather_cls_rows_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, const int* __restrict__ cu,
                                        int H, __half* __restrict__ out_hi, __half* __restrict__ out_lo) {
@@ -593,11 +693,13 @@ constexpr int kClsAttWarps = 4;
 // nkeys non-null ([B] int32, full mode without a bias): sequence b attends to its first min(max(nkeys[b], 1), S_b) rows.
 // dis non-null (DeBERTa-v2, d_h = 64, neither a bias nor a key limit): the position terms of launch_position_terms are
 // added to every score (warps must be 10); in CLS mode its c2p rows are the compact CLS rows, offset here per slice.
+// window > 0 (ModernBERT's local layers; full mode, 10 warps, none of the above): key j is visible to query i iff
+// |i - j| <= window (the Window pack).
 constexpr int kMaxGridY = 65535;
 static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __half* cls_q_hi, const __half* cls_q_lo,
                             const int* cu, int B, int H, int heads, int max_seqlen, int warps, __half* ctx_hi,
                             __half* ctx_lo, cudaStream_t st, const float* rel_bias = nullptr, const int* nkeys = nullptr,
-                            const Disentangled* dis = nullptr) {
+                            const Disentangled* dis = nullptr, int window = 0) {
     const int DH = H / heads;
     const bool cls = cls_q_hi != nullptr;
     const bool bias = rel_bias != nullptr;
@@ -607,6 +709,11 @@ static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __
     }
     if (dis && (bias || nkeys || DH != 64 || (!cls && warps != kAttWarps))) {
         set_error("attention: the disentangled position terms run with head_dim 64 and 10 warps, without a bias or key limit");
+        return RMU_ERR_ARG;
+    }
+    if (window < 0 || (window > 0 && (cls || bias || nkeys || dis || warps != kAttWarps))) {
+        set_error("attention: a sliding window (window > 0) runs in full mode with 10 warps, without a bias, key limit or "
+                  "position terms");
         return RMU_ERR_ARG;
     }
     if (cls) warps = kClsAttWarps;
@@ -634,7 +741,10 @@ static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __
                           : attention_planes_kernel<64, 1, kAttWarps, false, KeyLimit>;
     auto dkern = cls ? attention_planes_kernel<64, 2, kClsAttWarps, true, Disentangled>
                      : attention_planes_kernel<64, 1, kAttWarps, false, Disentangled>;
-    if (dis) RMU_CUDA(cudaFuncSetAttribute(dkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
+    auto wkern = DH == 32 ? attention_planes_kernel<32, 2, kAttWarps, false, Window>
+                          : attention_planes_kernel<64, 1, kAttWarps, false, Window>;
+    if (window > 0) RMU_CUDA(cudaFuncSetAttribute(wkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
+    else if (dis) RMU_CUDA(cudaFuncSetAttribute(dkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
     else if (bias) RMU_CUDA(cudaFuncSetAttribute(bkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
     else if (nkeys) RMU_CUDA(cudaFuncSetAttribute(lkern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
     else RMU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)));
@@ -643,7 +753,9 @@ static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __
         // full mode addresses Q and the context by token (cu[b] is absolute), CLS mode by sequence
         const size_t roff = cls ? static_cast<size_t>(s0) * H : 0;
         dim3 pg(static_cast<unsigned>(heads), static_cast<unsigned>(nb), zblocks);
-        if (dis) {
+        if (window > 0) {
+            wkern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, nullptr, nullptr, cu + s0, H, ksb, ctx_hi, ctx_lo, Window{window});
+        } else if (dis) {
             Disentangled d = *dis;
             if (cls) d.c2p += static_cast<size_t>(s0) * heads * d.W;
             dkern<<<pg, warps * 32, smem, st>>>(qkv_hi, qkv_lo, cls ? cls_q_hi + roff : nullptr, cls ? cls_q_lo + roff : nullptr,
@@ -706,6 +818,25 @@ static int launch_cls_head(const __half* hi, const __half* lo, const int* cu, in
     ProfScope _ps(PROF_POOL_HEAD, st);
     cls_head_kernel<<<B, 256, 2 * H * sizeof(float), st>>>(hi, lo, cu, H, num_labels, compact ? 1 : 0, pw, pb, cw, cb,
                                                            head_act, out);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// E4 mb_head_kernel: one 256-thread block per pooled row -> out [B, num_labels]
+static int launch_mb_head(const float* pooled, int B, int H, int num_labels, const float* dw, const float* db,
+                          const float* ng, const float* nb, float eps, const float* cw, const float* cb, float* out,
+                          cudaStream_t st) {
+    ProfScope _ps(PROF_POOL_HEAD, st);
+    mb_head_kernel<<<B, 256, 2 * H * sizeof(float), st>>>(pooled, H, num_labels, dw, db, ng, nb, eps, cw, cb, out);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+static int launch_seq_positions(const int* cu, int B, int T, int* pos, cudaStream_t st) {
+    ProfScope _ps(PROF_MISC, st);
+    seq_positions_kernel<<<static_cast<unsigned>((T + 255) / 256), 256, 0, st>>>(cu, B, T, pos);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
@@ -984,6 +1115,7 @@ struct EncLayer {
     SplitOperand D1, D2;                  // adapter_dim > 0: X-MOD's language adapter, dense1 [A, H] and dense2 [H, A]
     float *d1 = nullptr, *d2 = nullptr;
     __half *pos_hi = nullptr, *pos_lo = nullptr;   // position_buckets > 0: PQ' | PK planes [2s, 2H] of the layer
+    int window = 0;                       // ModernBERT: the layer's attention half-window (0 = global attention)
 };
 
 struct rmu_encoder {
@@ -996,6 +1128,13 @@ struct rmu_encoder {
     std::vector<EncLayer> layers;
     SplitOperand last_wq, last_wkv;       // views of the last layer's Wqkv: rows 0..H (q) and H..3H (k | v)
     float *pw = nullptr, *pb = nullptr, *cw = nullptr, *cb = nullptr;
+    // ModernBERT (pre-LN, run_modernbert): ln1 = attn_norm (null in layer 0), W1 = Wi with its rows in GeGLU blocks, ln2 =
+    // mlp_norm; final_norm; the head's norm (pw / pb = head.dense); rope tables [max_pos, d_h / 2] of global (0) and
+    // local (1) layers; the classifier's pooling
+    bool modern = false;
+    float *fng = nullptr, *fnb = nullptr, *hng = nullptr, *hnb = nullptr;
+    float *rope_cos[2] = {nullptr, nullptr}, *rope_sin[2] = {nullptr, nullptr};
+    int mb_pool = RMU_POOL_CLS;
     // activations
     int tok_cap = 0, seq_cap = 0;
     std::vector<void*> act_allocs;
@@ -1005,6 +1144,7 @@ struct rmu_encoder {
     SplitOperand X_cls, Q_cls, CTX_cls, X1_cls, FF_cls;
     float* PRE_cls = nullptr;
     SplitOperand FFA, FFA_cls;            // adapter_dim > 0: the FF / FF_cls planes seen as [rows, adapter_dim]
+    int* POSI = nullptr;                  // ModernBERT: each token's position within its sequence [tok_cap]
     // position_buckets > 0 (DeBERTa): cidx over |i - j| <= max_pos - 1 (host copy and device table), and the position
     // terms' workspace, grown under mu
     std::vector<int> cidx_h;
@@ -1114,6 +1254,7 @@ static int ensure_tokens(rmu_encoder* e, int T, int B) {
     const int A = e->cfg.adapter_dim;
     if (rc == RMU_OK && A > 0) rc = make_split_operand(&e->FFA, e->FF.hi, e->FF.lo, cap, A);
     if (rc == RMU_OK && A > 0) rc = make_split_operand(&e->FFA_cls, e->FF_cls.hi, e->FF_cls.lo, scap, A);
+    if (rc == RMU_OK && e->modern) rc = dev_alloc(e->act_allocs, &e->POSI, cap);
     if (rc != RMU_OK) { free_acts(e); return rc; }
     e->tok_cap = cap;
     e->seq_cap = scap;
@@ -1191,6 +1332,61 @@ static int run_last_layer_cls(rmu_encoder* e, const EncLayer& L, const int32_t* 
     return launch_layernorm(e->PRE_cls, B, H, L.ln2g, L.ln2b, c.ln_eps, e->X_cls.hi, e->X_cls.lo, st);
 }
 
+// ModernBERT's pre-LN stack (every layer in full): leaves final_norm of the residual stream in e->X.  The residual stream
+// is never normalised, so it stays fp32, in e->PRE, updated in place by the fp32-residual epilogue:
+//   x = LN_emb(tok_embeddings[id])                      (embed_ln_kernel with zero position / token-type rows)
+//   per layer: a = (l == 0 ? x : LN_a(x)); x += Wo attn(rope(Wqkv a)); x += Wo2 geglu(Wi LN_m(x))
+//   out = LN_final(x)
+// Global layers (window 0) attend to the whole sequence with the rope tables of global_rope_theta, local ones to
+// |i - j| <= window with those of local_rope_theta.
+static int run_modernbert(rmu_encoder* e, const int32_t* ids, const int32_t* type_ids, const int32_t* cu, int B, int T,
+                          int max_seqlen, cudaStream_t st) {
+    const rmu_bert_config& c = e->cfg;
+    const int H = c.hidden, F = c.ffn, DH = H / c.heads;
+    int rc = ensure_tokens(e, T, B);
+    if (rc != RMU_OK) return rc;
+    RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace is shared by all callers
+    rc = launch_seq_positions(cu, B, T, e->POSI, st);
+    // one zero row for both the position and the token-type table: (w + 0) + 0 == w
+    if (rc == RMU_OK)
+        rc = launch_embed_ln(ids, type_ids, cu, B, T, H, c.vocab_size, 1, 1, e->word, e->pos, e->typ, e->eg, e->eb, c.ln_eps,
+                             e->X.hi, e->X.lo, st);
+    if (rc == RMU_OK) rc = launch_join_planes(e->X.hi, e->X.lo, static_cast<size_t>(T) * H, e->PRE, st);
+    if (rc != RMU_OK) return rc;
+    const float qscale = 1.4426950408889634f / sqrtf(static_cast<float>(DH));
+    for (int l = 0; l < c.layers; ++l) {
+        const EncLayer& L = e->layers[l];
+        if (l > 0) {
+            rc = launch_layernorm(e->PRE, T, H, L.ln1g, L.ln1b, c.ln_eps, e->X.hi, e->X.lo, st);
+            if (rc != RMU_OK) return rc;
+        }
+        const int tab = L.window > 0 ? 1 : 0;
+        GemmParams g{};
+        g.M = T; g.N = 3 * H; g.K = H; g.bias = L.bqkv;
+        g.out_hi = e->QKVP.hi; g.out_lo = e->QKVP.lo; g.qcols = H; g.qscale = qscale;
+        g.pos = e->POSI; g.rope_cos = e->rope_cos[tab]; g.rope_sin = e->rope_sin[tab]; g.rope_hd = DH; g.rope_rows = c.max_pos;
+        rc = launch_gemm(GEMM_BIAS_SPLIT_ROPE, e->X, L.Wqkv, g, e->sms, st);
+        if (rc == RMU_OK)
+            rc = launch_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, H, c.heads, max_seqlen, kAttWarps, e->CTX.hi,
+                                  e->CTX.lo, st, nullptr, nullptr, nullptr, L.window);
+        if (rc != RMU_OK) return rc;
+        g = GemmParams{};
+        g.M = T; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
+        rc = launch_gemm(GEMM_BIAS_RESF32_F32, e->CTX, L.Wo, g, e->sms, st);
+        if (rc == RMU_OK) rc = launch_layernorm(e->PRE, T, H, L.ln2g, L.ln2b, c.ln_eps, e->X1.hi, e->X1.lo, st);
+        if (rc != RMU_OK) return rc;
+        g = GemmParams{};
+        g.M = T; g.N = 2 * F; g.K = H; g.bias = L.b1; g.out_hi = e->FF.hi; g.out_lo = e->FF.lo;
+        rc = launch_gemm(GEMM_BIAS_GEGLU_SPLIT, e->X1, L.W1, g, e->sms, st);
+        if (rc != RMU_OK) return rc;
+        g = GemmParams{};
+        g.M = T; g.N = H; g.K = F; g.bias = L.b2; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
+        rc = launch_gemm(GEMM_BIAS_RESF32_F32, e->FF, L.W2, g, e->sms, st);
+        if (rc != RMU_OK) return rc;
+    }
+    return launch_layernorm(e->PRE, T, H, e->fng, e->fnb, c.ln_eps, e->X.hi, e->X.lo, st);
+}
+
 // the encoder stack: leaves the last hidden state in e->X (split planes), or with cls_only that of the CLS rows alone in
 // e->X_cls (row b = sequence b; e->X then holds the input of the last layer).  nkeys ([B] device int32, not with
 // cls_only): every layer's attention keys of sequence b stop at row nkeys[b] (ColBERT's [MASK] query padding).
@@ -1205,6 +1401,7 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
                              : "sequence longer than max_position_embeddings");
         return RMU_ERR_ARG;
     }
+    if (e->modern) return run_modernbert(e, ids, type_ids, cu, B, T, max_seqlen, st);
     int rc = ensure_tokens(e, T, B);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace is shared by all callers
@@ -1472,6 +1669,147 @@ int rmu_encoder_create_ex(const rmu_bert_config* cfg, const rmu_encoder_ext* ext
     return RMU_OK;
 }
 
+// ModernBERT: GeGLU's Wi [2F, cols] (rows 0..F inputs, F..2F gates) -> 128-row blocks of 64 input rows followed by the
+// 64 matching gate rows, so one E1 tile holds both halves of 64 output columns
+static std::vector<float> geglu_rows(const float* w, int F, int cols) {
+    std::vector<float> out(static_cast<size_t>(2) * F * cols);
+    for (int k = 0; k < F / 64; ++k)
+        for (int half = 0; half < 2; ++half)
+            std::copy(w + (static_cast<size_t>(half) * F + 64 * k) * cols, w + (static_cast<size_t>(half) * F + 64 * k + 64) * cols,
+                      out.begin() + (static_cast<size_t>(128) * k + 64 * half) * cols);
+    return out;
+}
+
+int rmu_encoder_create_modernbert(const rmu_bert_config* cfg, const rmu_modernbert_ext* mb, const float* const* w,
+                                  int n_weights, int has_head, rmu_encoder** out) {
+    if (!cfg || !mb || !w || !out || !mb->half_window_h) { set_error("rmu_encoder_create_modernbert: bad argument"); return RMU_ERR_ARG; }
+    const int H = cfg->hidden, F = cfg->ffn, L = cfg->layers, nh = cfg->heads;
+    if (cfg->position_mode != RMU_POS_ABSOLUTE || cfg->rel_buckets != 0 || cfg->adapter_dim != 0) {
+        set_error("rmu_encoder_create_modernbert: position_mode, rel_buckets and adapter_dim must be 0 (rotary positions, no "
+                  "relative bias, no adapters)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (L < 1 || nh <= 0 || H % 128 != 0 || H > 1024 || H % nh != 0 || (H / nh != 32 && H / nh != 64) || F <= 0 ||
+        F % 64 != 0 || cfg->vocab_size <= 0 || cfg->max_pos <= 0 || cfg->num_labels <= 0) {
+        set_error("rmu_encoder_create_modernbert: unsupported shape (hidden a multiple of 128 up to 1024, head_dim 32 or 64, "
+                  "intermediate_size a multiple of 64, at least one layer)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (mb->head_form != RMU_MB_HEAD_DENSE_GELU_LN) {
+        set_error("rmu_encoder_create_modernbert: head_form must be RMU_MB_HEAD_DENSE_GELU_LN (0)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (mb->pooling != RMU_POOL_CLS && mb->pooling != RMU_POOL_MEAN) {
+        set_error("rmu_encoder_create_modernbert: pooling must be RMU_POOL_CLS or RMU_POOL_MEAN");
+        return RMU_ERR_ARG;
+    }
+    for (int l = 0; l < L; ++l)
+        if (mb->half_window_h[l] < 0) {
+            set_error("rmu_encoder_create_modernbert: layer " + std::to_string(l) + " has a negative half-window");
+            return RMU_ERR_ARG;
+        }
+    const int DH = H / nh;
+    if (mb->rope_rows != cfg->max_pos || mb->rope_half != DH / 2) {
+        set_error("rmu_encoder_create_modernbert: the rope tables must be [max_pos, head_dim / 2] = [" +
+                  std::to_string(cfg->max_pos) + ", " + std::to_string(DH / 2) + "]");
+        return RMU_ERR_ARG;
+    }
+    const int head0 = 3 + 12 * L + 2, rope0 = head0 + (has_head ? 6 : 0), expect = rope0 + 4;
+    if (n_weights != expect) {
+        set_error("rmu_encoder_create_modernbert: expected " + std::to_string(expect) + " weight tensors");
+        return RMU_ERR_ARG;
+    }
+    for (int j = 0; j < expect; ++j) {
+        const bool layer0_attn_norm = j == 3 || j == 4;                // layer 0 has no attn_norm (identity)
+        if (!w[j] && !layer0_attn_norm) {
+            set_error(j >= rope0 ? "rmu_encoder_create_modernbert: null rope table"
+                                 : "rmu_encoder_create_modernbert: null weight tensor " + std::to_string(j));
+            return RMU_ERR_ARG;
+        }
+    }
+    for (int l = 0; l < L; ++l) {
+        static const char* const kName[] = {"Wqkv", "attention Wo", "mlp Wi", "mlp Wo"};
+        const int slot[] = {2, 4, 8, 10};
+        const size_t count[] = {size_t(3) * H * H, size_t(H) * H, size_t(2) * F * H, size_t(H) * F};
+        for (int k = 0; k < 4; ++k) {
+            const float* p = w[3 + 12 * l + slot[k]];
+            for (size_t j = 0; j < count[k]; ++j) {
+                if (std::fabs(p[j]) >= 65520.0f) {
+                    set_error("rmu_encoder_create_modernbert: layer " + std::to_string(l) + " " + kName[k] + " weight [" +
+                              std::to_string(j) + "] = " + std::to_string(p[j]) +
+                              " is outside the split fp16 planes' range (|w| < 65520)");
+                    return RMU_ERR_UNSUPPORTED;
+                }
+            }
+        }
+    }
+    rmu_encoder* e = new rmu_encoder();
+    e->cfg = *cfg;
+    e->has_head = has_head;
+    e->modern = true;
+    e->mb_pool = mb->pooling;
+    if (cudaGetDevice(&e->device) != cudaSuccess || (e->sms = device_sm_count()) <= 0 ||
+        cudaEventCreateWithFlags(&e->ws_done, cudaEventDisableTiming) != cudaSuccess) {
+        set_error("rmu_encoder_create_modernbert: no CUDA device (this library has no CPU path)");
+        delete e;
+        return RMU_ERR_CUDA;
+    }
+    int rc = RMU_OK;
+    int i = 0;
+    auto up = [&](float** dst, size_t n) { if (rc == RMU_OK) rc = upload(e, dst, w[i], n); ++i; };
+    up(&e->word, static_cast<size_t>(cfg->vocab_size) * H);
+    up(&e->eg, H);
+    up(&e->eb, H);
+    const std::vector<float> zeros(H, 0.f);
+    if (rc == RMU_OK) rc = upload(e, &e->pos, zeros.data(), H);
+    if (rc == RMU_OK) rc = upload(e, &e->typ, zeros.data(), H);
+    e->layers.resize(L);
+    for (int l = 0; l < L && rc == RMU_OK; ++l) {
+        EncLayer& Ly = e->layers[l];
+        Ly.window = mb->half_window_h[l];
+        if (l > 0) { up(&Ly.ln1g, H); up(&Ly.ln1b, H); } else i += 2;
+        if (rc == RMU_OK) rc = upload_split(e, &Ly.Wqkv, {w[i]}, 3 * H, H);
+        ++i;
+        up(&Ly.bqkv, static_cast<size_t>(3) * H);
+        if (rc == RMU_OK) rc = upload_split(e, &Ly.Wo, {w[i]}, H, H);
+        ++i;
+        up(&Ly.bo, H);
+        up(&Ly.ln2g, H);
+        up(&Ly.ln2b, H);
+        if (rc == RMU_OK) {
+            const std::vector<float> wi = geglu_rows(w[i], F, H);
+            rc = upload_split(e, &Ly.W1, {wi.data()}, 2 * F, H);
+        }
+        ++i;
+        if (rc == RMU_OK) {
+            const std::vector<float> bi = geglu_rows(w[i], F, 1);
+            rc = upload(e, &Ly.b1, bi.data(), bi.size());
+        }
+        ++i;
+        if (rc == RMU_OK) rc = upload_split(e, &Ly.W2, {w[i]}, H, F);
+        ++i;
+        up(&Ly.b2, H);
+    }
+    up(&e->fng, H);
+    up(&e->fnb, H);
+    if (has_head) {
+        up(&e->pw, static_cast<size_t>(H) * H);
+        up(&e->pb, H);
+        up(&e->hng, H);
+        up(&e->hnb, H);
+        up(&e->cw, static_cast<size_t>(cfg->num_labels) * H);
+        up(&e->cb, cfg->num_labels);
+    }
+    const size_t tab = static_cast<size_t>(cfg->max_pos) * (DH / 2);
+    up(&e->rope_cos[0], tab);
+    up(&e->rope_sin[0], tab);
+    up(&e->rope_cos[1], tab);
+    up(&e->rope_sin[1], tab);
+    if (rc != RMU_OK) { rmu_encoder_destroy(e); return rc; }
+    *out = e;
+    return RMU_OK;
+}
+
 void rmu_encoder_destroy(rmu_encoder* e) {
     if (!e) return;
     cudaDeviceSynchronize();
@@ -1489,7 +1827,7 @@ int rmu_encoder_embed(rmu_encoder* e, const int32_t* ids, const int32_t* type_id
     if (pool_mode != RMU_POOL_MEAN && pool_mode != RMU_POOL_CLS) { set_error("bad pool_mode"); return RMU_ERR_ARG; }
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool cls = pool_mode == RMU_POOL_CLS;
+    const bool cls = pool_mode == RMU_POOL_CLS && !e->modern;     // ModernBERT runs every layer in full
     rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, cls, st);
     if (rc != RMU_OK) return rc;
     const SplitOperand& h = cls ? e->X_cls : e->X;
@@ -1508,6 +1846,16 @@ int rmu_encoder_classify(rmu_encoder* e, const int32_t* ids, const int32_t* type
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, true, st);
     if (rc != RMU_OK) return rc;
+    if (e->modern) {
+        // pool the final hidden state (CLS or mean) into PRE_cls, then the head
+        rc = launch_pool(e->X.hi, e->X.lo, cu, B, e->cfg.hidden, e->mb_pool, 0, false, e->PRE_cls, st);
+        if (rc == RMU_OK)
+            rc = launch_mb_head(e->PRE_cls, B, e->cfg.hidden, e->cfg.num_labels, e->pw, e->pb, e->hng, e->hnb, e->cfg.ln_eps,
+                                e->cw, e->cb, out, st);
+        if (rc != RMU_OK) return rc;
+        RMU_CUDA(cudaEventRecord(e->ws_done, st));
+        return RMU_OK;
+    }
     rc = launch_cls_head(e->X_cls.hi, e->X_cls.lo, cu, B, e->cfg.hidden, e->cfg.num_labels, true, e->pw, e->pb, e->cw, e->cb,
                          out, st, e->ext.head_act);
     if (rc != RMU_OK) return rc;
@@ -2015,6 +2363,37 @@ int rmu_debug_cls_head_act(const uint16_t* hi, const uint16_t* lo, const int32_t
     }
     return launch_cls_head(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), cu, B, H, num_labels,
                            false, pw, pb, cw, cb, out, static_cast<cudaStream_t>(stream), head_act);
+}
+
+int rmu_debug_attention_window(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu, int B, int H, int heads,
+                               int max_seqlen, int window, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream) {
+    if (!qkv_hi || !qkv_lo || !cu || !ctx_hi || !ctx_lo || B <= 0 || heads <= 0 || H <= 0 || max_seqlen <= 0 || window <= 0) {
+        set_error("rmu_debug_attention_window: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H % heads != 0 || (H / heads != 32 && H / heads != 64)) {
+        set_error("rmu_debug_attention_window: head_dim must be 32 or 64");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_attention(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), nullptr, nullptr,
+                            cu, B, H, heads, max_seqlen, kAttWarps, reinterpret_cast<__half*>(ctx_hi),
+                            reinterpret_cast<__half*>(ctx_lo), static_cast<cudaStream_t>(stream), nullptr, nullptr, nullptr,
+                            window);
+}
+
+int rmu_debug_modernbert_head(const float* pooled, int B, int H, int num_labels, const float* dense_w, const float* dense_b,
+                              const float* norm_w, const float* norm_b, float eps, const float* cw, const float* cb,
+                              float* out, void* stream) {
+    if (!pooled || !dense_w || !dense_b || !norm_w || !norm_b || !cw || !cb || !out || B <= 0 || H <= 0 || num_labels <= 0) {
+        set_error("rmu_debug_modernbert_head: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H > 1024) {
+        set_error("rmu_debug_modernbert_head: hidden must be at most 1024");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_mb_head(pooled, B, H, num_labels, dense_w, dense_b, norm_w, norm_b, eps, cw, cb, out,
+                          static_cast<cudaStream_t>(stream));
 }
 
 int rmu_debug_split_planes(const float* src, int64_t n, uint16_t* hi, uint16_t* lo, void* stream) {

@@ -45,6 +45,12 @@ enum GemmMode {
     GEMM_BIAS_GELU_SPLIT = 1, // out planes = split(gelu_erf(acc + bias))
     GEMM_BIAS_RESID_F32 = 2,  // out_f32 = acc + bias + (res_hi + res_lo)
     GEMM_BIAS_SPLIT_QSCALE = 3, // out planes = split((acc + bias) * (col < qcols ? qscale : 1))   (QKV projection)
+    // ModernBERT (pre-LN, rotary positions, GeGLU):
+    GEMM_BIAS_SPLIT_ROPE = 4,   // GEMM_BIAS_SPLIT_QSCALE with the q and k columns (col < 2 qcols) rotated per head at the
+                                // row's position: x'[c] = x[c] cos - x[c + d/2] sin, x'[c + d/2] = x[c + d/2] cos + x[c] sin
+    GEMM_BIAS_GEGLU_SPLIT = 5,  // W's rows in 128-row blocks of 64 input rows | the 64 matching gate rows: out planes
+                                // [M, N / 2] = split(gelu_erf(in + b_in) * (gate + b_gate))
+    GEMM_BIAS_RESF32_F32 = 6,   // out_f32 = acc + bias + res_f32 (res_f32 may be out_f32: in place)
 };
 
 struct GemmParams {
@@ -55,6 +61,11 @@ struct GemmParams {
     const __half* res_hi; const __half* res_lo;  // [M, N]
     int qcols; float qscale;              // GEMM_BIAS_SPLIT_QSCALE
     int out_ld;                           // row pitch of out_f32 / out_hi / out_lo in elements (0 = N)
+    // (appended, so the fields above keep their offsets)
+    const float* res_f32;                 // [M, N] GEMM_BIAS_RESF32_F32
+    const int* pos;                       // [M] GEMM_BIAS_SPLIT_ROPE: each row's position within its sequence
+    const float* rope_cos; const float* rope_sin;   // [rope_rows, rope_hd / 2] fp32 tables
+    int rope_hd, rope_rows;               // head dim (32 or 64) and the tables' rows (positions clamp into them)
 };
 
 __device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {
@@ -142,6 +153,71 @@ __device__ __forceinline__ int gemm_mainloop_tile(float (&acc0)[64], float (&acc
     return prev;
 }
 
+// GEMM_BIAS_SPLIT_ROPE's values of one 64-column block (block c of the tile, first column col0) -> w (hi pair, lo pair).
+// The block is one head (d_h = 64) or two (d_h = 32); HALF8 = d_h / 16 is the distance, in 8-column groups, between the
+// two columns of a rotated pair, so both live in this thread (groups j and j + HALF8) and every index is static.  The
+// rotated values replace the accumulators of the block (which nothing reads afterwards), so no more registers are live
+// than in the other split modes.
+template <int HALF8>
+__device__ __forceinline__ void rope_rotate(float (&acc)[2][64], const GemmParams& p, int row0, int c, int csub) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int grow = row0 + r * 64 + 8 * h;
+            int ps = grow < p.M ? __ldg(p.pos + grow) : 0;
+            ps = ps < 0 ? 0 : (ps >= p.rope_rows ? p.rope_rows - 1 : ps);
+            const float* ct = p.rope_cos + static_cast<size_t>(ps) * (HALF8 * 8);
+            const float* st = p.rope_sin + static_cast<size_t>(ps) * (HALF8 * 8);
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+                if ((jj / HALF8) % 2 != 0) continue;                 // the second half of a head: rotated with its partner
+                const int i = 8 * (jj % HALF8) + csub;               // frequency index of columns (i, i + 1)
+                const float2 cs = __ldg(reinterpret_cast<const float2*>(ct + i));
+                const float2 sn = __ldg(reinterpret_cast<const float2*>(st + i));
+                float* a = &acc[r][4 * (8 * c + jj) + 2 * h];
+                float* b = &acc[r][4 * (8 * c + jj + HALF8) + 2 * h];
+                const float a0 = a[0], a1 = a[1], b0 = b[0], b1 = b[1];
+                a[0] = a0 * cs.x - b0 * sn.x; a[1] = a1 * cs.y - b1 * sn.y;
+                b[0] = b0 * cs.x + a0 * sn.x; b[1] = b1 * cs.y + a1 * sn.y;
+            }
+        }
+    }
+}
+
+__device__ __forceinline__ void rope_epilogue(float (&acc)[2][64], uint32_t (&w)[2][2][8][2], const GemmParams& p,
+                                              int row0, int col0, int c, int csub) {
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+        const float2 bia2 = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * jj + csub));
+        const int j = 8 * c + jj;
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                acc[r][4 * j + 2 * h] += bia2.x;
+                acc[r][4 * j + 2 * h + 1] += bia2.y;
+            }
+    }
+    if (col0 < 2 * p.qcols) {                                        // q and k: rotated; v (col >= 2 qcols) is not
+        if (p.rope_hd == 64) rope_rotate<4>(acc, p, row0, c, csub);
+        else rope_rotate<2>(acc, p, row0, c, csub);
+    }
+    const float sc = col0 < p.qcols ? p.qscale : 1.0f;
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+                const int j = 8 * c + jj;
+                __half2 h2, l2;
+                split_f16x2(make_float2(acc[r][4 * j + 2 * h] * sc, acc[r][4 * j + 2 * h + 1] * sc), h2, l2);
+                w[r][h][jj][0] = *reinterpret_cast<const uint32_t*>(&h2);
+                w[r][h][jj][1] = *reinterpret_cast<const uint32_t*>(&l2);
+            }
+}
+
 // Accumulator layout of wgmma m64nN (f32): thread t of the warpgroup holds rows 16 * (t / 32) + (t % 32) / 4 and + 8,
 // columns 8 j + 2 (t % 4) + {0, 1} for j < N / 8, as d[4 j + 2 h + e] (h = second row, e = second column).
 //
@@ -155,8 +231,9 @@ gemm_f16x3_kernel(const __grid_constant__ CUtensorMap tAh, const __grid_constant
                   const __grid_constant__ CUtensorMap tWh, const __grid_constant__ CUtensorMap tWl,
                   const __grid_constant__ CUtensorMap tOa, const __grid_constant__ CUtensorMap tOb,
                   const GemmParams p) {
-    constexpr bool kF32Out = MODE == GEMM_BIAS_F32 || MODE == GEMM_BIAS_RESID_F32;
+    constexpr bool kF32Out = MODE == GEMM_BIAS_F32 || MODE == GEMM_BIAS_RESID_F32 || MODE == GEMM_BIAS_RESF32_F32;
     constexpr int kJB = kF32Out ? 4 : 8;                       // 8-column groups per 128-byte box row
+    constexpr int kBoxes = MODE == GEMM_BIAS_GEGLU_SPLIT ? 1 : kGemmBN / 8 / kJB;   // GeGLU: 64 output columns per tile
     extern __shared__ uint8_t gemm_smem_raw[];
     // 1024-byte alignment by OFFSET into the shared array (the 128-byte swizzle repeats every 1024 B)
     uint8_t* smem = gemm_smem_raw + ((1024u - (smem_u32(gemm_smem_raw) & 1023u)) & 1023u);
@@ -215,8 +292,31 @@ gemm_f16x3_kernel(const __grid_constant__ CUtensorMap tAh, const __grid_constant
         // ---- epilogue per column block of 32 (fp32) / 64 (split) columns: values into registers, then one 128-row x
         // 128-byte box per output plane through the staging buffer
 #pragma unroll
-        for (int c = 0; c < kGemmBN / 8 / kJB; ++c) {
+        for (int c = 0; c < kBoxes; ++c) {
             uint32_t w[2][2][kJB][2];                                  // [r][h][jj]: fp32 (x, y) or (hi pair, lo pair)
+            if constexpr (MODE == GEMM_BIAS_SPLIT_ROPE) {
+                rope_epilogue(acc, w, p, mb * kGemmBM + rsub, nb * kGemmBN + 64 * c, c, csub);
+            } else if constexpr (MODE == GEMM_BIAS_GEGLU_SPLIT) {
+                // columns 8 jj + csub of the block are inputs, 64 + 8 jj + csub their gates: both in this thread
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+#pragma unroll
+                    for (int jj = 0; jj < 8; ++jj) {
+                        const int col = nb * kGemmBN + 8 * jj + csub;
+                        const float2 bi = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+                        const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + col + 64));
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const float2 v = make_float2(gelu_erf(acc[r][4 * jj + 2 * h] + bi.x) * (acc[r][4 * (jj + 8) + 2 * h] + bg.x),
+                                                         gelu_erf(acc[r][4 * jj + 2 * h + 1] + bi.y) * (acc[r][4 * (jj + 8) + 2 * h + 1] + bg.y));
+                            __half2 h2, l2;
+                            split_f16x2(v, h2, l2);
+                            w[r][h][jj][0] = *reinterpret_cast<const uint32_t*>(&h2);
+                            w[r][h][jj][1] = *reinterpret_cast<const uint32_t*>(&l2);
+                        }
+                    }
+                }
+            } else {
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
 #pragma unroll
@@ -237,6 +337,10 @@ gemm_f16x3_kernel(const __grid_constant__ CUtensorMap tAh, const __grid_constant
                             const float2 rl = __half22float2(*reinterpret_cast<const __half2*>(p.res_lo + o));
                             v = make_float2(v.x + (rh.x + rl.x), v.y + (rh.y + rl.y));
                         }
+                        if (MODE == GEMM_BIAS_RESF32_F32 && grow < p.M) {
+                            const float2 rr = *reinterpret_cast<const float2*>(p.res_f32 + static_cast<size_t>(grow) * p.N + col);
+                            v = make_float2(v.x + rr.x, v.y + rr.y);
+                        }
                         if (kF32Out) {
                             w[r][h][jj][0] = __float_as_uint(v.x);
                             w[r][h][jj][1] = __float_as_uint(v.y);
@@ -248,6 +352,7 @@ gemm_f16x3_kernel(const __grid_constant__ CUtensorMap tAh, const __grid_constant
                         }
                     }
                 }
+            }
             }
 #pragma unroll
             for (int pl = 0; pl < (kF32Out ? 1 : 2); ++pl) {
@@ -270,7 +375,8 @@ gemm_f16x3_kernel(const __grid_constant__ CUtensorMap tAh, const __grid_constant
                 fence_proxy_async_smem();                              // generic-proxy writes -> visible to the TMA store
                 bar_sync_named(kGemmEpiBar + wg, 128);
                 if (store_lead) {
-                    tma_store_2d(pl ? &tOb : &tOa, staging, nb * kGemmBN + 8 * kJB * c, mb * kGemmBM);
+                    tma_store_2d(pl ? &tOb : &tOa, staging, MODE == GEMM_BIAS_GEGLU_SPLIT ? nb * 64 : nb * kGemmBN + 8 * kJB * c,
+                                 mb * kGemmBM);
                     bulk_commit();
                 }
             }

@@ -21,7 +21,7 @@ import numpy as np
 from . import _lib
 from .encoder import MAX_TOKENS_PER_CALL, BertEncoder
 from .tokenizer import RaggedTokenizer, load_tokenizer, pipelined
-from .weights import MPNetConfig, XLMRConfig, resolve_model
+from .weights import ModernBertConfig, MPNetConfig, XLMRConfig, resolve_model
 
 PIPE_TEXTS = 1000     # texts per pipelined chunk of a bulk embed_documents() call
 
@@ -56,10 +56,12 @@ class HuggingFaceEmbeddings:
         # sentence-transformers applies the model's own Normalize module; encode_kwargs can force it
         self.normalize = bool(normalize or self.encode_kwargs.get("normalize_embeddings", False))
         self.max_seq_length = int(max_len)
-        xlmr = isinstance(cfg, XLMRConfig)
-        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, mpnet=isinstance(cfg, MPNetConfig), xlmr=xlmr)
+        xlmr, modern = isinstance(cfg, XLMRConfig), isinstance(cfg, ModernBertConfig)
+        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, mpnet=isinstance(cfg, MPNetConfig), xlmr=xlmr,
+                                        modernbert=modern)
         self._ragged = RaggedTokenizer(self.tokenizer, self.max_seq_length)
-        self._types = not xlmr         # XLM-R / RoBERTa take no token types: a null pointer, all zeros
+        # XLM-R / RoBERTa take no token types, ModernBERT has none: a null pointer, all zeros
+        self._types = not (xlmr or modern)
         self.client = BertEncoder(cfg, w, with_head=False, device=device)
 
     # -- tensor fast path (additional to the reference surface)

@@ -6,6 +6,11 @@ intermediate/output/LayerNorm, then pooler + classifier when a head is present, 
 relative attention bias [32, heads] when the config has one, then X-MOD's language adapter of every layer, for the
 config's one language, when it has ``adapter_dim > 0``, then DeBERTa's relative embeddings and LN_rel when it has
 ``position_buckets > 0``).
+
+ModernBERT takes its own order (``weights.modernbert_weight_names``, ``rmu_encoder_create_modernbert``): the token
+embeddings and their norm; per layer attn_norm (layer 0: placeholders, not read), Wqkv, Wo, mlp_norm, Wi, mlp Wo, each
+with its bias (zeros where the checkpoint has none); final_norm; with a head, head.dense, head.norm and the classifier;
+then the four rope tables of ``weights.rope_tables``, computed here from the config.
 """
 from __future__ import annotations
 
@@ -15,7 +20,7 @@ from typing import Dict, Optional
 import numpy as np
 
 from . import _lib
-from .weights import BertConfig, weight_names
+from .weights import BertConfig, ModernBertConfig, rope_tables, weight_names
 
 POOL = {"mean": 0, "cls": 1}
 MAX_TOKENS_PER_CALL = 131072    # bounds the activation workspace (~19 KB/token for MiniLM shapes => ~2.5 GB)
@@ -46,11 +51,20 @@ class BertEncoder:
             if tuple(a.shape) != tuple(shape):
                 raise ValueError(f"{name}: expected shape {shape}, got {a.shape}")
             arrs.append(a)
+        modern = isinstance(cfg, ModernBertConfig)
+        if modern:
+            arrs += list(rope_tables(cfg))
         ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
         cc = _lib.bert_config_c(cfg)
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):
-            if cfg.position_buckets or cfg.head_act:
+            if modern:
+                win = np.ascontiguousarray(cfg.layer_windows, dtype=np.int32)
+                mb = _lib.ModernBertExtC(win.ctypes.data, POOL[cfg.classifier_pooling], 0, cfg.max_pos, cfg.head_dim // 2)
+                _lib.check(_lib.lib().rmu_encoder_create_modernbert(C.byref(cc), C.byref(mb), ptrs, len(arrs),
+                                                                    int(self.with_head), C.byref(self._h)),
+                           "rmu_encoder_create_modernbert")
+            elif cfg.position_buckets or cfg.head_act:
                 ext = _lib.encoder_ext_c(cfg)
                 _lib.check(_lib.lib().rmu_encoder_create_ex(C.byref(cc), C.byref(ext), ptrs, len(arrs), int(self.with_head),
                                                             C.byref(self._h)), "rmu_encoder_create_ex")

@@ -170,11 +170,18 @@ def build_deberta_unigram(pieces: Sequence[Tuple[str, float]]) -> Tokenizer:
 
 
 def load_tokenizer(source: Optional[str], vocab_size: int = 30522, mpnet: bool = False, xlmr: bool = False,
-                   deberta: bool = False) -> Tokenizer:
+                   deberta: bool = False, modernbert: bool = False) -> Tokenizer:
     """``source`` = snapshot dir (tokenizer.json or vocab.txt) or None -> synthetic vocab; ``mpnet`` selects MPNet's
     vocabulary layout and templates where the snapshot has no tokenizer.json.  ``xlmr`` (XLM-R / RoBERTa) and
     ``deberta`` (DeBERTa-v2 / v3): a snapshot must have tokenizer.json (read by ``tokenizers``); None -> the synthetic
-    Unigram vocabulary of that family."""
+    Unigram vocabulary of that family.  ``modernbert``: a snapshot must have tokenizer.json (ModernBERT's BPE with the
+    template ``[CLS] A [SEP] B [SEP]``); None -> the synthetic WordPiece vocabulary, which has the same template."""
+    if modernbert and source is not None:
+        tj = os.path.join(source, "tokenizer.json")
+        if os.path.exists(tj):
+            return Tokenizer.from_file(tj)
+        raise FileNotFoundError(f"{source}: ModernBERT snapshots need tokenizer.json (its BPE tokenizer has no other "
+                                f"file form)")
     if deberta:
         if source is None:
             return build_deberta_unigram(synthetic_deberta_pieces(vocab_size))

@@ -234,6 +234,145 @@ class DebertaConfig(BertConfig):
                              max_relative_positions=mrp if mrp >= 1 else max_pos)
 
 
+def modernbert_windows(layers: int, global_every: int = 3, local_attention: int = 128) -> Tuple[int, ...]:
+    """per-layer half-windows of ModernBERT's release config form: layer l is global (0) when l % global_every == 0,
+    else local with half-window local_attention // 2"""
+    return tuple(0 if l % global_every == 0 else local_attention // 2 for l in range(layers))
+
+
+@dataclass
+class ModernBertConfig(BertConfig):
+    """ModernBERT (transformers ``ModernBertModel`` / ``ModernBertForSequenceClassification``; gte-reranker-modernbert,
+    modernbert-embed, gte-modernbert): a pre-LN encoder, ``x += Wo attn(LN_a(x))``, ``x += Wo mlp(LN_m(x))``, then
+    ``final_norm``, with ``LN_a`` the identity in layer 0.  Rotary positions on q and k (``global_theta`` on global
+    layers, ``local_theta`` on local ones, no position table), a GeGLU feed-forward (``Wi`` [2F, H]: ``gelu(input) *
+    gate``), sliding-window attention ``|i - j| <= layer_windows[l]`` on the local layers (0 = global), and the head
+    ``classifier(LN(gelu(dense(p))))`` on the CLS row or the mean of the final hidden state (``classifier_pooling``).
+    Absent biases and LayerNorm shifts are zero tensors in the weight dict."""
+    vocab_size: int = 50368
+    hidden: int = 768
+    layers: int = 22
+    heads: int = 12
+    ffn: int = 1152
+    max_pos: int = 8192
+    type_vocab: int = 1
+    ln_eps: float = 1e-5
+    layer_windows: Tuple[int, ...] = ()
+    global_theta: float = 160000.0
+    local_theta: float = 10000.0
+    classifier_pooling: str = "cls"
+
+    def __post_init__(self):
+        if not self.layer_windows:
+            self.layer_windows = modernbert_windows(self.layers)
+        self.layer_windows = tuple(int(x) for x in self.layer_windows)
+        if len(self.layer_windows) != self.layers:
+            raise ValueError(f"modernbert: {len(self.layer_windows)} layer windows for {self.layers} layers")
+
+    @staticmethod
+    def from_hf(d: dict) -> "ModernBertConfig":
+        """config.json of a ``modernbert`` checkpoint, in the release form (``global_attn_every_n_layers``,
+        ``global_rope_theta``, ``local_rope_theta``, ``local_attention``) or transformers 5's (``layer_types``,
+        ``rope_parameters``) -> ModernBertConfig; refuses, naming the field, what the encoder does not compute"""
+        def refuse(field, value, why):
+            raise ValueError(f"modernbert with {field} = {value!r} is not supported: {why}")
+        for key in ("hidden_activation", "classifier_activation"):
+            if d.get(key, "gelu") != "gelu":
+                refuse(key, d.get(key), "only erf-GELU is computed")
+        pooling = d.get("classifier_pooling", "cls")
+        if pooling not in ("cls", "mean"):
+            refuse("classifier_pooling", pooling, "the head pools by cls or mean")
+        H, nh, L = int(d["hidden_size"]), int(d["num_attention_heads"]), int(d["num_hidden_layers"])
+        if d.get("head_dim") is not None and int(d["head_dim"]) != H // nh:
+            refuse("head_dim", d["head_dim"], f"it must be hidden_size / num_attention_heads = {H // nh}")
+        half = int(d.get("local_attention", 128)) // 2
+        types = d.get("layer_types")
+        if types:
+            if len(types) != L:
+                refuse("layer_types", types, f"it must name {L} layers")
+            for t in types:
+                if t not in ("full_attention", "sliding_attention"):
+                    refuse("layer_types", t, "layers are full_attention or sliding_attention")
+            windows = tuple(0 if t == "full_attention" else half for t in types)
+        else:
+            windows = modernbert_windows(L, int(d.get("global_attn_every_n_layers", 3)), 2 * half)
+        theta = {"full_attention": float(d.get("global_rope_theta", 160000.0)),
+                 "sliding_attention": float(d.get("local_rope_theta", 10000.0))}
+        if d.get("rope_scaling"):
+            refuse("rope_scaling", d["rope_scaling"], "RoPE scaling is not computed")
+        rp = d.get("rope_parameters")
+        if rp:
+            for t in theta:
+                p = rp.get(t, rp) or {}
+                if p.get("rope_type", "default") != "default":
+                    refuse("rope_type", p.get("rope_type"), "only the default rotary embedding is computed")
+                if p.get("rope_theta") is not None:
+                    theta[t] = float(p["rope_theta"])
+        return ModernBertConfig(vocab_size=int(d["vocab_size"]), hidden=H, layers=L, heads=nh,
+                                ffn=int(d["intermediate_size"]), max_pos=int(d.get("max_position_embeddings", 8192)),
+                                ln_eps=float(d.get("norm_eps", 1e-5)),
+                                num_labels=len(d["id2label"]) if "id2label" in d else d.get("num_labels", 1),
+                                layer_windows=windows, global_theta=theta["full_attention"],
+                                local_theta=theta["sliding_attention"], classifier_pooling=pooling)
+
+
+def rope_tables(cfg: ModernBertConfig):
+    """(cos_global, sin_global, cos_local, sin_local), each [max_pos, d_h / 2] float32, as transformers'
+    ``ModernBertRotaryEmbedding`` computes them: ``inv_freq = 1 / (theta ** (arange(0, d, 2).float() / d))``, the angle
+    ``pos * inv_freq`` in float32, then ``.cos()`` / ``.sin()``.  At pos ~ 8000 one float32 ulp of the angle is ~5e-4 rad,
+    so these float32 tables define the model: the float64 oracle looks its cos / sin up in them too."""
+    import torch
+    d = cfg.head_dim
+    pos = torch.arange(cfg.max_pos, dtype=torch.int64).float()
+    out = []
+    for theta in (cfg.global_theta, cfg.local_theta):
+        inv_freq = 1.0 / (theta ** (torch.arange(0, d, 2, dtype=torch.int64).float() / d))
+        ang = pos[:, None] * inv_freq[None, :]
+        out += [np.ascontiguousarray(ang.cos().numpy(), dtype=np.float32),
+                np.ascontiguousarray(ang.sin().numpy(), dtype=np.float32)]
+    return tuple(out)
+
+
+def modernbert_weight_names(cfg: ModernBertConfig, with_head: bool):
+    """canonical ModernBERT tensors (transformers' names without ``model.``) in rmu_encoder_create_modernbert's order;
+    ``layers.0.attn_norm.*`` are placeholders (ones, zeros) that the encoder does not read"""
+    H, F = cfg.hidden, cfg.ffn
+    names = [("embeddings.tok_embeddings.weight", (cfg.vocab_size, H)), ("embeddings.norm.weight", (H,)),
+             ("embeddings.norm.bias", (H,))]
+    for l in range(cfg.layers):
+        p = f"layers.{l}."
+        names += [(p + "attn_norm.weight", (H,)), (p + "attn_norm.bias", (H,)),
+                  (p + "attn.Wqkv.weight", (3 * H, H)), (p + "attn.Wqkv.bias", (3 * H,)),
+                  (p + "attn.Wo.weight", (H, H)), (p + "attn.Wo.bias", (H,)),
+                  (p + "mlp_norm.weight", (H,)), (p + "mlp_norm.bias", (H,)),
+                  (p + "mlp.Wi.weight", (2 * F, H)), (p + "mlp.Wi.bias", (2 * F,)),
+                  (p + "mlp.Wo.weight", (H, F)), (p + "mlp.Wo.bias", (H,))]
+    names += [("final_norm.weight", (H,)), ("final_norm.bias", (H,))]
+    if with_head:
+        names += [("head.dense.weight", (H, H)), ("head.dense.bias", (H,)), ("head.norm.weight", (H,)),
+                  ("head.norm.bias", (H,)), ("classifier.weight", (cfg.num_labels, H)),
+                  ("classifier.bias", (cfg.num_labels,))]
+    return names
+
+
+def modernbert_to_canonical(raw: Dict[str, np.ndarray], cfg: ModernBertConfig, with_head: bool) -> Dict[str, np.ndarray]:
+    """ModernBERT tensors (under ``model.``, as both transformers classes save them, or bare) plus ``head.*`` /
+    ``classifier.*`` -> the names of ``modernbert_weight_names``.  Zero vectors stand in for the biases and LayerNorm
+    shifts a checkpoint does not have (``attention_bias``, ``mlp_bias``, ``norm_bias`` and ``classifier_bias`` false),
+    and ones / zeros for layer 0's absent ``attn_norm``.  The masked-LM head (``head.*`` without a classifier, and
+    ``decoder.*``) is dropped."""
+    w: Dict[str, np.ndarray] = {}
+    for k, v in raw.items():
+        if k.startswith("decoder.") or (not with_head and k.startswith("head.")):
+            continue
+        k = k[6:] if k.startswith("model.") else k
+        w[k] = np.ascontiguousarray(v, dtype=np.float32)
+    for name, shape in modernbert_weight_names(cfg, with_head):
+        if name not in w and (name.endswith(".bias") or name == "layers.0.attn_norm.weight"):
+            w[name] = (np.ones if name.endswith("attn_norm.weight") else np.zeros)(shape, np.float32)
+    return w
+
+
 REL_EMB = "encoder.rel_embeddings.weight"
 REL_LN = ("encoder.LayerNorm.weight", "encoder.LayerNorm.bias")
 
@@ -261,7 +400,7 @@ def adapter_prefix(layer: int, language: str) -> str:
 
 
 # config.json model_type -> how the snapshot is read; a config without model_type is read as BERT
-MODEL_TYPES = ("bert", "mpnet", "roberta", "xlm-roberta", "xmod", "deberta-v2")
+MODEL_TYPES = ("bert", "mpnet", "roberta", "xlm-roberta", "xmod", "deberta-v2", "modernbert")
 
 
 # shapes of the models BASELINE.json / .env.template name (SURVEY.md §2.2 table)
@@ -300,10 +439,26 @@ PRESETS: Dict[str, Tuple[BertConfig, str, int]] = {
     "mxbai-rerank-base-v1": (DebertaConfig(hidden=768, layers=12, heads=12, ffn=3072), "cls", 512),
     "mxbai-rerank-large-v1": (DebertaConfig(hidden=1024, layers=24, heads=16, ffn=4096), "cls", 512),
     "tiny-deberta": (DebertaConfig(vocab_size=2000, hidden=128, layers=2, heads=2, ffn=256), "cls", 512),
+    # ModernBERT: the base and large shapes of the published configs [3P-recall: not checkable here]; the reranker
+    # pools by CLS (the base model's classifier_pooling default), modernbert-embed by mean + Normalize, gte-modernbert
+    # by CLS.  A snapshot's config.json and sentence-transformers modules override all of this.
+    "modernbert-base": (ModernBertConfig(hidden=768, layers=22, heads=12, ffn=1152), "cls", 8192),
+    "modernbert-large": (ModernBertConfig(hidden=1024, layers=28, heads=16, ffn=2624), "cls", 8192),
+    "gte-reranker-modernbert-base": (ModernBertConfig(hidden=768, layers=22, heads=12, ffn=1152), "cls", 8192),
+    "modernbert-embed-base": (ModernBertConfig(hidden=768, layers=22, heads=12, ffn=1152, classifier_pooling="mean"),
+                              "mean", 8192),
+    "gte-modernbert-base": (ModernBertConfig(hidden=768, layers=22, heads=12, ffn=1152), "cls", 8192),
+    # four layers, so both layer types and layer 0's identity attn_norm appear; and a small window (|i - j| <= 16), so
+    # short sequences cross many window blocks
+    "tiny-modernbert": (ModernBertConfig(vocab_size=1000, hidden=128, layers=4, heads=2, ffn=192, max_pos=1024),
+                        "mean", 1024),
+    "tiny-modernbert-window": (ModernBertConfig(vocab_size=1000, hidden=128, layers=4, heads=2, ffn=192, max_pos=1024,
+                                                layer_windows=modernbert_windows(4, 3, 32), classifier_pooling="mean"),
+                               "mean", 1024),
 }
 
 # presets whose sentence-transformers pipeline has no Normalize module
-UNNORMALIZED_PRESETS = {"multi-qa-mpnet-base-dot-v1", "paraphrase-multilingual-mpnet-base-v2"}
+UNNORMALIZED_PRESETS = {"multi-qa-mpnet-base-dot-v1", "paraphrase-multilingual-mpnet-base-v2", "gte-modernbert-base"}
 
 # FlashRank's model names -> the public HuggingFace checkpoints its ONNX files were exported from [3P-recall: flashrank
 # 0.2.x; the mapping is recalled, not read, and is unverified].  Only the BERT cross-encoders are here: FlashRank's T5
@@ -316,6 +471,8 @@ FLASHRANK_MODELS: Dict[str, str] = {
 
 
 def weight_names(cfg: BertConfig, with_head: bool):
+    if isinstance(cfg, ModernBertConfig):
+        return modernbert_weight_names(cfg, with_head)
     H, F = cfg.hidden, cfg.ffn
     names = [
         ("embeddings.word_embeddings.weight", (cfg.vocab_size, H)),
@@ -414,7 +571,15 @@ def synthetic_bert_weights(cfg: BertConfig, seed: int = 0, with_head: bool = Fal
         rng2 = np.random.default_rng(seed + 104729)
         names += [(n, s, rng2) for lang in cfg.languages for l in range(cfg.layers) for n, s in adapter_names(cfg, l, lang)]
     for name, shape, rng in names:
-        if name == REL_BIAS:                     # a few units across buckets, as trained MPNet biases spread
+        if isinstance(cfg, ModernBertConfig) and (name.endswith(".bias") or name.startswith("layers.0.attn_norm.")):
+            # ModernBERT has no biases or LayerNorm shifts (attention_bias, mlp_bias, norm_bias false), and no attn_norm
+            # in layer 0
+            a = np.ones(shape) if name == "layers.0.attn_norm.weight" else np.zeros(shape)
+        elif isinstance(cfg, ModernBertConfig) and name.endswith("norm.weight"):
+            a = 1.0 + 0.1 * rng.standard_normal(shape)
+        elif isinstance(cfg, ModernBertConfig) and name.startswith("embeddings."):
+            a = 0.02 * rng.standard_normal(shape) * (3.0 if scale > 1 else 1.0)
+        elif name == REL_BIAS:                     # a few units across buckets, as trained MPNet biases spread
             a = rng.standard_normal(shape)
         elif name == "embeddings.token_type_embeddings.weight" and isinstance(cfg, (MPNetConfig, DebertaConfig)):
             a = np.zeros(shape)                    # MPNet and DeBERTa have no token types (XLM-R's one row is trained)
@@ -477,12 +642,15 @@ def load_hf_snapshot(path: str, with_head: bool):
     if kind not in MODEL_TYPES:
         raise ValueError(f"{path}: model_type {kind!r} is not supported; the encoder runs {', '.join(MODEL_TYPES)}")
     mpnet, xlmr, deberta = kind == "mpnet", kind in ("roberta", "xlm-roberta", "xmod"), kind == "deberta-v2"
+    modern = kind == "modernbert"
     if mpnet and with_head:
         raise ValueError(f"{path}: MPNet cross-encoders are not supported (MPNet runs as a sentence embedder only)")
     if deberta and not with_head:
         raise ValueError(f"{path}: model_type 'deberta-v2' runs as a cross-encoder (reranker) only, not as an embedder")
     if kind == "xmod":
         cfg = XmodConfig.from_hf(cfgd, path)
+    elif modern:
+        cfg = ModernBertConfig.from_hf(cfgd)
     elif deberta:
         cfg = DebertaConfig.from_hf(cfgd)
     else:
@@ -490,6 +658,8 @@ def load_hf_snapshot(path: str, with_head: bool):
     raw = _load_tensors(path, _xmod_keep(cfg.language) if cfg.adapter_dim else None)
     if mpnet:
         w = mpnet_to_canonical(raw, cfg)
+    elif modern:
+        w = modernbert_to_canonical(raw, cfg, with_head)
     elif deberta:
         w = deberta_to_canonical(raw, cfg)
     elif xlmr:
@@ -504,6 +674,12 @@ def load_hf_snapshot(path: str, with_head: bool):
     if missing:
         raise KeyError(f"{path}: missing tensors {missing[:4]}...")
     pooling, normalize, max_len = "mean", False, min(cfg.max_pos - cfg.position_offset, 512)
+    if modern:
+        # sequences up to max_position_embeddings, within the tokenizer's model_max_length
+        max_len = cfg.max_pos
+        tc = _read_json(os.path.join(path, "tokenizer_config.json")) or {}
+        if tc.get("model_max_length") is not None:
+            max_len = min(int(tc["model_max_length"]), max_len)
     if deberta:
         # CrossEncoder passes max_length=None: the tokenizer's model_max_length, within max_position_embeddings
         max_len = cfg.max_pos
@@ -564,7 +740,8 @@ def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] 
             cfg.language = select_language(cfg.languages, cfg.language, model_name)
         w = synthetic_bert_weights(cfg, seed=seed, with_head=with_head, scale=scale)
         # an XLM-R preset scores as its checkpoint does: one label, no sbert_ce_default_activation_function -> sigmoid
-        act = "sigmoid" if with_head and isinstance(cfg, (XLMRConfig, DebertaConfig)) and cfg.num_labels == 1 else "identity"
+        act = ("sigmoid" if with_head and isinstance(cfg, (XLMRConfig, DebertaConfig, ModernBertConfig)) and cfg.num_labels == 1
+               else "identity")
         return cfg, w, pooling, preset not in UNNORMALIZED_PRESETS, max_len, act, None
     cands = [model_name]
     for root in (cache_folder, os.environ.get("RAGMEUP_MODEL_DIR")):
@@ -661,6 +838,9 @@ def load_colbert_snapshot(path: str):
     if kind == "deberta-v2":
         raise ValueError(f"{path}: a ColBERT checkpoint of model_type 'deberta-v2' is not supported: DeBERTa runs as a "
                          f"cross-encoder only")
+    if kind == "modernbert":
+        raise ValueError(f"{path}: a ColBERT checkpoint of model_type 'modernbert' is not supported: ModernBERT runs as a "
+                         f"cross-encoder or an embedder")
     if kind not in ("bert", "xlm-roberta", "roberta", "xmod"):
         raise ValueError(f"{path}: a ColBERT checkpoint of model_type {kind!r} is not supported (bert, xlm-roberta, "
                          f"roberta and xmod are)")
@@ -728,6 +908,9 @@ def resolve_colbert(model_name: str, cache_folder: Optional[str] = None):
 
 
 def _refuse_xlmr_flashrank(cfg: BertConfig, where: str) -> None:
+    if isinstance(cfg, ModernBertConfig):
+        raise ValueError(f"{where}: a ModernBERT (model_type 'modernbert') model is not a FlashRank model (FlashRank's "
+                         f"rerankers are BERT checkpoints); use HuggingFaceCrossEncoder for it")
     if isinstance(cfg, DebertaConfig):
         raise ValueError(f"{where}: a DeBERTa-v2 (model_type 'deberta-v2') model is not a FlashRank model (FlashRank's "
                          f"rerankers are BERT checkpoints); use HuggingFaceCrossEncoder for it")
