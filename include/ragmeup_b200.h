@@ -32,6 +32,7 @@ extern "C" {
 #define RMU_ERR_ARG -1
 #define RMU_ERR_CUDA -2
 #define RMU_ERR_UNSUPPORTED -3
+#define RMU_ERR_RANGE -4         /* an activation left the range its storage can hold (Qwen3's fp16 planes) */
 
 /* metric ids — Milvus FLAT/L2 is the reference default store metric (langchain-milvus 0.1.3
  * via server/RAGHelper.py:388-394); PGVector uses cosine distance (server/RAGHelper.py:399-404). */
@@ -259,10 +260,46 @@ typedef struct rmu_modernbert_ext {
 } rmu_modernbert_ext;
 int rmu_encoder_create_modernbert(const rmu_bert_config* cfg, const rmu_modernbert_ext* mb, const float* const* weights_h,
                                   int n_weights, int has_head, rmu_encoder** out);
+
+/* Qwen3 (transformers Qwen3Model / Qwen3ForSequenceClassification / Qwen3ForCausalLM, model_type "qwen3"): a decoder
+ * run as an encoder, with RMSNorm, grouped-query causal attention, rotary positions and a SwiGLU feed-forward.  With h
+ * the fp32 residual stream and RMS(x) = x * rsqrt(mean(x^2) + eps) (the weight multiplies it, not 1 + weight):
+ *   h = embed_tokens[id];  per layer:  x = w_in RMS(h);  q = Wq x, k = Wk x, v = Wv x (no biases);
+ *   q, k: per head wq_norm RMS(.) / wk_norm RMS(.) over head_dim, then rotate-half rotary at the token's position;
+ *   h += Wo attn(q, k, v) with query i seeing keys j <= i of its sequence, query head h reading kv head h / (heads /
+ *   kv_heads), scale head_dim^-0.5;  h += Wdown (silu(Wgate x2) * (Wup x2)) with x2 = w_post RMS(h);
+ *   hidden = w_norm RMS(h).
+ * The outputs take one row per sequence: its last token (embed, RMU_POOL_LAST only, then optionally L2-normalised), or
+ * with a head (classify) the rightmost token whose id != pad_token_id (pad_token_id < 0: the last token; no such token:
+ * the first), and logits = head [num_labels, H] . hidden(row) (no bias).
+ *
+ * weights_h (host fp32), in this order: embed_tokens [V, H]; per layer: input_layernorm [H], q_proj [heads d, H],
+ * k_proj [kv_heads d, H], v_proj [kv_heads d, H], q_norm [d], k_norm [d], o_proj [H, heads d], post_attention_layernorm
+ * [H], gate_proj [F, H], up_proj [F, H], down_proj [H, F]; norm [H]; with has_head: head [num_labels, H]; then the rope
+ * tables cos, sin, each [max_pos, d / 2] (row p, column i = cos / sin of p * inv_freq[i] in float32).  1 + 11 layers + 1
+ * (+ 1) + 2 tensors.  cfg: vocab_size, hidden, layers, heads, ffn (F), max_pos, num_labels and ln_eps (rms_norm_eps)
+ * are read.  Refused before any CUDA call: position_mode, rel_buckets or adapter_dim != 0, head_dim != 128, hidden not a
+ * multiple of 128 or above 4096, F % 64 != 0, kv_heads < 1 or heads % kv_heads != 0, and a GEMM weight with |w| >=
+ * 65520 (RMU_ERR_UNSUPPORTED); rope_rows != max_pos, rope_half != 64, head_form that disagrees with has_head, a wrong
+ * tensor count or a null tensor (RMU_ERR_ARG).
+ * Activations enter the GEMMs and attention as split fp16 planes, which cannot hold |x| > 65504: a forward whose
+ * normalised rows, q / k / v or SwiGLU outputs leave that range returns RMU_ERR_RANGE and writes no output.  The
+ * Qwen3 forward synchronises `stream` to read that flag.  Sequences may hold max_pos tokens. */
+#define RMU_QWEN3_HEAD_NONE 0
+#define RMU_QWEN3_HEAD_LAST 1
+typedef struct rmu_qwen3_ext {
+    int32_t kv_heads, head_dim;     /* num_key_value_heads, head_dim (128) */
+    int32_t rope_rows, rope_half;   /* shape of each rope table: max_pos, head_dim / 2 */
+    int32_t head_form;              /* RMU_QWEN3_HEAD_NONE (has_head 0) or RMU_QWEN3_HEAD_LAST (has_head 1) */
+    int32_t pad_token_id;           /* the head's row: the rightmost token whose id differs; < 0: the last token */
+} rmu_qwen3_ext;
+int rmu_encoder_create_qwen3(const rmu_bert_config* cfg, const rmu_qwen3_ext* ext, const float* const* weights_h,
+                             int n_weights, int has_head, rmu_encoder** out);
 void rmu_encoder_destroy(rmu_encoder* enc);
 
 #define RMU_POOL_MEAN 0
 #define RMU_POOL_CLS 1
+#define RMU_POOL_LAST 2   /* each sequence's last token: Qwen3 encoders only, which accept no other pooling */
 
 /* ragged batch: ids/type_ids [total_tokens] int32, cu_seqlens [B+1] int32 (all device); type_ids may be null (all 0).
  * max_seqlen must be at least the longest sequence in cu_seqlens; only max_seqlen itself is checked against
@@ -343,6 +380,8 @@ int rmu_colbert_score_host(rmu_colbert* cb, const int32_t* q_ids_h, const int32_
 #define RMU_GEMM_BIAS_GEGLU_SPLIT 5   /* W in 128-row blocks of 64 input | 64 gate rows: out planes [M, N / 2] =
                                        * split(gelu_erf(in + b_in) * (gate + b_gate))                           */
 #define RMU_GEMM_BIAS_RESF32_F32 6    /* out_f32 = A W^T + bias + res_f32 (res_f32 may equal out_f32)            */
+#define RMU_GEMM_BIAS_SWIGLU_SPLIT 7  /* W blocked as mode 5: out planes [M, N / 2] = split(silu(in + b_in) *
+                                       * (gate + b_gate)), silu(g) = g / (1 + exp(-g))                          */
 
 /* For tests: E1 on A [a_rows, K] (rows M..a_rows are read by the TMA loads but never reach the output) and
  * W [N, K]; bias [N], res [M, N], out [M, N].  N % 128 == 0, K % 64 == 0, a_rows >= M.  max_ctas caps the
@@ -369,6 +408,33 @@ int rmu_debug_attention_window(const uint16_t* qkv_hi, const uint16_t* qkv_lo, c
 int rmu_debug_modernbert_head(const float* pooled, int B, int H, int num_labels, const float* dense_w, const float* dense_b,
                               const float* norm_w, const float* norm_b, float eps, const float* cw, const float* cb,
                               float* out, void* stream);
+/* For tests: E1 in mode 7 (SwiGLU), shapes as rmu_debug_gemm, out planes [M, N / 2].  range_flag (device int32, may be
+ * NULL) is set to 1 when an output of rows 0..M has |x| > 65504 or is NaN; it is never cleared. */
+int rmu_debug_gemm_swiglu(const uint16_t* a_hi, const uint16_t* a_lo, int64_t a_rows, const uint16_t* w_hi,
+                          const uint16_t* w_lo, int M, int N, int K, const float* bias, int max_ctas, uint16_t* out_hi,
+                          uint16_t* out_lo, int32_t* range_flag, void* stream);
+/* For tests: Qwen3's RMSNorm of T fp32 rows [T, H] (device) -> split planes [T, H] = split(w * (x * rsqrt(mean(x^2) +
+ * eps))).  H a multiple of 128 up to 4096.  range_flag (device, may be NULL) as rmu_debug_gemm_swiglu's. */
+int rmu_debug_rmsnorm(const float* x, int T, int H, const float* w, float eps, uint16_t* hi, uint16_t* lo,
+                      int32_t* range_flag, void* stream);
+/* For tests: Qwen3's q / k step on the fp32 QKV rows [T, (heads + 2 kv_heads) 128] (q | k | v, heads of 128): per
+ * token and q or k head, RMSNorm over the head with q_norm / k_norm [128], rotate-half rotary at pos[t] (clamped into
+ * the cos / sin tables [rope_rows, 64]), q times qscale; v unchanged; all written as split planes of the same shape.
+ * range_flag as above. */
+int rmu_debug_qk_norm_rope(const float* qkv, int T, int heads, int kv_heads, const int32_t* pos, const float* q_norm,
+                           const float* k_norm, float eps, float qscale, const float* rope_cos, const float* rope_sin,
+                           int rope_rows, uint16_t* hi, uint16_t* lo, int32_t* range_flag, void* stream);
+/* For tests: Qwen3's causal grouped-query attention on the planes [T, (heads + 2 kv_heads) 128] of a ragged batch (q
+ * pre-scaled by log2(e) / sqrt(128)), cu_seqlens [B+1] -> ctx planes [T, heads 128].  Query i of a sequence sees its
+ * keys j <= i; query head h reads kv head h / (heads / kv_heads).  heads % kv_heads != 0 returns RMU_ERR_UNSUPPORTED. */
+int rmu_debug_attention_causal(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu_seqlens, int B,
+                               int heads, int kv_heads, int max_seqlen, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream);
+/* For tests: Qwen3's output rows on fp32 residual rows x [T, H] (device): per sequence b the row cu[b + 1] - 1
+ * (pad_id < 0) or the rightmost row whose ids[] != pad_id (none: the first row), y = w RMS(x_row); then out [B, H] = y
+ * (optionally L2-normalised) when head is NULL, else out [B, num_labels] = head [num_labels, H] . y.  An empty sequence
+ * gives zeros.  H a multiple of 128 up to 4096. */
+int rmu_debug_last_token(const float* x, const int32_t* ids, const int32_t* cu_seqlens, int B, int H, const float* w,
+                         float eps, int pad_id, int normalize, const float* head, int num_labels, float* out, void* stream);
 /* For tests: E2 on the QKV planes [T, 3H] of a ragged batch (q | k | v, q pre-scaled by log2(e) / sqrt(d_h) as the
  * QKV epilogue leaves it), cu_seqlens [B+1] int32 -> ctx planes [T, H].  d_h = H / heads is 32 or 64; warps is 10,
  * or 5 with d_h = 32. */

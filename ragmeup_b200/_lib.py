@@ -36,6 +36,11 @@ class ModernBertExtC(C.Structure):
                 ("rope_half", C.c_int32)]
 
 
+class Qwen3ExtC(C.Structure):
+    _fields_ = [("kv_heads", C.c_int32), ("head_dim", C.c_int32), ("rope_rows", C.c_int32), ("rope_half", C.c_int32),
+                ("head_form", C.c_int32), ("pad_token_id", C.c_int32)]
+
+
 def bert_config_c(cfg) -> BertConfigC:
     """weights.BertConfig (or a subclass) -> the C struct; adapter_dim is 0 for every family but X-MOD"""
     return BertConfigC(cfg.vocab_size, cfg.hidden, cfg.layers, cfg.heads, cfg.ffn, cfg.max_pos, cfg.type_vocab,
@@ -99,6 +104,8 @@ SIGNATURES = {
                                         C.c_int, C.POINTER(C.c_void_p)]),
     "rmu_encoder_create_modernbert": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(ModernBertExtC), C.POINTER(C.c_void_p),
                                                 C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
+    "rmu_encoder_create_qwen3": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(Qwen3ExtC), C.POINTER(C.c_void_p), C.c_int,
+                                           C.c_int, C.POINTER(C.c_void_p)]),
     "rmu_encoder_destroy": (None, [C.c_void_p]),
     "rmu_encoder_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_void_p, C.c_void_p]),
@@ -158,6 +165,17 @@ SIGNATURES = {
                                              C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_modernbert_head": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_gemm_swiglu": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                        C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_rmsnorm": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p]),
+    "rmu_debug_qk_norm_rope": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p]),
+    "rmu_debug_attention_causal": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                             C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_last_token": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float,
+                                       C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "rmu_debug_split_planes": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_join_planes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "rmu_debug_bm25_select": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

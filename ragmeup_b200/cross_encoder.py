@@ -12,6 +12,12 @@ truncate to ``min(model_max_length, max_position_embeddings)`` and run in calls 
 tokens, which bounds the attention position terms' workspace.  ModernBERT rerankers (gte-reranker-modernbert-base) pair
 the same way, send no token types and truncate to ``min(model_max_length, max_position_embeddings)`` (8192); their head
 pools by ``classifier_pooling`` (CLS or mean).
+Qwen3 cross-encoders take two forms.  A ``Qwen3ForSequenceClassification`` snapshot (``score.weight``) pairs as its
+tokenizer makes of (query, document), truncated ``longest_first``, and its head reads the rightmost token that is not
+``pad_token_id``.  A ``Qwen3ForCausalLM`` snapshot (Qwen3-Reranker) scores as its model card does, a documented
+deviation from the reference (whose CrossEncoder would put an untrained ``score`` head on it): the text is
+``prefix + tokens("<Instruct>: {instruction}\n<Query>: {q}\n<Document>: {d}") + suffix`` and the score P(yes) =
+``exp(log_softmax([logit_no, logit_yes])[1])`` at the last token (``Qwen3RerankPrompt``).
 A ColBERT checkpoint (colbert-ir/colbertv2.0, the reference README's accuracy pick) scores by late interaction instead:
 ``score`` returns raw MaxSim scores (``colbert.ColBERTScorer``), where the reference's CrossEncoder would put an
 untrained classification head on the checkpoint (INTEGRATION.md).  ColBERT-XM (antoinelouis/colbert-xm, the README's
@@ -23,13 +29,55 @@ from __future__ import annotations
 from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
+from tokenizers import Tokenizer
 
 from .embeddings import _check_device
 from .encoder import BertEncoder
 from .tokenizer import PairAssembler, RaggedTokenizer, load_tokenizer, pipelined
-from .weights import DebertaConfig, ModernBertConfig, XLMRConfig, resolve_colbert, resolve_model
+from .weights import (QWEN3_RERANK_INSTRUCTION, QWEN3_RERANK_PREFIX, QWEN3_RERANK_SUFFIX, DebertaConfig,
+                      ModernBertConfig, Qwen3Config, XLMRConfig, resolve_colbert, resolve_model)
 
 PIPE_PAIRS = 512      # pairs per pipelined chunk of a bulk score() call (one 100-pair rerank is a single chunk)
+
+
+class Qwen3RerankPrompt:
+    """(query, document) pairs -> Qwen3-Reranker's ragged batch: ``prefix + tokens(text) + suffix`` with ``text =
+    "<Instruct>: {instruction}\n<Query>: {q}\n<Document>: {d}"`` tokenised as the snapshot's tokenizer does (its
+    post-processor included) and truncated to ``max_length - len(prefix) - len(suffix)``; prefix and suffix are
+    tokenised without special tokens.  Returns (ids, None, cu_seqlens)."""
+
+    def __init__(self, tok: Tokenizer, max_length: int, instruction: str = QWEN3_RERANK_INSTRUCTION,
+                 prefix: str = QWEN3_RERANK_PREFIX, suffix: str = QWEN3_RERANK_SUFFIX):
+        self.instruction = instruction
+        self._tok = Tokenizer.from_str(tok.to_str())
+        self._tok.no_padding()
+        self._tok.no_truncation()
+        self.prefix = np.asarray(self._tok.encode(prefix, add_special_tokens=False).ids, dtype=np.int32)
+        self.suffix = np.asarray(self._tok.encode(suffix, add_special_tokens=False).ids, dtype=np.int32)
+        room = int(max_length) - len(self.prefix) - len(self.suffix)
+        if room < 1:
+            raise ValueError(f"Qwen3 reranker: max_length {max_length} leaves no room between its prompt's prefix and suffix")
+        self._tok.enable_truncation(max_length=room, strategy="longest_first")
+
+    def text(self, query: str, doc: str) -> str:
+        return f"<Instruct>: {self.instruction}\n<Query>: {query}\n<Document>: {doc}"
+
+    def __call__(self, queries: Sequence[str], docs: Sequence[str]):
+        enc = self._tok.encode_batch([self.text(q, d) for q, d in zip(queries, docs)])
+        seqs = [np.concatenate([self.prefix, np.asarray(e.ids, dtype=np.int32), self.suffix]) for e in enc]
+        cu = np.zeros(len(seqs) + 1, dtype=np.int32)
+        np.cumsum([len(x) for x in seqs], out=cu[1:])
+        return np.concatenate(seqs).astype(np.int32), None, cu
+
+
+def yes_probability(logits):
+    """[n, 2] (no, yes) logits -> exp(log_softmax(.)[:, 1]), numpy float32 or a torch tensor"""
+    if isinstance(logits, np.ndarray):
+        x = logits.astype(np.float64)
+        m = x.max(1, keepdims=True)
+        lse = m[:, 0] + np.log(np.exp(x - m).sum(1))
+        return np.exp(x[:, 1] - lse).astype(np.float32)
+    return logits.log_softmax(1)[:, 1].exp()
 
 
 class BaseCrossEncoder:
@@ -64,18 +112,26 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
         self.max_length = min(int(max_len), cfg.max_pos)
         self.activation = activation
         xlmr, deberta = isinstance(cfg, XLMRConfig), isinstance(cfg, DebertaConfig)
-        modern = isinstance(cfg, ModernBertConfig)
-        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, xlmr=xlmr, deberta=deberta, modernbert=modern)
+        modern, qwen = isinstance(cfg, ModernBertConfig), isinstance(cfg, Qwen3Config)
+        self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, xlmr=xlmr, deberta=deberta, modernbert=modern,
+                                        qwen3=qwen)
         self._ragged = RaggedTokenizer(self.tokenizer, self.max_length)
-        # pair batches assembled from cached per-text ids (identical to self._ragged(a, b); tests/test_host_logic.py)
-        self._pairs = PairAssembler(self.tokenizer, self.max_length)
-        # XLM-R / RoBERTa take no token types (their tokenizers return none), and DeBERTa-v3 and ModernBERT have no
-        # token-type table: a null pointer, all zeros
-        self._types = not (xlmr or deberta or modern)
+        if qwen and cfg.reranker:
+            self._pairs = Qwen3RerankPrompt(self.tokenizer, self.max_length)
+        elif qwen:
+            self._pairs = lambda a, b: self._ragged(a, b)      # the tokenizer's own pair encoding, longest_first
+        else:
+            # pair batches assembled from cached per-text ids (identical to self._ragged(a, b); tests/test_host_logic.py)
+            self._pairs = PairAssembler(self.tokenizer, self.max_length)
+        # XLM-R / RoBERTa take no token types (their tokenizers return none), and DeBERTa-v3, ModernBERT and Qwen3 have
+        # no token-type table: a null pointer, all zeros
+        self._types = not (xlmr or deberta or modern or qwen)
         self.client = BertEncoder(cfg, w, with_head=True, device=device)
         self._max_tokens = self.client.max_tokens_per_call
 
     def _post(self, logits: np.ndarray) -> np.ndarray:
+        if self.activation == "yes_prob":
+            return yes_probability(logits)
         if self.activation == "sigmoid":
             logits = 1.0 / (1.0 + np.exp(-logits.astype(np.float32)))
         # num_labels == 1 -> scalar per pair; otherwise langchain takes column 1
@@ -112,6 +168,8 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
             outs.append(self.client.classify_tokens(ids[t0:t1], typ[t0:t1] if self._types else None, sub_cu,
                                                     int(np.max(np.diff(sub_cu)))))
         logits = outs[0] if len(outs) == 1 else torch.cat(outs, 0)
+        if self.activation == "yes_prob":
+            return yes_probability(logits)
         if self.activation == "sigmoid":
             logits = torch.sigmoid(logits)
         return logits[:, 0] if self.config.num_labels == 1 else logits[:, 1]

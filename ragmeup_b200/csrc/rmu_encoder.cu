@@ -1104,6 +1104,446 @@ static int launch_colbert_maxsim(const float* q, const int* q_cu, const float* d
     return RMU_OK;
 }
 
+
+// ------------------------------------------------------------------------------------ Qwen3
+// Qwen3 runs as an encoder on an fp32 residual stream.  Its GEMM and attention inputs are split fp16 planes, which
+// cannot hold |x| > 65504: every kernel that writes such planes here sets *flag (when non-null) on a value outside that
+// range or a NaN, and the forward reports it instead of returning what the overflow made of the output.
+constexpr int kQwenHD = 128;                  // head_dim (the only one the kernels take)
+constexpr int kRmsThreads = 128;              // rms_split_kernel: thread i holds columns i, i + 128, ... (H <= 4096)
+constexpr int kRmsMaxPerThread = 32;
+
+__device__ __forceinline__ bool outside_f16(float v) { return !(fabsf(v) <= 65504.0f); }
+
+// Qwen3RMSNorm of one fp32 row per block -> split planes: y = w * (x * (1 / sqrt(mean(x^2) + eps))), all fp32.  The sum
+// of squares is per thread in column order, then the warps' shuffle trees, then the four warp sums in a fixed order.
+__global__ void __launch_bounds__(kRmsThreads) rms_split_kernel(const float* __restrict__ x, int H, const float* __restrict__ w,
+                                                               float eps, __half* __restrict__ hi, __half* __restrict__ lo,
+                                                               int* __restrict__ flag) {
+    __shared__ float red[kRmsThreads / 32];
+    const size_t row = blockIdx.x;
+    const float* xr = x + row * H;
+    const int n = H / kRmsThreads;
+    float v[kRmsMaxPerThread];
+    float ss = 0.f;
+#pragma unroll
+    for (int i = 0; i < kRmsMaxPerThread; ++i)
+        if (i < n) { v[i] = xr[i * kRmsThreads + threadIdx.x]; ss = fmaf(v[i], v[i], ss); }
+    for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
+    __syncthreads();
+    const float rs = 1.0f / sqrtf(((red[0] + red[1]) + (red[2] + red[3])) / static_cast<float>(H) + eps);
+    bool bad = false;
+#pragma unroll
+    for (int i = 0; i < kRmsMaxPerThread; ++i) {
+        if (i < n) {
+            const int c = i * kRmsThreads + threadIdx.x;
+            const float y = w[c] * (v[i] * rs);
+            __half h, l;
+            split_f16(y, h, l);
+            hi[row * H + c] = h;
+            lo[row * H + c] = l;
+            bad |= outside_f16(y);
+        }
+    }
+    if (bad && flag) atomicOr(flag, 1);
+}
+
+// h = embed_tokens[id] (fp32 rows, ids clamped into [0, vocab)): one float4 per thread
+__global__ void embed_rows_kernel(const int* __restrict__ ids, size_t n4, int H, int vocab, const float* __restrict__ table,
+                                  float* __restrict__ out) {
+    const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= n4) return;
+    const size_t t = i / (H / 4), c4 = i % (H / 4);
+    int id = ids[t];
+    id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
+    reinterpret_cast<float4*>(out)[i] = reinterpret_cast<const float4*>(table + static_cast<size_t>(id) * H)[c4];
+}
+
+// Qwen3's q / k step: one warp per (token, head) of the fp32 QKV rows [T, NH 128], NH = heads + 2 kv_heads (the q
+// heads, then k, then v); lane l holds dims 4l .. 4l + 3.  q and k heads: RMSNorm over the head with q_norm / k_norm,
+// then rotate-half rotary at the token's position, x'[c] = x[c] cos[c] - x[c + 64] sin[c] and x'[c + 64] = x[c + 64]
+// cos[c] + x[c] sin[c] for c < 64 (lane l < 16 holds c, lane l + 16 its partner), and q times qscale (log2(e) / sqrt(d),
+// the softmax runs in base 2).  Every head leaves as split planes of the same layout.
+__global__ void __launch_bounds__(256) qk_norm_rope_kernel(const float* __restrict__ qkv, int T, int heads, int kv_heads,
+                                                           const int* __restrict__ pos, const float* __restrict__ qn,
+                                                           const float* __restrict__ kn, float eps, float qscale,
+                                                           const float* __restrict__ rcos, const float* __restrict__ rsin,
+                                                           int rope_rows, __half* __restrict__ hi, __half* __restrict__ lo,
+                                                           int* __restrict__ flag) {
+    const int NH = heads + 2 * kv_heads;
+    const size_t gw = static_cast<size_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (gw >= static_cast<size_t>(T) * NH) return;
+    const int t = static_cast<int>(gw / NH), hh = static_cast<int>(gw % NH);
+    const int lane = threadIdx.x & 31;
+    const size_t o = gw * kQwenHD + lane * 4;
+    const float4 in = *reinterpret_cast<const float4*>(qkv + o);
+    float x[4] = {in.x, in.y, in.z, in.w};
+    if (hh < heads + kv_heads) {
+        float ss = 0.f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) ss = fmaf(x[i], x[i], ss);
+        for (int k = 16; k > 0; k >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, k);
+        const float rs = 1.0f / sqrtf(ss / static_cast<float>(kQwenHD) + eps);
+        const float4 nw = *reinterpret_cast<const float4*>((hh < heads ? qn : kn) + lane * 4);
+        x[0] = nw.x * (x[0] * rs); x[1] = nw.y * (x[1] * rs); x[2] = nw.z * (x[2] * rs); x[3] = nw.w * (x[3] * rs);
+        int p = pos[t];
+        p = p < 0 ? 0 : (p >= rope_rows ? rope_rows - 1 : p);
+        const int fi = (lane & 15) * 4;
+        const float4 c4 = *reinterpret_cast<const float4*>(rcos + static_cast<size_t>(p) * (kQwenHD / 2) + fi);
+        const float4 s4 = *reinterpret_cast<const float4*>(rsin + static_cast<size_t>(p) * (kQwenHD / 2) + fi);
+        const float cs[4] = {c4.x, c4.y, c4.z, c4.w}, sn[4] = {s4.x, s4.y, s4.z, s4.w};
+        const float sc = hh < heads ? qscale : 1.0f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float partner = __shfl_xor_sync(0xffffffffu, x[i], 16);
+            x[i] = (lane < 16 ? x[i] * cs[i] - partner * sn[i] : x[i] * cs[i] + partner * sn[i]) * sc;
+        }
+    }
+    uint32_t ph[2], pl[2];
+    split_pack(x[0], x[1], ph[0], pl[0]);
+    split_pack(x[2], x[3], ph[1], pl[1]);
+    *reinterpret_cast<uint2*>(hi + o) = make_uint2(ph[0], ph[1]);
+    *reinterpret_cast<uint2*>(lo + o) = make_uint2(pl[0], pl[1]);
+    const bool bad = outside_f16(x[0]) || outside_f16(x[1]) || outside_f16(x[2]) || outside_f16(x[3]);
+    if (bad && flag) atomicOr(flag, 1);
+}
+
+// Qwen3's output rows: one 256-thread block per sequence.  The row is the sequence's last (pad_id < 0) or its rightmost
+// token whose id != pad_id, the first when there is none (transformers' last_non_pad_token); y = w RMS(x_row) as in
+// rms_split_kernel; then out [B, H] = y, L2-normalised when `normalize` (x / max(|x|, 1e-12), sentence-transformers'
+// Normalize), or with a head out [B, num_labels] = head . y, one warp's fmaf chain per label.  An empty sequence: zeros.
+__global__ void __launch_bounds__(256) last_token_kernel(const float* __restrict__ x, const int* __restrict__ ids,
+                                                         const int* __restrict__ cu, int H, const float* __restrict__ w,
+                                                         float eps, int pad_id, int normalize, const float* __restrict__ head,
+                                                         int num_labels, float* __restrict__ out) {
+    extern __shared__ float yrow[];     // [H]
+    __shared__ float red[32];
+    __shared__ int sel;
+    const int b = blockIdx.x;
+    const int t0 = cu[b], S = cu[b + 1] - t0;
+    const int warp = threadIdx.x >> 5, nw = blockDim.x >> 5, lane = threadIdx.x & 31;
+    const int ow = head ? num_labels : H;
+    if (S <= 0) {
+        for (int c = threadIdx.x; c < ow; c += blockDim.x) out[static_cast<size_t>(b) * ow + c] = 0.f;
+        return;
+    }
+    if (warp == 0) {
+        int r = S - 1;
+        if (pad_id >= 0) {
+            r = 0;
+            for (int k0 = S; k0 > 0; k0 -= 32) {            // windows [k0 - 32, k0), right to left
+                const int k = k0 - 32 + lane;
+                const unsigned m = __ballot_sync(0xffffffffu, k >= 0 && ids[t0 + k] != pad_id);
+                if (m) { r = k0 - 32 + 31 - __clz(static_cast<int>(m)); break; }
+            }
+        }
+        if (lane == 0) sel = r;
+    }
+    __syncthreads();
+    auto block_sum = [&](float v) {
+        for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+        if (lane == 0) red[warp] = v;
+        __syncthreads();
+        float s = 0.f;
+        for (int i = 0; i < nw; ++i) s += red[i];
+        __syncthreads();
+        return s;
+    };
+    const float* xr = x + static_cast<size_t>(t0 + sel) * H;
+    float ss = 0.f;
+    for (int c = threadIdx.x; c < H; c += blockDim.x) { const float v = xr[c]; yrow[c] = v; ss = fmaf(v, v, ss); }
+    const float rs = 1.0f / sqrtf(block_sum(ss) / static_cast<float>(H) + eps);
+    float s2 = 0.f;
+    for (int c = threadIdx.x; c < H; c += blockDim.x) { const float v = w[c] * (yrow[c] * rs); yrow[c] = v; s2 = fmaf(v, v, s2); }
+    if (!head) {
+        const float tot = block_sum(s2);
+        const float inv = normalize ? 1.0f / fmaxf(sqrtf(tot), 1e-12f) : 1.0f;
+        for (int c = threadIdx.x; c < H; c += blockDim.x) out[static_cast<size_t>(b) * H + c] = yrow[c] * inv;
+        return;
+    }
+    __syncthreads();
+    for (int c = warp; c < num_labels; c += nw) {
+        const float* wr = head + static_cast<size_t>(c) * H;
+        float s = 0.f;
+        for (int d = lane; d < H; d += 32) s = fmaf(wr[d], yrow[d], s);
+        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+        if (lane == 0) out[static_cast<size_t>(b) * num_labels + c] = s;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// attention_causal_kernel: Qwen3's causal grouped-query attention at head_dim 128 (mma.sync m16n8k16, fp32 accumulate,
+// the three split products hi*hi + lo*hi + hi*lo of the other encoder kernels).  The planes [T, NH 128] hold q (pre-scaled
+// by log2(e) / sqrt(128)) | k | v, NH = heads + 2 kv_heads.  One CTA = (sequence, kv head, hpc of the kv head's G =
+// heads / kv_heads query heads, a block of 16 rb query rows, rb = 8 / hpc): its K / V are staged once for all hpc query
+// heads.  Warp w computes query head w % hpc on rows 16 (w / hpc) .. + 15 of the block.  The keys run in blocks of
+// kCausalKB through shared memory with an online softmax, so any length runs; a warp stops at its rows' diagonal and
+// masks j > i in the block that crosses it.  Every block a warp reads holds a key <= each of its rows (blocks start at
+// multiples of 32, its rows at a multiple of 16), so a row's running max is finite after the first block.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kCausalWarps = 8;
+constexpr int kCausalKB = 64;                 // keys staged per step
+constexpr int kCausalKSTR = kQwenHD + 8;      // staging row pitch in halves: conflict-free ldmatrix rows
+constexpr size_t kCausalSmem = 4 * sizeof(__half) * static_cast<size_t>(kCausalKB) * kCausalKSTR;
+
+__global__ void __launch_bounds__(kCausalWarps * 32, 1) attention_causal_kernel(const __half* __restrict__ ph,
+                                                                                 const __half* __restrict__ pl,
+                                                                                 const int* __restrict__ cu, int heads,
+                                                                                 int kv_heads, int hpc,
+                                                                                 __half* __restrict__ ctx_hi,
+                                                                                 __half* __restrict__ ctx_lo) {
+    constexpr int DH = kQwenHD, KS = DH / 16, NT = DH / 8, KSTR = kCausalKSTR;
+    extern __shared__ __align__(16) unsigned char causal_smem[];
+    __half* Kh = reinterpret_cast<__half*>(causal_smem);
+    __half* Kl = Kh + kCausalKB * KSTR;
+    __half* Vh = Kl + kCausalKB * KSTR;
+    __half* Vl = Vh + kCausalKB * KSTR;
+
+    const int G = heads / kv_heads, subs = G / hpc, rb = kCausalWarps / hpc;
+    const int kvh = blockIdx.x / subs, sub = blockIdx.x % subs;
+    const int b = blockIdx.y;
+    const int t0 = cu[b], S = cu[b + 1] - t0;
+    const int rbase = blockIdx.z * 16 * rb;
+    if (rbase >= S) return;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const size_t ld = static_cast<size_t>(heads + 2 * kv_heads) * DH;
+    const size_t kcol = static_cast<size_t>(heads + kvh) * DH, vcol = static_cast<size_t>(heads + kv_heads + kvh) * DH;
+    const int qh = kvh * G + sub * hpc + warp % hpc;
+    const int r0 = rbase + 16 * (warp / hpc);
+    const bool warp_live = warp < hpc * rb && r0 < S;
+
+    uint32_t qhf[KS][4], qlf[KS][4];
+    {
+        const __half* qhb = ph + static_cast<size_t>(t0) * ld + qh * DH;
+        const __half* qlb = pl + static_cast<size_t>(t0) * ld + qh * DH;
+        const int ra = r0 + g, rc = r0 + g + 8;
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) { qhf[ks][i] = 0u; qlf[ks][i] = 0u; }
+            if (warp_live && ra < S) {
+                qhf[ks][0] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t);
+                qlf[ks][0] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t);
+                qhf[ks][2] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t + 8);
+                qlf[ks][2] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t + 8);
+            }
+            if (warp_live && rc < S) {
+                qhf[ks][1] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t);
+                qlf[ks][1] = *reinterpret_cast<const uint32_t*>(qlb + rc * ld + ks * 16 + 2 * t);
+                qhf[ks][3] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t + 8);
+                qlf[ks][3] = *reinterpret_cast<const uint32_t*>(qlb + rc * ld + ks * 16 + 2 * t + 8);
+            }
+        }
+    }
+    float oacc[NT][4];
+#pragma unroll
+    for (int n = 0; n < NT; ++n) oacc[n][0] = oacc[n][1] = oacc[n][2] = oacc[n][3] = 0.f;
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+
+    const int kend = min(S, rbase + 16 * rb);       // keys any row of the CTA can see
+    for (int sb0 = 0; sb0 < kend; sb0 += kCausalKB) {
+        const int nk = min(kCausalKB, kend - sb0);
+        __syncthreads();
+        for (int e = threadIdx.x; e < kCausalKB * (DH / 8); e += blockDim.x) {
+            const int j = e / (DH / 8), c8 = (e % (DH / 8)) * 8;
+            uint4 kh = make_uint4(0, 0, 0, 0), kl = kh, vh = kh, vl = kh;
+            if (j < nk) {
+                const size_t o = static_cast<size_t>(t0 + sb0 + j) * ld + c8;
+                kh = *reinterpret_cast<const uint4*>(ph + o + kcol);
+                kl = *reinterpret_cast<const uint4*>(pl + o + kcol);
+                vh = *reinterpret_cast<const uint4*>(ph + o + vcol);
+                vl = *reinterpret_cast<const uint4*>(pl + o + vcol);
+            }
+            *reinterpret_cast<uint4*>(Kh + j * KSTR + c8) = kh;
+            *reinterpret_cast<uint4*>(Kl + j * KSTR + c8) = kl;
+            *reinterpret_cast<uint4*>(Vh + j * KSTR + c8) = vh;
+            *reinterpret_cast<uint4*>(Vl + j * KSTR + c8) = vl;
+        }
+        __syncthreads();
+        if (!warp_live) continue;
+        for (int kb0 = 0; kb0 < kCausalKB; kb0 += 32) {
+            const int j0 = sb0 + kb0;
+            if (j0 > r0 + 15) break;                      // above the diagonal of every row of the warp
+            float sacc[4][4];
+#pragma unroll
+            for (int n = 0; n < 4; ++n) sacc[n][0] = sacc[n][1] = sacc[n][2] = sacc[n][3] = 0.f;
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks) {
+                uint32_t bh[4][2], bl[4][2];
+                const int lrow = (lane & 7) + ((lane >> 4) << 3);
+                const int lcol = ks * 16 + ((lane >> 3) & 1) * 8;
+#pragma unroll
+                for (int n2 = 0; n2 < 2; ++n2) {
+                    uint32_t th[4], tl[4];
+                    ldmatrix_x4(th, Kh + (kb0 + n2 * 16 + lrow) * KSTR + lcol);
+                    ldmatrix_x4(tl, Kl + (kb0 + n2 * 16 + lrow) * KSTR + lcol);
+                    bh[2 * n2][0] = th[0]; bh[2 * n2][1] = th[1]; bh[2 * n2 + 1][0] = th[2]; bh[2 * n2 + 1][1] = th[3];
+                    bl[2 * n2][0] = tl[0]; bl[2 * n2][1] = tl[1]; bl[2 * n2 + 1][0] = tl[2]; bl[2 * n2 + 1][1] = tl[3];
+                }
+#pragma unroll
+                for (int n = 0; n < 4; ++n) mma16816(sacc[n], qhf[ks], bh[n]);
+#pragma unroll
+                for (int n = 0; n < 4; ++n) mma16816(sacc[n], qlf[ks], bh[n]);
+#pragma unroll
+                for (int n = 0; n < 4; ++n) mma16816(sacc[n], qhf[ks], bl[n]);
+            }
+            if (j0 + 31 > r0) {                            // the block crosses the diagonal: key j > row i is masked
+#pragma unroll
+                for (int n = 0; n < 4; ++n) {
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const int j = j0 + n * 8 + 2 * t + c;
+                        if (j > r0 + g) sacc[n][c] = -INFINITY;
+                        if (j > r0 + g + 8) sacc[n][2 + c] = -INFINITY;
+                    }
+                }
+            }
+            float bm0 = -INFINITY, bm1 = -INFINITY;
+#pragma unroll
+            for (int n = 0; n < 4; ++n) {
+                bm0 = fmaxf(bm0, fmaxf(sacc[n][0], sacc[n][1]));
+                bm1 = fmaxf(bm1, fmaxf(sacc[n][2], sacc[n][3]));
+            }
+            bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 1));
+            bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 2));
+            bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 1));
+            bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 2));
+            const float mn0 = fmaxf(m0, bm0), mn1 = fmaxf(m1, bm1);
+            const float c0 = fast_exp2(m0 - mn0), c1 = fast_exp2(m1 - mn1);
+            m0 = mn0; m1 = mn1;
+            float ps0 = 0.f, ps1 = 0.f;
+#pragma unroll
+            for (int n = 0; n < 4; ++n) {
+                sacc[n][0] = fast_exp2(sacc[n][0] - mn0); sacc[n][1] = fast_exp2(sacc[n][1] - mn0);
+                sacc[n][2] = fast_exp2(sacc[n][2] - mn1); sacc[n][3] = fast_exp2(sacc[n][3] - mn1);
+                ps0 += sacc[n][0] + sacc[n][1];
+                ps1 += sacc[n][2] + sacc[n][3];
+            }
+            l0 = l0 * c0 + ps0;
+            l1 = l1 * c1 + ps1;
+#pragma unroll
+            for (int n = 0; n < NT; ++n) { oacc[n][0] *= c0; oacc[n][1] *= c0; oacc[n][2] *= c1; oacc[n][3] *= c1; }
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk) {
+                if (j0 + kk * 16 > r0 + 15) continue;       // every key of the half is masked for every row
+                uint32_t pfh[4], pfl[4];
+                split_pack(sacc[2 * kk][0], sacc[2 * kk][1], pfh[0], pfl[0]);
+                split_pack(sacc[2 * kk][2], sacc[2 * kk][3], pfh[1], pfl[1]);
+                split_pack(sacc[2 * kk + 1][0], sacc[2 * kk + 1][1], pfh[2], pfl[2]);
+                split_pack(sacc[2 * kk + 1][2], sacc[2 * kk + 1][3], pfh[3], pfl[3]);
+                const int krow = kb0 + kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+                const int dsel = (lane >> 4) * 8;
+#pragma unroll
+                for (int n2 = 0; n2 < NT / 2; ++n2) {
+                    uint32_t vh4[4], vl4[4];
+                    ldmatrix_x4_trans(vh4, Vh + krow * KSTR + n2 * 16 + dsel);
+                    ldmatrix_x4_trans(vl4, Vl + krow * KSTR + n2 * 16 + dsel);
+                    const uint32_t ha[2] = {vh4[0], vh4[1]}, hb[2] = {vh4[2], vh4[3]};
+                    const uint32_t la[2] = {vl4[0], vl4[1]}, lb[2] = {vl4[2], vl4[3]};
+                    mma16816(oacc[2 * n2], pfh, ha);
+                    mma16816(oacc[2 * n2 + 1], pfh, hb);
+                    mma16816(oacc[2 * n2], pfl, ha);
+                    mma16816(oacc[2 * n2 + 1], pfl, hb);
+                    mma16816(oacc[2 * n2], pfh, la);
+                    mma16816(oacc[2 * n2 + 1], pfh, lb);
+                }
+            }
+        }
+    }
+    if (!warp_live) return;
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    const float i0 = 1.0f / l0, i1 = 1.0f / l1;
+    const int ra = r0 + g, rc = r0 + g + 8;
+    const size_t cld = static_cast<size_t>(heads) * DH;
+#pragma unroll
+    for (int n = 0; n < NT; ++n) {
+        const int col = qh * DH + n * 8 + 2 * t;
+        uint32_t hv, lv;
+        if (ra < S) {
+            split_pack(oacc[n][0] * i0, oacc[n][1] * i0, hv, lv);
+            *reinterpret_cast<uint32_t*>(ctx_hi + static_cast<size_t>(t0 + ra) * cld + col) = hv;
+            *reinterpret_cast<uint32_t*>(ctx_lo + static_cast<size_t>(t0 + ra) * cld + col) = lv;
+        }
+        if (rc < S) {
+            split_pack(oacc[n][2] * i1, oacc[n][3] * i1, hv, lv);
+            *reinterpret_cast<uint32_t*>(ctx_hi + static_cast<size_t>(t0 + rc) * cld + col) = hv;
+            *reinterpret_cast<uint32_t*>(ctx_lo + static_cast<size_t>(t0 + rc) * cld + col) = lv;
+        }
+    }
+}
+
+// query heads per CTA for a group of G: all of them up to 8, else the largest divisor of G up to 8
+static int causal_heads_per_cta(int G) {
+    int h = std::min(G, kCausalWarps);
+    while (G % h != 0) --h;
+    return h;
+}
+
+// E3 rms_split_kernel over T rows of H (H % 128 == 0, H <= 4096)
+static int launch_rms_split(const float* x, int T, int H, const float* w, float eps, __half* hi, __half* lo, int* flag,
+                            cudaStream_t st) {
+    if (T <= 0) return RMU_OK;
+    ProfScope _ps(PROF_LN, st);
+    rms_split_kernel<<<static_cast<unsigned>(T), kRmsThreads, 0, st>>>(x, H, w, eps, hi, lo, flag);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+static int launch_embed_rows(const int* ids, int T, int H, int vocab, const float* table, float* out, cudaStream_t st) {
+    const size_t n4 = static_cast<size_t>(T) * (H / 4);
+    ProfScope _ps(PROF_EMBED, st);
+    embed_rows_kernel<<<static_cast<unsigned>((n4 + 255) / 256), 256, 0, st>>>(ids, n4, H, vocab, table, out);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+static int launch_qk_norm_rope(const float* qkv, int T, int heads, int kv_heads, const int* pos, const float* qn,
+                               const float* kn, float eps, float qscale, const float* rcos, const float* rsin, int rope_rows,
+                               __half* hi, __half* lo, int* flag, cudaStream_t st) {
+    const size_t warps = static_cast<size_t>(T) * (heads + 2 * kv_heads);
+    ProfScope _ps(PROF_MISC, st);
+    qk_norm_rope_kernel<<<static_cast<unsigned>((warps + 7) / 8), 256, 0, st>>>(qkv, T, heads, kv_heads, pos, qn, kn, eps,
+                                                                             qscale, rcos, rsin, rope_rows, hi, lo, flag);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+static int launch_last_token(const float* x, const int* ids, const int* cu, int B, int H, const float* w, float eps,
+                             int pad_id, int normalize, const float* head, int num_labels, float* out, cudaStream_t st) {
+    ProfScope _ps(PROF_POOL_HEAD, st);
+    last_token_kernel<<<B, 256, H * sizeof(float), st>>>(x, ids, cu, H, w, eps, pad_id, normalize, head, num_labels, out);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// attention_causal_kernel over a ragged batch; the sequence index is gridDim.y, so batches above 65 535 sequences run
+// in slices, each launch with cu offset by the slice start (the token rows stay absolute)
+static int launch_attention_causal(const __half* qkv_hi, const __half* qkv_lo, const int* cu, int B, int heads, int kv_heads,
+                                   int max_seqlen, __half* ctx_hi, __half* ctx_lo, cudaStream_t st) {
+    const int G = heads / kv_heads, hpc = causal_heads_per_cta(G), rows = 16 * (kCausalWarps / hpc);
+    ProfScope _ps(PROF_ATTN, st);
+    RMU_CUDA(cudaFuncSetAttribute(attention_causal_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(kCausalSmem)));
+    const unsigned zb = static_cast<unsigned>((max_seqlen + rows - 1) / rows);
+    for (int s0 = 0; s0 < B; s0 += kMaxGridY) {
+        const int nb = std::min(kMaxGridY, B - s0);
+        dim3 grid(static_cast<unsigned>(kv_heads * (G / hpc)), static_cast<unsigned>(nb), zb);
+        attention_causal_kernel<<<grid, kCausalWarps * 32, kCausalSmem, st>>>(qkv_hi, qkv_lo, cu + s0, heads, kv_heads, hpc,
+                                                                              ctx_hi, ctx_lo);
+        count_launch();
+        RMU_CHECK_LAUNCH();
+    }
+    return RMU_OK;
+}
+
 }  // namespace rmu
 
 using namespace rmu;
@@ -1116,6 +1556,7 @@ struct EncLayer {
     float *d1 = nullptr, *d2 = nullptr;
     __half *pos_hi = nullptr, *pos_lo = nullptr;   // position_buckets > 0: PQ' | PK planes [2s, 2H] of the layer
     int window = 0;                       // ModernBERT: the layer's attention half-window (0 = global attention)
+    float *qn = nullptr, *kn = nullptr;   // Qwen3: q_norm, k_norm [128]
 };
 
 struct rmu_encoder {
@@ -1135,6 +1576,15 @@ struct rmu_encoder {
     float *fng = nullptr, *fnb = nullptr, *hng = nullptr, *hnb = nullptr;
     float *rope_cos[2] = {nullptr, nullptr}, *rope_sin[2] = {nullptr, nullptr};
     int mb_pool = RMU_POOL_CLS;
+    // Qwen3 (run_qwen3): ln1g = input_layernorm, Wqkv = q | k | v proj, Wo = o_proj, ln2g = post_attention_layernorm, W1 =
+    // gate | up in 64-row SwiGLU blocks, W2 = down_proj; fng = norm; cw = the last-token head [num_labels, H];
+    // rope_cos / rope_sin[0]; zeros = a zero bias for every projection (Qwen3 has none); QKVF the fp32 q | k | v rows
+    // before the q / k step; range_flag the fp16-range flag of the split kernels, read back after the layers
+    bool qwen = false;
+    rmu_qwen3_ext qext{};
+    float* zeros = nullptr;
+    float* QKVF = nullptr;
+    int* range_flag = nullptr;
     // activations
     int tok_cap = 0, seq_cap = 0;
     std::vector<void*> act_allocs;
@@ -1455,6 +1905,98 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
         }
         rc = launch_layernorm(e->PRE, T, H, L.ln2g, L.ln2b, c.ln_eps, e->X.hi, e->X.lo, st);
         if (rc != RMU_OK) return rc;
+    }
+    return RMU_OK;
+}
+
+// Qwen3's activation workspace (grown like ensure_tokens): X [cap, H] and CTX [cap, heads 128] planes (GEMM inputs), FF
+// [cap, F] planes, QKVP [cap, NQKV] planes and QKVF fp32, the residual stream PRE [cap, H] fp32, and POSI
+static int ensure_tokens_qwen3(rmu_encoder* e, int T, int B) {
+    if (T <= e->tok_cap && B + 1 <= e->seq_cap) return RMU_OK;
+    RMU_CUDA(cudaDeviceSynchronize());
+    free_acts(e);
+    const int H = e->cfg.hidden, F = e->cfg.ffn, QD = e->cfg.heads * kQwenHD;
+    const int NQKV = QD + 2 * e->qext.kv_heads * kQwenHD;
+    const int cap = (std::max(T, 1024) + 127) / 128 * 128, scap = std::max(B + 1, 1024);
+    auto planes = [&](SplitOperand* op, int cols) -> int {
+        __half *hi = nullptr, *lo = nullptr;
+        int rc = dev_alloc(e->act_allocs, &hi, static_cast<size_t>(cap) * cols);
+        if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &lo, static_cast<size_t>(cap) * cols);
+        if (rc != RMU_OK) return rc;
+        // zeros, as ensure_tokens: the GEMMs' A rows past a call's T are read (their outputs are clipped)
+        RMU_CUDA(cudaMemset(hi, 0, static_cast<size_t>(cap) * cols * sizeof(__half)));
+        RMU_CUDA(cudaMemset(lo, 0, static_cast<size_t>(cap) * cols * sizeof(__half)));
+        return make_split_operand(op, hi, lo, cap, cols);
+    };
+    int rc = planes(&e->X, H);
+    if (rc == RMU_OK) rc = planes(&e->CTX, QD);
+    if (rc == RMU_OK) rc = planes(&e->FF, F);
+    if (rc == RMU_OK) rc = planes(&e->QKVP, NQKV);
+    if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->QKVF, static_cast<size_t>(cap) * NQKV);
+    if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->PRE, static_cast<size_t>(cap) * H);
+    if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->POSI, cap);
+    if (rc != RMU_OK) { free_acts(e); return rc; }
+    e->tok_cap = cap;
+    e->seq_cap = scap;
+    return RMU_OK;
+}
+
+// Qwen3's layers (the header's formula): leaves the residual stream h, before the final norm, in e->PRE [T, H] fp32.
+// Per layer: X = split(w_in RMS(h)); QKVF = X Wqkv^T (fp32); QKVP = the q / k step; CTX = causal GQA attention;
+// h += CTX Wo^T (in place); X = split(w_post RMS(h)); FF = split(silu(X Wgate^T) * (X Wup^T)); h += FF Wdown^T.
+// The range flag is cleared first; the caller reads it (qwen3_check_range) before it writes an output.
+static int run_qwen3(rmu_encoder* e, const int32_t* ids, const int32_t* cu, int B, int T, int max_seqlen, cudaStream_t st) {
+    const rmu_bert_config& c = e->cfg;
+    if (max_seqlen > c.max_pos) { set_error("sequence longer than max_position_embeddings"); return RMU_ERR_ARG; }
+    const int H = c.hidden, F = c.ffn, nh = c.heads, kv = e->qext.kv_heads, QD = nh * kQwenHD;
+    const int NQKV = QD + 2 * kv * kQwenHD;
+    int rc = ensure_tokens_qwen3(e, T, B);
+    if (rc != RMU_OK) return rc;
+    RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace is shared by all callers
+    RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
+    rc = launch_seq_positions(cu, B, T, e->POSI, st);
+    if (rc == RMU_OK) rc = launch_embed_rows(ids, T, H, c.vocab_size, e->word, e->PRE, st);
+    if (rc != RMU_OK) return rc;
+    const float qscale = 1.4426950408889634f / sqrtf(static_cast<float>(kQwenHD));
+    for (int l = 0; l < c.layers; ++l) {
+        const EncLayer& L = e->layers[l];
+        rc = launch_rms_split(e->PRE, T, H, L.ln1g, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
+        if (rc != RMU_OK) return rc;
+        GemmParams g{};
+        g.M = T; g.N = NQKV; g.K = H; g.bias = e->zeros; g.out_f32 = e->QKVF;
+        rc = launch_gemm(GEMM_BIAS_F32, e->X, L.Wqkv, g, e->sms, st);
+        if (rc == RMU_OK)
+            rc = launch_qk_norm_rope(e->QKVF, T, nh, kv, e->POSI, L.qn, L.kn, c.ln_eps, qscale, e->rope_cos[0], e->rope_sin[0],
+                                     c.max_pos, e->QKVP.hi, e->QKVP.lo, e->range_flag, st);
+        if (rc == RMU_OK)
+            rc = launch_attention_causal(e->QKVP.hi, e->QKVP.lo, cu, B, nh, kv, max_seqlen, e->CTX.hi, e->CTX.lo, st);
+        if (rc != RMU_OK) return rc;
+        g = GemmParams{};
+        g.M = T; g.N = H; g.K = QD; g.bias = e->zeros; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
+        rc = launch_gemm(GEMM_BIAS_RESF32_F32, e->CTX, L.Wo, g, e->sms, st);
+        if (rc == RMU_OK) rc = launch_rms_split(e->PRE, T, H, L.ln2g, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
+        if (rc != RMU_OK) return rc;
+        g = GemmParams{};
+        g.M = T; g.N = 2 * F; g.K = H; g.bias = e->zeros; g.out_hi = e->FF.hi; g.out_lo = e->FF.lo; g.range_flag = e->range_flag;
+        rc = launch_gemm(GEMM_BIAS_SWIGLU_SPLIT, e->X, L.W1, g, e->sms, st);
+        if (rc != RMU_OK) return rc;
+        g = GemmParams{};
+        g.M = T; g.N = H; g.K = F; g.bias = e->zeros; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
+        rc = launch_gemm(GEMM_BIAS_RESF32_F32, e->FF, L.W2, g, e->sms, st);
+        if (rc != RMU_OK) return rc;
+    }
+    return RMU_OK;
+}
+
+// reads the range flag of run_qwen3's split kernels (synchronises st): RMU_ERR_RANGE when an activation left fp16's range
+static int qwen3_check_range(rmu_encoder* e, cudaStream_t st) {
+    int flag = 0;
+    RMU_CUDA(cudaMemcpyAsync(&flag, e->range_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    RMU_CUDA(cudaStreamSynchronize(st));
+    if (flag) {
+        set_error("Qwen3 forward: an activation entering a GEMM or attention left the fp16 range of the split planes "
+                  "(|x| > 65504); the encoder cannot compute this model's activations for this input");
+        return RMU_ERR_RANGE;
     }
     return RMU_OK;
 }
@@ -1810,6 +2352,128 @@ int rmu_encoder_create_modernbert(const rmu_bert_config* cfg, const rmu_modernbe
     return RMU_OK;
 }
 
+int rmu_encoder_create_qwen3(const rmu_bert_config* cfg, const rmu_qwen3_ext* qx, const float* const* w, int n_weights,
+                             int has_head, rmu_encoder** out) {
+    if (!cfg || !qx || !w || !out) { set_error("rmu_encoder_create_qwen3: bad argument"); return RMU_ERR_ARG; }
+    const int H = cfg->hidden, F = cfg->ffn, L = cfg->layers, nh = cfg->heads, kv = qx->kv_heads;
+    if (cfg->position_mode != RMU_POS_ABSOLUTE || cfg->rel_buckets != 0 || cfg->adapter_dim != 0) {
+        set_error("rmu_encoder_create_qwen3: position_mode, rel_buckets and adapter_dim must be 0 (rotary positions, no "
+                  "relative bias, no adapters)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (qx->head_dim != kQwenHD) {
+        set_error("rmu_encoder_create_qwen3: head_dim must be 128, got " + std::to_string(qx->head_dim));
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (H <= 0 || H % 128 != 0 || H > 4096) {
+        set_error("rmu_encoder_create_qwen3: hidden_size must be a multiple of 128 up to 4096, got " + std::to_string(H));
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (F <= 0 || F % 64 != 0) {
+        set_error("rmu_encoder_create_qwen3: intermediate_size must be a positive multiple of 64, got " + std::to_string(F));
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (nh <= 0 || kv <= 0 || nh % kv != 0) {
+        set_error("rmu_encoder_create_qwen3: num_attention_heads must be a multiple of num_key_value_heads (" +
+                  std::to_string(nh) + " heads, " + std::to_string(kv) + " kv heads)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (L < 1 || cfg->vocab_size <= 0 || cfg->max_pos <= 0 || cfg->num_labels <= 0) {
+        set_error("rmu_encoder_create_qwen3: unsupported shape (at least one layer, positive vocab, max_pos, num_labels)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (qx->rope_rows != cfg->max_pos || qx->rope_half != kQwenHD / 2) {
+        set_error("rmu_encoder_create_qwen3: the rope tables must be [max_pos, 64] = [" + std::to_string(cfg->max_pos) + ", 64]");
+        return RMU_ERR_ARG;
+    }
+    if (qx->head_form != (has_head ? RMU_QWEN3_HEAD_LAST : RMU_QWEN3_HEAD_NONE)) {
+        set_error("rmu_encoder_create_qwen3: head_form must be RMU_QWEN3_HEAD_LAST with a head, RMU_QWEN3_HEAD_NONE without");
+        return RMU_ERR_ARG;
+    }
+    const int QD = nh * kQwenHD, KD = kv * kQwenHD, NQKV = QD + 2 * KD;
+    const int norm0 = 1 + 11 * L, rope0 = norm0 + 1 + (has_head ? 1 : 0), expect = rope0 + 2;
+    if (n_weights != expect) {
+        set_error("rmu_encoder_create_qwen3: expected " + std::to_string(expect) + " weight tensors");
+        return RMU_ERR_ARG;
+    }
+    for (int j = 0; j < expect; ++j)
+        if (!w[j]) { set_error("rmu_encoder_create_qwen3: null weight tensor " + std::to_string(j)); return RMU_ERR_ARG; }
+    for (int l = 0; l < L; ++l) {
+        static const char* const kName[] = {"q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj"};
+        const int slot[] = {1, 2, 3, 6, 8, 9, 10};
+        const size_t count[] = {size_t(QD) * H, size_t(KD) * H, size_t(KD) * H, size_t(H) * QD, size_t(F) * H,
+                                size_t(F) * H, size_t(H) * F};
+        for (int k = 0; k < 7; ++k) {
+            const float* p = w[1 + 11 * l + slot[k]];
+            for (size_t j = 0; j < count[k]; ++j) {
+                if (std::fabs(p[j]) >= 65520.0f) {
+                    set_error("rmu_encoder_create_qwen3: layer " + std::to_string(l) + " " + kName[k] + " weight [" +
+                              std::to_string(j) + "] = " + std::to_string(p[j]) +
+                              " is outside the split fp16 planes' range (|w| < 65520)");
+                    return RMU_ERR_UNSUPPORTED;
+                }
+            }
+        }
+    }
+    rmu_encoder* e = new rmu_encoder();
+    e->cfg = *cfg;
+    e->has_head = has_head;
+    e->qwen = true;
+    e->qext = *qx;
+    if (cudaGetDevice(&e->device) != cudaSuccess || (e->sms = device_sm_count()) <= 0 ||
+        cudaEventCreateWithFlags(&e->ws_done, cudaEventDisableTiming) != cudaSuccess) {
+        set_error("rmu_encoder_create_qwen3: no CUDA device (this library has no CPU path)");
+        delete e;
+        return RMU_ERR_CUDA;
+    }
+    int rc = RMU_OK;
+    int i = 0;
+    auto up = [&](float** dst, size_t n) { if (rc == RMU_OK) rc = upload(e, dst, w[i], n); ++i; };
+    up(&e->word, static_cast<size_t>(cfg->vocab_size) * H);
+    e->layers.resize(L);
+    for (int l = 0; l < L && rc == RMU_OK; ++l) {
+        EncLayer& Ly = e->layers[l];
+        up(&Ly.ln1g, H);
+        if (rc == RMU_OK) {
+            std::vector<float> qkv(static_cast<size_t>(NQKV) * H);
+            std::copy(w[i], w[i] + size_t(QD) * H, qkv.begin());
+            std::copy(w[i + 1], w[i + 1] + size_t(KD) * H, qkv.begin() + size_t(QD) * H);
+            std::copy(w[i + 2], w[i + 2] + size_t(KD) * H, qkv.begin() + size_t(QD + KD) * H);
+            rc = upload_split(e, &Ly.Wqkv, {qkv.data()}, NQKV, H);
+        }
+        i += 3;
+        up(&Ly.qn, kQwenHD);
+        up(&Ly.kn, kQwenHD);
+        if (rc == RMU_OK) rc = upload_split(e, &Ly.Wo, {w[i]}, H, QD);
+        ++i;
+        up(&Ly.ln2g, H);
+        if (rc == RMU_OK) {
+            // gate | up -> 128-row blocks of 64 gate rows (silu's input) and the 64 matching up rows
+            std::vector<float> gu(static_cast<size_t>(2) * F * H);
+            std::copy(w[i], w[i] + size_t(F) * H, gu.begin());
+            std::copy(w[i + 1], w[i + 1] + size_t(F) * H, gu.begin() + size_t(F) * H);
+            const std::vector<float> blocked = geglu_rows(gu.data(), F, H);
+            rc = upload_split(e, &Ly.W1, {blocked.data()}, 2 * F, H);
+        }
+        i += 2;
+        if (rc == RMU_OK) rc = upload_split(e, &Ly.W2, {w[i]}, H, F);
+        ++i;
+    }
+    up(&e->fng, H);
+    if (has_head) up(&e->cw, static_cast<size_t>(cfg->num_labels) * H);
+    const size_t tab = static_cast<size_t>(cfg->max_pos) * (kQwenHD / 2);
+    up(&e->rope_cos[0], tab);
+    up(&e->rope_sin[0], tab);
+    if (rc == RMU_OK) {
+        const std::vector<float> zeros(static_cast<size_t>(std::max({NQKV, 2 * F, H})), 0.f);
+        rc = upload(e, &e->zeros, zeros.data(), zeros.size());
+    }
+    if (rc == RMU_OK) rc = dev_alloc(e->allocs, &e->range_flag, 1);
+    if (rc != RMU_OK) { rmu_encoder_destroy(e); return rc; }
+    *out = e;
+    return RMU_OK;
+}
+
 void rmu_encoder_destroy(rmu_encoder* e) {
     if (!e) return;
     cudaDeviceSynchronize();
@@ -1824,6 +2488,18 @@ int rmu_encoder_embed(rmu_encoder* e, const int32_t* ids, const int32_t* type_id
                       int max_seqlen, int pool_mode, int normalize, float* out, void* stream) {
     int rc = check_batch(e, ids, cu, B, T, out);
     if (rc != RMU_OK) return rc;
+    if (e->qwen) {
+        if (pool_mode != RMU_POOL_LAST) { set_error("Qwen3 encoders pool by the last token only (RMU_POOL_LAST)"); return RMU_ERR_ARG; }
+        std::lock_guard<std::mutex> g(e->mu);
+        cudaStream_t st = static_cast<cudaStream_t>(stream);
+        rc = run_qwen3(e, ids, cu, B, T, max_seqlen, st);
+        if (rc == RMU_OK) rc = qwen3_check_range(e, st);
+        if (rc == RMU_OK)
+            rc = launch_last_token(e->PRE, ids, cu, B, e->cfg.hidden, e->fng, e->cfg.ln_eps, -1, normalize, nullptr, 0, out, st);
+        if (rc != RMU_OK) return rc;
+        RMU_CUDA(cudaEventRecord(e->ws_done, st));
+        return RMU_OK;
+    }
     if (pool_mode != RMU_POOL_MEAN && pool_mode != RMU_POOL_CLS) { set_error("bad pool_mode"); return RMU_ERR_ARG; }
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1844,6 +2520,16 @@ int rmu_encoder_classify(rmu_encoder* e, const int32_t* ids, const int32_t* type
     if (!e->has_head) { set_error("rmu_encoder_classify: encoder was created without a classification head"); return RMU_ERR_ARG; }
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (e->qwen) {
+        rc = run_qwen3(e, ids, cu, B, T, max_seqlen, st);
+        if (rc == RMU_OK) rc = qwen3_check_range(e, st);
+        if (rc == RMU_OK)
+            rc = launch_last_token(e->PRE, ids, cu, B, e->cfg.hidden, e->fng, e->cfg.ln_eps, e->qext.pad_token_id, 0, e->cw,
+                                   e->cfg.num_labels, out, st);
+        if (rc != RMU_OK) return rc;
+        RMU_CUDA(cudaEventRecord(e->ws_done, st));
+        return RMU_OK;
+    }
     rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, true, st);
     if (rc != RMU_OK) return rc;
     if (e->modern) {
@@ -1869,7 +2555,14 @@ int rmu_encoder_hidden(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
     if (rc != RMU_OK) return rc;
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, false, st);
+    if (e->qwen) {
+        // the final norm into the X planes, then joined like every other encoder's hidden state
+        rc = run_qwen3(e, ids, cu, B, T, max_seqlen, st);
+        if (rc == RMU_OK) rc = launch_rms_split(e->PRE, T, e->cfg.hidden, e->fng, e->cfg.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
+        if (rc == RMU_OK) rc = qwen3_check_range(e, st);
+    } else {
+        rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, false, st);
+    }
     if (rc != RMU_OK) return rc;
     rc = launch_join_planes(e->X.hi, e->X.lo, static_cast<size_t>(T) * e->cfg.hidden, out, st);
     if (rc != RMU_OK) return rc;
@@ -2394,6 +3087,52 @@ int rmu_debug_modernbert_head(const float* pooled, int B, int H, int num_labels,
     }
     return launch_mb_head(pooled, B, H, num_labels, dense_w, dense_b, norm_w, norm_b, eps, cw, cb, out,
                           static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_rmsnorm(const float* x, int T, int H, const float* w, float eps, uint16_t* hi, uint16_t* lo,
+                      int32_t* range_flag, void* stream) {
+    if (!x || !w || !hi || !lo || T <= 0 || H <= 0) { set_error("rmu_debug_rmsnorm: bad argument"); return RMU_ERR_ARG; }
+    if (H % 128 != 0 || H > 4096) { set_error("rmu_debug_rmsnorm: H must be a multiple of 128 up to 4096"); return RMU_ERR_UNSUPPORTED; }
+    return launch_rms_split(x, T, H, w, eps, reinterpret_cast<__half*>(hi), reinterpret_cast<__half*>(lo), range_flag,
+                            static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_qk_norm_rope(const float* qkv, int T, int heads, int kv_heads, const int32_t* pos, const float* q_norm,
+                           const float* k_norm, float eps, float qscale, const float* rope_cos, const float* rope_sin,
+                           int rope_rows, uint16_t* hi, uint16_t* lo, int32_t* range_flag, void* stream) {
+    if (!qkv || !pos || !q_norm || !k_norm || !rope_cos || !rope_sin || !hi || !lo || T <= 0 || heads <= 0 ||
+        kv_heads <= 0 || rope_rows <= 0) {
+        set_error("rmu_debug_qk_norm_rope: bad argument");
+        return RMU_ERR_ARG;
+    }
+    return launch_qk_norm_rope(qkv, T, heads, kv_heads, pos, q_norm, k_norm, eps, qscale, rope_cos, rope_sin, rope_rows,
+                               reinterpret_cast<__half*>(hi), reinterpret_cast<__half*>(lo), range_flag,
+                               static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_attention_causal(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu, int B, int heads,
+                               int kv_heads, int max_seqlen, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream) {
+    if (!qkv_hi || !qkv_lo || !cu || !ctx_hi || !ctx_lo || B <= 0 || heads <= 0 || kv_heads <= 0 || max_seqlen <= 0) {
+        set_error("rmu_debug_attention_causal: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (heads % kv_heads != 0) {
+        set_error("rmu_debug_attention_causal: heads must be a multiple of kv_heads");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_attention_causal(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), cu, B,
+                                   heads, kv_heads, max_seqlen, reinterpret_cast<__half*>(ctx_hi),
+                                   reinterpret_cast<__half*>(ctx_lo), static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_last_token(const float* x, const int32_t* ids, const int32_t* cu, int B, int H, const float* w, float eps,
+                         int pad_id, int normalize, const float* head, int num_labels, float* out, void* stream) {
+    if (!x || !ids || !cu || !w || !out || B <= 0 || H <= 0 || (head && num_labels <= 0)) {
+        set_error("rmu_debug_last_token: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (H % 128 != 0 || H > 4096) { set_error("rmu_debug_last_token: H must be a multiple of 128 up to 4096"); return RMU_ERR_UNSUPPORTED; }
+    return launch_last_token(x, ids, cu, B, H, w, eps, pad_id, normalize, head, num_labels, out, static_cast<cudaStream_t>(stream));
 }
 
 int rmu_debug_split_planes(const float* src, int64_t n, uint16_t* hi, uint16_t* lo, void* stream) {

@@ -51,7 +51,13 @@ enum GemmMode {
     GEMM_BIAS_GEGLU_SPLIT = 5,  // W's rows in 128-row blocks of 64 input rows | the 64 matching gate rows: out planes
                                 // [M, N / 2] = split(gelu_erf(in + b_in) * (gate + b_gate))
     GEMM_BIAS_RESF32_F32 = 6,   // out_f32 = acc + bias + res_f32 (res_f32 may be out_f32: in place)
+    // Qwen3 (SwiGLU):
+    GEMM_BIAS_SWIGLU_SPLIT = 7, // GEMM_BIAS_GEGLU_SPLIT's row blocks with silu in place of gelu: out planes [M, N / 2] =
+                                // split(silu(in + b_in) * (gate + b_gate)); an output row < M with |x| > 65504 (or
+                                // NaN) sets *range_flag when it is non-null
 };
+// the modes whose W holds 64-row input | gate blocks and whose tiles write 64 output columns
+__host__ __device__ constexpr bool gemm_gated(int mode) { return mode == GEMM_BIAS_GEGLU_SPLIT || mode == GEMM_BIAS_SWIGLU_SPLIT; }
 
 struct GemmParams {
     int M, N, K;
@@ -66,6 +72,7 @@ struct GemmParams {
     const int* pos;                       // [M] GEMM_BIAS_SPLIT_ROPE: each row's position within its sequence
     const float* rope_cos; const float* rope_sin;   // [rope_rows, rope_hd / 2] fp32 tables
     int rope_hd, rope_rows;               // head dim (32 or 64) and the tables' rows (positions clamp into them)
+    int* range_flag;                      // GEMM_BIAS_SWIGLU_SPLIT: set to 1 when an output leaves the fp16 range
 };
 
 __device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {
@@ -233,7 +240,7 @@ gemm_f16x3_kernel(const __grid_constant__ CUtensorMap tAh, const __grid_constant
                   const GemmParams p) {
     constexpr bool kF32Out = MODE == GEMM_BIAS_F32 || MODE == GEMM_BIAS_RESID_F32 || MODE == GEMM_BIAS_RESF32_F32;
     constexpr int kJB = kF32Out ? 4 : 8;                       // 8-column groups per 128-byte box row
-    constexpr int kBoxes = MODE == GEMM_BIAS_GEGLU_SPLIT ? 1 : kGemmBN / 8 / kJB;   // GeGLU: 64 output columns per tile
+    constexpr int kBoxes = gemm_gated(MODE) ? 1 : kGemmBN / 8 / kJB;   // GeGLU / SwiGLU: 64 output columns per tile
     extern __shared__ uint8_t gemm_smem_raw[];
     // 1024-byte alignment by OFFSET into the shared array (the 128-byte swizzle repeats every 1024 B)
     uint8_t* smem = gemm_smem_raw + ((1024u - (smem_u32(gemm_smem_raw) & 1023u)) & 1023u);
@@ -296,7 +303,7 @@ gemm_f16x3_kernel(const __grid_constant__ CUtensorMap tAh, const __grid_constant
             uint32_t w[2][2][kJB][2];                                  // [r][h][jj]: fp32 (x, y) or (hi pair, lo pair)
             if constexpr (MODE == GEMM_BIAS_SPLIT_ROPE) {
                 rope_epilogue(acc, w, p, mb * kGemmBM + rsub, nb * kGemmBN + 64 * c, c, csub);
-            } else if constexpr (MODE == GEMM_BIAS_GEGLU_SPLIT) {
+            } else if constexpr (gemm_gated(MODE)) {
                 // columns 8 jj + csub of the block are inputs, 64 + 8 jj + csub their gates: both in this thread
 #pragma unroll
                 for (int r = 0; r < 2; ++r) {
@@ -307,8 +314,19 @@ gemm_f16x3_kernel(const __grid_constant__ CUtensorMap tAh, const __grid_constant
                         const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + col + 64));
 #pragma unroll
                         for (int h = 0; h < 2; ++h) {
-                            const float2 v = make_float2(gelu_erf(acc[r][4 * jj + 2 * h] + bi.x) * (acc[r][4 * (jj + 8) + 2 * h] + bg.x),
-                                                         gelu_erf(acc[r][4 * jj + 2 * h + 1] + bi.y) * (acc[r][4 * (jj + 8) + 2 * h + 1] + bg.y));
+                            float2 v;
+                            if constexpr (MODE == GEMM_BIAS_SWIGLU_SPLIT) {
+                                const float g0 = acc[r][4 * jj + 2 * h] + bi.x, g1 = acc[r][4 * jj + 2 * h + 1] + bi.y;
+                                v = make_float2(g0 / (1.0f + expf(-g0)) * (acc[r][4 * (jj + 8) + 2 * h] + bg.x),
+                                                g1 / (1.0f + expf(-g1)) * (acc[r][4 * (jj + 8) + 2 * h + 1] + bg.y));
+                                // rows past M hold whatever the A rows past M made (the TMA store clips them): not checked
+                                const int grow = mb * kGemmBM + r * 64 + rsub + 8 * h;
+                                if (p.range_flag && grow < p.M && !(fabsf(v.x) <= 65504.0f && fabsf(v.y) <= 65504.0f))
+                                    atomicOr(p.range_flag, 1);
+                            } else {
+                                v = make_float2(gelu_erf(acc[r][4 * jj + 2 * h] + bi.x) * (acc[r][4 * (jj + 8) + 2 * h] + bg.x),
+                                                gelu_erf(acc[r][4 * jj + 2 * h + 1] + bi.y) * (acc[r][4 * (jj + 8) + 2 * h + 1] + bg.y));
+                            }
                             __half2 h2, l2;
                             split_f16x2(v, h2, l2);
                             w[r][h][jj][0] = *reinterpret_cast<const uint32_t*>(&h2);
@@ -375,7 +393,7 @@ gemm_f16x3_kernel(const __grid_constant__ CUtensorMap tAh, const __grid_constant
                 fence_proxy_async_smem();                              // generic-proxy writes -> visible to the TMA store
                 bar_sync_named(kGemmEpiBar + wg, 128);
                 if (store_lead) {
-                    tma_store_2d(pl ? &tOb : &tOa, staging, MODE == GEMM_BIAS_GEGLU_SPLIT ? nb * 64 : nb * kGemmBN + 8 * kJB * c,
+                    tma_store_2d(pl ? &tOb : &tOa, staging, gemm_gated(MODE) ? nb * 64 : nb * kGemmBN + 8 * kJB * c,
                                  mb * kGemmBM);
                     bulk_commit();
                 }

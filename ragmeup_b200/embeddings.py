@@ -21,7 +21,7 @@ import numpy as np
 from . import _lib
 from .encoder import MAX_TOKENS_PER_CALL, BertEncoder
 from .tokenizer import RaggedTokenizer, load_tokenizer, pipelined
-from .weights import ModernBertConfig, MPNetConfig, XLMRConfig, resolve_model
+from .weights import ModernBertConfig, MPNetConfig, Qwen3Config, XLMRConfig, resolve_model
 
 PIPE_TEXTS = 1000     # texts per pipelined chunk of a bulk embed_documents() call
 
@@ -57,11 +57,14 @@ class HuggingFaceEmbeddings:
         self.normalize = bool(normalize or self.encode_kwargs.get("normalize_embeddings", False))
         self.max_seq_length = int(max_len)
         xlmr, modern = isinstance(cfg, XLMRConfig), isinstance(cfg, ModernBertConfig)
+        qwen = isinstance(cfg, Qwen3Config)
         self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, mpnet=isinstance(cfg, MPNetConfig), xlmr=xlmr,
-                                        modernbert=modern)
+                                        modernbert=modern, qwen3=qwen)
         self._ragged = RaggedTokenizer(self.tokenizer, self.max_seq_length)
-        # XLM-R / RoBERTa take no token types, ModernBERT has none: a null pointer, all zeros
-        self._types = not (xlmr or modern)
+        # XLM-R / RoBERTa take no token types, ModernBERT and Qwen3 have none: a null pointer, all zeros
+        self._types = not (xlmr or modern or qwen)
+        # Qwen3: the snapshot's default prompt (config_sentence_transformers.json default_prompt_name), if it sets one
+        self._prompt = cfg.prompt if qwen else ""
         self.client = BertEncoder(cfg, w, with_head=False, device=device)
 
     # -- tensor fast path (additional to the reference surface)
@@ -70,7 +73,7 @@ class HuggingFaceEmbeddings:
         torch = self.client.torch
         if len(texts) == 0:
             return torch.empty((0, self.config.hidden), dtype=torch.float32, device=self.client.device)
-        texts = [t.replace("\n", " ").strip() for t in texts]
+        texts = [self._prompt + t.replace("\n", " ").strip() for t in texts]
         ids, typ, cu = self._ragged(texts)
         outs = []
         for s, e in BertEncoder._chunks(cu, MAX_TOKENS_PER_CALL):
@@ -83,7 +86,7 @@ class HuggingFaceEmbeddings:
     def _encode_host(self, texts: List[str]) -> np.ndarray:
         if len(texts) == 0:
             return np.zeros((0, self.config.hidden), dtype=np.float32)
-        texts = [t.replace("\n", " ").strip() for t in texts]
+        texts = [self._prompt + t.replace("\n", " ").strip() for t in texts]
         # bulk calls: WordPiece of chunk i+1 overlapped with the device encode of chunk i
         chunks = [texts[s:s + PIPE_TEXTS] for s in range(0, len(texts), PIPE_TEXTS)]
         outs = pipelined(chunks, self._ragged, lambda t: self.client.embed_host(t[0], t[1] if self._types else None, t[2],

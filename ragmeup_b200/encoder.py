@@ -11,6 +11,12 @@ ModernBERT takes its own order (``weights.modernbert_weight_names``, ``rmu_encod
 embeddings and their norm; per layer attn_norm (layer 0: placeholders, not read), Wqkv, Wo, mlp_norm, Wi, mlp Wo, each
 with its bias (zeros where the checkpoint has none); final_norm; with a head, head.dense, head.norm and the classifier;
 then the four rope tables of ``weights.rope_tables``, computed here from the config.
+
+Qwen3 takes its own order too (``weights.qwen3_weight_names``, ``rmu_encoder_create_qwen3``): embed_tokens; per layer
+input_layernorm, q / k / v_proj, q_norm, k_norm, o_proj, post_attention_layernorm, gate / up / down_proj; norm; with a
+head the [num_labels, H] last-token head; then the cos / sin tables of ``weights.rope_table``.  It pools by the last
+token only (``pooling="last"``), and a forward whose activations leave the fp16 range of the split planes raises
+``RmuError`` naming the model.
 """
 from __future__ import annotations
 
@@ -20,9 +26,10 @@ from typing import Dict, Optional
 import numpy as np
 
 from . import _lib
-from .weights import BertConfig, ModernBertConfig, rope_tables, weight_names
+from .weights import BertConfig, ModernBertConfig, Qwen3Config, rope_table, rope_tables, weight_names
 
-POOL = {"mean": 0, "cls": 1}
+POOL = {"mean": 0, "cls": 1, "last": 2}
+RMU_ERR_RANGE = -4
 MAX_TOKENS_PER_CALL = 131072    # bounds the activation workspace (~19 KB/token for MiniLM shapes => ~2.5 GB)
 POSITION_WS_BYTES = 1 << 30     # DeBERTa: bound of the attention position terms' workspace, 2 T heads W fp32 per call
 
@@ -51,14 +58,21 @@ class BertEncoder:
             if tuple(a.shape) != tuple(shape):
                 raise ValueError(f"{name}: expected shape {shape}, got {a.shape}")
             arrs.append(a)
-        modern = isinstance(cfg, ModernBertConfig)
+        modern, qwen = isinstance(cfg, ModernBertConfig), isinstance(cfg, Qwen3Config)
         if modern:
             arrs += list(rope_tables(cfg))
+        if qwen:
+            arrs += list(rope_table(cfg.rope_theta, cfg.head_dim, cfg.max_pos))
         ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
         cc = _lib.bert_config_c(cfg)
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):
-            if modern:
+            if qwen:
+                qx = _lib.Qwen3ExtC(cfg.kv_heads, cfg.head_dim, cfg.max_pos, cfg.head_dim // 2, int(self.with_head),
+                                    cfg.head_pad_id)
+                _lib.check(_lib.lib().rmu_encoder_create_qwen3(C.byref(cc), C.byref(qx), ptrs, len(arrs), int(self.with_head),
+                                                               C.byref(self._h)), "rmu_encoder_create_qwen3")
+            elif modern:
                 win = np.ascontiguousarray(cfg.layer_windows, dtype=np.int32)
                 mb = _lib.ModernBertExtC(win.ctypes.data, POOL[cfg.classifier_pooling], 0, cfg.max_pos, cfg.head_dim // 2)
                 _lib.check(_lib.lib().rmu_encoder_create_modernbert(C.byref(cc), C.byref(mb), ptrs, len(arrs),
@@ -81,6 +95,13 @@ class BertEncoder:
                 pass
             self._h = C.c_void_p()
 
+    def _check(self, rc: int, what: str) -> None:
+        """``_lib.check``; an activation that left the fp16 range (Qwen3) raises naming the model"""
+        if rc == RMU_ERR_RANGE:
+            msg = _lib.lib().rmu_last_error()
+            raise _lib.RmuError(f"{getattr(self.cfg, 'name', 'model')}: {what} failed: {msg.decode() if msg else '?'}")
+        _lib.check(rc, what)
+
     # ------------------------------------------------------------------ device-tensor entry points
     def _dev(self, a, dtype):
         torch = self.torch
@@ -97,7 +118,7 @@ class BertEncoder:
         B = cu.numel() - 1
         out = torch.empty((B, self.cfg.hidden), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().rmu_encoder_embed(self._h, ids.data_ptr(), None if typ is None else typ.data_ptr(),
+            self._check(_lib.lib().rmu_encoder_embed(self._h, ids.data_ptr(), None if typ is None else typ.data_ptr(),
                                                     cu.data_ptr(), B, ids.numel(), int(max_seqlen), POOL[pooling],
                                                     int(bool(normalize)), out.data_ptr(), _lib.stream_ptr()),
                        "rmu_encoder_embed")
@@ -112,7 +133,7 @@ class BertEncoder:
         B = cu.numel() - 1
         out = torch.empty((B, self.cfg.num_labels), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().rmu_encoder_classify(self._h, ids.data_ptr(), None if typ is None else typ.data_ptr(),
+            self._check(_lib.lib().rmu_encoder_classify(self._h, ids.data_ptr(), None if typ is None else typ.data_ptr(),
                                                        cu.data_ptr(), B, ids.numel(), int(max_seqlen), out.data_ptr(),
                                                        _lib.stream_ptr()), "rmu_encoder_classify")
         return out
@@ -126,7 +147,7 @@ class BertEncoder:
         B = cu.numel() - 1
         out = torch.empty((ids.numel(), self.cfg.hidden), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().rmu_encoder_hidden(self._h, ids.data_ptr(), None if typ is None else typ.data_ptr(),
+            self._check(_lib.lib().rmu_encoder_hidden(self._h, ids.data_ptr(), None if typ is None else typ.data_ptr(),
                                                      cu.data_ptr(), B, ids.numel(), int(max_seqlen), out.data_ptr(),
                                                      _lib.stream_ptr()), "rmu_encoder_hidden")
         return out
@@ -160,7 +181,7 @@ class BertEncoder:
                 sub_typ = None if typ is None else typ[t0:t1]
                 o = out[s:e]
                 maxlen = int(np.max(np.diff(sub_cu)))
-                _lib.check(_lib.lib().rmu_encoder_embed_host(
+                self._check(_lib.lib().rmu_encoder_embed_host(
                     self._h, sub_ids.ctypes.data, None if sub_typ is None else sub_typ.ctypes.data, sub_cu.ctypes.data,
                     e - s, t1 - t0, maxlen, POOL[pooling], int(bool(normalize)), o.ctypes.data, _lib.stream_ptr()),
                     "rmu_encoder_embed_host")
@@ -181,7 +202,7 @@ class BertEncoder:
                 sub_typ = None if typ is None else typ[t0:t1]
                 o = out[s:e]
                 maxlen = int(np.max(np.diff(sub_cu)))
-                _lib.check(_lib.lib().rmu_encoder_classify_host(
+                self._check(_lib.lib().rmu_encoder_classify_host(
                     self._h, sub_ids.ctypes.data, None if sub_typ is None else sub_typ.ctypes.data, sub_cu.ctypes.data,
                     e - s, t1 - t0, maxlen, o.ctypes.data, _lib.stream_ptr()), "rmu_encoder_classify_host")
         return out

@@ -169,13 +169,72 @@ def build_deberta_unigram(pieces: Sequence[Tuple[str, float]]) -> Tokenizer:
     return tok
 
 
+QWEN3_SPECIALS = ("<|endoftext|>", "<|im_start|>", "<|im_end|>")
+
+
+def build_byte_bpe(words: Sequence[str], specials: Sequence[str] = QWEN3_SPECIALS, append: Optional[str] = None) -> Tokenizer:
+    """A byte-level BPE in Qwen's form (ByteLevel pre-tokenizer and decoder, no unknown token): the 256 byte symbols,
+    then each of ``words`` (and its space-prefixed form) as one token through left-to-right merges, then ``specials`` as
+    special added tokens.  ``append`` (a special): the post-processor appends it to every single text and pair, as some
+    embedders' tokenizers append <|endoftext|>; else nothing is added."""
+    from tokenizers import decoders, models, pre_tokenizers
+    alphabet = pre_tokenizers.ByteLevel.alphabet()
+    vocab = {c: i for i, c in enumerate(sorted(alphabet))}
+    merges = []
+    for w in words:
+        for form in ("\u0120" + w, w):        # the space-prefixed form first: its merges must outrank the bare word's
+            form = "".join(bytes_to_byte_level(form))
+            cur = form[0]
+            for ch in form[1:]:
+                if cur + ch not in vocab:
+                    merges.append((cur, ch))
+                    vocab[cur + ch] = len(vocab)
+                cur = cur + ch
+    tok = Tokenizer(models.BPE(vocab=vocab, merges=merges))
+    tok.pre_tokenizer = pre_tokenizers.ByteLevel(add_prefix_space=False, use_regex=True)
+    tok.decoder = decoders.ByteLevel()
+    tok.add_special_tokens(list(specials))
+    if append is None:
+        tok.post_processor = processors.ByteLevel(trim_offsets=False)
+    else:
+        tok.post_processor = processors.TemplateProcessing(single=f"$A {append}", pair=f"$A $B:1 {append}:1",
+                                                           special_tokens=[(append, tok.token_to_id(append))])
+    return tok
+
+
+def bytes_to_byte_level(text: str) -> List[str]:
+    """text -> its ByteLevel symbols (GPT-2's byte-to-unicode map; the space-prefix marker \u0120 is kept as it is)"""
+    from tokenizers import pre_tokenizers
+    if text.startswith("\u0120"):
+        return ["\u0120"] + bytes_to_byte_level(text[1:])
+    pieces = pre_tokenizers.ByteLevel(add_prefix_space=False, use_regex=False).pre_tokenize_str(text)
+    return list("".join(p for p, _ in pieces))
+
+
+def synthetic_qwen3_tokenizer(vocab_size: int) -> Tokenizer:
+    """the synthetic presets' byte-level BPE: the words of synthetic_vocab that fit below vocab_size, with the Qwen
+    specials and single ``yes`` / ``no`` tokens"""
+    room = max(0, vocab_size - 256 - len(QWEN3_SPECIALS) - 16)
+    words = ["yes", "no"] + [w for w in synthetic_vocab(min(30522, max(room, 1))) if w.isalpha() and len(w) > 2]
+    tok = build_byte_bpe(words[:max(2, room // 8)])
+    if tok.get_vocab_size() > vocab_size:
+        raise ValueError(f"synthetic Qwen3 tokenizer: {tok.get_vocab_size()} tokens do not fit vocab_size {vocab_size}")
+    return tok
+
+
 def load_tokenizer(source: Optional[str], vocab_size: int = 30522, mpnet: bool = False, xlmr: bool = False,
-                   deberta: bool = False, modernbert: bool = False) -> Tokenizer:
+                   deberta: bool = False, modernbert: bool = False, qwen3: bool = False) -> Tokenizer:
     """``source`` = snapshot dir (tokenizer.json or vocab.txt) or None -> synthetic vocab; ``mpnet`` selects MPNet's
     vocabulary layout and templates where the snapshot has no tokenizer.json.  ``xlmr`` (XLM-R / RoBERTa) and
     ``deberta`` (DeBERTa-v2 / v3): a snapshot must have tokenizer.json (read by ``tokenizers``); None -> the synthetic
     Unigram vocabulary of that family.  ``modernbert``: a snapshot must have tokenizer.json (ModernBERT's BPE with the
-    template ``[CLS] A [SEP] B [SEP]``); None -> the synthetic WordPiece vocabulary, which has the same template."""
+    template ``[CLS] A [SEP] B [SEP]``); None -> the synthetic WordPiece vocabulary, which has the same template.
+    ``qwen3``: a snapshot's tokenizer.json (its byte-level BPE and post-processor as they are); None -> the synthetic
+    byte-level BPE of ``synthetic_qwen3_tokenizer``."""
+    if qwen3:
+        if source is None:
+            return synthetic_qwen3_tokenizer(vocab_size)
+        return Tokenizer.from_file(os.path.join(source, "tokenizer.json"))
     if modernbert and source is not None:
         tj = os.path.join(source, "tokenizer.json")
         if os.path.exists(tj):

@@ -321,16 +321,20 @@ def rope_tables(cfg: ModernBertConfig):
     ``ModernBertRotaryEmbedding`` computes them: ``inv_freq = 1 / (theta ** (arange(0, d, 2).float() / d))``, the angle
     ``pos * inv_freq`` in float32, then ``.cos()`` / ``.sin()``.  At pos ~ 8000 one float32 ulp of the angle is ~5e-4 rad,
     so these float32 tables define the model: the float64 oracle looks its cos / sin up in them too."""
+    return (*rope_table(cfg.global_theta, cfg.head_dim, cfg.max_pos), *rope_table(cfg.local_theta, cfg.head_dim, cfg.max_pos))
+
+
+def rope_table(theta: float, head_dim: int, rows: int):
+    """(cos, sin), each [rows, head_dim / 2] float32, of the default rotary embedding as transformers computes it
+    (``ModernBertRotaryEmbedding``, ``Qwen3RotaryEmbedding``): ``inv_freq = 1 / (theta ** (arange(0, d, 2).float() /
+    d))``, the angle ``pos * inv_freq`` in float32, then ``.cos()`` / ``.sin()``."""
     import torch
-    d = cfg.head_dim
-    pos = torch.arange(cfg.max_pos, dtype=torch.int64).float()
-    out = []
-    for theta in (cfg.global_theta, cfg.local_theta):
-        inv_freq = 1.0 / (theta ** (torch.arange(0, d, 2, dtype=torch.int64).float() / d))
-        ang = pos[:, None] * inv_freq[None, :]
-        out += [np.ascontiguousarray(ang.cos().numpy(), dtype=np.float32),
-                np.ascontiguousarray(ang.sin().numpy(), dtype=np.float32)]
-    return tuple(out)
+    d = head_dim
+    pos = torch.arange(rows, dtype=torch.int64).float()
+    inv_freq = 1.0 / (theta ** (torch.arange(0, d, 2, dtype=torch.int64).float() / d))
+    ang = pos[:, None] * inv_freq[None, :]
+    return (np.ascontiguousarray(ang.cos().numpy(), dtype=np.float32),
+            np.ascontiguousarray(ang.sin().numpy(), dtype=np.float32))
 
 
 def modernbert_weight_names(cfg: ModernBertConfig, with_head: bool):
@@ -373,6 +377,138 @@ def modernbert_to_canonical(raw: Dict[str, np.ndarray], cfg: ModernBertConfig, w
     return w
 
 
+@dataclass
+class Qwen3Config(BertConfig):
+    """Qwen3 (transformers ``Qwen3Model`` / ``Qwen3ForSequenceClassification`` / ``Qwen3ForCausalLM``; Qwen3-Embedding,
+    Qwen3-Reranker): a decoder run as an encoder.  RMSNorm (``w * (x * rsqrt(mean(x^2) + eps))``), grouped-query causal
+    attention with ``kv_heads`` key / value heads of ``head_dim`` (128), per-head RMSNorm of q and k, rotary positions
+    (``rope_theta``), a SwiGLU feed-forward and no biases.  Its outputs take one row per sequence: the last token
+    (embedders), or with a head the rightmost token whose id != ``pad_token_id`` (``Qwen3ForSequenceClassification``)
+    or the last token (the causal-LM reranker, ``head_pad_id`` -1).  ``head`` in the weight dict is the [num_labels, H]
+    last-token head; ``name`` names the model in errors."""
+    vocab_size: int = 151669
+    hidden: int = 1024
+    layers: int = 28
+    heads: int = 16
+    ffn: int = 3072
+    max_pos: int = 40960
+    type_vocab: int = 1
+    ln_eps: float = 1e-6
+    kv_heads: int = 8
+    head_dim: int = 128
+    rope_theta: float = 1000000.0
+    tie_word_embeddings: bool = True
+    pad_token_id: Optional[int] = None
+    name: str = "qwen3"
+    reranker: bool = False      # a Qwen3ForCausalLM reranker: head = the [no, yes] rows of lm_head, read at the last token
+    prompt: str = ""            # the embedder's default prompt (config_sentence_transformers.json), prepended to texts
+
+    @property
+    def head_pad_id(self) -> int:
+        """the id the last-token head skips from the right: ``pad_token_id`` (sequence classification); -1 (the last
+        token) for the causal-LM reranker or without a pad id"""
+        return -1 if self.reranker or self.pad_token_id is None else int(self.pad_token_id)
+
+    @staticmethod
+    def from_hf(d: dict, name: str = "qwen3") -> "Qwen3Config":
+        """config.json of a ``qwen3`` checkpoint -> Qwen3Config; refuses, naming the field, what the encoder does not
+        compute"""
+        def refuse(field, value, why):
+            raise ValueError(f"{name}: qwen3 with {field} = {value!r} is not supported: {why}")
+        if d.get("model_type", "qwen3") != "qwen3":
+            refuse("model_type", d.get("model_type"), "only model_type 'qwen3' runs as Qwen3 (not MoE or Qwen2)")
+        if d.get("hidden_act", "silu") != "silu":
+            refuse("hidden_act", d.get("hidden_act"), "only SwiGLU (silu) is computed")
+        if d.get("attention_bias", False):
+            refuse("attention_bias", d["attention_bias"], "q / k / v / o have no biases in the encoder")
+        if d.get("use_sliding_window", False):
+            refuse("use_sliding_window", d["use_sliding_window"], "only full causal attention is computed")
+        for t in d.get("layer_types") or ():
+            if t != "full_attention":
+                refuse("layer_types", t, "only full_attention layers are computed")
+        if d.get("rope_scaling"):
+            refuse("rope_scaling", d["rope_scaling"], "RoPE scaling is not computed")
+        rp = d.get("rope_parameters") or {}
+        if rp.get("rope_type", "default") != "default":
+            refuse("rope_type", rp.get("rope_type"), "only the default rotary embedding is computed")
+        theta = rp.get("rope_theta", d.get("rope_theta", 10000.0))
+        H, nh = int(d["hidden_size"]), int(d["num_attention_heads"])
+        pad = d.get("pad_token_id")
+        return Qwen3Config(vocab_size=int(d["vocab_size"]), hidden=H, layers=int(d["num_hidden_layers"]), heads=nh,
+                           ffn=int(d["intermediate_size"]), max_pos=int(d.get("max_position_embeddings", 40960)),
+                           ln_eps=float(d.get("rms_norm_eps", 1e-6)),
+                           num_labels=len(d["id2label"]) if "id2label" in d else d.get("num_labels", 1),
+                           kv_heads=int(d.get("num_key_value_heads") or nh), head_dim=int(d.get("head_dim") or H // nh),
+                           rope_theta=float(theta), tie_word_embeddings=bool(d.get("tie_word_embeddings", False)),
+                           pad_token_id=None if pad is None else int(pad), name=name)
+
+
+def qwen3_weight_names(cfg: Qwen3Config, with_head: bool):
+    """canonical Qwen3 tensors (transformers' names without ``model.``) in rmu_encoder_create_qwen3's order; ``head``
+    [num_labels, H] is the last-token head (``score.weight``, or the yes / no rows of ``lm_head``)"""
+    H, F, d = cfg.hidden, cfg.ffn, cfg.head_dim
+    names = [("embed_tokens.weight", (cfg.vocab_size, H))]
+    for l in range(cfg.layers):
+        p = f"layers.{l}."
+        names += [(p + "input_layernorm.weight", (H,)), (p + "self_attn.q_proj.weight", (cfg.heads * d, H)),
+                  (p + "self_attn.k_proj.weight", (cfg.kv_heads * d, H)),
+                  (p + "self_attn.v_proj.weight", (cfg.kv_heads * d, H)), (p + "self_attn.q_norm.weight", (d,)),
+                  (p + "self_attn.k_norm.weight", (d,)), (p + "self_attn.o_proj.weight", (H, cfg.heads * d)),
+                  (p + "post_attention_layernorm.weight", (H,)), (p + "mlp.gate_proj.weight", (F, H)),
+                  (p + "mlp.up_proj.weight", (F, H)), (p + "mlp.down_proj.weight", (H, F))]
+    names.append(("norm.weight", (H,)))
+    if with_head:
+        names.append(("head", (cfg.num_labels, H)))
+    return names
+
+
+def qwen3_to_canonical(raw: Dict[str, np.ndarray], cfg: Qwen3Config) -> Dict[str, np.ndarray]:
+    """Qwen3 tensors under ``model.`` (as every transformers class saves them) or bare -> the names of
+    ``qwen3_weight_names``; ``score.weight`` (sequence classification) becomes ``head``, ``lm_head.weight`` is dropped
+    (the reranker reads its two rows itself)."""
+    w: Dict[str, np.ndarray] = {}
+    for k, v in raw.items():
+        if k == "lm_head.weight":
+            continue
+        k = "head" if k == "score.weight" else (k[6:] if k.startswith("model.") else k)
+        w[k] = np.ascontiguousarray(v, dtype=np.float32)
+    return w
+
+
+def synthetic_qwen3_weights(cfg: Qwen3Config, seed: int = 0, with_head: bool = False,
+                            scale: float = 1.0) -> Dict[str, np.ndarray]:
+    """seeded Qwen3 weights: projections N(0, 0.02 scale), norm weights near 1, embeddings N(0, 0.02) (transformers'
+    init, with norm gains spread so a wrong weight layout shows in the numbers)"""
+    rng = np.random.default_rng(seed)
+    out: Dict[str, np.ndarray] = {}
+    for name, shape in qwen3_weight_names(cfg, with_head):
+        if name.endswith("norm.weight") or name.endswith("layernorm.weight"):
+            a = 1.0 + 0.1 * rng.standard_normal(shape)
+        elif name == "embed_tokens.weight":
+            a = 0.02 * rng.standard_normal(shape) * (3.0 if scale > 1 else 1.0)
+        else:
+            a = 0.02 * scale * rng.standard_normal(shape)
+        out[name] = np.ascontiguousarray(a, dtype=np.float32)
+    return out
+
+
+def qwen3_lm_rows(path: str, cfg: Qwen3Config, ids) -> np.ndarray:
+    """rows ``ids`` of ``lm_head.weight`` (``embed_tokens`` when the embeddings are tied or the head is absent), read
+    one row at a time from the snapshot's safetensors -> float32 [len(ids), H]"""
+    import torch
+    from safetensors import safe_open
+    names = ["lm_head.weight"] if not cfg.tie_word_embeddings else []
+    names += ["model.embed_tokens.weight", "embed_tokens.weight"]
+    files = _safetensors_files(path)
+    for name in names:
+        for f in files:
+            with safe_open(f, framework="pt") as fh:
+                if name in fh.keys():
+                    sl = fh.get_slice(name)
+                    return np.stack([sl[int(i):int(i) + 1].to(torch.float32).numpy()[0] for i in ids]).astype(np.float32)
+    raise KeyError(f"{path}: no lm_head.weight or embed_tokens.weight to read the reranker's yes / no rows from")
+
+
 REL_EMB = "encoder.rel_embeddings.weight"
 REL_LN = ("encoder.LayerNorm.weight", "encoder.LayerNorm.bias")
 
@@ -400,7 +536,7 @@ def adapter_prefix(layer: int, language: str) -> str:
 
 
 # config.json model_type -> how the snapshot is read; a config without model_type is read as BERT
-MODEL_TYPES = ("bert", "mpnet", "roberta", "xlm-roberta", "xmod", "deberta-v2", "modernbert")
+MODEL_TYPES = ("bert", "mpnet", "roberta", "xlm-roberta", "xmod", "deberta-v2", "modernbert", "qwen3")
 
 
 # shapes of the models BASELINE.json / .env.template name (SURVEY.md §2.2 table)
@@ -455,6 +591,12 @@ PRESETS: Dict[str, Tuple[BertConfig, str, int]] = {
     "tiny-modernbert-window": (ModernBertConfig(vocab_size=1000, hidden=128, layers=4, heads=2, ffn=192, max_pos=1024,
                                                 layer_windows=modernbert_windows(4, 3, 32), classifier_pooling="mean"),
                                "mean", 1024),
+    # Qwen3: the 0.6B shape of Qwen3-Embedding-0.6B and Qwen3-Reranker-0.6B [3P-recall: their config.json is not read
+    # here]; pooling "last" is the last-token row.  tiny-qwen3: head_dim 128, two query heads per kv head, three layers.
+    "qwen3-embedding-0.6b": (Qwen3Config(), "last", 8192),
+    "qwen3-reranker-0.6b": (Qwen3Config(reranker=True, num_labels=2), "last", 8192),
+    "tiny-qwen3": (Qwen3Config(vocab_size=1000, hidden=256, layers=3, heads=4, ffn=384, max_pos=8192, kv_heads=2,
+                               rope_theta=10000.0, tie_word_embeddings=False, pad_token_id=0), "last", 8192),
 }
 
 # presets whose sentence-transformers pipeline has no Normalize module
@@ -471,6 +613,8 @@ FLASHRANK_MODELS: Dict[str, str] = {
 
 
 def weight_names(cfg: BertConfig, with_head: bool):
+    if isinstance(cfg, Qwen3Config):
+        return qwen3_weight_names(cfg, with_head)
     if isinstance(cfg, ModernBertConfig):
         return modernbert_weight_names(cfg, with_head)
     H, F = cfg.hidden, cfg.ffn
@@ -618,12 +762,41 @@ def _load_tensors(path: str, keep=None) -> Dict[str, np.ndarray]:
         sd = torch.load(pt, weights_only=True, map_location="cpu")
         return {k: v.detach().to(torch.float32).numpy() for k, v in sd.items()
                 if v.is_floating_point() and (keep is None or keep(k))}
-    if keep is None:
-        from safetensors.numpy import load_file
-        return load_file(st)
+    if not os.path.exists(st) and os.path.exists(os.path.join(path, SHARD_INDEX)):
+        out: Dict[str, np.ndarray] = {}
+        for f in _safetensors_files(path):
+            out.update(_load_safetensors(f, keep))
+        return out
+    return _load_safetensors(st, keep)
+
+
+SHARD_INDEX = "model.safetensors.index.json"
+
+
+def _safetensors_files(path: str):
+    """``model.safetensors``, or the shards ``model.safetensors.index.json`` lists, in its order"""
+    st = os.path.join(path, "model.safetensors")
+    idx = _read_json(os.path.join(path, SHARD_INDEX))
+    if os.path.exists(st) or idx is None:
+        return [st]
+    return [os.path.join(path, f) for f in dict.fromkeys(idx["weight_map"].values())]
+
+
+def _load_safetensors(st: str, keep=None) -> Dict[str, np.ndarray]:
+    """one safetensors file (all tensors, or those ``keep`` selects) read by numpy; a file numpy cannot read (bfloat16,
+    which numpy has no type for) is read through torch instead, its bfloat16 tensors widened to float32 (exact)"""
     from safetensors import safe_open
-    with safe_open(st, framework="numpy") as f:
-        return {k: f.get_tensor(k) for k in f.keys() if keep(k)}
+    try:
+        if keep is None:
+            from safetensors.numpy import load_file
+            return load_file(st)
+        with safe_open(st, framework="numpy") as f:
+            return {k: f.get_tensor(k) for k in f.keys() if keep(k)}
+    except TypeError:
+        import torch
+        with safe_open(st, framework="pt") as f:
+            return {k: (t.to(torch.float32) if t.dtype == torch.bfloat16 else t).numpy()
+                    for k in f.keys() if keep is None or keep(k) for t in (f.get_tensor(k),)}
 
 
 def _xmod_keep(language: str):
@@ -641,6 +814,8 @@ def load_hf_snapshot(path: str, with_head: bool):
     kind = cfgd.get("model_type", "bert")
     if kind not in MODEL_TYPES:
         raise ValueError(f"{path}: model_type {kind!r} is not supported; the encoder runs {', '.join(MODEL_TYPES)}")
+    if kind == "qwen3":
+        return _load_qwen3_snapshot(path, cfgd, with_head)
     mpnet, xlmr, deberta = kind == "mpnet", kind in ("roberta", "xlm-roberta", "xmod"), kind == "deberta-v2"
     modern = kind == "modernbert"
     if mpnet and with_head:
@@ -718,6 +893,81 @@ def load_hf_snapshot(path: str, with_head: bool):
     return cfg, w, pooling, normalize, max_len, act
 
 
+# Qwen3-Reranker's prompt, from its model card [3P-recall: the card is not readable here]: the chat prefix with the
+# judging instruction, the suffix that opens an empty <think> block, and the default task instruction.  The score is
+# P(yes) = exp(log_softmax([logit("no"), logit("yes")])[1]) at the last token.
+QWEN3_RERANK_PREFIX = ("<|im_start|>system\nJudge whether the Document meets the requirements based on the Query and the "
+                       "Instruct provided. Note that the answer can only be \"yes\" or \"no\".<|im_end|>\n"
+                       "<|im_start|>user\n")
+QWEN3_RERANK_SUFFIX = "<|im_end|>\n<|im_start|>assistant\n<think>\n\n</think>\n\n"
+QWEN3_RERANK_INSTRUCTION = "Given a web search query, retrieve relevant passages that answer the query"
+QWEN3_RERANK_MAX_LENGTH = 8192      # the model card's max_length [3P-recall]
+
+
+def _load_qwen3_snapshot(path: str, cfgd: dict, with_head: bool):
+    """a ``qwen3`` snapshot -> (config, weights, pooling, normalize, max_len, activation).  Embedders (no head) pool by
+    the last token; ``1_Pooling`` must say ``pooling_mode_lasttoken``.  With a head: ``Qwen3ForSequenceClassification``
+    (``score.weight``, needs ``pad_token_id``), or a causal LM (``Qwen3ForCausalLM``, Qwen3-Reranker), which scores
+    P(yes) from the [no, yes] rows of ``lm_head`` (activation ``"yes_prob"``)."""
+    if not os.path.exists(os.path.join(path, "tokenizer.json")):
+        raise ValueError(f"{path}: a qwen3 snapshot needs tokenizer.json (its byte-level BPE has no other file form here)")
+    cfg = Qwen3Config.from_hf(cfgd, name=path)
+    archs = cfgd.get("architectures") or []
+    names = set().union(*[_tensor_names_file(f) for f in _safetensors_files(path)])
+    seqcls = "score.weight" in names or "Qwen3ForSequenceClassification" in archs
+    keep = (lambda n: n not in ("lm_head.weight", "score.weight")) if not with_head else (lambda n: n != "lm_head.weight")
+    w = qwen3_to_canonical(_load_tensors(path, keep), cfg)
+    act = "identity"
+    if with_head and seqcls:
+        if cfg.pad_token_id is None:
+            raise ValueError(f"{path}: a Qwen3ForSequenceClassification snapshot needs pad_token_id: its head reads the "
+                             f"rightmost token that is not padding (transformers refuses batches without it)")
+        cfg.num_labels = int(w["head"].shape[0])
+        a = cfgd.get("sbert_ce_default_activation_function")
+        act = ("sigmoid" if cfg.num_labels == 1 else "identity") if a is None else ("sigmoid" if "Sigmoid" in a else "identity")
+    elif with_head:
+        from tokenizers import Tokenizer
+        tok = Tokenizer.from_file(os.path.join(path, "tokenizer.json"))
+        yes, no = tok.token_to_id("yes"), tok.token_to_id("no")
+        if yes is None or no is None:
+            raise ValueError(f"{path}: the reranker's tokenizer has no single 'yes' / 'no' tokens to score with")
+        cfg.reranker, cfg.num_labels = True, 2
+        w["head"] = qwen3_lm_rows(path, cfg, [no, yes])
+        act = "yes_prob"
+    missing = [n for n, _ in qwen3_weight_names(cfg, with_head) if n not in w]
+    if missing:
+        raise KeyError(f"{path}: missing tensors {missing[:4]}...")
+    tc = _read_json(os.path.join(path, "tokenizer_config.json")) or {}
+    max_len = cfg.max_pos
+    if cfg.reranker:
+        max_len = min(max_len, QWEN3_RERANK_MAX_LENGTH)
+    if tc.get("model_max_length") is not None:
+        max_len = min(int(tc["model_max_length"]), max_len)
+    normalize = False
+    for m in _read_json(os.path.join(path, "modules.json")) or []:
+        if m.get("type", "").endswith("Pooling"):
+            pc = _read_json(os.path.join(path, m["path"], "config.json")) or {}
+            other = [k for k, v in pc.items() if k.startswith("pooling_mode_") and v and k != "pooling_mode_lasttoken"]
+            if not pc.get("pooling_mode_lasttoken") or other:
+                raise ValueError(f"{path}: Qwen3 embedders pool by the last token only; {m['path']} asks for "
+                                 f"{other or 'no pooling_mode_lasttoken'}")
+        if m.get("type", "").endswith("Normalize"):
+            normalize = True
+    sb = _read_json(os.path.join(path, "sentence_bert_config.json"))
+    if sb and sb.get("max_seq_length"):
+        max_len = min(int(sb["max_seq_length"]), cfg.max_pos)
+    st = _read_json(os.path.join(path, "config_sentence_transformers.json")) or {}
+    if st.get("default_prompt_name"):
+        cfg.prompt = (st.get("prompts") or {})[st["default_prompt_name"]]
+    return cfg, {n: w[n] for n, _ in qwen3_weight_names(cfg, with_head)}, "last", normalize, max_len, act
+
+
+def _tensor_names_file(st: str):
+    from safetensors import safe_open
+    with safe_open(st, framework="numpy") as f:
+        return set(f.keys())
+
+
 def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] = None):
     """model id -> (cfg, weights, pooling, normalize, max_seq_length, activation, vocab_source).
 
@@ -736,6 +986,11 @@ def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] 
         if isinstance(cfg, DebertaConfig) and not with_head:
             raise ValueError(f"synthetic preset {preset!r}: model_type 'deberta-v2' runs as a cross-encoder only")
         cfg = type(cfg)(**asdict(cfg))
+        if isinstance(cfg, Qwen3Config):
+            cfg.name = model_name
+            w = synthetic_qwen3_weights(cfg, seed=seed, with_head=with_head, scale=scale)
+            act = ("yes_prob" if cfg.reranker else "sigmoid") if with_head else "identity"
+            return cfg, w, pooling, preset not in UNNORMALIZED_PRESETS, max_len, act, None
         if isinstance(cfg, XmodConfig):
             cfg.language = select_language(cfg.languages, cfg.language, model_name)
         w = synthetic_bert_weights(cfg, seed=seed, with_head=with_head, scale=scale)
@@ -841,6 +1096,9 @@ def load_colbert_snapshot(path: str):
     if kind == "modernbert":
         raise ValueError(f"{path}: a ColBERT checkpoint of model_type 'modernbert' is not supported: ModernBERT runs as a "
                          f"cross-encoder or an embedder")
+    if kind == "qwen3":
+        raise ValueError(f"{path}: a ColBERT checkpoint of model_type 'qwen3' is not supported: Qwen3 runs as a "
+                         f"cross-encoder or an embedder")
     if kind not in ("bert", "xlm-roberta", "roberta", "xmod"):
         raise ValueError(f"{path}: a ColBERT checkpoint of model_type {kind!r} is not supported (bert, xlm-roberta, "
                          f"roberta and xmod are)")
@@ -896,7 +1154,8 @@ def resolve_colbert(model_name: str, cache_folder: Optional[str] = None):
     for c in cands:
         if os.path.isdir(c):
             cfgd = _read_json(os.path.join(c, "config.json"))
-            if cfgd is None or cfgd.get("model_type", "bert") not in MODEL_TYPES or not is_colbert_snapshot(c):
+            if cfgd is None or cfgd.get("model_type", "bert") not in MODEL_TYPES or cfgd.get("model_type") == "qwen3" \
+                    or not is_colbert_snapshot(c):
                 return None
             if cfgd.get("model_type") == "xmod":
                 try:
@@ -908,6 +1167,9 @@ def resolve_colbert(model_name: str, cache_folder: Optional[str] = None):
 
 
 def _refuse_xlmr_flashrank(cfg: BertConfig, where: str) -> None:
+    if isinstance(cfg, Qwen3Config):
+        raise ValueError(f"{where}: a Qwen3 (model_type 'qwen3') model is not a FlashRank model (FlashRank's rerankers "
+                         f"are BERT checkpoints); use HuggingFaceCrossEncoder for it")
     if isinstance(cfg, ModernBertConfig):
         raise ValueError(f"{where}: a ModernBERT (model_type 'modernbert') model is not a FlashRank model (FlashRank's "
                          f"rerankers are BERT checkpoints); use HuggingFaceCrossEncoder for it")
