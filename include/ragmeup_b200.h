@@ -295,6 +295,25 @@ typedef struct rmu_qwen3_ext {
 } rmu_qwen3_ext;
 int rmu_encoder_create_qwen3(const rmu_bert_config* cfg, const rmu_qwen3_ext* ext, const float* const* weights_h,
                              int n_weights, int has_head, rmu_encoder** out);
+/* Llama-3 (transformers LlamaModel, model_type "llama"): the Qwen3 decoder above without the per-head q / k RMSNorm.
+ * weights_h in Qwen3's order without q_norm and k_norm: embed_tokens; per layer input_layernorm, q_proj, k_proj, v_proj,
+ * o_proj, post_attention_layernorm, gate_proj, up_proj, down_proj; norm; rope cos, sin (the caller's table, e.g. with
+ * llama3 frequency scaling).  1 + 9 layers + 1 + 2 tensors.  No head: ext->head_form must be RMU_QWEN3_HEAD_NONE.  The
+ * shape and weight refusals of rmu_encoder_create_qwen3 apply, before any CUDA call.  rmu_encoder_embed (RMU_POOL_LAST)
+ * and rmu_encoder_hidden take it like a Qwen3 embedder. */
+int rmu_encoder_create_llama(const rmu_bert_config* cfg, const rmu_qwen3_ext* ext, const float* const* weights_h,
+                             int n_weights, rmu_encoder** out);
+/* Attention mass of the last layer over token spans of ONE sequence ids [T] (device int32):
+ *   out[a][b] = sum over query heads h, rows i in span a, keys j in span b of P_h[i, j]
+ * (device float64 [n_spans, n_spans]), P_h the last layer's causal softmax (0 for j > i; query head h reads kv head
+ * h / (heads / kv_heads)).  spans [n_spans][2] device int32 (start, end): rows / keys start <= i < end, clamped into
+ * [0, T); end <= start is empty; spans may overlap, nest or repeat.  Layers 0..L-2 run as the forward does; the last
+ * runs to its q / k step only, and P is never stored.  Each out[a][b] is a float64 sum in a fixed order (the same
+ * inputs give the same bits).  Only encoders from rmu_encoder_create_qwen3 without a head or rmu_encoder_create_llama;
+ * another encoder, null pointers, T < 1, T > max_pos or n_spans < 1 return RMU_ERR_ARG before any CUDA call; an
+ * activation outside the split planes' fp16 range returns RMU_ERR_RANGE and writes nothing.  Synchronises `stream`. */
+int rmu_decoder_attention_spans(rmu_encoder* enc, const int32_t* ids, int T, const int32_t* spans, int n_spans,
+                                double* out, void* stream);
 void rmu_encoder_destroy(rmu_encoder* enc);
 
 #define RMU_POOL_MEAN 0
@@ -429,6 +448,12 @@ int rmu_debug_qk_norm_rope(const float* qkv, int T, int heads, int kv_heads, con
  * keys j <= i; query head h reads kv head h / (heads / kv_heads).  heads % kv_heads != 0 returns RMU_ERR_UNSUPPORTED. */
 int rmu_debug_attention_causal(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu_seqlens, int B,
                                int heads, int kv_heads, int max_seqlen, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream);
+/* For tests: the span attention of rmu_decoder_attention_spans on given planes [T, (heads + 2 kv_heads) 128] of one
+ * sequence (q pre-scaled by log2(e) / sqrt(128), as the q / k step leaves it) -> out [n_spans, n_spans] float64, spans as
+ * there.  Allocates its workspace stream-ordered on `stream`.  Null pointers, T, heads, kv_heads or n_spans < 1 return
+ * RMU_ERR_ARG, heads % kv_heads != 0 RMU_ERR_UNSUPPORTED, before any CUDA call. */
+int rmu_debug_attention_spans(const uint16_t* qkv_hi, const uint16_t* qkv_lo, int T, int heads, int kv_heads,
+                              const int32_t* spans, int n_spans, double* out, void* stream);
 /* For tests: Qwen3's output rows on fp32 residual rows x [T, H] (device): per sequence b the row cu[b + 1] - 1
  * (pad_id < 0) or the rightmost row whose ids[] != pad_id (none: the first row), y = w RMS(x_row); then out [B, H] = y
  * (optionally L2-normalised) when head is NULL, else out [B, num_labels] = head [num_labels, H] . y.  An empty sequence

@@ -106,6 +106,10 @@ SIGNATURES = {
                                                 C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "rmu_encoder_create_qwen3": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(Qwen3ExtC), C.POINTER(C.c_void_p), C.c_int,
                                            C.c_int, C.POINTER(C.c_void_p)]),
+    "rmu_encoder_create_llama": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(Qwen3ExtC), C.POINTER(C.c_void_p), C.c_int,
+                                           C.POINTER(C.c_void_p)]),
+    "rmu_decoder_attention_spans": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                              C.c_void_p]),
     "rmu_encoder_destroy": (None, [C.c_void_p]),
     "rmu_encoder_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_void_p, C.c_void_p]),
@@ -174,6 +178,8 @@ SIGNATURES = {
                                          C.c_void_p, C.c_void_p]),
     "rmu_debug_attention_causal": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                              C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_attention_spans": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                            C.c_void_p, C.c_void_p]),
     "rmu_debug_last_token": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float,
                                        C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "rmu_debug_split_planes": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),

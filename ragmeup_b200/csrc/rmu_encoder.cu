@@ -1164,7 +1164,9 @@ __global__ void embed_rows_kernel(const int* __restrict__ ids, size_t n4, int H,
 // heads, then k, then v); lane l holds dims 4l .. 4l + 3.  q and k heads: RMSNorm over the head with q_norm / k_norm,
 // then rotate-half rotary at the token's position, x'[c] = x[c] cos[c] - x[c + 64] sin[c] and x'[c + 64] = x[c + 64]
 // cos[c] + x[c] sin[c] for c < 64 (lane l < 16 holds c, lane l + 16 its partner), and q times qscale (log2(e) / sqrt(d),
-// the softmax runs in base 2).  Every head leaves as split planes of the same layout.
+// the softmax runs in base 2).  Every head leaves as split planes of the same layout.  kQkNorm false (Llama): no
+// per-head RMSNorm, qn / kn unread.
+template <bool kQkNorm>
 __global__ void __launch_bounds__(256) qk_norm_rope_kernel(const float* __restrict__ qkv, int T, int heads, int kv_heads,
                                                            const int* __restrict__ pos, const float* __restrict__ qn,
                                                            const float* __restrict__ kn, float eps, float qscale,
@@ -1180,13 +1182,15 @@ __global__ void __launch_bounds__(256) qk_norm_rope_kernel(const float* __restri
     const float4 in = *reinterpret_cast<const float4*>(qkv + o);
     float x[4] = {in.x, in.y, in.z, in.w};
     if (hh < heads + kv_heads) {
-        float ss = 0.f;
+        if (kQkNorm) {
+            float ss = 0.f;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) ss = fmaf(x[i], x[i], ss);
-        for (int k = 16; k > 0; k >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, k);
-        const float rs = 1.0f / sqrtf(ss / static_cast<float>(kQwenHD) + eps);
-        const float4 nw = *reinterpret_cast<const float4*>((hh < heads ? qn : kn) + lane * 4);
-        x[0] = nw.x * (x[0] * rs); x[1] = nw.y * (x[1] * rs); x[2] = nw.z * (x[2] * rs); x[3] = nw.w * (x[3] * rs);
+            for (int i = 0; i < 4; ++i) ss = fmaf(x[i], x[i], ss);
+            for (int k = 16; k > 0; k >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, k);
+            const float rs = 1.0f / sqrtf(ss / static_cast<float>(kQwenHD) + eps);
+            const float4 nw = *reinterpret_cast<const float4*>((hh < heads ? qn : kn) + lane * 4);
+            x[0] = nw.x * (x[0] * rs); x[1] = nw.y * (x[1] * rs); x[2] = nw.z * (x[2] * rs); x[3] = nw.w * (x[3] * rs);
+        }
         int p = pos[t];
         p = p < 0 ? 0 : (p >= rope_rows ? rope_rows - 1 : p);
         const int fi = (lane & 15) * 4;
@@ -1503,13 +1507,19 @@ static int launch_embed_rows(const int* ids, int T, int H, int vocab, const floa
     return RMU_OK;
 }
 
+// qn == nullptr (Llama): the q / k step without the per-head RMSNorm
 static int launch_qk_norm_rope(const float* qkv, int T, int heads, int kv_heads, const int* pos, const float* qn,
                                const float* kn, float eps, float qscale, const float* rcos, const float* rsin, int rope_rows,
                                __half* hi, __half* lo, int* flag, cudaStream_t st) {
     const size_t warps = static_cast<size_t>(T) * (heads + 2 * kv_heads);
     ProfScope _ps(PROF_MISC, st);
-    qk_norm_rope_kernel<<<static_cast<unsigned>((warps + 7) / 8), 256, 0, st>>>(qkv, T, heads, kv_heads, pos, qn, kn, eps,
-                                                                             qscale, rcos, rsin, rope_rows, hi, lo, flag);
+    const unsigned grid = static_cast<unsigned>((warps + 7) / 8);
+    if (qn)
+        qk_norm_rope_kernel<true><<<grid, 256, 0, st>>>(qkv, T, heads, kv_heads, pos, qn, kn, eps, qscale, rcos, rsin,
+                                                        rope_rows, hi, lo, flag);
+    else
+        qk_norm_rope_kernel<false><<<grid, 256, 0, st>>>(qkv, T, heads, kv_heads, pos, qn, kn, eps, qscale, rcos, rsin,
+                                                         rope_rows, hi, lo, flag);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
@@ -1538,6 +1548,349 @@ static int launch_attention_causal(const __half* qkv_hi, const __half* qkv_lo, c
         dim3 grid(static_cast<unsigned>(kv_heads * (G / hpc)), static_cast<unsigned>(nb), zb);
         attention_causal_kernel<<<grid, kCausalWarps * 32, kCausalSmem, st>>>(qkv_hi, qkv_lo, cu + s0, heads, kv_heads, hpc,
                                                                               ctx_hi, ctx_lo);
+        count_launch();
+        RMU_CHECK_LAUNCH();
+    }
+    return RMU_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Attention mass over token spans (rmu_decoder_attention_spans): out[a][b] = sum over query heads h, rows i in span a
+// and keys j in span b of P_h[i, j], P the causal softmax of one sequence's planes [T, NH 128] as
+// attention_causal_kernel reads them, never materialised.  Three kernels:
+//   A (spans_rowstat_kernel): per query head and row, the base-2 row max m and sum l = sum_j exp2(s_ij - m) of the
+//     causal scores, with attention_causal_kernel's CTA layout (K staged once per kv head for its query heads) and its
+//     three-product split mma.sync QK^T; [heads, T] each.
+//   B (spans_mass_kernel): the scores again, for 32-key blocks on or below the diagonal that meet a column span of the
+//     chunk (kSpanChunk spans per launch, so any span count runs); p = exp2(s - m) / l; each warp adds, per span of the
+//     chunk, its masked row sums into its own shared-memory rows [16][kSpanChunk] in key order, then writes
+//     M[h][b][i] (fp32) for its rows.  Every span's own keys are summed directly (no prefix differences).
+//   C (spans_reduce_kernel): out[a][b] = sum_h sum_{i in a} M[h][b][i] in float64, a fixed thread -> element map and
+//     a fixed tree, so the result is deterministic.
+// A and B skip every CTA whose rows meet no span.  Spans are [start, end) pairs (device), clamped into [0, T); end <=
+// start is empty.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kSpanChunk = 32;                // column spans per launch of B (one bit each in a warp's mask)
+constexpr size_t kSpanKSmem = 2 * sizeof(__half) * static_cast<size_t>(kCausalKB) * kCausalKSTR;
+
+__device__ __forceinline__ void span_bounds(const int* spans, int s, int T, int& lo, int& hi) {
+    lo = min(max(spans[2 * s], 0), T);
+    hi = min(max(spans[2 * s + 1], lo), T);
+}
+
+// 1 when rows [r0, r1) meet some span (block-uniform; every thread of the block calls it)
+__device__ __forceinline__ int rows_meet_spans(const int* spans, int n, int T, int r0, int r1) {
+    int hit = 0;
+    for (int s = threadIdx.x; s < n && !hit; s += blockDim.x) {
+        int lo, hi;
+        span_bounds(spans, s, T, lo, hi);
+        hit = lo < hi && lo < r1 && hi > r0;
+    }
+    return __syncthreads_or(hit);
+}
+
+// the warp's q fragments of rows r0 .. r0 + 15 of head qh (zero past T), as attention_causal_kernel loads them
+__device__ __forceinline__ void load_q_frags(const __half* ph, const __half* pl, size_t ld, int qh, int r0, int T, bool live,
+                                             uint32_t (&qhf)[kQwenHD / 16][4], uint32_t (&qlf)[kQwenHD / 16][4]) {
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const __half* qhb = ph + qh * kQwenHD;
+    const __half* qlb = pl + qh * kQwenHD;
+    const int ra = r0 + g, rc = r0 + g + 8;
+#pragma unroll
+    for (int ks = 0; ks < kQwenHD / 16; ++ks) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { qhf[ks][i] = 0u; qlf[ks][i] = 0u; }
+        if (live && ra < T) {
+            qhf[ks][0] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t);
+            qlf[ks][0] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t);
+            qhf[ks][2] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t + 8);
+            qlf[ks][2] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t + 8);
+        }
+        if (live && rc < T) {
+            qhf[ks][1] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t);
+            qlf[ks][1] = *reinterpret_cast<const uint32_t*>(qlb + rc * ld + ks * 16 + 2 * t);
+            qhf[ks][3] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t + 8);
+            qlf[ks][3] = *reinterpret_cast<const uint32_t*>(qlb + rc * ld + ks * 16 + 2 * t + 8);
+        }
+    }
+}
+
+// stage keys [sb0, sb0 + kCausalKB) of kv column kcol into Kh / Kl (zeros past T); the caller synchronises around it
+__device__ __forceinline__ void stage_keys(const __half* ph, const __half* pl, size_t ld, size_t kcol, int sb0, int T,
+                                           __half* Kh, __half* Kl) {
+    const int nk = min(kCausalKB, T - sb0);
+    for (int e = threadIdx.x; e < kCausalKB * (kQwenHD / 8); e += blockDim.x) {
+        const int j = e / (kQwenHD / 8), c8 = (e % (kQwenHD / 8)) * 8;
+        uint4 kh = make_uint4(0, 0, 0, 0), kl = kh;
+        if (j < nk) {
+            const size_t o = static_cast<size_t>(sb0 + j) * ld + kcol + c8;
+            kh = *reinterpret_cast<const uint4*>(ph + o);
+            kl = *reinterpret_cast<const uint4*>(pl + o);
+        }
+        *reinterpret_cast<uint4*>(Kh + j * kCausalKSTR + c8) = kh;
+        *reinterpret_cast<uint4*>(Kl + j * kCausalKSTR + c8) = kl;
+    }
+}
+
+// s[n][.] = the warp's 16 x 32 base-2 scores against staged keys kb0 .. kb0 + 31, keys j > row masked to -inf
+// (attention_causal_kernel's products and mask)
+__device__ __forceinline__ void score_block(const uint32_t (&qhf)[kQwenHD / 16][4], const uint32_t (&qlf)[kQwenHD / 16][4],
+                                            const __half* Kh, const __half* Kl, int kb0, int j0, int r0,
+                                            float (&sacc)[4][4]) {
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+#pragma unroll
+    for (int n = 0; n < 4; ++n) sacc[n][0] = sacc[n][1] = sacc[n][2] = sacc[n][3] = 0.f;
+#pragma unroll
+    for (int ks = 0; ks < kQwenHD / 16; ++ks) {
+        uint32_t bh[4][2], bl[4][2];
+        const int lrow = (lane & 7) + ((lane >> 4) << 3);
+        const int lcol = ks * 16 + ((lane >> 3) & 1) * 8;
+#pragma unroll
+        for (int n2 = 0; n2 < 2; ++n2) {
+            uint32_t th[4], tl[4];
+            ldmatrix_x4(th, Kh + (kb0 + n2 * 16 + lrow) * kCausalKSTR + lcol);
+            ldmatrix_x4(tl, Kl + (kb0 + n2 * 16 + lrow) * kCausalKSTR + lcol);
+            bh[2 * n2][0] = th[0]; bh[2 * n2][1] = th[1]; bh[2 * n2 + 1][0] = th[2]; bh[2 * n2 + 1][1] = th[3];
+            bl[2 * n2][0] = tl[0]; bl[2 * n2][1] = tl[1]; bl[2 * n2 + 1][0] = tl[2]; bl[2 * n2 + 1][1] = tl[3];
+        }
+#pragma unroll
+        for (int n = 0; n < 4; ++n) mma16816(sacc[n], qhf[ks], bh[n]);
+#pragma unroll
+        for (int n = 0; n < 4; ++n) mma16816(sacc[n], qlf[ks], bh[n]);
+#pragma unroll
+        for (int n = 0; n < 4; ++n) mma16816(sacc[n], qhf[ks], bl[n]);
+    }
+    if (j0 + 31 > r0) {
+#pragma unroll
+        for (int n = 0; n < 4; ++n) {
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const int j = j0 + n * 8 + 2 * t + c;
+                if (j > r0 + g) sacc[n][c] = -INFINITY;
+                if (j > r0 + g + 8) sacc[n][2 + c] = -INFINITY;
+            }
+        }
+    }
+}
+
+// A: grid (kv_heads * G / hpc, 1, row blocks of 16 rb rows), kCausalWarps warps; m / l [heads, T]
+__global__ void __launch_bounds__(kCausalWarps * 32, 1) spans_rowstat_kernel(const __half* __restrict__ ph,
+                                                                              const __half* __restrict__ pl, int T,
+                                                                              int heads, int kv_heads, int hpc,
+                                                                              const int* __restrict__ spans, int n_spans,
+                                                                              float* __restrict__ m_out,
+                                                                              float* __restrict__ l_out) {
+    extern __shared__ __align__(16) unsigned char span_smem[];
+    __half* Kh = reinterpret_cast<__half*>(span_smem);
+    __half* Kl = Kh + kCausalKB * kCausalKSTR;
+    const int G = heads / kv_heads, subs = G / hpc, rb = kCausalWarps / hpc;
+    const int kvh = blockIdx.x / subs, sub = blockIdx.x % subs;
+    const int rbase = blockIdx.z * 16 * rb;
+    const int kend = min(T, rbase + 16 * rb);
+    if (!rows_meet_spans(spans, n_spans, T, rbase, kend)) return;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const size_t ld = static_cast<size_t>(heads + 2 * kv_heads) * kQwenHD;
+    const size_t kcol = static_cast<size_t>(heads + kvh) * kQwenHD;
+    const int qh = kvh * G + sub * hpc + warp % hpc;
+    const int r0 = rbase + 16 * (warp / hpc);
+    const bool warp_live = warp < hpc * rb && r0 < T;
+    uint32_t qhf[kQwenHD / 16][4], qlf[kQwenHD / 16][4];
+    load_q_frags(ph, pl, ld, qh, r0, T, warp_live, qhf, qlf);
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+    for (int sb0 = 0; sb0 < kend; sb0 += kCausalKB) {
+        __syncthreads();
+        stage_keys(ph, pl, ld, kcol, sb0, T, Kh, Kl);
+        __syncthreads();
+        if (!warp_live) continue;
+        for (int kb0 = 0; kb0 < kCausalKB; kb0 += 32) {
+            const int j0 = sb0 + kb0;
+            if (j0 > r0 + 15) break;
+            float sacc[4][4];
+            score_block(qhf, qlf, Kh, Kl, kb0, j0, r0, sacc);
+            float bm0 = -INFINITY, bm1 = -INFINITY;
+#pragma unroll
+            for (int n = 0; n < 4; ++n) {
+                bm0 = fmaxf(bm0, fmaxf(sacc[n][0], sacc[n][1]));
+                bm1 = fmaxf(bm1, fmaxf(sacc[n][2], sacc[n][3]));
+            }
+            bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 1));
+            bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 2));
+            bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 1));
+            bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 2));
+            const float mn0 = fmaxf(m0, bm0), mn1 = fmaxf(m1, bm1);
+            float ps0 = 0.f, ps1 = 0.f;
+#pragma unroll
+            for (int n = 0; n < 4; ++n) {
+                ps0 += fast_exp2(sacc[n][0] - mn0) + fast_exp2(sacc[n][1] - mn0);
+                ps1 += fast_exp2(sacc[n][2] - mn1) + fast_exp2(sacc[n][3] - mn1);
+            }
+            l0 = l0 * fast_exp2(m0 - mn0) + ps0;
+            l1 = l1 * fast_exp2(m1 - mn1) + ps1;
+            m0 = mn0; m1 = mn1;
+        }
+    }
+    if (!warp_live) return;
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    if (t == 0) {
+        const size_t o = static_cast<size_t>(qh) * T;
+        if (r0 + g < T) { m_out[o + r0 + g] = m0; l_out[o + r0 + g] = l0; }
+        if (r0 + g + 8 < T) { m_out[o + r0 + g + 8] = m1; l_out[o + r0 + g + 8] = l1; }
+    }
+}
+
+// B: grid as A; column spans c0 .. c0 + nc - 1 (nc <= kSpanChunk); M [heads, kSpanChunk, T] fp32, M[h][b][i] = the
+// mass row i of head h gives span c0 + b
+__global__ void __launch_bounds__(kCausalWarps * 32, 1) spans_mass_kernel(const __half* __restrict__ ph,
+                                                                           const __half* __restrict__ pl, int T, int heads,
+                                                                           int kv_heads, int hpc,
+                                                                           const int* __restrict__ spans, int n_spans,
+                                                                           int c0, int nc, const float* __restrict__ m_in,
+                                                                           const float* __restrict__ l_in,
+                                                                           float* __restrict__ M) {
+    extern __shared__ __align__(16) unsigned char span_smem[];
+    __half* Kh = reinterpret_cast<__half*>(span_smem);
+    __half* Kl = Kh + kCausalKB * kCausalKSTR;
+    float* acc = reinterpret_cast<float*>(Kl + kCausalKB * kCausalKSTR);   // [warps][16][kSpanChunk]
+    __shared__ int clo[kSpanChunk], chi[kSpanChunk];
+    const int G = heads / kv_heads, subs = G / hpc, rb = kCausalWarps / hpc;
+    const int kvh = blockIdx.x / subs, sub = blockIdx.x % subs;
+    const int rbase = blockIdx.z * 16 * rb;
+    const int kend = min(T, rbase + 16 * rb);
+    if (!rows_meet_spans(spans, n_spans, T, rbase, kend)) return;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    if (threadIdx.x < kSpanChunk) {
+        int lo = 0, hi = 0;
+        if (threadIdx.x < nc) span_bounds(spans, c0 + threadIdx.x, T, lo, hi);
+        clo[threadIdx.x] = lo;
+        chi[threadIdx.x] = hi;
+    }
+    float* wacc = acc + warp * 16 * kSpanChunk;
+    for (int e = lane; e < 16 * kSpanChunk; e += 32) wacc[e] = 0.f;
+    __syncthreads();
+    // the keys the chunk can see: from its first span start to the CTA's last row
+    int kmin = kend;
+    for (int b = 0; b < nc; ++b)
+        if (clo[b] < chi[b]) kmin = min(kmin, clo[b]);
+    const size_t ld = static_cast<size_t>(heads + 2 * kv_heads) * kQwenHD;
+    const size_t kcol = static_cast<size_t>(heads + kvh) * kQwenHD;
+    const int qh = kvh * G + sub * hpc + warp % hpc;
+    const int r0 = rbase + 16 * (warp / hpc);
+    const bool warp_live = warp < hpc * rb && r0 < T;
+    uint32_t qhf[kQwenHD / 16][4], qlf[kQwenHD / 16][4];
+    load_q_frags(ph, pl, ld, qh, r0, T, warp_live, qhf, qlf);
+    // rows past T take 1 / l = 0, so every p of theirs is 0
+    float mr0 = 0.f, mr1 = 0.f, il0 = 0.f, il1 = 0.f;
+    if (warp_live && r0 + g < T) { mr0 = m_in[static_cast<size_t>(qh) * T + r0 + g]; il0 = 1.0f / l_in[static_cast<size_t>(qh) * T + r0 + g]; }
+    if (warp_live && r0 + g + 8 < T) { mr1 = m_in[static_cast<size_t>(qh) * T + r0 + g + 8]; il1 = 1.0f / l_in[static_cast<size_t>(qh) * T + r0 + g + 8]; }
+    for (int sb0 = kmin / kCausalKB * kCausalKB; sb0 < kend; sb0 += kCausalKB) {
+        // a staged block that meets no span of the chunk is skipped (block-uniform)
+        bool any = false;
+        for (int b = 0; b < nc; ++b) any |= clo[b] < chi[b] && clo[b] < sb0 + kCausalKB && chi[b] > sb0;
+        if (!any) continue;
+        __syncthreads();
+        stage_keys(ph, pl, ld, kcol, sb0, T, Kh, Kl);
+        __syncthreads();
+        if (!warp_live) continue;
+        for (int kb0 = 0; kb0 < kCausalKB; kb0 += 32) {
+            const int j0 = sb0 + kb0;
+            if (j0 > r0 + 15) break;
+            const bool meets = lane < nc && clo[lane] < chi[lane] && clo[lane] < j0 + 32 && chi[lane] > j0;
+            unsigned mask = __ballot_sync(0xffffffffu, meets);
+            if (!mask) continue;
+            float sacc[4][4];
+            score_block(qhf, qlf, Kh, Kl, kb0, j0, r0, sacc);
+#pragma unroll
+            for (int n = 0; n < 4; ++n) {
+                sacc[n][0] = fast_exp2(sacc[n][0] - mr0) * il0; sacc[n][1] = fast_exp2(sacc[n][1] - mr0) * il0;
+                sacc[n][2] = fast_exp2(sacc[n][2] - mr1) * il1; sacc[n][3] = fast_exp2(sacc[n][3] - mr1) * il1;
+            }
+            while (mask) {
+                const int b = __ffs(mask) - 1;
+                mask &= mask - 1;
+                const int lo = clo[b], hi = chi[b];
+                float v0 = 0.f, v1 = 0.f;
+#pragma unroll
+                for (int n = 0; n < 4; ++n) {
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const int j = j0 + n * 8 + 2 * t + c;
+                        if (j >= lo && j < hi) { v0 += sacc[n][c]; v1 += sacc[n][2 + c]; }
+                    }
+                }
+                v0 += __shfl_xor_sync(0xffffffffu, v0, 1);
+                v0 += __shfl_xor_sync(0xffffffffu, v0, 2);
+                v1 += __shfl_xor_sync(0xffffffffu, v1, 1);
+                v1 += __shfl_xor_sync(0xffffffffu, v1, 2);
+                if (t == 0) {
+                    wacc[g * kSpanChunk + b] += v0;
+                    wacc[(g + 8) * kSpanChunk + b] += v1;
+                }
+            }
+        }
+    }
+    if (!warp_live) return;
+    __syncwarp();
+    for (int e = lane; e < 16 * nc; e += 32) {
+        const int b = e / 16, r = e % 16;
+        if (r0 + r < T) M[(static_cast<size_t>(qh) * kSpanChunk + b) * T + r0 + r] = wacc[r * kSpanChunk + b];
+    }
+}
+
+// C: grid (n_spans, nc), 256 threads; out[a * n_spans + c0 + b] = sum_h sum_{i in a} M[h][b][i] in float64
+constexpr int kSpanReduceThreads = 256;
+__global__ void __launch_bounds__(kSpanReduceThreads) spans_reduce_kernel(const float* __restrict__ M, int T, int heads,
+                                                                          const int* __restrict__ spans, int n_spans, int c0,
+                                                                          double* __restrict__ out) {
+    __shared__ double red[kSpanReduceThreads];
+    const int a = blockIdx.x, b = blockIdx.y;
+    int lo, hi;
+    span_bounds(spans, a, T, lo, hi);
+    double s = 0.0;
+    for (int h = 0; h < heads; ++h) {
+        const float* row = M + (static_cast<size_t>(h) * kSpanChunk + b) * T;
+        for (int i = lo + threadIdx.x; i < hi; i += kSpanReduceThreads) s += static_cast<double>(row[i]);
+    }
+    red[threadIdx.x] = s;
+    __syncthreads();
+    for (int k = kSpanReduceThreads / 2; k > 0; k >>= 1) {
+        if (threadIdx.x < k) red[threadIdx.x] += red[threadIdx.x + k];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) out[static_cast<size_t>(a) * n_spans + c0 + b] = red[0];
+}
+
+// workspace floats of launch_attention_spans: m and l [heads, T], M [heads, kSpanChunk, T]
+static size_t attention_spans_ws_floats(int T, int heads) {
+    return static_cast<size_t>(heads) * T * (2 + kSpanChunk);
+}
+
+// A, then per chunk of kSpanChunk column spans B and C -> out [n_spans, n_spans] (device float64)
+static int launch_attention_spans(const __half* qkv_hi, const __half* qkv_lo, int T, int heads, int kv_heads,
+                                  const int* spans, int n_spans, float* ws, double* out, cudaStream_t st) {
+    const int G = heads / kv_heads, hpc = causal_heads_per_cta(G), rows = 16 * (kCausalWarps / hpc);
+    float* m = ws;
+    float* l = m + static_cast<size_t>(heads) * T;
+    float* M = l + static_cast<size_t>(heads) * T;
+    const size_t smem_b = kSpanKSmem + sizeof(float) * kCausalWarps * 16 * kSpanChunk;
+    ProfScope _ps(PROF_ATTN, st);
+    RMU_CUDA(cudaFuncSetAttribute(spans_rowstat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSpanKSmem)));
+    RMU_CUDA(cudaFuncSetAttribute(spans_mass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_b)));
+    const dim3 grid(static_cast<unsigned>(kv_heads * (G / hpc)), 1, static_cast<unsigned>((T + rows - 1) / rows));
+    spans_rowstat_kernel<<<grid, kCausalWarps * 32, kSpanKSmem, st>>>(qkv_hi, qkv_lo, T, heads, kv_heads, hpc, spans,
+                                                                      n_spans, m, l);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    for (int c0 = 0; c0 < n_spans; c0 += kSpanChunk) {
+        const int nc = std::min(kSpanChunk, n_spans - c0);
+        spans_mass_kernel<<<grid, kCausalWarps * 32, smem_b, st>>>(qkv_hi, qkv_lo, T, heads, kv_heads, hpc, spans, n_spans,
+                                                                   c0, nc, m, l, M);
+        count_launch();
+        RMU_CHECK_LAUNCH();
+        spans_reduce_kernel<<<dim3(static_cast<unsigned>(n_spans), static_cast<unsigned>(nc)), kSpanReduceThreads, 0, st>>>(
+            M, T, heads, spans, n_spans, c0, out);
         count_launch();
         RMU_CHECK_LAUNCH();
     }
@@ -1585,6 +1938,12 @@ struct rmu_encoder {
     float* zeros = nullptr;
     float* QKVF = nullptr;
     int* range_flag = nullptr;
+    // Llama (rmu_encoder_create_llama) runs as Qwen3 with qn = kn = null (no per-head q / k RMSNorm); the span
+    // attention's workspace (launch_attention_spans) and its one-sequence cu_seqlens [0, T], grown under mu
+    bool llama = false;
+    float* span_ws = nullptr;
+    size_t span_ws_cap = 0;
+    int* span_cu = nullptr;
     // activations
     int tok_cap = 0, seq_cap = 0;
     std::vector<void*> act_allocs;
@@ -1654,6 +2013,22 @@ static void free_acts(rmu_encoder* e) {
     cudaFree(e->pos_ws);
     e->pos_ws = nullptr;
     e->pos_ws_cap = 0;
+    cudaFree(e->span_ws);
+    e->span_ws = nullptr;
+    e->span_ws_cap = 0;
+}
+
+// the span attention's workspace for a sequence of T tokens, grown to fit
+static int ensure_span_ws(rmu_encoder* e, int T) {
+    const size_t need = attention_spans_ws_floats(T, e->cfg.heads);
+    if (need <= e->span_ws_cap) return RMU_OK;
+    RMU_CUDA(cudaDeviceSynchronize());
+    cudaFree(e->span_ws);
+    e->span_ws = nullptr;
+    e->span_ws_cap = 0;
+    RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->span_ws), need * sizeof(float)));
+    e->span_ws_cap = need;
+    return RMU_OK;
 }
 
 // DeBERTa: the position terms' workspace for a call (qrows query rows, T keys), grown to fit
@@ -1941,15 +2316,31 @@ static int ensure_tokens_qwen3(rmu_encoder* e, int T, int B) {
     return RMU_OK;
 }
 
+// one decoder layer up to its attention inputs: X = split(w_in RMS(h)); QKVF = X Wqkv^T (fp32); QKVP = the q / k step
+static int qwen3_attention_inputs(rmu_encoder* e, const EncLayer& L, int T, cudaStream_t st) {
+    const rmu_bert_config& c = e->cfg;
+    const int nh = c.heads, kv = e->qext.kv_heads, NQKV = (nh + 2 * kv) * kQwenHD;
+    const float qscale = 1.4426950408889634f / sqrtf(static_cast<float>(kQwenHD));
+    int rc = launch_rms_split(e->PRE, T, c.hidden, L.ln1g, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
+    if (rc != RMU_OK) return rc;
+    GemmParams g{};
+    g.M = T; g.N = NQKV; g.K = c.hidden; g.bias = e->zeros; g.out_f32 = e->QKVF;
+    rc = launch_gemm(GEMM_BIAS_F32, e->X, L.Wqkv, g, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    return launch_qk_norm_rope(e->QKVF, T, nh, kv, e->POSI, L.qn, L.kn, c.ln_eps, qscale, e->rope_cos[0], e->rope_sin[0],
+                               c.max_pos, e->QKVP.hi, e->QKVP.lo, e->range_flag, st);
+}
+
 // Qwen3's layers (the header's formula): leaves the residual stream h, before the final norm, in e->PRE [T, H] fp32.
-// Per layer: X = split(w_in RMS(h)); QKVF = X Wqkv^T (fp32); QKVP = the q / k step; CTX = causal GQA attention;
-// h += CTX Wo^T (in place); X = split(w_post RMS(h)); FF = split(silu(X Wgate^T) * (X Wup^T)); h += FF Wdown^T.
+// Per layer: the attention inputs (above); CTX = causal GQA attention; h += CTX Wo^T (in place); X = split(w_post
+// RMS(h)); FF = split(silu(X Wgate^T) * (X Wup^T)); h += FF Wdown^T.  With attn_last (the span attention), the last
+// layer stops at its attention inputs, which QKVP then holds.
 // The range flag is cleared first; the caller reads it (qwen3_check_range) before it writes an output.
-static int run_qwen3(rmu_encoder* e, const int32_t* ids, const int32_t* cu, int B, int T, int max_seqlen, cudaStream_t st) {
+static int run_qwen3(rmu_encoder* e, const int32_t* ids, const int32_t* cu, int B, int T, int max_seqlen, cudaStream_t st,
+                     bool attn_last = false) {
     const rmu_bert_config& c = e->cfg;
     if (max_seqlen > c.max_pos) { set_error("sequence longer than max_position_embeddings"); return RMU_ERR_ARG; }
     const int H = c.hidden, F = c.ffn, nh = c.heads, kv = e->qext.kv_heads, QD = nh * kQwenHD;
-    const int NQKV = QD + 2 * kv * kQwenHD;
     int rc = ensure_tokens_qwen3(e, T, B);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace is shared by all callers
@@ -1957,21 +2348,13 @@ static int run_qwen3(rmu_encoder* e, const int32_t* ids, const int32_t* cu, int 
     rc = launch_seq_positions(cu, B, T, e->POSI, st);
     if (rc == RMU_OK) rc = launch_embed_rows(ids, T, H, c.vocab_size, e->word, e->PRE, st);
     if (rc != RMU_OK) return rc;
-    const float qscale = 1.4426950408889634f / sqrtf(static_cast<float>(kQwenHD));
     for (int l = 0; l < c.layers; ++l) {
         const EncLayer& L = e->layers[l];
-        rc = launch_rms_split(e->PRE, T, H, L.ln1g, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
+        rc = qwen3_attention_inputs(e, L, T, st);
+        if (rc != RMU_OK || (attn_last && l == c.layers - 1)) return rc;
+        rc = launch_attention_causal(e->QKVP.hi, e->QKVP.lo, cu, B, nh, kv, max_seqlen, e->CTX.hi, e->CTX.lo, st);
         if (rc != RMU_OK) return rc;
         GemmParams g{};
-        g.M = T; g.N = NQKV; g.K = H; g.bias = e->zeros; g.out_f32 = e->QKVF;
-        rc = launch_gemm(GEMM_BIAS_F32, e->X, L.Wqkv, g, e->sms, st);
-        if (rc == RMU_OK)
-            rc = launch_qk_norm_rope(e->QKVF, T, nh, kv, e->POSI, L.qn, L.kn, c.ln_eps, qscale, e->rope_cos[0], e->rope_sin[0],
-                                     c.max_pos, e->QKVP.hi, e->QKVP.lo, e->range_flag, st);
-        if (rc == RMU_OK)
-            rc = launch_attention_causal(e->QKVP.hi, e->QKVP.lo, cu, B, nh, kv, max_seqlen, e->CTX.hi, e->CTX.lo, st);
-        if (rc != RMU_OK) return rc;
-        g = GemmParams{};
         g.M = T; g.N = H; g.K = QD; g.bias = e->zeros; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
         rc = launch_gemm(GEMM_BIAS_RESF32_F32, e->CTX, L.Wo, g, e->sms, st);
         if (rc == RMU_OK) rc = launch_rms_split(e->PRE, T, H, L.ln2g, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
@@ -1994,7 +2377,7 @@ static int qwen3_check_range(rmu_encoder* e, cudaStream_t st) {
     RMU_CUDA(cudaMemcpyAsync(&flag, e->range_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
     RMU_CUDA(cudaStreamSynchronize(st));
     if (flag) {
-        set_error("Qwen3 forward: an activation entering a GEMM or attention left the fp16 range of the split planes "
+        set_error(std::string(e->llama ? "Llama" : "Qwen3") + " forward: an activation entering a GEMM or attention left the fp16 range of the split planes "
                   "(|x| > 65504); the encoder cannot compute this model's activations for this input");
         return RMU_ERR_RANGE;
     }
@@ -2352,62 +2735,69 @@ int rmu_encoder_create_modernbert(const rmu_bert_config* cfg, const rmu_modernbe
     return RMU_OK;
 }
 
-int rmu_encoder_create_qwen3(const rmu_bert_config* cfg, const rmu_qwen3_ext* qx, const float* const* w, int n_weights,
-                             int has_head, rmu_encoder** out) {
-    if (!cfg || !qx || !w || !out) { set_error("rmu_encoder_create_qwen3: bad argument"); return RMU_ERR_ARG; }
+}  // extern "C"
+
+// rmu_encoder_create_qwen3 (qk_norm) and rmu_encoder_create_llama (no q_norm / k_norm tensors: 9 per layer, no head);
+// `who` prefixes the errors
+static int create_decoder(const char* who, bool qk_norm, const rmu_bert_config* cfg, const rmu_qwen3_ext* qx,
+                          const float* const* w, int n_weights, int has_head, rmu_encoder** out) {
+    const std::string fn(who);
+    if (!cfg || !qx || !w || !out) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
     const int H = cfg->hidden, F = cfg->ffn, L = cfg->layers, nh = cfg->heads, kv = qx->kv_heads;
     if (cfg->position_mode != RMU_POS_ABSOLUTE || cfg->rel_buckets != 0 || cfg->adapter_dim != 0) {
-        set_error("rmu_encoder_create_qwen3: position_mode, rel_buckets and adapter_dim must be 0 (rotary positions, no "
+        set_error(fn + ": position_mode, rel_buckets and adapter_dim must be 0 (rotary positions, no "
                   "relative bias, no adapters)");
         return RMU_ERR_UNSUPPORTED;
     }
     if (qx->head_dim != kQwenHD) {
-        set_error("rmu_encoder_create_qwen3: head_dim must be 128, got " + std::to_string(qx->head_dim));
+        set_error(fn + ": head_dim must be 128, got " + std::to_string(qx->head_dim));
         return RMU_ERR_UNSUPPORTED;
     }
     if (H <= 0 || H % 128 != 0 || H > 4096) {
-        set_error("rmu_encoder_create_qwen3: hidden_size must be a multiple of 128 up to 4096, got " + std::to_string(H));
+        set_error(fn + ": hidden_size must be a multiple of 128 up to 4096, got " + std::to_string(H));
         return RMU_ERR_UNSUPPORTED;
     }
     if (F <= 0 || F % 64 != 0) {
-        set_error("rmu_encoder_create_qwen3: intermediate_size must be a positive multiple of 64, got " + std::to_string(F));
+        set_error(fn + ": intermediate_size must be a positive multiple of 64, got " + std::to_string(F));
         return RMU_ERR_UNSUPPORTED;
     }
     if (nh <= 0 || kv <= 0 || nh % kv != 0) {
-        set_error("rmu_encoder_create_qwen3: num_attention_heads must be a multiple of num_key_value_heads (" +
+        set_error(fn + ": num_attention_heads must be a multiple of num_key_value_heads (" +
                   std::to_string(nh) + " heads, " + std::to_string(kv) + " kv heads)");
         return RMU_ERR_UNSUPPORTED;
     }
     if (L < 1 || cfg->vocab_size <= 0 || cfg->max_pos <= 0 || cfg->num_labels <= 0) {
-        set_error("rmu_encoder_create_qwen3: unsupported shape (at least one layer, positive vocab, max_pos, num_labels)");
+        set_error(fn + ": unsupported shape (at least one layer, positive vocab, max_pos, num_labels)");
         return RMU_ERR_UNSUPPORTED;
     }
     if (qx->rope_rows != cfg->max_pos || qx->rope_half != kQwenHD / 2) {
-        set_error("rmu_encoder_create_qwen3: the rope tables must be [max_pos, 64] = [" + std::to_string(cfg->max_pos) + ", 64]");
+        set_error(fn + ": the rope tables must be [max_pos, 64] = [" + std::to_string(cfg->max_pos) + ", 64]");
         return RMU_ERR_ARG;
     }
     if (qx->head_form != (has_head ? RMU_QWEN3_HEAD_LAST : RMU_QWEN3_HEAD_NONE)) {
-        set_error("rmu_encoder_create_qwen3: head_form must be RMU_QWEN3_HEAD_LAST with a head, RMU_QWEN3_HEAD_NONE without");
+        set_error(fn + ": head_form must be RMU_QWEN3_HEAD_LAST with a head, RMU_QWEN3_HEAD_NONE without");
         return RMU_ERR_ARG;
     }
     const int QD = nh * kQwenHD, KD = kv * kQwenHD, NQKV = QD + 2 * KD;
-    const int norm0 = 1 + 11 * L, rope0 = norm0 + 1 + (has_head ? 1 : 0), expect = rope0 + 2;
+    const int per = qk_norm ? 11 : 9;                // tensors per layer
+    const int norm0 = 1 + per * L, rope0 = norm0 + 1 + (has_head ? 1 : 0), expect = rope0 + 2;
     if (n_weights != expect) {
-        set_error("rmu_encoder_create_qwen3: expected " + std::to_string(expect) + " weight tensors");
+        set_error(fn + ": expected " + std::to_string(expect) + " weight tensors");
         return RMU_ERR_ARG;
     }
     for (int j = 0; j < expect; ++j)
-        if (!w[j]) { set_error("rmu_encoder_create_qwen3: null weight tensor " + std::to_string(j)); return RMU_ERR_ARG; }
+        if (!w[j]) { set_error(fn + ": null weight tensor " + std::to_string(j)); return RMU_ERR_ARG; }
     for (int l = 0; l < L; ++l) {
         static const char* const kName[] = {"q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj"};
-        const int slot[] = {1, 2, 3, 6, 8, 9, 10};
+        const int slot11[] = {1, 2, 3, 6, 8, 9, 10}, slot9[] = {1, 2, 3, 4, 6, 7, 8};
+        const int* slot = qk_norm ? slot11 : slot9;
         const size_t count[] = {size_t(QD) * H, size_t(KD) * H, size_t(KD) * H, size_t(H) * QD, size_t(F) * H,
                                 size_t(F) * H, size_t(H) * F};
         for (int k = 0; k < 7; ++k) {
-            const float* p = w[1 + 11 * l + slot[k]];
+            const float* p = w[1 + per * l + slot[k]];
             for (size_t j = 0; j < count[k]; ++j) {
                 if (std::fabs(p[j]) >= 65520.0f) {
-                    set_error("rmu_encoder_create_qwen3: layer " + std::to_string(l) + " " + kName[k] + " weight [" +
+                    set_error(fn + ": layer " + std::to_string(l) + " " + kName[k] + " weight [" +
                               std::to_string(j) + "] = " + std::to_string(p[j]) +
                               " is outside the split fp16 planes' range (|w| < 65520)");
                     return RMU_ERR_UNSUPPORTED;
@@ -2419,10 +2809,11 @@ int rmu_encoder_create_qwen3(const rmu_bert_config* cfg, const rmu_qwen3_ext* qx
     e->cfg = *cfg;
     e->has_head = has_head;
     e->qwen = true;
+    e->llama = !qk_norm;
     e->qext = *qx;
     if (cudaGetDevice(&e->device) != cudaSuccess || (e->sms = device_sm_count()) <= 0 ||
         cudaEventCreateWithFlags(&e->ws_done, cudaEventDisableTiming) != cudaSuccess) {
-        set_error("rmu_encoder_create_qwen3: no CUDA device (this library has no CPU path)");
+        set_error(fn + ": no CUDA device (this library has no CPU path)");
         delete e;
         return RMU_ERR_CUDA;
     }
@@ -2442,8 +2833,10 @@ int rmu_encoder_create_qwen3(const rmu_bert_config* cfg, const rmu_qwen3_ext* qx
             rc = upload_split(e, &Ly.Wqkv, {qkv.data()}, NQKV, H);
         }
         i += 3;
-        up(&Ly.qn, kQwenHD);
-        up(&Ly.kn, kQwenHD);
+        if (qk_norm) {
+            up(&Ly.qn, kQwenHD);
+            up(&Ly.kn, kQwenHD);
+        }
         if (rc == RMU_OK) rc = upload_split(e, &Ly.Wo, {w[i]}, H, QD);
         ++i;
         up(&Ly.ln2g, H);
@@ -2469,9 +2862,26 @@ int rmu_encoder_create_qwen3(const rmu_bert_config* cfg, const rmu_qwen3_ext* qx
         rc = upload(e, &e->zeros, zeros.data(), zeros.size());
     }
     if (rc == RMU_OK) rc = dev_alloc(e->allocs, &e->range_flag, 1);
+    if (rc == RMU_OK) rc = dev_alloc(e->allocs, &e->span_cu, 2);
     if (rc != RMU_OK) { rmu_encoder_destroy(e); return rc; }
     *out = e;
     return RMU_OK;
+}
+
+extern "C" {
+
+int rmu_encoder_create_qwen3(const rmu_bert_config* cfg, const rmu_qwen3_ext* qx, const float* const* w, int n_weights,
+                             int has_head, rmu_encoder** out) {
+    return create_decoder("rmu_encoder_create_qwen3", true, cfg, qx, w, n_weights, has_head, out);
+}
+
+int rmu_encoder_create_llama(const rmu_bert_config* cfg, const rmu_qwen3_ext* qx, const float* const* w, int n_weights,
+                             rmu_encoder** out) {
+    if (qx && qx->head_form != RMU_QWEN3_HEAD_NONE) {
+        set_error("rmu_encoder_create_llama: head_form must be RMU_QWEN3_HEAD_NONE (Llama runs without a head)");
+        return RMU_ERR_ARG;
+    }
+    return create_decoder("rmu_encoder_create_llama", false, cfg, qx, w, n_weights, 0, out);
 }
 
 void rmu_encoder_destroy(rmu_encoder* e) {
@@ -2565,6 +2975,39 @@ int rmu_encoder_hidden(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
     }
     if (rc != RMU_OK) return rc;
     rc = launch_join_planes(e->X.hi, e->X.lo, static_cast<size_t>(T) * e->cfg.hidden, out, st);
+    if (rc != RMU_OK) return rc;
+    RMU_CUDA(cudaEventRecord(e->ws_done, st));
+    return RMU_OK;
+}
+
+int rmu_decoder_attention_spans(rmu_encoder* e, const int32_t* ids, int T, const int32_t* spans, int n_spans, double* out,
+                                void* stream) {
+    if (!e || !ids || !spans || !out || T <= 0 || n_spans <= 0) {
+        set_error("rmu_decoder_attention_spans: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (!e->qwen || e->has_head) {
+        set_error("rmu_decoder_attention_spans: the encoder must come from rmu_encoder_create_qwen3 without a head or from "
+                  "rmu_encoder_create_llama");
+        return RMU_ERR_ARG;
+    }
+    if (T > e->cfg.max_pos) {
+        set_error("rmu_decoder_attention_spans: " + std::to_string(T) + " tokens exceed max_position_embeddings (" +
+                  std::to_string(e->cfg.max_pos) + ")");
+        return RMU_ERR_ARG;
+    }
+    std::lock_guard<std::mutex> g(e->mu);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int cu_h[2] = {0, T};
+    // pageable source: the copy has taken cu_h when the call returns; span_cu is read by run_qwen3 only, which the
+    // range check below has finished before this entry point returns
+    RMU_CUDA(cudaMemcpyAsync(e->span_cu, cu_h, sizeof(cu_h), cudaMemcpyHostToDevice, st));
+    int rc = run_qwen3(e, ids, e->span_cu, 1, T, T, st, true);
+    if (rc == RMU_OK) rc = qwen3_check_range(e, st);
+    if (rc == RMU_OK) rc = ensure_span_ws(e, T);
+    if (rc == RMU_OK)
+        rc = launch_attention_spans(e->QKVP.hi, e->QKVP.lo, T, e->cfg.heads, e->qext.kv_heads, spans, n_spans, e->span_ws,
+                                    out, st);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
@@ -3123,6 +3566,25 @@ int rmu_debug_attention_causal(const uint16_t* qkv_hi, const uint16_t* qkv_lo, c
     return launch_attention_causal(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), cu, B,
                                    heads, kv_heads, max_seqlen, reinterpret_cast<__half*>(ctx_hi),
                                    reinterpret_cast<__half*>(ctx_lo), static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_attention_spans(const uint16_t* qkv_hi, const uint16_t* qkv_lo, int T, int heads, int kv_heads,
+                              const int32_t* spans, int n_spans, double* out, void* stream) {
+    if (!qkv_hi || !qkv_lo || !spans || !out || T <= 0 || heads <= 0 || kv_heads <= 0 || n_spans <= 0) {
+        set_error("rmu_debug_attention_spans: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (heads % kv_heads != 0) {
+        set_error("rmu_debug_attention_spans: heads must be a multiple of kv_heads");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float* ws = nullptr;
+    RMU_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&ws), attention_spans_ws_floats(T, heads) * sizeof(float), st));
+    const int rc = launch_attention_spans(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), T,
+                                          heads, kv_heads, spans, n_spans, ws, out, st);
+    RMU_CUDA(cudaFreeAsync(ws, st));
+    return rc;
 }
 
 int rmu_debug_last_token(const float* x, const int32_t* ids, const int32_t* cu, int B, int H, const float* w, float eps,

@@ -17,6 +17,9 @@ input_layernorm, q / k / v_proj, q_norm, k_norm, o_proj, post_attention_layernor
 head the [num_labels, H] last-token head; then the cos / sin tables of ``weights.rope_table``.  It pools by the last
 token only (``pooling="last"``), and a forward whose activations leave the fp16 range of the split planes raises
 ``RmuError`` naming the model.
+
+Llama (``weights.LlamaConfig``, ``rmu_encoder_create_llama``) takes Qwen3's order without q_norm / k_norm and without a
+head, with the config's own rope tables (``llama3`` scaling); it is built for attention provenance only.
 """
 from __future__ import annotations
 
@@ -26,7 +29,7 @@ from typing import Dict, Optional
 import numpy as np
 
 from . import _lib
-from .weights import BertConfig, ModernBertConfig, Qwen3Config, rope_table, rope_tables, weight_names
+from .weights import BertConfig, LlamaConfig, ModernBertConfig, Qwen3Config, rope_table, rope_tables, weight_names
 
 POOL = {"mean": 0, "cls": 1, "last": 2}
 RMU_ERR_RANGE = -4
@@ -58,16 +61,24 @@ class BertEncoder:
             if tuple(a.shape) != tuple(shape):
                 raise ValueError(f"{name}: expected shape {shape}, got {a.shape}")
             arrs.append(a)
-        modern, qwen = isinstance(cfg, ModernBertConfig), isinstance(cfg, Qwen3Config)
+        modern, qwen, llama = isinstance(cfg, ModernBertConfig), isinstance(cfg, Qwen3Config), isinstance(cfg, LlamaConfig)
         if modern:
             arrs += list(rope_tables(cfg))
         if qwen:
             arrs += list(rope_table(cfg.rope_theta, cfg.head_dim, cfg.max_pos))
+        if llama:
+            if self.with_head:
+                raise ValueError(f"{cfg.name}: Llama runs without a head")
+            arrs += list(cfg.rope_tables())
         ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
         cc = _lib.bert_config_c(cfg)
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):
-            if qwen:
+            if llama:
+                qx = _lib.Qwen3ExtC(cfg.kv_heads, cfg.head_dim, cfg.max_pos, cfg.head_dim // 2, 0, -1)
+                _lib.check(_lib.lib().rmu_encoder_create_llama(C.byref(cc), C.byref(qx), ptrs, len(arrs), C.byref(self._h)),
+                           "rmu_encoder_create_llama")
+            elif qwen:
                 qx = _lib.Qwen3ExtC(cfg.kv_heads, cfg.head_dim, cfg.max_pos, cfg.head_dim // 2, int(self.with_head),
                                     cfg.head_pad_id)
                 _lib.check(_lib.lib().rmu_encoder_create_qwen3(C.byref(cc), C.byref(qx), ptrs, len(arrs), int(self.with_head),

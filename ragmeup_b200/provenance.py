@@ -1,6 +1,10 @@
 """Provenance attribution helpers that reuse the encoder / cross-encoder / cosine primitives (SURVEY.md §8 row f4).
 
-Drop-ins for the two attribution methods of ``server/provenance.py`` that sit on this path:
+Drop-ins for the three attribution methods of ``server/provenance.py`` that sit on this path:
+
+* ``compute_attention`` (``server/provenance.py:19-98``): how much last-layer attention the query and the answer
+  exchange with each retrieved document inside the chat thread, from a Llama or Qwen3 decoder on the GPU
+  (``DecoderAttention``).  The decoder sums the softmax over token spans directly; no attention map is stored.
 
 * ``compute_rerank_provenance`` (``server/provenance.py:100-108``): re-score the retrieved documents against
   ``answer`` (or ``query + "\\n" + answer`` when ``attribute_include_query == "True"``) with the reranker.
@@ -20,6 +24,7 @@ import numpy as np
 
 from . import _lib
 from .index import FlatIndex
+from .weights import find_snapshot, resolve_decoder
 
 
 def compute_rerank_provenance(reranker: Any, query: str, documents: Sequence[Any], answer: str) -> Sequence[Any]:
@@ -66,3 +71,99 @@ class DocumentSimilarityAttribution:
         total = sum(similarity)
         out = [s / total for s in similarity] if total > 0 else similarity
         return [float(s) for s in out]
+
+
+class DecoderAttention:
+    """A Llama or Qwen3 decoder (``weights.resolve_decoder``: a snapshot directory or ``synthetic:<preset>``) on the
+    GPU, for attention provenance.  Its weights are uploaded once; ``span_mass`` then runs one thread per call."""
+
+    def __init__(self, model_name: str, device: Optional[int] = None):
+        from .encoder import BertEncoder
+        cfg, w = resolve_decoder(model_name)
+        self.cfg = cfg
+        self.encoder = BertEncoder(cfg, w, with_head=False, device=device)
+
+    @property
+    def name(self) -> str:
+        return self.cfg.name
+
+    def span_mass(self, ids: Sequence[int], spans: Sequence[Sequence[int]]) -> np.ndarray:
+        """the last layer's attention summed over heads, the rows of span a and the keys of span b -> float64
+        [n, n]; spans are [start, end) token ranges of ``ids`` (``rmu_decoder_attention_spans``)"""
+        T = len(ids)
+        if T > self.cfg.max_pos:
+            raise ValueError(f"{self.name}: a thread of {T} tokens exceeds max_position_embeddings ({self.cfg.max_pos})")
+        if T == 0 or len(spans) == 0:
+            raise ValueError(f"{self.name}: attention provenance needs a non-empty thread and at least one span")
+        enc = self.encoder
+        torch = enc.torch
+        d_ids = enc._dev(np.asarray(ids, dtype=np.int32), torch.int32)
+        d_spans = enc._dev(np.asarray(spans, dtype=np.int32).reshape(-1, 2), torch.int32)
+        out = torch.empty((len(spans), len(spans)), dtype=torch.float64, device=enc.device)
+        with torch.cuda.device(enc.device):
+            enc._check(_lib.lib().rmu_decoder_attention_spans(enc._h, d_ids.data_ptr(), T, d_spans.data_ptr(), len(spans),
+                                                              out.data_ptr(), _lib.stream_ptr()),
+                       "rmu_decoder_attention_spans")
+        return out.cpu().numpy()
+
+
+_DECODERS: dict = {}
+
+
+def _decoder(model: Any) -> DecoderAttention:
+    """``model`` as compute_attention takes it: a DecoderAttention, a model name, or a transformers model whose
+    ``name_or_path`` names a snapshot (found as every other drop-in finds one); one handle per (path, device)"""
+    if isinstance(model, DecoderAttention):
+        return model
+    name = model if isinstance(model, str) else getattr(model, "name_or_path", None)
+    if not name:
+        raise TypeError("compute_attention: model must be a DecoderAttention, a model name or a transformers model with "
+                        "name_or_path")
+    torch = _lib.require_cuda()
+    key = (name if name.startswith("synthetic:") else os.path.realpath(find_snapshot(name)), torch.cuda.current_device())
+    if key not in _DECODERS:
+        _DECODERS[key] = DecoderAttention(name, device=key[1])
+    return _DECODERS[key]
+
+
+def _find_part(thread: List[int], part: List[int]):
+    """the first occurrence of ``part`` in ``thread`` as the reference slices it, [i : i + len - 1] (its last token
+    left out; an empty part is [0 : -1]), normalised as Python normalises that slice -> [start, end)"""
+    n = len(part)
+    for i in range(len(thread) - n + 1):
+        if thread[i:i + n] == part:
+            s, e, _ = slice(i, i + n - 1).indices(len(thread))
+            return s, max(s, e)
+    raise ValueError("Sublist not found")
+
+
+def compute_attention(model: Any, tokenizer: Any, thread: str, query: str, context: Sequence[Any],
+                      answer: str) -> List[np.float64]:
+    """each document's share of the attention the query and answer exchange with the documents and each other in the
+    last layer, over the mean of all those shares (the reference's return value: one np.float64 per document)"""
+    include_query = os.getenv("attribute_include_query") != "False"
+    dec = _decoder(model)
+
+    def enc(text):
+        return list(tokenizer.encode(text, add_special_tokens=False))
+
+    ids = enc(thread)
+    texts = [c.page_content if hasattr(c, "page_content") else c for c in context]
+    spans = [_find_part(ids, enc(query)), _find_part(ids, enc(answer))] + [_find_part(ids, enc(t)) for t in texts]
+    mass = dec.span_mass(ids, spans)
+    heads = dec.cfg.heads
+
+    def mean(x, y):
+        n = heads * (spans[x][1] - spans[x][0]) * (spans[y][1] - spans[y][0])
+        return mass[x, y] / n if n else np.float64("nan")
+
+    Q, A = 0, 1
+    total = [v for v in (mean(Q, Q), mean(Q, A), mean(A, A), mean(A, Q)) if v > 0]
+    scores = []
+    for d in range(2, len(spans)):
+        pairs = [(A, d), (d, A)] + ([(Q, d), (d, Q)] if include_query else [])
+        kept = [v for v in (mean(x, y) for x, y in pairs) if v > 0]
+        total += kept
+        scores.append(np.mean(kept) if kept else np.float64("nan"))
+    mean_total = np.mean(total) if total else np.float64("nan")
+    return [np.float64(sc / mean_total) for sc in scores]

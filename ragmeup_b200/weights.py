@@ -324,14 +324,26 @@ def rope_tables(cfg: ModernBertConfig):
     return (*rope_table(cfg.global_theta, cfg.head_dim, cfg.max_pos), *rope_table(cfg.local_theta, cfg.head_dim, cfg.max_pos))
 
 
-def rope_table(theta: float, head_dim: int, rows: int):
+def rope_table(theta: float, head_dim: int, rows: int, llama3: Optional[Tuple[float, float, float, int]] = None):
     """(cos, sin), each [rows, head_dim / 2] float32, of the default rotary embedding as transformers computes it
     (``ModernBertRotaryEmbedding``, ``Qwen3RotaryEmbedding``): ``inv_freq = 1 / (theta ** (arange(0, d, 2).float() /
-    d))``, the angle ``pos * inv_freq`` in float32, then ``.cos()`` / ``.sin()``."""
+    d))``, the angle ``pos * inv_freq`` in float32, then ``.cos()`` / ``.sin()``.  ``llama3`` = (factor, low_freq_factor,
+    high_freq_factor, original_max_position_embeddings) applies Llama-3.1's frequency scaling to inv_freq first, in
+    float32 as transformers' ``llama3`` rope init does: wavelengths 2 pi / inv_freq above old / low_freq_factor are
+    divided by factor, those below old / high_freq_factor kept, and those between interpolated."""
+    import math
     import torch
     d = head_dim
     pos = torch.arange(rows, dtype=torch.int64).float()
     inv_freq = 1.0 / (theta ** (torch.arange(0, d, 2, dtype=torch.int64).float() / d))
+    if llama3 is not None:
+        factor, low, high, old = llama3
+        wavelen = 2 * math.pi / inv_freq
+        scaled = torch.where(wavelen > old / low, inv_freq / factor, inv_freq)
+        smooth = (old / wavelen - low) / (high - low)
+        smoothed = (1 - smooth) * scaled / factor + smooth * scaled
+        medium = ~(wavelen < old / high) * ~(wavelen > old / low)
+        inv_freq = torch.where(medium, smoothed, scaled)
     ang = pos[:, None] * inv_freq[None, :]
     return (np.ascontiguousarray(ang.cos().numpy(), dtype=np.float32),
             np.ascontiguousarray(ang.sin().numpy(), dtype=np.float32))
@@ -509,6 +521,152 @@ def qwen3_lm_rows(path: str, cfg: Qwen3Config, ids) -> np.ndarray:
     raise KeyError(f"{path}: no lm_head.weight or embed_tokens.weight to read the reranker's yes / no rows from")
 
 
+@dataclass
+class LlamaConfig(BertConfig):
+    """Llama-3 (transformers ``LlamaModel``, model_type ``llama``): Qwen3's decoder without the per-head q / k RMSNorm,
+    with ``llama3`` rope scaling (``rope_scaling`` = (factor, low_freq_factor, high_freq_factor,
+    original_max_position_embeddings)) or the default rotary embedding (``rope_scaling`` None).  It runs for attention
+    provenance only (``provenance.DecoderAttention``), never as an embedder or reranker, and ``lm_head`` is never read.
+    Defaults: the Llama-3.1-8B shape."""
+    vocab_size: int = 128256
+    hidden: int = 4096
+    layers: int = 32
+    heads: int = 32
+    ffn: int = 14336
+    max_pos: int = 131072
+    type_vocab: int = 1
+    ln_eps: float = 1e-5
+    kv_heads: int = 8
+    head_dim: int = 128
+    rope_theta: float = 500000.0
+    rope_scaling: Optional[Tuple[float, float, float, int]] = (8.0, 1.0, 4.0, 8192)
+    name: str = "llama"
+
+    def rope_tables(self):
+        return rope_table(self.rope_theta, self.head_dim, self.max_pos, self.rope_scaling)
+
+    @staticmethod
+    def from_hf(d: dict, name: str = "llama") -> "LlamaConfig":
+        """config.json of a ``llama`` checkpoint, with ``rope_scaling`` (the release form) or ``rope_parameters``
+        (transformers 5) -> LlamaConfig; refuses, naming the field, what the decoder does not compute"""
+        def refuse(field, value, why):
+            raise ValueError(f"{name}: llama with {field} = {value!r} is not supported: {why}")
+        if d.get("model_type", "llama") != "llama":
+            refuse("model_type", d.get("model_type"), "only model_type 'llama' runs as Llama")
+        if d.get("hidden_act", "silu") != "silu":
+            refuse("hidden_act", d.get("hidden_act"), "only SwiGLU (silu) is computed")
+        for field in ("attention_bias", "mlp_bias"):
+            if d.get(field, False):
+                refuse(field, d[field], "the projections have no biases in the decoder")
+        rp = d.get("rope_parameters") or d.get("rope_scaling") or {}
+        kind = rp.get("rope_type", rp.get("type", "default"))
+        if kind not in ("default", "llama3"):
+            refuse("rope_type", kind, "only the default and llama3 rotary embeddings are computed")
+        theta = float(rp.get("rope_theta", d.get("rope_theta", 10000.0)))
+        H, nh = int(d["hidden_size"]), int(d["num_attention_heads"])
+        hd = int(d.get("head_dim") or H // nh)
+        if hd != 128:
+            refuse("head_dim", hd, "the decoder's attention kernels take head_dim 128 only")
+        max_pos = int(d.get("max_position_embeddings", 2048))
+        scaling = None
+        if kind == "llama3":
+            scaling = (float(rp["factor"]), float(rp["low_freq_factor"]), float(rp["high_freq_factor"]),
+                       int(rp.get("original_max_position_embeddings") or max_pos))
+        return LlamaConfig(vocab_size=int(d["vocab_size"]), hidden=H, layers=int(d["num_hidden_layers"]), heads=nh,
+                           ffn=int(d["intermediate_size"]), max_pos=max_pos, ln_eps=float(d.get("rms_norm_eps", 1e-6)),
+                           kv_heads=int(d.get("num_key_value_heads") or nh), head_dim=hd, rope_theta=theta,
+                           rope_scaling=scaling, name=name)
+
+
+def llama_weight_names(cfg: LlamaConfig):
+    """canonical Llama tensors (transformers' names without ``model.``) in rmu_encoder_create_llama's order"""
+    drop = (".self_attn.q_norm.weight", ".self_attn.k_norm.weight")
+    return [(n, shape) for n, shape in qwen3_weight_names(cfg, False) if not n.endswith(drop)]
+
+
+def synthetic_llama_weights(cfg: LlamaConfig, seed: int = 0, scale: float = 1.0) -> Dict[str, np.ndarray]:
+    """seeded Llama weights, drawn as ``synthetic_qwen3_weights`` draws them"""
+    rng = np.random.default_rng(seed)
+    out: Dict[str, np.ndarray] = {}
+    for name, shape in llama_weight_names(cfg):
+        if name.endswith("norm.weight") or name.endswith("layernorm.weight"):
+            a = 1.0 + 0.1 * rng.standard_normal(shape)
+        elif name == "embed_tokens.weight":
+            a = 0.02 * rng.standard_normal(shape) * (3.0 if scale > 1 else 1.0)
+        else:
+            a = 0.02 * scale * rng.standard_normal(shape)
+        out[name] = np.ascontiguousarray(a, dtype=np.float32)
+    return out
+
+
+# decoders for attention provenance (provenance.DecoderAttention), apart from PRESETS: the embedders, rerankers and
+# ColBERT never take them.  tiny-llama: head_dim 128, two query heads per kv head, three layers, and llama3 scaling
+# with original_max_position_embeddings 64, so that several of its frequencies are divided or interpolated.
+# llama-3.1-8b: Meta-Llama-3.1-8B-Instruct's shape [3P-recall: its config.json is not read here].
+DECODER_PRESETS: Dict[str, BertConfig] = {
+    "tiny-llama": LlamaConfig(vocab_size=1000, hidden=256, layers=3, heads=4, ffn=384, max_pos=8192, kv_heads=2,
+                              rope_theta=10000.0, rope_scaling=(8.0, 1.0, 4.0, 64)),
+    "llama-3.1-8b": LlamaConfig(),
+}
+
+
+def _load_decoder_snapshot(path: str):
+    """a ``llama`` or ``qwen3`` snapshot -> (config, weights) of the decoder without any head; ``lm_head`` (and a
+    sequence-classification ``score``) is never read"""
+    cfgd = _read_json(os.path.join(path, "config.json"))
+    if cfgd is None:
+        raise FileNotFoundError(f"{path}: no config.json")
+    kind = cfgd.get("model_type")
+    if kind == "llama":
+        cfg = LlamaConfig.from_hf(cfgd, name=path)
+    elif kind == "qwen3":
+        cfg = Qwen3Config.from_hf(cfgd, name=path)
+    else:
+        raise ValueError(f"{path}: model_type {kind!r} is not supported for attention provenance (llama, qwen3)")
+    names = llama_weight_names(cfg) if kind == "llama" else qwen3_weight_names(cfg, False)
+    w = qwen3_to_canonical(_load_tensors(path, lambda n: n not in ("lm_head.weight", "score.weight")), cfg)
+    missing = [n for n, _ in names if n not in w]
+    if missing:
+        raise KeyError(f"{path}: missing tensors {missing[:4]}...")
+    return cfg, {n: w[n] for n, _ in names}
+
+
+def resolve_decoder(model_name: str, cache_folder: Optional[str] = None):
+    """decoder name -> (config, weights): ``synthetic:<preset>[:seed[:scale]]`` (DECODER_PRESETS, or a Qwen3 preset of
+    PRESETS), else a local snapshot directory found as ``resolve_model`` finds one"""
+    if model_name.startswith("synthetic:"):
+        parts = model_name.split(":")
+        preset = parts[1]
+        seed = int(parts[2]) if len(parts) > 2 else 0
+        scale = float(parts[3]) if len(parts) > 3 else 1.0
+        if preset in DECODER_PRESETS:
+            cfg = LlamaConfig(**asdict(DECODER_PRESETS[preset]))
+            cfg.name = model_name
+            return cfg, synthetic_llama_weights(cfg, seed=seed, scale=scale)
+        if preset in PRESETS and isinstance(PRESETS[preset][0], Qwen3Config):
+            cfg = Qwen3Config(**asdict(PRESETS[preset][0]))
+            cfg.name, cfg.reranker, cfg.num_labels = model_name, False, 1
+            return cfg, synthetic_qwen3_weights(cfg, seed=seed, with_head=False, scale=scale)
+        raise ValueError(f"unknown synthetic decoder preset {preset!r}; have {sorted(DECODER_PRESETS)} and the qwen3 "
+                         f"presets")
+    return _load_decoder_snapshot(find_snapshot(model_name, cache_folder))
+
+
+def find_snapshot(model_name: str, cache_folder: Optional[str] = None) -> str:
+    """the local snapshot directory of a model id: the id itself, or ``<cache>/<name>`` / ``$RAGMEUP_MODEL_DIR/<name>``
+    (each also with the id's last path component)"""
+    cands = [model_name]
+    for root in (cache_folder, os.environ.get("RAGMEUP_MODEL_DIR")):
+        if root:
+            cands += [os.path.join(root, model_name), os.path.join(root, model_name.split("/")[-1])]
+    for c in cands:
+        if os.path.isdir(c):
+            return c
+    raise FileNotFoundError(
+        f"model {model_name!r} not found locally (no network in this deployment): point "
+        f"RAGMEUP_MODEL_DIR at a directory holding its HuggingFace snapshot, or use 'synthetic:<preset>'")
+
+
 REL_EMB = "encoder.rel_embeddings.weight"
 REL_LN = ("encoder.LayerNorm.weight", "encoder.LayerNorm.bias")
 
@@ -613,6 +771,8 @@ FLASHRANK_MODELS: Dict[str, str] = {
 
 
 def weight_names(cfg: BertConfig, with_head: bool):
+    if isinstance(cfg, LlamaConfig):
+        return llama_weight_names(cfg)
     if isinstance(cfg, Qwen3Config):
         return qwen3_weight_names(cfg, with_head)
     if isinstance(cfg, ModernBertConfig):
@@ -998,16 +1158,8 @@ def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] 
         act = ("sigmoid" if with_head and isinstance(cfg, (XLMRConfig, DebertaConfig, ModernBertConfig)) and cfg.num_labels == 1
                else "identity")
         return cfg, w, pooling, preset not in UNNORMALIZED_PRESETS, max_len, act, None
-    cands = [model_name]
-    for root in (cache_folder, os.environ.get("RAGMEUP_MODEL_DIR")):
-        if root:
-            cands += [os.path.join(root, model_name), os.path.join(root, model_name.split("/")[-1])]
-    for c in cands:
-        if os.path.isdir(c):
-            return (*load_hf_snapshot(c, with_head), c)
-    raise FileNotFoundError(
-        f"model {model_name!r} not found locally (no network in this deployment): point "
-        f"RAGMEUP_MODEL_DIR at a directory holding its HuggingFace snapshot, or use 'synthetic:<preset>'")
+    c = find_snapshot(model_name, cache_folder)
+    return (*load_hf_snapshot(c, with_head), c)
 
 
 @dataclass
