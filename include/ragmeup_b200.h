@@ -195,10 +195,11 @@ typedef struct rmu_bert_config {
  * R = LN_rel(rel_embeddings[0:2s]) and, per layer, PQ = Wq R + bq, PK = Wk R + bk split by head like Q and K, every
  * attention score is (Q_i.K_j + Q_i.PK[c] + K_j.PQ[c]) / sqrt(3 d_h), c = clamp(s + bucket(i - j), 0, 2s - 1).
  * Sequences may hold max_pos tokens; d_h must be 64, and rel_buckets and adapter_dim 0.  head_act selects the
- * activation between the pooler and the classifier: RMU_HEAD_TANH (BERT's pooler, 0) or RMU_HEAD_GELU (DeBERTa's
- * ContextPooler, erf-GELU). */
+ * activation between the pooler and the classifier: RMU_HEAD_TANH (BERT's pooler, 0), RMU_HEAD_GELU (DeBERTa's
+ * ContextPooler, erf-GELU) or RMU_HEAD_RELU (DistilBERT's pre_classifier and ReLU; position_buckets must be 0). */
 #define RMU_HEAD_TANH 0
 #define RMU_HEAD_GELU 1
+#define RMU_HEAD_RELU 2
 typedef struct rmu_encoder_ext {
     int32_t position_buckets, max_relative_positions, head_act;
 } rmu_encoder_ext;
@@ -347,6 +348,19 @@ int rmu_encoder_embed_host(rmu_encoder* enc, const int32_t* ids_h, const int32_t
 int rmu_encoder_classify_host(rmu_encoder* enc, const int32_t* ids_h, const int32_t* type_ids_h,
                               const int32_t* cu_seqlens_h, int B, int total_tokens, int max_seqlen, float* out_h,
                               void* stream);
+
+/* sentence-transformers Dense modules after Pooling (distiluse-base-multilingual-cased-v2, LaBSE): attaches the chain
+ * y_{l+1} = act_l(W_l y_l + b_l), l = 0..n_layers-1, with y_0 the pooled row [dims[0] = hidden], W_l [dims[l+1], dims[l]]
+ * and b_l [dims[l+1]] host fp32 (b_h or any b_h[l] may be NULL: no bias), act_l RMU_DENSE_IDENTITY or RMU_DENSE_TANH.
+ * Afterwards rmu_encoder_embed and rmu_encoder_embed_host pool without normalising, run the chain in fp32 (one fmaf
+ * chain per output, fixed order, no atomics) and then, when normalize, apply Normalize: they write [B, dims[n_layers]].
+ * rmu_encoder_hidden and rmu_encoder_classify are unchanged.  Refused: a null handle, dims, W_h or acts, n_layers <= 0,
+ * dims[0] != hidden, a width <= 0, a null W_h[l], or a second call (RMU_ERR_ARG); an act other than 0 or 1, or a
+ * Qwen3 / Llama handle (RMU_ERR_UNSUPPORTED). */
+#define RMU_DENSE_IDENTITY 0
+#define RMU_DENSE_TANH 1
+int rmu_encoder_set_dense(rmu_encoder* enc, int n_layers, const int32_t* dims, const float* const* W_h,
+                          const float* const* b_h, const int32_t* acts);
 
 /* ------------------------------------------------------------------ ColBERT late interaction
  * Stands behind HuggingFaceCrossEncoder.score on a ColBERT checkpoint (the reference README's `rerank_model`
@@ -537,6 +551,12 @@ int rmu_debug_cls_head_act(const uint16_t* hi, const uint16_t* lo, const int32_t
 /* For tests: n fp32 values -> (hi, lo) planes, as every GEMM weight is uploaded; and hi + lo -> n fp32 values, as
  * rmu_encoder_hidden returns the last hidden state.  n < 0 or a null pointer return RMU_ERR_ARG; n = 0 launches
  * nothing. */
+/* For tests: one Dense module on device rows x [B, n_in] fp32: y [B, n_out] = act(W x + b) with W [n_out, n_in], b
+ * [n_out] or NULL, act RMU_DENSE_IDENTITY or RMU_DENSE_TANH, then y / max(||y||, 1e-12) per row when normalize, as
+ * rmu_encoder_set_dense's chain runs it.  A null pointer or a width or B <= 0 returns RMU_ERR_ARG, another act
+ * RMU_ERR_UNSUPPORTED. */
+int rmu_debug_dense(const float* x, int B, int n_in, int n_out, const float* W, const float* b, int act, int normalize,
+                    float* y, void* stream);
 int rmu_debug_split_planes(const float* src, int64_t n, uint16_t* hi, uint16_t* lo, void* stream);
 int rmu_debug_join_planes(const uint16_t* hi, const uint16_t* lo, int64_t n, float* out, void* stream);
 /* For tests: the BM25 select stage alone (bm25_select_kernel rounds, through the launcher rmu_bm25_search uses) on

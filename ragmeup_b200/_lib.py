@@ -121,6 +121,8 @@ SIGNATURES = {
                                          C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "rmu_encoder_classify_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                             C.c_void_p, C.c_void_p]),
+    "rmu_encoder_set_dense": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                        C.c_void_p]),
     "rmu_colbert_create": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(C.c_void_p), C.c_int, C.c_void_p, C.c_int,
                                      C.POINTER(C.c_void_p)]),
     "rmu_colbert_destroy": (None, [C.c_void_p]),
@@ -157,6 +159,8 @@ SIGNATURES = {
     "rmu_debug_encoder_position_planes": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_cls_head_act": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "rmu_debug_dense": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                  C.c_void_p, C.c_void_p]),
     "rmu_debug_pool": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                  C.c_void_p]),
     "rmu_debug_cls_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

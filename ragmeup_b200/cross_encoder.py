@@ -123,9 +123,9 @@ class HuggingFaceCrossEncoder(BaseCrossEncoder):
         else:
             # pair batches assembled from cached per-text ids (identical to self._ragged(a, b); tests/test_host_logic.py)
             self._pairs = PairAssembler(self.tokenizer, self.max_length)
-        # XLM-R / RoBERTa take no token types (their tokenizers return none), and DeBERTa-v3, ModernBERT and Qwen3 have
-        # no token-type table: a null pointer, all zeros
-        self._types = not (xlmr or deberta or modern or qwen)
+        # XLM-R / RoBERTa take no token types (their tokenizers return none), and DeBERTa-v3, ModernBERT, Qwen3 and a
+        # one-row table (DistilBERT) have none to select: a null pointer, all zeros
+        self._types = not (xlmr or deberta or modern or qwen) and cfg.type_vocab > 1
         self.client = BertEncoder(cfg, w, with_head=True, device=device)
         self._max_tokens = self.client.max_tokens_per_call
 

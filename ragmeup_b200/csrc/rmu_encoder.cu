@@ -555,7 +555,7 @@ __global__ void __launch_bounds__(256) pool_kernel(const __half* __restrict__ hi
 }
 
 // BertPooler (tanh(W_p h_cls + b_p)) + classifier -> logits [B, num_labels]; head_act RMU_HEAD_GELU: DeBERTa's ContextPooler,
-// erf-GELU in place of tanh.  An empty sequence has h_cls = 0 (its row
+// erf-GELU in place of tanh; RMU_HEAD_RELU: DistilBERT's pre_classifier and ReLU.  An empty sequence has h_cls = 0 (its row
 // cu[b] belongs to the next sequence, or lies past T).  compact: h_cls of sequence b is row b of [B, H] planes.
 __global__ void __launch_bounds__(256) cls_head_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo,
                                                        const int* __restrict__ cu, int H, int num_labels, int compact,
@@ -578,7 +578,7 @@ __global__ void __launch_bounds__(256) cls_head_kernel(const __half* __restrict_
         for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
         if (lane_id() == 0) {
             const float x = s + pb[j];
-            pooled[j] = head_act == RMU_HEAD_GELU ? gelu_erf(x) : tanhf(x);
+            pooled[j] = head_act == RMU_HEAD_GELU ? gelu_erf(x) : head_act == RMU_HEAD_RELU ? fmaxf(x, 0.f) : tanhf(x);
         }
     }
     __syncthreads();
@@ -640,6 +640,55 @@ __global__ void __launch_bounds__(256) mb_head_kernel(const float* __restrict__ 
         for (int off = 16; off > 0; off >>= 1) t += __shfl_xor_sync(0xffffffffu, t, off);
         if (lane_id() == 0) out[static_cast<size_t>(b) * num_labels + c] = t + cb[c];
     }
+}
+
+// sentence-transformers Dense on pooled rows: y [B, n_out] = act(W x + b) with x [B, n_in], W [n_out, n_in], b [n_out] or
+// null, act RMU_DENSE_IDENTITY or RMU_DENSE_TANH.  A block takes kDenseRows rows and kDenseCols outputs, one warp per
+// output at a time, so each W row is read once for kDenseRows rows.  Output j of row r is lane l's fmaf chain over
+// d = l, l + 32, ... in order, then a fixed xor tree, then the bias and act: the same operations whatever rows share its
+// block, so a row's bits do not depend on the batch it came in.  A plain SIMT kernel: at the ingest shape the projection
+// is < 0.01 % of the encoder's FLOPs.  It is a launch of its own rather than part of pool_kernel, whose one block per
+// sequence would read all of W once per row.
+constexpr int kDenseRows = 8, kDenseCols = 64;
+__global__ void __launch_bounds__(256) dense_kernel(const float* __restrict__ x, int B, int n_in, int n_out,
+                                                    const float* __restrict__ W, const float* __restrict__ bias, int act,
+                                                    float* __restrict__ y) {
+    const int r0 = blockIdx.x * kDenseRows;
+    const int nr = min(kDenseRows, B - r0);
+    const int warp = threadIdx.x >> 5, lane = lane_id();
+    const int j_end = min(n_out, static_cast<int>(blockIdx.y + 1) * kDenseCols);
+    for (int j = blockIdx.y * kDenseCols + warp; j < j_end; j += blockDim.x >> 5) {
+        const float* wr = W + static_cast<size_t>(j) * n_in;
+        float s[kDenseRows];
+#pragma unroll
+        for (int r = 0; r < kDenseRows; ++r) s[r] = 0.f;
+        for (int d = lane; d < n_in; d += 32) {
+            const float w = __ldg(wr + d);
+#pragma unroll
+            for (int r = 0; r < kDenseRows; ++r)
+                if (r < nr) s[r] = fmaf(w, x[static_cast<size_t>(r0 + r) * n_in + d], s[r]);
+        }
+#pragma unroll
+        for (int r = 0; r < kDenseRows; ++r) {
+            float v = s[r];
+            for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+            if (bias) v += bias[j];
+            if (act == RMU_DENSE_TANH) v = tanhf(v);
+            if (lane == 0 && r < nr) y[static_cast<size_t>(r0 + r) * n_out + j] = v;
+        }
+    }
+}
+
+// sentence-transformers Normalize: y[r] /= max(||y[r]||, 1e-12), one warp per row (lane-strided fmaf chain, xor tree)
+__global__ void __launch_bounds__(256) l2_normalize_rows_kernel(float* __restrict__ y, int B, int n) {
+    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= B) return;
+    float* yr = y + static_cast<size_t>(row) * n;
+    float ss = 0.f;
+    for (int d = lane_id(); d < n; d += 32) ss = fmaf(yr[d], yr[d], ss);
+    for (int off = 16; off > 0; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
+    const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
+    for (int d = lane_id(); d < n; d += 32) yr[d] *= inv;
 }
 
 // pos[t] = t - cu[b] for token t of sequence b: each row's position within its sequence (the rotary epilogue's input)
@@ -820,6 +869,22 @@ static int launch_cls_head(const __half* hi, const __half* lo, const int* cu, in
                                                            head_act, out);
     count_launch();
     RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// E4 dense_kernel, then l2_normalize_rows_kernel when normalize: x [B, n_in] -> y [B, n_out]
+static int launch_dense(const float* x, int B, int n_in, int n_out, const float* W, const float* b, int act, int normalize,
+                        float* y, cudaStream_t st) {
+    ProfScope _ps(PROF_POOL_HEAD, st);
+    dense_kernel<<<dim3((B + kDenseRows - 1) / kDenseRows, (n_out + kDenseCols - 1) / kDenseCols), 256, 0, st>>>(
+        x, B, n_in, n_out, W, b, act, y);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    if (normalize) {
+        l2_normalize_rows_kernel<<<(B + 7) / 8, 256, 0, st>>>(y, B, n_out);
+        count_launch();
+        RMU_CHECK_LAUNCH();
+    }
     return RMU_OK;
 }
 
@@ -1944,6 +2009,13 @@ struct rmu_encoder {
     float* span_ws = nullptr;
     size_t span_ws_cap = 0;
     int* span_cu = nullptr;
+    // sentence-transformers Dense modules after pooling (rmu_encoder_set_dense): dense_dims [n + 1], per layer W [out, in],
+    // b [out] or null, act; dense_ws holds two [B, max width] ping-pong rows, grown under mu
+    std::vector<int> dense_dims;
+    std::vector<float*> dense_w, dense_b;
+    std::vector<int> dense_act;
+    float* dense_ws = nullptr;
+    size_t dense_ws_cap = 0;
     // activations
     int tok_cap = 0, seq_cap = 0;
     std::vector<void*> act_allocs;
@@ -1964,7 +2036,7 @@ struct rmu_encoder {
     // concurrent device-pointer caller may free and re-allocate under mu)
     int *d_ids = nullptr, *d_typ = nullptr, *d_cu = nullptr;
     float* d_out = nullptr;
-    int stage_tok_cap = 0, stage_seq_cap = 0;
+    int stage_tok_cap = 0, stage_seq_cap = 0, stage_out_w = 0;
     cudaEvent_t ws_done = nullptr;   // last use of the shared activation workspace (callers on other streams wait on it)
     std::mutex mu;
     std::mutex host_mu;   // the *_host entry points share the staging buffers above: one at a time per handle
@@ -2029,6 +2101,38 @@ static int ensure_span_ws(rmu_encoder* e, int T) {
     RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->span_ws), need * sizeof(float)));
     e->span_ws_cap = need;
     return RMU_OK;
+}
+
+// the width rmu_encoder_embed writes: the last Dense module's out_features, else hidden
+static int embed_width(const rmu_encoder* e) { return e->dense_dims.empty() ? e->cfg.hidden : e->dense_dims.back(); }
+
+static int ensure_dense_ws(rmu_encoder* e, int B) {
+    const size_t need = 2 * static_cast<size_t>(B) * *std::max_element(e->dense_dims.begin(), e->dense_dims.end());
+    if (need <= e->dense_ws_cap) return RMU_OK;
+    RMU_CUDA(cudaDeviceSynchronize());
+    cudaFree(e->dense_ws);
+    e->dense_ws = nullptr;
+    e->dense_ws_cap = 0;
+    RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->dense_ws), need * sizeof(float)));
+    e->dense_ws_cap = need;
+    return RMU_OK;
+}
+
+// mu held: the pooled rows (not normalised) -> the Dense chain -> out [B, embed_width], normalised last when asked
+static int run_dense(rmu_encoder* e, const SplitOperand& h, const int* cu, int B, int pool_mode, bool compact, int normalize,
+                     float* out, cudaStream_t st) {
+    int rc = ensure_dense_ws(e, B);
+    if (rc != RMU_OK) return rc;
+    const size_t half = e->dense_ws_cap / 2;
+    float* buf[2] = {e->dense_ws, e->dense_ws + half};
+    rc = launch_pool(h.hi, h.lo, cu, B, e->cfg.hidden, pool_mode, 0, compact, buf[0], st);
+    const int n = static_cast<int>(e->dense_w.size());
+    for (int l = 0; l < n && rc == RMU_OK; ++l) {
+        const bool last = l == n - 1;
+        rc = launch_dense(buf[l & 1], B, e->dense_dims[l], e->dense_dims[l + 1], e->dense_w[l], e->dense_b[l], e->dense_act[l],
+                          last ? normalize : 0, last ? out : buf[(l + 1) & 1], st);
+    }
+    return rc;
 }
 
 // DeBERTa: the position terms' workspace for a call (qrows query rows, T keys), grown to fit
@@ -2413,11 +2517,16 @@ int rmu_encoder_create_ex(const rmu_bert_config* cfg, const rmu_encoder_ext* ext
         set_error("rmu_encoder_create: adapter_dim must be 0 (no adapter) or a multiple of 128 no larger than ffn");
         return RMU_ERR_UNSUPPORTED;
     }
-    if (ext.head_act != RMU_HEAD_TANH && ext.head_act != RMU_HEAD_GELU) {
-        set_error("rmu_encoder_create: head_act must be RMU_HEAD_TANH (0) or RMU_HEAD_GELU (1)");
+    const int PB = ext.position_buckets, MRP = ext.max_relative_positions;
+    if (ext.head_act != RMU_HEAD_TANH && ext.head_act != RMU_HEAD_GELU && ext.head_act != RMU_HEAD_RELU) {
+        set_error("rmu_encoder_create: head_act must be RMU_HEAD_TANH (0), RMU_HEAD_GELU (1) or RMU_HEAD_RELU (2)");
         return RMU_ERR_UNSUPPORTED;
     }
-    const int PB = ext.position_buckets, MRP = ext.max_relative_positions;
+    if (ext.head_act == RMU_HEAD_RELU && PB != 0) {
+        // DistilBERT's head; no model pairs it with disentangled attention
+        set_error("rmu_encoder_create: head_act RMU_HEAD_RELU (DistilBERT's head) takes position_buckets 0");
+        return RMU_ERR_UNSUPPORTED;
+    }
     if (PB < 0 || (PB == 0 && MRP != 0) || PB > 4096) {
         set_error("rmu_encoder_create: position_buckets must be 0 (with max_relative_positions 0) or 1..4096");
         return RMU_ERR_UNSUPPORTED;
@@ -2889,6 +2998,7 @@ void rmu_encoder_destroy(rmu_encoder* e) {
     cudaDeviceSynchronize();
     free_acts(e);
     cudaFree(e->d_ids); cudaFree(e->d_typ); cudaFree(e->d_cu); cudaFree(e->d_out);
+    cudaFree(e->dense_ws);
     for (void* p : e->allocs) cudaFree(p);
     if (e->ws_done) cudaEventDestroy(e->ws_done);
     delete e;
@@ -2917,7 +3027,10 @@ int rmu_encoder_embed(rmu_encoder* e, const int32_t* ids, const int32_t* type_id
     rc = run_encoder(e, ids, type_ids, cu, B, T, max_seqlen, cls, st);
     if (rc != RMU_OK) return rc;
     const SplitOperand& h = cls ? e->X_cls : e->X;
-    rc = launch_pool(h.hi, h.lo, cu, B, e->cfg.hidden, pool_mode, normalize, cls, out, st);
+    if (e->dense_w.empty())
+        rc = launch_pool(h.hi, h.lo, cu, B, e->cfg.hidden, pool_mode, normalize, cls, out, st);
+    else
+        rc = run_dense(e, h, cu, B, pool_mode, cls, normalize, out, st);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
@@ -3016,18 +3129,20 @@ int rmu_decoder_attention_spans(rmu_encoder* e, const int32_t* ids, int T, const
 // host_mu held: the staging buffers belong to the *_host entry points only
 static int stage_batch(rmu_encoder* e, const int32_t* ids_h, const int32_t* typ_h, const int32_t* cu_h, int B, int T,
                        cudaStream_t st) {
-    if (T > e->stage_tok_cap || B + 1 > e->stage_seq_cap) {
+    const int out_w = std::max(embed_width(e), e->cfg.num_labels);
+    if (T > e->stage_tok_cap || B + 1 > e->stage_seq_cap || out_w > e->stage_out_w) {
         RMU_CUDA(cudaStreamSynchronize(st));              // earlier *_host calls on this stream are complete (they synchronise)
         cudaFree(e->d_ids); cudaFree(e->d_typ); cudaFree(e->d_cu); cudaFree(e->d_out);
         e->d_ids = e->d_typ = e->d_cu = nullptr; e->d_out = nullptr;
-        e->stage_tok_cap = e->stage_seq_cap = 0;
+        e->stage_tok_cap = e->stage_seq_cap = e->stage_out_w = 0;
         const int cap = (std::max(T, 1024) + 127) / 128 * 128, scap = std::max(B + 1, 1024);
         RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->d_ids), static_cast<size_t>(cap) * sizeof(int)));
         RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->d_typ), static_cast<size_t>(cap) * sizeof(int)));
         RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->d_cu), static_cast<size_t>(scap) * sizeof(int)));
-        RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->d_out), static_cast<size_t>(scap) * std::max(e->cfg.hidden, e->cfg.num_labels) * sizeof(float)));
+        RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->d_out), static_cast<size_t>(scap) * out_w * sizeof(float)));
         e->stage_tok_cap = cap;
         e->stage_seq_cap = scap;
+        e->stage_out_w = out_w;
     }
     RMU_CUDA(cudaMemcpyAsync(e->d_ids, ids_h, static_cast<size_t>(T) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     if (typ_h) RMU_CUDA(cudaMemcpyAsync(e->d_typ, typ_h, static_cast<size_t>(T) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
@@ -3045,7 +3160,7 @@ int rmu_encoder_embed_host(rmu_encoder* e, const int32_t* ids_h, const int32_t* 
     if (rc != RMU_OK) return rc;
     rc = rmu_encoder_embed(e, e->d_ids, typ_h ? e->d_typ : nullptr, e->d_cu, B, T, max_seqlen, pool_mode, normalize, e->d_out, st);
     if (rc != RMU_OK) return rc;
-    RMU_CUDA(cudaMemcpyAsync(out_h, e->d_out, static_cast<size_t>(B) * e->cfg.hidden * sizeof(float), cudaMemcpyDeviceToHost, st));
+    RMU_CUDA(cudaMemcpyAsync(out_h, e->d_out, static_cast<size_t>(B) * embed_width(e) * sizeof(float), cudaMemcpyDeviceToHost, st));
     RMU_CUDA(cudaStreamSynchronize(st));
     return RMU_OK;
 }
@@ -3062,6 +3177,45 @@ int rmu_encoder_classify_host(rmu_encoder* e, const int32_t* ids_h, const int32_
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaMemcpyAsync(out_h, e->d_out, static_cast<size_t>(B) * e->cfg.num_labels * sizeof(float), cudaMemcpyDeviceToHost, st));
     RMU_CUDA(cudaStreamSynchronize(st));
+    return RMU_OK;
+}
+
+int rmu_encoder_set_dense(rmu_encoder* e, int n_layers, const int32_t* dims, const float* const* W_h, const float* const* b_h,
+                          const int32_t* acts) {
+    if (!e || n_layers <= 0 || !dims || !W_h || !acts) { set_error("rmu_encoder_set_dense: bad argument"); return RMU_ERR_ARG; }
+    if (e->qwen) {
+        set_error("rmu_encoder_set_dense: Qwen3 and Llama encoders take no Dense modules (their last-token kernel "
+                  "normalises its row itself)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    if (dims[0] != e->cfg.hidden) {
+        set_error("rmu_encoder_set_dense: dims[0] = " + std::to_string(dims[0]) + " must equal hidden (" +
+                  std::to_string(e->cfg.hidden) + ")");
+        return RMU_ERR_ARG;
+    }
+    for (int l = 0; l < n_layers; ++l) {
+        if (dims[l + 1] <= 0 || !W_h[l]) {
+            set_error("rmu_encoder_set_dense: layer " + std::to_string(l) + " needs a positive width and a weight");
+            return RMU_ERR_ARG;
+        }
+        if (acts[l] != RMU_DENSE_IDENTITY && acts[l] != RMU_DENSE_TANH) {
+            set_error("rmu_encoder_set_dense: act must be RMU_DENSE_IDENTITY (0) or RMU_DENSE_TANH (1)");
+            return RMU_ERR_UNSUPPORTED;
+        }
+    }
+    std::lock_guard<std::mutex> hg(e->host_mu);
+    std::lock_guard<std::mutex> g(e->mu);
+    if (!e->dense_w.empty()) { set_error("rmu_encoder_set_dense: a projection is already attached"); return RMU_ERR_ARG; }
+    std::vector<float*> w(n_layers, nullptr), b(n_layers, nullptr);
+    for (int l = 0; l < n_layers; ++l) {
+        int rc = upload(e, &w[l], W_h[l], static_cast<size_t>(dims[l + 1]) * dims[l]);
+        if (rc == RMU_OK && b_h && b_h[l]) rc = upload(e, &b[l], b_h[l], dims[l + 1]);
+        if (rc != RMU_OK) return rc;
+    }
+    e->dense_dims.assign(dims, dims + n_layers + 1);
+    e->dense_w = w;
+    e->dense_b = b;
+    e->dense_act.assign(acts, acts + n_layers);
     return RMU_OK;
 }
 
@@ -3489,7 +3643,7 @@ int rmu_debug_cls_head_act(const uint16_t* hi, const uint16_t* lo, const int32_t
                            const float* pw, const float* pb, const float* cw, const float* cb, int head_act, float* out,
                            void* stream) {
     if (!hi || !lo || !cu || !pw || !pb || !cw || !cb || !out || B <= 0 || H <= 0 || num_labels <= 0 ||
-        (head_act != RMU_HEAD_TANH && head_act != RMU_HEAD_GELU)) {
+        (head_act != RMU_HEAD_TANH && head_act != RMU_HEAD_GELU && head_act != RMU_HEAD_RELU)) {
         set_error("rmu_debug_cls_head_act: bad argument");
         return RMU_ERR_ARG;
     }
@@ -3499,6 +3653,16 @@ int rmu_debug_cls_head_act(const uint16_t* hi, const uint16_t* lo, const int32_t
     }
     return launch_cls_head(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), cu, B, H, num_labels,
                            false, pw, pb, cw, cb, out, static_cast<cudaStream_t>(stream), head_act);
+}
+
+int rmu_debug_dense(const float* x, int B, int n_in, int n_out, const float* W, const float* b, int act, int normalize,
+                    float* y, void* stream) {
+    if (!x || !W || !y || B <= 0 || n_in <= 0 || n_out <= 0) { set_error("rmu_debug_dense: bad argument"); return RMU_ERR_ARG; }
+    if (act != RMU_DENSE_IDENTITY && act != RMU_DENSE_TANH) {
+        set_error("rmu_debug_dense: act must be RMU_DENSE_IDENTITY (0) or RMU_DENSE_TANH (1)");
+        return RMU_ERR_UNSUPPORTED;
+    }
+    return launch_dense(x, B, n_in, n_out, W, b, act, normalize, y, static_cast<cudaStream_t>(stream));
 }
 
 int rmu_debug_attention_window(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu, int B, int H, int heads,

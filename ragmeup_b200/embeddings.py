@@ -61,8 +61,9 @@ class HuggingFaceEmbeddings:
         self.tokenizer = load_tokenizer(vocab_src, cfg.vocab_size, mpnet=isinstance(cfg, MPNetConfig), xlmr=xlmr,
                                         modernbert=modern, qwen3=qwen)
         self._ragged = RaggedTokenizer(self.tokenizer, self.max_seq_length)
-        # XLM-R / RoBERTa take no token types, ModernBERT and Qwen3 have none: a null pointer, all zeros
-        self._types = not (xlmr or modern or qwen)
+        # XLM-R / RoBERTa take no token types, ModernBERT and Qwen3 have none, nor has a one-row table (DistilBERT): a
+        # null pointer, all zeros
+        self._types = not (xlmr or modern or qwen) and cfg.type_vocab > 1
         # Qwen3: the snapshot's default prompt (config_sentence_transformers.json default_prompt_name), if it sets one
         self._prompt = cfg.prompt if qwen else ""
         self.client = BertEncoder(cfg, w, with_head=False, device=device)
@@ -72,7 +73,7 @@ class HuggingFaceEmbeddings:
         """texts -> CUDA fp32 [n, dim] (stays on the device)."""
         torch = self.client.torch
         if len(texts) == 0:
-            return torch.empty((0, self.config.hidden), dtype=torch.float32, device=self.client.device)
+            return torch.empty((0, self.client.embed_dim), dtype=torch.float32, device=self.client.device)
         texts = [self._prompt + t.replace("\n", " ").strip() for t in texts]
         ids, typ, cu = self._ragged(texts)
         outs = []
@@ -85,7 +86,7 @@ class HuggingFaceEmbeddings:
 
     def _encode_host(self, texts: List[str]) -> np.ndarray:
         if len(texts) == 0:
-            return np.zeros((0, self.config.hidden), dtype=np.float32)
+            return np.zeros((0, self.client.embed_dim), dtype=np.float32)
         texts = [self._prompt + t.replace("\n", " ").strip() for t in texts]
         # bulk calls: WordPiece of chunk i+1 overlapped with the device encode of chunk i
         chunks = [texts[s:s + PIPE_TEXTS] for s in range(0, len(texts), PIPE_TEXTS)]

@@ -20,6 +20,9 @@ token only (``pooling="last"``), and a forward whose activations leave the fp16 
 
 Llama (``weights.LlamaConfig``, ``rmu_encoder_create_llama``) takes Qwen3's order without q_norm / k_norm and without a
 head, with the config's own rope tables (``llama3`` scaling); it is built for attention provenance only.
+
+A weight dict that holds sentence-transformers Dense modules (``weights.dense_layers``) attaches them to the handle
+(``rmu_encoder_set_dense``): the embed entry points then return ``embed_dim`` = the last Dense width per row.
 """
 from __future__ import annotations
 
@@ -29,7 +32,8 @@ from typing import Dict, Optional
 import numpy as np
 
 from . import _lib
-from .weights import BertConfig, LlamaConfig, ModernBertConfig, Qwen3Config, rope_table, rope_tables, weight_names
+from .weights import (BertConfig, LlamaConfig, ModernBertConfig, Qwen3Config, dense_layers, rope_table, rope_tables,
+                      weight_names)
 
 POOL = {"mean": 0, "cls": 1, "last": 2}
 RMU_ERR_RANGE = -4
@@ -96,6 +100,17 @@ class BertEncoder:
             else:
                 _lib.check(_lib.lib().rmu_encoder_create(C.byref(cc), ptrs, len(arrs), int(self.with_head),
                                                          C.byref(self._h)), "rmu_encoder_create")
+            dense = dense_layers(weights)
+            self.embed_dim = int(dense[-1][0].shape[0]) if dense else cfg.hidden
+            if dense:
+                Ws = [np.ascontiguousarray(W, dtype=np.float32) for W, _b, _a in dense]
+                bs = [None if b is None else np.ascontiguousarray(b, dtype=np.float32) for _W, b, _a in dense]
+                dims = np.asarray([cfg.hidden] + [W.shape[0] for W in Ws], dtype=np.int32)
+                acts = np.asarray([a for _W, _b, a in dense], dtype=np.int32)
+                _lib.check(_lib.lib().rmu_encoder_set_dense(
+                    self._h, len(Ws), dims.ctypes.data, (C.c_void_p * len(Ws))(*[W.ctypes.data for W in Ws]),
+                    (C.c_void_p * len(bs))(*[None if b is None else b.ctypes.data for b in bs]), acts.ctypes.data),
+                    "rmu_encoder_set_dense")
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -121,13 +136,13 @@ class BertEncoder:
         return a.to(device=self.device, dtype=dtype, non_blocking=True).contiguous()
 
     def embed_tokens(self, ids, type_ids, cu_seqlens, max_seqlen: int, pooling: str = "mean", normalize: bool = True):
-        """ragged token batch -> CUDA fp32 [B, hidden] sentence embeddings."""
+        """ragged token batch -> CUDA fp32 [B, embed_dim] sentence embeddings."""
         torch = self.torch
         ids = self._dev(ids, torch.int32)
         typ = None if type_ids is None else self._dev(type_ids, torch.int32)
         cu = self._dev(cu_seqlens, torch.int32)
         B = cu.numel() - 1
-        out = torch.empty((B, self.cfg.hidden), dtype=torch.float32, device=self.device)
+        out = torch.empty((B, self.embed_dim), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             self._check(_lib.lib().rmu_encoder_embed(self._h, ids.data_ptr(), None if typ is None else typ.data_ptr(),
                                                     cu.data_ptr(), B, ids.numel(), int(max_seqlen), POOL[pooling],
@@ -178,9 +193,9 @@ class BertEncoder:
 
     def embed_host(self, ids: np.ndarray, type_ids: Optional[np.ndarray], cu: np.ndarray, pooling: str = "mean",
                    normalize: bool = True) -> np.ndarray:
-        """host int32 token batch -> host fp32 [B, hidden] (H2D/D2H inside the C call)."""
+        """host int32 token batch -> host fp32 [B, embed_dim] (H2D/D2H inside the C call)."""
         B = len(cu) - 1
-        out = np.empty((B, self.cfg.hidden), dtype=np.float32)
+        out = np.empty((B, self.embed_dim), dtype=np.float32)
         ids = np.ascontiguousarray(ids, dtype=np.int32)
         typ = None if type_ids is None else np.ascontiguousarray(type_ids, dtype=np.int32)
         cu = np.ascontiguousarray(cu, dtype=np.int32)

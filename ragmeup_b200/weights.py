@@ -126,6 +126,62 @@ class XLMRConfig(BertConfig):
                           num_labels=len(d["id2label"]) if "id2label" in d else d.get("num_labels", 1))
 
 
+@dataclass
+class DistilBertConfig(BertConfig):
+    """DistilBERT (transformers ``DistilBertModel`` / ``DistilBertForSequenceClassification``; distiluse-base-multilingual-
+    cased-v2): BERT's post-LN encoder with erf-GELU, LayerNorm eps 1e-12, learned positions and BERT's attention scaling,
+    under other tensor names (``distilbert_to_canonical``) and without token types.  The encoder gets a zero [1, H]
+    token-type table, so no type id can select a non-zero row: (w + 0) + p == w + p exactly.  It runs BERT's forward as
+    it is; only the head differs: ``classifier(relu(pre_classifier(h_CLS)))`` (``head_act`` RMU_HEAD_RELU)."""
+    vocab_size: int = 30522
+    hidden: int = 768
+    layers: int = 6
+    heads: int = 12
+    ffn: int = 3072
+    type_vocab: int = 1
+    head_act: ClassVar[int] = 2
+
+    @staticmethod
+    def from_hf(d: dict) -> "DistilBertConfig":
+        """config.json of a ``distilbert`` checkpoint -> DistilBertConfig; eps is 1e-12, which DistilBERT hard-codes"""
+        if d.get("activation", "gelu") != "gelu":
+            raise ValueError(f"distilbert with activation = {d.get('activation')!r} is not supported: only erf-GELU is "
+                             f"computed")
+        for field in ("vocab_size", "dim", "n_layers", "n_heads", "hidden_dim"):
+            if field not in d:
+                raise ValueError(f"distilbert config.json without {field!r} is not supported: a DistilBERT checkpoint "
+                                 f"states its shape in vocab_size, dim, n_layers, n_heads and hidden_dim")
+        return DistilBertConfig(vocab_size=int(d["vocab_size"]), hidden=int(d["dim"]), layers=int(d["n_layers"]),
+                                heads=int(d["n_heads"]), ffn=int(d["hidden_dim"]),
+                                max_pos=int(d.get("max_position_embeddings", 512)),
+                                num_labels=len(d["id2label"]) if "id2label" in d else d.get("num_labels", 1))
+
+
+# DistilBERT checkpoint names -> the BERT names of ``weight_names`` (the embeddings have BERT's names already)
+_DISTILBERT_RENAME = (("transformer.layer.", "encoder.layer."), ("attention.q_lin.", "attention.self.query."),
+                      ("attention.k_lin.", "attention.self.key."), ("attention.v_lin.", "attention.self.value."),
+                      ("attention.out_lin.", "attention.output.dense."), ("sa_layer_norm.", "attention.output.LayerNorm."),
+                      ("ffn.lin1.", "intermediate.dense."), ("ffn.lin2.", "output.dense."),
+                      ("output_layer_norm.", "output.LayerNorm."), ("pre_classifier.", "pooler.dense."))
+
+
+def distilbert_to_canonical(raw: Dict[str, np.ndarray], cfg: DistilBertConfig) -> Dict[str, np.ndarray]:
+    """DistilBERT tensors (bare, or under ``distilbert.`` as the sequence-classification model saves them) -> the
+    canonical names of ``weight_names``, with a zero [1, H] token-type table.  ``position_embeddings.weight`` is read as
+    stored, also for ``sinusoidal_pos_embds`` checkpoints (transformers keeps that table in the state dict).  The
+    masked-LM head (``vocab_transform``, ``vocab_layer_norm``, ``vocab_projector``) is dropped."""
+    w: Dict[str, np.ndarray] = {}
+    for k, v in raw.items():
+        k = k[11:] if k.startswith("distilbert.") else k
+        if k.startswith(("vocab_transform.", "vocab_layer_norm.", "vocab_projector.")):
+            continue
+        for a, b in _DISTILBERT_RENAME:
+            k = k.replace(a, b)
+        w[k] = np.ascontiguousarray(v, dtype=np.float32)
+    w["embeddings.token_type_embeddings.weight"] = np.zeros((1, cfg.hidden), np.float32)
+    return w
+
+
 XMOD_LANGUAGE_ENV = "RMU_XMOD_LANGUAGE"
 SYNTHETIC_LANGUAGES = ("en_XX", "de_DE", "fr_XX")
 
@@ -694,7 +750,7 @@ def adapter_prefix(layer: int, language: str) -> str:
 
 
 # config.json model_type -> how the snapshot is read; a config without model_type is read as BERT
-MODEL_TYPES = ("bert", "mpnet", "roberta", "xlm-roberta", "xmod", "deberta-v2", "modernbert", "qwen3")
+MODEL_TYPES = ("bert", "mpnet", "roberta", "xlm-roberta", "xmod", "deberta-v2", "modernbert", "qwen3", "distilbert")
 
 
 # shapes of the models BASELINE.json / .env.template name (SURVEY.md §2.2 table)
@@ -755,10 +811,25 @@ PRESETS: Dict[str, Tuple[BertConfig, str, int]] = {
     "qwen3-reranker-0.6b": (Qwen3Config(reranker=True, num_labels=2), "last", 8192),
     "tiny-qwen3": (Qwen3Config(vocab_size=1000, hidden=256, layers=3, heads=4, ffn=384, max_pos=8192, kv_heads=2,
                                rope_theta=10000.0, tie_word_embeddings=False, pad_token_id=0), "last", 8192),
+    # sentence-transformers models with a Dense module after pooling (DENSE_PRESETS) [3P-recall: their config.json and
+    # module files are not read here].  distiluse-base-multilingual-cased-v2: DistilBERT, mean pooling, Dense 768 -> 512
+    # tanh, no Normalize.  LaBSE: BERT, CLS pooling, Dense 768 -> 768 tanh, Normalize.  tiny-distilbert: a widening
+    # Dense, so the output is wider than hidden.
+    "distiluse-base-multilingual-cased-v2": (DistilBertConfig(vocab_size=119547), "mean", 128),
+    "LaBSE": (BertConfig(vocab_size=501153, hidden=768, layers=12, heads=12, ffn=3072), "cls", 256),
+    "tiny-distilbert": (DistilBertConfig(vocab_size=1000, hidden=128, layers=2, heads=4, ffn=256, max_pos=128), "mean", 64),
 }
 
 # presets whose sentence-transformers pipeline has no Normalize module
-UNNORMALIZED_PRESETS = {"multi-qa-mpnet-base-dot-v1", "paraphrase-multilingual-mpnet-base-v2", "gte-modernbert-base"}
+UNNORMALIZED_PRESETS = {"multi-qa-mpnet-base-dot-v1", "paraphrase-multilingual-mpnet-base-v2", "gte-modernbert-base",
+                        "distiluse-base-multilingual-cased-v2", "tiny-distilbert"}
+
+# Dense modules of the presets above, in order: (out_features, bias, activation)
+DENSE_PRESETS: Dict[str, Tuple[Tuple[int, bool, str], ...]] = {
+    "distiluse-base-multilingual-cased-v2": ((512, True, "tanh"),),
+    "LaBSE": ((768, True, "tanh"),),
+    "tiny-distilbert": ((200, True, "tanh"),),
+}
 
 # FlashRank's model names -> the public HuggingFace checkpoints its ONNX files were exported from [3P-recall: flashrank
 # 0.2.x; the mapping is recalled, not read, and is unverified].  Only the BERT cross-encoders are here: FlashRank's T5
@@ -885,8 +956,9 @@ def synthetic_bert_weights(cfg: BertConfig, seed: int = 0, with_head: bool = Fal
             a = 0.02 * rng.standard_normal(shape) * (3.0 if scale > 1 else 1.0)
         elif name == REL_BIAS:                     # a few units across buckets, as trained MPNet biases spread
             a = rng.standard_normal(shape)
-        elif name == "embeddings.token_type_embeddings.weight" and isinstance(cfg, (MPNetConfig, DebertaConfig)):
-            a = np.zeros(shape)                    # MPNet and DeBERTa have no token types (XLM-R's one row is trained)
+        elif name == "embeddings.token_type_embeddings.weight" and isinstance(cfg, (MPNetConfig, DebertaConfig,
+                                                                                   DistilBertConfig)):
+            a = np.zeros(shape)                    # MPNet, DeBERTa and DistilBERT have no token types (XLM-R's one row is trained)
         elif name == "embeddings.position_embeddings.weight" and isinstance(cfg, DebertaConfig):
             a = np.zeros(shape)                    # nor absolute positions (position_biased_input false)
         elif name.endswith("LayerNorm.weight"):
@@ -901,6 +973,91 @@ def synthetic_bert_weights(cfg: BertConfig, seed: int = 0, with_head: bool = Fal
             a = 0.02 * scale * rng.standard_normal(shape)
         out[name] = np.ascontiguousarray(a, dtype=np.float32)
     return out
+
+
+# sentence-transformers Dense activations -> RMU_DENSE_IDENTITY / RMU_DENSE_TANH
+DENSE_ACTIVATIONS = {"identity": 0, "tanh": 1}
+_DENSE_CLASSES = {"torch.nn.modules.linear.Identity": "identity", "torch.nn.modules.activation.Tanh": "tanh"}
+MODULE_KINDS = ("Transformer", "Pooling", "Dense", "Normalize")
+
+
+def dense_layers(w: Dict[str, np.ndarray]):
+    """the Dense chain a weight dict holds, in order: [(weight [out, in], bias [out] or None, RMU_DENSE_* code)], from
+    ``dense.<i>.weight``, ``dense.<i>.bias`` (absent without a bias) and ``dense.<i>.activation`` (a 0-d int32 code)"""
+    out = []
+    while f"dense.{len(out)}.weight" in w:
+        i = len(out)
+        out.append((w[f"dense.{i}.weight"], w.get(f"dense.{i}.bias"), int(w[f"dense.{i}.activation"])))
+    return out
+
+
+def synthetic_dense_weights(hidden: int, layers, seed: int = 0, scale: float = 1.0) -> Dict[str, np.ndarray]:
+    """seeded Dense modules of DENSE_PRESETS' form, N(0, 0.02 scale) weights and biases, from a stream of their own (the
+    encoder's weights are those of the same preset without Dense)"""
+    rng = np.random.default_rng(seed + 15485863)
+    w: Dict[str, np.ndarray] = {}
+    d_in = hidden
+    for i, (d_out, bias, act) in enumerate(layers):
+        w[f"dense.{i}.weight"] = (0.02 * scale * rng.standard_normal((d_out, d_in))).astype(np.float32)
+        if bias:
+            w[f"dense.{i}.bias"] = (0.02 * scale * rng.standard_normal(d_out)).astype(np.float32)
+        w[f"dense.{i}.activation"] = np.array(DENSE_ACTIVATIONS[act], np.int32)
+        d_in = d_out
+    return w
+
+
+def module_entries(path: str):
+    """modules.json of a sentence-transformers snapshot -> [(kind, module dir)] in order; a module type other than
+    Transformer, Pooling, Dense or Normalize is refused with a ValueError naming the module (the encoder would return a
+    vector that module never saw)"""
+    entries = []
+    for m in _read_json(os.path.join(path, "modules.json")) or []:
+        t = m.get("type", "")
+        kind = t.rsplit(".", 1)[-1]
+        if kind not in MODULE_KINDS:
+            raise ValueError(f"{path}: sentence-transformers module {m.get('path') or m.get('name')!r} of type {t!r} is "
+                             f"not supported: the encoder computes {', '.join(MODULE_KINDS)} modules only")
+        entries.append((kind, m.get("path", "")))
+    return entries
+
+
+def read_modules(path: str, hidden: int):
+    """``module_entries`` and the Dense weights in the form of ``dense_layers``.  Refused with a ValueError naming the
+    module or field: a Dense before Pooling or a Normalize before a Dense (sentence-transformers runs Pooling ->
+    Dense... -> Normalize); a Dense activation other than Tanh or Identity; in_features that do not chain from hidden;
+    a weight or bias that does not match its config."""
+    entries = module_entries(path)
+    kinds = [k for k, _ in entries]
+    w: Dict[str, np.ndarray] = {}
+    d_in, i = hidden, 0
+    for pos, (kind, mdir) in enumerate(entries):
+        if kind != "Dense":
+            continue
+        if "Pooling" not in kinds[:pos]:
+            raise ValueError(f"{path}: Dense module {mdir!r} comes before Pooling; the encoder runs Pooling -> Dense")
+        if "Normalize" in kinds[:pos]:
+            raise ValueError(f"{path}: Normalize comes before Dense module {mdir!r}; the encoder runs Dense -> Normalize")
+        dc = _read_json(os.path.join(path, mdir, "config.json")) or {}
+        act = _DENSE_CLASSES.get(dc.get("activation_function", "torch.nn.modules.activation.Tanh"))
+        if act is None:
+            raise ValueError(f"{path}: Dense module {mdir!r} with activation_function = {dc['activation_function']!r} is "
+                             f"not supported: Tanh and Identity are computed")
+        if int(dc.get("in_features", -1)) != d_in:
+            raise ValueError(f"{path}: Dense module {mdir!r} with in_features = {dc.get('in_features')!r} does not chain: "
+                             f"its input is {d_in} wide")
+        d_out, bias = int(dc.get("out_features", 0)), bool(dc.get("bias", True))
+        t = _load_tensors(os.path.join(path, mdir))
+        W, b = t.get("linear.weight"), t.get("linear.bias")
+        if W is None or W.shape != (d_out, d_in) or (b is not None) != bias or (bias and b.shape != (d_out,)):
+            raise ValueError(f"{path}: Dense module {mdir!r}: linear.weight {None if W is None else W.shape} / linear.bias "
+                             f"{None if b is None else b.shape} do not match out_features = {d_out}, in_features = "
+                             f"{d_in}, bias = {bias}")
+        w[f"dense.{i}.weight"] = np.ascontiguousarray(W, dtype=np.float32)
+        if bias:
+            w[f"dense.{i}.bias"] = np.ascontiguousarray(b, dtype=np.float32)
+        w[f"dense.{i}.activation"] = np.array(DENSE_ACTIVATIONS[act], np.int32)
+        d_in, i = d_out, i + 1
+    return entries, w
 
 
 def _read_json(path: str) -> Optional[dict]:
@@ -977,7 +1134,7 @@ def load_hf_snapshot(path: str, with_head: bool):
     if kind == "qwen3":
         return _load_qwen3_snapshot(path, cfgd, with_head)
     mpnet, xlmr, deberta = kind == "mpnet", kind in ("roberta", "xlm-roberta", "xmod"), kind == "deberta-v2"
-    modern = kind == "modernbert"
+    modern, distil = kind == "modernbert", kind == "distilbert"
     if mpnet and with_head:
         raise ValueError(f"{path}: MPNet cross-encoders are not supported (MPNet runs as a sentence embedder only)")
     if deberta and not with_head:
@@ -988,6 +1145,8 @@ def load_hf_snapshot(path: str, with_head: bool):
         cfg = ModernBertConfig.from_hf(cfgd)
     elif deberta:
         cfg = DebertaConfig.from_hf(cfgd)
+    elif distil:
+        cfg = DistilBertConfig.from_hf(cfgd)
     else:
         cfg = MPNetConfig.from_hf(cfgd) if mpnet else XLMRConfig.from_hf(cfgd) if xlmr else BertConfig.from_hf(cfgd)
     raw = _load_tensors(path, _xmod_keep(cfg.language) if cfg.adapter_dim else None)
@@ -999,6 +1158,8 @@ def load_hf_snapshot(path: str, with_head: bool):
         w = deberta_to_canonical(raw, cfg)
     elif xlmr:
         w = xlmr_to_canonical(raw)
+    elif distil:
+        w = distilbert_to_canonical(raw, cfg)
     else:
         w: Dict[str, np.ndarray] = {}
         for k, v in raw.items():
@@ -1028,17 +1189,18 @@ def load_hf_snapshot(path: str, with_head: bool):
         tc = _read_json(os.path.join(path, "tokenizer_config.json")) or {}
         if tc.get("model_max_length") is not None:
             max_len = min(int(tc["model_max_length"]), max_len)
-    mods = _read_json(os.path.join(path, "modules.json")) or []
-    for m in mods:
-        if m.get("type", "").endswith("Pooling"):
-            pc = _read_json(os.path.join(path, m["path"], "config.json")) or {}
+    mods, dense = read_modules(path, cfg.hidden)
+    w.update(dense)
+    for kind, mdir in mods:
+        if kind == "Pooling":
+            pc = _read_json(os.path.join(path, mdir, "config.json")) or {}
             if pc.get("pooling_mode_cls_token"):
                 pooling = "cls"
             elif pc.get("pooling_mode_mean_tokens", True):
                 pooling = "mean"
             else:
-                raise ValueError("unsupported pooling mode in " + m["path"])
-        if m.get("type", "").endswith("Normalize"):
+                raise ValueError("unsupported pooling mode in " + mdir)
+        if kind == "Normalize":
             normalize = True
     sb = _read_json(os.path.join(path, "sentence_bert_config.json"))
     if sb and sb.get("max_seq_length"):
@@ -1104,14 +1266,17 @@ def _load_qwen3_snapshot(path: str, cfgd: dict, with_head: bool):
     if tc.get("model_max_length") is not None:
         max_len = min(int(tc["model_max_length"]), max_len)
     normalize = False
-    for m in _read_json(os.path.join(path, "modules.json")) or []:
-        if m.get("type", "").endswith("Pooling"):
-            pc = _read_json(os.path.join(path, m["path"], "config.json")) or {}
+    for kind, mdir in module_entries(path):
+        if kind == "Dense":
+            raise ValueError(f"{path}: Dense module {mdir!r} in a Qwen3 snapshot is not supported: Qwen3 encoders "
+                             f"normalise their last-token row themselves and take no projection")
+        if kind == "Pooling":
+            pc = _read_json(os.path.join(path, mdir, "config.json")) or {}
             other = [k for k, v in pc.items() if k.startswith("pooling_mode_") and v and k != "pooling_mode_lasttoken"]
             if not pc.get("pooling_mode_lasttoken") or other:
-                raise ValueError(f"{path}: Qwen3 embedders pool by the last token only; {m['path']} asks for "
+                raise ValueError(f"{path}: Qwen3 embedders pool by the last token only; {mdir} asks for "
                                  f"{other or 'no pooling_mode_lasttoken'}")
-        if m.get("type", "").endswith("Normalize"):
+        if kind == "Normalize":
             normalize = True
     sb = _read_json(os.path.join(path, "sentence_bert_config.json"))
     if sb and sb.get("max_seq_length"):
@@ -1154,9 +1319,10 @@ def resolve_model(model_name: str, with_head: bool, cache_folder: Optional[str] 
         if isinstance(cfg, XmodConfig):
             cfg.language = select_language(cfg.languages, cfg.language, model_name)
         w = synthetic_bert_weights(cfg, seed=seed, with_head=with_head, scale=scale)
+        w.update(synthetic_dense_weights(cfg.hidden, DENSE_PRESETS.get(preset, ()), seed=seed, scale=scale))
         # an XLM-R preset scores as its checkpoint does: one label, no sbert_ce_default_activation_function -> sigmoid
-        act = ("sigmoid" if with_head and isinstance(cfg, (XLMRConfig, DebertaConfig, ModernBertConfig)) and cfg.num_labels == 1
-               else "identity")
+        act = ("sigmoid" if with_head and isinstance(cfg, (XLMRConfig, DebertaConfig, ModernBertConfig, DistilBertConfig))
+               and cfg.num_labels == 1 else "identity")
         return cfg, w, pooling, preset not in UNNORMALIZED_PRESETS, max_len, act, None
     c = find_snapshot(model_name, cache_folder)
     return (*load_hf_snapshot(c, with_head), c)
@@ -1251,6 +1417,9 @@ def load_colbert_snapshot(path: str):
     if kind == "qwen3":
         raise ValueError(f"{path}: a ColBERT checkpoint of model_type 'qwen3' is not supported: Qwen3 runs as a "
                          f"cross-encoder or an embedder")
+    if kind == "distilbert":
+        raise ValueError(f"{path}: a ColBERT checkpoint of model_type 'distilbert' is not supported: DistilBERT runs as a "
+                         f"cross-encoder or an embedder")
     if kind not in ("bert", "xlm-roberta", "roberta", "xmod"):
         raise ValueError(f"{path}: a ColBERT checkpoint of model_type {kind!r} is not supported (bert, xlm-roberta, "
                          f"roberta and xmod are)")
@@ -1324,6 +1493,9 @@ def _refuse_xlmr_flashrank(cfg: BertConfig, where: str) -> None:
                          f"are BERT checkpoints); use HuggingFaceCrossEncoder for it")
     if isinstance(cfg, ModernBertConfig):
         raise ValueError(f"{where}: a ModernBERT (model_type 'modernbert') model is not a FlashRank model (FlashRank's "
+                         f"rerankers are BERT checkpoints); use HuggingFaceCrossEncoder for it")
+    if isinstance(cfg, DistilBertConfig):
+        raise ValueError(f"{where}: a DistilBERT (model_type 'distilbert') model is not a FlashRank model (FlashRank's "
                          f"rerankers are BERT checkpoints); use HuggingFaceCrossEncoder for it")
     if isinstance(cfg, DebertaConfig):
         raise ValueError(f"{where}: a DeBERTa-v2 (model_type 'deberta-v2') model is not a FlashRank model (FlashRank's "
