@@ -475,8 +475,8 @@ int rmu_debug_attention_spans(const uint16_t* qkv_hi, const uint16_t* qkv_lo, in
 int rmu_debug_last_token(const float* x, const int32_t* ids, const int32_t* cu_seqlens, int B, int H, const float* w,
                          float eps, int pad_id, int normalize, const float* head, int num_labels, float* out, void* stream);
 /* For tests: E2 on the QKV planes [T, 3H] of a ragged batch (q | k | v, q pre-scaled by log2(e) / sqrt(d_h) as the
- * QKV epilogue leaves it), cu_seqlens [B+1] int32 -> ctx planes [T, H].  d_h = H / heads is 32 or 64; warps is 10,
- * or 5 with d_h = 32. */
+ * QKV epilogue leaves it), cu_seqlens [B+1] int32 -> ctx planes [T, H].  d_h = H / heads is 32 or 64; warps must be
+ * 10 (160 query rows per CTA), any other value returns RMU_ERR_ARG. */
 int rmu_debug_attention(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu_seqlens, int B, int H,
                         int heads, int max_seqlen, int warps, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream);
 /* For tests: E2 with a key limit per sequence, as rmu_colbert_vectors runs it: nkeys [B] int32 on the device, sequence

@@ -732,7 +732,7 @@ __global__ void join_planes_kernel(const __half* __restrict__ hi, const __half* 
 constexpr int kClsAttWarps = 4;
 
 // E2 on the QKV planes [T, 3H] (q pre-scaled by log2(e) / sqrt(d_h)) of a ragged batch -> ctx planes [T, H].
-// warps = 10 (160-row CTAs), or 5 (80-row CTAs, four per SM) with d_h = 32.
+// warps = 10 (160-row CTAs).
 // cls_q_hi / cls_q_lo non-null: query row 0 of each sequence only, q from those compact planes [B, H] -> ctx [B, H]
 // (the K / V columns of the QKV planes are read as above; their Q columns are not); `warps` is ignored.
 // The sequence index is gridDim.y, at most 65 535: a larger batch runs in slices of 65 535 sequences, each launch with
@@ -752,22 +752,22 @@ static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __
     const int DH = H / heads;
     const bool cls = cls_q_hi != nullptr;
     const bool bias = rel_bias != nullptr;
+    if (cls) warps = kClsAttWarps;
+    else if (warps != kAttWarps) {
+        set_error("attention: warps must be 10");
+        return RMU_ERR_ARG;
+    }
     if (nkeys && (cls || bias)) {
         set_error("attention: a key limit runs on every query row and without a relative bias");
         return RMU_ERR_ARG;
     }
-    if (dis && (bias || nkeys || DH != 64 || (!cls && warps != kAttWarps))) {
-        set_error("attention: the disentangled position terms run with head_dim 64 and 10 warps, without a bias or key limit");
+    if (dis && (bias || nkeys || DH != 64)) {
+        set_error("attention: the disentangled position terms run with head_dim 64, without a bias or key limit");
         return RMU_ERR_ARG;
     }
-    if (window < 0 || (window > 0 && (cls || bias || nkeys || dis || warps != kAttWarps))) {
-        set_error("attention: a sliding window (window > 0) runs in full mode with 10 warps, without a bias, key limit or "
-                  "position terms");
-        return RMU_ERR_ARG;
-    }
-    if (cls) warps = kClsAttWarps;
-    else if (!(warps == kAttWarps || (warps == 5 && DH == 32 && !bias))) {
-        set_error("attention: warps must be 10, or 5 with head_dim 32 and no relative bias");
+    if (window < 0 || (window > 0 && (cls || bias || nkeys || dis))) {
+        set_error("attention: a sliding window (window > 0) runs in full mode, without a bias, key limit or position "
+                  "terms");
         return RMU_ERR_ARG;
     }
     ProfScope _ps(PROF_ATTN, st);
@@ -778,15 +778,13 @@ static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __
     const size_t smem_max = 4 * sizeof(__half) * static_cast<size_t>(kKeySB) * (DH + 8) + tab;
     const size_t smem = 4 * sizeof(__half) * static_cast<size_t>(ksb) * (DH + 8) + tab;
     auto kern = cls ? (DH == 32 ? attention_planes_kernel<32, 4, kClsAttWarps, true> : attention_planes_kernel<64, 2, kClsAttWarps, true>)
-              : DH == 32 ? (warps == 5 ? attention_planes_kernel<32, 4, 5> : attention_planes_kernel<32, 2>)
-                         : attention_planes_kernel<64, 1>;   // d_h = 64 needs > 96 registers
+              : DH == 32 ? attention_planes_kernel<32, 2> : attention_planes_kernel<64, 1>;   // d_h = 64 needs > 96 registers
     using Tab = const float*;
     auto bkern = cls ? (DH == 32 ? attention_planes_kernel<32, 4, kClsAttWarps, true, Tab>
                                  : attention_planes_kernel<64, 2, kClsAttWarps, true, Tab>)
                      : (DH == 32 ? attention_planes_kernel<32, 2, kAttWarps, false, Tab>
                                  : attention_planes_kernel<64, 1, kAttWarps, false, Tab>);
-    auto lkern = DH == 32 ? (warps == 5 ? attention_planes_kernel<32, 4, 5, false, KeyLimit>
-                                        : attention_planes_kernel<32, 2, kAttWarps, false, KeyLimit>)
+    auto lkern = DH == 32 ? attention_planes_kernel<32, 2, kAttWarps, false, KeyLimit>
                           : attention_planes_kernel<64, 1, kAttWarps, false, KeyLimit>;
     auto dkern = cls ? attention_planes_kernel<64, 2, kClsAttWarps, true, Disentangled>
                      : attention_planes_kernel<64, 1, kAttWarps, false, Disentangled>;
@@ -1977,6 +1975,30 @@ struct EncLayer {
     float *qn = nullptr, *kn = nullptr;   // Qwen3: q_norm, k_norm [128]
 };
 
+// A device scratch buffer that only grows.  The caller's lock keeps other users of the buffer out.
+struct DevBuf {
+    void* p = nullptr;
+    size_t cap = 0;                       // bytes
+    template <typename T> T* as() const { return static_cast<T*>(p); }
+    void release() { cudaFree(p); p = nullptr; cap = 0; }
+};
+
+// make b hold at least `need` bytes; when it must grow it allocates max(need, alloc).  The device is synchronised
+// first: work queued on any stream may still read the old allocation.
+static int grow(DevBuf& b, size_t need, size_t alloc = 0) {
+    if (need <= b.cap) return RMU_OK;
+    RMU_CUDA(cudaDeviceSynchronize());
+    b.release();
+    alloc = std::max(need, alloc);
+    RMU_CUDA(cudaMalloc(&b.p, alloc));
+    b.cap = alloc;
+    return RMU_OK;
+}
+
+// rows of the per-token and per-sequence buffers grown for T tokens and B sequences
+static size_t token_rows(int T) { return (std::max(T, 1024) + 127) / 128 * 128; }
+static size_t seq_rows(int B) { return std::max(B + 1, 1024); }
+
 struct rmu_encoder {
     rmu_bert_config cfg{};
     rmu_encoder_ext ext{};                // DeBERTa's fields, zero for every other model
@@ -2006,18 +2028,19 @@ struct rmu_encoder {
     // Llama (rmu_encoder_create_llama) runs as Qwen3 with qn = kn = null (no per-head q / k RMSNorm); the span
     // attention's workspace (launch_attention_spans) and its one-sequence cu_seqlens [0, T], grown under mu
     bool llama = false;
-    float* span_ws = nullptr;
-    size_t span_ws_cap = 0;
+    DevBuf span_ws;
     int* span_cu = nullptr;
     // sentence-transformers Dense modules after pooling (rmu_encoder_set_dense): dense_dims [n + 1], per layer W [out, in],
     // b [out] or null, act; dense_ws holds two [B, max width] ping-pong rows, grown under mu
     std::vector<int> dense_dims;
     std::vector<float*> dense_w, dense_b;
     std::vector<int> dense_act;
-    float* dense_ws = nullptr;
-    size_t dense_ws_cap = 0;
-    // activations
+    DevBuf dense_ws;
+    // activations, in the shape the create path records: QKVP's and CTX's widths, and which optional buffers exist
+    // (X1, the CLS rows, QKVF, POSI)
     int tok_cap = 0, seq_cap = 0;
+    int qkv_w = 0, ctx_w = 0;
+    bool has_x1 = false, has_cls_rows = false, has_qkvf = false, has_posi = false;
     std::vector<void*> act_allocs;
     SplitOperand X, CTX, X1, FF, QKVP;   // QKVP: q (pre-scaled) | k | v as split planes [T, 3H]
     float* PRE = nullptr;                 // fp32 pre-LayerNorm rows: projection + bias + residual
@@ -2030,17 +2053,41 @@ struct rmu_encoder {
     // terms' workspace, grown under mu
     std::vector<int> cidx_h;
     int* cidx = nullptr;
-    float* pos_ws = nullptr;
-    size_t pos_ws_cap = 0;
+    DevBuf pos_ws;
     // staging of the *_host entry points: owned by host_mu alone (NOT part of the activation workspace, which a
     // concurrent device-pointer caller may free and re-allocate under mu)
-    int *d_ids = nullptr, *d_typ = nullptr, *d_cu = nullptr;
-    float* d_out = nullptr;
-    int stage_tok_cap = 0, stage_seq_cap = 0, stage_out_w = 0;
+    DevBuf d_ids, d_typ, d_cu, d_out;
     cudaEvent_t ws_done = nullptr;   // last use of the shared activation workspace (callers on other streams wait on it)
     std::mutex mu;
     std::mutex host_mu;   // the *_host entry points share the staging buffers above: one at a time per handle
 };
+
+// a handle on the current device with cfg and has_head set; null (and `who: no CUDA device`) without a device
+static rmu_encoder* new_handle(const std::string& who, const rmu_bert_config& cfg, int has_head) {
+    rmu_encoder* e = new rmu_encoder();
+    e->cfg = cfg;
+    e->has_head = has_head;
+    if (cudaGetDevice(&e->device) != cudaSuccess || (e->sms = device_sm_count()) <= 0 ||
+        cudaEventCreateWithFlags(&e->ws_done, cudaEventDisableTiming) != cudaSuccess) {
+        set_error(who + ": no CUDA device (this library has no CPU path)");
+        delete e;
+        return nullptr;
+    }
+    return e;
+}
+
+// The GEMM weights travel as split fp16 planes: |w| >= 65520 rounds hi to inf and turns every output it touches into
+// NaN.  Refuses the first of the n floats at p outside that range, on the host, before any CUDA call.
+static int check_split_range(const std::string& who, const std::string& what, const float* p, size_t n) {
+    for (size_t j = 0; j < n; ++j) {
+        if (std::fabs(p[j]) >= 65520.0f) {
+            set_error(who + ": " + what + " weight [" + std::to_string(j) + "] = " + std::to_string(p[j]) +
+                      " is outside the split fp16 planes' range (|w| < 65520)");
+            return RMU_ERR_UNSUPPORTED;
+        }
+    }
+    return RMU_OK;
+}
 
 template <typename T>
 static int dev_alloc(std::vector<void*>& keep, T** p, size_t count) {
@@ -2082,49 +2129,21 @@ static void free_acts(rmu_encoder* e) {
     for (void* p : e->act_allocs) cudaFree(p);
     e->act_allocs.clear();
     e->tok_cap = 0;
-    cudaFree(e->pos_ws);
-    e->pos_ws = nullptr;
-    e->pos_ws_cap = 0;
-    cudaFree(e->span_ws);
-    e->span_ws = nullptr;
-    e->span_ws_cap = 0;
-}
-
-// the span attention's workspace for a sequence of T tokens, grown to fit
-static int ensure_span_ws(rmu_encoder* e, int T) {
-    const size_t need = attention_spans_ws_floats(T, e->cfg.heads);
-    if (need <= e->span_ws_cap) return RMU_OK;
-    RMU_CUDA(cudaDeviceSynchronize());
-    cudaFree(e->span_ws);
-    e->span_ws = nullptr;
-    e->span_ws_cap = 0;
-    RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->span_ws), need * sizeof(float)));
-    e->span_ws_cap = need;
-    return RMU_OK;
+    e->pos_ws.release();
+    e->span_ws.release();
 }
 
 // the width rmu_encoder_embed writes: the last Dense module's out_features, else hidden
 static int embed_width(const rmu_encoder* e) { return e->dense_dims.empty() ? e->cfg.hidden : e->dense_dims.back(); }
 
-static int ensure_dense_ws(rmu_encoder* e, int B) {
-    const size_t need = 2 * static_cast<size_t>(B) * *std::max_element(e->dense_dims.begin(), e->dense_dims.end());
-    if (need <= e->dense_ws_cap) return RMU_OK;
-    RMU_CUDA(cudaDeviceSynchronize());
-    cudaFree(e->dense_ws);
-    e->dense_ws = nullptr;
-    e->dense_ws_cap = 0;
-    RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->dense_ws), need * sizeof(float)));
-    e->dense_ws_cap = need;
-    return RMU_OK;
-}
-
-// mu held: the pooled rows (not normalised) -> the Dense chain -> out [B, embed_width], normalised last when asked
+// mu held: the pooled rows (not normalised) -> the Dense chain -> out [B, embed_width], normalised last when asked.
+// dense_ws holds two [B, max width] ping-pong rows.
 static int run_dense(rmu_encoder* e, const SplitOperand& h, const int* cu, int B, int pool_mode, bool compact, int normalize,
                      float* out, cudaStream_t st) {
-    int rc = ensure_dense_ws(e, B);
+    const size_t half = static_cast<size_t>(B) * *std::max_element(e->dense_dims.begin(), e->dense_dims.end());
+    int rc = grow(e->dense_ws, 2 * half * sizeof(float));
     if (rc != RMU_OK) return rc;
-    const size_t half = e->dense_ws_cap / 2;
-    float* buf[2] = {e->dense_ws, e->dense_ws + half};
+    float* buf[2] = {e->dense_ws.as<float>(), e->dense_ws.as<float>() + half};
     rc = launch_pool(h.hi, h.lo, cu, B, e->cfg.hidden, pool_mode, 0, compact, buf[0], st);
     const int n = static_cast<int>(e->dense_w.size());
     for (int l = 0; l < n && rc == RMU_OK; ++l) {
@@ -2135,28 +2154,20 @@ static int run_dense(rmu_encoder* e, const SplitOperand& h, const int* cu, int B
     return rc;
 }
 
-// DeBERTa: the position terms' workspace for a call (qrows query rows, T keys), grown to fit
+// DeBERTa: grow the position terms' workspace to fit a call (qrows query rows, T keys)
 static int ensure_position_ws(rmu_encoder* e, int qrows, int T, int max_seqlen) {
-    const int rmax = e->cfg.max_pos - 1;
-    const size_t need = position_ws_floats(e->cidx_h.data(), rmax, max_seqlen, qrows, T, e->cfg.heads);
-    if (need <= e->pos_ws_cap) return RMU_OK;
-    RMU_CUDA(cudaDeviceSynchronize());
-    cudaFree(e->pos_ws);
-    e->pos_ws = nullptr;
-    e->pos_ws_cap = 0;
-    RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->pos_ws), need * sizeof(float)));
-    e->pos_ws_cap = need;
-    return RMU_OK;
+    const size_t floats = position_ws_floats(e->cidx_h.data(), e->cfg.max_pos - 1, max_seqlen, qrows, T, e->cfg.heads);
+    return grow(e->pos_ws, floats * sizeof(float));
 }
 
+// the activation workspace for T tokens in B sequences, in the shape the create path recorded on the handle
 static int ensure_tokens(rmu_encoder* e, int T, int B) {
     if (T <= e->tok_cap && B + 1 <= e->seq_cap) return RMU_OK;
     RMU_CUDA(cudaDeviceSynchronize());
     free_acts(e);
     const int H = e->cfg.hidden, F = e->cfg.ffn;
-    int cap = std::max(T, 1024);
-    cap = (cap + 127) / 128 * 128;
-    const int scap = std::max(B + 1, 1024);
+    const int cap = static_cast<int>(token_rows(T)), scap = static_cast<int>(seq_rows(B));
+    // zero-filled: the GEMMs read A rows past a call's T (their outputs are clipped)
     auto planes = [&](SplitOperand* op, int rows, int cols) -> int {
         __half *hi = nullptr, *lo = nullptr;
         int rc = dev_alloc(e->act_allocs, &hi, static_cast<size_t>(rows) * cols);
@@ -2167,23 +2178,26 @@ static int ensure_tokens(rmu_encoder* e, int T, int B) {
         return make_split_operand(op, hi, lo, rows, cols);
     };
     int rc = planes(&e->X, cap, H);
-    if (rc == RMU_OK) rc = planes(&e->CTX, cap, H);
-    if (rc == RMU_OK) rc = planes(&e->X1, cap, H);
+    if (rc == RMU_OK) rc = planes(&e->CTX, cap, e->ctx_w);
+    if (rc == RMU_OK && e->has_x1) rc = planes(&e->X1, cap, H);
     if (rc == RMU_OK) rc = planes(&e->FF, cap, F);
-    if (rc == RMU_OK) rc = planes(&e->QKVP, cap, 3 * H);
+    if (rc == RMU_OK) rc = planes(&e->QKVP, cap, e->qkv_w);
+    if (rc == RMU_OK && e->has_qkvf) rc = dev_alloc(e->act_allocs, &e->QKVF, static_cast<size_t>(cap) * e->qkv_w);
     if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->PRE, static_cast<size_t>(cap) * H);
-    // one row per sequence: B exceeds T when sequences are empty
-    if (rc == RMU_OK) rc = planes(&e->X_cls, scap, H);
-    if (rc == RMU_OK) rc = planes(&e->Q_cls, scap, H);
-    if (rc == RMU_OK) rc = planes(&e->CTX_cls, scap, H);
-    if (rc == RMU_OK) rc = planes(&e->X1_cls, scap, H);
-    if (rc == RMU_OK) rc = planes(&e->FF_cls, scap, F);
-    if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->PRE_cls, static_cast<size_t>(scap) * H);
+    if (e->has_cls_rows) {
+        // one row per sequence: B exceeds T when sequences are empty
+        if (rc == RMU_OK) rc = planes(&e->X_cls, scap, H);
+        if (rc == RMU_OK) rc = planes(&e->Q_cls, scap, H);
+        if (rc == RMU_OK) rc = planes(&e->CTX_cls, scap, H);
+        if (rc == RMU_OK) rc = planes(&e->X1_cls, scap, H);
+        if (rc == RMU_OK) rc = planes(&e->FF_cls, scap, F);
+        if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->PRE_cls, static_cast<size_t>(scap) * H);
+    }
     // the adapter's bottleneck activations reuse the FF planes (adapter_dim <= ffn)
     const int A = e->cfg.adapter_dim;
     if (rc == RMU_OK && A > 0) rc = make_split_operand(&e->FFA, e->FF.hi, e->FF.lo, cap, A);
     if (rc == RMU_OK && A > 0) rc = make_split_operand(&e->FFA_cls, e->FF_cls.hi, e->FF_cls.lo, scap, A);
-    if (rc == RMU_OK && e->modern) rc = dev_alloc(e->act_allocs, &e->POSI, cap);
+    if (rc == RMU_OK && e->has_posi) rc = dev_alloc(e->act_allocs, &e->POSI, cap);
     if (rc != RMU_OK) { free_acts(e); return rc; }
     e->tok_cap = cap;
     e->seq_cap = scap;
@@ -2233,8 +2247,8 @@ static int run_last_layer_cls(rmu_encoder* e, const EncLayer& L, const int32_t* 
         rc = ensure_position_ws(e, B, T, max_seqlen);
         if (rc == RMU_OK)
             rc = run_disentangled_attention(e->QKVP.hi, e->QKVP.lo, e->Q_cls.hi, e->Q_cls.lo, cu, B, T, H, c.heads, max_seqlen,
-                                            L.pos_hi, L.pos_lo, e->cidx, e->cidx_h.data(), c.max_pos - 1, e->pos_ws,
-                                            e->CTX_cls.hi, e->CTX_cls.lo, st);
+                                            L.pos_hi, L.pos_lo, e->cidx, e->cidx_h.data(), c.max_pos - 1,
+                                            e->pos_ws.as<float>(), e->CTX_cls.hi, e->CTX_cls.lo, st);
     } else {
         rc = launch_attention(e->QKVP.hi, e->QKVP.lo, e->Q_cls.hi, e->Q_cls.lo, cu, B, H, c.heads, max_seqlen, 0, e->CTX_cls.hi,
                               e->CTX_cls.lo, st, e->rel);
@@ -2350,18 +2364,15 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
         g.out_hi = e->QKVP.hi; g.out_lo = e->QKVP.lo; g.qcols = H; g.qscale = qscale;
         rc = launch_gemm(GEMM_BIAS_SPLIT_QSCALE, e->X, L.Wqkv, g, e->sms, st);
         if (rc != RMU_OK) return rc;
-        // RMU_ATTN_WARPS = 5: 80-row CTAs, four per SM (same warps/SM, K/V staged twice per 147-token sequence)
-        static const int nw_env = [] { const char* e = getenv("RMU_ATTN_WARPS"); return e ? atoi(e) : kAttWarps; }();
         if (e->ext.position_buckets > 0) {
             rc = ensure_position_ws(e, T, T, max_seqlen);
             if (rc == RMU_OK)
                 rc = run_disentangled_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, T, H, c.heads, max_seqlen,
-                                                L.pos_hi, L.pos_lo, e->cidx, e->cidx_h.data(), c.max_pos - 1, e->pos_ws,
-                                                e->CTX.hi, e->CTX.lo, st);
+                                                L.pos_hi, L.pos_lo, e->cidx, e->cidx_h.data(), c.max_pos - 1,
+                                                e->pos_ws.as<float>(), e->CTX.hi, e->CTX.lo, st);
         } else {
-            rc = launch_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, H, c.heads, max_seqlen,
-                                  (nw_env == 5 && DH == 32 && !e->rel) ? 5 : kAttWarps, e->CTX.hi, e->CTX.lo, st, e->rel,
-                                  nkeys);
+            rc = launch_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, H, c.heads, max_seqlen, kAttWarps, e->CTX.hi,
+                                  e->CTX.lo, st, e->rel, nkeys);
         }
         if (rc != RMU_OK) return rc;
         g = GemmParams{};
@@ -2385,38 +2396,6 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
         rc = launch_layernorm(e->PRE, T, H, L.ln2g, L.ln2b, c.ln_eps, e->X.hi, e->X.lo, st);
         if (rc != RMU_OK) return rc;
     }
-    return RMU_OK;
-}
-
-// Qwen3's activation workspace (grown like ensure_tokens): X [cap, H] and CTX [cap, heads 128] planes (GEMM inputs), FF
-// [cap, F] planes, QKVP [cap, NQKV] planes and QKVF fp32, the residual stream PRE [cap, H] fp32, and POSI
-static int ensure_tokens_qwen3(rmu_encoder* e, int T, int B) {
-    if (T <= e->tok_cap && B + 1 <= e->seq_cap) return RMU_OK;
-    RMU_CUDA(cudaDeviceSynchronize());
-    free_acts(e);
-    const int H = e->cfg.hidden, F = e->cfg.ffn, QD = e->cfg.heads * kQwenHD;
-    const int NQKV = QD + 2 * e->qext.kv_heads * kQwenHD;
-    const int cap = (std::max(T, 1024) + 127) / 128 * 128, scap = std::max(B + 1, 1024);
-    auto planes = [&](SplitOperand* op, int cols) -> int {
-        __half *hi = nullptr, *lo = nullptr;
-        int rc = dev_alloc(e->act_allocs, &hi, static_cast<size_t>(cap) * cols);
-        if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &lo, static_cast<size_t>(cap) * cols);
-        if (rc != RMU_OK) return rc;
-        // zeros, as ensure_tokens: the GEMMs' A rows past a call's T are read (their outputs are clipped)
-        RMU_CUDA(cudaMemset(hi, 0, static_cast<size_t>(cap) * cols * sizeof(__half)));
-        RMU_CUDA(cudaMemset(lo, 0, static_cast<size_t>(cap) * cols * sizeof(__half)));
-        return make_split_operand(op, hi, lo, cap, cols);
-    };
-    int rc = planes(&e->X, H);
-    if (rc == RMU_OK) rc = planes(&e->CTX, QD);
-    if (rc == RMU_OK) rc = planes(&e->FF, F);
-    if (rc == RMU_OK) rc = planes(&e->QKVP, NQKV);
-    if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->QKVF, static_cast<size_t>(cap) * NQKV);
-    if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->PRE, static_cast<size_t>(cap) * H);
-    if (rc == RMU_OK) rc = dev_alloc(e->act_allocs, &e->POSI, cap);
-    if (rc != RMU_OK) { free_acts(e); return rc; }
-    e->tok_cap = cap;
-    e->seq_cap = scap;
     return RMU_OK;
 }
 
@@ -2445,7 +2424,7 @@ static int run_qwen3(rmu_encoder* e, const int32_t* ids, const int32_t* cu, int 
     const rmu_bert_config& c = e->cfg;
     if (max_seqlen > c.max_pos) { set_error("sequence longer than max_position_embeddings"); return RMU_ERR_ARG; }
     const int H = c.hidden, F = c.ffn, nh = c.heads, kv = e->qext.kv_heads, QD = nh * kQwenHD;
-    int rc = ensure_tokens_qwen3(e, T, B);
+    int rc = ensure_tokens(e, T, B);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace is shared by all callers
     RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
@@ -2556,7 +2535,6 @@ int rmu_encoder_create_ex(const rmu_bert_config* cfg, const rmu_encoder_ext* ext
         set_error("rmu_encoder_create: unsupported shape (hidden/ffn multiples of 128, hidden <= 1024, head_dim 32 or 64)");
         return RMU_ERR_UNSUPPORTED;
     }
-    // the GEMM weights travel as fp16 planes: |w| >= 65520 rounds hi to inf and turns every output it touches into NaN
     for (int l = 0; l < L; ++l) {
         static const char* const kName[] = {"query", "key", "value", "attention output", "intermediate", "output"};
         const int slot[] = {0, 2, 4, 6, 10, 12};                  // weight offsets within the layer's 16 tensors
@@ -2564,38 +2542,24 @@ int rmu_encoder_create_ex(const rmu_bert_config* cfg, const rmu_encoder_ext* ext
         for (int k = 0; k < 6; ++k) {
             const float* p = w[5 + 16 * l + slot[k]];
             if (!p) { set_error("rmu_encoder_create: null weight tensor"); return RMU_ERR_ARG; }
-            for (size_t j = 0; j < count[k]; ++j) {
-                if (std::fabs(p[j]) >= 65520.0f) {
-                    set_error("rmu_encoder_create: layer " + std::to_string(l) + " " + kName[k] + " weight [" + std::to_string(j) +
-                              "] = " + std::to_string(p[j]) + " is outside the split fp16 planes' range (|w| < 65520)");
-                    return RMU_ERR_UNSUPPORTED;
-                }
-            }
+            const int rc = check_split_range("rmu_encoder_create", "layer " + std::to_string(l) + " " + kName[k], p, count[k]);
+            if (rc != RMU_OK) return rc;
         }
     }
     for (int l = 0; l < L && A > 0; ++l) {
         for (int k = 0; k < 2; ++k) {                             // dense1 [A, H] and dense2 [H, A]
-            const float* p = w[adapter0 + 4 * l + 2 * k];
-            for (size_t j = 0; j < static_cast<size_t>(A) * H; ++j) {
-                if (std::fabs(p[j]) >= 65520.0f) {
-                    set_error("rmu_encoder_create: layer " + std::to_string(l) + " adapter dense" + std::to_string(k + 1) +
-                              " weight [" + std::to_string(j) + "] = " + std::to_string(p[j]) +
-                              " is outside the split fp16 planes' range (|w| < 65520)");
-                    return RMU_ERR_UNSUPPORTED;
-                }
-            }
+            const int rc = check_split_range("rmu_encoder_create",
+                                             "layer " + std::to_string(l) + " adapter dense" + std::to_string(k + 1),
+                                             w[adapter0 + 4 * l + 2 * k], static_cast<size_t>(A) * H);
+            if (rc != RMU_OK) return rc;
         }
     }
-    rmu_encoder* e = new rmu_encoder();
-    e->cfg = *cfg;
+    rmu_encoder* e = new_handle("rmu_encoder_create", *cfg, has_head);
+    if (!e) return RMU_ERR_CUDA;
     e->ext = ext;
-    e->has_head = has_head;
-    if (cudaGetDevice(&e->device) != cudaSuccess || (e->sms = device_sm_count()) <= 0 ||
-        cudaEventCreateWithFlags(&e->ws_done, cudaEventDisableTiming) != cudaSuccess) {
-        set_error("rmu_encoder_create: no CUDA device (this library has no CPU path)");
-        delete e;
-        return RMU_ERR_CUDA;
-    }
+    e->qkv_w = 3 * H;
+    e->ctx_w = H;
+    e->has_x1 = e->has_cls_rows = true;
     int rc = RMU_OK;
     int i = 0;
     auto up = [&](float** dst, size_t n) { if (rc == RMU_OK) rc = upload(e, dst, w[i], n); ++i; };
@@ -2766,28 +2730,19 @@ int rmu_encoder_create_modernbert(const rmu_bert_config* cfg, const rmu_modernbe
         const int slot[] = {2, 4, 8, 10};
         const size_t count[] = {size_t(3) * H * H, size_t(H) * H, size_t(2) * F * H, size_t(H) * F};
         for (int k = 0; k < 4; ++k) {
-            const float* p = w[3 + 12 * l + slot[k]];
-            for (size_t j = 0; j < count[k]; ++j) {
-                if (std::fabs(p[j]) >= 65520.0f) {
-                    set_error("rmu_encoder_create_modernbert: layer " + std::to_string(l) + " " + kName[k] + " weight [" +
-                              std::to_string(j) + "] = " + std::to_string(p[j]) +
-                              " is outside the split fp16 planes' range (|w| < 65520)");
-                    return RMU_ERR_UNSUPPORTED;
-                }
-            }
+            // Wi as the checkpoint holds it, before geglu_rows reorders it
+            const int rc = check_split_range("rmu_encoder_create_modernbert", "layer " + std::to_string(l) + " " + kName[k],
+                                             w[3 + 12 * l + slot[k]], count[k]);
+            if (rc != RMU_OK) return rc;
         }
     }
-    rmu_encoder* e = new rmu_encoder();
-    e->cfg = *cfg;
-    e->has_head = has_head;
+    rmu_encoder* e = new_handle("rmu_encoder_create_modernbert", *cfg, has_head);
+    if (!e) return RMU_ERR_CUDA;
     e->modern = true;
     e->mb_pool = mb->pooling;
-    if (cudaGetDevice(&e->device) != cudaSuccess || (e->sms = device_sm_count()) <= 0 ||
-        cudaEventCreateWithFlags(&e->ws_done, cudaEventDisableTiming) != cudaSuccess) {
-        set_error("rmu_encoder_create_modernbert: no CUDA device (this library has no CPU path)");
-        delete e;
-        return RMU_ERR_CUDA;
-    }
+    e->qkv_w = 3 * H;
+    e->ctx_w = H;
+    e->has_x1 = e->has_cls_rows = e->has_posi = true;
     int rc = RMU_OK;
     int i = 0;
     auto up = [&](float** dst, size_t n) { if (rc == RMU_OK) rc = upload(e, dst, w[i], n); ++i; };
@@ -2903,29 +2858,19 @@ static int create_decoder(const char* who, bool qk_norm, const rmu_bert_config* 
         const size_t count[] = {size_t(QD) * H, size_t(KD) * H, size_t(KD) * H, size_t(H) * QD, size_t(F) * H,
                                 size_t(F) * H, size_t(H) * F};
         for (int k = 0; k < 7; ++k) {
-            const float* p = w[1 + per * l + slot[k]];
-            for (size_t j = 0; j < count[k]; ++j) {
-                if (std::fabs(p[j]) >= 65520.0f) {
-                    set_error(fn + ": layer " + std::to_string(l) + " " + kName[k] + " weight [" +
-                              std::to_string(j) + "] = " + std::to_string(p[j]) +
-                              " is outside the split fp16 planes' range (|w| < 65520)");
-                    return RMU_ERR_UNSUPPORTED;
-                }
-            }
+            const int rc = check_split_range(fn, "layer " + std::to_string(l) + " " + kName[k], w[1 + per * l + slot[k]],
+                                             count[k]);
+            if (rc != RMU_OK) return rc;
         }
     }
-    rmu_encoder* e = new rmu_encoder();
-    e->cfg = *cfg;
-    e->has_head = has_head;
+    rmu_encoder* e = new_handle(fn, *cfg, has_head);
+    if (!e) return RMU_ERR_CUDA;
     e->qwen = true;
     e->llama = !qk_norm;
     e->qext = *qx;
-    if (cudaGetDevice(&e->device) != cudaSuccess || (e->sms = device_sm_count()) <= 0 ||
-        cudaEventCreateWithFlags(&e->ws_done, cudaEventDisableTiming) != cudaSuccess) {
-        set_error(fn + ": no CUDA device (this library has no CPU path)");
-        delete e;
-        return RMU_ERR_CUDA;
-    }
+    e->qkv_w = NQKV;
+    e->ctx_w = QD;
+    e->has_qkvf = e->has_posi = true;
     int rc = RMU_OK;
     int i = 0;
     auto up = [&](float** dst, size_t n) { if (rc == RMU_OK) rc = upload(e, dst, w[i], n); ++i; };
@@ -2997,8 +2942,7 @@ void rmu_encoder_destroy(rmu_encoder* e) {
     if (!e) return;
     cudaDeviceSynchronize();
     free_acts(e);
-    cudaFree(e->d_ids); cudaFree(e->d_typ); cudaFree(e->d_cu); cudaFree(e->d_out);
-    cudaFree(e->dense_ws);
+    for (DevBuf* b : {&e->span_ws, &e->dense_ws, &e->pos_ws, &e->d_ids, &e->d_typ, &e->d_cu, &e->d_out}) b->release();
     for (void* p : e->allocs) cudaFree(p);
     if (e->ws_done) cudaEventDestroy(e->ws_done);
     delete e;
@@ -3117,10 +3061,10 @@ int rmu_decoder_attention_spans(rmu_encoder* e, const int32_t* ids, int T, const
     RMU_CUDA(cudaMemcpyAsync(e->span_cu, cu_h, sizeof(cu_h), cudaMemcpyHostToDevice, st));
     int rc = run_qwen3(e, ids, e->span_cu, 1, T, T, st, true);
     if (rc == RMU_OK) rc = qwen3_check_range(e, st);
-    if (rc == RMU_OK) rc = ensure_span_ws(e, T);
+    if (rc == RMU_OK) rc = grow(e->span_ws, attention_spans_ws_floats(T, e->cfg.heads) * sizeof(float));
     if (rc == RMU_OK)
-        rc = launch_attention_spans(e->QKVP.hi, e->QKVP.lo, T, e->cfg.heads, e->qext.kv_heads, spans, n_spans, e->span_ws,
-                                    out, st);
+        rc = launch_attention_spans(e->QKVP.hi, e->QKVP.lo, T, e->cfg.heads, e->qext.kv_heads, spans, n_spans,
+                                    e->span_ws.as<float>(), out, st);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
@@ -3129,24 +3073,15 @@ int rmu_decoder_attention_spans(rmu_encoder* e, const int32_t* ids, int T, const
 // host_mu held: the staging buffers belong to the *_host entry points only
 static int stage_batch(rmu_encoder* e, const int32_t* ids_h, const int32_t* typ_h, const int32_t* cu_h, int B, int T,
                        cudaStream_t st) {
-    const int out_w = std::max(embed_width(e), e->cfg.num_labels);
-    if (T > e->stage_tok_cap || B + 1 > e->stage_seq_cap || out_w > e->stage_out_w) {
-        RMU_CUDA(cudaStreamSynchronize(st));              // earlier *_host calls on this stream are complete (they synchronise)
-        cudaFree(e->d_ids); cudaFree(e->d_typ); cudaFree(e->d_cu); cudaFree(e->d_out);
-        e->d_ids = e->d_typ = e->d_cu = nullptr; e->d_out = nullptr;
-        e->stage_tok_cap = e->stage_seq_cap = e->stage_out_w = 0;
-        const int cap = (std::max(T, 1024) + 127) / 128 * 128, scap = std::max(B + 1, 1024);
-        RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->d_ids), static_cast<size_t>(cap) * sizeof(int)));
-        RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->d_typ), static_cast<size_t>(cap) * sizeof(int)));
-        RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->d_cu), static_cast<size_t>(scap) * sizeof(int)));
-        RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->d_out), static_cast<size_t>(scap) * out_w * sizeof(float)));
-        e->stage_tok_cap = cap;
-        e->stage_seq_cap = scap;
-        e->stage_out_w = out_w;
-    }
-    RMU_CUDA(cudaMemcpyAsync(e->d_ids, ids_h, static_cast<size_t>(T) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    if (typ_h) RMU_CUDA(cudaMemcpyAsync(e->d_typ, typ_h, static_cast<size_t>(T) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    RMU_CUDA(cudaMemcpyAsync(e->d_cu, cu_h, static_cast<size_t>(B + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    const size_t i4 = sizeof(int32_t), out_w = std::max(embed_width(e), e->cfg.num_labels);
+    int rc = grow(e->d_ids, T * i4, token_rows(T) * i4);
+    if (rc == RMU_OK) rc = grow(e->d_typ, T * i4, token_rows(T) * i4);
+    if (rc == RMU_OK) rc = grow(e->d_cu, (B + 1) * i4, seq_rows(B) * i4);
+    if (rc == RMU_OK) rc = grow(e->d_out, B * out_w * sizeof(float), seq_rows(B) * out_w * sizeof(float));
+    if (rc != RMU_OK) return rc;
+    RMU_CUDA(cudaMemcpyAsync(e->d_ids.p, ids_h, T * i4, cudaMemcpyHostToDevice, st));
+    if (typ_h) RMU_CUDA(cudaMemcpyAsync(e->d_typ.p, typ_h, T * i4, cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(e->d_cu.p, cu_h, (B + 1) * i4, cudaMemcpyHostToDevice, st));
     return RMU_OK;
 }
 
@@ -3158,9 +3093,10 @@ int rmu_encoder_embed_host(rmu_encoder* e, const int32_t* ids_h, const int32_t* 
     std::lock_guard<std::mutex> hg(e->host_mu);
     rc = stage_batch(e, ids_h, typ_h, cu_h, B, T, st);
     if (rc != RMU_OK) return rc;
-    rc = rmu_encoder_embed(e, e->d_ids, typ_h ? e->d_typ : nullptr, e->d_cu, B, T, max_seqlen, pool_mode, normalize, e->d_out, st);
+    rc = rmu_encoder_embed(e, e->d_ids.as<int32_t>(), typ_h ? e->d_typ.as<int32_t>() : nullptr, e->d_cu.as<int32_t>(), B, T,
+                           max_seqlen, pool_mode, normalize, e->d_out.as<float>(), st);
     if (rc != RMU_OK) return rc;
-    RMU_CUDA(cudaMemcpyAsync(out_h, e->d_out, static_cast<size_t>(B) * embed_width(e) * sizeof(float), cudaMemcpyDeviceToHost, st));
+    RMU_CUDA(cudaMemcpyAsync(out_h, e->d_out.p, static_cast<size_t>(B) * embed_width(e) * sizeof(float), cudaMemcpyDeviceToHost, st));
     RMU_CUDA(cudaStreamSynchronize(st));
     return RMU_OK;
 }
@@ -3173,9 +3109,10 @@ int rmu_encoder_classify_host(rmu_encoder* e, const int32_t* ids_h, const int32_
     std::lock_guard<std::mutex> hg(e->host_mu);
     rc = stage_batch(e, ids_h, typ_h, cu_h, B, T, st);
     if (rc != RMU_OK) return rc;
-    rc = rmu_encoder_classify(e, e->d_ids, typ_h ? e->d_typ : nullptr, e->d_cu, B, T, max_seqlen, e->d_out, st);
+    rc = rmu_encoder_classify(e, e->d_ids.as<int32_t>(), typ_h ? e->d_typ.as<int32_t>() : nullptr, e->d_cu.as<int32_t>(), B, T,
+                              max_seqlen, e->d_out.as<float>(), st);
     if (rc != RMU_OK) return rc;
-    RMU_CUDA(cudaMemcpyAsync(out_h, e->d_out, static_cast<size_t>(B) * e->cfg.num_labels * sizeof(float), cudaMemcpyDeviceToHost, st));
+    RMU_CUDA(cudaMemcpyAsync(out_h, e->d_out.p, static_cast<size_t>(B) * e->cfg.num_labels * sizeof(float), cudaMemcpyDeviceToHost, st));
     RMU_CUDA(cudaStreamSynchronize(st));
     return RMU_OK;
 }
@@ -3222,34 +3159,16 @@ int rmu_encoder_set_dense(rmu_encoder* e, int n_layers, const int32_t* dims, con
 }  // extern "C"
 
 // ---- ColBERT: the encoder without a head, `linear` on the last hidden state, per-token normalisation, MaxSim
-struct DevBuf {
-    void* p = nullptr;
-    size_t cap = 0;
-};
-
 struct rmu_colbert {
     rmu_encoder* enc = nullptr;
     int dim = 0, dpad = 0;                // dpad: dim rounded up to E1's 128-column tile (zero rows of `linear`)
     SplitOperand lin;                     // linear [dpad, H] as split planes (allocations owned by enc)
     float* zero_bias = nullptr;           // [dpad]
-    float* proj = nullptr;                // [proj_cap, dpad] fp32 projections: workspace, used under enc->mu
-    int proj_cap = 0;
+    DevBuf proj;                          // [rows, dpad] fp32 projections: workspace, used under enc->mu
     // staging of rmu_colbert_score_host, owned by host_mu
     DevBuf s_qids, s_qcu, s_qnk, s_dids, s_dcu, s_dkeep, s_qv, s_dv, s_pq, s_pd, s_out;
     std::mutex host_mu;
 };
-
-// grow a staging buffer; the caller holds host_mu and the previous score_host call has synchronised its stream
-static int grow(DevBuf& b, size_t bytes) {
-    if (bytes <= b.cap) return RMU_OK;
-    cudaFree(b.p);
-    b.p = nullptr;
-    b.cap = 0;
-    const size_t cap = std::max<size_t>(bytes + bytes / 2, 4096);
-    RMU_CUDA(cudaMalloc(&b.p, cap));
-    b.cap = cap;
-    return RMU_OK;
-}
 
 // token vectors of a ragged batch -> out [T, dim]: the encoder (keys limited by nkeys when given), E1 mode 0 with
 // `linear` and a zero bias on the last hidden state's split planes -> proj fp32, then C1
@@ -3257,22 +3176,15 @@ static int colbert_vectors(rmu_colbert* cb, const int32_t* ids, const int32_t* c
                            int B, int T, int max_seqlen, float* out, cudaStream_t st) {
     rmu_encoder* e = cb->enc;
     std::lock_guard<std::mutex> g(e->mu);
-    if (T > cb->proj_cap) {
-        RMU_CUDA(cudaDeviceSynchronize());
-        cudaFree(cb->proj);
-        cb->proj = nullptr;
-        cb->proj_cap = 0;
-        const int cap = (std::max(T, 1024) + 127) / 128 * 128;
-        RMU_CUDA(cudaMalloc(reinterpret_cast<void**>(&cb->proj), static_cast<size_t>(cap) * cb->dpad * sizeof(float)));
-        cb->proj_cap = cap;
-    }
-    int rc = run_encoder(e, ids, nullptr, cu, B, T, max_seqlen, false, st, nkeys);
+    const size_t row = cb->dpad * sizeof(float);
+    int rc = grow(cb->proj, T * row, token_rows(T) * row);
+    if (rc == RMU_OK) rc = run_encoder(e, ids, nullptr, cu, B, T, max_seqlen, false, st, nkeys);
     if (rc != RMU_OK) return rc;
     GemmParams g2{};
-    g2.M = T; g2.N = cb->dpad; g2.K = e->cfg.hidden; g2.bias = cb->zero_bias; g2.out_f32 = cb->proj;
+    g2.M = T; g2.N = cb->dpad; g2.K = e->cfg.hidden; g2.bias = cb->zero_bias; g2.out_f32 = cb->proj.as<float>();
     rc = launch_gemm(GEMM_BIAS_F32, e->X, cb->lin, g2, e->sms, st);
     if (rc != RMU_OK) return rc;
-    rc = launch_colbert_normalize(cb->proj, T, cb->dpad, cb->dim, keep, out, st);
+    rc = launch_colbert_normalize(cb->proj.as<float>(), T, cb->dpad, cb->dim, keep, out, st);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
@@ -3296,15 +3208,10 @@ int rmu_colbert_create(const rmu_bert_config* cfg, const float* const* w, int n_
     }
     const int H = cfg->hidden;
     const size_t n = static_cast<size_t>(dim) * H;
-    for (size_t j = 0; j < n; ++j) {
-        if (std::fabs(linear_h[j]) >= 65520.0f) {
-            set_error("rmu_colbert_create: linear weight [" + std::to_string(j) + "] = " + std::to_string(linear_h[j]) +
-                      " is outside the split fp16 planes' range (|w| < 65520)");
-            return RMU_ERR_UNSUPPORTED;
-        }
-    }
+    int rc = check_split_range("rmu_colbert_create", "linear", linear_h, n);
+    if (rc != RMU_OK) return rc;
     rmu_encoder* enc = nullptr;
-    int rc = rmu_encoder_create(cfg, w, n_weights, 0, &enc);
+    rc = rmu_encoder_create(cfg, w, n_weights, 0, &enc);
     if (rc != RMU_OK) return rc;
     rmu_colbert* cb = new rmu_colbert();
     cb->enc = enc;
@@ -3323,10 +3230,9 @@ int rmu_colbert_create(const rmu_bert_config* cfg, const float* const* w, int n_
 void rmu_colbert_destroy(rmu_colbert* cb) {
     if (!cb) return;
     cudaDeviceSynchronize();
-    cudaFree(cb->proj);
-    for (DevBuf* b : {&cb->s_qids, &cb->s_qcu, &cb->s_qnk, &cb->s_dids, &cb->s_dcu, &cb->s_dkeep, &cb->s_qv, &cb->s_dv,
-                      &cb->s_pq, &cb->s_pd, &cb->s_out})
-        cudaFree(b->p);
+    for (DevBuf* b : {&cb->proj, &cb->s_qids, &cb->s_qcu, &cb->s_qnk, &cb->s_dids, &cb->s_dcu, &cb->s_dkeep, &cb->s_qv,
+                      &cb->s_dv, &cb->s_pq, &cb->s_pd, &cb->s_out})
+        b->release();
     rmu_encoder_destroy(cb->enc);
     delete cb;
 }
@@ -3397,7 +3303,7 @@ int rmu_colbert_score_host(rmu_colbert* cb, const int32_t* q_ids_h, const int32_
              {&cb->s_qv, static_cast<size_t>(q_tokens) * dim * sizeof(float)},
              {&cb->s_dv, static_cast<size_t>(d_tokens) * dim * sizeof(float)}, {&cb->s_pq, n_pairs * i4},
              {&cb->s_pd, n_pairs * i4}, {&cb->s_out, n_pairs * sizeof(float)}}) {
-        if (rc == RMU_OK) rc = grow(*buf, bytes);
+        if (rc == RMU_OK) rc = grow(*buf, bytes, std::max<size_t>(bytes + bytes / 2, 4096));
     }
     if (rc != RMU_OK) return rc;
     auto* qids = static_cast<int32_t*>(cb->s_qids.p);

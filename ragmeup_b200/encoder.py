@@ -93,13 +93,10 @@ class BertEncoder:
                 _lib.check(_lib.lib().rmu_encoder_create_modernbert(C.byref(cc), C.byref(mb), ptrs, len(arrs),
                                                                     int(self.with_head), C.byref(self._h)),
                            "rmu_encoder_create_modernbert")
-            elif cfg.position_buckets or cfg.head_act:
+            else:
                 ext = _lib.encoder_ext_c(cfg)
                 _lib.check(_lib.lib().rmu_encoder_create_ex(C.byref(cc), C.byref(ext), ptrs, len(arrs), int(self.with_head),
                                                             C.byref(self._h)), "rmu_encoder_create_ex")
-            else:
-                _lib.check(_lib.lib().rmu_encoder_create(C.byref(cc), ptrs, len(arrs), int(self.with_head),
-                                                         C.byref(self._h)), "rmu_encoder_create")
             dense = dense_layers(weights)
             self.embed_dim = int(dense[-1][0].shape[0]) if dense else cfg.hidden
             if dense:
@@ -135,48 +132,33 @@ class BertEncoder:
             a = torch.from_numpy(np.ascontiguousarray(a))
         return a.to(device=self.device, dtype=dtype, non_blocking=True).contiguous()
 
-    def embed_tokens(self, ids, type_ids, cu_seqlens, max_seqlen: int, pooling: str = "mean", normalize: bool = True):
-        """ragged token batch -> CUDA fp32 [B, embed_dim] sentence embeddings."""
+    def _run_tokens(self, name: str, ids, type_ids, cu_seqlens, max_seqlen: int, width: int, *args, per_token=False):
+        """the ragged batch as CUDA int32 tensors -> the rmu_encoder_<name> entry point -> CUDA fp32 [B, width], or
+        [total_tokens, width] with per_token; ``args`` go between max_seqlen and the output"""
         torch = self.torch
         ids = self._dev(ids, torch.int32)
         typ = None if type_ids is None else self._dev(type_ids, torch.int32)
         cu = self._dev(cu_seqlens, torch.int32)
-        B = cu.numel() - 1
-        out = torch.empty((B, self.embed_dim), dtype=torch.float32, device=self.device)
+        B, T = cu.numel() - 1, ids.numel()
+        out = torch.empty((T if per_token else B, width), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            self._check(_lib.lib().rmu_encoder_embed(self._h, ids.data_ptr(), None if typ is None else typ.data_ptr(),
-                                                    cu.data_ptr(), B, ids.numel(), int(max_seqlen), POOL[pooling],
-                                                    int(bool(normalize)), out.data_ptr(), _lib.stream_ptr()),
-                       "rmu_encoder_embed")
+            self._check(getattr(_lib.lib(), name)(self._h, ids.data_ptr(), None if typ is None else typ.data_ptr(),
+                                                  cu.data_ptr(), B, T, int(max_seqlen), *args, out.data_ptr(),
+                                                  _lib.stream_ptr()), name)
         return out
+
+    def embed_tokens(self, ids, type_ids, cu_seqlens, max_seqlen: int, pooling: str = "mean", normalize: bool = True):
+        """ragged token batch -> CUDA fp32 [B, embed_dim] sentence embeddings."""
+        return self._run_tokens("rmu_encoder_embed", ids, type_ids, cu_seqlens, max_seqlen, self.embed_dim, POOL[pooling],
+                                int(bool(normalize)))
 
     def classify_tokens(self, ids, type_ids, cu_seqlens, max_seqlen: int):
         """ragged (pair) token batch -> CUDA fp32 [B, num_labels] raw logits."""
-        torch = self.torch
-        ids = self._dev(ids, torch.int32)
-        typ = None if type_ids is None else self._dev(type_ids, torch.int32)
-        cu = self._dev(cu_seqlens, torch.int32)
-        B = cu.numel() - 1
-        out = torch.empty((B, self.cfg.num_labels), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            self._check(_lib.lib().rmu_encoder_classify(self._h, ids.data_ptr(), None if typ is None else typ.data_ptr(),
-                                                       cu.data_ptr(), B, ids.numel(), int(max_seqlen), out.data_ptr(),
-                                                       _lib.stream_ptr()), "rmu_encoder_classify")
-        return out
+        return self._run_tokens("rmu_encoder_classify", ids, type_ids, cu_seqlens, max_seqlen, self.cfg.num_labels)
 
     def hidden_tokens(self, ids, type_ids, cu_seqlens, max_seqlen: int):
         """last hidden state, CUDA fp32 [total_tokens, hidden]."""
-        torch = self.torch
-        ids = self._dev(ids, torch.int32)
-        typ = None if type_ids is None else self._dev(type_ids, torch.int32)
-        cu = self._dev(cu_seqlens, torch.int32)
-        B = cu.numel() - 1
-        out = torch.empty((ids.numel(), self.cfg.hidden), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            self._check(_lib.lib().rmu_encoder_hidden(self._h, ids.data_ptr(), None if typ is None else typ.data_ptr(),
-                                                     cu.data_ptr(), B, ids.numel(), int(max_seqlen), out.data_ptr(),
-                                                     _lib.stream_ptr()), "rmu_encoder_hidden")
-        return out
+        return self._run_tokens("rmu_encoder_hidden", ids, type_ids, cu_seqlens, max_seqlen, self.cfg.hidden, per_token=True)
 
     # ------------------------------------------------------------------ host-buffer entry points
     @staticmethod
@@ -191,44 +173,34 @@ class BertEncoder:
             yield s, e
             s = e
 
+    def _run_host(self, name: str, ids: np.ndarray, type_ids: Optional[np.ndarray], cu: np.ndarray, width: int,
+                  *args) -> np.ndarray:
+        """host int32 token batch -> the rmu_encoder_<name> entry point (H2D/D2H inside the C call), in runs of at most
+        max_tokens_per_call tokens -> host fp32 [B, width]; ``args`` go between max_seqlen and the output"""
+        B = len(cu) - 1
+        out = np.empty((B, width), dtype=np.float32)
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        typ = None if type_ids is None else np.ascontiguousarray(type_ids, dtype=np.int32)
+        cu = np.ascontiguousarray(cu, dtype=np.int32)
+        fn = getattr(_lib.lib(), name)
+        with self.torch.cuda.device(self.device):
+            for s, e in self._chunks(cu, self.max_tokens_per_call):
+                t0, t1 = int(cu[s]), int(cu[e])
+                sub_cu = np.ascontiguousarray(cu[s:e + 1] - cu[s], dtype=np.int32)
+                sub_ids = ids[t0:t1]
+                sub_typ = None if typ is None else typ[t0:t1]
+                o = out[s:e]
+                maxlen = int(np.max(np.diff(sub_cu)))
+                self._check(fn(self._h, sub_ids.ctypes.data, None if sub_typ is None else sub_typ.ctypes.data,
+                               sub_cu.ctypes.data, e - s, t1 - t0, maxlen, *args, o.ctypes.data, _lib.stream_ptr()), name)
+        return out
+
     def embed_host(self, ids: np.ndarray, type_ids: Optional[np.ndarray], cu: np.ndarray, pooling: str = "mean",
                    normalize: bool = True) -> np.ndarray:
         """host int32 token batch -> host fp32 [B, embed_dim] (H2D/D2H inside the C call)."""
-        B = len(cu) - 1
-        out = np.empty((B, self.embed_dim), dtype=np.float32)
-        ids = np.ascontiguousarray(ids, dtype=np.int32)
-        typ = None if type_ids is None else np.ascontiguousarray(type_ids, dtype=np.int32)
-        cu = np.ascontiguousarray(cu, dtype=np.int32)
-        with self.torch.cuda.device(self.device):
-            for s, e in self._chunks(cu, self.max_tokens_per_call):
-                t0, t1 = int(cu[s]), int(cu[e])
-                sub_cu = np.ascontiguousarray(cu[s:e + 1] - cu[s], dtype=np.int32)
-                sub_ids = ids[t0:t1]
-                sub_typ = None if typ is None else typ[t0:t1]
-                o = out[s:e]
-                maxlen = int(np.max(np.diff(sub_cu)))
-                self._check(_lib.lib().rmu_encoder_embed_host(
-                    self._h, sub_ids.ctypes.data, None if sub_typ is None else sub_typ.ctypes.data, sub_cu.ctypes.data,
-                    e - s, t1 - t0, maxlen, POOL[pooling], int(bool(normalize)), o.ctypes.data, _lib.stream_ptr()),
-                    "rmu_encoder_embed_host")
-        return out
+        return self._run_host("rmu_encoder_embed_host", ids, type_ids, cu, self.embed_dim, POOL[pooling],
+                              int(bool(normalize)))
 
     def classify_host(self, ids: np.ndarray, type_ids: Optional[np.ndarray], cu: np.ndarray) -> np.ndarray:
         """host int32 pair-token batch -> host fp32 [B, num_labels] raw logits."""
-        B = len(cu) - 1
-        out = np.empty((B, self.cfg.num_labels), dtype=np.float32)
-        ids = np.ascontiguousarray(ids, dtype=np.int32)
-        typ = None if type_ids is None else np.ascontiguousarray(type_ids, dtype=np.int32)
-        cu = np.ascontiguousarray(cu, dtype=np.int32)
-        with self.torch.cuda.device(self.device):
-            for s, e in self._chunks(cu, self.max_tokens_per_call):
-                t0, t1 = int(cu[s]), int(cu[e])
-                sub_cu = np.ascontiguousarray(cu[s:e + 1] - cu[s], dtype=np.int32)
-                sub_ids = ids[t0:t1]
-                sub_typ = None if typ is None else typ[t0:t1]
-                o = out[s:e]
-                maxlen = int(np.max(np.diff(sub_cu)))
-                self._check(_lib.lib().rmu_encoder_classify_host(
-                    self._h, sub_ids.ctypes.data, None if sub_typ is None else sub_typ.ctypes.data, sub_cu.ctypes.data,
-                    e - s, t1 - t0, maxlen, o.ctypes.data, _lib.stream_ptr()), "rmu_encoder_classify_host")
-        return out
+        return self._run_host("rmu_encoder_classify_host", ids, type_ids, cu, self.cfg.num_labels)

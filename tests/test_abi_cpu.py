@@ -78,7 +78,8 @@ def test_kernel_test_entry_points_reject_before_any_cuda_call(built_lib):
     assert attn(H=384, heads=8) == -3                       # d_h = 48
     assert attn(H=384, heads=4) == -3                       # d_h = 96
     assert attn(H=100, heads=3) == -3
-    assert attn(H=768, heads=12, warps=5) == -1             # the 5-warp variant is d_h = 32 only
+    assert attn(H=768, heads=12, warps=5) == -1             # warps must be 10
+    assert attn(H=384, heads=12, warps=5) == -1
     assert attn(warps=7) == -1 and attn(warps=0) == -1
     assert attn(B=0) == -1 and attn(max_seqlen=0) == -1 and attn(cu=None) == -1
 

@@ -182,3 +182,30 @@ def test_oracle_maxsim_skips_dropped_tokens():
     assert float(colbert_ref.colbert_score(Q, D, keep)[0]) == -0.5
     s, _ = colbert_ref.maxsim_fsum(Q.numpy(), [0, 1], D[0].numpy(), [0, 3], keep[0].numpy(), [0], [0])
     assert s[0] == -0.5
+
+
+def test_c_create_refuses_a_linear_weight_the_split_planes_cannot_hold(tiny):
+    """`linear` travels as split fp16 planes like every GEMM weight: rmu_colbert_create refuses |w| >= 65520 on the
+    host, before any CUDA call, naming the tensor and the index"""
+    import ctypes as C
+    from ragmeup_b200 import _lib
+    cfg, w, lin, spec = tiny
+    arrs = [np.ascontiguousarray(w[n], dtype=np.float32) for n, _ in W.weight_names(cfg, False)]
+    ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
+
+    def create(linear):
+        h = C.c_void_p()
+        rc = _lib.lib().rmu_colbert_create(C.byref(_lib.bert_config_c(cfg)), ptrs, len(arrs), linear.ctypes.data, spec.dim,
+                                           C.byref(h))
+        if rc == 0:
+            _lib.lib().rmu_colbert_destroy(h)
+        return rc
+
+    for v in (7e4, -7e4, 65520.0, np.inf):
+        big = lin.copy()
+        big.reshape(-1)[37] = v
+        assert create(big) == -3, v
+        assert "linear weight [37]" in _lib.lib().rmu_last_error().decode()
+    ok = lin.copy()
+    ok.reshape(-1)[37] = 65519.0
+    assert create(ok) in (0, -2)                                       # accepted: without a device the next step fails

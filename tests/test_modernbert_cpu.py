@@ -269,3 +269,34 @@ def test_c_refusals_before_any_cuda_call():
         rel_buckets = 32
     assert _create(WithAdapter(**asdict(cfg)), win) == UNSUP
     assert _create(WithRel(**asdict(cfg)), win) == UNSUP
+
+
+def test_c_refuses_gemm_weights_the_split_planes_cannot_hold():
+    """GEMM weights travel as split fp16 planes: |w| >= 65520 is refused on the host, before any CUDA call, with its
+    index in the checkpoint's layout (Wi's is taken before the GeGLU row blocks reorder it)"""
+    from ragmeup_b200 import _lib
+    cfg = ModernBertConfig(**asdict(PRESETS["tiny-modernbert"][0]))
+    names = [n for n, _ in modernbert_weight_names(cfg, False)]
+    arrs = [np.zeros(shape, np.float32) for _, shape in modernbert_weight_names(cfg, False)]
+    arrs += [np.ascontiguousarray(t, dtype=np.float32) for t in rope_tables(cfg)]
+    ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
+    win = np.ascontiguousarray(cfg.layer_windows, dtype=np.int32)
+    mb = _lib.ModernBertExtC(win.ctypes.data, 1, 0, cfg.max_pos, cfg.head_dim // 2)
+
+    def create():
+        h = C.c_void_p()
+        rc = _lib.lib().rmu_encoder_create_modernbert(C.byref(_lib.bert_config_c(cfg)), C.byref(mb), ptrs, len(arrs), 0,
+                                                      C.byref(h))
+        if rc == 0:
+            _lib.lib().rmu_encoder_destroy(h)
+        return rc
+
+    wi = arrs[names.index("layers.1.mlp.Wi.weight")].reshape(-1)
+    j = cfg.ffn * cfg.hidden + 5                                       # a gate row, which the GeGLU blocks move
+    for v in (7e4, -65520.0, np.inf):
+        wi[j] = v
+        assert create() == -3, v
+        msg = _lib.lib().rmu_last_error().decode()
+        assert "65520" in msg and f"layer 1 mlp Wi weight [{j}]" in msg, msg
+    wi[j] = 65519.0
+    assert create() in (0, -2)                                         # accepted: without a device the next step fails
