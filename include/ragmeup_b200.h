@@ -163,6 +163,35 @@ int rmu_bm25_csr_export(const rmu_bm25_csr* c, int64_t* doc_len, int64_t* post_p
                         int32_t* post_tf, int64_t* vocab_off, char* vocab_bytes);
 int rmu_bm25_csr_free(rmu_bm25_csr* c);
 
+/* ------------------------------------------------------------------ pg_search BM25 (Postgres sparse leg)
+ * Stands behind the reference's PostgresBM25Retriever (server/PostgresBM25Retriever.py, server/RAGHelper.py:445-462):
+ * `content @@@ '<query>' ORDER BY paradedb.score DESC LIMIT k`, tantivy's float32 Bm25Weight.  The index is a list of
+ * immutable segments over consecutive global rows: postings CSR by term (rows within the segment ascending inside a
+ * term, tf >= 1 and a position list per posting, pos_start[e] = sum of the earlier tfs), a fieldnorm id per row, and
+ * one alive bitmap over all global rows (bit r of word r / 32).  The host appends segments and drops trailing ones to
+ * replace them by their merge. */
+typedef struct rmu_pgbm25 rmu_pgbm25;
+int rmu_pgbm25_create(rmu_pgbm25** out);
+int rmu_pgbm25_destroy(rmu_pgbm25* h);
+/* rows [row0, row0 + n_rows) after every row of the existing segments; host arrays, copied to the device */
+int rmu_pgbm25_push_segment(rmu_pgbm25* h, int64_t row0, int64_t n_rows, int64_t n_terms, const int64_t* post_ptr_h,
+                            const int32_t* post_row_h, const int32_t* post_tf_h, const int64_t* pos_start_h,
+                            const int32_t* pos_h, const uint8_t* fnorm_h);
+int rmu_pgbm25_pop_segments(rmu_pgbm25* h, int n);          /* drops the last n segments */
+int rmu_pgbm25_segments(const rmu_pgbm25* h);
+int rmu_pgbm25_set_alive(rmu_pgbm25* h, const uint32_t* words_h, int64_t n_words);
+/* Q queries; clauses of query q are q_ptr[q] .. q_ptr[q+1], clause c has occur c_occur[c] (0 SHOULD, 1 MUST,
+ * 2 MUST_NOT), weight c_weight[c] = (sum of its term idfs) * (1 + K1), and terms ct_term / position offsets ct_off at
+ * c_tptr[c] .. c_tptr[c+1] (1..128; the first drives a phrase, so the host puts the rarest first).  cache[256] is the
+ * document-length part of the denominator per fieldnorm id.  A row matches when it is alive, matches every MUST
+ * clause and no MUST_NOT clause, and (without MUST clauses) at least one SHOULD clause; its score is the float32 sum
+ * of weight * (tf / (tf + cache[fieldnorm])) over its matched MUST / SHOULD clauses in clause order (a phrase's tf is
+ * its number of occurrences).  out_scores [Q, k] float32 and out_rows [Q, k] int64 global rows, score descending,
+ * ties by lower row, -1 padded past the matches.  1 <= k <= 256.  Host buffers; synchronises the stream. */
+int rmu_pgbm25_search_host(rmu_pgbm25* h, int Q, const int32_t* q_ptr_h, const int32_t* c_occur_h, const float* c_weight_h,
+                           const int32_t* c_tptr_h, const int32_t* ct_term_h, const int32_t* ct_off_h, const float* cache_h,
+                           int k, float* out_scores_h, int64_t* out_rows_h, void* stream);
+
 /* ------------------------------------------------------------------ BERT encoder
  * Stands behind HuggingFaceEmbeddings.embed_documents/embed_query (sentence-transformers
  * encode -> BertModel -> Pooling -> Normalize) and HuggingFaceCrossEncoder.score

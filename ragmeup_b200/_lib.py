@@ -98,6 +98,15 @@ SIGNATURES = {
     "rmu_bm25_csr_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]),
     "rmu_bm25_csr_free": (C.c_int, [C.c_void_p]),
+    "rmu_pgbm25_create": (C.c_int, [C.POINTER(C.c_void_p)]),
+    "rmu_pgbm25_destroy": (C.c_int, [C.c_void_p]),
+    "rmu_pgbm25_push_segment": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_pgbm25_pop_segments": (C.c_int, [C.c_void_p, C.c_int]),
+    "rmu_pgbm25_segments": (C.c_int, [C.c_void_p]),
+    "rmu_pgbm25_set_alive": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64]),
+    "rmu_pgbm25_search_host": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_encoder_create": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(C.c_void_p), C.c_int, C.c_int,
                                      C.POINTER(C.c_void_p)]),
     "rmu_encoder_create_ex": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(EncoderExtC), C.POINTER(C.c_void_p), C.c_int,

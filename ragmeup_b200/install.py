@@ -8,6 +8,7 @@
     from langchain_postgres.vectorstores import PGVector                     RAGHelper.py:29
     from langchain_community.cross_encoders import HuggingFaceCrossEncoder   RAGHelper.py:12
     from ScoredCrossEncoderReranker import ScoredCrossEncoderReranker        RAGHelper.py:33
+    from PostgresBM25Retriever import PostgresBM25Retriever                  RAGHelper.py:32
     from langchain.retrievers.document_compressors import FlashrankRerank   RAGHelper.py:11
         (also langchain_community.document_compressors[.flashrank_rerank])
     from langchain_community.retrievers import BM25Retriever                 RAGHelper.py:24
@@ -49,6 +50,7 @@ def build_classes() -> Dict[str, Any]:
     from .cross_encoder import HuggingFaceCrossEncoder
     from .embeddings import HuggingFaceEmbeddings
     from .flashrank import FlashrankRerank
+    from .pg_bm25 import PostgresBM25Retriever
     from .reranker import ScoredCrossEncoderReranker
     from .retrievers import BM25Retriever, ContextualCompressionRetriever, EnsembleRetriever
     from .vectorstore import Milvus, PGVector
@@ -56,7 +58,7 @@ def build_classes() -> Dict[str, Any]:
     out = dict(HuggingFaceEmbeddings=HuggingFaceEmbeddings, HuggingFaceCrossEncoder=HuggingFaceCrossEncoder,
                ScoredCrossEncoderReranker=ScoredCrossEncoderReranker, FlashrankRerank=FlashrankRerank,
                Milvus=Milvus, PGVector=PGVector, BM25Retriever=BM25Retriever, EnsembleRetriever=EnsembleRetriever,
-               ContextualCompressionRetriever=ContextualCompressionRetriever)
+               ContextualCompressionRetriever=ContextualCompressionRetriever, PostgresBM25Retriever=PostgresBM25Retriever)
     try:  # pragma: no cover - LangChain is not present in the build image
         from langchain_core.embeddings import Embeddings
         from langchain_core.vectorstores import VectorStore
@@ -143,6 +145,40 @@ def build_classes() -> Dict[str, Any]:
 
     LCBM25Retriever.__name__ = "BM25Retriever"
     out.update(BM25Retriever=LCBM25Retriever)
+
+    from pydantic import PrivateAttr
+
+    class LCPostgresBM25Retriever(BaseRetriever):  # type: ignore[misc]
+        """pydantic form of pg_bm25.PostgresBM25Retriever (the reference's fields; the GPU index behind them)"""
+        connection_uri: Any = None
+        table_name: str = "sparse_vectors"
+        k: int = 4
+        conn: Any = None
+        cur: Any = None
+        _impl: Any = PrivateAttr(default=None)
+        model_config = ConfigDict(arbitrary_types_allowed=True)
+
+        def __init__(self, **data: Any):
+            super().__init__(**data)
+            self._impl = PostgresBM25Retriever(connection_uri=self.connection_uri, table_name=self.table_name, k=self.k)
+
+        def add_documents(self, documents, ids=None):
+            return self._impl.add_documents(documents, ids)
+
+        def _get_relevant_documents(self, query, *, run_manager=None):
+            from langchain_core.documents import Document as LCDocument
+            self._impl.k = self.k
+            return [LCDocument(page_content=d.page_content, metadata=d.metadata)
+                    for d in self._impl._get_relevant_documents(query)]
+
+        def delete(self, ids):
+            self._impl.delete(ids)
+
+        def close(self):
+            self._impl.close()
+
+    LCPostgresBM25Retriever.__name__ = "PostgresBM25Retriever"
+    out.update(PostgresBM25Retriever=LCPostgresBM25Retriever)
     try:   # LangChain's own fusion / compression retrievers work unchanged over BaseRetriever objects
         from langchain.retrievers import ContextualCompressionRetriever as LCC, EnsembleRetriever as LCE
         out.update(EnsembleRetriever=LCE, ContextualCompressionRetriever=LCC)
@@ -178,6 +214,8 @@ def install() -> Dict[str, Any]:
     except Exception:
         _module("langchain_community.cross_encoders", HuggingFaceCrossEncoder=c["HuggingFaceCrossEncoder"])
     _module("ScoredCrossEncoderReranker", ScoredCrossEncoderReranker=c["ScoredCrossEncoderReranker"])
+    # vector_store=postgres: the BM25 leg (RAGHelper.py:32,445-462) runs on the GPU instead of ParadeDB
+    _module("PostgresBM25Retriever", PostgresBM25Retriever=c["PostgresBM25Retriever"])
     try:
         import langchain_community.retrievers as lcr  # type: ignore  # pragma: no cover
         lcr.BM25Retriever = c["BM25Retriever"]  # pragma: no cover

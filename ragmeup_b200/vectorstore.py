@@ -30,11 +30,9 @@ variable is set, otherwise the collection only lives in GPU memory (said once on
 from __future__ import annotations
 
 import ast
-import atexit
 import glob
 import json
 import os
-import queue
 import re
 import shutil
 import sys
@@ -47,6 +45,7 @@ import numpy as np
 from . import _lib
 from .documents import Document, Runnable
 from .index import FlatIndex, mmr_select
+from .segments import SegmentWriter, atomic_savez
 
 
 _OPEN_STORES: Dict[str, "weakref.WeakSet"] = {}     # storage directory -> live stores writing segments into it
@@ -105,11 +104,9 @@ class B200VectorStore:
         self._lock = threading.RLock()
         self._storage_dir = storage_dir
         self._segments = 0
-        self._sync_writes = os.environ.get("RMU_STORE_SYNC", "0") == "1"
-        self._writer: Optional[threading.Thread] = None
-        self._queue: Optional["queue.Queue"] = None
-        self._writer_error: Optional[BaseException] = None
+        self._segw: Optional[SegmentWriter] = None
         if storage_dir is not None:
+            self._segw = SegmentWriter(self._write_segment)
             key = os.path.abspath(storage_dir)
             for other in list(_OPEN_STORES.get(key, ())):       # another store of this process may still be writing there
                 other.flush()
@@ -188,13 +185,7 @@ class B200VectorStore:
         with self._lock:                                    # default ids, rows and the host tables move together
             pks = [str(self._added + i) for i in range(n)] if ids is None else [str(i) for i in ids]
             self._insert_locked(vectors, texts, metas, pks)
-            if self._storage_dir is not None:
-                seg = self._segments
-                self._segments += 1
-                if self._sync_writes:
-                    self._write_segment(seg, vectors, texts, metas, pks)
-                else:
-                    self._enqueue_segment(seg, vectors, texts, metas, pks)
+            self._persist(vectors, texts, metas, pks)
         return pks
 
     def add_texts(self, texts: Iterable[str], metadatas: Optional[List[dict]] = None, ids: Optional[List[str]] = None,
@@ -238,13 +229,7 @@ class B200VectorStore:
             if not rows:
                 return 0
             self._remove_locked(rows)
-            if self._storage_dir is not None:
-                seg = self._segments
-                self._segments += 1
-                if self._sync_writes:
-                    self._write_segment(seg, None, [], [], [], deleted=rows)
-                else:
-                    self._enqueue_segment(seg, None, [], [], [], deleted=rows)
+            self._persist(None, [], [], [], deleted=rows)
         return len(rows)
 
     def _delete_by_ids(self, ids: Iterable[Any]) -> int:
@@ -267,41 +252,26 @@ class B200VectorStore:
         return DeleteResult(self._delete_rows(lambda r: self._metas[r].get(field, _NO_VALUE) in values))
 
     # ------------------------------------------------------------------ persistence: one segment per add call
-    # Segments are written by one background thread per store, in insertion order: the device->host copy of the vectors,
-    # the JSON table and the file write (together as long as the GPU work of a 1000-document batch) stay off the ingest
-    # loop.  ``flush()`` waits for everything queued so far and re-raises a writer error; it runs at interpreter exit, in
-    # ``save`` and before segments are re-read.  RMU_STORE_SYNC=1 writes inside ``add_*`` instead.
-    def _enqueue_segment(self, seg: int, vectors, texts, metas, pks, deleted: Optional[List[int]] = None,
-                         added: Optional[int] = None) -> None:
-        if self._writer is None:
-            self._queue = queue.Queue(maxsize=8)             # bounds the vectors kept alive for the writer
-            self._writer = threading.Thread(target=self._writer_loop, name="rmu-segment-writer", daemon=True)
-            self._writer.start()
-            atexit.register(self.flush)
-        if self._writer_error is not None:
-            self.flush()
-        self._queue.put((seg, vectors, list(texts), [dict(m) for m in metas], list(pks), deleted, added))
+    # written in order by the store's SegmentWriter (segments.py); ``flush()`` runs in ``save`` and before segments are
+    # re-read
+    @property
+    def _writer(self):
+        """the background writer thread, None until the first asynchronous segment"""
+        return self._segw.thread if self._segw is not None else None
 
-    def _writer_loop(self) -> None:
-        while True:
-            item = self._queue.get()
-            try:
-                if item is not None and self._writer_error is None:
-                    self._write_segment(*item)
-            except BaseException as e:                       # surfaced by the next add / flush
-                self._writer_error = e
-            finally:
-                self._queue.task_done()
-            if item is None:
-                return
+    def _persist(self, vectors, texts, metas, pks, deleted: Optional[List[int]] = None,
+                 added: Optional[int] = None) -> None:
+        """queue the next segment; ``self._lock`` held"""
+        if self._storage_dir is None:
+            return
+        seg = self._segments
+        self._segments += 1
+        self._segw.submit(seg, vectors, list(texts), [dict(m) for m in metas], list(pks), deleted, added)
 
     def flush(self) -> None:
         """Wait until every segment queued so far is on disk."""
-        if self._writer is not None:
-            self._queue.join()
-        if self._writer_error is not None:
-            e, self._writer_error = self._writer_error, None
-            raise RuntimeError(f"segment writer failed: {e!r}") from e
+        if self._segw is not None:
+            self._segw.flush()
 
     def _write_segment(self, seg: int, vectors, texts, metas, pks, deleted: Optional[List[int]] = None,
                        added: Optional[int] = None) -> None:
@@ -318,10 +288,8 @@ class B200VectorStore:
         else:
             vec = vectors if isinstance(vectors, np.ndarray) else vectors.detach().float().cpu().numpy()
             table = np.frombuffer(json.dumps({"pks": pks, "texts": texts, "metas": metas}).encode(), dtype=np.uint8)
-        path = os.path.join(self._storage_dir, f"seg_{seg:08d}.npz")
-        tmp = path + ".tmp.npz"
-        np.savez(tmp, vectors=np.ascontiguousarray(vec, dtype=np.float32), metric=self.metric, table=table)
-        os.replace(tmp, path)                               # a crash never leaves a half-written segment behind
+        atomic_savez(os.path.join(self._storage_dir, f"seg_{seg:08d}.npz"),
+                     vectors=np.ascontiguousarray(vec, dtype=np.float32), metric=self.metric, table=table)
 
     def _load_segments(self) -> None:
         files = sorted(glob.glob(os.path.join(self._storage_dir, "seg_*.npz")))
@@ -479,13 +447,7 @@ class B200VectorStore:
             if added <= self._added:
                 return
             self._added = added
-            if self._storage_dir is not None:
-                seg = self._segments
-                self._segments += 1
-                if self._sync_writes:
-                    self._write_segment(seg, None, [], [], [], added=added)
-                else:
-                    self._enqueue_segment(seg, None, [], [], [], added=added)
+            self._persist(None, [], [], [], added=added)
 
 
 class Milvus(B200VectorStore):
