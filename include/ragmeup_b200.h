@@ -52,7 +52,8 @@ uint64_t rmu_launch_count(void);
 
 /* per-kernel-class device timing (CUDA events on the launching stream; used by bench.py for the
  * roofline objects).  classes: 0 scan, 1 finalize, 2 exact scan, 3 merge, 4 gemm, 5 attention,
- * 6 layernorm, 7 embedding, 8 pool/head, 9 misc, 10 second-pass scan launches (queries whose certificate failed; exit at once when there are none).  rmu_profile_read synchronises the recorded events. */
+ * 6 layernorm, 7 embedding, 8 pool/head, 9 misc, 10 second-pass scan launches (queries whose certificate failed; exit at once when there are none),
+ * 11 decode attention and KV cache writes, 12 LM head (its GEMM is also in 4), 13 sampler.  rmu_profile_read synchronises the recorded events. */
 void rmu_profile_enable(int on);
 void rmu_profile_reset(void);
 int rmu_profile_read(int cls, double* total_ms, int64_t* launches);
@@ -344,6 +345,39 @@ int rmu_encoder_create_llama(const rmu_bert_config* cfg, const rmu_qwen3_ext* ex
  * activation outside the split planes' fp16 range returns RMU_ERR_RANGE and writes nothing.  Synchronises `stream`. */
 int rmu_decoder_attention_spans(rmu_encoder* enc, const int32_t* ids, int T, const int32_t* spans, int n_spans,
                                 double* out, void* stream);
+/* Text generation on a decoder (rmu_encoder_create_qwen3 without a head, or rmu_encoder_create_llama).
+ * rmu_decoder_set_lm_head attaches lm_head W_h [vocab_size, hidden] (host fp32; embed_tokens when the embeddings are
+ * tied) as split fp16 planes.  Refused before any CUDA call: a null handle or W_h, another kind of encoder, a second
+ * call (RMU_ERR_ARG); vocab_size not a multiple of 128 or |w| >= 65520 (RMU_ERR_UNSUPPORTED). */
+int rmu_decoder_set_lm_head(rmu_encoder* enc, const float* W_h);
+/* Token selection, in transformers' order: the repetition penalty (x < 0 ? x * p : x / p) on every id of the prompt and
+ * of the generated tokens; then with do_sample 0 the largest logit (the lowest id among equal ones); with do_sample 1
+ * x / temperature, top-k (every logit >= the k-th largest survives; 1 <= top_k <= 256, and when more than 256 logits
+ * survive through ties at the k-th value, the lowest ids win), top-p over the ascending cumulative softmax (the largest
+ * always stays), and an inverse-CDF draw: the first survivor, largest first, whose cumulative weight exceeds u times
+ * their total, u a Philox4x32-10 uniform keyed by (seed, step) (no parity with torch.multinomial).  Generation stops
+ * after a token in eos_ids[0 .. n_eos) (which is returned), after max_new_tokens, or when prompt and output fill
+ * max_pos positions. */
+#define RMU_MAX_EOS 8
+typedef struct rmu_sampling {
+    int32_t do_sample;
+    float temperature, top_p, repetition_penalty;   /* repetition_penalty 1: none */
+    int32_t top_k;
+    int32_t n_eos;
+    int32_t eos_ids[RMU_MAX_EOS];
+} rmu_sampling;
+/* ids_h [T] host int32 prompt -> out_h [max_new_tokens] host int32 generated ids, *n_out of them; logits_h (host,
+ * nullable) [max_new_tokens, vocab_size] receives each step's logits before the penalty and sampling.  The prefill writes
+ * each layer's rotated k and v into the handle's KV cache (split fp16 planes [kv_heads, T + max_new_tokens, 128] per
+ * layer, grown when a call needs more and kept for the next); each step then runs the layers on one row with
+ * flash-decoding attention over the cache (fixed-order split merge, no atomics), the final norm, the LM head and the
+ * sampler, and synchronises `stream` once to read the token and the fp16 range flag.  Refused before any CUDA call:
+ * null pointers, T < 1, max_new_tokens < 1, T >= max_pos, an id outside [0, vocab_size), no LM head, another kind of
+ * encoder, n_eos outside 0..8, a repetition_penalty <= 0, and when sampling a temperature <= 0 or top_p outside (0, 1]
+ * (RMU_ERR_ARG) or top_k outside 1..256 (RMU_ERR_UNSUPPORTED).  A KV cache that cannot be allocated returns
+ * RMU_ERR_CUDA naming the bytes asked for; an activation outside the split planes' fp16 range RMU_ERR_RANGE. */
+int rmu_decoder_generate(rmu_encoder* enc, const int32_t* ids_h, int T, const rmu_sampling* s, uint64_t seed,
+                         int max_new_tokens, int32_t* out_h, int32_t* n_out, float* logits_h, void* stream);
 void rmu_encoder_destroy(rmu_encoder* enc);
 
 #define RMU_POOL_MEAN 0
@@ -586,6 +620,20 @@ int rmu_debug_cls_head_act(const uint16_t* hi, const uint16_t* lo, const int32_t
  * RMU_ERR_UNSUPPORTED. */
 int rmu_debug_dense(const float* x, int B, int n_in, int n_out, const float* W, const float* b, int act, int normalize,
                     float* y, void* stream);
+/* For tests: decode attention, as rmu_decoder_generate runs it, of one query row q [heads 128] planes (pre-scaled by
+ * log2(e) / sqrt(128)) against rows [0, n) of one layer's cache kv (fp16 planes K hi | K lo | V hi | V lo, each
+ * [kv_heads, cap, 128]) -> ctx planes [heads 128]; query head h reads kv head h / (heads / kv_heads).  ws holds
+ * heads * ceil(n / 64) * 130 floats.  Null pointers, heads or kv_heads < 1, n < 1, cap < n or a smaller ws return
+ * RMU_ERR_ARG, heads % kv_heads != 0 RMU_ERR_UNSUPPORTED, before any CUDA call. */
+int rmu_debug_attention_decode(const uint16_t* q_hi, const uint16_t* q_lo, const uint16_t* kv, int heads, int kv_heads,
+                               int cap, int n, float* ws, int64_t ws_elems, uint16_t* ctx_hi, uint16_t* ctx_lo,
+                               void* stream);
+/* For tests: the sampler of rmu_decoder_generate on logits [V] (device fp32, overwritten with the processed values),
+ * presence [ceil(V / 32)] (device, bit i of word i / 32 = id i is penalised; the chosen id's bit is set) and the
+ * uniform u in [0, 1) -> *token (device int32).  The settings are refused as rmu_decoder_generate refuses them, and a
+ * null pointer, V < 1 or u outside [0, 1) return RMU_ERR_ARG, before any CUDA call. */
+int rmu_debug_sample(float* logits, int V, uint32_t* presence, const rmu_sampling* s, float u, int32_t* token,
+                     void* stream);
 int rmu_debug_split_planes(const float* src, int64_t n, uint16_t* hi, uint16_t* lo, void* stream);
 int rmu_debug_join_planes(const uint16_t* hi, const uint16_t* lo, int64_t n, float* out, void* stream);
 /* For tests: the BM25 select stage alone (bm25_select_kernel rounds, through the launcher rmu_bm25_search uses) on

@@ -41,6 +41,15 @@ class Qwen3ExtC(C.Structure):
                 ("head_form", C.c_int32), ("pad_token_id", C.c_int32)]
 
 
+MAX_EOS = 8
+
+
+class SamplingC(C.Structure):
+    _fields_ = [("do_sample", C.c_int32), ("temperature", C.c_float), ("top_p", C.c_float),
+                ("repetition_penalty", C.c_float), ("top_k", C.c_int32), ("n_eos", C.c_int32),
+                ("eos_ids", C.c_int32 * MAX_EOS)]
+
+
 def bert_config_c(cfg) -> BertConfigC:
     """weights.BertConfig (or a subclass) -> the C struct; adapter_dim is 0 for every family but X-MOD"""
     return BertConfigC(cfg.vocab_size, cfg.hidden, cfg.layers, cfg.heads, cfg.ffn, cfg.max_pos, cfg.type_vocab,
@@ -119,6 +128,9 @@ SIGNATURES = {
                                            C.POINTER(C.c_void_p)]),
     "rmu_decoder_attention_spans": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
                                               C.c_void_p]),
+    "rmu_decoder_set_lm_head": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "rmu_decoder_generate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(SamplingC), C.c_uint64, C.c_int,
+                                       C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]),
     "rmu_encoder_destroy": (None, [C.c_void_p]),
     "rmu_encoder_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_void_p, C.c_void_p]),
@@ -195,6 +207,10 @@ SIGNATURES = {
                                             C.c_void_p, C.c_void_p]),
     "rmu_debug_last_token": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float,
                                        C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "rmu_debug_attention_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                             C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_sample": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(SamplingC), C.c_float, C.c_void_p,
+                                   C.c_void_p]),
     "rmu_debug_split_planes": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_join_planes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "rmu_debug_bm25_select": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

@@ -1960,6 +1960,301 @@ static int launch_attention_spans(const __half* qkv_hi, const __half* qkv_lo, in
     return RMU_OK;
 }
 
+#include "rmu_topk.cuh"
+
+// ---------------------------------------------------------------------------------------------------
+// Decoding (rmu_decoder_generate).  The KV cache holds, per layer, K and V as split fp16 planes [kv_heads, cap, 128]
+// (K hi | K lo | V hi | V lo, each kv_heads cap 128 halves), row p = the token at position p, as the q / k step left
+// its rotated k and its v.  kv_append_kernel copies them out of the QKV planes after each layer's q / k step, so the
+// prefill's own launches are unchanged.  A decode step's attention is flash-decoding: the keys [0, n) of a kv head are
+// cut into splits of kDecChunk keys, one CTA per (kv head, split, group of up to kDecMaxG query heads) computes the
+// partial (max, sum, unnormalised output) of each query head, and attention_decode_combine_kernel merges the splits in
+// split order.  No atomics: the same inputs give the same bits.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kDecChunk = 64;                 // keys per split: short serial walks, many CTAs
+constexpr int kDecThreads = 128;              // thread d owns output dim d in P.V
+constexpr int kDecWarps = kDecThreads / 32;
+constexpr int kDecMaxG = 8;                   // query heads per CTA; larger groups take several CTAs (grid z)
+constexpr int kDecPart = 2 + kQwenHD;         // a split's partial per query head: m, l, o[128]
+
+// rows [0, T) of the planes [T, NH 128] (q | k | v) -> cache rows pos0 + t of K and V: one uint4 (8 halves) per thread
+__global__ void kv_append_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, int T, int heads,
+                                 int kv_heads, int pos0, int cap, __half* __restrict__ kv) {
+    const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const size_t per_tok = static_cast<size_t>(kv_heads) * (kQwenHD / 8);
+    if (i >= static_cast<size_t>(T) * per_tok) return;
+    const int t = static_cast<int>(i / per_tok), r = static_cast<int>(i % per_tok);
+    const int h = r / (kQwenHD / 8), c8 = (r % (kQwenHD / 8)) * 8;
+    const size_t ld = static_cast<size_t>(heads + 2 * kv_heads) * kQwenHD;
+    const size_t ks = static_cast<size_t>(t) * ld + static_cast<size_t>(heads + h) * kQwenHD + c8;
+    const size_t vs = ks + static_cast<size_t>(kv_heads) * kQwenHD;
+    const size_t plane = static_cast<size_t>(kv_heads) * cap * kQwenHD;
+    const size_t d = (static_cast<size_t>(h) * cap + pos0 + t) * kQwenHD + c8;
+    *reinterpret_cast<uint4*>(kv + d) = *reinterpret_cast<const uint4*>(hi + ks);
+    *reinterpret_cast<uint4*>(kv + plane + d) = *reinterpret_cast<const uint4*>(lo + ks);
+    *reinterpret_cast<uint4*>(kv + 2 * plane + d) = *reinterpret_cast<const uint4*>(hi + vs);
+    *reinterpret_cast<uint4*>(kv + 3 * plane + d) = *reinterpret_cast<const uint4*>(lo + vs);
+}
+
+// One split of one kv head for query heads g0 .. g0 + ng of its group.  q [heads, 128] planes, pre-scaled by log2(e) /
+// sqrt(128) as the q / k step leaves it.  Scores: warp w takes keys w, w + 4, ..., lane l holds dims 4l .. 4l + 3 and
+// forms the prefill's three split products qh kh + ql kh + qh kl in one fp32 chain, then a butterfly over the lanes.
+// Softmax per query head in base 2: warp g % 4 takes head g, m = max, p = exp2(s - m), l = sum p (lane-strided, then
+// a butterfly).  P.V: thread d, keys in order, o += p (vh + vl) (vh + vl is the fp32 value the planes hold).
+// part [heads, nsplit, kDecPart] = (m, l, o).
+__global__ void __launch_bounds__(kDecThreads) attention_decode_kernel(const __half* __restrict__ qh,
+                                                                       const __half* __restrict__ ql,
+                                                                       const __half* __restrict__ kv, int heads,
+                                                                       int kv_heads, int cap, int n, int nsplit,
+                                                                       float* __restrict__ part) {
+    __shared__ float sp[kDecMaxG][kDecChunk];
+    __shared__ float sm[kDecMaxG], sl[kDecMaxG];
+    const int G = heads / kv_heads, kvh = blockIdx.x, split = blockIdx.y, g0 = blockIdx.z * kDecMaxG;
+    const int ng = min(kDecMaxG, G - g0);
+    const int j0 = split * kDecChunk, nk = min(kDecChunk, n - j0);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const size_t plane = static_cast<size_t>(kv_heads) * cap * kQwenHD;
+    const size_t kbase = (static_cast<size_t>(kvh) * cap + j0) * kQwenHD;
+    const __half* kh = kv + kbase;
+    const __half* kl = kh + plane;
+    const __half* vh = kh + 2 * plane;
+    const __half* vl = kh + 3 * plane;
+    float qhr[kDecMaxG][4], qlr[kDecMaxG][4];
+#pragma unroll
+    for (int g = 0; g < kDecMaxG; ++g) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { qhr[g][i] = 0.f; qlr[g][i] = 0.f; }
+        if (g < ng) {
+            const size_t o = static_cast<size_t>(kvh * G + g0 + g) * kQwenHD + lane * 4;
+            const uint2 h2 = *reinterpret_cast<const uint2*>(qh + o), l2 = *reinterpret_cast<const uint2*>(ql + o);
+            const __half2* hp = reinterpret_cast<const __half2*>(&h2);
+            const __half2* lp = reinterpret_cast<const __half2*>(&l2);
+            const float2 a = __half22float2(hp[0]), b = __half22float2(hp[1]);
+            const float2 c = __half22float2(lp[0]), d = __half22float2(lp[1]);
+            qhr[g][0] = a.x; qhr[g][1] = a.y; qhr[g][2] = b.x; qhr[g][3] = b.y;
+            qlr[g][0] = c.x; qlr[g][1] = c.y; qlr[g][2] = d.x; qlr[g][3] = d.y;
+        }
+    }
+    for (int j = warp; j < nk; j += kDecWarps) {
+        const uint2 h2 = *reinterpret_cast<const uint2*>(kh + static_cast<size_t>(j) * kQwenHD + lane * 4);
+        const uint2 l2 = *reinterpret_cast<const uint2*>(kl + static_cast<size_t>(j) * kQwenHD + lane * 4);
+        const __half2* hp = reinterpret_cast<const __half2*>(&h2);
+        const __half2* lp = reinterpret_cast<const __half2*>(&l2);
+        const float2 a = __half22float2(hp[0]), b = __half22float2(hp[1]);
+        const float2 c = __half22float2(lp[0]), d = __half22float2(lp[1]);
+        const float khf[4] = {a.x, a.y, b.x, b.y}, klf[4] = {c.x, c.y, d.x, d.y};
+#pragma unroll
+        for (int g = 0; g < kDecMaxG; ++g) {
+            if (g >= ng) break;
+            float s = 0.f;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                s = fmaf(qhr[g][i], khf[i], s);
+                s = fmaf(qlr[g][i], khf[i], s);
+                s = fmaf(qhr[g][i], klf[i], s);
+            }
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            if (lane == 0) sp[g][j] = s;
+        }
+    }
+    __syncthreads();
+    for (int g = warp; g < ng; g += kDecWarps) {
+        float m = -INFINITY;
+        for (int j = lane; j < nk; j += 32) m = fmaxf(m, sp[g][j]);
+        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+        float l = 0.f;
+        for (int j = lane; j < nk; j += 32) { const float p = fast_exp2(sp[g][j] - m); sp[g][j] = p; l += p; }
+        for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
+        if (lane == 0) { sm[g] = m; sl[g] = l; }
+    }
+    __syncthreads();
+    float acc[kDecMaxG];
+#pragma unroll
+    for (int g = 0; g < kDecMaxG; ++g) acc[g] = 0.f;
+#pragma unroll 8
+    for (int j = 0; j < nk; ++j) {
+        const float v = __half2float(vh[static_cast<size_t>(j) * kQwenHD + tid]) +
+                        __half2float(vl[static_cast<size_t>(j) * kQwenHD + tid]);
+#pragma unroll
+        for (int g = 0; g < kDecMaxG; ++g)
+            if (g < ng) acc[g] = fmaf(sp[g][j], v, acc[g]);
+    }
+    for (int g = 0; g < ng; ++g) {
+        float* pp = part + (static_cast<size_t>(kvh * G + g0 + g) * nsplit + split) * kDecPart;
+        if (tid == 0) { pp[0] = sm[g]; pp[1] = sl[g]; }
+        pp[2 + tid] = acc[g];
+    }
+}
+
+// one block per query head: the splits in order, M = max m_s, L = sum l_s exp2(m_s - M), o = sum o_s exp2(m_s - M) / L
+// -> the context planes [heads 128]
+__global__ void __launch_bounds__(kDecThreads) attention_decode_combine_kernel(const float* __restrict__ part, int nsplit,
+                                                                               __half* __restrict__ ctx_hi,
+                                                                               __half* __restrict__ ctx_lo) {
+    const int h = blockIdx.x, d = threadIdx.x;
+    const float* p = part + static_cast<size_t>(h) * nsplit * kDecPart;
+    float M = -INFINITY;
+    for (int s = 0; s < nsplit; ++s) M = fmaxf(M, p[static_cast<size_t>(s) * kDecPart]);
+    float L = 0.f, O = 0.f;
+    for (int s = 0; s < nsplit; ++s) {
+        const float* q = p + static_cast<size_t>(s) * kDecPart;
+        const float c = fast_exp2(q[0] - M);
+        L = fmaf(q[1], c, L);
+        O = fmaf(q[2 + d], c, O);
+    }
+    __half hv, lv;
+    split_f16(O / L, hv, lv);
+    ctx_hi[static_cast<size_t>(h) * kQwenHD + d] = hv;
+    ctx_lo[static_cast<size_t>(h) * kQwenHD + d] = lv;
+}
+
+static int decode_splits(int n) { return (n + kDecChunk - 1) / kDecChunk; }
+
+// the partial buffer of launch_attention_decode, in floats
+static size_t decode_part_floats(int heads, int n) { return static_cast<size_t>(heads) * decode_splits(n) * kDecPart; }
+
+static int launch_kv_append(const __half* hi, const __half* lo, int T, int heads, int kv_heads, int pos0, int cap,
+                            __half* kv, cudaStream_t st) {
+    const size_t n = static_cast<size_t>(T) * kv_heads * (kQwenHD / 8);
+    ProfScope _ps(PROF_DECODE_ATTN, st);
+    kv_append_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(hi, lo, T, heads, kv_heads, pos0, cap, kv);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// one query row q [heads 128] against cache rows [0, n) of one layer's kv -> ctx [heads 128]
+static int launch_attention_decode(const __half* q_hi, const __half* q_lo, const __half* kv, int heads, int kv_heads,
+                                   int cap, int n, float* part, __half* ctx_hi, __half* ctx_lo, cudaStream_t st) {
+    const int G = heads / kv_heads, ns = decode_splits(n);
+    ProfScope _ps(PROF_DECODE_ATTN, st);
+    const dim3 grid(static_cast<unsigned>(kv_heads), static_cast<unsigned>(ns),
+                    static_cast<unsigned>((G + kDecMaxG - 1) / kDecMaxG));
+    attention_decode_kernel<<<grid, kDecThreads, 0, st>>>(q_hi, q_lo, kv, heads, kv_heads, cap, n, ns, part);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    attention_decode_combine_kernel<<<static_cast<unsigned>(heads), kDecThreads, 0, st>>>(part, ns, ctx_hi, ctx_lo);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+__global__ void set_int_kernel(int* p, int v) { *p = v; }
+
+// ---------------------------------------------------------------------------------------------------
+// Token selection over fp32 logits [V] (one CTA), in transformers' order:
+//   repetition penalty: x = bit(i) ? (x < 0 ? x p : x / p) : x for the ids whose presence bit is set;
+//   greedy (do_sample 0): the largest x, the lowest index among equal ones;
+//   sampling: x / temperature; top-k keeps every x >= the k-th largest (ties included, but at most kSampleCap
+//   candidates: among ties at the k-th value the lowest indices win); top-p over the candidates sorted ascending,
+//   dropping those whose cumulative softmax is <= 1 - top_p (the largest always stays); then the inverse CDF: the
+//   first candidate, largest first, whose cumulative weight exceeds u times the kept total.
+// The candidates are the index's top-k tail (rmu_topk.cuh): keys (score desc, index asc), a radix select of the k-th
+// and of the kSampleCap-th key, the keys above the higher of the two, a bitonic sort.  Weights exp(x - max) are float64,
+// summed in a fixed order by one thread.  u is u_in when u_in >= 0, else the Philox4x32-10 uniform of (seed, step).
+// The chosen id is written to *token and its presence bit set.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kSampleThreads = 1024;
+constexpr int kSampleCap = 256;               // the largest top_k and the most candidates
+
+struct SampleArgs {
+    int do_sample, top_k;
+    float temperature, top_p, penalty;
+};
+
+// Philox4x32-10 (Salmon et al., SC'11) with counter (step, 0) and key seed: the first output word's high 24 bits / 2^24
+__host__ __device__ inline float philox_uniform(unsigned long long seed, unsigned long long step) {
+    uint32_t c0 = static_cast<uint32_t>(step), c1 = static_cast<uint32_t>(step >> 32), c2 = 0u, c3 = 0u;
+    uint32_t k0 = static_cast<uint32_t>(seed), k1 = static_cast<uint32_t>(seed >> 32);
+    for (int r = 0; r < 10; ++r) {
+        const unsigned long long p0 = 0xD2511F53ull * c0, p1 = 0xCD9E8D57ull * c2;
+        const uint32_t hi0 = static_cast<uint32_t>(p0 >> 32), lo0 = static_cast<uint32_t>(p0);
+        const uint32_t hi1 = static_cast<uint32_t>(p1 >> 32), lo1 = static_cast<uint32_t>(p1);
+        c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+    }
+    return static_cast<float>(c0 >> 8) * (1.0f / 16777216.0f);
+}
+
+__global__ void __launch_bounds__(kSampleThreads) sample_kernel(float* __restrict__ logits, int V,
+                                                                unsigned* __restrict__ presence, SampleArgs a, float u_in,
+                                                                unsigned long long seed, unsigned long long step,
+                                                                int* __restrict__ token) {
+    __shared__ unsigned long long sel[kSel2Max];
+    __shared__ int hist[256];
+    __shared__ unsigned long long s_prefix, s_best[kSampleThreads / 32];
+    __shared__ int s_remaining, s_ties, s_cnt;
+    __shared__ double w[kSampleCap];
+    const int tid = threadIdx.x;
+    unsigned long long best = 0ull;
+    for (int i = tid; i < V; i += blockDim.x) {
+        float x = logits[i];
+        if ((presence[i >> 5] >> (i & 31)) & 1u) x = x < 0.f ? x * a.penalty : __fdiv_rn(x, a.penalty);
+        if (a.do_sample) x = __fdiv_rn(x, a.temperature);
+        logits[i] = x;
+        const unsigned long long k = make_key(x, static_cast<uint32_t>(i));
+        best = k > best ? k : best;
+    }
+    if (!a.do_sample) {
+        for (int o = 16; o > 0; o >>= 1) { const unsigned long long b = __shfl_xor_sync(0xffffffffu, best, o); best = b > best ? b : best; }
+        if ((tid & 31) == 0) s_best[tid >> 5] = best;
+        __syncthreads();
+        if (tid == 0) {
+            for (int i = 1; i < static_cast<int>(blockDim.x >> 5); ++i) best = s_best[i] > best ? s_best[i] : best;
+            const int id = static_cast<int>(key_row(best));
+            *token = id;
+            presence[id >> 5] |= 1u << (id & 31);
+        }
+        return;
+    }
+    __syncthreads();                                            // the tempered logits are visible to the block
+    auto load_key = [&](long long i) -> unsigned long long { return make_key(logits[i], static_cast<uint32_t>(i)); };
+    const unsigned long long tk = block_radix_select(load_key, V, a.top_k, hist, &s_prefix, &s_remaining, &s_ties);
+    __syncthreads();
+    const unsigned long long tc = block_radix_select(load_key, V, kSampleCap, hist, &s_prefix, &s_remaining, &s_ties);
+    // every key whose score equals the k-th one's is >= (that score, low word 0)
+    const unsigned long long tks = tk == 1ull ? 1ull : (tk & 0xFFFFFFFF00000000ull);
+    const unsigned long long T = tks > tc ? tks : tc;
+    const int n = min(block_collect(load_key, V, T, sel, &s_cnt), kSampleCap);
+    block_sort_desc(sel, n);
+    const double m = static_cast<double>(key_score(sel[0]));
+    for (int r = tid; r < n; r += blockDim.x) w[r] = exp(static_cast<double>(key_score(sel[r])) - m);
+    __syncthreads();
+    if (tid == 0) {
+        double total = 0.0;
+        for (int r = 0; r < n; ++r) total += w[r];
+        // ascending cumulative softmax of candidate r = the sum over r..n-1; kept: r < nkeep
+        int nkeep = n;
+        double suf = 0.0;
+        for (int r = n - 1; r > 0; --r) {
+            suf += w[r];
+            if (suf / total <= 1.0 - static_cast<double>(a.top_p)) nkeep = r; else break;
+        }
+        double kept = 0.0;
+        for (int r = 0; r < nkeep; ++r) kept += w[r];
+        const double u = u_in >= 0.f ? static_cast<double>(u_in) : static_cast<double>(philox_uniform(seed, step));
+        const double target = u * kept;
+        int pick = nkeep - 1;
+        double cum = 0.0;
+        for (int r = 0; r < nkeep; ++r) {
+            cum += w[r];
+            if (target < cum) { pick = r; break; }
+        }
+        const int id = static_cast<int>(key_row(sel[pick]));
+        *token = id;
+        presence[id >> 5] |= 1u << (id & 31);
+    }
+}
+
+static int launch_sample(float* logits, int V, unsigned* presence, const SampleArgs& a, float u_in, unsigned long long seed,
+                         unsigned long long step, int* token, cudaStream_t st) {
+    ProfScope _ps(PROF_SAMPLE, st);
+    sample_kernel<<<1, kSampleThreads, 0, st>>>(logits, V, presence, a, u_in, seed, step, token);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
 }  // namespace rmu
 
 using namespace rmu;
@@ -2030,6 +2325,14 @@ struct rmu_encoder {
     bool llama = false;
     DevBuf span_ws;
     int* span_cu = nullptr;
+    // generation (rmu_decoder_set_lm_head, rmu_decoder_generate): the LM head [V, H] as split planes and a zero bias [V];
+    // the KV cache (layers x K hi | K lo | V hi | V lo [kv_heads, kv_cap, 128]); gen_ws = logits [V] | presence bits |
+    // the step's token | decode attention's partials.  Grown under mu.
+    SplitOperand lm_head;
+    bool has_lm_head = false;
+    float* lm_zero = nullptr;
+    DevBuf kv_cache, gen_ws;
+    int kv_cap = 0;
     // sentence-transformers Dense modules after pooling (rmu_encoder_set_dense): dense_dims [n + 1], per layer W [out, in],
     // b [out] or null, act; dense_ws holds two [B, max width] ping-pong rows, grown under mu
     std::vector<int> dense_dims;
@@ -2414,16 +2717,40 @@ static int qwen3_attention_inputs(rmu_encoder* e, const EncLayer& L, int T, cuda
                                c.max_pos, e->QKVP.hi, e->QKVP.lo, e->range_flag, st);
 }
 
+// one decoder layer after its attention, on M rows: h += CTX Wo^T (in place); X = split(w_post RMS(h)); FF =
+// split(silu(X Wgate^T) * (X Wup^T)); h += FF Wdown^T
+static int qwen3_layer_tail(rmu_encoder* e, const EncLayer& L, int M, cudaStream_t st) {
+    const rmu_bert_config& c = e->cfg;
+    const int H = c.hidden, F = c.ffn, QD = c.heads * kQwenHD;
+    GemmParams g{};
+    g.M = M; g.N = H; g.K = QD; g.bias = e->zeros; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
+    int rc = launch_gemm(GEMM_BIAS_RESF32_F32, e->CTX, L.Wo, g, e->sms, st);
+    if (rc == RMU_OK) rc = launch_rms_split(e->PRE, M, H, L.ln2g, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
+    if (rc != RMU_OK) return rc;
+    g = GemmParams{};
+    g.M = M; g.N = 2 * F; g.K = H; g.bias = e->zeros; g.out_hi = e->FF.hi; g.out_lo = e->FF.lo; g.range_flag = e->range_flag;
+    rc = launch_gemm(GEMM_BIAS_SWIGLU_SPLIT, e->X, L.W1, g, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    g = GemmParams{};
+    g.M = M; g.N = H; g.K = F; g.bias = e->zeros; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
+    return launch_gemm(GEMM_BIAS_RESF32_F32, e->FF, L.W2, g, e->sms, st);
+}
+
+// layer l's K / V planes in the KV cache (kv_append_kernel's layout)
+static __half* kv_layer(rmu_encoder* e, int l) {
+    return e->kv_cache.as<__half>() + static_cast<size_t>(l) * 4 * e->qext.kv_heads * e->kv_cap * kQwenHD;
+}
+
 // Qwen3's layers (the header's formula): leaves the residual stream h, before the final norm, in e->PRE [T, H] fp32.
-// Per layer: the attention inputs (above); CTX = causal GQA attention; h += CTX Wo^T (in place); X = split(w_post
-// RMS(h)); FF = split(silu(X Wgate^T) * (X Wup^T)); h += FF Wdown^T.  With attn_last (the span attention), the last
-// layer stops at its attention inputs, which QKVP then holds.
+// Per layer: the attention inputs (above); CTX = causal GQA attention; then qwen3_layer_tail.  With attn_last (the span
+// attention), the last layer stops at its attention inputs, which QKVP then holds.  With to_cache (one sequence, the
+// prefill of rmu_decoder_generate), each layer's k and v rows also go to the KV cache at positions 0 .. T - 1.
 // The range flag is cleared first; the caller reads it (qwen3_check_range) before it writes an output.
 static int run_qwen3(rmu_encoder* e, const int32_t* ids, const int32_t* cu, int B, int T, int max_seqlen, cudaStream_t st,
-                     bool attn_last = false) {
+                     bool attn_last = false, bool to_cache = false) {
     const rmu_bert_config& c = e->cfg;
     if (max_seqlen > c.max_pos) { set_error("sequence longer than max_position_embeddings"); return RMU_ERR_ARG; }
-    const int H = c.hidden, F = c.ffn, nh = c.heads, kv = e->qext.kv_heads, QD = nh * kQwenHD;
+    const int H = c.hidden, nh = c.heads, kv = e->qext.kv_heads;
     int rc = ensure_tokens(e, T, B);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace is shared by all callers
@@ -2435,20 +2762,10 @@ static int run_qwen3(rmu_encoder* e, const int32_t* ids, const int32_t* cu, int 
         const EncLayer& L = e->layers[l];
         rc = qwen3_attention_inputs(e, L, T, st);
         if (rc != RMU_OK || (attn_last && l == c.layers - 1)) return rc;
-        rc = launch_attention_causal(e->QKVP.hi, e->QKVP.lo, cu, B, nh, kv, max_seqlen, e->CTX.hi, e->CTX.lo, st);
-        if (rc != RMU_OK) return rc;
-        GemmParams g{};
-        g.M = T; g.N = H; g.K = QD; g.bias = e->zeros; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
-        rc = launch_gemm(GEMM_BIAS_RESF32_F32, e->CTX, L.Wo, g, e->sms, st);
-        if (rc == RMU_OK) rc = launch_rms_split(e->PRE, T, H, L.ln2g, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
-        if (rc != RMU_OK) return rc;
-        g = GemmParams{};
-        g.M = T; g.N = 2 * F; g.K = H; g.bias = e->zeros; g.out_hi = e->FF.hi; g.out_lo = e->FF.lo; g.range_flag = e->range_flag;
-        rc = launch_gemm(GEMM_BIAS_SWIGLU_SPLIT, e->X, L.W1, g, e->sms, st);
-        if (rc != RMU_OK) return rc;
-        g = GemmParams{};
-        g.M = T; g.N = H; g.K = F; g.bias = e->zeros; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
-        rc = launch_gemm(GEMM_BIAS_RESF32_F32, e->FF, L.W2, g, e->sms, st);
+        if (to_cache) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, T, nh, kv, 0, e->kv_cap, kv_layer(e, l), st);
+        if (rc == RMU_OK)
+            rc = launch_attention_causal(e->QKVP.hi, e->QKVP.lo, cu, B, nh, kv, max_seqlen, e->CTX.hi, e->CTX.lo, st);
+        if (rc == RMU_OK) rc = qwen3_layer_tail(e, L, T, st);
         if (rc != RMU_OK) return rc;
     }
     return RMU_OK;
@@ -2463,6 +2780,25 @@ static int qwen3_check_range(rmu_encoder* e, cudaStream_t st) {
         set_error(std::string(e->llama ? "Llama" : "Qwen3") + " forward: an activation entering a GEMM or attention left the fp16 range of the split planes "
                   "(|x| > 65504); the encoder cannot compute this model's activations for this input");
         return RMU_ERR_RANGE;
+    }
+    return RMU_OK;
+}
+
+// the sampling settings rmu_decoder_generate and rmu_debug_sample refuse, before any CUDA call
+static int check_sampling(const std::string& fn, const rmu_sampling* s) {
+    if (s->n_eos < 0 || s->n_eos > RMU_MAX_EOS || !(s->repetition_penalty > 0.f) || !std::isfinite(s->repetition_penalty)) {
+        set_error(fn + ": n_eos must be 0 .. 8 and repetition_penalty a positive finite number");
+        return RMU_ERR_ARG;
+    }
+    if (s->do_sample) {
+        if (s->top_k < 1 || s->top_k > kSampleCap) {
+            set_error(fn + ": top_k must be 1 .. 256 when sampling, got " + std::to_string(s->top_k));
+            return RMU_ERR_UNSUPPORTED;
+        }
+        if (!(s->temperature > 0.f) || !std::isfinite(s->temperature) || !(s->top_p > 0.f && s->top_p <= 1.f)) {
+            set_error(fn + ": temperature must be positive and finite and top_p in (0, 1] when sampling");
+            return RMU_ERR_ARG;
+        }
     }
     return RMU_OK;
 }
@@ -2942,7 +3278,8 @@ void rmu_encoder_destroy(rmu_encoder* e) {
     if (!e) return;
     cudaDeviceSynchronize();
     free_acts(e);
-    for (DevBuf* b : {&e->span_ws, &e->dense_ws, &e->pos_ws, &e->d_ids, &e->d_typ, &e->d_cu, &e->d_out}) b->release();
+    for (DevBuf* b : {&e->span_ws, &e->dense_ws, &e->pos_ws, &e->d_ids, &e->d_typ, &e->d_cu, &e->d_out, &e->kv_cache, &e->gen_ws})
+        b->release();
     for (void* p : e->allocs) cudaFree(p);
     if (e->ws_done) cudaEventDestroy(e->ws_done);
     delete e;
@@ -3153,6 +3490,142 @@ int rmu_encoder_set_dense(rmu_encoder* e, int n_layers, const int32_t* dims, con
     e->dense_w = w;
     e->dense_b = b;
     e->dense_act.assign(acts, acts + n_layers);
+    return RMU_OK;
+}
+
+int rmu_decoder_set_lm_head(rmu_encoder* e, const float* W_h) {
+    if (!e || !W_h) { set_error("rmu_decoder_set_lm_head: bad argument"); return RMU_ERR_ARG; }
+    if (!e->qwen || e->has_head) {
+        set_error("rmu_decoder_set_lm_head: the encoder must come from rmu_encoder_create_qwen3 without a head or from "
+                  "rmu_encoder_create_llama");
+        return RMU_ERR_ARG;
+    }
+    const int V = e->cfg.vocab_size, H = e->cfg.hidden;
+    if (V % 128 != 0) {
+        set_error("rmu_decoder_set_lm_head: vocab_size must be a multiple of 128 (the LM head GEMM's tile), got " +
+                  std::to_string(V));
+        return RMU_ERR_UNSUPPORTED;
+    }
+    std::lock_guard<std::mutex> hg(e->host_mu);
+    std::lock_guard<std::mutex> g(e->mu);
+    if (e->has_lm_head) { set_error("rmu_decoder_set_lm_head: an LM head is already attached"); return RMU_ERR_ARG; }
+    int rc = check_split_range("rmu_decoder_set_lm_head", "lm_head", W_h, static_cast<size_t>(V) * H);
+    if (rc != RMU_OK) return rc;
+    rc = upload_split(e, &e->lm_head, {W_h}, V, H);
+    if (rc == RMU_OK) {
+        const std::vector<float> zeros(static_cast<size_t>(V), 0.f);
+        rc = upload(e, &e->lm_zero, zeros.data(), zeros.size());
+    }
+    if (rc != RMU_OK) return rc;
+    e->has_lm_head = true;
+    return RMU_OK;
+}
+
+int rmu_decoder_generate(rmu_encoder* e, const int32_t* ids_h, int T, const rmu_sampling* s, uint64_t seed,
+                         int max_new_tokens, int32_t* out_h, int32_t* n_out, float* logits_h, void* stream) {
+    const std::string fn("rmu_decoder_generate");
+    if (!e || !ids_h || !s || !out_h || !n_out || T < 1 || max_new_tokens < 1) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
+    if (!e->qwen || e->has_head || !e->has_lm_head) {
+        set_error(fn + ": the encoder must be a decoder (rmu_encoder_create_qwen3 without a head, or rmu_encoder_create_llama) "
+                  "with an LM head attached by rmu_decoder_set_lm_head");
+        return RMU_ERR_ARG;
+    }
+    const rmu_bert_config& c = e->cfg;
+    if (T >= c.max_pos) {
+        set_error(fn + ": a prompt of " + std::to_string(T) + " tokens leaves no position for a new token (max_position_embeddings " +
+                  std::to_string(c.max_pos) + ")");
+        return RMU_ERR_ARG;
+    }
+    int rc = check_sampling(fn, s);
+    if (rc != RMU_OK) return rc;
+    for (int i = 0; i < T; ++i)
+        if (ids_h[i] < 0 || ids_h[i] >= c.vocab_size) { set_error(fn + ": token id out of range"); return RMU_ERR_ARG; }
+    std::lock_guard<std::mutex> hg(e->host_mu);
+    std::lock_guard<std::mutex> g(e->mu);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int V = c.vocab_size, H = c.hidden, nh = c.heads, kv = e->qext.kv_heads, L = c.layers;
+    const int cap = std::min(T + max_new_tokens, c.max_pos);
+    // the KV cache: grown (device synchronised first, as grow does) when a call needs more positions
+    if (cap > e->kv_cap) {
+        const size_t bytes = static_cast<size_t>(L) * 4 * kv * cap * kQwenHD * sizeof(__half);
+        RMU_CUDA(cudaDeviceSynchronize());
+        e->kv_cache.release();
+        e->kv_cap = 0;
+        if (cudaMalloc(&e->kv_cache.p, bytes) != cudaSuccess) {
+            cudaGetLastError();
+            e->kv_cache.p = nullptr;
+            set_error(fn + ": cannot allocate the KV cache: " + std::to_string(bytes) + " bytes for " + std::to_string(cap) +
+                      " positions");
+            return RMU_ERR_CUDA;
+        }
+        e->kv_cache.cap = bytes;
+        e->kv_cap = cap;
+    }
+    const size_t words = (static_cast<size_t>(V) + 31) / 32;
+    const size_t ws = (static_cast<size_t>(V) + words + 4 + decode_part_floats(nh, cap)) * sizeof(float);
+    rc = grow(e->gen_ws, ws);
+    if (rc == RMU_OK) rc = grow(e->d_ids, T * sizeof(int32_t), token_rows(T) * sizeof(int32_t));
+    if (rc != RMU_OK) return rc;
+    float* logits = e->gen_ws.as<float>();
+    unsigned* presence = reinterpret_cast<unsigned*>(logits + V);
+    int* tok = reinterpret_cast<int*>(presence + words);
+    float* part = reinterpret_cast<float*>(tok + 4);
+    std::vector<unsigned> bits(words, 0u);
+    for (int i = 0; i < T; ++i) bits[ids_h[i] >> 5] |= 1u << (ids_h[i] & 31);
+    const int cu_h[2] = {0, T};
+    // pageable sources: each copy has taken its bytes when it returns
+    RMU_CUDA(cudaMemcpyAsync(e->d_ids.p, ids_h, T * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(e->span_cu, cu_h, sizeof(cu_h), cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(presence, bits.data(), words * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
+    // the prefill writes the cache; its last row's hidden state gives the first token
+    rc = run_qwen3(e, e->d_ids.as<int32_t>(), e->span_cu, 1, T, T, st, false, true);
+    const float* last = e->PRE + static_cast<size_t>(T - 1) * H;
+    int n = 0;
+    for (int step = 0; rc == RMU_OK; ++step) {
+        if (step > 0) {
+            // the previous token at position p = T + step - 1 through every layer, its k / v into cache row p
+            const int p = T + step - 1;
+            set_int_kernel<<<1, 1, 0, st>>>(e->POSI, p);
+            count_launch();
+            RMU_CHECK_LAUNCH();
+            rc = launch_embed_rows(tok, 1, H, V, e->word, e->PRE, st);
+            for (int l = 0; l < L && rc == RMU_OK; ++l) {
+                const EncLayer& Ly = e->layers[l];
+                rc = qwen3_attention_inputs(e, Ly, 1, st);
+                if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, 1, nh, kv, p, e->kv_cap, kv_layer(e, l), st);
+                if (rc == RMU_OK)
+                    rc = launch_attention_decode(e->QKVP.hi, e->QKVP.lo, kv_layer(e, l), nh, kv, e->kv_cap, p + 1, part,
+                                                 e->CTX.hi, e->CTX.lo, st);
+                if (rc == RMU_OK) rc = qwen3_layer_tail(e, Ly, 1, st);
+            }
+            last = e->PRE;
+        }
+        // logits = lm_head . (w_norm RMS(h_last)), then the sampler
+        if (rc == RMU_OK) rc = launch_rms_split(last, 1, H, e->fng, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
+        if (rc == RMU_OK) {
+            ProfScope _ps(PROF_LM_HEAD, st);
+            GemmParams gp{};
+            gp.M = 1; gp.N = V; gp.K = H; gp.bias = e->lm_zero; gp.out_f32 = logits;
+            rc = launch_gemm(GEMM_BIAS_F32, e->X, e->lm_head, gp, e->sms, st);
+        }
+        if (rc == RMU_OK && logits_h)
+            RMU_CUDA(cudaMemcpyAsync(logits_h + static_cast<size_t>(step) * V, logits, static_cast<size_t>(V) * sizeof(float),
+                                     cudaMemcpyDeviceToHost, st));
+        if (rc == RMU_OK) rc = launch_sample(logits, V, presence, sa, -1.f, seed, static_cast<unsigned long long>(step), tok, st);
+        if (rc != RMU_OK) break;
+        int t_h = 0;
+        RMU_CUDA(cudaMemcpyAsync(&t_h, tok, sizeof(int), cudaMemcpyDeviceToHost, st));
+        rc = qwen3_check_range(e, st);        // synchronises st
+        if (rc != RMU_OK) break;
+        out_h[n++] = t_h;
+        bool eos = false;
+        for (int i = 0; i < s->n_eos; ++i) eos |= t_h == s->eos_ids[i];
+        if (eos || n == max_new_tokens || T + n >= c.max_pos) break;
+    }
+    *n_out = n;
+    if (rc != RMU_OK) return rc;
+    RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
 }
 
@@ -3683,6 +4156,37 @@ int rmu_debug_join_planes(const uint16_t* hi, const uint16_t* lo, int64_t n, flo
     }
     return launch_join_planes(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), static_cast<size_t>(n),
                               out, static_cast<cudaStream_t>(stream));
+}
+
+
+int rmu_debug_attention_decode(const uint16_t* q_hi, const uint16_t* q_lo, const uint16_t* kv, int heads, int kv_heads,
+                               int cap, int n, float* ws, int64_t ws_elems, uint16_t* ctx_hi, uint16_t* ctx_lo,
+                               void* stream) {
+    if (!q_hi || !q_lo || !kv || !ws || !ctx_hi || !ctx_lo || heads < 1 || kv_heads < 1 || n < 1 || cap < n) {
+        set_error("rmu_debug_attention_decode: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (heads % kv_heads != 0) { set_error("rmu_debug_attention_decode: heads % kv_heads != 0"); return RMU_ERR_UNSUPPORTED; }
+    if (ws_elems < 0 || static_cast<size_t>(ws_elems) < decode_part_floats(heads, n)) {
+        set_error("rmu_debug_attention_decode: the workspace needs " + std::to_string(decode_part_floats(heads, n)) + " floats");
+        return RMU_ERR_ARG;
+    }
+    return launch_attention_decode(reinterpret_cast<const __half*>(q_hi), reinterpret_cast<const __half*>(q_lo),
+                                   reinterpret_cast<const __half*>(kv), heads, kv_heads, cap, n, ws,
+                                   reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
+                                   static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_sample(float* logits, int V, uint32_t* presence, const rmu_sampling* s, float u, int32_t* token,
+                     void* stream) {
+    if (!logits || V < 1 || !presence || !s || !token || !(u >= 0.f && u < 1.f)) {
+        set_error("rmu_debug_sample: bad argument");
+        return RMU_ERR_ARG;
+    }
+    const int rc = check_sampling("rmu_debug_sample", s);
+    if (rc != RMU_OK) return rc;
+    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
+    return launch_sample(logits, V, presence, sa, u, 0ull, 0ull, token, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -1,0 +1,145 @@
+"""``HuggingFacePipeline`` — langchain's LLM wrapper around a transformers ``text-generation`` pipeline, with the
+model's ``generate`` on the GPU decoder (SURVEY.md §3.1: the chat model's replies are the reference's dominant wall
+time; ``server/RAGHelper_local.py:105`` builds the wrapper).
+
+Opt in by import, as attention provenance is: ``from ragmeup_b200.llms import HuggingFacePipeline`` in place of
+``from langchain_huggingface.llms import HuggingFacePipeline``.  Only ``generate`` is replaced:
+
+* the prompt is tokenised by the caller's pipeline (``preprocess`` with its ``_preprocess_params``), and the returned
+  text is built by the caller's ``postprocess`` (its ``_postprocess_params``), so both are whatever the installed
+  transformers does;
+* the decoder is found from ``pipeline.model.name_or_path`` as ``provenance.compute_attention`` finds it, and shares
+  ``provenance._DECODERS`` with it: one upload of the weights per (snapshot, device);
+* the settings are ``pipeline.generation_config`` updated with the pipeline's generate kwargs, transformers' defaults
+  for what is unset.  A setting the sampler does not compute raises a ``ValueError`` naming the field;
+* the seed is drawn from torch's CPU default generator, so ``torch.manual_seed`` makes a run repeat (the draw itself is
+  an inverse CDF over a Philox uniform, not ``torch.multinomial``: no parity with torch's random stream).
+
+The model the pipeline holds (the reference's NF4 model) stays loaded but generates nothing.
+"""
+from __future__ import annotations
+
+import copy
+import threading
+from typing import Any, List, Optional
+
+from . import provenance
+
+# GenerationConfig fields the GPU sampler does not compute: each must keep transformers' default value
+REFUSED_FIELDS = ("num_beams", "num_beam_groups", "num_return_sequences", "min_p", "typical_p", "no_repeat_ngram_size",
+                  "bad_words_ids", "sequence_bias", "suppress_tokens", "begin_suppress_tokens", "forced_bos_token_id",
+                  "forced_eos_token_id", "min_new_tokens", "min_length", "stop_strings", "epsilon_cutoff", "eta_cutoff",
+                  "guidance_scale", "encoder_repetition_penalty", "encoder_no_repeat_ngram_size", "diversity_penalty",
+                  "exponential_decay_length_penalty", "renormalize_logits", "constraints", "force_words_ids",
+                  "penalty_alpha", "watermarking_config", "top_h", "assistant_model", "prompt_lookup_num_tokens",
+                  "dola_layers")
+# unset fields hold None in a GenerationConfig built from scratch and False / 0 / [] in one built from a model's config:
+# these values all mean "off"
+
+
+def _off(v) -> bool:
+    return v is None or v is False or (not isinstance(v, bool) and isinstance(v, (int, float)) and v == 0) or v == [] \
+        or v == {}
+
+
+def resolve_settings(generation_config: Any, generate_kwargs: dict, prompt_len: int) -> dict:
+    """``generation_config`` (a transformers GenerationConfig) updated with ``generate_kwargs``, transformers' defaults
+    for the fields left unset -> the arguments of ``DecoderAttention.generate``; ValueError naming the first field the
+    sampler does not compute"""
+    from transformers import GenerationConfig
+    gc = copy.deepcopy(generation_config) if generation_config is not None else GenerationConfig()
+    unused = gc.update(**generate_kwargs)
+    if unused:
+        raise ValueError(f"generate kwarg {sorted(unused)[0]!r} is not supported by the GPU decoder")
+    defaults = GenerationConfig._get_default_generation_params()
+
+    def get(field):
+        v = getattr(gc, field, None)
+        return defaults.get(field) if v is None else v
+
+    for field in REFUSED_FIELDS:
+        v, d = get(field), defaults.get(field)
+        if v != d and not (_off(v) and _off(d)):
+            raise ValueError(f"generation setting {field} = {get(field)!r} is not supported by the GPU decoder's sampler")
+    do_sample = bool(get("do_sample"))
+    top_k = get("top_k")
+    if do_sample and not (top_k and 1 <= int(top_k) <= 256):
+        raise ValueError(f"generation setting top_k = {top_k!r} is not supported when sampling: the sampler keeps at "
+                         f"most 256 candidates (1 <= top_k <= 256)")
+    eos = gc.eos_token_id
+    eos = [] if eos is None else ([int(eos)] if isinstance(eos, int) else [int(t) for t in eos])
+    max_new = gc.max_new_tokens if gc.max_new_tokens is not None else int(get("max_length")) - int(prompt_len)
+    return dict(max_new_tokens=int(max_new), do_sample=do_sample, temperature=float(get("temperature")),
+                top_k=int(top_k or 0), top_p=float(get("top_p")), repetition_penalty=float(get("repetition_penalty")),
+                eos_token_ids=eos)
+
+
+class _PipelineGenerator:
+    """the parts shared by both forms of HuggingFacePipeline"""
+
+    def _setup(self, pipeline: Any) -> None:
+        self._pipe = pipeline
+        self._lock = threading.Lock()
+
+    def _decoder(self):
+        return provenance._decoder(self._pipe.model)
+
+    def _call(self, prompt: str) -> str:
+        import torch
+        pipe = self._pipe
+        with self._lock:
+            inputs = pipe.preprocess(prompt, **pipe._preprocess_params)
+            ids = inputs["input_ids"]
+            if ids.shape[0] != 1:
+                raise ValueError("one prompt per call: batched generation is not supported")
+            fwd = {k: v for k, v in pipe._forward_params.items() if k not in ("generation_config",)}
+            gen_cfg = pipe._forward_params.get("generation_config", getattr(pipe, "generation_config", None) or
+                                               pipe.model.generation_config)
+            settings = resolve_settings(gen_cfg, fwd, ids.shape[1])
+            seed = int(torch.randint(0, 2 ** 63 - 1, (1,)).item())
+            new = self._decoder().generate(ids[0].tolist(), seed=seed, **settings)
+            seq = torch.cat([ids[0].cpu(), torch.as_tensor(new, dtype=ids.dtype)])
+            model_outputs = {"generated_sequence": seq.view(1, 1, -1), "input_ids": ids,
+                             "prompt_text": inputs.get("prompt_text", prompt)}
+            out = pipe.postprocess(model_outputs, **pipe._postprocess_params)
+        return out[0]["generated_text"] if isinstance(out[0], dict) else out[0][0]["generated_text"]
+
+
+try:
+    from langchain_core.language_models.llms import BaseLLM
+    from langchain_core.outputs import Generation, LLMResult
+
+    class HuggingFacePipeline(BaseLLM, _PipelineGenerator):
+        """langchain ``BaseLLM`` around a transformers text-generation pipeline; ``generate`` on the GPU decoder"""
+        pipeline: Any = None
+
+        def __init__(self, pipeline: Any = None, **kwargs):
+            super().__init__(pipeline=pipeline, **kwargs)
+            self._setup(pipeline)
+
+        @property
+        def _llm_type(self) -> str:
+            return "ragmeup_b200_huggingface_pipeline"
+
+        def _generate(self, prompts: List[str], stop: Optional[List[str]] = None, run_manager: Any = None,
+                      **kwargs: Any) -> LLMResult:
+            if stop is not None:
+                raise ValueError("stop sequences are not supported by the GPU decoder")
+            return LLMResult(generations=[[Generation(text=self._call(p))] for p in prompts])
+
+except ImportError:
+    class HuggingFacePipeline(_PipelineGenerator):
+        """a transformers text-generation pipeline with ``generate`` on the GPU decoder (``invoke`` / ``batch``, as
+        langchain's wrapper offers them)"""
+
+        def __init__(self, pipeline: Any = None, **kwargs):
+            self.pipeline = pipeline
+            self._setup(pipeline)
+
+        def invoke(self, prompt: Any, stop: Optional[List[str]] = None, **kwargs: Any) -> str:
+            if stop is not None:
+                raise ValueError("stop sequences are not supported by the GPU decoder")
+            return self._call(prompt.to_string() if hasattr(prompt, "to_string") else str(prompt))
+
+        def batch(self, prompts: List[Any], **kwargs: Any) -> List[str]:
+            return [self.invoke(p, **kwargs) for p in prompts]

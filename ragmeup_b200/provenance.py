@@ -17,14 +17,16 @@ the final handful of float32 additions.
 """
 from __future__ import annotations
 
+import ctypes as C
 import os
+import threading
 from typing import Any, List, Optional, Sequence
 
 import numpy as np
 
 from . import _lib
 from .index import FlatIndex
-from .weights import find_snapshot, resolve_decoder
+from .weights import decoder_lm_head, find_snapshot, resolve_decoder
 
 
 def compute_rerank_provenance(reranker: Any, query: str, documents: Sequence[Any], answer: str) -> Sequence[Any]:
@@ -75,13 +77,17 @@ class DocumentSimilarityAttribution:
 
 class DecoderAttention:
     """A Llama or Qwen3 decoder (``weights.resolve_decoder``: a snapshot directory or ``synthetic:<preset>``) on the
-    GPU, for attention provenance.  Its weights are uploaded once; ``span_mass`` then runs one thread per call."""
+    GPU, for attention provenance and text generation (``llms.HuggingFacePipeline``).  Its weights are uploaded once;
+    ``span_mass`` then runs one thread per call, and ``generate`` attaches the LM head the first time it runs."""
 
     def __init__(self, model_name: str, device: Optional[int] = None):
         from .encoder import BertEncoder
         cfg, w = resolve_decoder(model_name)
         self.cfg = cfg
+        self.model_name = model_name
         self.encoder = BertEncoder(cfg, w, with_head=False, device=device)
+        self.lock = threading.Lock()
+        self._lm_head = False
 
     @property
     def name(self) -> str:
@@ -107,6 +113,34 @@ class DecoderAttention:
         return out.cpu().numpy()
 
 
+    def generate(self, ids: Sequence[int], max_new_tokens: int, do_sample: bool = False, temperature: float = 1.0,
+                 top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.0, eos_token_ids=(),
+                 seed: int = 0) -> List[int]:
+        """the new token ids after the prompt ``ids`` (``rmu_decoder_generate``), the eos token included when one
+        ends the run"""
+        if max_new_tokens < 1:
+            return []
+        eos = [int(t) for t in eos_token_ids]
+        if len(eos) > _lib.MAX_EOS:
+            raise ValueError(f"{self.name}: at most {_lib.MAX_EOS} eos ids, got {len(eos)}")
+        s = _lib.SamplingC(int(bool(do_sample)), float(temperature), float(top_p), float(repetition_penalty),
+                           int(top_k or 0), len(eos), (C.c_int32 * _lib.MAX_EOS)(*eos))
+        prompt = np.ascontiguousarray(list(ids), dtype=np.int32)
+        out = np.zeros(int(max_new_tokens), dtype=np.int32)
+        n = C.c_int32(0)
+        enc = self.encoder
+        with self.lock, enc.torch.cuda.device(enc.device):
+            if not self._lm_head:
+                W = decoder_lm_head(self.model_name, self.cfg)
+                enc._check(_lib.lib().rmu_decoder_set_lm_head(enc._h, W.ctypes.data), "rmu_decoder_set_lm_head")
+                self._lm_head = True
+            enc._check(_lib.lib().rmu_decoder_generate(enc._h, prompt.ctypes.data, len(prompt), C.byref(s),
+                                                       int(seed) & (2 ** 64 - 1), int(max_new_tokens), out.ctypes.data,
+                                                       C.byref(n), None, _lib.stream_ptr()), "rmu_decoder_generate")
+        return out[:n.value].tolist()
+
+
+# one decoder per (snapshot, device): compute_attention and llms.HuggingFacePipeline share its weights
 _DECODERS: dict = {}
 
 

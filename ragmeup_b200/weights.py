@@ -582,7 +582,8 @@ class LlamaConfig(BertConfig):
     """Llama-3 (transformers ``LlamaModel``, model_type ``llama``): Qwen3's decoder without the per-head q / k RMSNorm,
     with ``llama3`` rope scaling (``rope_scaling`` = (factor, low_freq_factor, high_freq_factor,
     original_max_position_embeddings)) or the default rotary embedding (``rope_scaling`` None).  It runs for attention
-    provenance only (``provenance.DecoderAttention``), never as an embedder or reranker, and ``lm_head`` is never read.
+    provenance and generation only (``provenance.DecoderAttention``), never as an embedder or reranker; ``lm_head`` is
+    read by ``decoder_lm_head`` when generation first runs.
     Defaults: the Llama-3.1-8B shape."""
     vocab_size: int = 128256
     hidden: int = 4096
@@ -706,6 +707,26 @@ def resolve_decoder(model_name: str, cache_folder: Optional[str] = None):
         raise ValueError(f"unknown synthetic decoder preset {preset!r}; have {sorted(DECODER_PRESETS)} and the qwen3 "
                          f"presets")
     return _load_decoder_snapshot(find_snapshot(model_name, cache_folder))
+
+
+def decoder_lm_head(model_name: str, cfg: BertConfig, cache_folder: Optional[str] = None) -> np.ndarray:
+    """the decoder's LM head [vocab_size, H] float32: ``lm_head.weight``, or ``embed_tokens`` when config.json sets
+    ``tie_word_embeddings`` (or the snapshot has no lm_head); for ``synthetic:<preset>[:seed[:scale]]`` seeded rows
+    N(0, 0.02 scale) drawn after the decoder's weights"""
+    if model_name.startswith("synthetic:"):
+        parts = model_name.split(":")
+        seed = int(parts[2]) if len(parts) > 2 else 0
+        scale = float(parts[3]) if len(parts) > 3 else 1.0
+        rng = np.random.default_rng([seed, 1])
+        return np.ascontiguousarray(0.02 * scale * rng.standard_normal((cfg.vocab_size, cfg.hidden)), dtype=np.float32)
+    path = find_snapshot(model_name, cache_folder)
+    tied = bool((_read_json(os.path.join(path, "config.json")) or {}).get("tie_word_embeddings", False))
+    names = ([] if tied else ["lm_head.weight"]) + ["model.embed_tokens.weight", "embed_tokens.weight"]
+    for name in names:
+        w = _load_tensors(path, lambda n, name=name: n == name)
+        if name in w:
+            return np.ascontiguousarray(w[name], dtype=np.float32)
+    raise KeyError(f"{path}: no lm_head.weight or embed_tokens.weight")
 
 
 def find_snapshot(model_name: str, cache_folder: Optional[str] = None) -> str:
