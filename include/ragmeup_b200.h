@@ -516,6 +516,7 @@ int rmu_debug_rmsnorm(const float* x, int T, int H, const float* w, float eps, u
 /* For tests: Qwen3's q / k step on the fp32 QKV rows [T, (heads + 2 kv_heads) 128] (q | k | v, heads of 128): per
  * token and q or k head, RMSNorm over the head with q_norm / k_norm [128], rotate-half rotary at pos[t] (clamped into
  * the cos / sin tables [rope_rows, 64]), q times qscale; v unchanged; all written as split planes of the same shape.
+ * q_norm and k_norm both NULL: Llama's step, the same without the RMSNorm; exactly one NULL returns RMU_ERR_ARG.
  * range_flag as above. */
 int rmu_debug_qk_norm_rope(const float* qkv, int T, int heads, int kv_heads, const int32_t* pos, const float* q_norm,
                            const float* k_norm, float eps, float qscale, const float* rope_cos, const float* rope_sin,
@@ -628,6 +629,13 @@ int rmu_debug_dense(const float* x, int B, int n_in, int n_out, const float* W, 
 int rmu_debug_attention_decode(const uint16_t* q_hi, const uint16_t* q_lo, const uint16_t* kv, int heads, int kv_heads,
                                int cap, int n, float* ws, int64_t ws_elems, uint16_t* ctx_hi, uint16_t* ctx_lo,
                                void* stream);
+/* For tests: the KV-cache append of rmu_decoder_generate.  Copies the k and v heads of rows [0, T) of the planes hi / lo
+ * [T, (heads + 2 kv_heads) 128] (q | k | v, as the q / k step leaves them) into rows pos0 .. pos0 + T - 1 of one layer's
+ * cache kv (K hi | K lo | V hi | V lo, each [kv_heads, cap, 128]); nothing else of kv is written.  Null pointers, T,
+ * heads or kv_heads < 1, pos0 < 0 or pos0 + T > cap return RMU_ERR_ARG, heads % kv_heads != 0 RMU_ERR_UNSUPPORTED,
+ * before any CUDA call. */
+int rmu_debug_kv_append(const uint16_t* hi, const uint16_t* lo, int T, int heads, int kv_heads, int pos0, int cap,
+                        uint16_t* kv, void* stream);
 /* For tests: the sampler of rmu_decoder_generate on logits [V] (device fp32, overwritten with the processed values),
  * presence [ceil(V / 32)] (device, bit i of word i / 32 = id i is penalised; the chosen id's bit is set) and the
  * uniform u in [0, 1) -> *token (device int32).  The settings are refused as rmu_decoder_generate refuses them, and a

@@ -6,7 +6,8 @@ lo = fp16_rn(v - hi) (``csrc/rmu_gemm.cuh``).  Each reference below takes the pl
 evaluates hi + lo in float64 (torch, on whichever device the inputs live), so what is left between kernel and
 reference is the kernel's own arithmetic:
 
-* ``gemm_ref``: E1 ``gemm_f16x3_kernel``, sum_k (ah wh + al wh + ah wl) and the four epilogues;
+* ``gemm_ref``: E1 ``gemm_f16x3_kernel``, sum_k (ah wh + al wh + ah wl) and the eight epilogues (BERT's bias, GELU,
+  residual and q-scale; the rotary, GeGLU, fp32-residual and SwiGLU epilogues of ModernBERT, Qwen3 and Llama);
 * ``attention_ref``: E2 ``attention_planes_kernel``, base-2 softmax over the keys of the same sequence;
 * ``layernorm_ref``: E3 ``ln_kernel``, two-pass LayerNorm, biased variance, eps inside the square root;
 * ``embed_ln_ref``: E3 ``embed_ln_kernel``, word + token-type + position rows (clamped as the kernel clamps), then
@@ -25,8 +26,10 @@ import math
 import numpy as np
 import torch
 
-# mode ids of rmu_debug_gemm (include/ragmeup_b200.h)
+# mode ids of rmu_debug_gemm, rmu_debug_gemm_ex and rmu_debug_gemm_swiglu (include/ragmeup_b200.h)
 GEMM_BIAS_F32, GEMM_BIAS_GELU_SPLIT, GEMM_BIAS_RESID_F32, GEMM_BIAS_SPLIT_QSCALE = 0, 1, 2, 3
+GEMM_BIAS_SPLIT_ROPE, GEMM_BIAS_GEGLU_SPLIT, GEMM_BIAS_RESF32_F32, GEMM_BIAS_SWIGLU_SPLIT = 4, 5, 6, 7
+GATED_MODES = (GEMM_BIAS_GEGLU_SPLIT, GEMM_BIAS_SWIGLU_SPLIT)
 
 
 def split_f16(v) -> tuple[np.ndarray, np.ndarray]:
@@ -55,14 +58,69 @@ def _f64(x) -> torch.Tensor:
     return x.to(torch.float64) if isinstance(x, torch.Tensor) else torch.from_numpy(np.asarray(x, np.float64))
 
 
+def deblock(t) -> torch.Tensor:
+    """[..., N] in the gated modes' column order (128-column blocks of 64 input | 64 gate columns) -> [..., N] with
+    every input column first, then every gate column (in | gate of the natural [2F] layout)"""
+    t = _f64(t)
+    blk = t.reshape(*t.shape[:-1], t.shape[-1] // 128, 2, 64)
+    return torch.cat([blk[..., 0, :].flatten(-2), blk[..., 1, :].flatten(-2)], -1)
+
+
+def rope_partner(t, qcols: int, head_dim: int) -> torch.Tensor:
+    """[M, N] -> the value at each column's rotation partner (c <-> c + d/2 within a head) for the q and k columns
+    (col < 2 qcols); v columns map to themselves"""
+    t = _f64(t)
+    n = 2 * qcols
+    h = t[:, :n].reshape(t.shape[0], n // head_dim, 2, head_dim // 2)
+    return torch.cat([h.flip(2).reshape(t.shape[0], n), t[:, n:]], 1)
+
+
+def rope_columns(pos, rope_cos, rope_sin, N: int, qcols: int, head_dim: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """(C, Sn) [M, N] float64 of the rotary epilogue: out_c = x_c C_c + x_partner(c) Sn_c, from the float32 tables at
+    each row's position clamped into [0, rope_rows) as the kernel clamps it.  Sn = -sin on the first half of a head,
+    +sin on the second; C = 1 and Sn = 0 on the v columns."""
+    c, s = _f64(rope_cos), _f64(rope_sin)
+    p = _long(pos, c.device).clamp(0, int(c.shape[0]) - 1)
+    M, n = int(p.shape[0]), 2 * qcols
+    cp, sp = c[p], s[p]                                       # [M, head_dim / 2]
+    C = torch.ones((M, N), dtype=torch.float64, device=c.device)
+    Sn = torch.zeros_like(C)
+    C[:, :n] = torch.cat([cp, cp], 1).repeat(1, n // head_dim)
+    Sn[:, :n] = torch.cat([-sp, sp], 1).repeat(1, n // head_dim)
+    return C, Sn
+
+
 def gemm_ref(mode: int, a_hi, a_lo, w_hi, w_lo, bias, res_hi=None, res_lo=None, qcols: int = 0,
-             qscale: float = 1.0) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+             qscale: float = 1.0, res_f32=None, pos=None, rope_cos=None, rope_sin=None,
+             head_dim: int = 64) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """E1 on A [M, K] and W [N, K] planes.  Returns (out, x, S): out [M, N] float64 after the epilogue of `mode`,
-    x = the pre-epilogue sum + bias (GELU's argument), and S_ij = sum_k |a_ik w_jk| for the error bound."""
+    x = the pre-epilogue sum + bias (GELU's argument), and S_ij = sum_k |a_ik w_jk| for the error bound.
+
+    * mode 4 (rotary): q | k columns (col < 2 qcols) rotated per head of head_dim at pos[row] (``rope_columns``), then
+      q (col < qcols) times float32(qscale); v as mode 3 leaves it.  x and S are before the rotation: the partner
+      column's are ``rope_partner(x / S, qcols, head_dim)``.
+    * modes 5 (GeGLU) and 7 (SwiGLU): W in the kernel's 128-row blocks of 64 input | 64 gate rows; out [M, N / 2] =
+      act(in) * gate with act = gelu_erf / silu, in natural column order.  x and S are ``deblock``-ed: columns
+      [0, N / 2) are the inputs', [N / 2, N) the gates'.
+    * mode 6: out = x + res_f32 (fp32 [M, N])."""
     ah, al, wh, wl = _f64(a_hi), _f64(a_lo), _f64(w_hi), _f64(w_lo)
     acc = ah @ wh.T + al @ wh.T + ah @ wl.T          # the three products the kernel issues (no lo * lo)
     S = (ah + al).abs() @ (wh + wl).abs().T
-    x = acc + _f64(bias)[None, :]
+    x = acc + _f64(bias).to(acc.device)[None, :]
+    if mode in GATED_MODES:
+        x, S = deblock(x), deblock(S)
+        F = x.shape[1] // 2
+        xin, gate = x[:, :F], x[:, F:]
+        act = 0.5 * xin * (1.0 + torch.special.erf(xin / math.sqrt(2.0))) if mode == GEMM_BIAS_GEGLU_SPLIT \
+            else xin * torch.sigmoid(xin)
+        return act * gate, x, S
+    if mode == GEMM_BIAS_SPLIT_ROPE:
+        C, Sn = rope_columns(pos, rope_cos, rope_sin, x.shape[1], qcols, head_dim)
+        out = x * C.to(x.device) + rope_partner(x, qcols, head_dim) * Sn.to(x.device)
+        out[:, :qcols] *= float(np.float32(qscale))
+        return out, x, S
+    if mode == GEMM_BIAS_RESF32_F32:
+        return x + _f64(res_f32).to(x.device), x, S
     if mode == GEMM_BIAS_F32:
         out = x
     elif mode == GEMM_BIAS_GELU_SPLIT:

@@ -209,6 +209,8 @@ SIGNATURES = {
                                        C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "rmu_debug_attention_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                              C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_kv_append": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                      C.c_void_p]),
     "rmu_debug_sample": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(SamplingC), C.c_float, C.c_void_p,
                                    C.c_void_p]),
     "rmu_debug_split_planes": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),

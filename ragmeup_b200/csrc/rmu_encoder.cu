@@ -4086,7 +4086,8 @@ int rmu_debug_rmsnorm(const float* x, int T, int H, const float* w, float eps, u
 int rmu_debug_qk_norm_rope(const float* qkv, int T, int heads, int kv_heads, const int32_t* pos, const float* q_norm,
                            const float* k_norm, float eps, float qscale, const float* rope_cos, const float* rope_sin,
                            int rope_rows, uint16_t* hi, uint16_t* lo, int32_t* range_flag, void* stream) {
-    if (!qkv || !pos || !q_norm || !k_norm || !rope_cos || !rope_sin || !hi || !lo || T <= 0 || heads <= 0 ||
+    // both norms null: Llama's step without the per-head RMSNorm; exactly one null is a caller error
+    if (!qkv || !pos || !q_norm != !k_norm || !rope_cos || !rope_sin || !hi || !lo || T <= 0 || heads <= 0 ||
         kv_heads <= 0 || rope_rows <= 0) {
         set_error("rmu_debug_qk_norm_rope: bad argument");
         return RMU_ERR_ARG;
@@ -4175,6 +4176,18 @@ int rmu_debug_attention_decode(const uint16_t* q_hi, const uint16_t* q_lo, const
                                    reinterpret_cast<const __half*>(kv), heads, kv_heads, cap, n, ws,
                                    reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
                                    static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_kv_append(const uint16_t* hi, const uint16_t* lo, int T, int heads, int kv_heads, int pos0, int cap,
+                        uint16_t* kv, void* stream) {
+    if (!hi || !lo || !kv || T < 1 || heads < 1 || kv_heads < 1 || pos0 < 0 ||
+        static_cast<int64_t>(pos0) + T > cap) {
+        set_error("rmu_debug_kv_append: bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (heads % kv_heads != 0) { set_error("rmu_debug_kv_append: heads % kv_heads != 0"); return RMU_ERR_UNSUPPORTED; }
+    return launch_kv_append(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), T, heads, kv_heads,
+                            pos0, cap, reinterpret_cast<__half*>(kv), static_cast<cudaStream_t>(stream));
 }
 
 int rmu_debug_sample(float* logits, int V, uint32_t* presence, const rmu_sampling* s, float u, int32_t* token,

@@ -154,6 +154,35 @@ def test_kernel_test_entry_points_reject_before_any_cuda_call(built_lib):
     assert bsel(m=4096, ws_elems=2 * 3 * 10 - 1) == -1 and bsel(m=4097, ws_elems=2 * 3 * 2 * 10 - 1) == -1
     assert bsel(Q=65535, m=1, k=256, ws_elems=2 * 65535 * 256 - 1) == -1
 
+    # the KV-cache append: rows pos0 .. pos0 + T - 1 of a cache of cap rows
+    def kva(T=4, heads=8, kv_heads=2, pos0=0, cap=16, **kw):
+        a = dict(hi=p, lo=p, kv=p)
+        a.update(kw)
+        return l.rmu_debug_kv_append(a["hi"], a["lo"], T, heads, kv_heads, pos0, cap, a["kv"], None)
+
+    for name in ("hi", "lo", "kv"):
+        assert kva(**{name: None}) == -1, name
+    for name in ("T", "heads", "kv_heads"):
+        assert kva(**{name: 0}) == -1 and kva(**{name: -1}) == -1, name
+    assert kva(pos0=-1) == -1 and b"rmu_debug_kv_append" in l.rmu_last_error()
+    assert kva(pos0=13) == -1 and kva(T=17) == -1 and kva(cap=0) == -1          # pos0 + T > cap
+    assert kva(T=1, pos0=2 ** 31 - 1, cap=2 ** 31 - 1) == -1                    # pos0 + T overflows int32
+    assert kva(heads=6, kv_heads=4) == -3 and kva(heads=3, kv_heads=2) == -3    # heads % kv_heads
+
+    # the q / k step: q_norm and k_norm both null (Llama) or both set; one of them alone is refused
+    def qk(qn=p, kn=p, T=3, heads=8, kv=2, rows=16, **kw):
+        a = dict(x=p, pos=p, cos=p, sin=p, hi=p, lo=p)
+        a.update(kw)
+        return l.rmu_debug_qk_norm_rope(a["x"], T, heads, kv, a["pos"], qn, kn, 1e-6, 1.0, a["cos"], a["sin"], rows,
+                                        a["hi"], a["lo"], None, None)
+
+    assert qk(qn=None) == -1 and qk(kn=None) == -1 and b"rmu_debug_qk_norm_rope" in l.rmu_last_error()
+    for norms in ((p, p), (None, None)):
+        for name in ("x", "pos", "cos", "sin", "hi", "lo"):
+            assert qk(*norms, **{name: None}) == -1, name
+        assert qk(*norms, T=0) == -1 and qk(*norms, heads=0) == -1 and qk(*norms, kv=0) == -1
+        assert qk(*norms, rows=0) == -1
+
 
 def test_encoder_create_refuses_weights_the_split_planes_cannot_hold(built_lib):
     """GEMM weights travel as fp16 planes, and fp16 rounds |w| >= 65520 to inf: rmu_encoder_create refuses such a

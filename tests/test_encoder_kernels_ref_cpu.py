@@ -82,6 +82,104 @@ def test_gemm_reference_with_zero_lo_is_the_float64_product():
     assert np.allclose(out.numpy(), want + 2.0 ** -12 * (a64.sum(1)[:, None] + w64.sum(1)[None, :]), rtol=0, atol=1e-12)
 
 
+def _blocked_rows(first, second):
+    """the gated modes' weight layout: 128-row blocks of 64 rows of `first` then the 64 matching rows of `second`"""
+    out = np.empty((2 * first.shape[0],) + first.shape[1:], first.dtype)
+    for k in range(first.shape[0] // 64):
+        out[128 * k:128 * k + 64] = first[64 * k:64 * k + 64]
+        out[128 * k + 64:128 * k + 128] = second[64 * k:64 * k + 64]
+    return out
+
+
+def _planes64(x):
+    hi, lo = ref.split_f16(x)
+    return hi, lo, torch.from_numpy(ref.join(hi, lo))
+
+
+@pytest.mark.parametrize("head_dim,qcols,N", [(64, 128, 384), (32, 128, 384), (64, 192, 640)])
+def test_gemm_reference_rope_mode_is_modernbert_rotate(head_dim, qcols, N):
+    """mode 4 against modernbert_ref.rotate per head on x = A W^T + b, positions clamped into the tables, q scaled by
+    float32(qscale), v untouched (columns past 3 qcols included)"""
+    from oracle import modernbert_ref as mr
+    from ragmeup_b200.weights import rope_table
+    rng = np.random.default_rng(head_dim + qcols)
+    M, K, rows = 9, 64, 50
+    ah, al, A = _planes64(rng.standard_normal((M, K)))
+    wh, wl, W = _planes64(0.1 * rng.standard_normal((N, K)))
+    bias = rng.standard_normal(N).astype(np.float32)
+    cos, sin = rope_table(10000.0, head_dim, rows)
+    pos = np.array([0, 1, rows - 1, -3, rows, rows + 70, 7, 23, 49], np.int32)
+    qs = 1.4426950408889634 / math.sqrt(head_dim)
+    out, x, S = ref.gemm_ref(ref.GEMM_BIAS_SPLIT_ROPE, ah, al, wh, wl, bias, qcols=qcols, qscale=qs, pos=pos,
+                             rope_cos=cos, rope_sin=sin, head_dim=head_dim)
+    acc = A @ W.T - torch.from_numpy(ref.join(al, np.zeros_like(al))).double() @ torch.from_numpy(
+        ref.join(wl, np.zeros_like(wl))).T                  # the kernel's three products: no al * wl
+    xx = acc + torch.from_numpy(bias).double()
+    assert torch.allclose(x, xx, rtol=1e-13, atol=1e-13)
+    assert torch.allclose(S, A.abs() @ W.abs().T, rtol=1e-13, atol=0)
+    pc = torch.from_numpy(np.clip(pos, 0, rows - 1)).long()
+    c, s = torch.from_numpy(cos).double()[pc], torch.from_numpy(sin).double()[pc]
+    want = xx.clone()
+    for part in (0, 1):
+        blk = xx[:, part * qcols:(part + 1) * qcols].reshape(M, qcols // head_dim, head_dim).transpose(0, 1)
+        want[:, part * qcols:(part + 1) * qcols] = mr.rotate(blk, c, s).transpose(0, 1).reshape(M, qcols)
+    want[:, :qcols] *= float(np.float32(qs))
+    assert torch.allclose(out, want, rtol=1e-13, atol=1e-13)
+    assert torch.equal(out[:, 2 * qcols:], x[:, 2 * qcols:])
+    # the partner of a q / k column is the other half of its head; a v column is its own
+    P = ref.rope_partner(x, qcols, head_dim)
+    h = head_dim // 2
+    assert torch.equal(P[:, 0], x[:, h]) and torch.equal(P[:, h], x[:, 0])
+    assert torch.equal(P[:, qcols + head_dim + 1], x[:, qcols + head_dim + h + 1])
+    assert torch.equal(P[:, 2 * qcols:], x[:, 2 * qcols:])
+
+
+@pytest.mark.parametrize("mode", [ref.GEMM_BIAS_GEGLU_SPLIT, ref.GEMM_BIAS_SWIGLU_SPLIT])
+def test_gemm_reference_gated_modes_on_natural_weights(mode):
+    """modes 5 and 7 on the blocked W against the natural layout: ModernBERT's gelu(in) * gate with in | gate = Wi x +
+    bi (modernbert_ref._gelu), Qwen3 / Llama's silu(gate_proj x) * up_proj x (torch.nn.functional.silu)"""
+    from oracle import modernbert_ref as mr
+    rng = np.random.default_rng(mode)
+    M, K, F = 7, 128, 192                                    # F not a multiple of 128
+    ah = rng.standard_normal((M, K)).astype(np.float16)     # fp16-exact A: the lo * lo term the kernel drops is 0
+    al = np.zeros_like(ah)
+    A = torch.from_numpy(ah.astype(np.float64))
+    w_in = (0.3 * rng.standard_normal((F, K))).astype(np.float32)
+    w_gate = (0.3 * rng.standard_normal((F, K))).astype(np.float32)
+    b_in = rng.standard_normal(F).astype(np.float32)
+    b_gate = rng.standard_normal(F).astype(np.float32)
+    wh, wl = ref.split_f16(_blocked_rows(w_in, w_gate))
+    bias = _blocked_rows(b_in[:, None], b_gate[:, None])[:, 0].copy()
+    out, x, S = ref.gemm_ref(mode, ah, al, wh, wl, bias)
+    Win = torch.from_numpy(ref.join(*ref.split_f16(w_in)))
+    Wg = torch.from_numpy(ref.join(*ref.split_f16(w_gate)))
+    xin = A @ Win.T + torch.from_numpy(b_in).double()
+    xg = A @ Wg.T + torch.from_numpy(b_gate).double()
+    if mode == ref.GEMM_BIAS_GEGLU_SPLIT:
+        want = mr._gelu(xin) * xg
+    else:
+        want = torch.nn.functional.silu(xin) * xg
+    assert out.shape == (M, F)
+    assert torch.allclose(out, want, rtol=1e-10, atol=1e-10)
+    assert torch.allclose(x[:, :F], xin, rtol=1e-10, atol=1e-10) and torch.allclose(x[:, F:], xg, rtol=1e-10, atol=1e-10)
+    assert torch.allclose(S[:, :F], A.abs() @ Win.abs().T, rtol=1e-12) and torch.allclose(S[:, F:], A.abs() @ Wg.abs().T,
+                                                                                      rtol=1e-12)
+
+
+def test_gemm_reference_fp32_residual_mode():
+    rng = np.random.default_rng(6)
+    M, N, K = 5, 256, 64
+    a = rng.standard_normal((M, K)).astype(np.float16)
+    w = rng.standard_normal((N, K)).astype(np.float16)
+    z = np.zeros_like
+    bias = rng.standard_normal(N).astype(np.float32)
+    res = (1e5 * rng.standard_normal((M, N))).astype(np.float32)
+    out, x, _ = ref.gemm_ref(ref.GEMM_BIAS_RESF32_F32, a, z(a), w, z(w), bias, res_f32=res)
+    want = a.astype(np.float64) @ w.astype(np.float64).T + bias.astype(np.float64) + res.astype(np.float64)
+    assert np.array_equal(out.numpy(), want)
+    assert np.array_equal((out - x).numpy(), res.astype(np.float64))
+
+
 def test_layernorm_reference_agrees_with_bert_ref():
     rng = np.random.default_rng(3)
     H = 384
