@@ -53,7 +53,8 @@ uint64_t rmu_launch_count(void);
 /* per-kernel-class device timing (CUDA events on the launching stream; used by bench.py for the
  * roofline objects).  classes: 0 scan, 1 finalize, 2 exact scan, 3 merge, 4 gemm, 5 attention,
  * 6 layernorm, 7 embedding, 8 pool/head, 9 misc, 10 second-pass scan launches (queries whose certificate failed; exit at once when there are none),
- * 11 decode attention and KV cache writes, 12 LM head (its GEMM is also in 4), 13 sampler.  rmu_profile_read synchronises the recorded events. */
+ * 11 decode attention and KV cache writes, 12 LM head (its GEMM is also in 4), 13 sampler, 14 the NF4 kernels
+ * (quantiser, dequantiser, decode GEMV; the prefill's E1 GEMMs on dequantised weights stay in 4).  rmu_profile_read synchronises the recorded events. */
 void rmu_profile_enable(int on);
 void rmu_profile_reset(void);
 int rmu_profile_read(int cls, double* total_ms, int64_t* launches);
@@ -350,6 +351,18 @@ int rmu_decoder_attention_spans(rmu_encoder* enc, const int32_t* ids, int T, con
  * tied) as split fp16 planes.  Refused before any CUDA call: a null handle or W_h, another kind of encoder, a second
  * call (RMU_ERR_ARG); vocab_size not a multiple of 128 or |w| >= 65520 (RMU_ERR_UNSUPPORTED). */
 int rmu_decoder_set_lm_head(rmu_encoder* enc, const float* W_h);
+/* NF4 weights for a decoder, as the reference's bitsandbytes load holds them (blocksize 64, fp32 absmax, no double
+ * quantisation): each layer's q | k | v, o, gate | up and down projections become packed 4-bit codes [N, K / 2] (the
+ * first element in the high nibble) and absmax [N, K / 64], quantised on the device from their hi planes (the fp16
+ * cast of the checkpoint's values), and their split planes are freed as the conversion goes, so the handle never holds
+ * more device memory than before the call.  The LM head, the embeddings and the norms are unchanged.  Afterwards
+ * rmu_decoder_generate and rmu_decoder_attention_spans compute with the dequantised weights fp16(code * absmax): each
+ * decode step's projections (M = 1) run a GEMV that reads the codes directly; a prefill dequantises each weight into
+ * one scratch plane pair (the size of the largest projection) and runs E1 on it.  Range flag and RMU_ERR_RANGE are as
+ * before.  Refused before any CUDA call: a null handle, another kind of encoder, a handle already converted
+ * (RMU_ERR_ARG); a projection whose K is not a multiple of 64 or exceeds 49 152 (RMU_ERR_UNSUPPORTED).  A failure
+ * part-way leaves a handle that every call refuses; destroy it.  Synchronises the device. */
+int rmu_decoder_quantize_nf4(rmu_encoder* enc, void* stream);
 /* Token selection, in transformers' order: the repetition penalty (x < 0 ? x * p : x / p) on every id of the prompt and
  * of the generated tokens; then with do_sample 0 the largest logit (the lowest id among equal ones); with do_sample 1
  * x / temperature, top-k (every logit >= the k-th largest survives; 1 <= top_k <= 256, and when more than 256 logits
@@ -634,6 +647,20 @@ int rmu_debug_attention_decode(const uint16_t* q_hi, const uint16_t* q_lo, const
  * cache kv (K hi | K lo | V hi | V lo, each [kv_heads, cap, 128]); nothing else of kv is written.  Null pointers, T,
  * heads or kv_heads < 1, pos0 < 0 or pos0 + T > cap return RMU_ERR_ARG, heads % kv_heads != 0 RMU_ERR_UNSUPPORTED,
  * before any CUDA call. */
+/* The NF4 kernels one at a time (device pointers; fp16 planes as uint16).  quantize: hi [n] -> codes [n / 2], absmax
+ * [n / 64]; dequantize: the reverse into hi [n]; gemv: one row x = x_hi + x_lo [K] against codes [N, K / 2] / absmax
+ * [N, K / 64] with E1's epilogue `mode` at M = 1: 0 out_f32 [N] = acc + bias; 6 out_f32 = acc + bias + res_f32 (res_f32
+ * may be out_f32); 7 SwiGLU on 128-row blocks of 64 gate | 64 up rows into out_hi / out_lo [N / 2], setting
+ * *range_flag (nullable) when an output leaves the fp16 range.  Refused before any CUDA call: null pointers, n < 1,
+ * a mode other than 0, 6, 7 (RMU_ERR_ARG); n or K not a multiple of 64, K > 49 152, N not a multiple of 128
+ * (RMU_ERR_UNSUPPORTED).  nf4_conversion reads, for a converted handle, the most its conversion's allocations ever
+ * exceeded the bytes held before it (<= 0) and their final difference, in bytes; RMU_ERR_ARG otherwise. */
+int rmu_debug_nf4_quantize(const uint16_t* hi, int64_t n, uint8_t* codes, float* absmax, void* stream);
+int rmu_debug_nf4_dequantize(const uint8_t* codes, const float* absmax, int64_t n, uint16_t* hi, void* stream);
+int rmu_debug_nf4_gemv(int mode, const uint16_t* x_hi, const uint16_t* x_lo, const uint8_t* codes, const float* absmax,
+                       int N, int K, const float* bias, const float* res_f32, float* out_f32, uint16_t* out_hi,
+                       uint16_t* out_lo, int32_t* range_flag, void* stream);
+int rmu_debug_nf4_conversion(const rmu_encoder* enc, int64_t* peak, int64_t* delta);
 int rmu_debug_kv_append(const uint16_t* hi, const uint16_t* lo, int T, int heads, int kv_heads, int pos0, int cap,
                         uint16_t* kv, void* stream);
 /* For tests: the sampler of rmu_decoder_generate on logits [V] (device fp32, overwritten with the processed values),

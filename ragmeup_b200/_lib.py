@@ -129,6 +129,7 @@ SIGNATURES = {
     "rmu_decoder_attention_spans": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
                                               C.c_void_p]),
     "rmu_decoder_set_lm_head": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "rmu_decoder_quantize_nf4": (C.c_int, [C.c_void_p, C.c_void_p]),
     "rmu_decoder_generate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(SamplingC), C.c_uint64, C.c_int,
                                        C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]),
     "rmu_encoder_destroy": (None, [C.c_void_p]),
@@ -211,6 +212,11 @@ SIGNATURES = {
                                              C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_kv_append": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                       C.c_void_p]),
+    "rmu_debug_nf4_quantize": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_nf4_dequantize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "rmu_debug_nf4_gemv": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_nf4_conversion": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "rmu_debug_sample": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(SamplingC), C.c_float, C.c_void_p,
                                    C.c_void_p]),
     "rmu_debug_split_planes": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libragmeup_b200.so")
 STAMP = os.path.join(CSRC, ".build_stamp")
-SOURCES = ["rmu_common.cu", "rmu_index.cu", "rmu_gemm.cu", "rmu_encoder.cu", "rmu_bm25.cu", "rmu_bm25_host.cu", "rmu_pgbm25.cu"]
+SOURCES = ["rmu_common.cu", "rmu_index.cu", "rmu_gemm.cu", "rmu_encoder.cu", "rmu_nf4.cu", "rmu_bm25.cu", "rmu_bm25_host.cu", "rmu_pgbm25.cu"]
 # every header under csrc/ takes part in the up-to-date check
 HEADERS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [os.path.join("..", "..", "include", "ragmeup_b200.h")]
 

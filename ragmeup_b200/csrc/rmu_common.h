@@ -19,7 +19,8 @@ inline void count_launch(int n = 1) { g_launches.fetch_add(static_cast<uint64_t>
 // ---- optional per-kernel-class timing (bench.py roofline): CUDA events on the launching stream
 enum ProfClass { PROF_SCAN = 0, PROF_FINALIZE, PROF_EXACT, PROF_MERGE, PROF_GEMM, PROF_ATTN, PROF_LN, PROF_EMBED,
                  PROF_POOL_HEAD, PROF_MISC, PROF_SCAN_LEAD /* second-pass scan launches */,
-                 PROF_DECODE_ATTN /* decode attention and the KV cache writes */, PROF_LM_HEAD, PROF_SAMPLE, PROF_NCLASS };
+                 PROF_DECODE_ATTN /* decode attention and the KV cache writes */, PROF_LM_HEAD, PROF_SAMPLE,
+                 PROF_NF4 /* NF4 weights: quantiser, dequantiser, decode GEMV */, PROF_NCLASS };
 extern std::atomic<int> g_prof_on;
 void prof_begin(int cls, cudaStream_t st);
 void prof_end(int cls, cudaStream_t st);

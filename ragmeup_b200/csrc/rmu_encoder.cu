@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "rmu_gemm.cuh"
+#include "rmu_nf4.cuh"
 
 namespace rmu {
 
@@ -2268,6 +2269,7 @@ struct EncLayer {
     __half *pos_hi = nullptr, *pos_lo = nullptr;   // position_buckets > 0: PQ' | PK planes [2s, 2H] of the layer
     int window = 0;                       // ModernBERT: the layer's attention half-window (0 = global attention)
     float *qn = nullptr, *kn = nullptr;   // Qwen3: q_norm, k_norm [128]
+    Nf4Weight nf4[4];                     // rmu_decoder_quantize_nf4: Wqkv, Wo, W1, W2 in NF4 (their split planes freed)
 };
 
 // A device scratch buffer that only grows.  The caller's lock keeps other users of the buffer out.
@@ -2333,6 +2335,14 @@ struct rmu_encoder {
     float* lm_zero = nullptr;
     DevBuf kv_cache, gen_ws;
     int kv_cap = 0;
+    // NF4 weights (rmu_decoder_quantize_nf4): the layers' projections live in EncLayer::nf4; a prefill dequantises
+    // each into the one scratch operand set nf4_hi | nf4_lo (lo all zero), seen through nf4_op[projection]'s tensor
+    // maps.  nf4_broken: a conversion failed part-way and the handle cannot run.  nf4_peak / nf4_delta: the most the
+    // conversion's allocations exceeded, and finally differ from, the bytes the handle held before it.
+    bool nf4 = false, nf4_broken = false;
+    __half *nf4_hi = nullptr, *nf4_lo = nullptr;
+    SplitOperand nf4_op[4];
+    int64_t nf4_peak = 0, nf4_delta = 0;
     // sentence-transformers Dense modules after pooling (rmu_encoder_set_dense): dense_dims [n + 1], per layer W [out, in],
     // b [out] or null, act; dense_ws holds two [B, max width] ping-pong rows, grown under mu
     std::vector<int> dense_dims;
@@ -2702,6 +2712,20 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
     return RMU_OK;
 }
 
+// projection `which` (0 Wqkv, 1 Wo, 2 W1, 3 W2) of a decoder layer, C = A W^T with E1's epilogue `mode`.  Split
+// planes: E1.  NF4: the decode GEMV at M = 1; otherwise the weight dequantised into the scratch planes, then E1 on
+// them (the scratch is reused by the next projection in stream order).
+static SplitOperand EncLayer::* const kDecoderSplit[4] = {&EncLayer::Wqkv, &EncLayer::Wo, &EncLayer::W1, &EncLayer::W2};
+
+static int decoder_gemm(rmu_encoder* e, int mode, const SplitOperand& A, const EncLayer& L, int which, const GemmParams& g,
+                        cudaStream_t st) {
+    if (!e->nf4) return launch_gemm(mode, A, L.*kDecoderSplit[which], g, e->sms, st);
+    const Nf4Weight& W = L.nf4[which];
+    if (g.M == 1) return launch_nf4_gemv(mode, A.hi, A.lo, W, g, e->sms, st);
+    const int rc = launch_nf4_dequantize(W.codes, W.absmax, static_cast<int64_t>(W.rows) * W.cols, e->nf4_hi, st);
+    return rc != RMU_OK ? rc : launch_gemm(mode, A, e->nf4_op[which], g, e->sms, st);
+}
+
 // one decoder layer up to its attention inputs: X = split(w_in RMS(h)); QKVF = X Wqkv^T (fp32); QKVP = the q / k step
 static int qwen3_attention_inputs(rmu_encoder* e, const EncLayer& L, int T, cudaStream_t st) {
     const rmu_bert_config& c = e->cfg;
@@ -2711,7 +2735,7 @@ static int qwen3_attention_inputs(rmu_encoder* e, const EncLayer& L, int T, cuda
     if (rc != RMU_OK) return rc;
     GemmParams g{};
     g.M = T; g.N = NQKV; g.K = c.hidden; g.bias = e->zeros; g.out_f32 = e->QKVF;
-    rc = launch_gemm(GEMM_BIAS_F32, e->X, L.Wqkv, g, e->sms, st);
+    rc = decoder_gemm(e, GEMM_BIAS_F32, e->X, L, 0, g, st);
     if (rc != RMU_OK) return rc;
     return launch_qk_norm_rope(e->QKVF, T, nh, kv, e->POSI, L.qn, L.kn, c.ln_eps, qscale, e->rope_cos[0], e->rope_sin[0],
                                c.max_pos, e->QKVP.hi, e->QKVP.lo, e->range_flag, st);
@@ -2724,16 +2748,16 @@ static int qwen3_layer_tail(rmu_encoder* e, const EncLayer& L, int M, cudaStream
     const int H = c.hidden, F = c.ffn, QD = c.heads * kQwenHD;
     GemmParams g{};
     g.M = M; g.N = H; g.K = QD; g.bias = e->zeros; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
-    int rc = launch_gemm(GEMM_BIAS_RESF32_F32, e->CTX, L.Wo, g, e->sms, st);
+    int rc = decoder_gemm(e, GEMM_BIAS_RESF32_F32, e->CTX, L, 1, g, st);
     if (rc == RMU_OK) rc = launch_rms_split(e->PRE, M, H, L.ln2g, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
     if (rc != RMU_OK) return rc;
     g = GemmParams{};
     g.M = M; g.N = 2 * F; g.K = H; g.bias = e->zeros; g.out_hi = e->FF.hi; g.out_lo = e->FF.lo; g.range_flag = e->range_flag;
-    rc = launch_gemm(GEMM_BIAS_SWIGLU_SPLIT, e->X, L.W1, g, e->sms, st);
+    rc = decoder_gemm(e, GEMM_BIAS_SWIGLU_SPLIT, e->X, L, 2, g, st);
     if (rc != RMU_OK) return rc;
     g = GemmParams{};
     g.M = M; g.N = H; g.K = F; g.bias = e->zeros; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
-    return launch_gemm(GEMM_BIAS_RESF32_F32, e->FF, L.W2, g, e->sms, st);
+    return decoder_gemm(e, GEMM_BIAS_RESF32_F32, e->FF, L, 3, g, st);
 }
 
 // layer l's K / V planes in the KV cache (kv_append_kernel's layout)
@@ -2750,6 +2774,10 @@ static int run_qwen3(rmu_encoder* e, const int32_t* ids, const int32_t* cu, int 
                      bool attn_last = false, bool to_cache = false) {
     const rmu_bert_config& c = e->cfg;
     if (max_seqlen > c.max_pos) { set_error("sequence longer than max_position_embeddings"); return RMU_ERR_ARG; }
+    if (e->nf4_broken) {
+        set_error("the handle's NF4 conversion failed part-way (rmu_decoder_quantize_nf4); destroy it");
+        return RMU_ERR_ARG;
+    }
     const int H = c.hidden, nh = c.heads, kv = e->qext.kv_heads;
     int rc = ensure_tokens(e, T, B);
     if (rc != RMU_OK) return rc;
@@ -3385,6 +3413,10 @@ int rmu_decoder_attention_spans(rmu_encoder* e, const int32_t* ids, int T, const
                   "rmu_encoder_create_llama");
         return RMU_ERR_ARG;
     }
+    if (e->nf4_broken) {
+        set_error("rmu_decoder_attention_spans: the handle's NF4 conversion failed part-way; destroy it");
+        return RMU_ERR_ARG;
+    }
     if (T > e->cfg.max_pos) {
         set_error("rmu_decoder_attention_spans: " + std::to_string(T) + " tokens exceed max_position_embeddings (" +
                   std::to_string(e->cfg.max_pos) + ")");
@@ -3521,6 +3553,83 @@ int rmu_decoder_set_lm_head(rmu_encoder* e, const float* W_h) {
     return RMU_OK;
 }
 
+int rmu_decoder_quantize_nf4(rmu_encoder* e, void* stream) {
+    const std::string fn("rmu_decoder_quantize_nf4");
+    if (!e) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
+    if (!e->qwen || e->has_head) {
+        set_error(fn + ": the encoder must come from rmu_encoder_create_qwen3 without a head or from rmu_encoder_create_llama");
+        return RMU_ERR_ARG;
+    }
+    const rmu_bert_config& c = e->cfg;
+    const int H = c.hidden, F = c.ffn, QD = c.heads * kQwenHD, NQKV = e->qkv_w;
+    // K of q | k | v, o, gate | up, down.  K % 64 == 0 keeps every quantisation block inside one row, so the handle's
+    // row orders (the fused q | k | v rows, W1's 64 + 64 gate / up blocks) move whole blocks and give the codes of the
+    // checkpoint's own tensors.
+    const int64_t shape[4][2] = {{NQKV, H}, {H, QD}, {2 * static_cast<int64_t>(F), H}, {H, F}};
+    for (const auto& sh : shape) {
+        if (sh[1] % kNf4Block != 0 || sh[1] > kNf4MaxK) {
+            set_error(fn + ": every projection's K must be a multiple of 64 up to " + std::to_string(kNf4MaxK) + ", got " +
+                      std::to_string(sh[1]));
+            return RMU_ERR_UNSUPPORTED;
+        }
+    }
+    std::lock_guard<std::mutex> hg(e->host_mu);
+    std::lock_guard<std::mutex> g(e->mu);
+    if (e->nf4 || e->nf4_broken) { set_error(fn + ": the handle's weights are already NF4"); return RMU_ERR_ARG; }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    RMU_CUDA(cudaDeviceSynchronize());                 // work queued on any stream may still read the split planes
+    int64_t delta = 0, peak = 0;
+    auto release = [&](void* p, int64_t bytes) -> int {
+        e->allocs.erase(std::find(e->allocs.begin(), e->allocs.end(), p));
+        RMU_CUDA(cudaFree(p));
+        delta -= bytes;
+        return RMU_OK;
+    };
+    auto convert = [&](EncLayer& L, int w) -> int {
+        SplitOperand& S = L.*kDecoderSplit[w];
+        Nf4Weight& Q = L.nf4[w];
+        const int64_t n = shape[w][0] * shape[w][1];
+        // the quantiser reads hi only: lo goes first, so the codes never raise the handle above its starting bytes.
+        // S is cleared at once: no tensor map over a freed plane outlives this call, even if it fails below.
+        __half* hi = S.hi;
+        void* lo = S.lo;
+        S = SplitOperand{};
+        int rc = release(lo, n * 2);
+        if (rc == RMU_OK) rc = dev_alloc(e->allocs, &Q.codes, n / 2);
+        if (rc == RMU_OK) rc = dev_alloc(e->allocs, &Q.absmax, n / kNf4Block);
+        if (rc != RMU_OK) return rc;
+        delta += n / 2 + n / kNf4Block * 4;
+        peak = std::max(peak, delta);
+        Q.rows = static_cast<int>(shape[w][0]);
+        Q.cols = static_cast<int>(shape[w][1]);
+        rc = launch_nf4_quantize(hi, n, Q.codes, Q.absmax, st);
+        if (rc != RMU_OK) return rc;
+        RMU_CUDA(cudaStreamSynchronize(st));
+        return release(hi, n * 2);
+    };
+    e->nf4_broken = true;                              // until every layer is converted
+    int rc = RMU_OK;
+    for (int l = 0; l < c.layers && rc == RMU_OK; ++l)
+        for (int w = 0; w < 4 && rc == RMU_OK; ++w) rc = convert(e->layers[l], w);
+    // the prefill's scratch, allocated once the split planes are gone: one hi | lo pair as large as the largest weight
+    int64_t most = 0;
+    for (const auto& sh : shape) most = std::max(most, sh[0] * sh[1]);
+    if (rc == RMU_OK) rc = dev_alloc(e->allocs, &e->nf4_hi, most);
+    if (rc == RMU_OK) rc = dev_alloc(e->allocs, &e->nf4_lo, most);
+    if (rc != RMU_OK) return rc;
+    delta += most * 4;
+    peak = std::max(peak, delta);
+    RMU_CUDA(cudaMemset(e->nf4_lo, 0, most * sizeof(__half)));
+    for (int w = 0; w < 4 && rc == RMU_OK; ++w)
+        rc = make_split_operand(&e->nf4_op[w], e->nf4_hi, e->nf4_lo, shape[w][0], static_cast<int>(shape[w][1]));
+    if (rc != RMU_OK) return rc;
+    e->nf4 = true;
+    e->nf4_broken = false;
+    e->nf4_peak = peak;
+    e->nf4_delta = delta;
+    return RMU_OK;
+}
+
 int rmu_decoder_generate(rmu_encoder* e, const int32_t* ids_h, int T, const rmu_sampling* s, uint64_t seed,
                          int max_new_tokens, int32_t* out_h, int32_t* n_out, float* logits_h, void* stream) {
     const std::string fn("rmu_decoder_generate");
@@ -3530,6 +3639,7 @@ int rmu_decoder_generate(rmu_encoder* e, const int32_t* ids_h, int T, const rmu_
                   "with an LM head attached by rmu_decoder_set_lm_head");
         return RMU_ERR_ARG;
     }
+    if (e->nf4_broken) { set_error(fn + ": the handle's NF4 conversion failed part-way; destroy it"); return RMU_ERR_ARG; }
     const rmu_bert_config& c = e->cfg;
     if (T >= c.max_pos) {
         set_error(fn + ": a prompt of " + std::to_string(T) + " tokens leaves no position for a new token (max_position_embeddings " +
@@ -4188,6 +4298,54 @@ int rmu_debug_kv_append(const uint16_t* hi, const uint16_t* lo, int T, int heads
     if (heads % kv_heads != 0) { set_error("rmu_debug_kv_append: heads % kv_heads != 0"); return RMU_ERR_UNSUPPORTED; }
     return launch_kv_append(reinterpret_cast<const __half*>(hi), reinterpret_cast<const __half*>(lo), T, heads, kv_heads,
                             pos0, cap, reinterpret_cast<__half*>(kv), static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_nf4_quantize(const uint16_t* hi, int64_t n, uint8_t* codes, float* absmax, void* stream) {
+    if (!hi || !codes || !absmax || n < 1) { set_error("rmu_debug_nf4_quantize: bad argument"); return RMU_ERR_ARG; }
+    if (n % kNf4Block != 0) { set_error("rmu_debug_nf4_quantize: n % 64 != 0"); return RMU_ERR_UNSUPPORTED; }
+    return launch_nf4_quantize(reinterpret_cast<const __half*>(hi), n, codes, absmax, static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_nf4_dequantize(const uint8_t* codes, const float* absmax, int64_t n, uint16_t* hi, void* stream) {
+    if (!codes || !absmax || !hi || n < 1) { set_error("rmu_debug_nf4_dequantize: bad argument"); return RMU_ERR_ARG; }
+    if (n % kNf4Block != 0) { set_error("rmu_debug_nf4_dequantize: n % 64 != 0"); return RMU_ERR_UNSUPPORTED; }
+    return launch_nf4_dequantize(codes, absmax, n, reinterpret_cast<__half*>(hi), static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_nf4_gemv(int mode, const uint16_t* x_hi, const uint16_t* x_lo, const uint8_t* codes, const float* absmax,
+                       int N, int K, const float* bias, const float* res_f32, float* out_f32, uint16_t* out_hi,
+                       uint16_t* out_lo, int32_t* range_flag, void* stream) {
+    const std::string fn("rmu_debug_nf4_gemv");
+    if (mode != GEMM_BIAS_F32 && mode != GEMM_BIAS_RESF32_F32 && mode != GEMM_BIAS_SWIGLU_SPLIT) {
+        set_error(fn + ": mode must be 0, 6 or 7");
+        return RMU_ERR_ARG;
+    }
+    const bool swiglu = mode == GEMM_BIAS_SWIGLU_SPLIT;
+    if (!x_hi || !x_lo || !codes || !absmax || !bias || N < 1 || K < 1 || (swiglu ? !out_hi || !out_lo : !out_f32) ||
+        (mode == GEMM_BIAS_RESF32_F32 && !res_f32)) {
+        set_error(fn + ": bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (N % 128 != 0 || K % kNf4Block != 0 || K > kNf4MaxK) {
+        set_error(fn + ": N must be a multiple of 128 and K a multiple of 64 up to " + std::to_string(kNf4MaxK));
+        return RMU_ERR_UNSUPPORTED;
+    }
+    GemmParams p{};
+    p.M = 1; p.N = N; p.K = K; p.bias = bias; p.out_f32 = out_f32; p.res_f32 = res_f32;
+    p.out_hi = reinterpret_cast<__half*>(out_hi); p.out_lo = reinterpret_cast<__half*>(out_lo);
+    p.range_flag = reinterpret_cast<int*>(range_flag);
+    Nf4Weight W;
+    W.codes = const_cast<uint8_t*>(codes); W.absmax = const_cast<float*>(absmax); W.rows = N; W.cols = K;
+    return launch_nf4_gemv(mode, reinterpret_cast<const __half*>(x_hi), reinterpret_cast<const __half*>(x_lo), W, p,
+                           device_sm_count(), static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_nf4_conversion(const rmu_encoder* e, int64_t* peak, int64_t* delta) {
+    if (!e || !peak || !delta) { set_error("rmu_debug_nf4_conversion: bad argument"); return RMU_ERR_ARG; }
+    if (!e->nf4) { set_error("rmu_debug_nf4_conversion: the handle's weights are not NF4"); return RMU_ERR_ARG; }
+    *peak = e->nf4_peak;
+    *delta = e->nf4_delta;
+    return RMU_OK;
 }
 
 int rmu_debug_sample(float* logits, int V, uint32_t* presence, const rmu_sampling* s, float u, int32_t* token,

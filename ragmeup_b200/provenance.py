@@ -78,14 +78,25 @@ class DocumentSimilarityAttribution:
 class DecoderAttention:
     """A Llama or Qwen3 decoder (``weights.resolve_decoder``: a snapshot directory or ``synthetic:<preset>``) on the
     GPU, for attention provenance and text generation (``llms.HuggingFacePipeline``).  Its weights are uploaded once;
-    ``span_mass`` then runs one thread per call, and ``generate`` attaches the LM head the first time it runs."""
+    ``span_mass`` then runs one thread per call, and ``generate`` attaches the LM head the first time it runs.
 
-    def __init__(self, model_name: str, device: Optional[int] = None):
+    ``weights="nf4"`` converts the layers' projections to NF4 right after the upload (``rmu_decoder_quantize_nf4``),
+    as the reference's bitsandbytes load holds them; ``"split"`` keeps the fp32-accurate split planes."""
+
+    def __init__(self, model_name: str, device: Optional[int] = None, weights: str = "split"):
         from .encoder import BertEncoder
+        if weights not in DECODER_WEIGHTS:
+            raise ValueError(f"DecoderAttention: weights must be one of {DECODER_WEIGHTS}, got {weights!r}")
         cfg, w = resolve_decoder(model_name)
         self.cfg = cfg
         self.model_name = model_name
+        self.weights = weights
         self.encoder = BertEncoder(cfg, w, with_head=False, device=device)
+        del w
+        if weights == "nf4":
+            enc = self.encoder
+            with enc.torch.cuda.device(enc.device):
+                enc._check(_lib.lib().rmu_decoder_quantize_nf4(enc._h, _lib.stream_ptr()), "rmu_decoder_quantize_nf4")
         self.lock = threading.Lock()
         self._lm_head = False
 
@@ -140,23 +151,39 @@ class DecoderAttention:
         return out[:n.value].tolist()
 
 
-# one decoder per (snapshot, device): compute_attention and llms.HuggingFacePipeline share its weights
+DECODER_WEIGHTS = ("split", "nf4")
+DECODER_WEIGHTS_ENV = "RMU_DECODER_WEIGHTS"
+
+
+def decoder_weights() -> str:
+    """the weights a decoder handle gets: ``$RMU_DECODER_WEIGHTS`` (``split`` or ``nf4``), ``split`` when unset, so
+    the reference's ``.env`` can select NF4 as its own ``BitsAndBytesConfig`` does"""
+    v = os.environ.get(DECODER_WEIGHTS_ENV, "split").strip().lower() or "split"
+    if v not in DECODER_WEIGHTS:
+        raise ValueError(f"{DECODER_WEIGHTS_ENV}={os.environ[DECODER_WEIGHTS_ENV]!r}: expected one of {DECODER_WEIGHTS}")
+    return v
+
+
+# one decoder per (snapshot, device, weights): compute_attention and llms.HuggingFacePipeline share its weights
 _DECODERS: dict = {}
 
 
 def _decoder(model: Any) -> DecoderAttention:
     """``model`` as compute_attention takes it: a DecoderAttention, a model name, or a transformers model whose
-    ``name_or_path`` names a snapshot (found as every other drop-in finds one); one handle per (path, device)"""
+    ``name_or_path`` names a snapshot (found as every other drop-in finds one); one handle per (path, device,
+    ``decoder_weights()``)"""
     if isinstance(model, DecoderAttention):
         return model
     name = model if isinstance(model, str) else getattr(model, "name_or_path", None)
     if not name:
         raise TypeError("compute_attention: model must be a DecoderAttention, a model name or a transformers model with "
                         "name_or_path")
+    weights = decoder_weights()
     torch = _lib.require_cuda()
-    key = (name if name.startswith("synthetic:") else os.path.realpath(find_snapshot(name)), torch.cuda.current_device())
+    key = (name if name.startswith("synthetic:") else os.path.realpath(find_snapshot(name)), torch.cuda.current_device(),
+           weights)
     if key not in _DECODERS:
-        _DECODERS[key] = DecoderAttention(name, device=key[1])
+        _DECODERS[key] = DecoderAttention(name, device=key[1], weights=weights)
     return _DECODERS[key]
 
 

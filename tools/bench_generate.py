@@ -1,6 +1,6 @@
 """Time generation on the Llama-3.1-8B shape (hidden 4096, 32 / 8 heads, F 14336, vocabulary 128 256), in one run:
 
-    python tools/bench_generate.py [--layers 4] [--tokens 32] [--json OUT]
+    python tools/bench_generate.py [--layers 4] [--tokens 32] [--weights split|nf4] [--json OUT]
 
 For prompts of T = 1 024 and 4 096 tokens, greedy, with CUDA events around whole rmu_decoder_generate calls:
 * prefill: a call that generates one token (the prefill, the LM head and the sampler);
@@ -11,6 +11,11 @@ The synthetic model has --layers layers (all 32 are about 32 GB of host fp32); t
 to 32 layers, which is a COMPUTED extrapolation, not a measurement.  The floor it compares against is computed too:
 30.0 GB of split-plane weights read once per token at 3.35 TB/s is at least 9.0 ms per token.  The card's name and
 power limit are read in the same run.
+
+With --weights nf4 the run holds two handles of the same weights, one split and one converted to NF4
+(rmu_decoder_quantize_nf4), and alternates their calls; the NF4 decode step's projections are the "nf4" timer class.
+It also times the decode GEMV alone on one layer's four projections of the full 8B shape (CUDA events over 200
+launches of each) and states the share of 3.35 TB/s that their NF4 bytes (codes and absmax) reach.
 """
 from __future__ import annotations
 
@@ -29,7 +34,8 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 FULL_LAYERS = 32
-PROF = {"gemm": 4, "decode_attention": 11, "lm_head": 12, "sampler": 13}
+PROF = {"gemm": 4, "decode_attention": 11, "lm_head": 12, "sampler": 13, "nf4": 14}
+HBM_TBPS = 3.35
 
 
 def card() -> dict:
@@ -46,11 +52,54 @@ def split_plane_bytes(cfg, layers: int) -> int:
     return 4 * (layers * per_layer + cfg.vocab_size * H)
 
 
+def gemv_share(cfg) -> dict:
+    """the decode GEMV alone on one layer's q | k | v, o, gate | up and down at M = 1 (CUDA events, 200 launches each)"""
+    import torch
+    from ragmeup_b200 import _lib
+    l = _lib.lib()
+    H, F, QD, KD = cfg.hidden, cfg.ffn, cfg.heads * 128, cfg.kv_heads * 128
+    shapes = {"qkv": (0, QD + 2 * KD, H), "o": (6, H, QD), "gate_up": (7, 2 * F, H), "down": (6, H, F)}
+    out, total_ms, total_bytes = {}, 0.0, 0
+    for name, (mode, N, K) in shapes.items():
+        w = (torch.randn(N, K, device="cuda") * 0.02).half()
+        codes = torch.empty(N * K // 2, dtype=torch.uint8, device="cuda")
+        amax = torch.empty(N * K // 64, device="cuda")
+        _lib.check(l.rmu_debug_nf4_quantize(w.data_ptr(), N * K, codes.data_ptr(), amax.data_ptr(), _lib.stream_ptr()))
+        del w
+        x = torch.randn(K, device="cuda").half()
+        bias = torch.zeros(N, device="cuda")
+        res = torch.zeros(N, device="cuda")
+        half = torch.empty(N, dtype=torch.float16, device="cuda")
+
+        def launch():
+            _lib.check(l.rmu_debug_nf4_gemv(mode, x.data_ptr(), x.data_ptr(), codes.data_ptr(), amax.data_ptr(), N, K,
+                                            bias.data_ptr(), res.data_ptr(), res.data_ptr(), half.data_ptr(),
+                                            half.data_ptr(), None, _lib.stream_ptr()))
+        for _ in range(20):
+            launch()
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        for _ in range(200):
+            launch()
+        b.record()
+        torch.cuda.synchronize()
+        ms = a.elapsed_time(b) / 200
+        nbytes = N * K // 2 + N * K // 64 * 4
+        out[name] = {"N": N, "K": K, "us": round(ms * 1e3, 2), "share_of_hbm_peak": round(nbytes / (ms * 1e-3) / (HBM_TBPS * 1e12), 3)}
+        total_ms += ms
+        total_bytes += nbytes
+        del codes, amax
+    out["layer"] = {"us": round(total_ms * 1e3, 2), "nf4_bytes": total_bytes,
+                    "share_of_hbm_peak": round(total_bytes / (total_ms * 1e-3) / (HBM_TBPS * 1e12), 3)}
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--layers", type=int, default=4)
     ap.add_argument("--tokens", type=int, default=32)
     ap.add_argument("--calls", type=int, default=3)
+    ap.add_argument("--weights", choices=("split", "nf4"), default="split")
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
@@ -59,13 +108,19 @@ def main():
     from ragmeup_b200.weights import DECODER_PRESETS, LlamaConfig, synthetic_llama_weights
 
     cfg = replace(LlamaConfig(**asdict(DECODER_PRESETS["llama-3.1-8b"])), layers=args.layers, name="llama-3.1-8b")
-    enc = BertEncoder(cfg, synthetic_llama_weights(cfg, seed=0), with_head=False)
     l = _lib.lib()
+    w = synthetic_llama_weights(cfg, seed=0)
     lm = (0.02 * np.random.default_rng(1).standard_normal((cfg.vocab_size, cfg.hidden))).astype(np.float32)
-    _lib.check(l.rmu_decoder_set_lm_head(enc._h, lm.ctypes.data), "rmu_decoder_set_lm_head")
-    del lm
+    handles = {}
+    for kind in (("split", "nf4") if args.weights == "nf4" else ("split",)):
+        enc = BertEncoder(cfg, w, with_head=False)
+        _lib.check(l.rmu_decoder_set_lm_head(enc._h, lm.ctypes.data), "rmu_decoder_set_lm_head")
+        if kind == "nf4":
+            _lib.check(l.rmu_decoder_quantize_nf4(enc._h, _lib.stream_ptr()), "rmu_decoder_quantize_nf4")
+        handles[kind] = enc
+    del lm, w
     s = _lib.SamplingC(0, 1.0, 1.0, 1.0, 50, 0, (C.c_int32 * _lib.MAX_EOS)())
-    res = {"card": card(), "shape": "llama-3.1-8b", "layers": cfg.layers, "rows": []}
+    res = {"card": card(), "shape": "llama-3.1-8b", "layers": cfg.layers, "weights": list(handles), "rows": []}
     print(json.dumps(res["card"]))
     full_gb = split_plane_bytes(cfg, FULL_LAYERS) / 1e9
     res["floor"] = {"split_plane_gb_32_layers_computed": round(full_gb, 2),
@@ -77,7 +132,7 @@ def main():
         out = np.zeros(args.tokens + 1, dtype=np.int32)
         n = C.c_int32(0)
 
-        def call(k):
+        def call(k, enc):
             t0 = time.perf_counter()
             enc._check(l.rmu_decoder_generate(enc._h, ids.ctypes.data, T, C.byref(s), 0, k, out.ctypes.data, C.byref(n),
                                               None, _lib.stream_ptr()), "rmu_decoder_generate")
@@ -85,29 +140,42 @@ def main():
             assert n.value == k
             return (time.perf_counter() - t0) * 1e3
 
-        call(args.tokens + 1)                                     # warm-up: cache and workspace growth, module load
-        one = statistics.median(call(1) for _ in range(args.calls))
-        many = statistics.median(call(args.tokens + 1) for _ in range(args.calls))
-        per_tok = (many - one) / args.tokens
-        parts = {}
-        for k in (1, args.tokens + 1):
-            l.rmu_profile_reset()
-            l.rmu_profile_enable(1)
-            call(k)
-            l.rmu_profile_enable(0)
-            for name, cls in PROF.items():
-                ms, cnt = C.c_double(), C.c_int64()
-                l.rmu_profile_read(cls, C.byref(ms), C.byref(cnt))
-                parts[name] = parts.get(name, 0.0) + (ms.value if k > 1 else -ms.value)
-        step = {k: v / args.tokens for k, v in parts.items()}
-        step["projections"] = step.pop("gemm") - step["lm_head"]
-        scale = FULL_LAYERS / cfg.layers
-        row = {"T": T, "prefill_ms": round(one, 3), "ms_per_token": round(per_tok, 3),
-               "step_ms": {k: round(v, 3) for k, v in step.items()},
-               "ms_per_token_32_layers_extrapolated": round(step["lm_head"] + step["sampler"] +
-                                                            scale * (per_tok - step["lm_head"] - step["sampler"]), 3)}
-        res["rows"].append(row)
-        print(json.dumps(row))
+        for enc in handles.values():
+            call(args.tokens + 1, enc)                            # warm-up: cache and workspace growth, module load
+        ones, manys = {k: [] for k in handles}, {k: [] for k in handles}
+        for _ in range(args.calls):                               # the handles alternate call by call
+            for kind, enc in handles.items():
+                ones[kind].append(call(1, enc))
+            for kind, enc in handles.items():
+                manys[kind].append(call(args.tokens + 1, enc))
+        for kind, enc in handles.items():
+            one, many = statistics.median(ones[kind]), statistics.median(manys[kind])
+            per_tok = (many - one) / args.tokens
+            parts = {}
+            for k in (1, args.tokens + 1):
+                l.rmu_profile_reset()
+                l.rmu_profile_enable(1)
+                call(k, enc)
+                l.rmu_profile_enable(0)
+                for name, cls in PROF.items():
+                    ms, cnt = C.c_double(), C.c_int64()
+                    l.rmu_profile_read(cls, C.byref(ms), C.byref(cnt))
+                    parts[name] = parts.get(name, 0.0) + (ms.value if k > 1 else -ms.value)
+            step = {k: v / args.tokens for k, v in parts.items()}
+            step["projections"] = step.pop("gemm") - step["lm_head"] + step.pop("nf4")
+            scale = FULL_LAYERS / cfg.layers
+            row = {"weights": kind, "T": T, "prefill_ms": round(one, 3), "ms_per_token": round(per_tok, 3),
+                   "step_ms": {k: round(v, 3) for k, v in step.items()},
+                   "ms_per_token_32_layers_extrapolated": round(step["lm_head"] + step["sampler"] +
+                                                                scale * (per_tok - step["lm_head"] - step["sampler"]), 3)}
+            res["rows"].append(row)
+            print(json.dumps(row))
+    if "nf4" in handles:
+        handles.clear()
+        import gc
+        gc.collect()
+        res["nf4_gemv"] = gemv_share(cfg)
+        print(json.dumps(res["nf4_gemv"]))
     if args.json:
         with open(args.json, "w") as f:
             json.dump(res, f, indent=1)
