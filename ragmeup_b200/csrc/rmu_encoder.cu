@@ -732,32 +732,28 @@ __global__ void join_planes_kernel(const __half* __restrict__ hi, const __half* 
 // per CTA only four warps per SM would issue it, so four warps stage and warp 0 computes.
 constexpr int kClsAttWarps = 4;
 
-// E2 on the QKV planes [T, 3H] (q pre-scaled by log2(e) / sqrt(d_h)) of a ragged batch -> ctx planes [T, H].
-// warps = 10 (160-row CTAs).
+// E2 on the QKV planes [T, 3H] (q pre-scaled by log2(e) / sqrt(d_h)) of a ragged batch -> ctx planes [T, H], in
+// kAttWarps-warp (160-row) CTAs.
 // cls_q_hi / cls_q_lo non-null: query row 0 of each sequence only, q from those compact planes [B, H] -> ctx [B, H]
-// (the K / V columns of the QKV planes are read as above; their Q columns are not); `warps` is ignored.
+// (the K / V columns of the QKV planes are read as above; their Q columns are not), in kClsAttWarps-warp CTAs.
 // The sequence index is gridDim.y, at most 65 535: a larger batch runs in slices of 65 535 sequences, each launch with
 // cu (and in CLS mode the compact Q and context rows) offset by the slice start.  Within a slice the grid and the
 // kernel are those of one launch, so the heads of a sequence still run together and every row is computed the same.
-// rel_bias non-null: the [heads, kRelSpan] table of build_relative_bias_table is added to every score (warps must be 10).
+// rel_bias non-null: the [heads, kRelSpan] table of build_relative_bias_table is added to every score.
 // nkeys non-null ([B] int32, full mode without a bias): sequence b attends to its first min(max(nkeys[b], 1), S_b) rows.
 // dis non-null (DeBERTa-v2, d_h = 64, neither a bias nor a key limit): the position terms of launch_position_terms are
-// added to every score (warps must be 10); in CLS mode its c2p rows are the compact CLS rows, offset here per slice.
-// window > 0 (ModernBERT's local layers; full mode, 10 warps, none of the above): key j is visible to query i iff
+// added to every score; in CLS mode its c2p rows are the compact CLS rows, offset here per slice.
+// window > 0 (ModernBERT's local layers; full mode, none of the above): key j is visible to query i iff
 // |i - j| <= window (the Window pack).
 constexpr int kMaxGridY = 65535;
 static int launch_attention(const __half* qkv_hi, const __half* qkv_lo, const __half* cls_q_hi, const __half* cls_q_lo,
-                            const int* cu, int B, int H, int heads, int max_seqlen, int warps, __half* ctx_hi,
-                            __half* ctx_lo, cudaStream_t st, const float* rel_bias = nullptr, const int* nkeys = nullptr,
+                            const int* cu, int B, int H, int heads, int max_seqlen, __half* ctx_hi, __half* ctx_lo,
+                            cudaStream_t st, const float* rel_bias = nullptr, const int* nkeys = nullptr,
                             const Disentangled* dis = nullptr, int window = 0) {
     const int DH = H / heads;
     const bool cls = cls_q_hi != nullptr;
     const bool bias = rel_bias != nullptr;
-    if (cls) warps = kClsAttWarps;
-    else if (warps != kAttWarps) {
-        set_error("attention: warps must be 10");
-        return RMU_ERR_ARG;
-    }
+    const int warps = cls ? kClsAttWarps : kAttWarps;
     if (nkeys && (cls || bias)) {
         set_error("attention: a key limit runs on every query row and without a relative bias");
         return RMU_ERR_ARG;
@@ -1079,8 +1075,8 @@ static int run_disentangled_attention(const __half* qkv_hi, const __half* qkv_lo
     rc = launch_position_terms(qkv_hi + H, qkv_lo + H, ld3, T, pos_hi, pos_lo, p_ld, heads, DH, c0, W, p2c, st);
     if (rc != RMU_OK) return rc;
     const Disentangled dis{c2p, p2c, cidx_d, rmax, c0, W};
-    return launch_attention(qkv_hi, qkv_lo, cls_q_hi, cls_q_lo, cu, B, H, heads, max_seqlen, kAttWarps, ctx_hi, ctx_lo, st,
-                            nullptr, nullptr, &dis);
+    return launch_attention(qkv_hi, qkv_lo, cls_q_hi, cls_q_lo, cu, B, H, heads, max_seqlen, ctx_hi, ctx_lo, st, nullptr,
+                            nullptr, &dis);
 }
 
 // floats of run_disentangled_attention's workspace
@@ -1348,12 +1344,150 @@ __global__ void __launch_bounds__(256) last_token_kernel(const float* __restrict
 // heads.  Warp w computes query head w % hpc on rows 16 (w / hpc) .. + 15 of the block.  The keys run in blocks of
 // kCausalKB through shared memory with an online softmax, so any length runs; a warp stops at its rows' diagonal and
 // masks j > i in the block that crosses it.  Every block a warp reads holds a key <= each of its rows (blocks start at
-// multiples of 32, its rows at a multiple of 16), so a row's running max is finite after the first block.
+// multiples of 32, its rows at a multiple of 16), so a row's running max is finite after the first block.  The span
+// kernels below compute the same scores: they share the CTA layout (CausalCta), the q fragments (load_q_frags), the
+// staging (stage_keys) and the products and mask (score_block) with this kernel.
 // ---------------------------------------------------------------------------------------------------
 constexpr int kCausalWarps = 8;
 constexpr int kCausalKB = 64;                 // keys staged per step
 constexpr int kCausalKSTR = kQwenHD + 8;      // staging row pitch in halves: conflict-free ldmatrix rows
 constexpr size_t kCausalSmem = 4 * sizeof(__half) * static_cast<size_t>(kCausalKB) * kCausalKSTR;
+
+// The causal CTA layout of attention_causal_kernel and the span kernels, over one sequence of T rows: grid x = kvh *
+// (G / hpc) + sub for kv head kvh, grid z = the block of 16 rb query rows from rbase; kend bounds the keys any row of
+// the CTA can see.  The warp computes query head qh() on rows r0() .. + 15; it is live when it has a query head and its
+// rows start before T.  The warp's coordinates are methods, computed where a kernel uses them (after the span kernels'
+// early exit).
+struct CausalCta {
+    int hpc, T, G, subs, rb, kvh, sub, rbase;
+    __device__ __forceinline__ CausalCta(int heads, int kv_heads, int hpc_, int T_)
+        : hpc(hpc_), T(T_), G(heads / kv_heads), subs(G / hpc), rb(kCausalWarps / hpc), kvh(blockIdx.x / subs),
+          sub(blockIdx.x % subs), rbase(blockIdx.z * 16 * rb) {}
+    __device__ __forceinline__ int kend() const { return min(T, rbase + 16 * rb); }
+    __device__ __forceinline__ static int warp() { return threadIdx.x >> 5; }
+    __device__ __forceinline__ int qh() const { return kvh * G + sub * hpc + warp() % hpc; }
+    __device__ __forceinline__ int r0() const { return rbase + 16 * (warp() / hpc); }
+    __device__ __forceinline__ bool warp_live() const { return warp() < hpc * rb && r0() < T; }
+};
+
+// v reduced over the quad of lanes that share an mma row (lanes 4g .. 4g + 3)
+__device__ __forceinline__ float quad_max(float v) {
+    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+    return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// the warp's q fragments of rows r0 .. r0 + 15 of head qh (zero past T) in the sequence whose rows start at row t0
+__device__ __forceinline__ void load_q_frags(const __half* ph, const __half* pl, size_t ld, int t0, int qh, int r0, int T,
+                                             bool live, uint32_t (&qhf)[kQwenHD / 16][4], uint32_t (&qlf)[kQwenHD / 16][4]) {
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const __half* qhb = ph + static_cast<size_t>(t0) * ld + qh * kQwenHD;
+    const __half* qlb = pl + static_cast<size_t>(t0) * ld + qh * kQwenHD;
+    const int ra = r0 + g, rc = r0 + g + 8;
+#pragma unroll
+    for (int ks = 0; ks < kQwenHD / 16; ++ks) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { qhf[ks][i] = 0u; qlf[ks][i] = 0u; }
+        if (live && ra < T) {
+            qhf[ks][0] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t);
+            qlf[ks][0] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t);
+            qhf[ks][2] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t + 8);
+            qlf[ks][2] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t + 8);
+        }
+        if (live && rc < T) {
+            qhf[ks][1] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t);
+            qlf[ks][1] = *reinterpret_cast<const uint32_t*>(qlb + rc * ld + ks * 16 + 2 * t);
+            qhf[ks][3] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t + 8);
+            qlf[ks][3] = *reinterpret_cast<const uint32_t*>(qlb + rc * ld + ks * 16 + 2 * t + 8);
+        }
+    }
+}
+
+// stage keys [sb0, sb0 + kCausalKB) of the sequence whose rows start at row t0, kv column kcol, into Kh / Kl, zeros
+// from key `bound` on; kWithV: the values of column vcol go into Vh / Vl in the same loop.  The caller synchronises
+// around it.
+template <bool kWithV = false>
+__device__ __forceinline__ void stage_keys(const __half* ph, const __half* pl, size_t ld, int t0, size_t kcol, int sb0,
+                                           int bound, __half* Kh, __half* Kl, size_t vcol = 0, __half* Vh = nullptr,
+                                           __half* Vl = nullptr) {
+    const int nk = min(kCausalKB, bound - sb0);
+    for (int e = threadIdx.x; e < kCausalKB * (kQwenHD / 8); e += blockDim.x) {
+        const int j = e / (kQwenHD / 8), c8 = (e % (kQwenHD / 8)) * 8;
+        uint4 kh = make_uint4(0, 0, 0, 0), kl = kh, vh = kh, vl = kh;
+        if (j < nk) {
+            const size_t o = static_cast<size_t>(t0 + sb0 + j) * ld + c8;
+            kh = *reinterpret_cast<const uint4*>(ph + o + kcol);
+            kl = *reinterpret_cast<const uint4*>(pl + o + kcol);
+            if (kWithV) {
+                vh = *reinterpret_cast<const uint4*>(ph + o + vcol);
+                vl = *reinterpret_cast<const uint4*>(pl + o + vcol);
+            }
+        }
+        *reinterpret_cast<uint4*>(Kh + j * kCausalKSTR + c8) = kh;
+        *reinterpret_cast<uint4*>(Kl + j * kCausalKSTR + c8) = kl;
+        if (kWithV) {
+            *reinterpret_cast<uint4*>(Vh + j * kCausalKSTR + c8) = vh;
+            *reinterpret_cast<uint4*>(Vl + j * kCausalKSTR + c8) = vl;
+        }
+    }
+}
+
+// s[n][.] = the warp's 16 x 32 base-2 scores (hi*hi + lo*hi + hi*lo) against the staged keys kb0 .. kb0 + 31, which
+// are keys j0 .. j0 + 31 of the sequence; keys j > row are masked to -inf
+__device__ __forceinline__ void score_block(const uint32_t (&qhf)[kQwenHD / 16][4], const uint32_t (&qlf)[kQwenHD / 16][4],
+                                            const __half* Kh, const __half* Kl, int kb0, int j0, int r0,
+                                            float (&sacc)[4][4]) {
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+#pragma unroll
+    for (int n = 0; n < 4; ++n) sacc[n][0] = sacc[n][1] = sacc[n][2] = sacc[n][3] = 0.f;
+#pragma unroll
+    for (int ks = 0; ks < kQwenHD / 16; ++ks) {
+        uint32_t bh[4][2], bl[4][2];
+        const int lrow = (lane & 7) + ((lane >> 4) << 3);
+        const int lcol = ks * 16 + ((lane >> 3) & 1) * 8;
+#pragma unroll
+        for (int n2 = 0; n2 < 2; ++n2) {
+            uint32_t th[4], tl[4];
+            ldmatrix_x4(th, Kh + (kb0 + n2 * 16 + lrow) * kCausalKSTR + lcol);
+            ldmatrix_x4(tl, Kl + (kb0 + n2 * 16 + lrow) * kCausalKSTR + lcol);
+            bh[2 * n2][0] = th[0]; bh[2 * n2][1] = th[1]; bh[2 * n2 + 1][0] = th[2]; bh[2 * n2 + 1][1] = th[3];
+            bl[2 * n2][0] = tl[0]; bl[2 * n2][1] = tl[1]; bl[2 * n2 + 1][0] = tl[2]; bl[2 * n2 + 1][1] = tl[3];
+        }
+#pragma unroll
+        for (int n = 0; n < 4; ++n) mma16816(sacc[n], qhf[ks], bh[n]);
+#pragma unroll
+        for (int n = 0; n < 4; ++n) mma16816(sacc[n], qlf[ks], bh[n]);
+#pragma unroll
+        for (int n = 0; n < 4; ++n) mma16816(sacc[n], qhf[ks], bl[n]);
+    }
+    if (j0 + 31 > r0) {
+#pragma unroll
+        for (int n = 0; n < 4; ++n) {
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const int j = j0 + n * 8 + 2 * t + c;
+                if (j > r0 + g) sacc[n][c] = -INFINITY;
+                if (j > r0 + g + 8) sacc[n][2 + c] = -INFINITY;
+            }
+        }
+    }
+}
+
+// the block maxima of the thread's rows g (bm0) and g + 8 (bm1) in a score block
+__device__ __forceinline__ void block_row_max(const float (&sacc)[4][4], float& bm0, float& bm1) {
+    bm0 = -INFINITY;
+    bm1 = -INFINITY;
+#pragma unroll
+    for (int n = 0; n < 4; ++n) {
+        bm0 = fmaxf(bm0, fmaxf(sacc[n][0], sacc[n][1]));
+        bm1 = fmaxf(bm1, fmaxf(sacc[n][2], sacc[n][3]));
+    }
+    bm0 = quad_max(bm0);
+    bm1 = quad_max(bm1);
+}
 
 __global__ void __launch_bounds__(kCausalWarps * 32, 1) attention_causal_kernel(const __half* __restrict__ ph,
                                                                                  const __half* __restrict__ pl,
@@ -1368,115 +1502,35 @@ __global__ void __launch_bounds__(kCausalWarps * 32, 1) attention_causal_kernel(
     __half* Vh = Kl + kCausalKB * KSTR;
     __half* Vl = Vh + kCausalKB * KSTR;
 
-    const int G = heads / kv_heads, subs = G / hpc, rb = kCausalWarps / hpc;
-    const int kvh = blockIdx.x / subs, sub = blockIdx.x % subs;
     const int b = blockIdx.y;
     const int t0 = cu[b], S = cu[b + 1] - t0;
-    const int rbase = blockIdx.z * 16 * rb;
-    if (rbase >= S) return;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const CausalCta c(heads, kv_heads, hpc, S);
+    if (c.rbase >= S) return;
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
     const size_t ld = static_cast<size_t>(heads + 2 * kv_heads) * DH;
-    const size_t kcol = static_cast<size_t>(heads + kvh) * DH, vcol = static_cast<size_t>(heads + kv_heads + kvh) * DH;
-    const int qh = kvh * G + sub * hpc + warp % hpc;
-    const int r0 = rbase + 16 * (warp / hpc);
-    const bool warp_live = warp < hpc * rb && r0 < S;
+    const size_t kcol = static_cast<size_t>(heads + c.kvh) * DH, vcol = static_cast<size_t>(heads + kv_heads + c.kvh) * DH;
+    const int qh = c.qh(), r0 = c.r0();
+    const bool warp_live = c.warp_live();
 
     uint32_t qhf[KS][4], qlf[KS][4];
-    {
-        const __half* qhb = ph + static_cast<size_t>(t0) * ld + qh * DH;
-        const __half* qlb = pl + static_cast<size_t>(t0) * ld + qh * DH;
-        const int ra = r0 + g, rc = r0 + g + 8;
-#pragma unroll
-        for (int ks = 0; ks < KS; ++ks) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) { qhf[ks][i] = 0u; qlf[ks][i] = 0u; }
-            if (warp_live && ra < S) {
-                qhf[ks][0] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t);
-                qlf[ks][0] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t);
-                qhf[ks][2] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t + 8);
-                qlf[ks][2] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t + 8);
-            }
-            if (warp_live && rc < S) {
-                qhf[ks][1] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t);
-                qlf[ks][1] = *reinterpret_cast<const uint32_t*>(qlb + rc * ld + ks * 16 + 2 * t);
-                qhf[ks][3] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t + 8);
-                qlf[ks][3] = *reinterpret_cast<const uint32_t*>(qlb + rc * ld + ks * 16 + 2 * t + 8);
-            }
-        }
-    }
+    load_q_frags(ph, pl, ld, t0, qh, r0, S, warp_live, qhf, qlf);
     float oacc[NT][4];
 #pragma unroll
     for (int n = 0; n < NT; ++n) oacc[n][0] = oacc[n][1] = oacc[n][2] = oacc[n][3] = 0.f;
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
 
-    const int kend = min(S, rbase + 16 * rb);       // keys any row of the CTA can see
+    const int kend = c.kend();
     for (int sb0 = 0; sb0 < kend; sb0 += kCausalKB) {
-        const int nk = min(kCausalKB, kend - sb0);
         __syncthreads();
-        for (int e = threadIdx.x; e < kCausalKB * (DH / 8); e += blockDim.x) {
-            const int j = e / (DH / 8), c8 = (e % (DH / 8)) * 8;
-            uint4 kh = make_uint4(0, 0, 0, 0), kl = kh, vh = kh, vl = kh;
-            if (j < nk) {
-                const size_t o = static_cast<size_t>(t0 + sb0 + j) * ld + c8;
-                kh = *reinterpret_cast<const uint4*>(ph + o + kcol);
-                kl = *reinterpret_cast<const uint4*>(pl + o + kcol);
-                vh = *reinterpret_cast<const uint4*>(ph + o + vcol);
-                vl = *reinterpret_cast<const uint4*>(pl + o + vcol);
-            }
-            *reinterpret_cast<uint4*>(Kh + j * KSTR + c8) = kh;
-            *reinterpret_cast<uint4*>(Kl + j * KSTR + c8) = kl;
-            *reinterpret_cast<uint4*>(Vh + j * KSTR + c8) = vh;
-            *reinterpret_cast<uint4*>(Vl + j * KSTR + c8) = vl;
-        }
+        stage_keys<true>(ph, pl, ld, t0, kcol, sb0, kend, Kh, Kl, vcol, Vh, Vl);
         __syncthreads();
         if (!warp_live) continue;
         for (int kb0 = 0; kb0 < kCausalKB; kb0 += 32) {
             const int j0 = sb0 + kb0;
             if (j0 > r0 + 15) break;                      // above the diagonal of every row of the warp
-            float sacc[4][4];
-#pragma unroll
-            for (int n = 0; n < 4; ++n) sacc[n][0] = sacc[n][1] = sacc[n][2] = sacc[n][3] = 0.f;
-#pragma unroll
-            for (int ks = 0; ks < KS; ++ks) {
-                uint32_t bh[4][2], bl[4][2];
-                const int lrow = (lane & 7) + ((lane >> 4) << 3);
-                const int lcol = ks * 16 + ((lane >> 3) & 1) * 8;
-#pragma unroll
-                for (int n2 = 0; n2 < 2; ++n2) {
-                    uint32_t th[4], tl[4];
-                    ldmatrix_x4(th, Kh + (kb0 + n2 * 16 + lrow) * KSTR + lcol);
-                    ldmatrix_x4(tl, Kl + (kb0 + n2 * 16 + lrow) * KSTR + lcol);
-                    bh[2 * n2][0] = th[0]; bh[2 * n2][1] = th[1]; bh[2 * n2 + 1][0] = th[2]; bh[2 * n2 + 1][1] = th[3];
-                    bl[2 * n2][0] = tl[0]; bl[2 * n2][1] = tl[1]; bl[2 * n2 + 1][0] = tl[2]; bl[2 * n2 + 1][1] = tl[3];
-                }
-#pragma unroll
-                for (int n = 0; n < 4; ++n) mma16816(sacc[n], qhf[ks], bh[n]);
-#pragma unroll
-                for (int n = 0; n < 4; ++n) mma16816(sacc[n], qlf[ks], bh[n]);
-#pragma unroll
-                for (int n = 0; n < 4; ++n) mma16816(sacc[n], qhf[ks], bl[n]);
-            }
-            if (j0 + 31 > r0) {                            // the block crosses the diagonal: key j > row i is masked
-#pragma unroll
-                for (int n = 0; n < 4; ++n) {
-#pragma unroll
-                    for (int c = 0; c < 2; ++c) {
-                        const int j = j0 + n * 8 + 2 * t + c;
-                        if (j > r0 + g) sacc[n][c] = -INFINITY;
-                        if (j > r0 + g + 8) sacc[n][2 + c] = -INFINITY;
-                    }
-                }
-            }
-            float bm0 = -INFINITY, bm1 = -INFINITY;
-#pragma unroll
-            for (int n = 0; n < 4; ++n) {
-                bm0 = fmaxf(bm0, fmaxf(sacc[n][0], sacc[n][1]));
-                bm1 = fmaxf(bm1, fmaxf(sacc[n][2], sacc[n][3]));
-            }
-            bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 1));
-            bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 2));
-            bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 1));
-            bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 2));
+            float sacc[4][4], bm0, bm1;
+            score_block(qhf, qlf, Kh, Kl, kb0, j0, r0, sacc);
+            block_row_max(sacc, bm0, bm1);
             const float mn0 = fmaxf(m0, bm0), mn1 = fmaxf(m1, bm1);
             const float c0 = fast_exp2(m0 - mn0), c1 = fast_exp2(m1 - mn1);
             m0 = mn0; m1 = mn1;
@@ -1520,10 +1574,8 @@ __global__ void __launch_bounds__(kCausalWarps * 32, 1) attention_causal_kernel(
         }
     }
     if (!warp_live) return;
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    l0 = quad_sum(l0);
+    l1 = quad_sum(l1);
     const float i0 = 1.0f / l0, i1 = 1.0f / l1;
     const int ra = r0 + g, rc = r0 + g + 8;
     const size_t cld = static_cast<size_t>(heads) * DH;
@@ -1544,11 +1596,20 @@ __global__ void __launch_bounds__(kCausalWarps * 32, 1) attention_causal_kernel(
     }
 }
 
-// query heads per CTA for a group of G: all of them up to 8, else the largest divisor of G up to 8
-static int causal_heads_per_cta(int G) {
-    int h = std::min(G, kCausalWarps);
-    while (G % h != 0) --h;
-    return h;
+// the causal layout's grid for sequences of up to T rows: hpc query heads per CTA (all of a group of G = heads /
+// kv_heads up to 8, else the largest divisor of G up to 8), x = kv_heads * G / hpc CTAs, z = blocks of 16 * (8 / hpc)
+// rows
+struct CausalGrid {
+    int hpc;
+    unsigned x, z;
+};
+
+static CausalGrid causal_grid(int heads, int kv_heads, int T) {
+    const int G = heads / kv_heads;
+    int hpc = std::min(G, kCausalWarps);
+    while (G % hpc != 0) --hpc;
+    const int rows = 16 * (kCausalWarps / hpc);
+    return {hpc, static_cast<unsigned>(kv_heads * (G / hpc)), static_cast<unsigned>((T + rows - 1) / rows)};
 }
 
 // E3 rms_split_kernel over T rows of H (H % 128 == 0, H <= 4096)
@@ -1602,16 +1663,15 @@ static int launch_last_token(const float* x, const int* ids, const int* cu, int 
 // in slices, each launch with cu offset by the slice start (the token rows stay absolute)
 static int launch_attention_causal(const __half* qkv_hi, const __half* qkv_lo, const int* cu, int B, int heads, int kv_heads,
                                    int max_seqlen, __half* ctx_hi, __half* ctx_lo, cudaStream_t st) {
-    const int G = heads / kv_heads, hpc = causal_heads_per_cta(G), rows = 16 * (kCausalWarps / hpc);
+    const CausalGrid cg = causal_grid(heads, kv_heads, max_seqlen);
     ProfScope _ps(PROF_ATTN, st);
     RMU_CUDA(cudaFuncSetAttribute(attention_causal_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kCausalSmem)));
-    const unsigned zb = static_cast<unsigned>((max_seqlen + rows - 1) / rows);
     for (int s0 = 0; s0 < B; s0 += kMaxGridY) {
         const int nb = std::min(kMaxGridY, B - s0);
-        dim3 grid(static_cast<unsigned>(kv_heads * (G / hpc)), static_cast<unsigned>(nb), zb);
-        attention_causal_kernel<<<grid, kCausalWarps * 32, kCausalSmem, st>>>(qkv_hi, qkv_lo, cu + s0, heads, kv_heads, hpc,
-                                                                              ctx_hi, ctx_lo);
+        const dim3 grid(cg.x, static_cast<unsigned>(nb), cg.z);
+        attention_causal_kernel<<<grid, kCausalWarps * 32, kCausalSmem, st>>>(qkv_hi, qkv_lo, cu + s0, heads, kv_heads,
+                                                                              cg.hpc, ctx_hi, ctx_lo);
         count_launch();
         RMU_CHECK_LAUNCH();
     }
@@ -1653,90 +1713,6 @@ __device__ __forceinline__ int rows_meet_spans(const int* spans, int n, int T, i
     return __syncthreads_or(hit);
 }
 
-// the warp's q fragments of rows r0 .. r0 + 15 of head qh (zero past T), as attention_causal_kernel loads them
-__device__ __forceinline__ void load_q_frags(const __half* ph, const __half* pl, size_t ld, int qh, int r0, int T, bool live,
-                                             uint32_t (&qhf)[kQwenHD / 16][4], uint32_t (&qlf)[kQwenHD / 16][4]) {
-    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    const __half* qhb = ph + qh * kQwenHD;
-    const __half* qlb = pl + qh * kQwenHD;
-    const int ra = r0 + g, rc = r0 + g + 8;
-#pragma unroll
-    for (int ks = 0; ks < kQwenHD / 16; ++ks) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { qhf[ks][i] = 0u; qlf[ks][i] = 0u; }
-        if (live && ra < T) {
-            qhf[ks][0] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t);
-            qlf[ks][0] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t);
-            qhf[ks][2] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t + 8);
-            qlf[ks][2] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t + 8);
-        }
-        if (live && rc < T) {
-            qhf[ks][1] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t);
-            qlf[ks][1] = *reinterpret_cast<const uint32_t*>(qlb + rc * ld + ks * 16 + 2 * t);
-            qhf[ks][3] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t + 8);
-            qlf[ks][3] = *reinterpret_cast<const uint32_t*>(qlb + rc * ld + ks * 16 + 2 * t + 8);
-        }
-    }
-}
-
-// stage keys [sb0, sb0 + kCausalKB) of kv column kcol into Kh / Kl (zeros past T); the caller synchronises around it
-__device__ __forceinline__ void stage_keys(const __half* ph, const __half* pl, size_t ld, size_t kcol, int sb0, int T,
-                                           __half* Kh, __half* Kl) {
-    const int nk = min(kCausalKB, T - sb0);
-    for (int e = threadIdx.x; e < kCausalKB * (kQwenHD / 8); e += blockDim.x) {
-        const int j = e / (kQwenHD / 8), c8 = (e % (kQwenHD / 8)) * 8;
-        uint4 kh = make_uint4(0, 0, 0, 0), kl = kh;
-        if (j < nk) {
-            const size_t o = static_cast<size_t>(sb0 + j) * ld + kcol + c8;
-            kh = *reinterpret_cast<const uint4*>(ph + o);
-            kl = *reinterpret_cast<const uint4*>(pl + o);
-        }
-        *reinterpret_cast<uint4*>(Kh + j * kCausalKSTR + c8) = kh;
-        *reinterpret_cast<uint4*>(Kl + j * kCausalKSTR + c8) = kl;
-    }
-}
-
-// s[n][.] = the warp's 16 x 32 base-2 scores against staged keys kb0 .. kb0 + 31, keys j > row masked to -inf
-// (attention_causal_kernel's products and mask)
-__device__ __forceinline__ void score_block(const uint32_t (&qhf)[kQwenHD / 16][4], const uint32_t (&qlf)[kQwenHD / 16][4],
-                                            const __half* Kh, const __half* Kl, int kb0, int j0, int r0,
-                                            float (&sacc)[4][4]) {
-    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-#pragma unroll
-    for (int n = 0; n < 4; ++n) sacc[n][0] = sacc[n][1] = sacc[n][2] = sacc[n][3] = 0.f;
-#pragma unroll
-    for (int ks = 0; ks < kQwenHD / 16; ++ks) {
-        uint32_t bh[4][2], bl[4][2];
-        const int lrow = (lane & 7) + ((lane >> 4) << 3);
-        const int lcol = ks * 16 + ((lane >> 3) & 1) * 8;
-#pragma unroll
-        for (int n2 = 0; n2 < 2; ++n2) {
-            uint32_t th[4], tl[4];
-            ldmatrix_x4(th, Kh + (kb0 + n2 * 16 + lrow) * kCausalKSTR + lcol);
-            ldmatrix_x4(tl, Kl + (kb0 + n2 * 16 + lrow) * kCausalKSTR + lcol);
-            bh[2 * n2][0] = th[0]; bh[2 * n2][1] = th[1]; bh[2 * n2 + 1][0] = th[2]; bh[2 * n2 + 1][1] = th[3];
-            bl[2 * n2][0] = tl[0]; bl[2 * n2][1] = tl[1]; bl[2 * n2 + 1][0] = tl[2]; bl[2 * n2 + 1][1] = tl[3];
-        }
-#pragma unroll
-        for (int n = 0; n < 4; ++n) mma16816(sacc[n], qhf[ks], bh[n]);
-#pragma unroll
-        for (int n = 0; n < 4; ++n) mma16816(sacc[n], qlf[ks], bh[n]);
-#pragma unroll
-        for (int n = 0; n < 4; ++n) mma16816(sacc[n], qhf[ks], bl[n]);
-    }
-    if (j0 + 31 > r0) {
-#pragma unroll
-        for (int n = 0; n < 4; ++n) {
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                const int j = j0 + n * 8 + 2 * t + c;
-                if (j > r0 + g) sacc[n][c] = -INFINITY;
-                if (j > r0 + g + 8) sacc[n][2 + c] = -INFINITY;
-            }
-        }
-    }
-}
-
 // A: grid (kv_heads * G / hpc, 1, row blocks of 16 rb rows), kCausalWarps warps; m / l [heads, T]
 __global__ void __launch_bounds__(kCausalWarps * 32, 1) spans_rowstat_kernel(const __half* __restrict__ ph,
                                                                               const __half* __restrict__ pl, int T,
@@ -1747,40 +1723,27 @@ __global__ void __launch_bounds__(kCausalWarps * 32, 1) spans_rowstat_kernel(con
     extern __shared__ __align__(16) unsigned char span_smem[];
     __half* Kh = reinterpret_cast<__half*>(span_smem);
     __half* Kl = Kh + kCausalKB * kCausalKSTR;
-    const int G = heads / kv_heads, subs = G / hpc, rb = kCausalWarps / hpc;
-    const int kvh = blockIdx.x / subs, sub = blockIdx.x % subs;
-    const int rbase = blockIdx.z * 16 * rb;
-    const int kend = min(T, rbase + 16 * rb);
-    if (!rows_meet_spans(spans, n_spans, T, rbase, kend)) return;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const CausalCta c(heads, kv_heads, hpc, T);
+    if (!rows_meet_spans(spans, n_spans, T, c.rbase, c.kend())) return;
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
     const size_t ld = static_cast<size_t>(heads + 2 * kv_heads) * kQwenHD;
-    const size_t kcol = static_cast<size_t>(heads + kvh) * kQwenHD;
-    const int qh = kvh * G + sub * hpc + warp % hpc;
-    const int r0 = rbase + 16 * (warp / hpc);
-    const bool warp_live = warp < hpc * rb && r0 < T;
+    const size_t kcol = static_cast<size_t>(heads + c.kvh) * kQwenHD;
+    const int qh = c.qh(), r0 = c.r0();
+    const bool warp_live = c.warp_live();
     uint32_t qhf[kQwenHD / 16][4], qlf[kQwenHD / 16][4];
-    load_q_frags(ph, pl, ld, qh, r0, T, warp_live, qhf, qlf);
+    load_q_frags(ph, pl, ld, 0, qh, r0, T, warp_live, qhf, qlf);
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-    for (int sb0 = 0; sb0 < kend; sb0 += kCausalKB) {
+    for (int sb0 = 0; sb0 < c.kend(); sb0 += kCausalKB) {
         __syncthreads();
-        stage_keys(ph, pl, ld, kcol, sb0, T, Kh, Kl);
+        stage_keys(ph, pl, ld, 0, kcol, sb0, T, Kh, Kl);
         __syncthreads();
         if (!warp_live) continue;
         for (int kb0 = 0; kb0 < kCausalKB; kb0 += 32) {
             const int j0 = sb0 + kb0;
             if (j0 > r0 + 15) break;
-            float sacc[4][4];
+            float sacc[4][4], bm0, bm1;
             score_block(qhf, qlf, Kh, Kl, kb0, j0, r0, sacc);
-            float bm0 = -INFINITY, bm1 = -INFINITY;
-#pragma unroll
-            for (int n = 0; n < 4; ++n) {
-                bm0 = fmaxf(bm0, fmaxf(sacc[n][0], sacc[n][1]));
-                bm1 = fmaxf(bm1, fmaxf(sacc[n][2], sacc[n][3]));
-            }
-            bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 1));
-            bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 2));
-            bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 1));
-            bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 2));
+            block_row_max(sacc, bm0, bm1);
             const float mn0 = fmaxf(m0, bm0), mn1 = fmaxf(m1, bm1);
             float ps0 = 0.f, ps1 = 0.f;
 #pragma unroll
@@ -1794,10 +1757,8 @@ __global__ void __launch_bounds__(kCausalWarps * 32, 1) spans_rowstat_kernel(con
         }
     }
     if (!warp_live) return;
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    l0 = quad_sum(l0);
+    l1 = quad_sum(l1);
     if (t == 0) {
         const size_t o = static_cast<size_t>(qh) * T;
         if (r0 + g < T) { m_out[o + r0 + g] = m0; l_out[o + r0 + g] = l0; }
@@ -1819,11 +1780,8 @@ __global__ void __launch_bounds__(kCausalWarps * 32, 1) spans_mass_kernel(const 
     __half* Kl = Kh + kCausalKB * kCausalKSTR;
     float* acc = reinterpret_cast<float*>(Kl + kCausalKB * kCausalKSTR);   // [warps][16][kSpanChunk]
     __shared__ int clo[kSpanChunk], chi[kSpanChunk];
-    const int G = heads / kv_heads, subs = G / hpc, rb = kCausalWarps / hpc;
-    const int kvh = blockIdx.x / subs, sub = blockIdx.x % subs;
-    const int rbase = blockIdx.z * 16 * rb;
-    const int kend = min(T, rbase + 16 * rb);
-    if (!rows_meet_spans(spans, n_spans, T, rbase, kend)) return;
+    const CausalCta c(heads, kv_heads, hpc, T);
+    if (!rows_meet_spans(spans, n_spans, T, c.rbase, c.kend())) return;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
     if (threadIdx.x < kSpanChunk) {
         int lo = 0, hi = 0;
@@ -1835,27 +1793,26 @@ __global__ void __launch_bounds__(kCausalWarps * 32, 1) spans_mass_kernel(const 
     for (int e = lane; e < 16 * kSpanChunk; e += 32) wacc[e] = 0.f;
     __syncthreads();
     // the keys the chunk can see: from its first span start to the CTA's last row
-    int kmin = kend;
+    int kmin = c.kend();
     for (int b = 0; b < nc; ++b)
         if (clo[b] < chi[b]) kmin = min(kmin, clo[b]);
     const size_t ld = static_cast<size_t>(heads + 2 * kv_heads) * kQwenHD;
-    const size_t kcol = static_cast<size_t>(heads + kvh) * kQwenHD;
-    const int qh = kvh * G + sub * hpc + warp % hpc;
-    const int r0 = rbase + 16 * (warp / hpc);
-    const bool warp_live = warp < hpc * rb && r0 < T;
+    const size_t kcol = static_cast<size_t>(heads + c.kvh) * kQwenHD;
+    const int qh = c.qh(), r0 = c.r0();
+    const bool warp_live = c.warp_live();
     uint32_t qhf[kQwenHD / 16][4], qlf[kQwenHD / 16][4];
-    load_q_frags(ph, pl, ld, qh, r0, T, warp_live, qhf, qlf);
+    load_q_frags(ph, pl, ld, 0, qh, r0, T, warp_live, qhf, qlf);
     // rows past T take 1 / l = 0, so every p of theirs is 0
     float mr0 = 0.f, mr1 = 0.f, il0 = 0.f, il1 = 0.f;
     if (warp_live && r0 + g < T) { mr0 = m_in[static_cast<size_t>(qh) * T + r0 + g]; il0 = 1.0f / l_in[static_cast<size_t>(qh) * T + r0 + g]; }
     if (warp_live && r0 + g + 8 < T) { mr1 = m_in[static_cast<size_t>(qh) * T + r0 + g + 8]; il1 = 1.0f / l_in[static_cast<size_t>(qh) * T + r0 + g + 8]; }
-    for (int sb0 = kmin / kCausalKB * kCausalKB; sb0 < kend; sb0 += kCausalKB) {
+    for (int sb0 = kmin / kCausalKB * kCausalKB; sb0 < c.kend(); sb0 += kCausalKB) {
         // a staged block that meets no span of the chunk is skipped (block-uniform)
         bool any = false;
         for (int b = 0; b < nc; ++b) any |= clo[b] < chi[b] && clo[b] < sb0 + kCausalKB && chi[b] > sb0;
         if (!any) continue;
         __syncthreads();
-        stage_keys(ph, pl, ld, kcol, sb0, T, Kh, Kl);
+        stage_keys(ph, pl, ld, 0, kcol, sb0, T, Kh, Kl);
         __syncthreads();
         if (!warp_live) continue;
         for (int kb0 = 0; kb0 < kCausalKB; kb0 += 32) {
@@ -1884,10 +1841,8 @@ __global__ void __launch_bounds__(kCausalWarps * 32, 1) spans_mass_kernel(const 
                         if (j >= lo && j < hi) { v0 += sacc[n][c]; v1 += sacc[n][2 + c]; }
                     }
                 }
-                v0 += __shfl_xor_sync(0xffffffffu, v0, 1);
-                v0 += __shfl_xor_sync(0xffffffffu, v0, 2);
-                v1 += __shfl_xor_sync(0xffffffffu, v1, 1);
-                v1 += __shfl_xor_sync(0xffffffffu, v1, 2);
+                v0 = quad_sum(v0);
+                v1 = quad_sum(v1);
                 if (t == 0) {
                     wacc[g * kSpanChunk + b] += v0;
                     wacc[(g + 8) * kSpanChunk + b] += v1;
@@ -1934,7 +1889,7 @@ static size_t attention_spans_ws_floats(int T, int heads) {
 // A, then per chunk of kSpanChunk column spans B and C -> out [n_spans, n_spans] (device float64)
 static int launch_attention_spans(const __half* qkv_hi, const __half* qkv_lo, int T, int heads, int kv_heads,
                                   const int* spans, int n_spans, float* ws, double* out, cudaStream_t st) {
-    const int G = heads / kv_heads, hpc = causal_heads_per_cta(G), rows = 16 * (kCausalWarps / hpc);
+    const CausalGrid cg = causal_grid(heads, kv_heads, T);
     float* m = ws;
     float* l = m + static_cast<size_t>(heads) * T;
     float* M = l + static_cast<size_t>(heads) * T;
@@ -1942,15 +1897,15 @@ static int launch_attention_spans(const __half* qkv_hi, const __half* qkv_lo, in
     ProfScope _ps(PROF_ATTN, st);
     RMU_CUDA(cudaFuncSetAttribute(spans_rowstat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSpanKSmem)));
     RMU_CUDA(cudaFuncSetAttribute(spans_mass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_b)));
-    const dim3 grid(static_cast<unsigned>(kv_heads * (G / hpc)), 1, static_cast<unsigned>((T + rows - 1) / rows));
-    spans_rowstat_kernel<<<grid, kCausalWarps * 32, kSpanKSmem, st>>>(qkv_hi, qkv_lo, T, heads, kv_heads, hpc, spans,
+    const dim3 grid(cg.x, 1, cg.z);
+    spans_rowstat_kernel<<<grid, kCausalWarps * 32, kSpanKSmem, st>>>(qkv_hi, qkv_lo, T, heads, kv_heads, cg.hpc, spans,
                                                                       n_spans, m, l);
     count_launch();
     RMU_CHECK_LAUNCH();
     for (int c0 = 0; c0 < n_spans; c0 += kSpanChunk) {
         const int nc = std::min(kSpanChunk, n_spans - c0);
-        spans_mass_kernel<<<grid, kCausalWarps * 32, smem_b, st>>>(qkv_hi, qkv_lo, T, heads, kv_heads, hpc, spans, n_spans,
-                                                                   c0, nc, m, l, M);
+        spans_mass_kernel<<<grid, kCausalWarps * 32, smem_b, st>>>(qkv_hi, qkv_lo, T, heads, kv_heads, cg.hpc, spans,
+                                                                   n_spans, c0, nc, m, l, M);
         count_launch();
         RMU_CHECK_LAUNCH();
         spans_reduce_kernel<<<dim3(static_cast<unsigned>(n_spans), static_cast<unsigned>(nc)), kSpanReduceThreads, 0, st>>>(
@@ -2281,13 +2236,20 @@ struct DevBuf {
 };
 
 // make b hold at least `need` bytes; when it must grow it allocates max(need, alloc).  The device is synchronised
-// first: work queued on any stream may still read the old allocation.
+// first: work queued on any stream may still read the old allocation.  A failed allocation leaves b empty, clears the
+// CUDA error (an out-of-memory is not sticky, so the handle stays usable) and names the bytes it asked for.
 static int grow(DevBuf& b, size_t need, size_t alloc = 0) {
     if (need <= b.cap) return RMU_OK;
     RMU_CUDA(cudaDeviceSynchronize());
     b.release();
     alloc = std::max(need, alloc);
-    RMU_CUDA(cudaMalloc(&b.p, alloc));
+    const cudaError_t err = cudaMalloc(&b.p, alloc);
+    if (err != cudaSuccess) {
+        cudaGetLastError();
+        b.p = nullptr;
+        set_error("cannot allocate " + std::to_string(alloc) + " bytes of device memory: " + cudaGetErrorString(err));
+        return RMU_ERR_CUDA;
+    }
     b.cap = alloc;
     return RMU_OK;
 }
@@ -2536,6 +2498,59 @@ static int run_adapter(rmu_encoder* e, const EncLayer& L, int M, float* pre, con
     return launch_gemm(GEMM_BIAS_RESID_F32, ffa, L.D2, g, e->sms, st);
 }
 
+// The planes a post-LN layer runs on after its QKV projection: every token row (X, CTX, X1, FF, FFA, PRE) or one row
+// per sequence (the _cls set of run_last_layer_cls).  x is the layer's input and, at the end, its output.
+struct PostLnActs {
+    const SplitOperand &x, &ctx, &x1, &ff, &ffa;
+    float* pre;
+};
+
+// the layer's attention -> a.ctx: DeBERTa's disentangled attention when the model has position buckets, else E2 (with
+// the relative bias table and, full rows only, the key limit nkeys).  cls_q non-null: the query rows are the CLS rows'
+// compact q planes.
+static int run_layer_attention(rmu_encoder* e, const EncLayer& L, const SplitOperand* cls_q, const int32_t* cu, int B,
+                               int T, int max_seqlen, const SplitOperand& ctx, cudaStream_t st,
+                               const int32_t* nkeys = nullptr) {
+    const rmu_bert_config& c = e->cfg;
+    const __half* q_hi = cls_q ? cls_q->hi : nullptr;
+    const __half* q_lo = cls_q ? cls_q->lo : nullptr;
+    if (e->ext.position_buckets > 0) {
+        int rc = ensure_position_ws(e, cls_q ? B : T, T, max_seqlen);
+        if (rc != RMU_OK) return rc;
+        return run_disentangled_attention(e->QKVP.hi, e->QKVP.lo, q_hi, q_lo, cu, B, T, c.hidden, c.heads, max_seqlen,
+                                          L.pos_hi, L.pos_lo, e->cidx, e->cidx_h.data(), c.max_pos - 1,
+                                          e->pos_ws.as<float>(), ctx.hi, ctx.lo, st);
+    }
+    return launch_attention(e->QKVP.hi, e->QKVP.lo, q_hi, q_lo, cu, B, c.hidden, c.heads, max_seqlen, ctx.hi, ctx.lo, st,
+                            e->rel, nkeys);
+}
+
+// a post-LN layer after its attention, on M rows: pre = ctx Wo^T + bo + x; x1 = LN1(pre); ff = gelu(x1 W1^T + b1);
+// pre = ff W2^T + b2 + x1; X-MOD's adapter; x = LN2(pre)
+static int run_post_ln_tail(rmu_encoder* e, const EncLayer& L, int M, const PostLnActs& a, cudaStream_t st) {
+    const rmu_bert_config& c = e->cfg;
+    const int H = c.hidden, F = c.ffn;
+    GemmParams g{};
+    g.M = M; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = a.pre; g.res_hi = a.x.hi; g.res_lo = a.x.lo;
+    int rc = launch_gemm(GEMM_BIAS_RESID_F32, a.ctx, L.Wo, g, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    rc = launch_layernorm(a.pre, M, H, L.ln1g, L.ln1b, c.ln_eps, a.x1.hi, a.x1.lo, st);
+    if (rc != RMU_OK) return rc;
+    g = GemmParams{};
+    g.M = M; g.N = F; g.K = H; g.bias = L.b1; g.out_hi = a.ff.hi; g.out_lo = a.ff.lo;
+    rc = launch_gemm(GEMM_BIAS_GELU_SPLIT, a.x1, L.W1, g, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    g = GemmParams{};
+    g.M = M; g.N = H; g.K = F; g.bias = L.b2; g.out_f32 = a.pre; g.res_hi = a.x1.hi; g.res_lo = a.x1.lo;
+    rc = launch_gemm(GEMM_BIAS_RESID_F32, a.ff, L.W2, g, e->sms, st);
+    if (rc != RMU_OK) return rc;
+    if (c.adapter_dim > 0) {
+        rc = run_adapter(e, L, M, a.pre, a.x1, a.ffa, st);
+        if (rc != RMU_OK) return rc;
+    }
+    return launch_layernorm(a.pre, M, H, L.ln2g, L.ln2b, c.ln_eps, a.x.hi, a.x.lo, st);
+}
+
 // The last layer when only the CLS rows leave the encoder (classifier head, CLS pooling).  The CLS query attends to
 // every key, so K and V are projected for all T rows, into the k | v columns of QKVP; everything else runs on row cu[b]
 // of each sequence alone, gathered into row b of the compact planes, and leaves that row's hidden state in e->X_cls.
@@ -2543,8 +2558,7 @@ static int run_adapter(rmu_encoder* e, const EncLayer& L, int M, float* pre, con
 // whatever the other query rows, ln_kernel one warp per row), so those rows are bit-identical to the full layer's.
 static int run_last_layer_cls(rmu_encoder* e, const EncLayer& L, const int32_t* cu, int B, int T, int max_seqlen,
                               float qscale, cudaStream_t st) {
-    const rmu_bert_config& c = e->cfg;
-    const int H = c.hidden, F = c.ffn;
+    const int H = e->cfg.hidden;
     GemmParams g{};
     g.M = T; g.N = 2 * H; g.K = H; g.bias = L.bqkv + H;
     g.out_hi = e->QKVP.hi + H; g.out_lo = e->QKVP.lo + H; g.out_ld = 3 * H; g.qcols = 0; g.qscale = 1.0f;
@@ -2555,37 +2569,9 @@ static int run_last_layer_cls(rmu_encoder* e, const EncLayer& L, const int32_t* 
     g = GemmParams{};
     g.M = B; g.N = H; g.K = H; g.bias = L.bqkv; g.out_hi = e->Q_cls.hi; g.out_lo = e->Q_cls.lo; g.qcols = H; g.qscale = qscale;
     rc = launch_gemm(GEMM_BIAS_SPLIT_QSCALE, e->X_cls, e->last_wq, g, e->sms, st);
+    if (rc == RMU_OK) rc = run_layer_attention(e, L, &e->Q_cls, cu, B, T, max_seqlen, e->CTX_cls, st);
     if (rc != RMU_OK) return rc;
-    if (e->ext.position_buckets > 0) {
-        rc = ensure_position_ws(e, B, T, max_seqlen);
-        if (rc == RMU_OK)
-            rc = run_disentangled_attention(e->QKVP.hi, e->QKVP.lo, e->Q_cls.hi, e->Q_cls.lo, cu, B, T, H, c.heads, max_seqlen,
-                                            L.pos_hi, L.pos_lo, e->cidx, e->cidx_h.data(), c.max_pos - 1,
-                                            e->pos_ws.as<float>(), e->CTX_cls.hi, e->CTX_cls.lo, st);
-    } else {
-        rc = launch_attention(e->QKVP.hi, e->QKVP.lo, e->Q_cls.hi, e->Q_cls.lo, cu, B, H, c.heads, max_seqlen, 0, e->CTX_cls.hi,
-                              e->CTX_cls.lo, st, e->rel);
-    }
-    if (rc != RMU_OK) return rc;
-    g = GemmParams{};
-    g.M = B; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE_cls; g.res_hi = e->X_cls.hi; g.res_lo = e->X_cls.lo;
-    rc = launch_gemm(GEMM_BIAS_RESID_F32, e->CTX_cls, L.Wo, g, e->sms, st);
-    if (rc != RMU_OK) return rc;
-    rc = launch_layernorm(e->PRE_cls, B, H, L.ln1g, L.ln1b, c.ln_eps, e->X1_cls.hi, e->X1_cls.lo, st);
-    if (rc != RMU_OK) return rc;
-    g = GemmParams{};
-    g.M = B; g.N = F; g.K = H; g.bias = L.b1; g.out_hi = e->FF_cls.hi; g.out_lo = e->FF_cls.lo;
-    rc = launch_gemm(GEMM_BIAS_GELU_SPLIT, e->X1_cls, L.W1, g, e->sms, st);
-    if (rc != RMU_OK) return rc;
-    g = GemmParams{};
-    g.M = B; g.N = H; g.K = F; g.bias = L.b2; g.out_f32 = e->PRE_cls; g.res_hi = e->X1_cls.hi; g.res_lo = e->X1_cls.lo;
-    rc = launch_gemm(GEMM_BIAS_RESID_F32, e->FF_cls, L.W2, g, e->sms, st);
-    if (rc != RMU_OK) return rc;
-    if (c.adapter_dim > 0) {
-        rc = run_adapter(e, L, B, e->PRE_cls, e->X1_cls, e->FFA_cls, st);
-        if (rc != RMU_OK) return rc;
-    }
-    return launch_layernorm(e->PRE_cls, B, H, L.ln2g, L.ln2b, c.ln_eps, e->X_cls.hi, e->X_cls.lo, st);
+    return run_post_ln_tail(e, L, B, {e->X_cls, e->CTX_cls, e->X1_cls, e->FF_cls, e->FFA_cls, e->PRE_cls}, st);
 }
 
 // ModernBERT's pre-LN stack (every layer in full): leaves final_norm of the residual stream in e->X.  The residual stream
@@ -2623,7 +2609,7 @@ static int run_modernbert(rmu_encoder* e, const int32_t* ids, const int32_t* typ
         g.pos = e->POSI; g.rope_cos = e->rope_cos[tab]; g.rope_sin = e->rope_sin[tab]; g.rope_hd = DH; g.rope_rows = c.max_pos;
         rc = launch_gemm(GEMM_BIAS_SPLIT_ROPE, e->X, L.Wqkv, g, e->sms, st);
         if (rc == RMU_OK)
-            rc = launch_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, H, c.heads, max_seqlen, kAttWarps, e->CTX.hi,
+            rc = launch_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, H, c.heads, max_seqlen, e->CTX.hi,
                                   e->CTX.lo, st, nullptr, nullptr, nullptr, L.window);
         if (rc != RMU_OK) return rc;
         g = GemmParams{};
@@ -2649,7 +2635,7 @@ static int run_modernbert(rmu_encoder* e, const int32_t* ids, const int32_t* typ
 static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_ids, const int32_t* cu, int B, int T,
                        int max_seqlen, bool cls_only, cudaStream_t st, const int32_t* nkeys = nullptr) {
     const rmu_bert_config& c = e->cfg;
-    const int H = c.hidden, F = c.ffn, DH = H / c.heads;
+    const int H = c.hidden, DH = H / c.heads;
     // the last position a sequence can reach is its length - 1 plus the offset (2 with padding-offset positions)
     const int pos_offset = c.position_mode == RMU_POS_OFFSET ? kPadId + 1 : 0;
     if (max_seqlen + pos_offset > c.max_pos) {
@@ -2676,37 +2662,8 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
         g.M = T; g.N = 3 * H; g.K = H; g.bias = L.bqkv;
         g.out_hi = e->QKVP.hi; g.out_lo = e->QKVP.lo; g.qcols = H; g.qscale = qscale;
         rc = launch_gemm(GEMM_BIAS_SPLIT_QSCALE, e->X, L.Wqkv, g, e->sms, st);
-        if (rc != RMU_OK) return rc;
-        if (e->ext.position_buckets > 0) {
-            rc = ensure_position_ws(e, T, T, max_seqlen);
-            if (rc == RMU_OK)
-                rc = run_disentangled_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, T, H, c.heads, max_seqlen,
-                                                L.pos_hi, L.pos_lo, e->cidx, e->cidx_h.data(), c.max_pos - 1,
-                                                e->pos_ws.as<float>(), e->CTX.hi, e->CTX.lo, st);
-        } else {
-            rc = launch_attention(e->QKVP.hi, e->QKVP.lo, nullptr, nullptr, cu, B, H, c.heads, max_seqlen, kAttWarps, e->CTX.hi,
-                                  e->CTX.lo, st, e->rel, nkeys);
-        }
-        if (rc != RMU_OK) return rc;
-        g = GemmParams{};
-        g.M = T; g.N = H; g.K = H; g.bias = L.bo; g.out_f32 = e->PRE; g.res_hi = e->X.hi; g.res_lo = e->X.lo;
-        rc = launch_gemm(GEMM_BIAS_RESID_F32, e->CTX, L.Wo, g, e->sms, st);
-        if (rc != RMU_OK) return rc;
-        rc = launch_layernorm(e->PRE, T, H, L.ln1g, L.ln1b, c.ln_eps, e->X1.hi, e->X1.lo, st);
-        if (rc != RMU_OK) return rc;
-        g = GemmParams{};
-        g.M = T; g.N = F; g.K = H; g.bias = L.b1; g.out_hi = e->FF.hi; g.out_lo = e->FF.lo;
-        rc = launch_gemm(GEMM_BIAS_GELU_SPLIT, e->X1, L.W1, g, e->sms, st);
-        if (rc != RMU_OK) return rc;
-        g = GemmParams{};
-        g.M = T; g.N = H; g.K = F; g.bias = L.b2; g.out_f32 = e->PRE; g.res_hi = e->X1.hi; g.res_lo = e->X1.lo;
-        rc = launch_gemm(GEMM_BIAS_RESID_F32, e->FF, L.W2, g, e->sms, st);
-        if (rc != RMU_OK) return rc;
-        if (c.adapter_dim > 0) {
-            rc = run_adapter(e, L, T, e->PRE, e->X1, e->FFA, st);
-            if (rc != RMU_OK) return rc;
-        }
-        rc = launch_layernorm(e->PRE, T, H, L.ln2g, L.ln2b, c.ln_eps, e->X.hi, e->X.lo, st);
+        if (rc == RMU_OK) rc = run_layer_attention(e, L, nullptr, cu, B, T, max_seqlen, e->CTX, st, nkeys);
+        if (rc == RMU_OK) rc = run_post_ln_tail(e, L, T, {e->X, e->CTX, e->X1, e->FF, e->FFA, e->PRE}, st);
         if (rc != RMU_OK) return rc;
     }
     return RMU_OK;
@@ -2765,6 +2722,20 @@ static __half* kv_layer(rmu_encoder* e, int l) {
     return e->kv_cache.as<__half>() + static_cast<size_t>(l) * 4 * e->qext.kv_heads * e->kv_cap * kQwenHD;
 }
 
+// the rmu_decoder_* entry points run on decoder handles only
+static int check_decoder(const rmu_encoder* e, const std::string& fn) {
+    if (e->qwen && !e->has_head) return RMU_OK;
+    set_error(fn + ": the encoder must come from rmu_encoder_create_qwen3 without a head or from rmu_encoder_create_llama");
+    return RMU_ERR_ARG;
+}
+
+// a handle whose NF4 conversion failed part-way runs nothing
+static int check_nf4_intact(const rmu_encoder* e, const std::string& fn) {
+    if (!e->nf4_broken) return RMU_OK;
+    set_error(fn + ": the handle's NF4 conversion failed part-way (rmu_decoder_quantize_nf4); destroy it");
+    return RMU_ERR_ARG;
+}
+
 // Qwen3's layers (the header's formula): leaves the residual stream h, before the final norm, in e->PRE [T, H] fp32.
 // Per layer: the attention inputs (above); CTX = causal GQA attention; then qwen3_layer_tail.  With attn_last (the span
 // attention), the last layer stops at its attention inputs, which QKVP then holds.  With to_cache (one sequence, the
@@ -2774,12 +2745,10 @@ static int run_qwen3(rmu_encoder* e, const int32_t* ids, const int32_t* cu, int 
                      bool attn_last = false, bool to_cache = false) {
     const rmu_bert_config& c = e->cfg;
     if (max_seqlen > c.max_pos) { set_error("sequence longer than max_position_embeddings"); return RMU_ERR_ARG; }
-    if (e->nf4_broken) {
-        set_error("the handle's NF4 conversion failed part-way (rmu_decoder_quantize_nf4); destroy it");
-        return RMU_ERR_ARG;
-    }
+    int rc = check_nf4_intact(e, e->llama ? "Llama forward" : "Qwen3 forward");
+    if (rc != RMU_OK) return rc;
     const int H = c.hidden, nh = c.heads, kv = e->qext.kv_heads;
-    int rc = ensure_tokens(e, T, B);
+    rc = ensure_tokens(e, T, B);
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace is shared by all callers
     RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
@@ -3404,22 +3373,14 @@ int rmu_encoder_hidden(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
 
 int rmu_decoder_attention_spans(rmu_encoder* e, const int32_t* ids, int T, const int32_t* spans, int n_spans, double* out,
                                 void* stream) {
-    if (!e || !ids || !spans || !out || T <= 0 || n_spans <= 0) {
-        set_error("rmu_decoder_attention_spans: bad argument");
-        return RMU_ERR_ARG;
-    }
-    if (!e->qwen || e->has_head) {
-        set_error("rmu_decoder_attention_spans: the encoder must come from rmu_encoder_create_qwen3 without a head or from "
-                  "rmu_encoder_create_llama");
-        return RMU_ERR_ARG;
-    }
-    if (e->nf4_broken) {
-        set_error("rmu_decoder_attention_spans: the handle's NF4 conversion failed part-way; destroy it");
-        return RMU_ERR_ARG;
-    }
+    const std::string fn("rmu_decoder_attention_spans");
+    if (!e || !ids || !spans || !out || T <= 0 || n_spans <= 0) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
+    int rc = check_decoder(e, fn);
+    if (rc == RMU_OK) rc = check_nf4_intact(e, fn);
+    if (rc != RMU_OK) return rc;
     if (T > e->cfg.max_pos) {
-        set_error("rmu_decoder_attention_spans: " + std::to_string(T) + " tokens exceed max_position_embeddings (" +
-                  std::to_string(e->cfg.max_pos) + ")");
+        set_error(fn + ": " + std::to_string(T) + " tokens exceed max_position_embeddings (" + std::to_string(e->cfg.max_pos) +
+                  ")");
         return RMU_ERR_ARG;
     }
     std::lock_guard<std::mutex> g(e->mu);
@@ -3428,7 +3389,7 @@ int rmu_decoder_attention_spans(rmu_encoder* e, const int32_t* ids, int T, const
     // pageable source: the copy has taken cu_h when the call returns; span_cu is read by run_qwen3 only, which the
     // range check below has finished before this entry point returns
     RMU_CUDA(cudaMemcpyAsync(e->span_cu, cu_h, sizeof(cu_h), cudaMemcpyHostToDevice, st));
-    int rc = run_qwen3(e, ids, e->span_cu, 1, T, T, st, true);
+    rc = run_qwen3(e, ids, e->span_cu, 1, T, T, st, true);
     if (rc == RMU_OK) rc = qwen3_check_range(e, st);
     if (rc == RMU_OK) rc = grow(e->span_ws, attention_spans_ws_floats(T, e->cfg.heads) * sizeof(float));
     if (rc == RMU_OK)
@@ -3527,11 +3488,8 @@ int rmu_encoder_set_dense(rmu_encoder* e, int n_layers, const int32_t* dims, con
 
 int rmu_decoder_set_lm_head(rmu_encoder* e, const float* W_h) {
     if (!e || !W_h) { set_error("rmu_decoder_set_lm_head: bad argument"); return RMU_ERR_ARG; }
-    if (!e->qwen || e->has_head) {
-        set_error("rmu_decoder_set_lm_head: the encoder must come from rmu_encoder_create_qwen3 without a head or from "
-                  "rmu_encoder_create_llama");
-        return RMU_ERR_ARG;
-    }
+    int rc = check_decoder(e, "rmu_decoder_set_lm_head");
+    if (rc != RMU_OK) return rc;
     const int V = e->cfg.vocab_size, H = e->cfg.hidden;
     if (V % 128 != 0) {
         set_error("rmu_decoder_set_lm_head: vocab_size must be a multiple of 128 (the LM head GEMM's tile), got " +
@@ -3541,7 +3499,7 @@ int rmu_decoder_set_lm_head(rmu_encoder* e, const float* W_h) {
     std::lock_guard<std::mutex> hg(e->host_mu);
     std::lock_guard<std::mutex> g(e->mu);
     if (e->has_lm_head) { set_error("rmu_decoder_set_lm_head: an LM head is already attached"); return RMU_ERR_ARG; }
-    int rc = check_split_range("rmu_decoder_set_lm_head", "lm_head", W_h, static_cast<size_t>(V) * H);
+    rc = check_split_range("rmu_decoder_set_lm_head", "lm_head", W_h, static_cast<size_t>(V) * H);
     if (rc != RMU_OK) return rc;
     rc = upload_split(e, &e->lm_head, {W_h}, V, H);
     if (rc == RMU_OK) {
@@ -3556,10 +3514,8 @@ int rmu_decoder_set_lm_head(rmu_encoder* e, const float* W_h) {
 int rmu_decoder_quantize_nf4(rmu_encoder* e, void* stream) {
     const std::string fn("rmu_decoder_quantize_nf4");
     if (!e) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
-    if (!e->qwen || e->has_head) {
-        set_error(fn + ": the encoder must come from rmu_encoder_create_qwen3 without a head or from rmu_encoder_create_llama");
-        return RMU_ERR_ARG;
-    }
+    int rc = check_decoder(e, fn);
+    if (rc != RMU_OK) return rc;
     const rmu_bert_config& c = e->cfg;
     const int H = c.hidden, F = c.ffn, QD = c.heads * kQwenHD, NQKV = e->qkv_w;
     // K of q | k | v, o, gate | up, down.  K % 64 == 0 keeps every quantisation block inside one row, so the handle's
@@ -3608,7 +3564,6 @@ int rmu_decoder_quantize_nf4(rmu_encoder* e, void* stream) {
         return release(hi, n * 2);
     };
     e->nf4_broken = true;                              // until every layer is converted
-    int rc = RMU_OK;
     for (int l = 0; l < c.layers && rc == RMU_OK; ++l)
         for (int w = 0; w < 4 && rc == RMU_OK; ++w) rc = convert(e->layers[l], w);
     // the prefill's scratch, allocated once the split planes are gone: one hi | lo pair as large as the largest weight
@@ -3634,19 +3589,18 @@ int rmu_decoder_generate(rmu_encoder* e, const int32_t* ids_h, int T, const rmu_
                          int max_new_tokens, int32_t* out_h, int32_t* n_out, float* logits_h, void* stream) {
     const std::string fn("rmu_decoder_generate");
     if (!e || !ids_h || !s || !out_h || !n_out || T < 1 || max_new_tokens < 1) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
-    if (!e->qwen || e->has_head || !e->has_lm_head) {
-        set_error(fn + ": the encoder must be a decoder (rmu_encoder_create_qwen3 without a head, or rmu_encoder_create_llama) "
-                  "with an LM head attached by rmu_decoder_set_lm_head");
-        return RMU_ERR_ARG;
-    }
-    if (e->nf4_broken) { set_error(fn + ": the handle's NF4 conversion failed part-way; destroy it"); return RMU_ERR_ARG; }
+    int rc = check_decoder(e, fn);
+    if (rc != RMU_OK) return rc;
+    if (!e->has_lm_head) { set_error(fn + ": no LM head is attached (rmu_decoder_set_lm_head)"); return RMU_ERR_ARG; }
+    rc = check_nf4_intact(e, fn);
+    if (rc != RMU_OK) return rc;
     const rmu_bert_config& c = e->cfg;
     if (T >= c.max_pos) {
         set_error(fn + ": a prompt of " + std::to_string(T) + " tokens leaves no position for a new token (max_position_embeddings " +
                   std::to_string(c.max_pos) + ")");
         return RMU_ERR_ARG;
     }
-    int rc = check_sampling(fn, s);
+    rc = check_sampling(fn, s);
     if (rc != RMU_OK) return rc;
     for (int i = 0; i < T; ++i)
         if (ids_h[i] < 0 || ids_h[i] >= c.vocab_size) { set_error(fn + ": token id out of range"); return RMU_ERR_ARG; }
@@ -3655,20 +3609,14 @@ int rmu_decoder_generate(rmu_encoder* e, const int32_t* ids_h, int T, const rmu_
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int V = c.vocab_size, H = c.hidden, nh = c.heads, kv = e->qext.kv_heads, L = c.layers;
     const int cap = std::min(T + max_new_tokens, c.max_pos);
-    // the KV cache: grown (device synchronised first, as grow does) when a call needs more positions
+    // the KV cache: grown when a call needs more positions
     if (cap > e->kv_cap) {
-        const size_t bytes = static_cast<size_t>(L) * 4 * kv * cap * kQwenHD * sizeof(__half);
-        RMU_CUDA(cudaDeviceSynchronize());
-        e->kv_cache.release();
-        e->kv_cap = 0;
-        if (cudaMalloc(&e->kv_cache.p, bytes) != cudaSuccess) {
-            cudaGetLastError();
-            e->kv_cache.p = nullptr;
-            set_error(fn + ": cannot allocate the KV cache: " + std::to_string(bytes) + " bytes for " + std::to_string(cap) +
-                      " positions");
-            return RMU_ERR_CUDA;
+        e->kv_cap = 0;                                  // until grow succeeds: it may free the old cache first
+        rc = grow(e->kv_cache, static_cast<size_t>(L) * 4 * kv * cap * kQwenHD * sizeof(__half));
+        if (rc != RMU_OK) {
+            set_error(fn + ": the KV cache for " + std::to_string(cap) + " positions: " + rmu_last_error());
+            return rc;
         }
-        e->kv_cache.cap = bytes;
         e->kv_cap = cap;
     }
     const size_t words = (static_cast<size_t>(V) + 31) / 32;
@@ -3937,8 +3885,9 @@ int rmu_debug_attention_keys(const uint16_t* qkv_hi, const uint16_t* qkv_lo, con
         set_error("rmu_debug_attention_keys: head_dim must be 32 or 64");
         return RMU_ERR_UNSUPPORTED;
     }
+    if (warps != kAttWarps) { set_error("rmu_debug_attention_keys: warps must be 10"); return RMU_ERR_ARG; }
     return launch_attention(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), nullptr, nullptr,
-                            cu, B, H, heads, max_seqlen, warps, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
+                            cu, B, H, heads, max_seqlen, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
                             static_cast<cudaStream_t>(stream), nullptr, nkeys);
 }
 
@@ -3953,8 +3902,9 @@ int rmu_debug_attention(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const in
         set_error("rmu_debug_attention: head_dim must be 32 or 64");
         return RMU_ERR_UNSUPPORTED;
     }
+    if (warps != kAttWarps) { set_error("rmu_debug_attention: warps must be 10"); return RMU_ERR_ARG; }
     return launch_attention(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), nullptr, nullptr,
-                            cu, B, H, heads, max_seqlen, warps, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
+                            cu, B, H, heads, max_seqlen, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
                             static_cast<cudaStream_t>(stream));
 }
 
@@ -4031,7 +3981,7 @@ int rmu_debug_attention_bias(const uint16_t* qkv_hi, const uint16_t* qkv_lo, con
     }
     return launch_attention(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo),
                             reinterpret_cast<const __half*>(cls_q_hi), reinterpret_cast<const __half*>(cls_q_lo), cu, B, H,
-                            heads, max_seqlen, kAttWarps, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
+                            heads, max_seqlen, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
                             static_cast<cudaStream_t>(stream), rel_table);
 }
 
@@ -4165,9 +4115,8 @@ int rmu_debug_attention_window(const uint16_t* qkv_hi, const uint16_t* qkv_lo, c
         return RMU_ERR_UNSUPPORTED;
     }
     return launch_attention(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), nullptr, nullptr,
-                            cu, B, H, heads, max_seqlen, kAttWarps, reinterpret_cast<__half*>(ctx_hi),
-                            reinterpret_cast<__half*>(ctx_lo), static_cast<cudaStream_t>(stream), nullptr, nullptr, nullptr,
-                            window);
+                            cu, B, H, heads, max_seqlen, reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo),
+                            static_cast<cudaStream_t>(stream), nullptr, nullptr, nullptr, window);
 }
 
 int rmu_debug_modernbert_head(const float* pooled, int B, int H, int num_labels, const float* dense_w, const float* dense_b,
