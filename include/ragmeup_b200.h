@@ -391,6 +391,24 @@ typedef struct rmu_sampling {
  * RMU_ERR_CUDA naming the bytes asked for; an activation outside the split planes' fp16 range RMU_ERR_RANGE. */
 int rmu_decoder_generate(rmu_encoder* enc, const int32_t* ids_h, int T, const rmu_sampling* s, uint64_t seed,
                          int max_new_tokens, int32_t* out_h, int32_t* n_out, float* logits_h, void* stream);
+/* B prompts at once: prompt b = ids_h[cu_h[b] .. cu_h[b + 1]) (host), with seed seeds_h[b] -> out_h [B,
+ * max_new_tokens] (row b's first n_out_h[b] entries written, the rest untouched) and logits_h (nullable) [B,
+ * max_new_tokens, vocab_size].  Row b is bit for bit what rmu_decoder_generate returns for prompt b and seeds_h[b]:
+ * the same tokens and the same logits, on split and NF4 handles, greedy and sampled.  The prompts' longest common
+ * prefix (capped so that every prompt keeps one token of its own; none when B = 1) is prefilled once into a shared
+ * region of the KV cache, the suffixes as one varlen prefill at their positions after it, and each decode step runs
+ * the rows still live at M = live (NF4: one GEMV reads each weight once for all rows), with decode attention over the
+ * shared prefix and the row's own keys, the LM head and one sampler CTA per row, and one synchronise of `stream` per
+ * step.  Each row stops by rmu_decoder_generate's rules; the call ends when all have stopped.  An activation outside
+ * the fp16 range in any row fails the whole call with RMU_ERR_RANGE.  Any failure (a refusal, RMU_ERR_RANGE or a CUDA
+ * error) leaves n_out_h[0 .. min(B, 16)) all 0; out_h and logits_h are then unspecified.  Refused before any CUDA call,
+ * with rmu_decoder_generate's codes: null pointers, B < 1 or B > RMU_MAX_GENERATE_BATCH, an empty prompt,
+ * max_new_tokens < 1, no LM head, another kind of encoder, a broken NF4 handle, a prompt of >= max_pos tokens, the
+ * sampling settings rmu_decoder_generate refuses, an id outside [0, vocab_size). */
+#define RMU_MAX_GENERATE_BATCH 16
+int rmu_decoder_generate_batch(rmu_encoder* enc, const int32_t* ids_h, const int32_t* cu_h, int B, const rmu_sampling* s,
+                               const uint64_t* seeds_h, int max_new_tokens, int32_t* out_h, int32_t* n_out_h,
+                               float* logits_h, void* stream);
 void rmu_encoder_destroy(rmu_encoder* enc);
 
 #define RMU_POOL_MEAN 0
@@ -634,6 +652,24 @@ int rmu_debug_cls_head_act(const uint16_t* hi, const uint16_t* lo, const int32_t
  * RMU_ERR_UNSUPPORTED. */
 int rmu_debug_dense(const float* x, int B, int n_in, int n_out, const float* W, const float* b, int act, int normalize,
                     float* y, void* stream);
+/* For tests: the batched decode's attention.  Row b's q sits qld halves after row b - 1's ([heads 128] each); it reads
+ * keys [0, pos_h[b] + 1) of the cache kv, key k at row k when k < P, else k + shift_h[b] (pos_h, shift_h host int32
+ * [B]) -> ctx [B, heads 128].  Row b equals rmu_debug_attention_decode on a cache holding those keys at rows 0 ..
+ * pos_h[b].  ws holds B * heads * ceil(n / 64) * 130 + 2 B floats, n the largest pos_h + 1.  Null pointers, B outside
+ * 1 .. 65 535, heads or kv_heads < 1, qld < heads 128, a row reading past cap or a smaller ws return RMU_ERR_ARG,
+ * heads % kv_heads != 0 RMU_ERR_UNSUPPORTED. */
+int rmu_debug_attention_decode_rows(const uint16_t* q_hi, const uint16_t* q_lo, int64_t qld, int B, const uint16_t* kv,
+                                    int heads, int kv_heads, int cap, int P, const int32_t* pos_h, const int32_t* shift_h,
+                                    float* ws, int64_t ws_elems, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream);
+/* For tests: the batched prefill's attention (attention_causal_kernel over cached keys).  qkv planes [rows, (heads + 2
+ * kv_heads) 128] hold only the own rows of B sequences (device cu [B + 1]); sequence b is P prefix rows then its own
+ * rows, and every key comes from the cache kv [4][kv_heads, cap, 128]: key k at row k when k < P, else k +
+ * shift[cu[b]] (device int32 per plane row).  -> ctx [rows, heads 128], each row equal to rmu_debug_attention_causal's
+ * row on the full sequence.  max_own: the longest own part.  Null pointers, B outside 1 .. 65 535, heads, kv_heads
+ * or max_own < 1, P < 0 or cap < P return RMU_ERR_ARG, heads % kv_heads != 0 RMU_ERR_UNSUPPORTED. */
+int rmu_debug_attention_cached(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu, int B, int heads,
+                               int kv_heads, const uint16_t* kv, int cap, int P, const int32_t* shift, int max_own,
+                               uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream);
 /* For tests: decode attention, as rmu_decoder_generate runs it, of one query row q [heads 128] planes (pre-scaled by
  * log2(e) / sqrt(128)) against rows [0, n) of one layer's cache kv (fp16 planes K hi | K lo | V hi | V lo, each
  * [kv_heads, cap, 128]) -> ctx planes [heads 128]; query head h reads kv head h / (heads / kv_heads).  ws holds
@@ -661,6 +697,12 @@ int rmu_debug_nf4_gemv(int mode, const uint16_t* x_hi, const uint16_t* x_lo, con
                        int N, int K, const float* bias, const float* res_f32, float* out_f32, uint16_t* out_hi,
                        uint16_t* out_lo, int32_t* range_flag, void* stream);
 int rmu_debug_nf4_conversion(const rmu_encoder* enc, int64_t* peak, int64_t* delta);
+/* For tests: the batched decode's NF4 GEMV (rmu_decoder_generate_batch) on M rows x [M, K] (row pitch K) -> out_f32
+ * [M, N] or out_hi / out_lo [M, N / 2]; res_f32 [M, N].  Row m's bits are rmu_debug_nf4_gemv's on row m alone.  The
+ * arguments are refused as rmu_debug_nf4_gemv refuses them, and M outside 1..16 returns RMU_ERR_ARG. */
+int rmu_debug_nf4_gemv_rows(int mode, int M, const uint16_t* x_hi, const uint16_t* x_lo, const uint8_t* codes,
+                            const float* absmax, int N, int K, const float* bias, const float* res_f32, float* out_f32,
+                            uint16_t* out_hi, uint16_t* out_lo, int32_t* range_flag, void* stream);
 int rmu_debug_kv_append(const uint16_t* hi, const uint16_t* lo, int T, int heads, int kv_heads, int pos0, int cap,
                         uint16_t* kv, void* stream);
 /* For tests: the sampler of rmu_decoder_generate on logits [V] (device fp32, overwritten with the processed values),
@@ -669,6 +711,12 @@ int rmu_debug_kv_append(const uint16_t* hi, const uint16_t* lo, int T, int heads
  * null pointer, V < 1 or u outside [0, 1) return RMU_ERR_ARG, before any CUDA call. */
 int rmu_debug_sample(float* logits, int V, uint32_t* presence, const rmu_sampling* s, float u, int32_t* token,
                      void* stream);
+/* For tests: the batched decode's sampler, one CTA per row r of logits [B, V] (device): the presence bits [.., ceil(V /
+ * 32)] and Philox seed of sequence seq[r] (device int32 [B], device uint64 seeds), u = philox(seed, step) -> token[r].
+ * Row r equals rmu_debug_sample on that row, those bits and that u.  Refused as rmu_debug_sample refuses, and a null
+ * pointer, B < 1 or step < 0 return RMU_ERR_ARG. */
+int rmu_debug_sample_rows(float* logits, int V, int B, uint32_t* presence, const int32_t* seq, const uint64_t* seeds,
+                          int64_t step, const rmu_sampling* s, int32_t* token, void* stream);
 int rmu_debug_split_planes(const float* src, int64_t n, uint16_t* hi, uint16_t* lo, void* stream);
 int rmu_debug_join_planes(const uint16_t* hi, const uint16_t* lo, int64_t n, float* out, void* stream);
 /* For tests: the BM25 select stage alone (bm25_select_kernel rounds, through the launcher rmu_bm25_search uses) on

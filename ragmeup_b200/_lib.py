@@ -42,6 +42,7 @@ class Qwen3ExtC(C.Structure):
 
 
 MAX_EOS = 8
+MAX_GENERATE_BATCH = 16            # RMU_MAX_GENERATE_BATCH
 
 
 class SamplingC(C.Structure):
@@ -132,6 +133,8 @@ SIGNATURES = {
     "rmu_decoder_quantize_nf4": (C.c_int, [C.c_void_p, C.c_void_p]),
     "rmu_decoder_generate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(SamplingC), C.c_uint64, C.c_int,
                                        C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]),
+    "rmu_decoder_generate_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(SamplingC),
+                                             C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_encoder_destroy": (None, [C.c_void_p]),
     "rmu_encoder_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_void_p, C.c_void_p]),
@@ -210,12 +213,22 @@ SIGNATURES = {
                                        C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "rmu_debug_attention_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                              C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_attention_decode_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int,
+                                                  C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_attention_cached": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                             C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_sample_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                        C.POINTER(SamplingC), C.c_void_p, C.c_void_p]),
     "rmu_debug_kv_append": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                       C.c_void_p]),
     "rmu_debug_nf4_quantize": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_nf4_dequantize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "rmu_debug_nf4_gemv": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_nf4_gemv_rows": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                          C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p]),
     "rmu_debug_nf4_conversion": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "rmu_debug_sample": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(SamplingC), C.c_float, C.c_void_p,
                                    C.c_void_p]),

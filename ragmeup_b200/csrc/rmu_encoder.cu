@@ -13,6 +13,7 @@
 // Activations between kernels are split fp16 planes (see rmu_gemm.cuh); LayerNorm, softmax, GELU,
 // residual adds, pooling and the classifier head are fp32.
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <mutex>
@@ -1380,24 +1381,27 @@ __device__ __forceinline__ float quad_sum(float v) {
     return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// the warp's q fragments of rows r0 .. r0 + 15 of head qh (zero past T) in the sequence whose rows start at row t0
+// the warp's q fragments of rows r0 .. r0 + 15 of head qh (zero past T, and before row `first`) in the sequence whose
+// row r is plane row t0 + r - first
 __device__ __forceinline__ void load_q_frags(const __half* ph, const __half* pl, size_t ld, int t0, int qh, int r0, int T,
-                                             bool live, uint32_t (&qhf)[kQwenHD / 16][4], uint32_t (&qlf)[kQwenHD / 16][4]) {
+                                             bool live, uint32_t (&qhf)[kQwenHD / 16][4], uint32_t (&qlf)[kQwenHD / 16][4],
+                                             int first = 0) {
     const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
     const __half* qhb = ph + static_cast<size_t>(t0) * ld + qh * kQwenHD;
     const __half* qlb = pl + static_cast<size_t>(t0) * ld + qh * kQwenHD;
     const int ra = r0 + g, rc = r0 + g + 8;
+    if (first) { qhb -= static_cast<size_t>(first) * ld; qlb -= static_cast<size_t>(first) * ld; }
 #pragma unroll
     for (int ks = 0; ks < kQwenHD / 16; ++ks) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) { qhf[ks][i] = 0u; qlf[ks][i] = 0u; }
-        if (live && ra < T) {
+        if (live && ra < T && ra >= first) {
             qhf[ks][0] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t);
             qlf[ks][0] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t);
             qhf[ks][2] = *reinterpret_cast<const uint32_t*>(qhb + ra * ld + ks * 16 + 2 * t + 8);
             qlf[ks][2] = *reinterpret_cast<const uint32_t*>(qlb + ra * ld + ks * 16 + 2 * t + 8);
         }
-        if (live && rc < T) {
+        if (live && rc < T && rc >= first) {
             qhf[ks][1] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t);
             qlf[ks][1] = *reinterpret_cast<const uint32_t*>(qlb + rc * ld + ks * 16 + 2 * t);
             qhf[ks][3] = *reinterpret_cast<const uint32_t*>(qhb + rc * ld + ks * 16 + 2 * t + 8);
@@ -1407,18 +1411,20 @@ __device__ __forceinline__ void load_q_frags(const __half* ph, const __half* pl,
 }
 
 // stage keys [sb0, sb0 + kCausalKB) of the sequence whose rows start at row t0, kv column kcol, into Kh / Kl, zeros
-// from key `bound` on; kWithV: the values of column vcol go into Vh / Vl in the same loop.  The caller synchronises
-// around it.
+// from key `bound` on; kWithV: the values of column vcol go into Vh / Vl in the same loop.  Key k >= split is read
+// from row t0 + k + shift (the batched prefill's own cache region after the shared prefix; the defaults fold away).
+// The caller synchronises around it.
 template <bool kWithV = false>
 __device__ __forceinline__ void stage_keys(const __half* ph, const __half* pl, size_t ld, int t0, size_t kcol, int sb0,
                                            int bound, __half* Kh, __half* Kl, size_t vcol = 0, __half* Vh = nullptr,
-                                           __half* Vl = nullptr) {
+                                           __half* Vl = nullptr, int split = INT_MAX, int shift = 0) {
     const int nk = min(kCausalKB, bound - sb0);
     for (int e = threadIdx.x; e < kCausalKB * (kQwenHD / 8); e += blockDim.x) {
         const int j = e / (kQwenHD / 8), c8 = (e % (kQwenHD / 8)) * 8;
         uint4 kh = make_uint4(0, 0, 0, 0), kl = kh, vh = kh, vl = kh;
         if (j < nk) {
-            const size_t o = static_cast<size_t>(t0 + sb0 + j) * ld + c8;
+            const int k = sb0 + j;
+            const size_t o = static_cast<size_t>(t0 + k + (k >= split ? shift : 0)) * ld + c8;
             kh = *reinterpret_cast<const uint4*>(ph + o + kcol);
             kl = *reinterpret_cast<const uint4*>(pl + o + kcol);
             if (kWithV) {
@@ -1489,12 +1495,27 @@ __device__ __forceinline__ void block_row_max(const float (&sacc)[4][4], float& 
     bm1 = quad_max(bm1);
 }
 
+// The batched prefill (rmu_decoder_generate_batch) runs this kernel on the suffixes of B prompts that share a prefix
+// of P tokens (kCached): sequence b is then the P prefix rows and its cu[b + 1] - cu[b] own rows, the planes hold
+// only the own rows (row r of the sequence at plane row cu[b] + r - P), and every key comes from the KV cache: key k
+// at cache row k when k < P, else k + shift[cu[b]], where the layer's k / v were appended before the launch.  The
+// query rows keep their blocks of 16 from the sequence's start, rows before P compute nothing and are not written,
+// and the staged keys hold the bits the full launch stages: each row's arithmetic is the full prompt's.  z0 skips the
+// row blocks that lie inside the prefix.
+struct PrefixKeys {
+    const __half* kv = nullptr;           // the layer's cache planes (kv_append_kernel's layout)
+    const int* shift = nullptr;           // per plane row: sequence b's own keys start at cache row P + shift[cu[b]]
+    int cap = 0, P = 0, z0 = 0;
+};
+
+template <bool kCached = false>
 __global__ void __launch_bounds__(kCausalWarps * 32, 1) attention_causal_kernel(const __half* __restrict__ ph,
                                                                                  const __half* __restrict__ pl,
                                                                                  const int* __restrict__ cu, int heads,
                                                                                  int kv_heads, int hpc,
                                                                                  __half* __restrict__ ctx_hi,
-                                                                                 __half* __restrict__ ctx_lo) {
+                                                                                 __half* __restrict__ ctx_lo,
+                                                                                 PrefixKeys pk = PrefixKeys{}) {
     constexpr int DH = kQwenHD, KS = DH / 16, NT = DH / 8, KSTR = kCausalKSTR;
     extern __shared__ __align__(16) unsigned char causal_smem[];
     __half* Kh = reinterpret_cast<__half*>(causal_smem);
@@ -1503,17 +1524,27 @@ __global__ void __launch_bounds__(kCausalWarps * 32, 1) attention_causal_kernel(
     __half* Vl = Vh + kCausalKB * KSTR;
 
     const int b = blockIdx.y;
-    const int t0 = cu[b], S = cu[b + 1] - t0;
-    const CausalCta c(heads, kv_heads, hpc, S);
+    const int P = kCached ? pk.P : 0;
+    const int t0 = cu[b], S = cu[b + 1] - t0 + P;
+    CausalCta c(heads, kv_heads, hpc, S);
+    if (kCached) c.rbase += pk.z0 * 16 * c.rb;
     if (c.rbase >= S) return;
     const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
     const size_t ld = static_cast<size_t>(heads + 2 * kv_heads) * DH;
     const size_t kcol = static_cast<size_t>(heads + c.kvh) * DH, vcol = static_cast<size_t>(heads + kv_heads + c.kvh) * DH;
     const int qh = c.qh(), r0 = c.r0();
-    const bool warp_live = c.warp_live();
+    const bool warp_live = c.warp_live() && r0 + 15 >= P;
+    // the cache seen as planes of row pitch 128: K hi at kv, K lo at kv + plane, V at 2 planes further
+    const size_t plane = static_cast<size_t>(kv_heads) * pk.cap * DH;
+    const __half* kph = kCached ? pk.kv : ph;
+    const __half* kpl = kCached ? pk.kv + plane : pl;
+    const size_t kld = kCached ? static_cast<size_t>(DH) : ld;
+    const size_t kkcol = kCached ? static_cast<size_t>(c.kvh) * pk.cap * DH : kcol;
+    const size_t kvcol = kCached ? 2 * plane + static_cast<size_t>(c.kvh) * pk.cap * DH : vcol;
+    const int kt0 = kCached ? 0 : t0, ksplit = kCached ? P : INT_MAX, kshift = kCached ? pk.shift[t0] : 0;
 
     uint32_t qhf[KS][4], qlf[KS][4];
-    load_q_frags(ph, pl, ld, t0, qh, r0, S, warp_live, qhf, qlf);
+    load_q_frags(ph, pl, ld, t0, qh, r0, S, warp_live, qhf, qlf, P);
     float oacc[NT][4];
 #pragma unroll
     for (int n = 0; n < NT; ++n) oacc[n][0] = oacc[n][1] = oacc[n][2] = oacc[n][3] = 0.f;
@@ -1522,7 +1553,7 @@ __global__ void __launch_bounds__(kCausalWarps * 32, 1) attention_causal_kernel(
     const int kend = c.kend();
     for (int sb0 = 0; sb0 < kend; sb0 += kCausalKB) {
         __syncthreads();
-        stage_keys<true>(ph, pl, ld, t0, kcol, sb0, kend, Kh, Kl, vcol, Vh, Vl);
+        stage_keys<true>(kph, kpl, kld, kt0, kkcol, sb0, kend, Kh, Kl, kvcol, Vh, Vl, ksplit, kshift);
         __syncthreads();
         if (!warp_live) continue;
         for (int kb0 = 0; kb0 < kCausalKB; kb0 += 32) {
@@ -1583,15 +1614,15 @@ __global__ void __launch_bounds__(kCausalWarps * 32, 1) attention_causal_kernel(
     for (int n = 0; n < NT; ++n) {
         const int col = qh * DH + n * 8 + 2 * t;
         uint32_t hv, lv;
-        if (ra < S) {
+        if (ra < S && ra >= P) {
             split_pack(oacc[n][0] * i0, oacc[n][1] * i0, hv, lv);
-            *reinterpret_cast<uint32_t*>(ctx_hi + static_cast<size_t>(t0 + ra) * cld + col) = hv;
-            *reinterpret_cast<uint32_t*>(ctx_lo + static_cast<size_t>(t0 + ra) * cld + col) = lv;
+            *reinterpret_cast<uint32_t*>(ctx_hi + static_cast<size_t>(t0 + ra - P) * cld + col) = hv;
+            *reinterpret_cast<uint32_t*>(ctx_lo + static_cast<size_t>(t0 + ra - P) * cld + col) = lv;
         }
-        if (rc < S) {
+        if (rc < S && rc >= P) {
             split_pack(oacc[n][2] * i1, oacc[n][3] * i1, hv, lv);
-            *reinterpret_cast<uint32_t*>(ctx_hi + static_cast<size_t>(t0 + rc) * cld + col) = hv;
-            *reinterpret_cast<uint32_t*>(ctx_lo + static_cast<size_t>(t0 + rc) * cld + col) = lv;
+            *reinterpret_cast<uint32_t*>(ctx_hi + static_cast<size_t>(t0 + rc - P) * cld + col) = hv;
+            *reinterpret_cast<uint32_t*>(ctx_lo + static_cast<size_t>(t0 + rc - P) * cld + col) = lv;
         }
     }
 }
@@ -1665,16 +1696,33 @@ static int launch_attention_causal(const __half* qkv_hi, const __half* qkv_lo, c
                                    int max_seqlen, __half* ctx_hi, __half* ctx_lo, cudaStream_t st) {
     const CausalGrid cg = causal_grid(heads, kv_heads, max_seqlen);
     ProfScope _ps(PROF_ATTN, st);
-    RMU_CUDA(cudaFuncSetAttribute(attention_causal_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    RMU_CUDA(cudaFuncSetAttribute(attention_causal_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kCausalSmem)));
     for (int s0 = 0; s0 < B; s0 += kMaxGridY) {
         const int nb = std::min(kMaxGridY, B - s0);
         const dim3 grid(cg.x, static_cast<unsigned>(nb), cg.z);
-        attention_causal_kernel<<<grid, kCausalWarps * 32, kCausalSmem, st>>>(qkv_hi, qkv_lo, cu + s0, heads, kv_heads,
-                                                                              cg.hpc, ctx_hi, ctx_lo);
+        attention_causal_kernel<false><<<grid, kCausalWarps * 32, kCausalSmem, st>>>(qkv_hi, qkv_lo, cu + s0, heads,
+                                                                                     kv_heads, cg.hpc, ctx_hi, ctx_lo);
         count_launch();
         RMU_CHECK_LAUNCH();
     }
+    return RMU_OK;
+}
+
+// the batched prefill's suffix attention (PrefixKeys): B <= kMaxGridY sequences, the longest max_own own rows after
+// the prefix
+static int launch_attention_cached(const __half* qkv_hi, const __half* qkv_lo, const int* cu, int B, int heads, int kv_heads,
+                                   int max_own, PrefixKeys pk, __half* ctx_hi, __half* ctx_lo, cudaStream_t st) {
+    const CausalGrid cg = causal_grid(heads, kv_heads, pk.P + max_own);
+    pk.z0 = pk.P / (16 * (kCausalWarps / cg.hpc));
+    ProfScope _ps(PROF_ATTN, st);
+    RMU_CUDA(cudaFuncSetAttribute(attention_causal_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(kCausalSmem)));
+    const dim3 grid(cg.x, static_cast<unsigned>(B), cg.z - static_cast<unsigned>(pk.z0));
+    attention_causal_kernel<true><<<grid, kCausalWarps * 32, kCausalSmem, st>>>(qkv_hi, qkv_lo, cu, heads, kv_heads,
+                                                                                cg.hpc, ctx_hi, ctx_lo, pk);
+    count_launch();
+    RMU_CHECK_LAUNCH();
     return RMU_OK;
 }
 
@@ -1933,9 +1981,11 @@ constexpr int kDecWarps = kDecThreads / 32;
 constexpr int kDecMaxG = 8;                   // query heads per CTA; larger groups take several CTAs (grid z)
 constexpr int kDecPart = 2 + kQwenHD;         // a split's partial per query head: m, l, o[128]
 
-// rows [0, T) of the planes [T, NH 128] (q | k | v) -> cache rows pos0 + t of K and V: one uint4 (8 halves) per thread
+// rows [0, T) of the planes [T, NH 128] (q | k | v) -> cache rows pos0 + t of K and V, or with per-row positions
+// (the batched decode) rows pos[t] + shift[t]: one uint4 (8 halves) per thread
 __global__ void kv_append_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, int T, int heads,
-                                 int kv_heads, int pos0, int cap, __half* __restrict__ kv) {
+                                 int kv_heads, int pos0, int cap, __half* __restrict__ kv, const int* __restrict__ pos,
+                                 const int* __restrict__ shift) {
     const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     const size_t per_tok = static_cast<size_t>(kv_heads) * (kQwenHD / 8);
     if (i >= static_cast<size_t>(T) * per_tok) return;
@@ -1945,12 +1995,24 @@ __global__ void kv_append_kernel(const __half* __restrict__ hi, const __half* __
     const size_t ks = static_cast<size_t>(t) * ld + static_cast<size_t>(heads + h) * kQwenHD + c8;
     const size_t vs = ks + static_cast<size_t>(kv_heads) * kQwenHD;
     const size_t plane = static_cast<size_t>(kv_heads) * cap * kQwenHD;
-    const size_t d = (static_cast<size_t>(h) * cap + pos0 + t) * kQwenHD + c8;
+    const int row = pos ? pos[t] + shift[t] : pos0 + t;
+    const size_t d = (static_cast<size_t>(h) * cap + row) * kQwenHD + c8;
     *reinterpret_cast<uint4*>(kv + d) = *reinterpret_cast<const uint4*>(hi + ks);
     *reinterpret_cast<uint4*>(kv + plane + d) = *reinterpret_cast<const uint4*>(lo + ks);
     *reinterpret_cast<uint4*>(kv + 2 * plane + d) = *reinterpret_cast<const uint4*>(hi + vs);
     *reinterpret_cast<uint4*>(kv + 3 * plane + d) = *reinterpret_cast<const uint4*>(lo + vs);
 }
+
+// The batched decode's rows (rmu_decoder_generate_batch): grid z = row b * gz + the group block; row b's q sits qld
+// halves after row b - 1's, it sees keys [0, pos[b] + 1), key k at cache row k when k < P, else k + shift[b] (the
+// shared prefix, then the row's own region), and its partials and context follow the same row order.  The splits still
+// count from key 0, so one may straddle P; pos null: one row of n keys at rows 0 .. n - 1.
+struct DecRows {
+    const int* pos = nullptr;
+    const int* shift = nullptr;
+    int P = 0, gz = 1;
+    size_t qld = 0;
+};
 
 // One split of one kv head for query heads g0 .. g0 + ng of its group.  q [heads, 128] planes, pre-scaled by log2(e) /
 // sqrt(128) as the q / k step leaves it.  Scores: warp w takes keys w, w + 4, ..., lane l holds dims 4l .. 4l + 3 and
@@ -1962,19 +2024,30 @@ __global__ void __launch_bounds__(kDecThreads) attention_decode_kernel(const __h
                                                                        const __half* __restrict__ ql,
                                                                        const __half* __restrict__ kv, int heads,
                                                                        int kv_heads, int cap, int n, int nsplit,
-                                                                       float* __restrict__ part) {
+                                                                       float* __restrict__ part, DecRows rows) {
     __shared__ float sp[kDecMaxG][kDecChunk];
     __shared__ float sm[kDecMaxG], sl[kDecMaxG];
-    const int G = heads / kv_heads, kvh = blockIdx.x, split = blockIdx.y, g0 = blockIdx.z * kDecMaxG;
+    const int b = blockIdx.z / rows.gz;
+    const int G = heads / kv_heads, kvh = blockIdx.x, split = blockIdx.y, g0 = (blockIdx.z % rows.gz) * kDecMaxG;
+    if (rows.pos) n = rows.pos[b] + 1;
     const int ng = min(kDecMaxG, G - g0);
     const int j0 = split * kDecChunk, nk = min(kDecChunk, n - j0);
+    if (nk <= 0) return;                          // past this row's keys (a shorter row of the batch)
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int P = rows.pos ? rows.P : INT_MAX, sh = rows.pos ? rows.shift[b] : 0;
     const size_t plane = static_cast<size_t>(kv_heads) * cap * kQwenHD;
-    const size_t kbase = (static_cast<size_t>(kvh) * cap + j0) * kQwenHD;
-    const __half* kh = kv + kbase;
+    // key j0 + j of the split: its cache row's offset from kh
+    auto krow = [&](int j) -> size_t {
+        const int k = j0 + j;
+        return (static_cast<size_t>(kvh) * cap + k + (k >= P ? sh : 0)) * kQwenHD;
+    };
+    const __half* kh = kv;
     const __half* kl = kh + plane;
     const __half* vh = kh + 2 * plane;
     const __half* vl = kh + 3 * plane;
+    qh += b * rows.qld;
+    ql += b * rows.qld;
+    part += static_cast<size_t>(b) * heads * nsplit * kDecPart;
     float qhr[kDecMaxG][4], qlr[kDecMaxG][4];
 #pragma unroll
     for (int g = 0; g < kDecMaxG; ++g) {
@@ -1992,8 +2065,9 @@ __global__ void __launch_bounds__(kDecThreads) attention_decode_kernel(const __h
         }
     }
     for (int j = warp; j < nk; j += kDecWarps) {
-        const uint2 h2 = *reinterpret_cast<const uint2*>(kh + static_cast<size_t>(j) * kQwenHD + lane * 4);
-        const uint2 l2 = *reinterpret_cast<const uint2*>(kl + static_cast<size_t>(j) * kQwenHD + lane * 4);
+        const size_t kr = krow(j);
+        const uint2 h2 = *reinterpret_cast<const uint2*>(kh + kr + lane * 4);
+        const uint2 l2 = *reinterpret_cast<const uint2*>(kl + kr + lane * 4);
         const __half2* hp = reinterpret_cast<const __half2*>(&h2);
         const __half2* lp = reinterpret_cast<const __half2*>(&l2);
         const float2 a = __half22float2(hp[0]), b = __half22float2(hp[1]);
@@ -2029,8 +2103,8 @@ __global__ void __launch_bounds__(kDecThreads) attention_decode_kernel(const __h
     for (int g = 0; g < kDecMaxG; ++g) acc[g] = 0.f;
 #pragma unroll 8
     for (int j = 0; j < nk; ++j) {
-        const float v = __half2float(vh[static_cast<size_t>(j) * kQwenHD + tid]) +
-                        __half2float(vl[static_cast<size_t>(j) * kQwenHD + tid]);
+        const size_t kr = krow(j);
+        const float v = __half2float(vh[kr + tid]) + __half2float(vl[kr + tid]);
 #pragma unroll
         for (int g = 0; g < kDecMaxG; ++g)
             if (g < ng) acc[g] = fmaf(sp[g][j], v, acc[g]);
@@ -2042,17 +2116,19 @@ __global__ void __launch_bounds__(kDecThreads) attention_decode_kernel(const __h
     }
 }
 
-// one block per query head: the splits in order, M = max m_s, L = sum l_s exp2(m_s - M), o = sum o_s exp2(m_s - M) / L
-// -> the context planes [heads 128]
+// one block per (row, query head): the row's splits in order, M = max m_s, L = sum l_s exp2(m_s - M), o = sum o_s
+// exp2(m_s - M) / L -> the context planes [rows, heads 128]
 __global__ void __launch_bounds__(kDecThreads) attention_decode_combine_kernel(const float* __restrict__ part, int nsplit,
                                                                                __half* __restrict__ ctx_hi,
-                                                                               __half* __restrict__ ctx_lo) {
+                                                                               __half* __restrict__ ctx_lo,
+                                                                               const int* __restrict__ pos, int heads) {
     const int h = blockIdx.x, d = threadIdx.x;
+    const int ns = pos ? (pos[h / heads] + kDecChunk) / kDecChunk : nsplit;   // decode_splits(pos + 1)
     const float* p = part + static_cast<size_t>(h) * nsplit * kDecPart;
     float M = -INFINITY;
-    for (int s = 0; s < nsplit; ++s) M = fmaxf(M, p[static_cast<size_t>(s) * kDecPart]);
+    for (int s = 0; s < ns; ++s) M = fmaxf(M, p[static_cast<size_t>(s) * kDecPart]);
     float L = 0.f, O = 0.f;
-    for (int s = 0; s < nsplit; ++s) {
+    for (int s = 0; s < ns; ++s) {
         const float* q = p + static_cast<size_t>(s) * kDecPart;
         const float c = fast_exp2(q[0] - M);
         L = fmaf(q[1], c, L);
@@ -2070,26 +2146,30 @@ static int decode_splits(int n) { return (n + kDecChunk - 1) / kDecChunk; }
 static size_t decode_part_floats(int heads, int n) { return static_cast<size_t>(heads) * decode_splits(n) * kDecPart; }
 
 static int launch_kv_append(const __half* hi, const __half* lo, int T, int heads, int kv_heads, int pos0, int cap,
-                            __half* kv, cudaStream_t st) {
+                            __half* kv, cudaStream_t st, const int* pos = nullptr, const int* shift = nullptr) {
     const size_t n = static_cast<size_t>(T) * kv_heads * (kQwenHD / 8);
     ProfScope _ps(PROF_DECODE_ATTN, st);
-    kv_append_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(hi, lo, T, heads, kv_heads, pos0, cap, kv);
+    kv_append_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(hi, lo, T, heads, kv_heads, pos0, cap, kv,
+                                                                              pos, shift);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
 }
 
-// one query row q [heads 128] against cache rows [0, n) of one layer's kv -> ctx [heads 128]
+// one query row q [heads 128] against cache rows [0, n) of one layer's kv -> ctx [heads 128]; with rows.pos, B rows
+// (DecRows) of at most n keys each -> ctx [B, heads 128]
 static int launch_attention_decode(const __half* q_hi, const __half* q_lo, const __half* kv, int heads, int kv_heads,
-                                   int cap, int n, float* part, __half* ctx_hi, __half* ctx_lo, cudaStream_t st) {
+                                   int cap, int n, float* part, __half* ctx_hi, __half* ctx_lo, cudaStream_t st,
+                                   int B = 1, DecRows rows = DecRows{}) {
     const int G = heads / kv_heads, ns = decode_splits(n);
+    rows.gz = (G + kDecMaxG - 1) / kDecMaxG;
     ProfScope _ps(PROF_DECODE_ATTN, st);
-    const dim3 grid(static_cast<unsigned>(kv_heads), static_cast<unsigned>(ns),
-                    static_cast<unsigned>((G + kDecMaxG - 1) / kDecMaxG));
-    attention_decode_kernel<<<grid, kDecThreads, 0, st>>>(q_hi, q_lo, kv, heads, kv_heads, cap, n, ns, part);
+    const dim3 grid(static_cast<unsigned>(kv_heads), static_cast<unsigned>(ns), static_cast<unsigned>(B * rows.gz));
+    attention_decode_kernel<<<grid, kDecThreads, 0, st>>>(q_hi, q_lo, kv, heads, kv_heads, cap, n, ns, part, rows);
     count_launch();
     RMU_CHECK_LAUNCH();
-    attention_decode_combine_kernel<<<static_cast<unsigned>(heads), kDecThreads, 0, st>>>(part, ns, ctx_hi, ctx_lo);
+    attention_decode_combine_kernel<<<static_cast<unsigned>(B * heads), kDecThreads, 0, st>>>(part, ns, ctx_hi, ctx_lo,
+                                                                                               rows.pos, heads);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
@@ -2108,7 +2188,8 @@ __global__ void set_int_kernel(int* p, int v) { *p = v; }
 // The candidates are the index's top-k tail (rmu_topk.cuh): keys (score desc, index asc), a radix select of the k-th
 // and of the kSampleCap-th key, the keys above the higher of the two, a bitonic sort.  Weights exp(x - max) are float64,
 // summed in a fixed order by one thread.  u is u_in when u_in >= 0, else the Philox4x32-10 uniform of (seed, step).
-// The chosen id is written to *token and its presence bit set.
+// The chosen id is written to *token and its presence bit set.  The batched decode runs one CTA per live row r
+// (SampleRows): logits row r, token r, and the presence bits and Philox seed of the row's sequence seq[r].
 // ---------------------------------------------------------------------------------------------------
 constexpr int kSampleThreads = 1024;
 constexpr int kSampleCap = 256;               // the largest top_k and the most candidates
@@ -2116,6 +2197,12 @@ constexpr int kSampleCap = 256;               // the largest top_k and the most 
 struct SampleArgs {
     int do_sample, top_k;
     float temperature, top_p, penalty;
+};
+
+struct SampleRows {
+    const int* seq = nullptr;                     // null: one row, `seed`, presence at its start
+    const unsigned long long* seeds = nullptr;    // [sequences]
+    size_t words = 0;                             // presence words per sequence
 };
 
 // Philox4x32-10 (Salmon et al., SC'11) with counter (step, 0) and key seed: the first output word's high 24 bits / 2^24
@@ -2135,13 +2222,20 @@ __host__ __device__ inline float philox_uniform(unsigned long long seed, unsigne
 __global__ void __launch_bounds__(kSampleThreads) sample_kernel(float* __restrict__ logits, int V,
                                                                 unsigned* __restrict__ presence, SampleArgs a, float u_in,
                                                                 unsigned long long seed, unsigned long long step,
-                                                                int* __restrict__ token) {
+                                                                int* __restrict__ token, SampleRows rows) {
     __shared__ unsigned long long sel[kSel2Max];
     __shared__ int hist[256];
     __shared__ unsigned long long s_prefix, s_best[kSampleThreads / 32];
     __shared__ int s_remaining, s_ties, s_cnt;
     __shared__ double w[kSampleCap];
     const int tid = threadIdx.x;
+    if (rows.seq) {
+        const int q = rows.seq[blockIdx.x];
+        logits += static_cast<size_t>(blockIdx.x) * V;
+        token += blockIdx.x;
+        presence += q * rows.words;
+        seed = rows.seeds[q];
+    }
     unsigned long long best = 0ull;
     for (int i = tid; i < V; i += blockDim.x) {
         float x = logits[i];
@@ -2203,9 +2297,9 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(float* __restric
 }
 
 static int launch_sample(float* logits, int V, unsigned* presence, const SampleArgs& a, float u_in, unsigned long long seed,
-                         unsigned long long step, int* token, cudaStream_t st) {
+                         unsigned long long step, int* token, cudaStream_t st, int B = 1, SampleRows rows = SampleRows{}) {
     ProfScope _ps(PROF_SAMPLE, st);
-    sample_kernel<<<1, kSampleThreads, 0, st>>>(logits, V, presence, a, u_in, seed, step, token);
+    sample_kernel<<<B, kSampleThreads, 0, st>>>(logits, V, presence, a, u_in, seed, step, token, rows);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
@@ -2297,6 +2391,8 @@ struct rmu_encoder {
     float* lm_zero = nullptr;
     DevBuf kv_cache, gen_ws;
     int kv_cap = 0;
+    // rmu_decoder_generate_batch's own workspace (run_batch_prefill, the batched decode steps), grown under mu
+    DevBuf batch_ws;
     // NF4 weights (rmu_decoder_quantize_nf4): the layers' projections live in EncLayer::nf4; a prefill dequantises
     // each into the one scratch operand set nf4_hi | nf4_lo (lo all zero), seen through nf4_op[projection]'s tensor
     // maps.  nf4_broken: a conversion failed part-way and the handle cannot run.  nf4_peak / nf4_delta: the most the
@@ -2670,21 +2766,25 @@ static int run_encoder(rmu_encoder* e, const int32_t* ids, const int32_t* type_i
 }
 
 // projection `which` (0 Wqkv, 1 Wo, 2 W1, 3 W2) of a decoder layer, C = A W^T with E1's epilogue `mode`.  Split
-// planes: E1.  NF4: the decode GEMV at M = 1; otherwise the weight dequantised into the scratch planes, then E1 on
-// them (the scratch is reused by the next projection in stream order).
+// planes: E1.  NF4 with `gemv` (a decode step, or the prefill of a one-token prompt): the decode GEMV, one row or
+// several; otherwise the weight dequantised into the scratch planes, then E1 on them (the scratch is reused by the
+// next projection in stream order).  The caller chooses by the prompt, not by M: a batched prefill's chunk of one
+// row takes the path the whole prompt's prefill takes.
 static SplitOperand EncLayer::* const kDecoderSplit[4] = {&EncLayer::Wqkv, &EncLayer::Wo, &EncLayer::W1, &EncLayer::W2};
 
 static int decoder_gemm(rmu_encoder* e, int mode, const SplitOperand& A, const EncLayer& L, int which, const GemmParams& g,
-                        cudaStream_t st) {
+                        bool gemv, cudaStream_t st) {
     if (!e->nf4) return launch_gemm(mode, A, L.*kDecoderSplit[which], g, e->sms, st);
     const Nf4Weight& W = L.nf4[which];
-    if (g.M == 1) return launch_nf4_gemv(mode, A.hi, A.lo, W, g, e->sms, st);
+    if (gemv)
+        return g.M == 1 ? launch_nf4_gemv(mode, A.hi, A.lo, W, g, e->sms, st)
+                        : launch_nf4_gemv_rows(mode, A.hi, A.lo, W, g, e->sms, st);
     const int rc = launch_nf4_dequantize(W.codes, W.absmax, static_cast<int64_t>(W.rows) * W.cols, e->nf4_hi, st);
     return rc != RMU_OK ? rc : launch_gemm(mode, A, e->nf4_op[which], g, e->sms, st);
 }
 
 // one decoder layer up to its attention inputs: X = split(w_in RMS(h)); QKVF = X Wqkv^T (fp32); QKVP = the q / k step
-static int qwen3_attention_inputs(rmu_encoder* e, const EncLayer& L, int T, cudaStream_t st) {
+static int qwen3_attention_inputs(rmu_encoder* e, const EncLayer& L, int T, bool gemv, cudaStream_t st) {
     const rmu_bert_config& c = e->cfg;
     const int nh = c.heads, kv = e->qext.kv_heads, NQKV = (nh + 2 * kv) * kQwenHD;
     const float qscale = 1.4426950408889634f / sqrtf(static_cast<float>(kQwenHD));
@@ -2692,7 +2792,7 @@ static int qwen3_attention_inputs(rmu_encoder* e, const EncLayer& L, int T, cuda
     if (rc != RMU_OK) return rc;
     GemmParams g{};
     g.M = T; g.N = NQKV; g.K = c.hidden; g.bias = e->zeros; g.out_f32 = e->QKVF;
-    rc = decoder_gemm(e, GEMM_BIAS_F32, e->X, L, 0, g, st);
+    rc = decoder_gemm(e, GEMM_BIAS_F32, e->X, L, 0, g, gemv, st);
     if (rc != RMU_OK) return rc;
     return launch_qk_norm_rope(e->QKVF, T, nh, kv, e->POSI, L.qn, L.kn, c.ln_eps, qscale, e->rope_cos[0], e->rope_sin[0],
                                c.max_pos, e->QKVP.hi, e->QKVP.lo, e->range_flag, st);
@@ -2700,21 +2800,21 @@ static int qwen3_attention_inputs(rmu_encoder* e, const EncLayer& L, int T, cuda
 
 // one decoder layer after its attention, on M rows: h += CTX Wo^T (in place); X = split(w_post RMS(h)); FF =
 // split(silu(X Wgate^T) * (X Wup^T)); h += FF Wdown^T
-static int qwen3_layer_tail(rmu_encoder* e, const EncLayer& L, int M, cudaStream_t st) {
+static int qwen3_layer_tail(rmu_encoder* e, const EncLayer& L, int M, bool gemv, cudaStream_t st) {
     const rmu_bert_config& c = e->cfg;
     const int H = c.hidden, F = c.ffn, QD = c.heads * kQwenHD;
     GemmParams g{};
     g.M = M; g.N = H; g.K = QD; g.bias = e->zeros; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
-    int rc = decoder_gemm(e, GEMM_BIAS_RESF32_F32, e->CTX, L, 1, g, st);
+    int rc = decoder_gemm(e, GEMM_BIAS_RESF32_F32, e->CTX, L, 1, g, gemv, st);
     if (rc == RMU_OK) rc = launch_rms_split(e->PRE, M, H, L.ln2g, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
     if (rc != RMU_OK) return rc;
     g = GemmParams{};
     g.M = M; g.N = 2 * F; g.K = H; g.bias = e->zeros; g.out_hi = e->FF.hi; g.out_lo = e->FF.lo; g.range_flag = e->range_flag;
-    rc = decoder_gemm(e, GEMM_BIAS_SWIGLU_SPLIT, e->X, L, 2, g, st);
+    rc = decoder_gemm(e, GEMM_BIAS_SWIGLU_SPLIT, e->X, L, 2, g, gemv, st);
     if (rc != RMU_OK) return rc;
     g = GemmParams{};
     g.M = M; g.N = H; g.K = F; g.bias = e->zeros; g.out_f32 = e->PRE; g.res_f32 = e->PRE;
-    return decoder_gemm(e, GEMM_BIAS_RESF32_F32, e->FF, L, 3, g, st);
+    return decoder_gemm(e, GEMM_BIAS_RESF32_F32, e->FF, L, 3, g, gemv, st);
 }
 
 // layer l's K / V planes in the KV cache (kv_append_kernel's layout)
@@ -2757,12 +2857,12 @@ static int run_qwen3(rmu_encoder* e, const int32_t* ids, const int32_t* cu, int 
     if (rc != RMU_OK) return rc;
     for (int l = 0; l < c.layers; ++l) {
         const EncLayer& L = e->layers[l];
-        rc = qwen3_attention_inputs(e, L, T, st);
+        rc = qwen3_attention_inputs(e, L, T, T == 1, st);
         if (rc != RMU_OK || (attn_last && l == c.layers - 1)) return rc;
         if (to_cache) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, T, nh, kv, 0, e->kv_cap, kv_layer(e, l), st);
         if (rc == RMU_OK)
             rc = launch_attention_causal(e->QKVP.hi, e->QKVP.lo, cu, B, nh, kv, max_seqlen, e->CTX.hi, e->CTX.lo, st);
-        if (rc == RMU_OK) rc = qwen3_layer_tail(e, L, T, st);
+        if (rc == RMU_OK) rc = qwen3_layer_tail(e, L, T, T == 1, st);
         if (rc != RMU_OK) return rc;
     }
     return RMU_OK;
@@ -2779,6 +2879,31 @@ static int qwen3_check_range(rmu_encoder* e, cudaStream_t st) {
         return RMU_ERR_RANGE;
     }
     return RMU_OK;
+}
+
+// One prefill run of rmu_decoder_generate_batch over B sequences of T token rows in all (cu [B + 1]): each row's
+// position and cache row offset are in e->POSI and shift (uploaded by the caller), so token t of sequence b is at
+// position P + t and its k / v go to cache row P + t + shift; attention is attention_causal_kernel's cached form
+// (PrefixKeys), keys below P from the shared prefix rows.  The range flag is not cleared: the caller clears it once
+// per call.  The activation workspace must already hold T rows (ensure_tokens).
+static int run_batch_prefill(rmu_encoder* e, const int32_t* ids, const int32_t* cu, const int* shift, int B, int T,
+                             int max_own, int P, bool gemv, cudaStream_t st) {
+    const rmu_bert_config& c = e->cfg;
+    const int nh = c.heads, kv = e->qext.kv_heads;
+    int rc = launch_embed_rows(ids, T, c.hidden, c.vocab_size, e->word, e->PRE, st);
+    for (int l = 0; l < c.layers && rc == RMU_OK; ++l) {
+        const EncLayer& L = e->layers[l];
+        rc = qwen3_attention_inputs(e, L, T, gemv, st);
+        if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, T, nh, kv, 0, e->kv_cap, kv_layer(e, l), st, e->POSI, shift);
+        PrefixKeys pk;
+        pk.kv = kv_layer(e, l);
+        pk.shift = shift;
+        pk.cap = e->kv_cap;
+        pk.P = P;
+        if (rc == RMU_OK) rc = launch_attention_cached(e->QKVP.hi, e->QKVP.lo, cu, B, nh, kv, max_own, pk, e->CTX.hi, e->CTX.lo, st);
+        if (rc == RMU_OK) rc = qwen3_layer_tail(e, L, T, gemv, st);
+    }
+    return rc;
 }
 
 // the sampling settings rmu_decoder_generate and rmu_debug_sample refuse, before any CUDA call
@@ -3650,12 +3775,12 @@ int rmu_decoder_generate(rmu_encoder* e, const int32_t* ids_h, int T, const rmu_
             rc = launch_embed_rows(tok, 1, H, V, e->word, e->PRE, st);
             for (int l = 0; l < L && rc == RMU_OK; ++l) {
                 const EncLayer& Ly = e->layers[l];
-                rc = qwen3_attention_inputs(e, Ly, 1, st);
+                rc = qwen3_attention_inputs(e, Ly, 1, true, st);
                 if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, 1, nh, kv, p, e->kv_cap, kv_layer(e, l), st);
                 if (rc == RMU_OK)
                     rc = launch_attention_decode(e->QKVP.hi, e->QKVP.lo, kv_layer(e, l), nh, kv, e->kv_cap, p + 1, part,
                                                  e->CTX.hi, e->CTX.lo, st);
-                if (rc == RMU_OK) rc = qwen3_layer_tail(e, Ly, 1, st);
+                if (rc == RMU_OK) rc = qwen3_layer_tail(e, Ly, 1, true, st);
             }
             last = e->PRE;
         }
@@ -3682,6 +3807,219 @@ int rmu_decoder_generate(rmu_encoder* e, const int32_t* ids_h, int T, const rmu_
         if (eos || n == max_new_tokens || T + n >= c.max_pos) break;
     }
     *n_out = n;
+    if (rc != RMU_OK) return rc;
+    RMU_CUDA(cudaEventRecord(e->ws_done, st));
+    return RMU_OK;
+}
+
+// The batch layout.  P = the prompts' longest common prefix, capped so that every prompt keeps one own token (0 when
+// B = 1).  Per layer the KV cache holds the prefix at rows 0 .. P - 1 and prompt b's own keys (positions P ..) in rows
+// P + b R + (k - P), R = the most own positions any prompt can reach.  The prefix runs once; the suffixes run as one
+// varlen prefill at positions P + t (a one-token prompt of an NF4 handle runs alone, on the GEMV its own prefill takes);
+// each decode step runs the live rows at M = live, decode attention over [prefix | own region].  Row b's tokens and
+// logits are those of rmu_decoder_generate on prompt b with seeds_h[b] (DESIGN.md, "Batched decoding").
+int rmu_decoder_generate_batch(rmu_encoder* e, const int32_t* ids_h, const int32_t* cu_h, int B, const rmu_sampling* s,
+                               const uint64_t* seeds_h, int max_new_tokens, int32_t* out_h, int32_t* n_out_h,
+                               float* logits_h, void* stream) {
+    const std::string fn("rmu_decoder_generate_batch");
+    if (!e || !ids_h || !cu_h || !s || !seeds_h || !out_h || !n_out_h || B < 1 || max_new_tokens < 1) {
+        set_error(fn + ": bad argument");
+        return RMU_ERR_ARG;
+    }
+    // 0 until the call succeeds: any failure, refusal or CUDA error, leaves every count 0
+    for (int b = 0; b < std::min(B, RMU_MAX_GENERATE_BATCH); ++b) n_out_h[b] = 0;
+    if (B > RMU_MAX_GENERATE_BATCH) {
+        set_error(fn + ": at most " + std::to_string(RMU_MAX_GENERATE_BATCH) + " prompts per call, got " + std::to_string(B));
+        return RMU_ERR_ARG;
+    }
+    for (int b = 0; b < B; ++b)
+        if (cu_h[b + 1] <= cu_h[b] || cu_h[b] < 0) { set_error(fn + ": prompt " + std::to_string(b) + " is empty"); return RMU_ERR_ARG; }
+    int rc = check_decoder(e, fn);
+    if (rc != RMU_OK) return rc;
+    if (!e->has_lm_head) { set_error(fn + ": no LM head is attached (rmu_decoder_set_lm_head)"); return RMU_ERR_ARG; }
+    rc = check_nf4_intact(e, fn);
+    if (rc != RMU_OK) return rc;
+    const rmu_bert_config& c = e->cfg;
+    std::vector<int> Tb(B);
+    for (int b = 0; b < B; ++b) {
+        Tb[b] = cu_h[b + 1] - cu_h[b];
+        if (Tb[b] >= c.max_pos) {
+            set_error(fn + ": a prompt of " + std::to_string(Tb[b]) + " tokens leaves no position for a new token " +
+                      "(max_position_embeddings " + std::to_string(c.max_pos) + ")");
+            return RMU_ERR_ARG;
+        }
+    }
+    rc = check_sampling(fn, s);
+    if (rc != RMU_OK) return rc;
+    for (int i = cu_h[0]; i < cu_h[B]; ++i)
+        if (ids_h[i] < 0 || ids_h[i] >= c.vocab_size) { set_error(fn + ": token id out of range"); return RMU_ERR_ARG; }
+    const int32_t* prompt0 = ids_h + cu_h[0];
+    int P = B > 1 ? Tb[0] - 1 : 0;
+    for (int b = 1; b < B; ++b) {
+        P = std::min(P, Tb[b] - 1);
+        const int32_t* pb = ids_h + cu_h[b];
+        for (int i = 0; i < P; ++i)
+            if (pb[i] != prompt0[i]) { P = i; break; }
+    }
+    // own positions: prompt b reaches at most min(T_b + max_new, max_pos) - 1
+    int R = 1, most = 1;
+    for (int b = 0; b < B; ++b) {
+        const int end = std::min(Tb[b] + max_new_tokens, c.max_pos);
+        R = std::max(R, end - P);
+        most = std::max(most, end);
+    }
+    std::lock_guard<std::mutex> hg(e->host_mu);
+    std::lock_guard<std::mutex> g(e->mu);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int V = c.vocab_size, H = c.hidden, nh = c.heads, kv = e->qext.kv_heads, L = c.layers;
+    const int cap = P + B * R;
+    if (cap > e->kv_cap) {
+        e->kv_cap = 0;                                  // until grow succeeds: it may free the old cache first
+        rc = grow(e->kv_cache, static_cast<size_t>(L) * 4 * kv * cap * kQwenHD * sizeof(__half));
+        if (rc != RMU_OK) {
+            set_error(fn + ": the KV cache for " + std::to_string(cap) + " positions: " + rmu_last_error());
+            return rc;
+        }
+        e->kv_cap = cap;
+    }
+    // prefill groups: the prefix, the one-token prompts of an NF4 handle one by one, the other suffixes together
+    std::vector<int> group, solo;
+    for (int b = 0; b < B; ++b) (e->nf4 && Tb[b] == 1 ? solo : group).push_back(b);
+    int suffix_rows = 0;
+    for (int b : group) suffix_rows += Tb[b] - P;
+    const int rows_most = std::max({P, suffix_rows, B});
+    // batch_ws: logits [B, V] | last hidden rows [B, H] | decode partials | presence [B, words] | seeds [B] | tokens
+    // [B] | ints (ids, cu, shift of a prefill run; ids, shift, seq of a step)
+    const size_t words = (static_cast<size_t>(V) + 31) / 32;
+    auto al = [](size_t bytes) { return (bytes + 255) / 256 * 256; };
+    const size_t o_last = al(static_cast<size_t>(B) * V * 4), o_part = o_last + al(static_cast<size_t>(B) * H * 4);
+    const size_t o_pres = o_part + al(static_cast<size_t>(B) * decode_part_floats(nh, most) * 4);
+    const size_t o_seed = o_pres + al(static_cast<size_t>(B) * words * 4), o_tok = o_seed + al(static_cast<size_t>(B) * 8);
+    const size_t o_int = o_tok + al(static_cast<size_t>(B) * 4);
+    const size_t n_int = 2 * static_cast<size_t>(rows_most) + B + 1 + 3 * static_cast<size_t>(B);
+    rc = grow(e->batch_ws, o_int + n_int * 4);
+    if (rc == RMU_OK) rc = ensure_tokens(e, rows_most, B);
+    if (rc != RMU_OK) return rc;
+    char* base = e->batch_ws.as<char>();
+    float* logits = reinterpret_cast<float*>(base);
+    float* last = reinterpret_cast<float*>(base + o_last);
+    float* part = reinterpret_cast<float*>(base + o_part);
+    unsigned* presence = reinterpret_cast<unsigned*>(base + o_pres);
+    unsigned long long* seeds = reinterpret_cast<unsigned long long*>(base + o_seed);
+    int* tok = reinterpret_cast<int*>(base + o_tok);
+    int* ints = reinterpret_cast<int*>(base + o_int);
+    std::vector<unsigned> bits(static_cast<size_t>(B) * words, 0u);
+    for (int b = 0; b < B; ++b)
+        for (int i = cu_h[b]; i < cu_h[b + 1]; ++i) bits[b * words + (ids_h[i] >> 5)] |= 1u << (ids_h[i] & 31);
+    RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace is shared by all callers
+    RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
+    // pageable sources: each copy has taken its bytes when it returns
+    RMU_CUDA(cudaMemcpyAsync(presence, bits.data(), bits.size() * 4, cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(seeds, seeds_h, static_cast<size_t>(B) * 8, cudaMemcpyHostToDevice, st));
+    // one prefill run over the sequences `seqs` from token `from` of each: ids | cu | shift into ints, positions into
+    // POSI; the last row of each goes to last[b] (gather)
+    auto prefill = [&](const std::vector<int>& seqs, int from, int p0, bool gather, bool gemv) -> int {
+        std::vector<int> hid, hcu{0}, hshift, hpos;
+        int max_own = 0;
+        for (int b : seqs) {
+            const int n = (gather ? Tb[b] : p0) - from;
+            for (int t = 0; t < n; ++t) {
+                hid.push_back(ids_h[cu_h[b] + from + t]);
+                hpos.push_back(from + t);
+                hshift.push_back(gather ? b * R : 0);
+            }
+            hcu.push_back(hcu.back() + n);
+            max_own = std::max(max_own, n);
+        }
+        const int n = hcu.back(), nb = static_cast<int>(seqs.size());
+        std::vector<int> packed(hid);
+        packed.insert(packed.end(), hcu.begin(), hcu.end());
+        packed.insert(packed.end(), hshift.begin(), hshift.end());
+        RMU_CUDA(cudaMemcpyAsync(ints, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice, st));
+        RMU_CUDA(cudaMemcpyAsync(e->POSI, hpos.data(), hpos.size() * 4, cudaMemcpyHostToDevice, st));
+        int r = run_batch_prefill(e, ints, ints + n, ints + n + nb + 1, nb, n, max_own, gather ? P : 0, gemv, st);
+        for (int i = 0; i < nb && r == RMU_OK && gather; ++i)
+            RMU_CUDA(cudaMemcpyAsync(last + static_cast<size_t>(seqs[i]) * H, e->PRE + static_cast<size_t>(hcu[i + 1] - 1) * H,
+                                     static_cast<size_t>(H) * 4, cudaMemcpyDeviceToDevice, st));
+        return r;
+    };
+    if (P > 0) rc = prefill({0}, 0, P, false, false);
+    for (int b : solo)
+        if (rc == RMU_OK) rc = prefill({b}, 0, 0, true, true);
+    if (rc == RMU_OK && !group.empty()) rc = prefill(group, P, 0, true, false);
+
+    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
+    std::vector<int> live(B), n_b(B, 0), last_tok(B, 0);
+    for (int b = 0; b < B; ++b) live[b] = b;
+    const float* x_last = last;
+    for (int step = 0; rc == RMU_OK && !live.empty(); ++step) {
+        const int M = static_cast<int>(live.size());
+        // ints: ids [M] | shift [M] | seq [M]; POSI: the positions of the tokens this step feeds
+        std::vector<int> packed(3 * static_cast<size_t>(M)), hpos(M);
+        for (int r = 0; r < M; ++r) {
+            const int b = live[r];
+            packed[r] = last_tok[b];
+            packed[M + r] = b * R;
+            packed[2 * M + r] = b;
+            hpos[r] = Tb[b] + n_b[b] - 1;
+        }
+        RMU_CUDA(cudaMemcpyAsync(ints, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice, st));
+        if (step > 0) {
+            int maxn = 0;
+            for (int r = 0; r < M; ++r) maxn = std::max(maxn, hpos[r] + 1);
+            RMU_CUDA(cudaMemcpyAsync(e->POSI, hpos.data(), hpos.size() * 4, cudaMemcpyHostToDevice, st));
+            rc = launch_embed_rows(ints, M, H, V, e->word, e->PRE, st);
+            DecRows dr;
+            dr.pos = e->POSI;
+            dr.shift = ints + M;
+            dr.P = P;
+            dr.qld = static_cast<size_t>(nh + 2 * kv) * kQwenHD;
+            for (int l = 0; l < L && rc == RMU_OK; ++l) {
+                const EncLayer& Ly = e->layers[l];
+                rc = qwen3_attention_inputs(e, Ly, M, true, st);
+                if (rc == RMU_OK)
+                    rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, M, nh, kv, 0, e->kv_cap, kv_layer(e, l), st, e->POSI, ints + M);
+                if (rc == RMU_OK)
+                    rc = launch_attention_decode(e->QKVP.hi, e->QKVP.lo, kv_layer(e, l), nh, kv, e->kv_cap, maxn, part,
+                                                 e->CTX.hi, e->CTX.lo, st, M, dr);
+                if (rc == RMU_OK) rc = qwen3_layer_tail(e, Ly, M, true, st);
+            }
+            x_last = e->PRE;
+        }
+        // logits = lm_head . (w_norm RMS(h_last)) for the M live rows (step 0: last[b] in prompt order), then the sampler
+        if (rc == RMU_OK) rc = launch_rms_split(x_last, M, H, e->fng, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
+        if (rc == RMU_OK) {
+            ProfScope _ps(PROF_LM_HEAD, st);
+            GemmParams gp{};
+            gp.M = M; gp.N = V; gp.K = H; gp.bias = e->lm_zero; gp.out_f32 = logits;
+            rc = launch_gemm(GEMM_BIAS_F32, e->X, e->lm_head, gp, e->sms, st);
+        }
+        for (int r = 0; r < M && rc == RMU_OK && logits_h; ++r)
+            RMU_CUDA(cudaMemcpyAsync(logits_h + (static_cast<size_t>(live[r]) * max_new_tokens + step) * V,
+                                     logits + static_cast<size_t>(r) * V, static_cast<size_t>(V) * sizeof(float),
+                                     cudaMemcpyDeviceToHost, st));
+        SampleRows sr;
+        sr.seq = ints + 2 * M;
+        sr.seeds = seeds;
+        sr.words = words;
+        if (rc == RMU_OK) rc = launch_sample(logits, V, presence, sa, -1.f, 0ull, static_cast<unsigned long long>(step), tok, st, M, sr);
+        if (rc != RMU_OK) break;
+        std::vector<int> t_h(M);
+        RMU_CUDA(cudaMemcpyAsync(t_h.data(), tok, static_cast<size_t>(M) * sizeof(int), cudaMemcpyDeviceToHost, st));
+        rc = qwen3_check_range(e, st);        // synchronises st
+        if (rc != RMU_OK) break;
+        std::vector<int> next;
+        for (int r = 0; r < M; ++r) {
+            const int b = live[r];
+            out_h[static_cast<size_t>(b) * max_new_tokens + n_b[b]++] = t_h[r];
+            last_tok[b] = t_h[r];
+            bool eos = false;
+            for (int i = 0; i < s->n_eos; ++i) eos |= t_h[r] == s->eos_ids[i];
+            if (!(eos || n_b[b] == max_new_tokens || Tb[b] + n_b[b] >= c.max_pos)) next.push_back(b);
+        }
+        live.swap(next);
+    }
+    for (int b = 0; b < B; ++b) n_out_h[b] = rc == RMU_OK ? n_b[b] : 0;
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
@@ -4237,6 +4575,65 @@ int rmu_debug_attention_decode(const uint16_t* q_hi, const uint16_t* q_lo, const
                                    static_cast<cudaStream_t>(stream));
 }
 
+int rmu_debug_attention_decode_rows(const uint16_t* q_hi, const uint16_t* q_lo, int64_t qld, int B, const uint16_t* kv,
+                                    int heads, int kv_heads, int cap, int P, const int32_t* pos_h, const int32_t* shift_h,
+                                    float* ws, int64_t ws_elems, uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream) {
+    const std::string fn("rmu_debug_attention_decode_rows");
+    if (!q_hi || !q_lo || !kv || !pos_h || !shift_h || !ws || !ctx_hi || !ctx_lo || B < 1 || B > 65535 || heads < 1 ||
+        kv_heads < 1 || P < 0 || qld < static_cast<int64_t>(heads) * kQwenHD) {
+        set_error(fn + ": bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (heads % kv_heads != 0) { set_error(fn + ": heads % kv_heads != 0"); return RMU_ERR_UNSUPPORTED; }
+    int n = 1;
+    for (int b = 0; b < B; ++b) {
+        // every key the row reads lies in [0, cap): the prefix rows and its own rows pos + shift
+        if (pos_h[b] < 0 || shift_h[b] < 0 || std::min(pos_h[b] + 1, P) > cap ||
+            (pos_h[b] >= P && static_cast<int64_t>(pos_h[b]) + shift_h[b] >= cap)) {
+            set_error(fn + ": row " + std::to_string(b) + " reads past the cache");
+            return RMU_ERR_ARG;
+        }
+        n = std::max(n, pos_h[b] + 1);
+    }
+    const size_t part = static_cast<size_t>(B) * decode_part_floats(heads, n);
+    if (ws_elems < 0 || static_cast<size_t>(ws_elems) < part + 2 * static_cast<size_t>(B)) {
+        set_error(fn + ": the workspace needs " + std::to_string(part + 2 * static_cast<size_t>(B)) + " floats");
+        return RMU_ERR_ARG;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int* rows = reinterpret_cast<int*>(ws + part);
+    RMU_CUDA(cudaMemcpyAsync(rows, pos_h, static_cast<size_t>(B) * sizeof(int), cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(rows + B, shift_h, static_cast<size_t>(B) * sizeof(int), cudaMemcpyHostToDevice, st));
+    DecRows dr;
+    dr.pos = rows;
+    dr.shift = rows + B;
+    dr.P = P;
+    dr.qld = static_cast<size_t>(qld);
+    return launch_attention_decode(reinterpret_cast<const __half*>(q_hi), reinterpret_cast<const __half*>(q_lo),
+                                   reinterpret_cast<const __half*>(kv), heads, kv_heads, cap, n, ws,
+                                   reinterpret_cast<__half*>(ctx_hi), reinterpret_cast<__half*>(ctx_lo), st, B, dr);
+}
+
+int rmu_debug_attention_cached(const uint16_t* qkv_hi, const uint16_t* qkv_lo, const int32_t* cu, int B, int heads,
+                               int kv_heads, const uint16_t* kv, int cap, int P, const int32_t* shift, int max_own,
+                               uint16_t* ctx_hi, uint16_t* ctx_lo, void* stream) {
+    const std::string fn("rmu_debug_attention_cached");
+    if (!qkv_hi || !qkv_lo || !cu || !kv || !shift || !ctx_hi || !ctx_lo || B < 1 || B > kMaxGridY || heads < 1 ||
+        kv_heads < 1 || P < 0 || max_own < 1 || cap < P) {
+        set_error(fn + ": bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (heads % kv_heads != 0) { set_error(fn + ": heads must be a multiple of kv_heads"); return RMU_ERR_UNSUPPORTED; }
+    PrefixKeys pk;
+    pk.kv = reinterpret_cast<const __half*>(kv);
+    pk.shift = shift;
+    pk.cap = cap;
+    pk.P = P;
+    return launch_attention_cached(reinterpret_cast<const __half*>(qkv_hi), reinterpret_cast<const __half*>(qkv_lo), cu, B,
+                                   heads, kv_heads, max_own, pk, reinterpret_cast<__half*>(ctx_hi),
+                                   reinterpret_cast<__half*>(ctx_lo), static_cast<cudaStream_t>(stream));
+}
+
 int rmu_debug_kv_append(const uint16_t* hi, const uint16_t* lo, int T, int heads, int kv_heads, int pos0, int cap,
                         uint16_t* kv, void* stream) {
     if (!hi || !lo || !kv || T < 1 || heads < 1 || kv_heads < 1 || pos0 < 0 ||
@@ -4289,6 +4686,34 @@ int rmu_debug_nf4_gemv(int mode, const uint16_t* x_hi, const uint16_t* x_lo, con
                            device_sm_count(), static_cast<cudaStream_t>(stream));
 }
 
+int rmu_debug_nf4_gemv_rows(int mode, int M, const uint16_t* x_hi, const uint16_t* x_lo, const uint8_t* codes,
+                            const float* absmax, int N, int K, const float* bias, const float* res_f32, float* out_f32,
+                            uint16_t* out_hi, uint16_t* out_lo, int32_t* range_flag, void* stream) {
+    const std::string fn("rmu_debug_nf4_gemv_rows");
+    if (mode != GEMM_BIAS_F32 && mode != GEMM_BIAS_RESF32_F32 && mode != GEMM_BIAS_SWIGLU_SPLIT) {
+        set_error(fn + ": mode must be 0, 6 or 7");
+        return RMU_ERR_ARG;
+    }
+    const bool swiglu = mode == GEMM_BIAS_SWIGLU_SPLIT;
+    if (!x_hi || !x_lo || !codes || !absmax || !bias || M < 1 || M > kNf4MaxRows || N < 1 || K < 1 ||
+        (swiglu ? !out_hi || !out_lo : !out_f32) || (mode == GEMM_BIAS_RESF32_F32 && !res_f32)) {
+        set_error(fn + ": bad argument (M must be 1 .. " + std::to_string(kNf4MaxRows) + ")");
+        return RMU_ERR_ARG;
+    }
+    if (N % 128 != 0 || K % kNf4Block != 0 || K > kNf4MaxK) {
+        set_error(fn + ": N must be a multiple of 128 and K a multiple of 64 up to " + std::to_string(kNf4MaxK));
+        return RMU_ERR_UNSUPPORTED;
+    }
+    GemmParams p{};
+    p.M = M; p.N = N; p.K = K; p.bias = bias; p.out_f32 = out_f32; p.res_f32 = res_f32;
+    p.out_hi = reinterpret_cast<__half*>(out_hi); p.out_lo = reinterpret_cast<__half*>(out_lo);
+    p.range_flag = reinterpret_cast<int*>(range_flag);
+    Nf4Weight W;
+    W.codes = const_cast<uint8_t*>(codes); W.absmax = const_cast<float*>(absmax); W.rows = N; W.cols = K;
+    return launch_nf4_gemv_rows(mode, reinterpret_cast<const __half*>(x_hi), reinterpret_cast<const __half*>(x_lo), W, p,
+                                device_sm_count(), static_cast<cudaStream_t>(stream));
+}
+
 int rmu_debug_nf4_conversion(const rmu_encoder* e, int64_t* peak, int64_t* delta) {
     if (!e || !peak || !delta) { set_error("rmu_debug_nf4_conversion: bad argument"); return RMU_ERR_ARG; }
     if (!e->nf4) { set_error("rmu_debug_nf4_conversion: the handle's weights are not NF4"); return RMU_ERR_ARG; }
@@ -4307,6 +4732,23 @@ int rmu_debug_sample(float* logits, int V, uint32_t* presence, const rmu_samplin
     if (rc != RMU_OK) return rc;
     const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
     return launch_sample(logits, V, presence, sa, u, 0ull, 0ull, token, static_cast<cudaStream_t>(stream));
+}
+
+int rmu_debug_sample_rows(float* logits, int V, int B, uint32_t* presence, const int32_t* seq, const uint64_t* seeds,
+                          int64_t step, const rmu_sampling* s, int32_t* token, void* stream) {
+    if (!logits || V < 1 || B < 1 || !presence || !seq || !seeds || !s || !token || step < 0) {
+        set_error("rmu_debug_sample_rows: bad argument");
+        return RMU_ERR_ARG;
+    }
+    const int rc = check_sampling("rmu_debug_sample_rows", s);
+    if (rc != RMU_OK) return rc;
+    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
+    SampleRows sr;
+    sr.seq = seq;
+    sr.seeds = reinterpret_cast<const unsigned long long*>(seeds);
+    sr.words = (static_cast<size_t>(V) + 31) / 32;
+    return launch_sample(logits, V, presence, sa, -1.f, 0ull, static_cast<unsigned long long>(step), token,
+                         static_cast<cudaStream_t>(stream), B, sr);
 }
 
 }  // extern "C"

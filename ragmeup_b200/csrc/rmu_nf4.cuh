@@ -27,5 +27,10 @@ int launch_nf4_dequantize(const uint8_t* codes, const float* absmax, int64_t n, 
 constexpr int kNf4MaxK = 49152;           // x staged in shared memory as fp32: 192 KB
 int launch_nf4_gemv(int mode, const __half* x_hi, const __half* x_lo, const Nf4Weight& W, const GemmParams& p,
                     int sms, cudaStream_t st);
+// the same GEMV on p.M <= kNf4MaxRows rows x [M, K] (row pitch K; out row pitch p.out_ld, or N, N / 2 for SwiGLU),
+// each row's bits those of launch_nf4_gemv on that row alone
+constexpr int kNf4MaxRows = 16;
+int launch_nf4_gemv_rows(int mode, const __half* x_hi, const __half* x_lo, const Nf4Weight& W, const GemmParams& p,
+                         int sms, cudaStream_t st);
 
 }  // namespace rmu

@@ -1,10 +1,13 @@
 """Provenance attribution helpers that reuse the encoder / cross-encoder / cosine primitives (SURVEY.md §8 row f4).
 
-Drop-ins for the three attribution methods of ``server/provenance.py`` that sit on this path:
+Drop-ins for the four attribution methods of ``server/provenance.py`` that sit on this path:
 
 * ``compute_attention`` (``server/provenance.py:19-98``): how much last-layer attention the query and the answer
   exchange with each retrieved document inside the chat thread, from a Llama or Qwen3 decoder on the GPU
   (``DecoderAttention``).  The decoder sums the softmax over token spans directly; no attention map is stored.
+
+* ``compute_llm_provenance`` (``server/provenance.py:110-141``): ask the chat decoder to score each document for the
+  answer, one scoring prompt per document, every prompt decoded in one batched call (``generate_batch``).
 
 * ``compute_rerank_provenance`` (``server/provenance.py:100-108``): re-score the retrieved documents against
   ``answer`` (or ``query + "\\n" + answer`` when ``attribute_include_query == "True"``) with the reranker.
@@ -19,6 +22,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 import threading
 from typing import Any, List, Optional, Sequence
 
@@ -150,6 +154,43 @@ class DecoderAttention:
                                                        C.byref(n), None, _lib.stream_ptr()), "rmu_decoder_generate")
         return out[:n.value].tolist()
 
+    def generate_batch(self, prompts: Sequence[Sequence[int]], max_new_tokens: int, seeds: Sequence[int],
+                       do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0,
+                       repetition_penalty: float = 1.0, eos_token_ids=()) -> List[List[int]]:
+        """``generate`` on every prompt with its own seed, in calls of up to ``_lib.MAX_GENERATE_BATCH`` prompts
+        (``rmu_decoder_generate_batch``: their common prefix is prefilled once and the decode steps run all live rows
+        together).  Entry b is bit for bit ``generate(prompts[b], max_new_tokens, seed=seeds[b], ...)``."""
+        if len(seeds) != len(prompts):
+            raise ValueError(f"{self.name}: one seed per prompt, got {len(seeds)} for {len(prompts)} prompts")
+        if max_new_tokens < 1 or len(prompts) == 0:
+            return [[] for _ in prompts]
+        eos = [int(t) for t in eos_token_ids]
+        if len(eos) > _lib.MAX_EOS:
+            raise ValueError(f"{self.name}: at most {_lib.MAX_EOS} eos ids, got {len(eos)}")
+        s = _lib.SamplingC(int(bool(do_sample)), float(temperature), float(top_p), float(repetition_penalty),
+                           int(top_k or 0), len(eos), (C.c_int32 * _lib.MAX_EOS)(*eos))
+        enc = self.encoder
+        result: List[List[int]] = []
+        with self.lock, enc.torch.cuda.device(enc.device):
+            if not self._lm_head:
+                W = decoder_lm_head(self.model_name, self.cfg)
+                enc._check(_lib.lib().rmu_decoder_set_lm_head(enc._h, W.ctypes.data), "rmu_decoder_set_lm_head")
+                self._lm_head = True
+            for b0 in range(0, len(prompts), _lib.MAX_GENERATE_BATCH):
+                part = [list(p) for p in prompts[b0:b0 + _lib.MAX_GENERATE_BATCH]]
+                B = len(part)
+                ids = np.ascontiguousarray([t for p in part for t in p], dtype=np.int32)
+                cu = np.ascontiguousarray(np.cumsum([0] + [len(p) for p in part]), dtype=np.int32)
+                sd = np.ascontiguousarray([int(x) & (2 ** 64 - 1) for x in seeds[b0:b0 + B]], dtype=np.uint64)
+                out = np.zeros((B, int(max_new_tokens)), dtype=np.int32)
+                n = np.zeros(B, dtype=np.int32)
+                enc._check(_lib.lib().rmu_decoder_generate_batch(enc._h, ids.ctypes.data, cu.ctypes.data, B, C.byref(s),
+                                                                 sd.ctypes.data, int(max_new_tokens), out.ctypes.data,
+                                                                 n.ctypes.data, None, _lib.stream_ptr()),
+                           "rmu_decoder_generate_batch")
+                result += [out[b, :n[b]].tolist() for b in range(B)]
+        return result
+
 
 DECODER_WEIGHTS = ("split", "nf4")
 DECODER_WEIGHTS_ENV = "RMU_DECODER_WEIGHTS"
@@ -228,3 +269,51 @@ def compute_attention(model: Any, tokenizer: Any, thread: str, query: str, conte
         scores.append(np.mean(kept) if kept else np.float64("nan"))
     mean_total = np.mean(total) if total else np.float64("nan")
     return [np.float64(sc / mean_total) for sc in scores]
+
+
+def _llm_prompt(tokenizer: Any, query: str, doc: Any, answer: str) -> List[int]:
+    """the scoring prompt's ids for one document, as the reference builds it: ``provenance_llm_prompt`` formatted with
+    the query, the document and the answer, as the one user message of the chat template, tokenised by the caller's
+    tokenizer with truncation (and the special tokens it adds).  A ``Document`` gets its page_content's braces doubled
+    in place and is formatted through ``str``, as the reference does; a ``str`` is the document's text."""
+    if isinstance(doc, str):
+        text = doc
+    else:
+        doc.page_content = doc.page_content.replace("{", "{{").replace("}", "}}")
+        text = str(doc)
+    prompt = os.environ["provenance_llm_prompt"].format_map({"query": query, "context": text, "answer": answer})
+    chat = tokenizer.apply_chat_template([{"role": "user", "content": prompt}], tokenize=False)
+    return list(tokenizer(chat, truncation=True)["input_ids"])
+
+
+def _llm_score(tokenizer: Any, ids: Sequence[int], new: Sequence[int]) -> str:
+    """the reference's parse of one reply: the decoded thread after its last ``assistant\n\n`` (ValueError when
+    absent), commas as decimal points, the last number in it (IndexError when there is none)"""
+    text = tokenizer.decode(list(ids) + list(new), skip_special_tokens=True)
+    reply = text[text.rindex("assistant\n\n") + len("assistant\n\n"):]
+    return re.findall(r"\d+\.?\d*", reply.replace(",", "."))[-1]
+
+
+def compute_llm_provenance(tokenizer: Any, model: Any, query: str, context: Sequence[Any], answer: str) -> List[str]:
+    """each document's score as the chat decoder states it (the reference's return value: one string per document).
+    ``model`` resolves through ``_decoder``, so the handle is the one ``compute_attention`` and
+    ``llms.HuggingFacePipeline`` use; the settings are ``model.generation_config`` with ``max_new_tokens=10``, refused
+    as the pipeline refuses them; the seeds are drawn from torch's CPU default generator, one per document in order.
+    Every document is scored against ``answer`` (INTEGRATION.md lists where this differs from the reference)."""
+    import torch
+    from .llms import resolve_settings
+    if os.getenv("force_cpu") == "True":
+        raise _lib.RmuError("force_cpu=True: ragmeup_b200 runs on CUDA (sm_90a) only")
+    dec = _decoder(model)
+    tokenizer.pad_token = tokenizer.eos_token
+    tokenizer.pad_token_id = tokenizer.convert_tokens_to_ids(tokenizer.pad_token)
+    tokenizer.eos_token_id = tokenizer.convert_tokens_to_ids(tokenizer.eos_token)
+    prompts = [_llm_prompt(tokenizer, query, doc, answer) for doc in context]
+    if not prompts:
+        return []
+    settings = resolve_settings(getattr(model, "generation_config", None), {"max_new_tokens": 10},
+                                max(len(p) for p in prompts))
+    max_new = settings.pop("max_new_tokens")
+    seeds = [int(torch.randint(0, 2 ** 63 - 1, (1,)).item()) for _ in prompts]
+    new = dec.generate_batch(prompts, max_new, seeds, **settings)
+    return [_llm_score(tokenizer, p, n) for p, n in zip(prompts, new)]
