@@ -409,6 +409,27 @@ int rmu_decoder_generate(rmu_encoder* enc, const int32_t* ids_h, int T, const rm
 int rmu_decoder_generate_batch(rmu_encoder* enc, const int32_t* ids_h, const int32_t* cu_h, int B, const rmu_sampling* s,
                                const uint64_t* seeds_h, int max_new_tokens, int32_t* out_h, int32_t* n_out_h,
                                float* logits_h, void* stream);
+/* Prompt-lookup decoding (transformers' prompt_lookup_num_tokens): rmu_decoder_generate's tokens and logits, bit for
+ * bit, on split and NF4 handles, greedy and sampled, with fewer model passes when the reply copies the prompt.  After
+ * the prefill each pass feeds the pending token plus k drafts (k = min(lookup_tokens, 15), further capped so that no
+ * pass reaches past max_new_tokens or max_pos; 15 because a pass runs at most RMU_MAX_GENERATE_BATCH rows): the
+ * continuation of the first earlier match of the sequence's last n-gram (rmu_prompt_lookup_draft over the prompt and
+ * the tokens so far, max_length T + max_new_tokens).  The k + 1 rows run as one batched decode step whose row j
+ * computes exactly the sequential step's logits and samples with that step's penalty bits and Philox uniform; the
+ * host keeps row 0's token and row j's while row j - 1's token equals draft j.  logits_h receives the kept rows only.
+ * lookup_tokens 0 runs rmu_decoder_generate's steps.  A pass that raises the fp16 range flag is redone as a single-row
+ * step, and RMU_ERR_RANGE is returned only if that step raises it too.  n_passes (host, nullable) <- the model passes
+ * after the prefill.  Refused before any CUDA call as rmu_decoder_generate refuses, and lookup_tokens < 0 or
+ * max_ngram < 1 (RMU_ERR_ARG). */
+int rmu_decoder_generate_lookup(rmu_encoder* enc, const int32_t* ids_h, int T, const rmu_sampling* s, uint64_t seed,
+                                int max_new_tokens, int lookup_tokens, int max_ngram, int32_t* out_h, int32_t* n_out,
+                                float* logits_h, int32_t* n_passes, void* stream);
+/* The prompt-lookup drafter (host only, no CUDA call), as transformers' PromptLookupCandidateGenerator.get_candidates
+ * proposes without a logits processor or eos ids: for n-gram sizes g = min(max_ngram, n - 1) down to 1, the first
+ * position i (left to right) where ids[i .. i + g) equals the last g ids and ids[i + g .. min(i + g + k, n, max_len))
+ * is not empty; that continuation goes to out and its length is returned.  0 when nothing matches or max_len == n + 1.
+ * Null pointers, n < 1, k < 1 or max_ngram < 1 return RMU_ERR_ARG. */
+int rmu_prompt_lookup_draft(const int32_t* ids, int n, int k, int max_ngram, int max_len, int32_t* out);
 void rmu_encoder_destroy(rmu_encoder* enc);
 
 #define RMU_POOL_MEAN 0
@@ -717,6 +738,18 @@ int rmu_debug_sample(float* logits, int V, uint32_t* presence, const rmu_samplin
  * pointer, B < 1 or step < 0 return RMU_ERR_ARG. */
 int rmu_debug_sample_rows(float* logits, int V, int B, uint32_t* presence, const int32_t* seq, const uint64_t* seeds,
                           int64_t step, const rmu_sampling* s, int32_t* token, void* stream);
+/* For tests: a prompt-lookup verify pass's sampler.  Row j of logits [M, V] (device) samples with presence bits rows[j]
+ * = presence | the bits of ids[1 .. j] (device ids [M]: the pending token, then the drafts; rows [M, ceil(V / 32)] is
+ * written) and u = philox(seed, step0 + j) -> token[j]; presence is not written.  Refused as rmu_debug_sample refuses,
+ * and a null pointer, M outside 1..16 or step0 < 0 return RMU_ERR_ARG. */
+int rmu_debug_sample_verify_rows(float* logits, int V, int M, uint32_t* presence, const int32_t* ids, uint64_t seed,
+                                 int64_t step0, const rmu_sampling* s, uint32_t* rows, int32_t* token, void* stream);
+/* For tests and benchmarks: rmu_decoder_generate_lookup with the caller's drafts in place of the n-gram lookup: a pass
+ * after n output tokens proposes drafts_h[n .. n + k) (host [max_new_tokens] ids in [0, vocab_size), k capped as
+ * there).  Refused as rmu_decoder_generate_lookup refuses, and k < 0 or a draft id out of range (RMU_ERR_ARG). */
+int rmu_debug_generate_drafts(rmu_encoder* enc, const int32_t* ids_h, int T, const rmu_sampling* s, uint64_t seed,
+                              int max_new_tokens, const int32_t* drafts_h, int k, int32_t* out_h, int32_t* n_out,
+                              float* logits_h, int32_t* n_passes, void* stream);
 int rmu_debug_split_planes(const float* src, int64_t n, uint16_t* hi, uint16_t* lo, void* stream);
 int rmu_debug_join_planes(const uint16_t* hi, const uint16_t* lo, int64_t n, float* out, void* stream);
 /* For tests: the BM25 select stage alone (bm25_select_kernel rounds, through the launcher rmu_bm25_search uses) on

@@ -135,6 +135,10 @@ SIGNATURES = {
                                        C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]),
     "rmu_decoder_generate_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(SamplingC),
                                              C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_decoder_generate_lookup": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(SamplingC), C.c_uint64, C.c_int,
+                                              C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p,
+                                              C.POINTER(C.c_int32), C.c_void_p]),
+    "rmu_prompt_lookup_draft": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "rmu_encoder_destroy": (None, [C.c_void_p]),
     "rmu_encoder_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_void_p, C.c_void_p]),
@@ -220,6 +224,11 @@ SIGNATURES = {
                                              C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_sample_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                         C.POINTER(SamplingC), C.c_void_p, C.c_void_p]),
+    "rmu_debug_sample_verify_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64,
+                                               C.c_int64, C.POINTER(SamplingC), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_generate_drafts": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(SamplingC), C.c_uint64, C.c_int,
+                                            C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p,
+                                            C.POINTER(C.c_int32), C.c_void_p]),
     "rmu_debug_kv_append": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                       C.c_void_p]),
     "rmu_debug_nf4_quantize": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),

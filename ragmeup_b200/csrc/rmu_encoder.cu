@@ -16,6 +16,7 @@
 #include <climits>
 #include <cmath>
 #include <cstdlib>
+#include <functional>
 #include <mutex>
 #include <type_traits>
 #include <vector>
@@ -2189,7 +2190,9 @@ __global__ void set_int_kernel(int* p, int v) { *p = v; }
 // and of the kSampleCap-th key, the keys above the higher of the two, a bitonic sort.  Weights exp(x - max) are float64,
 // summed in a fixed order by one thread.  u is u_in when u_in >= 0, else the Philox4x32-10 uniform of (seed, step).
 // The chosen id is written to *token and its presence bit set.  The batched decode runs one CTA per live row r
-// (SampleRows): logits row r, token r, and the presence bits and Philox seed of the row's sequence seq[r].
+// (SampleRows): logits row r, token r, and the presence bits and Philox seed of the row's sequence seq[r].  A
+// prompt-lookup verify pass runs one CTA per row of one sequence: row r has its own presence bits (seq null), the
+// call's seed (seeds null) and step + r (row_step), so it samples as the sequential step it stands for.
 // ---------------------------------------------------------------------------------------------------
 constexpr int kSampleThreads = 1024;
 constexpr int kSampleCap = 256;               // the largest top_k and the most candidates
@@ -2200,9 +2203,10 @@ struct SampleArgs {
 };
 
 struct SampleRows {
-    const int* seq = nullptr;                     // null: one row, `seed`, presence at its start
-    const unsigned long long* seeds = nullptr;    // [sequences]
-    size_t words = 0;                             // presence words per sequence
+    const int* seq = nullptr;                     // row r's sequence; null: r
+    const unsigned long long* seeds = nullptr;    // [sequences]; null: `seed` for every row
+    size_t words = 0;                             // presence words per sequence; 0: one row, presence at its start
+    bool row_step = false;                        // row r draws at step + r
 };
 
 // Philox4x32-10 (Salmon et al., SC'11) with counter (step, 0) and key seed: the first output word's high 24 bits / 2^24
@@ -2229,12 +2233,13 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(float* __restric
     __shared__ int s_remaining, s_ties, s_cnt;
     __shared__ double w[kSampleCap];
     const int tid = threadIdx.x;
-    if (rows.seq) {
-        const int q = rows.seq[blockIdx.x];
+    if (rows.words) {
+        const int q = rows.seq ? rows.seq[blockIdx.x] : blockIdx.x;
         logits += static_cast<size_t>(blockIdx.x) * V;
         token += blockIdx.x;
         presence += q * rows.words;
-        seed = rows.seeds[q];
+        if (rows.seeds) seed = rows.seeds[q];
+        if (rows.row_step) step += blockIdx.x;
     }
     unsigned long long best = 0ull;
     for (int i = tid; i < V; i += blockDim.x) {
@@ -2300,6 +2305,29 @@ static int launch_sample(float* logits, int V, unsigned* presence, const SampleA
                          unsigned long long step, int* token, cudaStream_t st, int B = 1, SampleRows rows = SampleRows{}) {
     ProfScope _ps(PROF_SAMPLE, st);
     sample_kernel<<<B, kSampleThreads, 0, st>>>(logits, V, presence, a, u_in, seed, step, token, rows);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    return RMU_OK;
+}
+
+// A verify pass's presence bits: rows [M, words], row j = base | the bits of ids[1 .. j] (the drafts fed before row
+// j's own token), one thread per word of a row
+__global__ void presence_rows_kernel(const unsigned* __restrict__ base, size_t words, const int* __restrict__ ids, int M,
+                                     unsigned* __restrict__ rows) {
+    const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= words * M) return;
+    const int j = static_cast<int>(i / words);
+    const size_t w = i % words;
+    unsigned v = base[w];
+    for (int d = 1; d <= j; ++d)
+        if (static_cast<size_t>(ids[d] >> 5) == w) v |= 1u << (ids[d] & 31);
+    rows[i] = v;
+}
+
+static int launch_presence_rows(const unsigned* base, size_t words, const int* ids, int M, unsigned* rows, cudaStream_t st) {
+    const size_t n = words * M;
+    ProfScope _ps(PROF_SAMPLE, st);
+    presence_rows_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(base, words, ids, M, rows);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
@@ -2922,6 +2950,215 @@ static int check_sampling(const std::string& fn, const rmu_sampling* s) {
             return RMU_ERR_ARG;
         }
     }
+    return RMU_OK;
+}
+
+// One batched decode step's layers (rmu_decoder_generate_batch's steps, a prompt-lookup verify pass): M token rows
+// ids [M] (device) at the positions in e->POSI (uploaded by the caller), row r's k / v into cache row pos[r] +
+// shift[r] and its attention over keys [0, pos[r] + 1) with the DecRows prefix mapping P; maxn = the most keys of any
+// row; part holds M * decode_part_floats(heads, maxn) floats.  The rows' hidden states are left in e->PRE.
+static int run_decode_rows(rmu_encoder* e, const int* ids, int M, const int* shift, int P, int maxn, float* part,
+                           cudaStream_t st) {
+    const rmu_bert_config& c = e->cfg;
+    const int nh = c.heads, kv = e->qext.kv_heads;
+    int rc = launch_embed_rows(ids, M, c.hidden, c.vocab_size, e->word, e->PRE, st);
+    DecRows dr;
+    dr.pos = e->POSI;
+    dr.shift = shift;
+    dr.P = P;
+    dr.qld = static_cast<size_t>(nh + 2 * kv) * kQwenHD;
+    for (int l = 0; l < c.layers && rc == RMU_OK; ++l) {
+        const EncLayer& Ly = e->layers[l];
+        rc = qwen3_attention_inputs(e, Ly, M, true, st);
+        if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, M, nh, kv, 0, e->kv_cap, kv_layer(e, l), st, e->POSI, shift);
+        if (rc == RMU_OK)
+            rc = launch_attention_decode(e->QKVP.hi, e->QKVP.lo, kv_layer(e, l), nh, kv, e->kv_cap, maxn, part, e->CTX.hi,
+                                         e->CTX.lo, st, M, dr);
+        if (rc == RMU_OK) rc = qwen3_layer_tail(e, Ly, M, true, st);
+    }
+    return rc;
+}
+
+// logits [M, V] = lm_head . (w_norm RMS(x)) for M fp32 hidden rows x [M, H]
+static int run_lm_head(rmu_encoder* e, const float* x, int M, float* logits, cudaStream_t st) {
+    const rmu_bert_config& c = e->cfg;
+    int rc = launch_rms_split(x, M, c.hidden, e->fng, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
+    if (rc != RMU_OK) return rc;
+    ProfScope _ps(PROF_LM_HEAD, st);
+    GemmParams gp{};
+    gp.M = M; gp.N = c.vocab_size; gp.K = c.hidden; gp.bias = e->lm_zero; gp.out_f32 = logits;
+    return launch_gemm(GEMM_BIAS_F32, e->X, e->lm_head, gp, e->sms, st);
+}
+
+constexpr int kMaxDrafts = RMU_MAX_GENERATE_BATCH - 1;   // a verify pass feeds at most 16 rows
+
+// a prompt-lookup drafter: up to k ids that may follow seq (the prompt and the tokens so far) -> out, their count
+using Drafter = std::function<int(const std::vector<int32_t>& seq, int k, int32_t* out)>;
+
+// The generation loop of rmu_decoder_generate and its prompt-lookup forms (DESIGN.md, "Prompt-lookup decoding").  The
+// prefill's last row gives the first token; each later pass feeds the pending token at position p = T + n - 1 plus k
+// drafts at p + 1 .. p + k, k = 0 .. kmax.  k = 0 is the single-row step.  k >= 1 is a verify pass: run_decode_rows on
+// the k + 1 rows, row j sampling as sequential step n + j would (its own presence bits: the base plus drafts 1 .. j;
+// Philox step n + j); t_0 is kept, t_j while t_{j - 1} equals draft j.  A verify pass that raises the range flag is
+// redone as a k = 0 step at the same position, so RMU_ERR_RANGE means what it means without drafts.
+static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* ids_h, int T, const rmu_sampling* s,
+                         uint64_t seed, int max_new_tokens, int kmax, const Drafter& draft, int32_t* out_h, int32_t* n_out,
+                         float* logits_h, int32_t* n_passes, void* stream) {
+    int rc = check_decoder(e, fn);
+    if (rc != RMU_OK) return rc;
+    if (!e->has_lm_head) { set_error(fn + ": no LM head is attached (rmu_decoder_set_lm_head)"); return RMU_ERR_ARG; }
+    rc = check_nf4_intact(e, fn);
+    if (rc != RMU_OK) return rc;
+    const rmu_bert_config& c = e->cfg;
+    if (T >= c.max_pos) {
+        set_error(fn + ": a prompt of " + std::to_string(T) + " tokens leaves no position for a new token (max_position_embeddings " +
+                  std::to_string(c.max_pos) + ")");
+        return RMU_ERR_ARG;
+    }
+    rc = check_sampling(fn, s);
+    if (rc != RMU_OK) return rc;
+    for (int i = 0; i < T; ++i)
+        if (ids_h[i] < 0 || ids_h[i] >= c.vocab_size) { set_error(fn + ": token id out of range"); return RMU_ERR_ARG; }
+    std::lock_guard<std::mutex> hg(e->host_mu);
+    std::lock_guard<std::mutex> g(e->mu);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int V = c.vocab_size, H = c.hidden, nh = c.heads, kv = e->qext.kv_heads, L = c.layers;
+    const int cap = std::min(T + max_new_tokens, c.max_pos);
+    // the KV cache: grown when a call needs more positions
+    if (cap > e->kv_cap) {
+        e->kv_cap = 0;                                  // until grow succeeds: it may free the old cache first
+        rc = grow(e->kv_cache, static_cast<size_t>(L) * 4 * kv * cap * kQwenHD * sizeof(__half));
+        if (rc != RMU_OK) {
+            set_error(fn + ": the KV cache for " + std::to_string(cap) + " positions: " + rmu_last_error());
+            return rc;
+        }
+        e->kv_cap = cap;
+    }
+    // gen_ws: logits [R, V] | presence [words] | tokens [R, at least 4] | decode partials [R rows] and, for verify
+    // passes, presence rows [R, words] | ints: ids [R] | shift [R] (zeros); R = kmax + 1
+    const int R = kmax + 1;
+    const size_t words = (static_cast<size_t>(V) + 31) / 32, ntok = 4 * ((static_cast<size_t>(R) + 3) / 4);
+    const size_t part_f = decode_part_floats(nh, cap);
+    const size_t ws = (static_cast<size_t>(R) * V + words + ntok + R * part_f + (R > 1 ? R * words + 2 * R : 0)) * sizeof(float);
+    rc = grow(e->gen_ws, ws);
+    if (rc == RMU_OK) rc = grow(e->d_ids, T * sizeof(int32_t), token_rows(T) * sizeof(int32_t));
+    if (rc == RMU_OK && R > 1) rc = ensure_tokens(e, R, 1);
+    if (rc != RMU_OK) return rc;
+    float* logits = e->gen_ws.as<float>();
+    unsigned* presence = reinterpret_cast<unsigned*>(logits + static_cast<size_t>(R) * V);
+    int* tok = reinterpret_cast<int*>(presence + words);
+    float* part = reinterpret_cast<float*>(tok + ntok);
+    unsigned* prow = reinterpret_cast<unsigned*>(part + R * part_f);
+    int* ints = reinterpret_cast<int*>(prow + R * words);
+    std::vector<unsigned> bits(words, 0u);
+    for (int i = 0; i < T; ++i) bits[ids_h[i] >> 5] |= 1u << (ids_h[i] & 31);
+    const int cu_h[2] = {0, T};
+    // pageable sources: each copy has taken its bytes when it returns
+    RMU_CUDA(cudaMemcpyAsync(e->d_ids.p, ids_h, T * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(e->span_cu, cu_h, sizeof(cu_h), cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(presence, bits.data(), words * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+    std::vector<int> hints(2 * static_cast<size_t>(R), 0), hpos(R), t_h(R);
+    if (R > 1) RMU_CUDA(cudaMemcpyAsync(ints, hints.data(), hints.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    std::vector<int32_t> seq(ids_h, ids_h + T);          // the prompt and the tokens so far: what the drafter reads
+    std::vector<float> staged(logits_h && R > 1 ? static_cast<size_t>(R) * V : 0);
+    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
+    // the prefill writes the cache; its last row's hidden state gives the first token
+    rc = run_qwen3(e, e->d_ids.as<int32_t>(), e->span_cu, 1, T, T, st, false, true);
+    const float* last = e->PRE + static_cast<size_t>(T - 1) * H;
+    int n = 0, passes = 0;
+    bool redo = false;                                     // the last verify pass raised the range flag
+    while (rc == RMU_OK) {
+        const int p = T + n - 1;
+        int k = 0;
+        if (n > 0 && kmax > 0 && !redo) {
+            // a pass never writes past output index max_new_tokens - 1 or position max_pos - 1
+            k = std::min({kmax, max_new_tokens - 1 - n, c.max_pos - 1 - T - n});
+            if (k > 0) k = draft(seq, k, hints.data() + 1);
+        }
+        redo = false;
+        int acc = 1;                                       // tokens this pass keeps: t_h[0 .. acc)
+        if (k == 0) {
+            if (n > 0) {
+                // the previous token at position p through every layer, its k / v into cache row p
+                set_int_kernel<<<1, 1, 0, st>>>(e->POSI, p);
+                count_launch();
+                RMU_CHECK_LAUNCH();
+                // after a verify pass the pending token is the last kept row's, not tok[0]: it goes up through ints
+                const int* pending = tok;
+                if (kmax > 0) {
+                    hints[0] = seq.back();
+                    RMU_CUDA(cudaMemcpyAsync(ints, hints.data(), sizeof(int), cudaMemcpyHostToDevice, st));
+                    pending = ints;
+                }
+                rc = launch_embed_rows(pending, 1, H, V, e->word, e->PRE, st);
+                for (int l = 0; l < L && rc == RMU_OK; ++l) {
+                    const EncLayer& Ly = e->layers[l];
+                    rc = qwen3_attention_inputs(e, Ly, 1, true, st);
+                    if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, 1, nh, kv, p, e->kv_cap, kv_layer(e, l), st);
+                    if (rc == RMU_OK)
+                        rc = launch_attention_decode(e->QKVP.hi, e->QKVP.lo, kv_layer(e, l), nh, kv, e->kv_cap, p + 1, part,
+                                                     e->CTX.hi, e->CTX.lo, st);
+                    if (rc == RMU_OK) rc = qwen3_layer_tail(e, Ly, 1, true, st);
+                }
+                last = e->PRE;
+            }
+            if (rc == RMU_OK) rc = run_lm_head(e, last, 1, logits, st);
+            if (rc == RMU_OK && logits_h)
+                RMU_CUDA(cudaMemcpyAsync(logits_h + static_cast<size_t>(n) * V, logits, static_cast<size_t>(V) * sizeof(float),
+                                         cudaMemcpyDeviceToHost, st));
+            if (rc == RMU_OK) rc = launch_sample(logits, V, presence, sa, -1.f, seed, static_cast<unsigned long long>(n), tok, st);
+            if (rc != RMU_OK) break;
+            RMU_CUDA(cudaMemcpyAsync(t_h.data(), tok, sizeof(int), cudaMemcpyDeviceToHost, st));
+            rc = qwen3_check_range(e, st);        // synchronises st
+            if (rc != RMU_OK) break;
+        } else {
+            // rows j = 0 .. k: token hints[j] (the pending token, then the drafts) at position p + j, cache row p + j
+            const int M = k + 1;
+            hints[0] = seq.back();
+            for (int j = 0; j < M; ++j) hpos[j] = p + j;
+            RMU_CUDA(cudaMemcpyAsync(ints, hints.data(), M * sizeof(int), cudaMemcpyHostToDevice, st));
+            RMU_CUDA(cudaMemcpyAsync(e->POSI, hpos.data(), M * sizeof(int), cudaMemcpyHostToDevice, st));
+            rc = launch_presence_rows(presence, words, ints, M, prow, st);
+            if (rc == RMU_OK) rc = run_decode_rows(e, ints, M, ints + R, 0, p + M, part, st);
+            if (rc == RMU_OK) rc = run_lm_head(e, e->PRE, M, logits, st);
+            if (rc == RMU_OK && logits_h)
+                RMU_CUDA(cudaMemcpyAsync(staged.data(), logits, static_cast<size_t>(M) * V * sizeof(float),
+                                         cudaMemcpyDeviceToHost, st));
+            SampleRows sr;
+            sr.words = words;
+            sr.row_step = true;
+            if (rc == RMU_OK) rc = launch_sample(logits, V, prow, sa, -1.f, seed, static_cast<unsigned long long>(n), tok, st, M, sr);
+            if (rc != RMU_OK) break;
+            RMU_CUDA(cudaMemcpyAsync(t_h.data(), tok, M * sizeof(int), cudaMemcpyDeviceToHost, st));
+            ++passes;
+            if (qwen3_check_range(e, st) != RMU_OK) {      // synchronises st; a rejected draft's row may be the cause
+                RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
+                redo = true;
+                continue;
+            }
+            while (acc < M && t_h[acc - 1] == hints[acc]) ++acc;
+            // the last kept row's bits are the base plus every kept token: the next base
+            RMU_CUDA(cudaMemcpyAsync(presence, prow + static_cast<size_t>(acc - 1) * words, words * sizeof(unsigned),
+                                     cudaMemcpyDeviceToDevice, st));
+        }
+        if (n > 0 && k == 0) ++passes;
+        bool stop = false;
+        for (int j = 0; j < acc && !stop; ++j) {
+            if (k > 0 && logits_h)
+                std::copy(staged.begin() + static_cast<size_t>(j) * V, staged.begin() + static_cast<size_t>(j + 1) * V,
+                          logits_h + static_cast<size_t>(n) * V);
+            out_h[n++] = t_h[j];
+            seq.push_back(t_h[j]);
+            bool eos = false;
+            for (int i = 0; i < s->n_eos; ++i) eos |= t_h[j] == s->eos_ids[i];
+            stop = eos || n == max_new_tokens || T + n >= c.max_pos;
+        }
+        if (stop) break;
+    }
+    *n_out = n;
+    if (n_passes) *n_passes = passes;
+    if (rc != RMU_OK) return rc;
+    RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
 }
 
@@ -3714,102 +3951,60 @@ int rmu_decoder_generate(rmu_encoder* e, const int32_t* ids_h, int T, const rmu_
                          int max_new_tokens, int32_t* out_h, int32_t* n_out, float* logits_h, void* stream) {
     const std::string fn("rmu_decoder_generate");
     if (!e || !ids_h || !s || !out_h || !n_out || T < 1 || max_new_tokens < 1) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
-    int rc = check_decoder(e, fn);
-    if (rc != RMU_OK) return rc;
-    if (!e->has_lm_head) { set_error(fn + ": no LM head is attached (rmu_decoder_set_lm_head)"); return RMU_ERR_ARG; }
-    rc = check_nf4_intact(e, fn);
-    if (rc != RMU_OK) return rc;
-    const rmu_bert_config& c = e->cfg;
-    if (T >= c.max_pos) {
-        set_error(fn + ": a prompt of " + std::to_string(T) + " tokens leaves no position for a new token (max_position_embeddings " +
-                  std::to_string(c.max_pos) + ")");
+    return generate_loop(e, fn, ids_h, T, s, seed, max_new_tokens, 0, Drafter(), out_h, n_out, logits_h, nullptr, stream);
+}
+
+int rmu_prompt_lookup_draft(const int32_t* ids, int n, int k, int max_ngram, int max_len, int32_t* out) {
+    if (!ids || !out || n < 1 || k < 1 || max_ngram < 1) { set_error("rmu_prompt_lookup_draft: bad argument"); return RMU_ERR_ARG; }
+    if (max_len == n + 1) return 0;                      // the model's own next token already reaches max_len
+    for (int g = std::min(max_ngram, n - 1); g > 0; --g) {
+        const int32_t* tail = ids + n - g;
+        for (int i = 0; i + g <= n; ++i) {
+            if (!std::equal(ids + i, ids + i + g, tail)) continue;
+            const int start = i + g, end = std::min({start + k, n, max_len});
+            if (start < end) {
+                std::copy(ids + start, ids + end, out);
+                return end - start;
+            }
+        }
+    }
+    return 0;
+}
+
+int rmu_decoder_generate_lookup(rmu_encoder* e, const int32_t* ids_h, int T, const rmu_sampling* s, uint64_t seed,
+                                int max_new_tokens, int lookup_tokens, int max_ngram, int32_t* out_h, int32_t* n_out,
+                                float* logits_h, int32_t* n_passes, void* stream) {
+    const std::string fn("rmu_decoder_generate_lookup");
+    if (!e || !ids_h || !s || !out_h || !n_out || T < 1 || max_new_tokens < 1 || lookup_tokens < 0 || max_ngram < 1) {
+        set_error(fn + ": bad argument");
         return RMU_ERR_ARG;
     }
-    rc = check_sampling(fn, s);
-    if (rc != RMU_OK) return rc;
-    for (int i = 0; i < T; ++i)
-        if (ids_h[i] < 0 || ids_h[i] >= c.vocab_size) { set_error(fn + ": token id out of range"); return RMU_ERR_ARG; }
-    std::lock_guard<std::mutex> hg(e->host_mu);
-    std::lock_guard<std::mutex> g(e->mu);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int V = c.vocab_size, H = c.hidden, nh = c.heads, kv = e->qext.kv_heads, L = c.layers;
-    const int cap = std::min(T + max_new_tokens, c.max_pos);
-    // the KV cache: grown when a call needs more positions
-    if (cap > e->kv_cap) {
-        e->kv_cap = 0;                                  // until grow succeeds: it may free the old cache first
-        rc = grow(e->kv_cache, static_cast<size_t>(L) * 4 * kv * cap * kQwenHD * sizeof(__half));
-        if (rc != RMU_OK) {
-            set_error(fn + ": the KV cache for " + std::to_string(cap) + " positions: " + rmu_last_error());
-            return rc;
-        }
-        e->kv_cap = cap;
+    const int max_len = T + max_new_tokens;              // transformers' max_length
+    const Drafter draft = [&](const std::vector<int32_t>& seq, int k, int32_t* out) {
+        return std::max(0, rmu_prompt_lookup_draft(seq.data(), static_cast<int>(seq.size()), k, max_ngram, max_len, out));
+    };
+    return generate_loop(e, fn, ids_h, T, s, seed, max_new_tokens, std::min(lookup_tokens, kMaxDrafts), draft, out_h,
+                         n_out, logits_h, n_passes, stream);
+}
+
+int rmu_debug_generate_drafts(rmu_encoder* e, const int32_t* ids_h, int T, const rmu_sampling* s, uint64_t seed,
+                              int max_new_tokens, const int32_t* drafts_h, int k, int32_t* out_h, int32_t* n_out,
+                              float* logits_h, int32_t* n_passes, void* stream) {
+    const std::string fn("rmu_debug_generate_drafts");
+    if (!e || !ids_h || !s || !drafts_h || !out_h || !n_out || T < 1 || max_new_tokens < 1 || k < 0) {
+        set_error(fn + ": bad argument");
+        return RMU_ERR_ARG;
     }
-    const size_t words = (static_cast<size_t>(V) + 31) / 32;
-    const size_t ws = (static_cast<size_t>(V) + words + 4 + decode_part_floats(nh, cap)) * sizeof(float);
-    rc = grow(e->gen_ws, ws);
-    if (rc == RMU_OK) rc = grow(e->d_ids, T * sizeof(int32_t), token_rows(T) * sizeof(int32_t));
-    if (rc != RMU_OK) return rc;
-    float* logits = e->gen_ws.as<float>();
-    unsigned* presence = reinterpret_cast<unsigned*>(logits + V);
-    int* tok = reinterpret_cast<int*>(presence + words);
-    float* part = reinterpret_cast<float*>(tok + 4);
-    std::vector<unsigned> bits(words, 0u);
-    for (int i = 0; i < T; ++i) bits[ids_h[i] >> 5] |= 1u << (ids_h[i] & 31);
-    const int cu_h[2] = {0, T};
-    // pageable sources: each copy has taken its bytes when it returns
-    RMU_CUDA(cudaMemcpyAsync(e->d_ids.p, ids_h, T * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    RMU_CUDA(cudaMemcpyAsync(e->span_cu, cu_h, sizeof(cu_h), cudaMemcpyHostToDevice, st));
-    RMU_CUDA(cudaMemcpyAsync(presence, bits.data(), words * sizeof(unsigned), cudaMemcpyHostToDevice, st));
-    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
-    // the prefill writes the cache; its last row's hidden state gives the first token
-    rc = run_qwen3(e, e->d_ids.as<int32_t>(), e->span_cu, 1, T, T, st, false, true);
-    const float* last = e->PRE + static_cast<size_t>(T - 1) * H;
-    int n = 0;
-    for (int step = 0; rc == RMU_OK; ++step) {
-        if (step > 0) {
-            // the previous token at position p = T + step - 1 through every layer, its k / v into cache row p
-            const int p = T + step - 1;
-            set_int_kernel<<<1, 1, 0, st>>>(e->POSI, p);
-            count_launch();
-            RMU_CHECK_LAUNCH();
-            rc = launch_embed_rows(tok, 1, H, V, e->word, e->PRE, st);
-            for (int l = 0; l < L && rc == RMU_OK; ++l) {
-                const EncLayer& Ly = e->layers[l];
-                rc = qwen3_attention_inputs(e, Ly, 1, true, st);
-                if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, 1, nh, kv, p, e->kv_cap, kv_layer(e, l), st);
-                if (rc == RMU_OK)
-                    rc = launch_attention_decode(e->QKVP.hi, e->QKVP.lo, kv_layer(e, l), nh, kv, e->kv_cap, p + 1, part,
-                                                 e->CTX.hi, e->CTX.lo, st);
-                if (rc == RMU_OK) rc = qwen3_layer_tail(e, Ly, 1, true, st);
-            }
-            last = e->PRE;
-        }
-        // logits = lm_head . (w_norm RMS(h_last)), then the sampler
-        if (rc == RMU_OK) rc = launch_rms_split(last, 1, H, e->fng, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
-        if (rc == RMU_OK) {
-            ProfScope _ps(PROF_LM_HEAD, st);
-            GemmParams gp{};
-            gp.M = 1; gp.N = V; gp.K = H; gp.bias = e->lm_zero; gp.out_f32 = logits;
-            rc = launch_gemm(GEMM_BIAS_F32, e->X, e->lm_head, gp, e->sms, st);
-        }
-        if (rc == RMU_OK && logits_h)
-            RMU_CUDA(cudaMemcpyAsync(logits_h + static_cast<size_t>(step) * V, logits, static_cast<size_t>(V) * sizeof(float),
-                                     cudaMemcpyDeviceToHost, st));
-        if (rc == RMU_OK) rc = launch_sample(logits, V, presence, sa, -1.f, seed, static_cast<unsigned long long>(step), tok, st);
-        if (rc != RMU_OK) break;
-        int t_h = 0;
-        RMU_CUDA(cudaMemcpyAsync(&t_h, tok, sizeof(int), cudaMemcpyDeviceToHost, st));
-        rc = qwen3_check_range(e, st);        // synchronises st
-        if (rc != RMU_OK) break;
-        out_h[n++] = t_h;
-        bool eos = false;
-        for (int i = 0; i < s->n_eos; ++i) eos |= t_h == s->eos_ids[i];
-        if (eos || n == max_new_tokens || T + n >= c.max_pos) break;
-    }
-    *n_out = n;
-    if (rc != RMU_OK) return rc;
-    RMU_CUDA(cudaEventRecord(e->ws_done, st));
-    return RMU_OK;
+    if (check_decoder(e, fn) != RMU_OK) return RMU_ERR_ARG;
+    for (int i = 0; i < max_new_tokens; ++i)
+        if (drafts_h[i] < 0 || drafts_h[i] >= e->cfg.vocab_size) { set_error(fn + ": draft id out of range"); return RMU_ERR_ARG; }
+    // the draft at output index n: drafts_h[n .. n + k)
+    const Drafter draft = [&](const std::vector<int32_t>& seq, int kk, int32_t* out) {
+        std::copy(drafts_h + (seq.size() - T), drafts_h + (seq.size() - T) + kk, out);
+        return kk;
+    };
+    return generate_loop(e, fn, ids_h, T, s, seed, max_new_tokens, std::min(k, kMaxDrafts), draft, out_h, n_out, logits_h,
+                         n_passes, stream);
 }
 
 // The batch layout.  P = the prompts' longest common prefix, capped so that every prompt keeps one own token (0 when
@@ -3968,32 +4163,11 @@ int rmu_decoder_generate_batch(rmu_encoder* e, const int32_t* ids_h, const int32
             int maxn = 0;
             for (int r = 0; r < M; ++r) maxn = std::max(maxn, hpos[r] + 1);
             RMU_CUDA(cudaMemcpyAsync(e->POSI, hpos.data(), hpos.size() * 4, cudaMemcpyHostToDevice, st));
-            rc = launch_embed_rows(ints, M, H, V, e->word, e->PRE, st);
-            DecRows dr;
-            dr.pos = e->POSI;
-            dr.shift = ints + M;
-            dr.P = P;
-            dr.qld = static_cast<size_t>(nh + 2 * kv) * kQwenHD;
-            for (int l = 0; l < L && rc == RMU_OK; ++l) {
-                const EncLayer& Ly = e->layers[l];
-                rc = qwen3_attention_inputs(e, Ly, M, true, st);
-                if (rc == RMU_OK)
-                    rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, M, nh, kv, 0, e->kv_cap, kv_layer(e, l), st, e->POSI, ints + M);
-                if (rc == RMU_OK)
-                    rc = launch_attention_decode(e->QKVP.hi, e->QKVP.lo, kv_layer(e, l), nh, kv, e->kv_cap, maxn, part,
-                                                 e->CTX.hi, e->CTX.lo, st, M, dr);
-                if (rc == RMU_OK) rc = qwen3_layer_tail(e, Ly, M, true, st);
-            }
+            rc = run_decode_rows(e, ints, M, ints + M, P, maxn, part, st);
             x_last = e->PRE;
         }
-        // logits = lm_head . (w_norm RMS(h_last)) for the M live rows (step 0: last[b] in prompt order), then the sampler
-        if (rc == RMU_OK) rc = launch_rms_split(x_last, M, H, e->fng, c.ln_eps, e->X.hi, e->X.lo, e->range_flag, st);
-        if (rc == RMU_OK) {
-            ProfScope _ps(PROF_LM_HEAD, st);
-            GemmParams gp{};
-            gp.M = M; gp.N = V; gp.K = H; gp.bias = e->lm_zero; gp.out_f32 = logits;
-            rc = launch_gemm(GEMM_BIAS_F32, e->X, e->lm_head, gp, e->sms, st);
-        }
+        // logits for the M live rows (step 0: last[b] in prompt order), then the sampler
+        if (rc == RMU_OK) rc = run_lm_head(e, x_last, M, logits, st);
         for (int r = 0; r < M && rc == RMU_OK && logits_h; ++r)
             RMU_CUDA(cudaMemcpyAsync(logits_h + (static_cast<size_t>(live[r]) * max_new_tokens + step) * V,
                                      logits + static_cast<size_t>(r) * V, static_cast<size_t>(V) * sizeof(float),
@@ -4749,6 +4923,24 @@ int rmu_debug_sample_rows(float* logits, int V, int B, uint32_t* presence, const
     sr.words = (static_cast<size_t>(V) + 31) / 32;
     return launch_sample(logits, V, presence, sa, -1.f, 0ull, static_cast<unsigned long long>(step), token,
                          static_cast<cudaStream_t>(stream), B, sr);
+}
+
+int rmu_debug_sample_verify_rows(float* logits, int V, int M, uint32_t* presence, const int32_t* ids, uint64_t seed,
+                                 int64_t step0, const rmu_sampling* s, uint32_t* rows, int32_t* token, void* stream) {
+    if (!logits || V < 1 || M < 1 || M > RMU_MAX_GENERATE_BATCH || !presence || !ids || !s || !rows || !token || step0 < 0) {
+        set_error("rmu_debug_sample_verify_rows: bad argument");
+        return RMU_ERR_ARG;
+    }
+    int rc = check_sampling("rmu_debug_sample_verify_rows", s);
+    if (rc != RMU_OK) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
+    SampleRows sr;
+    sr.words = (static_cast<size_t>(V) + 31) / 32;
+    sr.row_step = true;
+    rc = launch_presence_rows(presence, sr.words, ids, M, rows, st);
+    if (rc != RMU_OK) return rc;
+    return launch_sample(logits, V, rows, sa, -1.f, seed, static_cast<unsigned long long>(step0), token, st, M, sr);
 }
 
 }  // extern "C"

@@ -20,6 +20,7 @@ The model the pipeline holds (the reference's NF4 model) stays loaded but genera
 from __future__ import annotations
 
 import copy
+import os
 import threading
 from typing import Any, List, Optional
 
@@ -31,8 +32,7 @@ REFUSED_FIELDS = ("num_beams", "num_beam_groups", "num_return_sequences", "min_p
                   "forced_eos_token_id", "min_new_tokens", "min_length", "stop_strings", "epsilon_cutoff", "eta_cutoff",
                   "guidance_scale", "encoder_repetition_penalty", "encoder_no_repeat_ngram_size", "diversity_penalty",
                   "exponential_decay_length_penalty", "renormalize_logits", "constraints", "force_words_ids",
-                  "penalty_alpha", "watermarking_config", "top_h", "assistant_model", "prompt_lookup_num_tokens",
-                  "dola_layers")
+                  "penalty_alpha", "watermarking_config", "top_h", "assistant_model", "dola_layers")
 # unset fields hold None in a GenerationConfig built from scratch and False / 0 / [] in one built from a model's config:
 # these values all mean "off"
 
@@ -69,9 +69,33 @@ def resolve_settings(generation_config: Any, generate_kwargs: dict, prompt_len: 
     eos = gc.eos_token_id
     eos = [] if eos is None else ([int(eos)] if isinstance(eos, int) else [int(t) for t in eos])
     max_new = gc.max_new_tokens if gc.max_new_tokens is not None else int(get("max_length")) - int(prompt_len)
-    return dict(max_new_tokens=int(max_new), do_sample=do_sample, temperature=float(get("temperature")),
-                top_k=int(top_k or 0), top_p=float(get("top_p")), repetition_penalty=float(get("repetition_penalty")),
-                eos_token_ids=eos)
+    out = dict(max_new_tokens=int(max_new), do_sample=do_sample, temperature=float(get("temperature")),
+               top_k=int(top_k or 0), top_p=float(get("top_p")), repetition_penalty=float(get("repetition_penalty")),
+               eos_token_ids=eos)
+    lookup = get("prompt_lookup_num_tokens")
+    if not _off(lookup):
+        # prompt-lookup decoding changes how many passes a reply takes, never its tokens
+        out.update(prompt_lookup_num_tokens=int(lookup), max_matching_ngram_size=int(get("max_matching_ngram_size") or 2))
+    return out
+
+
+PROMPT_LOOKUP_ENV = "RMU_PROMPT_LOOKUP_TOKENS"
+
+
+def prompt_lookup_tokens() -> int:
+    """``$RMU_PROMPT_LOOKUP_TOKENS``: the drafts per pass HuggingFacePipeline proposes when neither its generate kwargs
+    nor its generation_config set ``prompt_lookup_num_tokens`` (the reference builds its pipeline with fixed kwargs, so
+    its ``.env`` is where the setting can come from); unset or 0: off.  ValueError naming the key otherwise."""
+    raw = os.environ.get(PROMPT_LOOKUP_ENV, "").strip()
+    if not raw:
+        return 0
+    try:
+        v = int(raw)
+    except ValueError:
+        v = -1
+    if v < 0:
+        raise ValueError(f"{PROMPT_LOOKUP_ENV}={os.environ[PROMPT_LOOKUP_ENV]!r}: expected a non-negative integer")
+    return v
 
 
 class _PipelineGenerator:
@@ -96,6 +120,8 @@ class _PipelineGenerator:
             gen_cfg = pipe._forward_params.get("generation_config", getattr(pipe, "generation_config", None) or
                                                pipe.model.generation_config)
             settings = resolve_settings(gen_cfg, fwd, ids.shape[1])
+            if "prompt_lookup_num_tokens" not in settings and prompt_lookup_tokens():
+                settings.update(prompt_lookup_num_tokens=prompt_lookup_tokens(), max_matching_ngram_size=2)
             seed = int(torch.randint(0, 2 ** 63 - 1, (1,)).item())
             new = self._decoder().generate(ids[0].tolist(), seed=seed, **settings)
             seq = torch.cat([ids[0].cpu(), torch.as_tensor(new, dtype=ids.dtype)])

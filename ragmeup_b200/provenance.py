@@ -130,9 +130,11 @@ class DecoderAttention:
 
     def generate(self, ids: Sequence[int], max_new_tokens: int, do_sample: bool = False, temperature: float = 1.0,
                  top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.0, eos_token_ids=(),
-                 seed: int = 0) -> List[int]:
+                 seed: int = 0, prompt_lookup_num_tokens: int = 0, max_matching_ngram_size: int = 2) -> List[int]:
         """the new token ids after the prompt ``ids`` (``rmu_decoder_generate``), the eos token included when one
-        ends the run"""
+        ends the run.  ``prompt_lookup_num_tokens`` > 0 drafts that many tokens (at most 15) per pass from earlier
+        matches of the last ``max_matching_ngram_size``-gram (``rmu_decoder_generate_lookup``): the same tokens,
+        bit for bit, in fewer model passes when the reply copies the prompt."""
         if max_new_tokens < 1:
             return []
         eos = [int(t) for t in eos_token_ids]
@@ -149,9 +151,16 @@ class DecoderAttention:
                 W = decoder_lm_head(self.model_name, self.cfg)
                 enc._check(_lib.lib().rmu_decoder_set_lm_head(enc._h, W.ctypes.data), "rmu_decoder_set_lm_head")
                 self._lm_head = True
-            enc._check(_lib.lib().rmu_decoder_generate(enc._h, prompt.ctypes.data, len(prompt), C.byref(s),
-                                                       int(seed) & (2 ** 64 - 1), int(max_new_tokens), out.ctypes.data,
-                                                       C.byref(n), None, _lib.stream_ptr()), "rmu_decoder_generate")
+            if prompt_lookup_num_tokens:
+                enc._check(_lib.lib().rmu_decoder_generate_lookup(
+                    enc._h, prompt.ctypes.data, len(prompt), C.byref(s), int(seed) & (2 ** 64 - 1), int(max_new_tokens),
+                    int(prompt_lookup_num_tokens), int(max_matching_ngram_size), out.ctypes.data, C.byref(n), None, None,
+                    _lib.stream_ptr()), "rmu_decoder_generate_lookup")
+            else:
+                enc._check(_lib.lib().rmu_decoder_generate(enc._h, prompt.ctypes.data, len(prompt), C.byref(s),
+                                                           int(seed) & (2 ** 64 - 1), int(max_new_tokens),
+                                                           out.ctypes.data, C.byref(n), None, _lib.stream_ptr()),
+                           "rmu_decoder_generate")
         return out[:n.value].tolist()
 
     def generate_batch(self, prompts: Sequence[Sequence[int]], max_new_tokens: int, seeds: Sequence[int],
@@ -314,6 +323,8 @@ def compute_llm_provenance(tokenizer: Any, model: Any, query: str, context: Sequ
     settings = resolve_settings(getattr(model, "generation_config", None), {"max_new_tokens": 10},
                                 max(len(p) for p in prompts))
     max_new = settings.pop("max_new_tokens")
+    settings.pop("prompt_lookup_num_tokens", None)     # the batched path does not draft; its tokens are the same
+    settings.pop("max_matching_ngram_size", None)
     seeds = [int(torch.randint(0, 2 ** 63 - 1, (1,)).item()) for _ in prompts]
     new = dec.generate_batch(prompts, max_new, seeds, **settings)
     return [_llm_score(tokenizer, p, n) for p, n in zip(prompts, new)]
