@@ -33,6 +33,7 @@ extern "C" {
 #define RMU_ERR_CUDA -2
 #define RMU_ERR_UNSUPPORTED -3
 #define RMU_ERR_RANGE -4         /* an activation left the range its storage can hold (Qwen3's fp16 planes) */
+#define RMU_ERR_BUSY -5          /* a decode session has no free row, or its KV cache cannot grow while rows are live */
 
 /* metric ids — Milvus FLAT/L2 is the reference default store metric (langchain-milvus 0.1.3
  * via server/RAGHelper.py:388-394); PGVector uses cosine distance (server/RAGHelper.py:399-404). */
@@ -430,6 +431,53 @@ int rmu_decoder_generate_lookup(rmu_encoder* enc, const int32_t* ids_h, int T, c
  * is not empty; that continuation goes to out and its length is returned.  0 when nothing matches or max_len == n + 1.
  * Null pointers, n < 1, k < 1 or max_ngram < 1 return RMU_ERR_ARG. */
 int rmu_prompt_lookup_draft(const int32_t* ids, int n, int k, int max_ngram, int max_len, int32_t* out);
+/* Continuous batching: a decode session of one decoder handle (with an LM head) that outlives a call.  Requests join
+ * it (rmu_decoder_session_add) and leave it (when they stop, or rmu_decoder_session_cancel) between steps; each
+ * rmu_decoder_session_step runs one decode step over every live row at M = live (at most RMU_MAX_GENERATE_BATCH).
+ * Each request's tokens and logits are bit for bit what rmu_decoder_generate returns for its prompt, settings, seed and
+ * max_new_tokens, on split and NF4 handles, whenever it joins and whatever rows share its steps.
+ *
+ * The session owns its KV cache (the handle cache's layout; rmu_decoder_generate[_batch|_lookup] never touch it): a
+ * request of T prompt tokens holds the rows [base, base + min(T + max_new_tokens, max_pos)), placed first fit among the
+ * free gaps; when none fits the cache grows (one 2D copy to the new pitch, so no live row moves).  Every entry point
+ * holds the handle's lock for its own duration only, so other calls on the handle run between steps.  Calls may come
+ * from different threads on different streams: each waits on the session's last use and on the handle's workspace.
+ *
+ * rmu_decoder_session_create / _destroy: a handle's sessions are destroyed before the handle; destroy waits for the
+ * session's last use.  Refused: a null pointer or another kind of encoder (RMU_ERR_ARG). */
+typedef struct rmu_gen_session rmu_gen_session;
+int rmu_decoder_session_create(rmu_encoder* enc, rmu_gen_session** out);
+void rmu_decoder_session_destroy(rmu_gen_session* s);
+/* A row's status after a token: RMU_GEN_LIVE, or why it stopped (the row is then released in the same call), or a
+ * negative error code (RMU_ERR_RANGE: this request's own activations left the fp16 range; no token). */
+#define RMU_GEN_LIVE 0
+#define RMU_GEN_EOS 1
+#define RMU_GEN_MAX_NEW 2
+#define RMU_GEN_MAX_POS 3
+/* Admit B requests (1 .. RMU_MAX_GENERATE_BATCH): prompt b = ids_h[cu_h[b] .. cu_h[b + 1]) with settings s_h[b], seed
+ * seeds_h[b] and max_new_h[b] (all host).  They are prefilled together as one varlen run into their own regions (an
+ * NF4 handle's one-token prompts alone, on the decode GEMV), and each samples its first token: slot_h[b] <- its row
+ * (-1 when it stopped or failed), tok_h[b], status_h[b]; logits_h (host, nullable) [B, vocab_size] <- each first
+ * token's logits.  When the range flag rises the requests are redone one at a time, and only those whose own run
+ * raises it end with RMU_ERR_RANGE.  Refused before any CUDA call with rmu_decoder_generate's codes (null pointers,
+ * an empty prompt, max_new < 1, T >= max_pos, an id out of range, the sampling settings rmu_decoder_generate refuses,
+ * no LM head, a broken NF4 handle).  RMU_ERR_BUSY, with the session unchanged: fewer than B free rows, or a KV cache
+ * that cannot grow while rows are live (with no live row that failure is RMU_ERR_CUDA naming the positions).  Any
+ * other failure releases the call's new rows.  Synchronises `stream`. */
+int rmu_decoder_session_add(rmu_gen_session* s, const int32_t* ids_h, const int32_t* cu_h, int B, const rmu_sampling* s_h,
+                            const uint64_t* seeds_h, const int32_t* max_new_h, int32_t* slot_h, int32_t* tok_h,
+                            int32_t* status_h, float* logits_h, void* stream);
+/* One decode step over every live row, in slot order: *n_h <- the rows (0 when none is live: no CUDA call), row r ->
+ * slot_h[r], tok_h[r], status_h[r] and logits_h (host, nullable) [16, vocab_size] row r.  A range error is handled as
+ * in rmu_decoder_session_add.  A failed step (a CUDA error, an allocation that fails) releases every live row and
+ * reports none.  Synchronises `stream`. */
+int rmu_decoder_session_step(rmu_gen_session* s, int32_t* slot_h, int32_t* tok_h, int32_t* status_h, int32_t* n_h,
+                             float* logits_h, void* stream);
+/* Release a live row without output; a slot that is not live returns RMU_ERR_ARG.  No CUDA call. */
+int rmu_decoder_session_cancel(rmu_gen_session* s, int slot);
+/* The live rows, the KV cache's capacity in positions and live_mask (nullable): bit i set when slot i is live.  No
+ * CUDA call. */
+int rmu_decoder_session_info(rmu_gen_session* s, int32_t* live, int32_t* cap_positions, uint32_t* live_mask);
 void rmu_encoder_destroy(rmu_encoder* enc);
 
 #define RMU_POOL_MEAN 0
@@ -750,6 +798,19 @@ int rmu_debug_sample_verify_rows(float* logits, int V, int M, uint32_t* presence
 int rmu_debug_generate_drafts(rmu_encoder* enc, const int32_t* ids_h, int T, const rmu_sampling* s, uint64_t seed,
                               int max_new_tokens, const int32_t* drafts_h, int k, int32_t* out_h, int32_t* n_out,
                               float* logits_h, int32_t* n_passes, void* stream);
+/* For tests: a decode session's sampler.  Row r of logits [B, V] (device) samples with the presence bits [.., ceil(V /
+ * 32)], seed and Philox step of sequence seq[r] (device int32 [B], uint64 seeds and steps) and that sequence's settings
+ * s_h[seq[r]] (host [n_seq]) -> token[r].  Row r equals rmu_debug_sample on that row, those bits, those settings and u =
+ * philox(seed, step).  Refused as rmu_debug_sample refuses each s_h entry, and a null pointer, B < 1 or n_seq outside
+ * 1..16 return RMU_ERR_ARG.  Synchronises `stream`. */
+int rmu_debug_sample_session_rows(float* logits, int V, int B, uint32_t* presence, const int32_t* seq,
+                                  const uint64_t* seeds, const uint64_t* steps, int n_seq, const rmu_sampling* s_h,
+                                  int32_t* token, void* stream);
+/* For tests (host only): a decode session's region placement.  Op i > 0 places ops[i] rows (first fit, growing past
+ * the last used region when no gap fits) -> out[2 i] = the base; op i <= 0 frees the region at base -ops[i] -> out[2 i]
+ * = 0, or -1 when no region starts there; out[2 i + 1] = the capacity after the op.  Null pointers or n < 0 return
+ * RMU_ERR_ARG. */
+int rmu_debug_kv_regions(const int32_t* ops, int n, int32_t* out);
 int rmu_debug_split_planes(const float* src, int64_t n, uint16_t* hi, uint16_t* lo, void* stream);
 int rmu_debug_join_planes(const uint16_t* hi, const uint16_t* lo, int64_t n, float* out, void* stream);
 /* For tests: the BM25 select stage alone (bm25_select_kernel rounds, through the launcher rmu_bm25_search uses) on

@@ -43,6 +43,9 @@ class Qwen3ExtC(C.Structure):
 
 MAX_EOS = 8
 MAX_GENERATE_BATCH = 16            # RMU_MAX_GENERATE_BATCH
+ERR_RANGE = -4                     # RMU_ERR_RANGE
+ERR_BUSY = -5                      # RMU_ERR_BUSY
+GEN_LIVE, GEN_EOS, GEN_MAX_NEW, GEN_MAX_POS = 0, 1, 2, 3   # RMU_GEN_*: a session row's status
 
 
 class SamplingC(C.Structure):
@@ -139,6 +142,16 @@ SIGNATURES = {
                                               C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p,
                                               C.POINTER(C.c_int32), C.c_void_p]),
     "rmu_prompt_lookup_draft": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "rmu_decoder_session_create": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
+    "rmu_decoder_session_destroy": (None, [C.c_void_p]),
+    "rmu_decoder_session_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_decoder_session_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32),
+                                           C.c_void_p, C.c_void_p]),
+    "rmu_decoder_session_cancel": (C.c_int, [C.c_void_p, C.c_int]),
+    "rmu_decoder_session_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                           C.POINTER(C.c_uint32)]),
+    "rmu_debug_kv_regions": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "rmu_encoder_destroy": (None, [C.c_void_p]),
     "rmu_encoder_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_void_p, C.c_void_p]),
@@ -226,6 +239,8 @@ SIGNATURES = {
                                         C.POINTER(SamplingC), C.c_void_p, C.c_void_p]),
     "rmu_debug_sample_verify_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64,
                                                C.c_int64, C.POINTER(SamplingC), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rmu_debug_sample_session_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rmu_debug_generate_drafts": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(SamplingC), C.c_uint64, C.c_int,
                                             C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p,
                                             C.POINTER(C.c_int32), C.c_void_p]),

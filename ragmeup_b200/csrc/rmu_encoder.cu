@@ -17,6 +17,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <functional>
+#include <map>
 #include <mutex>
 #include <type_traits>
 #include <vector>
@@ -2192,7 +2193,9 @@ __global__ void set_int_kernel(int* p, int v) { *p = v; }
 // The chosen id is written to *token and its presence bit set.  The batched decode runs one CTA per live row r
 // (SampleRows): logits row r, token r, and the presence bits and Philox seed of the row's sequence seq[r].  A
 // prompt-lookup verify pass runs one CTA per row of one sequence: row r has its own presence bits (seq null), the
-// call's seed (seeds null) and step + r (row_step), so it samples as the sequential step it stands for.
+// call's seed (seeds null) and step + r (row_step), so it samples as the sequential step it stands for.  A decode
+// session's rows each carry their own settings and step (args, steps per sequence): row r then samples exactly as
+// sequential step steps[seq[r]] of its own request would.
 // ---------------------------------------------------------------------------------------------------
 constexpr int kSampleThreads = 1024;
 constexpr int kSampleCap = 256;               // the largest top_k and the most candidates
@@ -2207,6 +2210,8 @@ struct SampleRows {
     const unsigned long long* seeds = nullptr;    // [sequences]; null: `seed` for every row
     size_t words = 0;                             // presence words per sequence; 0: one row, presence at its start
     bool row_step = false;                        // row r draws at step + r
+    const SampleArgs* args = nullptr;             // [sequences]; null: `a` for every row
+    const unsigned long long* steps = nullptr;    // [sequences]: the sequence's Philox step; null: `step`
 };
 
 // Philox4x32-10 (Salmon et al., SC'11) with counter (step, 0) and key seed: the first output word's high 24 bits / 2^24
@@ -2240,6 +2245,8 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(float* __restric
         presence += q * rows.words;
         if (rows.seeds) seed = rows.seeds[q];
         if (rows.row_step) step += blockIdx.x;
+        if (rows.args) a = rows.args[q];
+        if (rows.steps) step = rows.steps[q];
     }
     unsigned long long best = 0ull;
     for (int i = tid; i < V; i += blockDim.x) {
@@ -2845,10 +2852,21 @@ static int qwen3_layer_tail(rmu_encoder* e, const EncLayer& L, int M, bool gemv,
     return decoder_gemm(e, GEMM_BIAS_RESF32_F32, e->FF, L, 3, g, gemv, st);
 }
 
-// layer l's K / V planes in the KV cache (kv_append_kernel's layout)
-static __half* kv_layer(rmu_encoder* e, int l) {
-    return e->kv_cache.as<__half>() + static_cast<size_t>(l) * 4 * e->qext.kv_heads * e->kv_cap * kQwenHD;
+// A KV cache in kv_append_kernel's layout, [layers][K hi | K lo | V hi | V lo][kv_heads][cap][128]: the handle's own
+// (handle_kv) or a decode session's
+struct KvView {
+    __half* base = nullptr;
+    int cap = 0;
+};
+
+static KvView handle_kv(rmu_encoder* e) { return KvView{e->kv_cache.as<__half>(), e->kv_cap}; }
+
+// layer l's K / V planes in the cache v
+static __half* kv_layer(const rmu_encoder* e, const KvView& v, int l) {
+    return v.base + static_cast<size_t>(l) * 4 * e->qext.kv_heads * v.cap * kQwenHD;
 }
+
+static __half* kv_layer(rmu_encoder* e, int l) { return kv_layer(e, handle_kv(e), l); }
 
 // the rmu_decoder_* entry points run on decoder handles only
 static int check_decoder(const rmu_encoder* e, const std::string& fn) {
@@ -2914,19 +2932,19 @@ static int qwen3_check_range(rmu_encoder* e, cudaStream_t st) {
 // position P + t and its k / v go to cache row P + t + shift; attention is attention_causal_kernel's cached form
 // (PrefixKeys), keys below P from the shared prefix rows.  The range flag is not cleared: the caller clears it once
 // per call.  The activation workspace must already hold T rows (ensure_tokens).
-static int run_batch_prefill(rmu_encoder* e, const int32_t* ids, const int32_t* cu, const int* shift, int B, int T,
-                             int max_own, int P, bool gemv, cudaStream_t st) {
+static int run_batch_prefill(rmu_encoder* e, const KvView& kvv, const int32_t* ids, const int32_t* cu, const int* shift,
+                             int B, int T, int max_own, int P, bool gemv, cudaStream_t st) {
     const rmu_bert_config& c = e->cfg;
     const int nh = c.heads, kv = e->qext.kv_heads;
     int rc = launch_embed_rows(ids, T, c.hidden, c.vocab_size, e->word, e->PRE, st);
     for (int l = 0; l < c.layers && rc == RMU_OK; ++l) {
         const EncLayer& L = e->layers[l];
         rc = qwen3_attention_inputs(e, L, T, gemv, st);
-        if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, T, nh, kv, 0, e->kv_cap, kv_layer(e, l), st, e->POSI, shift);
+        if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, T, nh, kv, 0, kvv.cap, kv_layer(e, kvv, l), st, e->POSI, shift);
         PrefixKeys pk;
-        pk.kv = kv_layer(e, l);
+        pk.kv = kv_layer(e, kvv, l);
         pk.shift = shift;
-        pk.cap = e->kv_cap;
+        pk.cap = kvv.cap;
         pk.P = P;
         if (rc == RMU_OK) rc = launch_attention_cached(e->QKVP.hi, e->QKVP.lo, cu, B, nh, kv, max_own, pk, e->CTX.hi, e->CTX.lo, st);
         if (rc == RMU_OK) rc = qwen3_layer_tail(e, L, T, gemv, st);
@@ -2957,8 +2975,8 @@ static int check_sampling(const std::string& fn, const rmu_sampling* s) {
 // ids [M] (device) at the positions in e->POSI (uploaded by the caller), row r's k / v into cache row pos[r] +
 // shift[r] and its attention over keys [0, pos[r] + 1) with the DecRows prefix mapping P; maxn = the most keys of any
 // row; part holds M * decode_part_floats(heads, maxn) floats.  The rows' hidden states are left in e->PRE.
-static int run_decode_rows(rmu_encoder* e, const int* ids, int M, const int* shift, int P, int maxn, float* part,
-                           cudaStream_t st) {
+static int run_decode_rows(rmu_encoder* e, const KvView& kvv, const int* ids, int M, const int* shift, int P, int maxn,
+                           float* part, cudaStream_t st) {
     const rmu_bert_config& c = e->cfg;
     const int nh = c.heads, kv = e->qext.kv_heads;
     int rc = launch_embed_rows(ids, M, c.hidden, c.vocab_size, e->word, e->PRE, st);
@@ -2970,9 +2988,9 @@ static int run_decode_rows(rmu_encoder* e, const int* ids, int M, const int* shi
     for (int l = 0; l < c.layers && rc == RMU_OK; ++l) {
         const EncLayer& Ly = e->layers[l];
         rc = qwen3_attention_inputs(e, Ly, M, true, st);
-        if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, M, nh, kv, 0, e->kv_cap, kv_layer(e, l), st, e->POSI, shift);
+        if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, M, nh, kv, 0, kvv.cap, kv_layer(e, kvv, l), st, e->POSI, shift);
         if (rc == RMU_OK)
-            rc = launch_attention_decode(e->QKVP.hi, e->QKVP.lo, kv_layer(e, l), nh, kv, e->kv_cap, maxn, part, e->CTX.hi,
+            rc = launch_attention_decode(e->QKVP.hi, e->QKVP.lo, kv_layer(e, kvv, l), nh, kv, kvv.cap, maxn, part, e->CTX.hi,
                                          e->CTX.lo, st, M, dr);
         if (rc == RMU_OK) rc = qwen3_layer_tail(e, Ly, M, true, st);
     }
@@ -3119,7 +3137,7 @@ static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* i
             RMU_CUDA(cudaMemcpyAsync(ints, hints.data(), M * sizeof(int), cudaMemcpyHostToDevice, st));
             RMU_CUDA(cudaMemcpyAsync(e->POSI, hpos.data(), M * sizeof(int), cudaMemcpyHostToDevice, st));
             rc = launch_presence_rows(presence, words, ints, M, prow, st);
-            if (rc == RMU_OK) rc = run_decode_rows(e, ints, M, ints + R, 0, p + M, part, st);
+            if (rc == RMU_OK) rc = run_decode_rows(e, handle_kv(e), ints, M, ints + R, 0, p + M, part, st);
             if (rc == RMU_OK) rc = run_lm_head(e, e->PRE, M, logits, st);
             if (rc == RMU_OK && logits_h)
                 RMU_CUDA(cudaMemcpyAsync(staged.data(), logits, static_cast<size_t>(M) * V * sizeof(float),
@@ -4132,7 +4150,7 @@ int rmu_decoder_generate_batch(rmu_encoder* e, const int32_t* ids_h, const int32
         packed.insert(packed.end(), hshift.begin(), hshift.end());
         RMU_CUDA(cudaMemcpyAsync(ints, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice, st));
         RMU_CUDA(cudaMemcpyAsync(e->POSI, hpos.data(), hpos.size() * 4, cudaMemcpyHostToDevice, st));
-        int r = run_batch_prefill(e, ints, ints + n, ints + n + nb + 1, nb, n, max_own, gather ? P : 0, gemv, st);
+        int r = run_batch_prefill(e, handle_kv(e), ints, ints + n, ints + n + nb + 1, nb, n, max_own, gather ? P : 0, gemv, st);
         for (int i = 0; i < nb && r == RMU_OK && gather; ++i)
             RMU_CUDA(cudaMemcpyAsync(last + static_cast<size_t>(seqs[i]) * H, e->PRE + static_cast<size_t>(hcu[i + 1] - 1) * H,
                                      static_cast<size_t>(H) * 4, cudaMemcpyDeviceToDevice, st));
@@ -4163,7 +4181,7 @@ int rmu_decoder_generate_batch(rmu_encoder* e, const int32_t* ids_h, const int32
             int maxn = 0;
             for (int r = 0; r < M; ++r) maxn = std::max(maxn, hpos[r] + 1);
             RMU_CUDA(cudaMemcpyAsync(e->POSI, hpos.data(), hpos.size() * 4, cudaMemcpyHostToDevice, st));
-            rc = run_decode_rows(e, ints, M, ints + M, P, maxn, part, st);
+            rc = run_decode_rows(e, handle_kv(e), ints, M, ints + M, P, maxn, part, st);
             x_last = e->PRE;
         }
         // logits for the M live rows (step 0: last[b] in prompt order), then the sampler
@@ -4196,6 +4214,553 @@ int rmu_decoder_generate_batch(rmu_encoder* e, const int32_t* ids_h, const int32
     for (int b = 0; b < B; ++b) n_out_h[b] = rc == RMU_OK ? n_b[b] : 0;
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
+    return RMU_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------
+// Continuous batching (DESIGN.md, "Continuous batching"): a decode session outlives one call.  Requests join it
+// (rmu_decoder_session_add) and leave it (a stop, rmu_decoder_session_cancel) between steps; each step
+// (rmu_decoder_session_step) runs every live row at M = live.  The session owns its KV cache, in the handle cache's
+// layout; a request of T prompt tokens holds the region [base, base + min(T + max_new, max_pos)) and reads key k at
+// row k + base (shift = base, P = 0).  Every entry point holds the handle's mu for its own duration only.
+// ---------------------------------------------------------------------------------------------------
+
+// The regions of a session's KV cache: the used ones by base; a gap is whatever lies between them, so a freed region
+// merges with its free neighbours by construction.  Placement is first fit; past the last used region the cache grows,
+// which moves no region, so every live row's shift stays valid.
+struct KvRegions {
+    std::map<int, int> used;                      // base -> rows
+    int cap = 0;
+    // the first gap of n rows; -1 when none fits, *need then the cap that fits n rows after the last used region
+    int fit(int n, int* need) const {
+        int at = 0;
+        for (const auto& r : used) {
+            if (r.first - at >= n) return at;
+            at = r.first + r.second;
+        }
+        if (cap - at >= n) return at;
+        *need = at + n;
+        return -1;
+    }
+    // place n rows, growing cap when no gap fits -> the base
+    int place(int n) {
+        int need = 0;
+        int base = fit(n, &need);
+        if (base < 0) { cap = need; base = need - n; }
+        used[base] = n;
+        return base;
+    }
+};
+
+struct rmu_gen_session {
+    rmu_encoder* e = nullptr;
+    KvRegions reg;
+    void* kv = nullptr;                           // [L][4][kv_heads][reg.cap][128] halves
+    // persistent device state, one entry per row slot: presence bits [16, words] | seeds [16] | settings [16] |
+    // Philox steps [16]
+    void* state = nullptr;
+    size_t words = 0, o_seed = 0, o_args = 0, o_steps = 0;
+    DevBuf ws;                                    // one call's scratch: logits, last rows, partials, tokens, ints
+    struct Row {
+        bool live = false;
+        int base = 0, T = 0, n = 0, max_new = 0, last = 0;
+        rmu_sampling s{};
+    };
+    Row rows[RMU_MAX_GENERATE_BATCH];
+    cudaEvent_t done = nullptr;                   // the session's last use of its buffers
+};
+
+namespace {
+
+KvView session_kv(rmu_gen_session* S) { return KvView{static_cast<__half*>(S->kv), S->reg.cap}; }
+unsigned* session_presence(rmu_gen_session* S, int slot) {
+    return static_cast<unsigned*>(S->state) + static_cast<size_t>(slot) * S->words;
+}
+
+// grow the session's cache to cap rows, each (layer, plane, head) block copied to the new pitch by one 2D copy
+int session_grow(rmu_gen_session* S, int cap, cudaStream_t st) {
+    rmu_encoder* e = S->e;
+    const size_t blocks = static_cast<size_t>(e->cfg.layers) * 4 * e->qext.kv_heads, row = kQwenHD * sizeof(__half);
+    void* p = nullptr;
+    const cudaError_t err = cudaMalloc(&p, blocks * cap * row);
+    if (err != cudaSuccess) {
+        cudaGetLastError();
+        set_error("cannot allocate " + std::to_string(blocks * cap * row) + " bytes of device memory: " +
+                  cudaGetErrorString(err));
+        return RMU_ERR_CUDA;
+    }
+    if (S->reg.cap > 0) {
+        cudaError_t ce = cudaMemcpy2DAsync(p, cap * row, S->kv, S->reg.cap * row, S->reg.cap * row, blocks,
+                                           cudaMemcpyDeviceToDevice, st);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+        if (ce != cudaSuccess) {                  // the old cache stays in place
+            cudaFree(p);
+            set_error(std::string("the session's KV cache copy failed: ") + cudaGetErrorString(ce));
+            return RMU_ERR_CUDA;
+        }
+    }
+    cudaFree(S->kv);
+    S->kv = p;
+    S->reg.cap = cap;
+    return RMU_OK;
+}
+
+// one call's scratch: logits [16, V] | last hidden rows [16, H] | decode partials | presence backup [16, words] |
+// tokens [16] | ints [n_int].  The partials are sized for 16 rows over the longest region in the session, and the
+// buffer grows with half again as much headroom, so a reply's steps do not re-grow it as its keys pass each split.
+struct SessionWs {
+    float *logits, *last, *part;
+    unsigned* backup;
+    int *tok, *ints;
+};
+
+int session_ws(rmu_gen_session* S, int M, size_t part_floats, size_t n_int, SessionWs* w) {
+    const rmu_bert_config& c = S->e->cfg;
+    auto al = [](size_t bytes) { return (bytes + 255) / 256 * 256; };
+    const size_t R = std::max(M, RMU_MAX_GENERATE_BATCH);
+    int longest = 1;
+    for (const auto& r : S->reg.used) longest = std::max(longest, r.second);
+    part_floats = std::max(part_floats, RMU_MAX_GENERATE_BATCH * decode_part_floats(c.heads, longest));
+    const size_t o_last = al(R * c.vocab_size * 4);
+    const size_t o_part = o_last + al(R * c.hidden * 4);
+    const size_t o_back = o_part + al(part_floats * 4);
+    const size_t o_tok = o_back + al(RMU_MAX_GENERATE_BATCH * S->words * 4);
+    const size_t o_int = o_tok + al(RMU_MAX_GENERATE_BATCH * 4);
+    const size_t need = o_int + n_int * 4;
+    const int rc = grow(S->ws, need, need + need / 2);
+    if (rc != RMU_OK) return rc;
+    char* b = S->ws.as<char>();
+    *w = SessionWs{reinterpret_cast<float*>(b), reinterpret_cast<float*>(b + o_last), reinterpret_cast<float*>(b + o_part),
+                   reinterpret_cast<unsigned*>(b + o_back), reinterpret_cast<int*>(b + o_tok),
+                   reinterpret_cast<int*>(b + o_int)};
+    return RMU_OK;
+}
+
+// the sampler over M rows whose slots are seq (device [M]), each with its slot's bits, seed, settings and step
+int session_sample(rmu_gen_session* S, float* logits, int M, const int* seq, int* tok, cudaStream_t st) {
+    const char* st8 = static_cast<const char*>(S->state);
+    SampleRows sr;
+    sr.seq = seq;
+    sr.seeds = reinterpret_cast<const unsigned long long*>(st8 + S->o_seed);
+    sr.words = S->words;
+    sr.args = reinterpret_cast<const SampleArgs*>(st8 + S->o_args);
+    sr.steps = reinterpret_cast<const unsigned long long*>(st8 + S->o_steps);
+    return launch_sample(logits, S->e->cfg.vocab_size, static_cast<unsigned*>(S->state), SampleArgs{}, -1.f, 0ull, 0ull,
+                         tok, st, M, sr);
+}
+
+// upload the Philox step of every slot (its tokens so far)
+int session_upload_steps(rmu_gen_session* S, cudaStream_t st) {
+    unsigned long long h[RMU_MAX_GENERATE_BATCH];
+    for (int i = 0; i < RMU_MAX_GENERATE_BATCH; ++i) h[i] = static_cast<unsigned long long>(S->rows[i].n);
+    RMU_CUDA(cudaMemcpyAsync(static_cast<char*>(S->state) + S->o_steps, h, sizeof(h), cudaMemcpyHostToDevice, st));
+    return RMU_OK;
+}
+
+// whether the fp16 range flag is raised, cleared again when it is (synchronises st)
+int session_read_range(rmu_encoder* e, bool* raised, cudaStream_t st) {
+    int flag = 0;
+    RMU_CUDA(cudaMemcpyAsync(&flag, e->range_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    RMU_CUDA(cudaStreamSynchronize(st));
+    *raised = flag != 0;
+    if (flag) RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
+    return RMU_OK;
+}
+
+// One pass over the slots `slots` (row r = slots[r]): with T null a decode step, each row feeding its last token at
+// position T + n - 1; else the prefill of new requests, prompt r = ids_h[cu_h[req[r]] ..) (one varlen run; gemv: one
+// one-token prompt on the decode GEMV).  Then the LM head, logits to logits_h (nullable, [M, V]), the sampler, the tokens
+// to t_h.  *raised <- the range flag; when raised, the presence bits are restored to what they were before the pass.
+int session_pass(rmu_gen_session* S, const std::vector<int>& slots, const int32_t* ids_h, const int32_t* cu_h,
+                 const std::vector<int>* req, bool gemv, float* logits_h, int* t_h, bool* raised, cudaStream_t st) {
+    rmu_encoder* e = S->e;
+    const rmu_bert_config& c = e->cfg;
+    const int M = static_cast<int>(slots.size()), V = c.vocab_size, H = c.hidden;
+    std::vector<int> hid, hcu{0}, hshift, hpos;
+    int maxn = 0, max_own = 0;
+    for (int r = 0; r < M; ++r) {
+        const rmu_gen_session::Row& w = S->rows[slots[r]];
+        if (req) {
+            const int b = (*req)[r], T = cu_h[b + 1] - cu_h[b];
+            for (int t = 0; t < T; ++t) {
+                hid.push_back(ids_h[cu_h[b] + t]);
+                hpos.push_back(t);
+                hshift.push_back(w.base);
+            }
+            hcu.push_back(hcu.back() + T);
+            max_own = std::max(max_own, T);
+        } else {
+            hid.push_back(w.last);
+            hpos.push_back(w.T + w.n - 1);
+            hshift.push_back(w.base);
+            maxn = std::max(maxn, w.T + w.n);
+        }
+    }
+    const int rows = static_cast<int>(hid.size());
+    std::vector<int> packed(hid);
+    packed.insert(packed.end(), hshift.begin(), hshift.end());
+    packed.insert(packed.end(), slots.begin(), slots.end());
+    packed.insert(packed.end(), hcu.begin(), hcu.end());
+    int* seq_off = nullptr;
+    SessionWs w;
+    const size_t part = req ? 0 : static_cast<size_t>(M) * decode_part_floats(c.heads, maxn);
+    int rc = session_ws(S, M, part, packed.size(), &w);
+    if (rc == RMU_OK) rc = ensure_tokens(e, rows, M);
+    if (rc != RMU_OK) return rc;
+    int* ids = w.ints;
+    int* shift = ids + rows;
+    seq_off = shift + rows;
+    int* cu = seq_off + M;
+    RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
+    // pageable sources: each copy has taken its bytes when it returns
+    RMU_CUDA(cudaMemcpyAsync(w.ints, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(e->POSI, hpos.data(), hpos.size() * 4, cudaMemcpyHostToDevice, st));
+    rc = session_upload_steps(S, st);
+    if (rc != RMU_OK) return rc;
+    RMU_CUDA(cudaMemcpyAsync(w.backup, S->state, RMU_MAX_GENERATE_BATCH * S->words * 4, cudaMemcpyDeviceToDevice, st));
+    const KvView kvv = session_kv(S);
+    const float* x = e->PRE;
+    if (req) {
+        rc = run_batch_prefill(e, kvv, ids, cu, shift, M, rows, max_own, 0, gemv, st);
+        for (int r = 0; r < M && rc == RMU_OK; ++r)
+            RMU_CUDA(cudaMemcpyAsync(w.last + static_cast<size_t>(r) * H, e->PRE + static_cast<size_t>(hcu[r + 1] - 1) * H,
+                                     static_cast<size_t>(H) * 4, cudaMemcpyDeviceToDevice, st));
+        x = w.last;
+    } else {
+        rc = run_decode_rows(e, kvv, ids, M, shift, 0, maxn, w.part, st);
+    }
+    if (rc == RMU_OK) rc = run_lm_head(e, x, M, w.logits, st);
+    if (rc == RMU_OK && logits_h)
+        RMU_CUDA(cudaMemcpyAsync(logits_h, w.logits, static_cast<size_t>(M) * V * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (rc == RMU_OK) rc = session_sample(S, w.logits, M, seq_off, w.tok, st);
+    if (rc != RMU_OK) return rc;
+    RMU_CUDA(cudaMemcpyAsync(t_h, w.tok, static_cast<size_t>(M) * sizeof(int), cudaMemcpyDeviceToHost, st));
+    rc = session_read_range(e, raised, st);       // synchronises st
+    if (rc == RMU_OK && *raised)
+        RMU_CUDA(cudaMemcpyAsync(S->state, w.backup, RMU_MAX_GENERATE_BATCH * S->words * 4, cudaMemcpyDeviceToDevice, st));
+    return rc;
+}
+
+// a row's status after its n-th token t: live, or why it stopped (rmu_decoder_generate's rules)
+int row_status(const rmu_gen_session::Row& w, int t, int max_pos) {
+    for (int i = 0; i < w.s.n_eos; ++i)
+        if (t == w.s.eos_ids[i]) return RMU_GEN_EOS;
+    if (w.n == w.max_new) return RMU_GEN_MAX_NEW;
+    if (w.T + w.n >= max_pos) return RMU_GEN_MAX_POS;
+    return RMU_GEN_LIVE;
+}
+
+void release_row(rmu_gen_session* S, int slot) {
+    S->reg.used.erase(S->rows[slot].base);
+    S->rows[slot].live = false;
+}
+
+// waits on the handle's workspace and the session's last use on st
+int session_begin(rmu_gen_session* S, cudaStream_t st) {
+    RMU_CUDA(cudaStreamWaitEvent(st, S->e->ws_done, 0));
+    RMU_CUDA(cudaStreamWaitEvent(st, S->done, 0));
+    return RMU_OK;
+}
+
+int session_end(rmu_gen_session* S, cudaStream_t st) {
+    RMU_CUDA(cudaEventRecord(S->done, st));
+    RMU_CUDA(cudaEventRecord(S->e->ws_done, st));
+    return RMU_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rmu_decoder_session_create(rmu_encoder* e, rmu_gen_session** out) {
+    const std::string fn("rmu_decoder_session_create");
+    if (!e || !out) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
+    *out = nullptr;
+    int rc = check_decoder(e, fn);
+    if (rc != RMU_OK) return rc;
+    std::lock_guard<std::mutex> g(e->mu);
+    rmu_gen_session* S = new rmu_gen_session();
+    S->e = e;
+    S->words = (static_cast<size_t>(e->cfg.vocab_size) + 31) / 32;
+    S->o_seed = (RMU_MAX_GENERATE_BATCH * S->words * 4 + 255) / 256 * 256;
+    S->o_args = S->o_seed + RMU_MAX_GENERATE_BATCH * 8;
+    S->o_steps = S->o_args + (RMU_MAX_GENERATE_BATCH * sizeof(SampleArgs) + 7) / 8 * 8;
+    const size_t bytes = S->o_steps + RMU_MAX_GENERATE_BATCH * 8;
+    cudaError_t err = cudaSetDevice(e->device);
+    if (err == cudaSuccess) err = cudaMalloc(&S->state, bytes);
+    if (err == cudaSuccess) err = cudaEventCreateWithFlags(&S->done, cudaEventDisableTiming);
+    if (err == cudaSuccess) err = cudaMemset(S->state, 0, bytes);
+    if (err != cudaSuccess) {
+        cudaGetLastError();
+        set_error(fn + ": " + cudaGetErrorString(err));
+        cudaFree(S->state);
+        if (S->done) cudaEventDestroy(S->done);
+        delete S;
+        return RMU_ERR_CUDA;
+    }
+    *out = S;
+    return RMU_OK;
+}
+
+void rmu_decoder_session_destroy(rmu_gen_session* S) {
+    if (!S) return;
+    {
+        std::lock_guard<std::mutex> g(S->e->mu);
+        cudaEventSynchronize(S->done);
+        cudaFree(S->kv);
+        cudaFree(S->state);
+        S->ws.release();
+        cudaEventDestroy(S->done);
+    }
+    delete S;
+}
+
+int rmu_decoder_session_add(rmu_gen_session* S, const int32_t* ids_h, const int32_t* cu_h, int B, const rmu_sampling* s_h,
+                            const uint64_t* seeds_h, const int32_t* max_new_h, int32_t* slot_h, int32_t* tok_h,
+                            int32_t* status_h, float* logits_h, void* stream) {
+    const std::string fn("rmu_decoder_session_add");
+    if (!S || !ids_h || !cu_h || !s_h || !seeds_h || !max_new_h || !slot_h || !tok_h || !status_h || B < 1 ||
+        B > RMU_MAX_GENERATE_BATCH) {
+        set_error(fn + ": bad argument");
+        return RMU_ERR_ARG;
+    }
+    rmu_encoder* e = S->e;
+    int rc = check_decoder(e, fn);
+    if (rc != RMU_OK) return rc;
+    if (!e->has_lm_head) { set_error(fn + ": no LM head is attached (rmu_decoder_set_lm_head)"); return RMU_ERR_ARG; }
+    rc = check_nf4_intact(e, fn);
+    if (rc != RMU_OK) return rc;
+    const rmu_bert_config& c = e->cfg;
+    std::vector<int> Tb(B), nrows(B);
+    for (int b = 0; b < B; ++b) {
+        if (cu_h[b + 1] <= cu_h[b] || cu_h[b] < 0) { set_error(fn + ": prompt " + std::to_string(b) + " is empty"); return RMU_ERR_ARG; }
+        if (max_new_h[b] < 1) { set_error(fn + ": max_new_tokens must be at least 1"); return RMU_ERR_ARG; }
+        Tb[b] = cu_h[b + 1] - cu_h[b];
+        if (Tb[b] >= c.max_pos) {
+            set_error(fn + ": a prompt of " + std::to_string(Tb[b]) + " tokens leaves no position for a new token " +
+                      "(max_position_embeddings " + std::to_string(c.max_pos) + ")");
+            return RMU_ERR_ARG;
+        }
+        rc = check_sampling(fn, s_h + b);
+        if (rc != RMU_OK) return rc;
+        for (int i = cu_h[b]; i < cu_h[b + 1]; ++i)
+            if (ids_h[i] < 0 || ids_h[i] >= c.vocab_size) { set_error(fn + ": token id out of range"); return RMU_ERR_ARG; }
+        nrows[b] = static_cast<int>(std::min<int64_t>(static_cast<int64_t>(Tb[b]) + max_new_h[b], c.max_pos));
+    }
+    std::lock_guard<std::mutex> g(e->mu);
+    std::vector<int> free_slots;
+    for (int i = 0; i < RMU_MAX_GENERATE_BATCH; ++i)
+        if (!S->rows[i].live) free_slots.push_back(i);
+    int live = RMU_MAX_GENERATE_BATCH - static_cast<int>(free_slots.size());
+    if (static_cast<int>(free_slots.size()) < B) {
+        set_error(fn + ": " + std::to_string(live) + " rows are live and " + std::to_string(B) + " more do not fit (at most " +
+                  std::to_string(RMU_MAX_GENERATE_BATCH) + ")");
+        return RMU_ERR_BUSY;
+    }
+    KvRegions reg = S->reg;
+    std::vector<int> base(B);
+    for (int b = 0; b < B; ++b) base[b] = reg.place(nrows[b]);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    RMU_CUDA(cudaSetDevice(e->device));
+    rc = session_begin(S, st);
+    if (rc != RMU_OK) return rc;
+    if (reg.cap > S->reg.cap) {
+        rc = session_grow(S, reg.cap, st);
+        if (rc != RMU_OK) {
+            if (live > 0) {
+                set_error(fn + ": the session's KV cache cannot grow to " + std::to_string(reg.cap) + " positions while " +
+                          std::to_string(live) + " rows are live: " + rmu_last_error());
+                return RMU_ERR_BUSY;
+            }
+            set_error(fn + ": the KV cache for " + std::to_string(reg.cap) + " positions: " + rmu_last_error());
+            return rc;
+        }
+    }
+    S->reg = reg;
+    std::vector<int> slots(B);
+    std::vector<unsigned> bits(S->words);
+    for (int b = 0; b < B; ++b) {
+        const int q = slots[b] = free_slots[b];
+        rmu_gen_session::Row& w = S->rows[q];
+        w = rmu_gen_session::Row{};
+        w.live = true;
+        w.base = base[b];
+        w.T = Tb[b];
+        w.max_new = max_new_h[b];
+        w.s = s_h[b];
+    }
+    // from here on a failure releases the new rows (a grown cache stays grown)
+    auto settings = [&]() -> int {
+        for (int b = 0; b < B; ++b) {
+            const rmu_sampling& sb = s_h[b];
+            const SampleArgs sa{sb.do_sample ? 1 : 0, sb.top_k, sb.temperature, sb.top_p, sb.repetition_penalty};
+            const unsigned long long seed = seeds_h[b];
+            char* st8 = static_cast<char*>(S->state);
+            RMU_CUDA(cudaMemcpyAsync(st8 + S->o_seed + slots[b] * 8, &seed, 8, cudaMemcpyHostToDevice, st));
+            RMU_CUDA(cudaMemcpyAsync(st8 + S->o_args + slots[b] * sizeof(SampleArgs), &sa, sizeof(SampleArgs),
+                                     cudaMemcpyHostToDevice, st));
+        }
+        return RMU_OK;
+    };
+    rc = settings();
+    // the prompt's presence bits of request b's slot
+    auto upload_bits = [&](int b) -> int {
+        std::fill(bits.begin(), bits.end(), 0u);
+        for (int i = cu_h[b]; i < cu_h[b + 1]; ++i) bits[ids_h[i] >> 5] |= 1u << (ids_h[i] & 31);
+        RMU_CUDA(cudaMemcpyAsync(session_presence(S, slots[b]), bits.data(), S->words * 4, cudaMemcpyHostToDevice, st));
+        return RMU_OK;
+    };
+    for (int b = 0; b < B && rc == RMU_OK; ++b) rc = upload_bits(b);
+    // prefill groups as rmu_decoder_generate_batch runs them: an NF4 handle's one-token prompts alone, on the GEMV,
+    // the others as one varlen run
+    const int V = c.vocab_size;
+    std::vector<int> t_h(B, 0), err(B, RMU_OK);
+    std::vector<std::vector<int>> groups;
+    std::vector<int> group;
+    for (int b = 0; b < B; ++b) {
+        if (e->nf4 && Tb[b] == 1) groups.push_back({b});
+        else group.push_back(b);
+    }
+    if (!group.empty()) groups.push_back(group);
+    auto run = [&](const std::vector<int>& g, bool* raised) -> int {
+        std::vector<int> sl, tt(g.size());
+        for (int b : g) sl.push_back(slots[b]);
+        const bool gemv = e->nf4 && g.size() == 1 && Tb[g[0]] == 1;
+        std::vector<float> lg(logits_h ? g.size() * static_cast<size_t>(V) : 0);
+        int r = session_pass(S, sl, ids_h, cu_h, &g, gemv, logits_h ? lg.data() : nullptr, tt.data(), raised, st);
+        if (r != RMU_OK || *raised) return r;
+        for (size_t i = 0; i < g.size(); ++i) {
+            t_h[g[i]] = tt[i];
+            if (logits_h) std::copy(lg.begin() + i * V, lg.begin() + (i + 1) * V, logits_h + static_cast<size_t>(g[i]) * V);
+        }
+        return RMU_OK;
+    };
+    for (const auto& gr : groups) {
+        if (rc != RMU_OK) break;
+        bool raised = false;
+        rc = run(gr, &raised);
+        if (rc != RMU_OK || !raised) continue;
+        // one request's activations left fp16's range: redo them one at a time, and end only those whose own run raises
+        // the flag too
+        for (int b : gr) {
+            if (gr.size() > 1) {
+                rc = upload_bits(b);
+                if (rc == RMU_OK) rc = run({b}, &raised);
+                if (rc != RMU_OK) break;
+            }
+            if (raised) err[b] = RMU_ERR_RANGE;
+        }
+    }
+    if (rc != RMU_OK) {
+        for (int b = 0; b < B; ++b) release_row(S, slots[b]);
+        return rc;
+    }
+    for (int b = 0; b < B; ++b) {
+        rmu_gen_session::Row& w = S->rows[slots[b]];
+        tok_h[b] = t_h[b];
+        if (err[b] != RMU_OK) {
+            status_h[b] = err[b];
+        } else {
+            w.n = 1;
+            w.last = t_h[b];
+            status_h[b] = row_status(w, t_h[b], c.max_pos);
+        }
+        slot_h[b] = status_h[b] == RMU_GEN_LIVE ? slots[b] : -1;
+        if (status_h[b] != RMU_GEN_LIVE) release_row(S, slots[b]);
+    }
+    return session_end(S, st);
+}
+
+int rmu_decoder_session_step(rmu_gen_session* S, int32_t* slot_h, int32_t* tok_h, int32_t* status_h, int32_t* n_h,
+                             float* logits_h, void* stream) {
+    const std::string fn("rmu_decoder_session_step");
+    if (!S || !slot_h || !tok_h || !status_h || !n_h) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
+    *n_h = 0;
+    rmu_encoder* e = S->e;
+    std::lock_guard<std::mutex> g(e->mu);
+    std::vector<int> slots;
+    for (int i = 0; i < RMU_MAX_GENERATE_BATCH; ++i)
+        if (S->rows[i].live) slots.push_back(i);
+    if (slots.empty()) return RMU_OK;
+    const int M = static_cast<int>(slots.size()), V = e->cfg.vocab_size;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int rc = RMU_OK;
+    const cudaError_t de = cudaSetDevice(e->device);
+    if (de != cudaSuccess) { set_error(fn + ": " + cudaGetErrorString(de)); rc = RMU_ERR_CUDA; }
+    if (rc == RMU_OK) rc = session_begin(S, st);
+    std::vector<int> t_h(M, 0), err(M, RMU_OK);
+    bool raised = false;
+    if (rc == RMU_OK) rc = session_pass(S, slots, nullptr, nullptr, nullptr, true, logits_h, t_h.data(), &raised, st);
+    if (rc == RMU_OK && raised) {
+        // redo the rows one at a time; only a row whose own step raises the flag ends, with RMU_ERR_RANGE
+        for (int r = 0; r < M && rc == RMU_OK; ++r) {
+            if (M > 1)
+                rc = session_pass(S, {slots[r]}, nullptr, nullptr, nullptr, true,
+                                  logits_h ? logits_h + static_cast<size_t>(r) * V : nullptr, &t_h[r], &raised, st);
+            if (raised) err[r] = RMU_ERR_RANGE;
+        }
+    }
+    if (rc != RMU_OK) {
+        // a failed step leaves its rows without a consistent state: every one of them is released
+        for (int q : slots) release_row(S, q);
+        return rc;
+    }
+    for (int r = 0; r < M; ++r) {
+        rmu_gen_session::Row& w = S->rows[slots[r]];
+        slot_h[r] = slots[r];
+        tok_h[r] = t_h[r];
+        if (err[r] != RMU_OK) {
+            status_h[r] = err[r];
+        } else {
+            ++w.n;
+            w.last = t_h[r];
+            status_h[r] = row_status(w, t_h[r], e->cfg.max_pos);
+        }
+        if (status_h[r] != RMU_GEN_LIVE) release_row(S, slots[r]);
+    }
+    *n_h = M;
+    return session_end(S, st);
+}
+
+int rmu_decoder_session_cancel(rmu_gen_session* S, int slot) {
+    if (!S || slot < 0 || slot >= RMU_MAX_GENERATE_BATCH) {
+        set_error("rmu_decoder_session_cancel: bad argument");
+        return RMU_ERR_ARG;
+    }
+    std::lock_guard<std::mutex> g(S->e->mu);
+    if (!S->rows[slot].live) { set_error("rmu_decoder_session_cancel: row " + std::to_string(slot) + " is not live"); return RMU_ERR_ARG; }
+    release_row(S, slot);
+    return RMU_OK;
+}
+
+int rmu_decoder_session_info(rmu_gen_session* S, int32_t* live, int32_t* cap_positions, uint32_t* live_mask) {
+    if (!S || !live || !cap_positions) { set_error("rmu_decoder_session_info: bad argument"); return RMU_ERR_ARG; }
+    std::lock_guard<std::mutex> g(S->e->mu);
+    int n = 0;
+    uint32_t mask = 0;
+    for (int i = 0; i < RMU_MAX_GENERATE_BATCH; ++i) {
+        n += S->rows[i].live ? 1 : 0;
+        mask |= S->rows[i].live ? 1u << i : 0u;
+    }
+    *live = n;
+    *cap_positions = S->reg.cap;
+    if (live_mask) *live_mask = mask;
+    return RMU_OK;
+}
+
+int rmu_debug_kv_regions(const int32_t* ops, int n, int32_t* out) {
+    if (!ops || !out || n < 0) { set_error("rmu_debug_kv_regions: bad argument"); return RMU_ERR_ARG; }
+    KvRegions reg;
+    for (int i = 0; i < n; ++i) {
+        if (ops[i] > 0) {
+            out[2 * i] = reg.place(ops[i]);
+        } else {
+            out[2 * i] = reg.used.erase(-ops[i]) ? 0 : -1;
+        }
+        out[2 * i + 1] = reg.cap;
+    }
     return RMU_OK;
 }
 
@@ -4941,6 +5506,41 @@ int rmu_debug_sample_verify_rows(float* logits, int V, int M, uint32_t* presence
     rc = launch_presence_rows(presence, sr.words, ids, M, rows, st);
     if (rc != RMU_OK) return rc;
     return launch_sample(logits, V, rows, sa, -1.f, seed, static_cast<unsigned long long>(step0), token, st, M, sr);
+}
+
+int rmu_debug_sample_session_rows(float* logits, int V, int B, uint32_t* presence, const int32_t* seq,
+                                  const uint64_t* seeds, const uint64_t* steps, int n_seq, const rmu_sampling* s_h,
+                                  int32_t* token, void* stream) {
+    const std::string fn("rmu_debug_sample_session_rows");
+    if (!logits || V < 1 || B < 1 || !presence || !seq || !seeds || !steps || n_seq < 1 ||
+        n_seq > RMU_MAX_GENERATE_BATCH || !s_h || !token) {
+        set_error(fn + ": bad argument");
+        return RMU_ERR_ARG;
+    }
+    SampleArgs sa[RMU_MAX_GENERATE_BATCH];
+    for (int q = 0; q < n_seq; ++q) {
+        const int rc = check_sampling(fn, s_h + q);
+        if (rc != RMU_OK) return rc;
+        sa[q] = SampleArgs{s_h[q].do_sample ? 1 : 0, s_h[q].top_k, s_h[q].temperature, s_h[q].top_p, s_h[q].repetition_penalty};
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SampleArgs* d_args = nullptr;
+    RMU_CUDA(cudaMalloc(&d_args, sizeof(sa)));
+    int rc = RMU_OK;
+    if (cudaMemcpyAsync(d_args, sa, sizeof(sa), cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        set_error(fn + ": cannot upload the settings");
+        rc = RMU_ERR_CUDA;
+    }
+    SampleRows sr;
+    sr.seq = seq;
+    sr.seeds = reinterpret_cast<const unsigned long long*>(seeds);
+    sr.words = (static_cast<size_t>(V) + 31) / 32;
+    sr.args = d_args;
+    sr.steps = reinterpret_cast<const unsigned long long*>(steps);
+    if (rc == RMU_OK) rc = launch_sample(logits, V, presence, SampleArgs{}, -1.f, 0ull, 0ull, token, st, B, sr);
+    if (cudaStreamSynchronize(st) != cudaSuccess && rc == RMU_OK) { set_error(fn + ": stream failed"); rc = RMU_ERR_CUDA; }
+    cudaFree(d_args);
+    return rc;
 }
 
 }  // extern "C"

@@ -22,6 +22,7 @@ from __future__ import annotations
 import copy
 import os
 import threading
+from concurrent.futures import ThreadPoolExecutor
 from typing import Any, List, Optional
 
 from . import provenance
@@ -108,9 +109,11 @@ class _PipelineGenerator:
     def _decoder(self):
         return provenance._decoder(self._pipe.model)
 
-    def _call(self, prompt: str) -> str:
+    def _call(self, prompt: str, seed: Optional[int] = None) -> str:
         import torch
         pipe = self._pipe
+        # the lock covers the pipeline's own tokenizer and post-processing; generation runs outside it, so calls from
+        # several threads share the decoder's session and their replies progress together
         with self._lock:
             inputs = pipe.preprocess(prompt, **pipe._preprocess_params)
             ids = inputs["input_ids"]
@@ -122,13 +125,34 @@ class _PipelineGenerator:
             settings = resolve_settings(gen_cfg, fwd, ids.shape[1])
             if "prompt_lookup_num_tokens" not in settings and prompt_lookup_tokens():
                 settings.update(prompt_lookup_num_tokens=prompt_lookup_tokens(), max_matching_ngram_size=2)
-            seed = int(torch.randint(0, 2 ** 63 - 1, (1,)).item())
-            new = self._decoder().generate(ids[0].tolist(), seed=seed, **settings)
+            if seed is None:
+                seed = int(torch.randint(0, 2 ** 63 - 1, (1,)).item())
+        new = self._decoder().generate(ids[0].tolist(), seed=seed, **settings)
+        with self._lock:
             seq = torch.cat([ids[0].cpu(), torch.as_tensor(new, dtype=ids.dtype)])
             model_outputs = {"generated_sequence": seq.view(1, 1, -1), "input_ids": ids,
                              "prompt_text": inputs.get("prompt_text", prompt)}
             out = pipe.postprocess(model_outputs, **pipe._postprocess_params)
         return out[0]["generated_text"] if isinstance(out[0], dict) else out[0][0]["generated_text"]
+
+    def _call_all(self, prompts: List[str]) -> List[str]:
+        """``_call`` on every prompt, all of them generating at once (one thread each), in prompt order; the seeds are
+        drawn in prompt order first, so torch.manual_seed repeats a batch as it repeats a call, and the workers run on
+        the caller's current CUDA device, which picks the decoder as a call on the caller's thread would"""
+        import torch
+        if len(prompts) <= 1:
+            return [self._call(p) for p in prompts]
+        seeds = [int(torch.randint(0, 2 ** 63 - 1, (1,)).item()) for _ in prompts]
+        device = torch.cuda.current_device() if torch.cuda.is_available() else None
+
+        def call(prompt, seed):
+            if device is None:
+                return self._call(prompt, seed)
+            with torch.cuda.device(device):
+                return self._call(prompt, seed)
+
+        with ThreadPoolExecutor(max_workers=min(len(prompts), 64)) as pool:
+            return list(pool.map(call, prompts, seeds))
 
 
 try:
@@ -151,7 +175,7 @@ try:
                       **kwargs: Any) -> LLMResult:
             if stop is not None:
                 raise ValueError("stop sequences are not supported by the GPU decoder")
-            return LLMResult(generations=[[Generation(text=self._call(p))] for p in prompts])
+            return LLMResult(generations=[[Generation(text=t)] for t in self._call_all(list(prompts))])
 
 except ImportError:
     class HuggingFacePipeline(_PipelineGenerator):
@@ -168,4 +192,6 @@ except ImportError:
             return self._call(prompt.to_string() if hasattr(prompt, "to_string") else str(prompt))
 
         def batch(self, prompts: List[Any], **kwargs: Any) -> List[str]:
-            return [self.invoke(p, **kwargs) for p in prompts]
+            if kwargs.get("stop") is not None:
+                raise ValueError("stop sequences are not supported by the GPU decoder")
+            return self._call_all([p.to_string() if hasattr(p, "to_string") else str(p) for p in prompts])

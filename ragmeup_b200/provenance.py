@@ -28,7 +28,7 @@ from typing import Any, List, Optional, Sequence
 
 import numpy as np
 
-from . import _lib
+from . import _lib, decode_session
 from .index import FlatIndex
 from .weights import decoder_lm_head, find_snapshot, resolve_decoder
 
@@ -103,6 +103,7 @@ class DecoderAttention:
                 enc._check(_lib.lib().rmu_decoder_quantize_nf4(enc._h, _lib.stream_ptr()), "rmu_decoder_quantize_nf4")
         self.lock = threading.Lock()
         self._lm_head = False
+        self._scheduler = None
 
     @property
     def name(self) -> str:
@@ -131,10 +132,12 @@ class DecoderAttention:
     def generate(self, ids: Sequence[int], max_new_tokens: int, do_sample: bool = False, temperature: float = 1.0,
                  top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.0, eos_token_ids=(),
                  seed: int = 0, prompt_lookup_num_tokens: int = 0, max_matching_ngram_size: int = 2) -> List[int]:
-        """the new token ids after the prompt ``ids`` (``rmu_decoder_generate``), the eos token included when one
-        ends the run.  ``prompt_lookup_num_tokens`` > 0 drafts that many tokens (at most 15) per pass from earlier
-        matches of the last ``max_matching_ngram_size``-gram (``rmu_decoder_generate_lookup``): the same tokens,
-        bit for bit, in fewer model passes when the reply copies the prompt."""
+        """the new token ids after the prompt ``ids`` (``rmu_decoder_generate``'s tokens), the eos token included when
+        one ends the run.  Concurrent calls share the handle's decode session (``decode_session``): a call joins it at
+        the next step boundary, so a second caller's reply starts before the first one's ends, and each reply is bit for
+        bit its solo run.  ``prompt_lookup_num_tokens`` > 0 drafts that many tokens (at most 15) per pass from earlier
+        matches of the last ``max_matching_ngram_size``-gram (``rmu_decoder_generate_lookup``, one whole call): the
+        same tokens, bit for bit, in fewer model passes when the reply copies the prompt."""
         if max_new_tokens < 1:
             return []
         eos = [int(t) for t in eos_token_ids]
@@ -142,26 +145,43 @@ class DecoderAttention:
             raise ValueError(f"{self.name}: at most {_lib.MAX_EOS} eos ids, got {len(eos)}")
         s = _lib.SamplingC(int(bool(do_sample)), float(temperature), float(top_p), float(repetition_penalty),
                            int(top_k or 0), len(eos), (C.c_int32 * _lib.MAX_EOS)(*eos))
+        enc = self.encoder
+        if not prompt_lookup_num_tokens:
+            req = decode_session.Request(ids, s, seed, max_new_tokens, name=self.name)
+            with enc.torch.cuda.device(enc.device):
+                try:
+                    return list(self.scheduler().run(req))
+                except decode_session.SessionBusy as e:
+                    raise _lib.RmuError(f"rmu_decoder_generate failed: {e}") from e
         prompt = np.ascontiguousarray(list(ids), dtype=np.int32)
         out = np.zeros(int(max_new_tokens), dtype=np.int32)
         n = C.c_int32(0)
-        enc = self.encoder
         with self.lock, enc.torch.cuda.device(enc.device):
-            if not self._lm_head:
-                W = decoder_lm_head(self.model_name, self.cfg)
-                enc._check(_lib.lib().rmu_decoder_set_lm_head(enc._h, W.ctypes.data), "rmu_decoder_set_lm_head")
-                self._lm_head = True
-            if prompt_lookup_num_tokens:
-                enc._check(_lib.lib().rmu_decoder_generate_lookup(
-                    enc._h, prompt.ctypes.data, len(prompt), C.byref(s), int(seed) & (2 ** 64 - 1), int(max_new_tokens),
-                    int(prompt_lookup_num_tokens), int(max_matching_ngram_size), out.ctypes.data, C.byref(n), None, None,
-                    _lib.stream_ptr()), "rmu_decoder_generate_lookup")
-            else:
-                enc._check(_lib.lib().rmu_decoder_generate(enc._h, prompt.ctypes.data, len(prompt), C.byref(s),
-                                                           int(seed) & (2 ** 64 - 1), int(max_new_tokens),
-                                                           out.ctypes.data, C.byref(n), None, _lib.stream_ptr()),
-                           "rmu_decoder_generate")
+            self._attach_lm_head()
+            enc._check(_lib.lib().rmu_decoder_generate_lookup(
+                enc._h, prompt.ctypes.data, len(prompt), C.byref(s), int(seed) & (2 ** 64 - 1), int(max_new_tokens),
+                int(prompt_lookup_num_tokens), int(max_matching_ngram_size), out.ctypes.data, C.byref(n), None, None,
+                _lib.stream_ptr()), "rmu_decoder_generate_lookup")
         return out[:n.value].tolist()
+
+    def _attach_lm_head(self) -> None:
+        """``rmu_decoder_set_lm_head`` the first time it is needed (under ``self.lock``)"""
+        if not self._lm_head:
+            enc = self.encoder
+            W = decoder_lm_head(self.model_name, self.cfg)
+            enc._check(_lib.lib().rmu_decoder_set_lm_head(enc._h, W.ctypes.data), "rmu_decoder_set_lm_head")
+            self._lm_head = True
+
+    def scheduler(self) -> "decode_session.Scheduler":
+        """the handle's decode session and its caller-driven scheduler, made (with the LM head) on first use"""
+        if self._scheduler is not None:
+            return self._scheduler
+        with self.lock:
+            if self._scheduler is None:
+                with self.encoder.torch.cuda.device(self.encoder.device):
+                    self._attach_lm_head()
+                    self._scheduler = decode_session.Scheduler(decode_session.DecodeSession(self.encoder))
+            return self._scheduler
 
     def generate_batch(self, prompts: Sequence[Sequence[int]], max_new_tokens: int, seeds: Sequence[int],
                        do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0,
@@ -181,10 +201,7 @@ class DecoderAttention:
         enc = self.encoder
         result: List[List[int]] = []
         with self.lock, enc.torch.cuda.device(enc.device):
-            if not self._lm_head:
-                W = decoder_lm_head(self.model_name, self.cfg)
-                enc._check(_lib.lib().rmu_decoder_set_lm_head(enc._h, W.ctypes.data), "rmu_decoder_set_lm_head")
-                self._lm_head = True
+            self._attach_lm_head()
             for b0 in range(0, len(prompts), _lib.MAX_GENERATE_BATCH):
                 part = [list(p) for p in prompts[b0:b0 + _lib.MAX_GENERATE_BATCH]]
                 B = len(part)
@@ -214,8 +231,10 @@ def decoder_weights() -> str:
     return v
 
 
-# one decoder per (snapshot, device, weights): compute_attention and llms.HuggingFacePipeline share its weights
+# one decoder per (snapshot, device, weights): compute_attention and llms.HuggingFacePipeline share its weights.  The
+# lock makes the first lookup build it once when several threads ask at the same time (each build uploads the model).
 _DECODERS: dict = {}
+_DECODERS_LOCK = threading.Lock()
 
 
 def _decoder(model: Any) -> DecoderAttention:
@@ -232,9 +251,10 @@ def _decoder(model: Any) -> DecoderAttention:
     torch = _lib.require_cuda()
     key = (name if name.startswith("synthetic:") else os.path.realpath(find_snapshot(name)), torch.cuda.current_device(),
            weights)
-    if key not in _DECODERS:
-        _DECODERS[key] = DecoderAttention(name, device=key[1], weights=weights)
-    return _DECODERS[key]
+    with _DECODERS_LOCK:
+        if key not in _DECODERS:
+            _DECODERS[key] = DecoderAttention(name, device=key[1], weights=weights)
+        return _DECODERS[key]
 
 
 def _find_part(thread: List[int], part: List[int]):
