@@ -364,6 +364,25 @@ int rmu_decoder_set_lm_head(rmu_encoder* enc, const float* W_h);
  * (RMU_ERR_ARG); a projection whose K is not a multiple of 64 or exceeds 49 152 (RMU_ERR_UNSUPPORTED).  A failure
  * part-way leaves a handle that every call refuses; destroy it.  Synchronises the device. */
 int rmu_decoder_quantize_nf4(rmu_encoder* enc, void* stream);
+/* An NF4 decoder built one layer at a time, so that no layer's weights ever exist on the device in any other form
+ * than their codes: Llama (qk_norm 0) or Qwen3 (qk_norm 1), hidden a multiple of 128 up to 8192 (split-plane handles
+ * stop at 4096).  rmu_decoder_create_nf4 uploads embed_tokens [vocab_size, hidden], the final norm [hidden] and the
+ * rope tables [max_pos, 64] (host fp32), and allocates the prefill's scratch plane pair, the size of the largest
+ * projection; the handle has no layers yet.  rmu_decoder_load_layer_nf4 takes layer `layer`'s 9 (Llama) or 11 (Qwen3)
+ * host fp32 tensors in rmu_encoder_create_llama's / _qwen3's per-layer order; layers load in order 0, 1, ...  Each
+ * projection goes up in chunks of 16 Mi fp32 values (96 MiB of staging with the discarded lo plane, freed when the
+ * call returns), becomes its fp16 hi plane in the scratch and is quantised from there: the codes and absmax are bit
+ * for bit those of rmu_encoder_create_llama / _qwen3 + rmu_decoder_quantize_nf4 on the same weights, and the device
+ * never holds more than the finished handle plus one staging chunk.  Every forward, span, generate and session entry
+ * refuses a handle whose layers are not all loaded (RMU_ERR_ARG, naming the missing layer).  Refused before any CUDA
+ * call: create_llama's shape refusals with the wider hidden limit, and a projection K not a multiple of 64 or above
+ * 49 152 (RMU_ERR_UNSUPPORTED); a layer outside [0, layers) or out of order, a null tensor, a handle not from
+ * rmu_decoder_create_nf4 (RMU_ERR_ARG); |w| >= 65520 in a projection (RMU_ERR_UNSUPPORTED, naming the layer and the projection).  A failed
+ * load leaves the layer unloaded; the same layer may be loaded again.  load synchronises `stream`. */
+int rmu_decoder_create_nf4(const rmu_bert_config* cfg, const rmu_qwen3_ext* ext, int qk_norm, const float* embed_h,
+                           const float* final_norm_h, const float* rope_cos_h, const float* rope_sin_h,
+                           rmu_encoder** out);
+int rmu_decoder_load_layer_nf4(rmu_encoder* enc, int layer, const float* const* tensors_h, void* stream);
 /* Token selection, in transformers' order: the repetition penalty (x < 0 ? x * p : x / p) on every id of the prompt and
  * of the generated tokens; then with do_sample 0 the largest logit (the lowest id among equal ones); with do_sample 1
  * x / temperature, top-k (every logit >= the k-th largest survives; 1 <= top_k <= 256, and when more than 256 logits
@@ -610,7 +629,8 @@ int rmu_debug_gemm_swiglu(const uint16_t* a_hi, const uint16_t* a_lo, int64_t a_
                           const uint16_t* w_lo, int M, int N, int K, const float* bias, int max_ctas, uint16_t* out_hi,
                           uint16_t* out_lo, int32_t* range_flag, void* stream);
 /* For tests: Qwen3's RMSNorm of T fp32 rows [T, H] (device) -> split planes [T, H] = split(w * (x * rsqrt(mean(x^2) +
- * eps))).  H a multiple of 128 up to 4096.  range_flag (device, may be NULL) as rmu_debug_gemm_swiglu's. */
+ * eps))).  H a multiple of 128 up to 8192 (256 threads per row above 4096).  range_flag (device, may be NULL) as
+ * rmu_debug_gemm_swiglu's. */
 int rmu_debug_rmsnorm(const float* x, int T, int H, const float* w, float eps, uint16_t* hi, uint16_t* lo,
                       int32_t* range_flag, void* stream);
 /* For tests: Qwen3's q / k step on the fp32 QKV rows [T, (heads + 2 kv_heads) 128] (q | k | v, heads of 128): per

@@ -134,6 +134,9 @@ SIGNATURES = {
                                               C.c_void_p]),
     "rmu_decoder_set_lm_head": (C.c_int, [C.c_void_p, C.c_void_p]),
     "rmu_decoder_quantize_nf4": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "rmu_decoder_create_nf4": (C.c_int, [C.POINTER(BertConfigC), C.POINTER(Qwen3ExtC), C.c_int, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "rmu_decoder_load_layer_nf4": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.c_void_p]),
     "rmu_decoder_generate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(SamplingC), C.c_uint64, C.c_int,
                                        C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]),
     "rmu_decoder_generate_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(SamplingC),

@@ -16,6 +16,7 @@
 #include <climits>
 #include <cmath>
 #include <cstdlib>
+#include <cstring>
 #include <functional>
 #include <map>
 #include <mutex>
@@ -1174,33 +1175,47 @@ static int launch_colbert_maxsim(const float* q, const int* q_cu, const float* d
 // range or a NaN, and the forward reports it instead of returning what the overflow made of the output.
 constexpr int kQwenHD = 128;                  // head_dim (the only one the kernels take)
 constexpr int kRmsThreads = 128;              // rms_split_kernel: thread i holds columns i, i + 128, ... (H <= 4096)
+constexpr int kRmsWideThreads = 256;          // its wide form: columns i, i + 256, ... (4096 < H <= 8192)
 constexpr int kRmsMaxPerThread = 32;
+constexpr int kRmsMaxHidden = kRmsWideThreads * kRmsMaxPerThread;
 
 __device__ __forceinline__ bool outside_f16(float v) { return !(fabsf(v) <= 65504.0f); }
 
+// the pairwise sum of r[0 .. N): ((r0 + r1) + (r2 + r3)) + ... in a fixed order
+template <int N>
+__device__ __forceinline__ float pair_tree(const float* r) {
+    if constexpr (N == 1) return r[0];
+    else return pair_tree<N / 2>(r) + pair_tree<N / 2>(r + N / 2);
+}
+
 // Qwen3RMSNorm of one fp32 row per block -> split planes: y = w * (x * (1 / sqrt(mean(x^2) + eps))), all fp32.  The sum
-// of squares is per thread in column order, then the warps' shuffle trees, then the four warp sums in a fixed order.
-__global__ void __launch_bounds__(kRmsThreads) rms_split_kernel(const float* __restrict__ x, int H, const float* __restrict__ w,
-                                                               float eps, __half* __restrict__ hi, __half* __restrict__ lo,
-                                                               int* __restrict__ flag) {
-    __shared__ float red[kRmsThreads / 32];
+// of squares is per thread in column order, then the warps' shuffle trees, then the warp sums' pairwise tree (four
+// warps: (r0 + r1) + (r2 + r3)).  kThreads 128 for H <= 4096; 256 for wider rows, where column c < H is guarded so
+// that any multiple of 128 up to 8192 fits.
+template <int kThreads>
+__global__ void __launch_bounds__(kThreads) rms_split_kernel(const float* __restrict__ x, int H, const float* __restrict__ w,
+                                                             float eps, __half* __restrict__ hi, __half* __restrict__ lo,
+                                                             int* __restrict__ flag) {
+    __shared__ float red[kThreads / 32];
     const size_t row = blockIdx.x;
     const float* xr = x + row * H;
-    const int n = H / kRmsThreads;
     float v[kRmsMaxPerThread];
     float ss = 0.f;
 #pragma unroll
     for (int i = 0; i < kRmsMaxPerThread; ++i)
-        if (i < n) { v[i] = xr[i * kRmsThreads + threadIdx.x]; ss = fmaf(v[i], v[i], ss); }
+        if (i * kThreads + static_cast<int>(threadIdx.x) < H) {
+            v[i] = xr[i * kThreads + threadIdx.x];
+            ss = fmaf(v[i], v[i], ss);
+        }
     for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
     __syncthreads();
-    const float rs = 1.0f / sqrtf(((red[0] + red[1]) + (red[2] + red[3])) / static_cast<float>(H) + eps);
+    const float rs = 1.0f / sqrtf(pair_tree<kThreads / 32>(red) / static_cast<float>(H) + eps);
     bool bad = false;
 #pragma unroll
     for (int i = 0; i < kRmsMaxPerThread; ++i) {
-        if (i < n) {
-            const int c = i * kRmsThreads + threadIdx.x;
+        const int c = i * kThreads + threadIdx.x;
+        if (c < H) {
             const float y = w[c] * (v[i] * rs);
             __half h, l;
             split_f16(y, h, l);
@@ -1645,12 +1660,15 @@ static CausalGrid causal_grid(int heads, int kv_heads, int T) {
     return {hpc, static_cast<unsigned>(kv_heads * (G / hpc)), static_cast<unsigned>((T + rows - 1) / rows)};
 }
 
-// E3 rms_split_kernel over T rows of H (H % 128 == 0, H <= 4096)
+// E3 rms_split_kernel over T rows of H (H % 128 == 0, H <= 8192): the 128-thread form up to 4096, the wide one above
 static int launch_rms_split(const float* x, int T, int H, const float* w, float eps, __half* hi, __half* lo, int* flag,
                             cudaStream_t st) {
     if (T <= 0) return RMU_OK;
     ProfScope _ps(PROF_LN, st);
-    rms_split_kernel<<<static_cast<unsigned>(T), kRmsThreads, 0, st>>>(x, H, w, eps, hi, lo, flag);
+    if (H <= kRmsThreads * kRmsMaxPerThread)
+        rms_split_kernel<kRmsThreads><<<static_cast<unsigned>(T), kRmsThreads, 0, st>>>(x, H, w, eps, hi, lo, flag);
+    else
+        rms_split_kernel<kRmsWideThreads><<<static_cast<unsigned>(T), kRmsWideThreads, 0, st>>>(x, H, w, eps, hi, lo, flag);
     count_launch();
     RMU_CHECK_LAUNCH();
     return RMU_OK;
@@ -2434,6 +2452,10 @@ struct rmu_encoder {
     // conversion's allocations exceeded, and finally differ from, the bytes the handle held before it.
     bool nf4 = false, nf4_broken = false;
     __half *nf4_hi = nullptr, *nf4_lo = nullptr;
+    // built layer by layer (rmu_decoder_create_nf4): layers 0 .. layers_loaded - 1 hold their weights, and the handle
+    // runs nothing until every layer does
+    bool by_layer = false;
+    int layers_loaded = 0;
     SplitOperand nf4_op[4];
     int64_t nf4_peak = 0, nf4_delta = 0;
     // sentence-transformers Dense modules after pooling (rmu_encoder_set_dense): dense_dims [n + 1], per layer W [out, in],
@@ -2875,8 +2897,14 @@ static int check_decoder(const rmu_encoder* e, const std::string& fn) {
     return RMU_ERR_ARG;
 }
 
-// a handle whose NF4 conversion failed part-way runs nothing
+// a handle whose NF4 conversion failed part-way, or one built layer by layer whose layers are not all loaded, runs
+// nothing
 static int check_nf4_intact(const rmu_encoder* e, const std::string& fn) {
+    if (e->by_layer && e->layers_loaded < e->cfg.layers) {
+        set_error(fn + ": layer " + std::to_string(e->layers_loaded) + " of " + std::to_string(e->cfg.layers) +
+                  " is not loaded (rmu_decoder_load_layer_nf4)");
+        return RMU_ERR_ARG;
+    }
     if (!e->nf4_broken) return RMU_OK;
     set_error(fn + ": the handle's NF4 conversion failed part-way (rmu_decoder_quantize_nf4); destroy it");
     return RMU_ERR_ARG;
@@ -3514,12 +3542,10 @@ int rmu_encoder_create_modernbert(const rmu_bert_config* cfg, const rmu_modernbe
 
 }  // extern "C"
 
-// rmu_encoder_create_qwen3 (qk_norm) and rmu_encoder_create_llama (no q_norm / k_norm tensors: 9 per layer, no head);
-// `who` prefixes the errors
-static int create_decoder(const char* who, bool qk_norm, const rmu_bert_config* cfg, const rmu_qwen3_ext* qx,
-                          const float* const* w, int n_weights, int has_head, rmu_encoder** out) {
-    const std::string fn(who);
-    if (!cfg || !qx || !w || !out) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
+// the shape refusals of a decoder handle, before any CUDA call: hidden a multiple of 128 up to max_hidden (4096 on
+// split planes, 8192 in NF4), head_dim 128, intermediate a multiple of 64, grouped kv heads, rope tables [max_pos, 64]
+static int check_decoder_shape(const std::string& fn, const rmu_bert_config* cfg, const rmu_qwen3_ext* qx, int has_head,
+                               int max_hidden) {
     const int H = cfg->hidden, F = cfg->ffn, L = cfg->layers, nh = cfg->heads, kv = qx->kv_heads;
     if (cfg->position_mode != RMU_POS_ABSOLUTE || cfg->rel_buckets != 0 || cfg->adapter_dim != 0) {
         set_error(fn + ": position_mode, rel_buckets and adapter_dim must be 0 (rotary positions, no "
@@ -3530,8 +3556,9 @@ static int create_decoder(const char* who, bool qk_norm, const rmu_bert_config* 
         set_error(fn + ": head_dim must be 128, got " + std::to_string(qx->head_dim));
         return RMU_ERR_UNSUPPORTED;
     }
-    if (H <= 0 || H % 128 != 0 || H > 4096) {
-        set_error(fn + ": hidden_size must be a multiple of 128 up to 4096, got " + std::to_string(H));
+    if (H <= 0 || H % 128 != 0 || H > max_hidden) {
+        set_error(fn + ": hidden_size must be a multiple of 128 up to " + std::to_string(max_hidden) + ", got " +
+                  std::to_string(H));
         return RMU_ERR_UNSUPPORTED;
     }
     if (F <= 0 || F % 64 != 0) {
@@ -3555,6 +3582,18 @@ static int create_decoder(const char* who, bool qk_norm, const rmu_bert_config* 
         set_error(fn + ": head_form must be RMU_QWEN3_HEAD_LAST with a head, RMU_QWEN3_HEAD_NONE without");
         return RMU_ERR_ARG;
     }
+    return RMU_OK;
+}
+
+// rmu_encoder_create_qwen3 (qk_norm) and rmu_encoder_create_llama (no q_norm / k_norm tensors: 9 per layer, no head);
+// `who` prefixes the errors
+static int create_decoder(const char* who, bool qk_norm, const rmu_bert_config* cfg, const rmu_qwen3_ext* qx,
+                          const float* const* w, int n_weights, int has_head, rmu_encoder** out) {
+    const std::string fn(who);
+    if (!cfg || !qx || !w || !out) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
+    const int H = cfg->hidden, F = cfg->ffn, L = cfg->layers, nh = cfg->heads, kv = qx->kv_heads;
+    const int shape_rc = check_decoder_shape(fn, cfg, qx, has_head, 4096);
+    if (shape_rc != RMU_OK) return shape_rc;
     const int QD = nh * kQwenHD, KD = kv * kQwenHD, NQKV = QD + 2 * KD;
     const int per = qk_norm ? 11 : 9;                // tensors per layer
     const int norm0 = 1 + per * L, rope0 = norm0 + 1 + (has_head ? 1 : 0), expect = rope0 + 2;
@@ -3962,6 +4001,186 @@ int rmu_decoder_quantize_nf4(rmu_encoder* e, void* stream) {
     e->nf4_broken = false;
     e->nf4_peak = peak;
     e->nf4_delta = delta;
+    return RMU_OK;
+}
+
+// the [rows, cols] shapes of a decoder layer's four projections (q | k | v, o, gate | up, down) in the handle's row order
+static void decoder_shapes(const rmu_encoder* e, int64_t shape[4][2]) {
+    const int64_t H = e->cfg.hidden, F = e->cfg.ffn, QD = static_cast<int64_t>(e->cfg.heads) * kQwenHD;
+    const int64_t s[4][2] = {{e->qkv_w, H}, {H, QD}, {2 * F, H}, {H, F}};
+    std::memcpy(shape, s, sizeof(s));
+}
+
+int rmu_decoder_create_nf4(const rmu_bert_config* cfg, const rmu_qwen3_ext* qx, int qk_norm, const float* embed_h,
+                           const float* final_norm_h, const float* rope_cos_h, const float* rope_sin_h,
+                           rmu_encoder** out) {
+    const std::string fn("rmu_decoder_create_nf4");
+    if (!cfg || !qx || !embed_h || !final_norm_h || !rope_cos_h || !rope_sin_h || !out || (qk_norm != 0 && qk_norm != 1)) {
+        set_error(fn + ": bad argument");
+        return RMU_ERR_ARG;
+    }
+    int rc = check_decoder_shape(fn, cfg, qx, 0, kRmsMaxHidden);
+    if (rc != RMU_OK) return rc;
+    const int H = cfg->hidden, F = cfg->ffn, QD = cfg->heads * kQwenHD, NQKV = QD + 2 * qx->kv_heads * kQwenHD;
+    const int64_t K[4] = {H, QD, H, F};
+    for (int64_t k : K) {
+        if (k % kNf4Block != 0 || k > kNf4MaxK) {
+            set_error(fn + ": every projection's K must be a multiple of 64 up to " + std::to_string(kNf4MaxK) + ", got " +
+                      std::to_string(k));
+            return RMU_ERR_UNSUPPORTED;
+        }
+    }
+    rmu_encoder* e = new_handle(fn, *cfg, 0);
+    if (!e) return RMU_ERR_CUDA;
+    e->qwen = true;
+    e->llama = !qk_norm;
+    e->qext = *qx;
+    e->qkv_w = NQKV;
+    e->ctx_w = QD;
+    e->has_qkvf = e->has_posi = true;
+    e->nf4 = e->by_layer = true;
+    e->layers.resize(cfg->layers);
+    const size_t tab = static_cast<size_t>(cfg->max_pos) * (kQwenHD / 2);
+    rc = upload(e, &e->word, embed_h, static_cast<size_t>(cfg->vocab_size) * H);
+    if (rc == RMU_OK) rc = upload(e, &e->fng, final_norm_h, H);
+    if (rc == RMU_OK) rc = upload(e, &e->rope_cos[0], rope_cos_h, tab);
+    if (rc == RMU_OK) rc = upload(e, &e->rope_sin[0], rope_sin_h, tab);
+    if (rc == RMU_OK) {
+        const std::vector<float> zeros(static_cast<size_t>(std::max({NQKV, 2 * F, H})), 0.f);
+        rc = upload(e, &e->zeros, zeros.data(), zeros.size());
+    }
+    if (rc == RMU_OK) rc = dev_alloc(e->allocs, &e->range_flag, 1);
+    if (rc == RMU_OK) rc = dev_alloc(e->allocs, &e->span_cu, 2);
+    // the prefill's scratch hi | lo pair (lo all zero), the size of the largest projection; each layer's load also
+    // builds its projections' hi planes in it
+    int64_t shape[4][2];
+    decoder_shapes(e, shape);
+    int64_t most = 0;
+    for (const auto& sh : shape) most = std::max(most, sh[0] * sh[1]);
+    if (rc == RMU_OK) rc = dev_alloc(e->allocs, &e->nf4_hi, most);
+    if (rc == RMU_OK) rc = dev_alloc(e->allocs, &e->nf4_lo, most);
+    if (rc == RMU_OK && cudaMemset(e->nf4_lo, 0, most * sizeof(__half)) != cudaSuccess) {
+        set_error(fn + ": " + cudaGetErrorString(cudaGetLastError()));
+        rc = RMU_ERR_CUDA;
+    }
+    for (int w = 0; w < 4 && rc == RMU_OK; ++w)
+        rc = make_split_operand(&e->nf4_op[w], e->nf4_hi, e->nf4_lo, shape[w][0], static_cast<int>(shape[w][1]));
+    if (rc != RMU_OK) { rmu_encoder_destroy(e); return rc; }
+    *out = e;
+    return RMU_OK;
+}
+
+// fp32 elements of one staging chunk of rmu_decoder_load_layer_nf4 (64 MiB, plus 32 MiB for the lo plane the split
+// kernel also writes, which the quantiser never reads)
+constexpr size_t kNf4LoadChunk = size_t(1) << 24;
+
+int rmu_decoder_load_layer_nf4(rmu_encoder* e, int layer, const float* const* w, void* stream) {
+    const std::string fn("rmu_decoder_load_layer_nf4");
+    if (!e || !w) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
+    int rc = check_decoder(e, fn);
+    if (rc != RMU_OK) return rc;
+    if (!e->by_layer) { set_error(fn + ": the handle must come from rmu_decoder_create_nf4"); return RMU_ERR_ARG; }
+    const rmu_bert_config& c = e->cfg;
+    if (layer < 0 || layer >= c.layers) {
+        set_error(fn + ": layer " + std::to_string(layer) + " is outside the model's " + std::to_string(c.layers) +
+                  " layers");
+        return RMU_ERR_ARG;
+    }
+    const bool qk = !e->llama;
+    const int per = qk ? 11 : 9;
+    for (int j = 0; j < per; ++j)
+        if (!w[j]) { set_error(fn + ": layer " + std::to_string(layer) + ": null weight tensor " + std::to_string(j)); return RMU_ERR_ARG; }
+    std::lock_guard<std::mutex> hg(e->host_mu);
+    std::lock_guard<std::mutex> g(e->mu);
+    if (layer != e->layers_loaded) {
+        set_error(fn + ": layers load in order: expected layer " + std::to_string(e->layers_loaded) + " of " +
+                  std::to_string(c.layers) + ", got " + std::to_string(layer));
+        return RMU_ERR_ARG;
+    }
+    const int H = c.hidden, F = c.ffn, QD = c.heads * kQwenHD, KD = e->qext.kv_heads * kQwenHD;
+    static const char* const kName[] = {"q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj"};
+    const int slot11[] = {1, 2, 3, 6, 8, 9, 10}, slot9[] = {1, 2, 3, 4, 6, 7, 8};
+    const int* slot = qk ? slot11 : slot9;
+    const size_t count[] = {size_t(QD) * H, size_t(KD) * H, size_t(KD) * H, size_t(H) * QD, size_t(F) * H,
+                            size_t(F) * H, size_t(H) * F};
+    for (int k = 0; k < 7; ++k) {
+        rc = check_split_range(fn, "layer " + std::to_string(layer) + " " + kName[k], w[slot[k]], count[k]);
+        if (rc != RMU_OK) return rc;
+    }
+    const float *q = w[slot[0]], *kw = w[slot[1]], *v = w[slot[2]], *o = w[slot[3]];
+    const float *gate = w[slot[4]], *up = w[slot[5]], *down = w[slot[6]];
+    // each projection as runs of consecutive source elements in the handle's row order: q | k | v; o; gate | up in
+    // 128-row blocks of 64 gate rows and the 64 matching up rows (geglu_rows); down
+    std::vector<std::pair<const float*, size_t>> runs[4];
+    runs[0] = {{q, count[0]}, {kw, count[1]}, {v, count[2]}};
+    runs[1] = {{o, count[3]}};
+    for (int b = 0; b < F / 64; ++b) {
+        runs[2].push_back({gate + size_t(64) * b * H, size_t(64) * H});
+        runs[2].push_back({up + size_t(64) * b * H, size_t(64) * H});
+    }
+    runs[3] = {{down, count[6]}};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    EncLayer& Ly = e->layers[layer];
+    // a retry after a failed load reuses what the failed attempt allocated
+    auto vec = [&](float** dst, const float* src, size_t n) -> int {
+        if (!*dst) {
+            const int r = dev_alloc(e->allocs, dst, n);
+            if (r != RMU_OK) return r;
+        }
+        RMU_CUDA(cudaMemcpy(*dst, src, n * sizeof(float), cudaMemcpyHostToDevice));
+        return RMU_OK;
+    };
+    rc = vec(&Ly.ln1g, w[0], H);
+    if (rc == RMU_OK) rc = vec(&Ly.ln2g, w[qk ? 7 : 5], H);
+    if (rc == RMU_OK && qk) rc = vec(&Ly.qn, w[4], kQwenHD);
+    if (rc == RMU_OK && qk) rc = vec(&Ly.kn, w[5], kQwenHD);
+    if (rc != RMU_OK) return rc;
+    int64_t shape[4][2];
+    decoder_shapes(e, shape);
+    void* stage = nullptr;
+    RMU_CUDA(cudaMalloc(&stage, kNf4LoadChunk * (sizeof(float) + sizeof(__half))));
+    float* stage_f = static_cast<float*>(stage);
+    __half* stage_lo = reinterpret_cast<__half*>(stage_f + kNf4LoadChunk);
+    // the same hi plane as upload_split's launch_split_planes, built chunk by chunk in the prefill scratch, then the
+    // same quantiser as rmu_decoder_quantize_nf4: the same codes and absmax
+    for (int p = 0; p < 4 && rc == RMU_OK; ++p) {
+        Nf4Weight& Q = Ly.nf4[p];
+        const int64_t n = shape[p][0] * shape[p][1];
+        if (!Q.codes) rc = dev_alloc(e->allocs, &Q.codes, n / 2);
+        if (rc == RMU_OK && !Q.absmax) rc = dev_alloc(e->allocs, &Q.absmax, n / kNf4Block);
+        if (rc != RMU_OK) break;
+        Q.rows = static_cast<int>(shape[p][0]);
+        Q.cols = static_cast<int>(shape[p][1]);
+        size_t done = 0, fill = 0;
+        auto flush = [&]() -> int {
+            const int r = launch_split_planes(stage_f, fill, e->nf4_hi + done, stage_lo, st);
+            done += fill;
+            fill = 0;
+            return r;
+        };
+        for (const auto& run : runs[p]) {
+            for (size_t at = 0; at < run.second && rc == RMU_OK;) {
+                const size_t take = std::min(run.second - at, kNf4LoadChunk - fill);
+                if (cudaMemcpyAsync(stage_f + fill, run.first + at, take * sizeof(float), cudaMemcpyHostToDevice, st) !=
+                    cudaSuccess) {
+                    set_error(fn + ": " + cudaGetErrorString(cudaGetLastError()));
+                    rc = RMU_ERR_CUDA;
+                    break;
+                }
+                fill += take;
+                at += take;
+                if (fill == kNf4LoadChunk) rc = flush();
+            }
+            if (rc != RMU_OK) break;
+        }
+        if (rc == RMU_OK) rc = flush();
+        if (rc == RMU_OK) rc = launch_nf4_quantize(e->nf4_hi, n, Q.codes, Q.absmax, st);
+    }
+    const cudaError_t err = cudaStreamSynchronize(st);
+    cudaFree(stage);
+    if (rc != RMU_OK) return rc;
+    if (err != cudaSuccess) { set_error(fn + ": " + cudaGetErrorString(err)); return RMU_ERR_CUDA; }
+    e->layers_loaded = layer + 1;
     return RMU_OK;
 }
 
@@ -4479,6 +4698,7 @@ int rmu_decoder_session_create(rmu_encoder* e, rmu_gen_session** out) {
     if (!e || !out) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
     *out = nullptr;
     int rc = check_decoder(e, fn);
+    if (rc == RMU_OK) rc = check_nf4_intact(e, fn);
     if (rc != RMU_OK) return rc;
     std::lock_guard<std::mutex> g(e->mu);
     rmu_gen_session* S = new rmu_gen_session();
@@ -5214,7 +5434,7 @@ int rmu_debug_modernbert_head(const float* pooled, int B, int H, int num_labels,
 int rmu_debug_rmsnorm(const float* x, int T, int H, const float* w, float eps, uint16_t* hi, uint16_t* lo,
                       int32_t* range_flag, void* stream) {
     if (!x || !w || !hi || !lo || T <= 0 || H <= 0) { set_error("rmu_debug_rmsnorm: bad argument"); return RMU_ERR_ARG; }
-    if (H % 128 != 0 || H > 4096) { set_error("rmu_debug_rmsnorm: H must be a multiple of 128 up to 4096"); return RMU_ERR_UNSUPPORTED; }
+    if (H % 128 != 0 || H > kRmsMaxHidden) { set_error("rmu_debug_rmsnorm: H must be a multiple of 128 up to 8192"); return RMU_ERR_UNSUPPORTED; }
     return launch_rms_split(x, T, H, w, eps, reinterpret_cast<__half*>(hi), reinterpret_cast<__half*>(lo), range_flag,
                             static_cast<cudaStream_t>(stream));
 }

@@ -109,6 +109,56 @@ class BertEncoder:
                     (C.c_void_p * len(bs))(*[None if b is None else b.ctypes.data for b in bs]), acts.ctypes.data),
                     "rmu_encoder_set_dense")
 
+    @classmethod
+    def nf4_decoder(cls, layers, device: Optional[int] = None, on_layer=None) -> "BertEncoder":
+        """a Llama or Qwen3 decoder in NF4 built one layer at a time from ``layers`` (``weights.DecoderLayers``):
+        ``rmu_decoder_create_nf4`` with the embeddings, final norm and rope tables, then ``rmu_decoder_load_layer_nf4``
+        per layer, so host memory holds the embeddings and one layer, and the device the finished handle and one
+        staging chunk.  ``on_layer(l)``, when given, runs after layer l is loaded."""
+        torch = _lib.require_cuda()
+        cfg = layers.cfg
+        llama = isinstance(cfg, LlamaConfig)
+        if not llama and not isinstance(cfg, Qwen3Config):
+            raise ValueError(f"{getattr(cfg, 'name', 'model')}: NF4 decoders are Llama or Qwen3")
+        self = cls.__new__(cls)
+        self.torch = torch
+        self.cfg = cfg
+        self.with_head = False
+        self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
+        self.max_tokens_per_call = MAX_TOKENS_PER_CALL
+        self.embed_dim = cfg.hidden
+        self._h = C.c_void_p()
+
+        def f32(a, shape, name):
+            a = np.ascontiguousarray(a, dtype=np.float32)
+            if tuple(a.shape) != tuple(shape):
+                raise ValueError(f"{name}: expected shape {shape}, got {a.shape}")
+            return a
+        g = layers.globals()
+        embed = f32(g["embed_tokens.weight"], (cfg.vocab_size, cfg.hidden), "embed_tokens.weight")
+        norm = f32(g["norm.weight"], (cfg.hidden,), "norm.weight")
+        cos, sin = cfg.rope_tables() if llama else rope_table(cfg.rope_theta, cfg.head_dim, cfg.max_pos)
+        cos, sin = np.ascontiguousarray(cos, dtype=np.float32), np.ascontiguousarray(sin, dtype=np.float32)
+        cc = _lib.bert_config_c(cfg)
+        qx = _lib.Qwen3ExtC(cfg.kv_heads, cfg.head_dim, cfg.max_pos, cfg.head_dim // 2, 0, -1)
+        lib = _lib.lib()
+        with torch.cuda.device(self.device):
+            _lib.check(lib.rmu_decoder_create_nf4(C.byref(cc), C.byref(qx), int(not llama), embed.ctypes.data,
+                                                  norm.ctypes.data, cos.ctypes.data, sin.ctypes.data, C.byref(self._h)),
+                       "rmu_decoder_create_nf4")
+            del embed, g
+            for l in range(cfg.layers):
+                t = layers.layer(l)
+                arrs = [f32(t[n], shape, n) for n, shape in layers.layer_names(l)]
+                del t
+                ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
+                _lib.check(lib.rmu_decoder_load_layer_nf4(self._h, l, ptrs, _lib.stream_ptr()),
+                           "rmu_decoder_load_layer_nf4")
+                del arrs
+                if on_layer is not None:
+                    on_layer(l)
+        return self
+
     def __del__(self):
         h = getattr(self, "_h", None)
         if h is not None and h.value:

@@ -21,6 +21,7 @@ the final handful of float32 additions.
 from __future__ import annotations
 
 import ctypes as C
+import logging
 import os
 import re
 import threading
@@ -30,7 +31,8 @@ import numpy as np
 
 from . import _lib, decode_session
 from .index import FlatIndex
-from .weights import decoder_lm_head, find_snapshot, resolve_decoder
+from .weights import (GB, check_decoder_plan, decoder_config, decoder_layers, decoder_lm_head, find_snapshot,
+                      resolve_decoder)
 
 
 def compute_rerank_provenance(reranker: Any, query: str, documents: Sequence[Any], answer: str) -> Sequence[Any]:
@@ -84,23 +86,36 @@ class DecoderAttention:
     GPU, for attention provenance and text generation (``llms.HuggingFacePipeline``).  Its weights are uploaded once;
     ``span_mass`` then runs one thread per call, and ``generate`` attaches the LM head the first time it runs.
 
-    ``weights="nf4"`` converts the layers' projections to NF4 right after the upload (``rmu_decoder_quantize_nf4``),
-    as the reference's bitsandbytes load holds them; ``"split"`` keeps the fp32-accurate split planes."""
+    ``weights="nf4"`` builds the handle in NF4 one layer at a time (``weights.decoder_layers``,
+    ``BertEncoder.nf4_decoder``), as the reference's bitsandbytes load holds the model: host memory holds the embeddings
+    and one layer, the device the finished handle and one staging chunk, and hidden sizes up to 8192 (the 70B class)
+    load.  ``"split"`` keeps the fp32-accurate split planes, up to hidden 4096.  The device-memory plan
+    (``weights.decoder_memory_plan``) is checked from the config before any tensor is read: split weights above hidden
+    4096, and an NF4 plan larger than the device's free memory, raise ValueError naming the bytes and the setting."""
 
     def __init__(self, model_name: str, device: Optional[int] = None, weights: str = "split"):
         from .encoder import BertEncoder
         if weights not in DECODER_WEIGHTS:
             raise ValueError(f"DecoderAttention: weights must be one of {DECODER_WEIGHTS}, got {weights!r}")
-        cfg, w = resolve_decoder(model_name)
-        self.cfg = cfg
+        cfg = decoder_config(model_name)
+        check_decoder_plan(cfg, weights)
+        torch = _lib.require_cuda()
+        dev = torch.cuda.current_device() if device is None else device
+        # split handles build as they always did; the NF4 build, whose size the plan states exactly, is refused when
+        # it cannot fit
+        self.plan = check_decoder_plan(cfg, weights, torch.cuda.mem_get_info(dev)[0] if weights == "nf4" else None)
         self.model_name = model_name
         self.weights = weights
-        self.encoder = BertEncoder(cfg, w, with_head=False, device=device)
-        del w
         if weights == "nf4":
-            enc = self.encoder
-            with enc.torch.cuda.device(enc.device):
-                enc._check(_lib.lib().rmu_decoder_quantize_nf4(enc._h, _lib.stream_ptr()), "rmu_decoder_quantize_nf4")
+            layers = decoder_layers(model_name)
+            self.cfg = layers.cfg
+            self.encoder = BertEncoder.nf4_decoder(layers, device=dev)
+            del layers
+        else:
+            cfg, w = resolve_decoder(model_name)
+            self.cfg = cfg
+            self.encoder = BertEncoder(cfg, w, with_head=False, device=dev)
+            del w
         self.lock = threading.Lock()
         self._lm_head = False
         self._scheduler = None
@@ -253,8 +268,68 @@ def _decoder(model: Any) -> DecoderAttention:
            weights)
     with _DECODERS_LOCK:
         if key not in _DECODERS:
+            if not isinstance(model, str):
+                # the plan's refusals (split weights above hidden 4096) come before the model is touched
+                plan = check_decoder_plan(decoder_config(name), weights)
+                release_model_if_needed(model, plan["build_peak"], key[1], weights)
             _DECODERS[key] = DecoderAttention(name, device=key[1], weights=weights)
         return _DECODERS[key]
+
+
+log = logging.getLogger(__name__)
+
+
+def _cuda_tensors(model: Any, device: int):
+    """the model's parameters and buffers on CUDA device ``device``"""
+    for m in model.modules():
+        for table in (m._parameters, m._buffers):
+            for t in table.values():
+                if t is not None and t.is_cuda and t.device.index == device:
+                    yield t
+
+
+def _held_bytes(t) -> int:
+    """a tensor's bytes, with bitsandbytes' absmax when it is on CUDA"""
+    import torch
+    n = t.numel() * t.element_size()
+    absmax = getattr(getattr(t, "quant_state", None), "absmax", None)
+    if isinstance(absmax, torch.Tensor) and absmax.is_cuda:
+        n += absmax.numel() * absmax.element_size()
+    return n
+
+
+def release_model_if_needed(model: Any, need: int, device: int, weights: str = "") -> int:
+    """The reference keeps its transformers copy of the chat model loaded (``RAGHelper_local._initialize_llm``, NF4 via
+    bitsandbytes), and the drop-ins read only its ``name_or_path``, ``config`` and ``generation_config``.  When the
+    decoder's planned ``need`` bytes do not fit in the device's free memory beside that copy, but do fit once the copy's
+    CUDA parameters and buffers on ``device`` are freed, free them (each becomes an empty CPU tensor, bitsandbytes'
+    quantisation state dropped), return the cached blocks to the driver (``torch.cuda.empty_cache``: the decoder
+    allocates with cudaMalloc, outside torch's allocator) and log the bytes released.  The model keeps its attributes
+    but can no longer run a forward.  When even that would not make room, raise ValueError naming the bytes and leave
+    the model as it was.  Returns the bytes released (0 when the decoder fits and nothing changes)."""
+    import torch
+    if getattr(model, "modules", None) is None:
+        return 0
+    free = torch.cuda.mem_get_info(device)[0]
+    if need <= free:
+        return 0
+    held = sum(_held_bytes(t) for t in _cuda_tensors(model, device))
+    if need > free + held:
+        raise ValueError(
+            f"{getattr(model, 'name_or_path', 'model')}: the GPU decoder needs {need} bytes ({need / GB:.1f} GB) with "
+            f"RMU_DECODER_WEIGHTS={weights or 'split'}; the device has {free} bytes free and the transformers model "
+            f"holds {held} bytes on it, so freeing the model would not make room: the model is left as it was")
+    freed = 0
+    for t in list(_cuda_tensors(model, device)):
+        freed += _held_bytes(t)
+        t.data = torch.empty(0, dtype=t.dtype)
+        if getattr(t, "quant_state", None) is not None:
+            t.quant_state = None
+    torch.cuda.empty_cache()
+    log.warning("released %d bytes (%.1f GB) of %s's CUDA parameters and buffers: the GPU decoder needs %d bytes and "
+                "did not fit beside them; the transformers model can no longer run forwards", freed, freed / GB,
+                getattr(model, "name_or_path", "the model"), need)
+    return freed
 
 
 def _find_part(thread: List[int], part: List[int]):

@@ -543,21 +543,24 @@ def qwen3_to_canonical(raw: Dict[str, np.ndarray], cfg: Qwen3Config) -> Dict[str
     return w
 
 
+def _synthetic_draw(rng: np.random.Generator, name: str, shape, scale: float) -> np.ndarray:
+    """one seeded decoder tensor from ``rng``'s stream: norm weights 1 + N(0, 0.1), embeddings N(0, 0.02) (three times
+    that when scale > 1), everything else N(0, 0.02 scale)"""
+    if name.endswith("norm.weight") or name.endswith("layernorm.weight"):
+        a = 1.0 + 0.1 * rng.standard_normal(shape)
+    elif name == "embed_tokens.weight":
+        a = 0.02 * rng.standard_normal(shape) * (3.0 if scale > 1 else 1.0)
+    else:
+        a = 0.02 * scale * rng.standard_normal(shape)
+    return np.ascontiguousarray(a, dtype=np.float32)
+
+
 def synthetic_qwen3_weights(cfg: Qwen3Config, seed: int = 0, with_head: bool = False,
                             scale: float = 1.0) -> Dict[str, np.ndarray]:
     """seeded Qwen3 weights: projections N(0, 0.02 scale), norm weights near 1, embeddings N(0, 0.02) (transformers'
     init, with norm gains spread so a wrong weight layout shows in the numbers)"""
     rng = np.random.default_rng(seed)
-    out: Dict[str, np.ndarray] = {}
-    for name, shape in qwen3_weight_names(cfg, with_head):
-        if name.endswith("norm.weight") or name.endswith("layernorm.weight"):
-            a = 1.0 + 0.1 * rng.standard_normal(shape)
-        elif name == "embed_tokens.weight":
-            a = 0.02 * rng.standard_normal(shape) * (3.0 if scale > 1 else 1.0)
-        else:
-            a = 0.02 * scale * rng.standard_normal(shape)
-        out[name] = np.ascontiguousarray(a, dtype=np.float32)
-    return out
+    return {name: _synthetic_draw(rng, name, shape, scale) for name, shape in qwen3_weight_names(cfg, with_head)}
 
 
 def qwen3_lm_rows(path: str, cfg: Qwen3Config, ids) -> np.ndarray:
@@ -644,43 +647,47 @@ def llama_weight_names(cfg: LlamaConfig):
 def synthetic_llama_weights(cfg: LlamaConfig, seed: int = 0, scale: float = 1.0) -> Dict[str, np.ndarray]:
     """seeded Llama weights, drawn as ``synthetic_qwen3_weights`` draws them"""
     rng = np.random.default_rng(seed)
-    out: Dict[str, np.ndarray] = {}
-    for name, shape in llama_weight_names(cfg):
-        if name.endswith("norm.weight") or name.endswith("layernorm.weight"):
-            a = 1.0 + 0.1 * rng.standard_normal(shape)
-        elif name == "embed_tokens.weight":
-            a = 0.02 * rng.standard_normal(shape) * (3.0 if scale > 1 else 1.0)
-        else:
-            a = 0.02 * scale * rng.standard_normal(shape)
-        out[name] = np.ascontiguousarray(a, dtype=np.float32)
-    return out
+    return {name: _synthetic_draw(rng, name, shape, scale) for name, shape in llama_weight_names(cfg)}
 
 
 # decoders for attention provenance (provenance.DecoderAttention), apart from PRESETS: the embedders, rerankers and
 # ColBERT never take them.  tiny-llama: head_dim 128, two query heads per kv head, three layers, and llama3 scaling
 # with original_max_position_embeddings 64, so that several of its frequencies are divided or interpolated.
 # llama-3.1-8b: Meta-Llama-3.1-8B-Instruct's shape [3P-recall: its config.json is not read here].
+# llama-3.1-70b: Llama-3.1-70B-Instruct's (and Llama-3.3-70B-Instruct's) shape, and qwen3-32b: Qwen3-32B's
+# [3P-recall: their config.json files are not read here]; both run in NF4 only (hidden above 4096).
 DECODER_PRESETS: Dict[str, BertConfig] = {
     "tiny-llama": LlamaConfig(vocab_size=1000, hidden=256, layers=3, heads=4, ffn=384, max_pos=8192, kv_heads=2,
                               rope_theta=10000.0, rope_scaling=(8.0, 1.0, 4.0, 64)),
     "llama-3.1-8b": LlamaConfig(),
+    "llama-3.1-70b": LlamaConfig(hidden=8192, layers=80, heads=64, ffn=28672),
+    "qwen3-32b": Qwen3Config(vocab_size=151936, hidden=5120, layers=64, heads=64, ffn=25600, kv_heads=8,
+                             tie_word_embeddings=False, num_labels=1),
 }
 
 
-def _load_decoder_snapshot(path: str):
-    """a ``llama`` or ``qwen3`` snapshot -> (config, weights) of the decoder without any head; ``lm_head`` (and a
-    sequence-classification ``score``) is never read"""
+def _decoder_config_of_snapshot(path: str) -> BertConfig:
     cfgd = _read_json(os.path.join(path, "config.json"))
     if cfgd is None:
         raise FileNotFoundError(f"{path}: no config.json")
     kind = cfgd.get("model_type")
     if kind == "llama":
-        cfg = LlamaConfig.from_hf(cfgd, name=path)
-    elif kind == "qwen3":
-        cfg = Qwen3Config.from_hf(cfgd, name=path)
-    else:
-        raise ValueError(f"{path}: model_type {kind!r} is not supported for attention provenance (llama, qwen3)")
-    names = llama_weight_names(cfg) if kind == "llama" else qwen3_weight_names(cfg, False)
+        return LlamaConfig.from_hf(cfgd, name=path)
+    if kind == "qwen3":
+        return Qwen3Config.from_hf(cfgd, name=path)
+    raise ValueError(f"{path}: model_type {kind!r} is not supported for attention provenance (llama, qwen3)")
+
+
+def decoder_weight_names(cfg: BertConfig):
+    """``llama_weight_names`` or, for a Qwen3 config, ``qwen3_weight_names`` without a head"""
+    return llama_weight_names(cfg) if isinstance(cfg, LlamaConfig) else qwen3_weight_names(cfg, False)
+
+
+def _load_decoder_snapshot(path: str):
+    """a ``llama`` or ``qwen3`` snapshot -> (config, weights) of the decoder without any head; ``lm_head`` (and a
+    sequence-classification ``score``) is never read"""
+    cfg = _decoder_config_of_snapshot(path)
+    names = decoder_weight_names(cfg)
     w = qwen3_to_canonical(_load_tensors(path, lambda n: n not in ("lm_head.weight", "score.weight")), cfg)
     missing = [n for n, _ in names if n not in w]
     if missing:
@@ -696,17 +703,208 @@ def resolve_decoder(model_name: str, cache_folder: Optional[str] = None):
         preset = parts[1]
         seed = int(parts[2]) if len(parts) > 2 else 0
         scale = float(parts[3]) if len(parts) > 3 else 1.0
-        if preset in DECODER_PRESETS:
-            cfg = LlamaConfig(**asdict(DECODER_PRESETS[preset]))
-            cfg.name = model_name
+        cfg = decoder_config(model_name)
+        if isinstance(cfg, LlamaConfig):
             return cfg, synthetic_llama_weights(cfg, seed=seed, scale=scale)
-        if preset in PRESETS and isinstance(PRESETS[preset][0], Qwen3Config):
-            cfg = Qwen3Config(**asdict(PRESETS[preset][0]))
-            cfg.name, cfg.reranker, cfg.num_labels = model_name, False, 1
-            return cfg, synthetic_qwen3_weights(cfg, seed=seed, with_head=False, scale=scale)
-        raise ValueError(f"unknown synthetic decoder preset {preset!r}; have {sorted(DECODER_PRESETS)} and the qwen3 "
-                         f"presets")
+        return cfg, synthetic_qwen3_weights(cfg, seed=seed, with_head=False, scale=scale)
     return _load_decoder_snapshot(find_snapshot(model_name, cache_folder))
+
+
+def decoder_config(model_name: str, cache_folder: Optional[str] = None) -> BertConfig:
+    """the config of ``resolve_decoder``'s decoder, read without any tensor: a synthetic preset's, or the snapshot's
+    config.json"""
+    if model_name.startswith("synthetic:"):
+        preset = model_name.split(":")[1]
+        if preset in DECODER_PRESETS:
+            base = DECODER_PRESETS[preset]
+        elif preset in PRESETS and isinstance(PRESETS[preset][0], Qwen3Config):
+            base = PRESETS[preset][0]
+        else:
+            raise ValueError(f"unknown synthetic decoder preset {preset!r}; have {sorted(DECODER_PRESETS)} and the "
+                             f"qwen3 presets")
+        cfg = type(base)(**asdict(base))
+        cfg.name = model_name
+        if isinstance(cfg, Qwen3Config):
+            cfg.reranker, cfg.num_labels = False, 1
+        return cfg
+    return _decoder_config_of_snapshot(find_snapshot(model_name, cache_folder))
+
+
+class DecoderLayers:
+    """A decoder's weights read one layer at a time (``rmu_decoder_create_nf4`` / ``rmu_decoder_load_layer_nf4``):
+    ``cfg``; ``globals()`` -> embed_tokens and the final norm; ``layer(l)`` -> layer l's tensors in
+    ``decoder_weight_names`` order (canonical names, float32).  Host memory holds the embeddings and one layer."""
+
+    def __init__(self, cfg: BertConfig):
+        self.cfg = cfg
+
+    def globals(self) -> Dict[str, np.ndarray]:
+        raise NotImplementedError
+
+    def layer(self, l: int) -> Dict[str, np.ndarray]:
+        raise NotImplementedError
+
+    def layer_names(self, l: int):
+        p = f"layers.{l}."
+        return [(n, shape) for n, shape in decoder_weight_names(self.cfg) if n.startswith(p)]
+
+
+class DictDecoderLayers(DecoderLayers):
+    """the layered view of a whole weight dict (``resolve_decoder``'s)"""
+
+    def __init__(self, cfg: BertConfig, w: Dict[str, np.ndarray]):
+        super().__init__(cfg)
+        self.w = w
+
+    def globals(self):
+        return {n: self.w[n] for n in ("embed_tokens.weight", "norm.weight")}
+
+    def layer(self, l):
+        return {n: self.w[n] for n, _ in self.layer_names(l)}
+
+
+class SyntheticDecoderLayers(DecoderLayers):
+    """``synthetic:<preset>[:seed[:scale]]`` drawn one layer at a time: the same tensors, bit for bit, as
+    ``synthetic_llama_weights`` / ``synthetic_qwen3_weights``, whose one seeded stream runs embeddings, layers 0 ..
+    L - 1, final norm.  The final norm is needed first, so ``globals`` walks the whole stream once, drawing each layer
+    and dropping it, and keeps only the generator's state at every layer's start; ``layer(l)`` then draws layer l again
+    from its state.  Every layer is therefore drawn twice, on the host in float64 (for a synthetic 70B about 68 G
+    normals each time: minutes, not seconds); ``tools/bench_generate.py`` draws its 70B weights on the device instead.
+    Nothing but those states is kept between calls."""
+
+    def __init__(self, cfg: BertConfig, seed: int = 0, scale: float = 1.0):
+        super().__init__(cfg)
+        self.seed, self.scale = seed, scale
+        self._states: list = []
+
+    def globals(self):
+        rng = np.random.default_rng(self.seed)
+        names = decoder_weight_names(self.cfg)
+        out = {names[0][0]: _synthetic_draw(rng, *names[0], self.scale)}
+        states = []
+        for l in range(self.cfg.layers):
+            states.append(rng.bit_generator.state)
+            for n, shape in self.layer_names(l):
+                _synthetic_draw(rng, n, shape, self.scale)
+        out[names[-1][0]] = _synthetic_draw(rng, *names[-1], self.scale)
+        self._states = states
+        return out
+
+    def layer(self, l):
+        if not self._states:
+            self.globals()
+        rng = np.random.default_rng()
+        rng.bit_generator.state = self._states[l]
+        return {n: _synthetic_draw(rng, n, shape, self.scale) for n, shape in self.layer_names(l)}
+
+
+class SnapshotDecoderLayers(DecoderLayers):
+    """a ``llama`` or ``qwen3`` snapshot read with safetensors' ``safe_open``, tensor by tensor, from
+    ``model.safetensors`` or the shards ``model.safetensors.index.json`` lists; bfloat16 is widened to float32 (exact)"""
+
+    def __init__(self, path: str):
+        super().__init__(_decoder_config_of_snapshot(path))
+        self.path = path
+        idx = _read_json(os.path.join(path, SHARD_INDEX))
+        single = os.path.join(path, "model.safetensors")
+        if os.path.exists(single) or idx is None:
+            from safetensors import safe_open
+            with safe_open(single, framework="pt") as f:
+                self.where = {k: single for k in f.keys()}
+        else:
+            self.where = {k: os.path.join(path, f) for k, f in idx["weight_map"].items()}
+
+    def _read(self, names) -> Dict[str, np.ndarray]:
+        import torch
+        from safetensors import safe_open
+        stored = {}
+        for n in names:
+            for k in ("model." + n, n):
+                if k in self.where:
+                    stored[n] = k
+                    break
+            else:
+                raise KeyError(f"{self.path}: missing tensor {n}")
+        out: Dict[str, np.ndarray] = {}
+        for f in dict.fromkeys(self.where[k] for k in stored.values()):
+            with safe_open(f, framework="pt") as fh:
+                for n, k in stored.items():
+                    if self.where[k] == f:
+                        out[n] = np.ascontiguousarray(fh.get_tensor(k).to(torch.float32).numpy())
+        return {n: out[n] for n in names}
+
+    def globals(self):
+        return self._read(["embed_tokens.weight", "norm.weight"])
+
+    def layer(self, l):
+        return self._read([n for n, _ in self.layer_names(l)])
+
+
+def decoder_layers(model_name: str, cache_folder: Optional[str] = None) -> DecoderLayers:
+    """``resolve_decoder``'s decoder as a ``DecoderLayers``: the same tensors, read or drawn one layer at a time"""
+    if model_name.startswith("synthetic:"):
+        parts = model_name.split(":")
+        return SyntheticDecoderLayers(decoder_config(model_name), seed=int(parts[2]) if len(parts) > 2 else 0,
+                                      scale=float(parts[3]) if len(parts) > 3 else 1.0)
+    path = find_snapshot(model_name, cache_folder)
+    if not _safetensors_snapshot(path):
+        # a snapshot that ships only pytorch_model.bin: a pickle cannot be read tensor by tensor, so it is read whole
+        # (with weights_only, as _load_tensors reads it) and handed over layer by layer
+        return DictDecoderLayers(*_load_decoder_snapshot(path))
+    return SnapshotDecoderLayers(path)
+
+
+def _safetensors_snapshot(path: str) -> bool:
+    """``model.safetensors`` or a sharded safetensors index is present"""
+    return os.path.exists(os.path.join(path, "model.safetensors")) or os.path.exists(os.path.join(path, SHARD_INDEX))
+
+
+GB = 1e9
+SPLIT_MAX_HIDDEN = 4096           # rmu_encoder_create_llama / _qwen3: split planes stop here; NF4 goes to 8192
+NF4_LOAD_STAGING = (1 << 24) * 6  # rmu_decoder_load_layer_nf4's staging chunk: 16 Mi fp32 values and their lo plane
+
+
+def decoder_memory_plan(cfg: BertConfig, weights: str) -> Dict[str, int]:
+    """the device bytes a decoder handle holds once built, computed from the config alone: ``layers`` (the projections:
+    NF4 codes + absmax, or split planes), ``embeddings`` (fp32), ``lm_head`` (split planes, attached at the first
+    generation), ``scratch`` (NF4's prefill plane pair, the size of the largest projection), ``other`` (norms, rope
+    tables, the zero bias) and their ``total``; ``build_peak`` adds the NF4 load's staging chunk.  The KV cache and the
+    activations grow with the calls and are not counted."""
+    H, F, L, V = cfg.hidden, cfg.ffn, cfg.layers, cfg.vocab_size
+    QD, KD = cfg.heads * cfg.head_dim, cfg.kv_heads * cfg.head_dim
+    shapes = [(QD + 2 * KD, H), (H, QD), (2 * F, H), (H, F)]
+    n = sum(a * b for a, b in shapes)
+    nf4 = weights == "nf4"
+    plan = {
+        "layers": L * (n // 2 + n // 64 * 4) if nf4 else L * n * 4,
+        "embeddings": V * H * 4,
+        "lm_head": V * H * 4 + V * 4,
+        "scratch": 4 * max(a * b for a, b in shapes) if nf4 else 0,
+        "other": 4 * (L * (2 * H + (2 * cfg.head_dim if isinstance(cfg, Qwen3Config) else 0)) + H
+                      + 2 * cfg.max_pos * cfg.head_dim // 2 + max(QD + 2 * KD, 2 * F, H)),
+    }
+    plan["total"] = sum(plan.values())
+    plan["build_peak"] = plan["total"] + (NF4_LOAD_STAGING if nf4 else 0)
+    return plan
+
+
+def check_decoder_plan(cfg: BertConfig, weights: str, free_bytes: Optional[int] = None) -> Dict[str, int]:
+    """``decoder_memory_plan``, refused with a ValueError naming the bytes and the setting: split weights above hidden
+    4096 (NF4 takes them), and, given the device's free bytes, a plan that does not fit"""
+    plan = decoder_memory_plan(cfg, weights)
+    name = getattr(cfg, "name", "decoder")
+    if weights != "nf4" and cfg.hidden > SPLIT_MAX_HIDDEN:
+        raise ValueError(
+            f"{name}: hidden_size {cfg.hidden} > {SPLIT_MAX_HIDDEN} runs on NF4 weights only; split planes would need "
+            f"{plan['layers'] / GB:.1f} GB for the layers ({plan['total']} bytes in all): set RMU_DECODER_WEIGHTS=nf4, "
+            f"which plans {decoder_memory_plan(cfg, 'nf4')['total'] / GB:.1f} GB")
+    if free_bytes is not None and plan["build_peak"] > free_bytes:
+        raise ValueError(
+            f"{name}: the decoder needs {plan['build_peak']} bytes ({plan['build_peak'] / GB:.1f} GB) of device memory "
+            f"with RMU_DECODER_WEIGHTS={weights}, and the device has {free_bytes} bytes ({free_bytes / GB:.1f} GB) free"
+            + ("; RMU_DECODER_WEIGHTS=nf4 plans " f"{decoder_memory_plan(cfg, 'nf4')['build_peak'] / GB:.1f} GB"
+               if weights != "nf4" else ""))
+    return plan
 
 
 def decoder_lm_head(model_name: str, cfg: BertConfig, cache_folder: Optional[str] = None) -> np.ndarray:

@@ -16,6 +16,15 @@ With --weights nf4 the run holds two handles of the same weights, one split and 
 (rmu_decoder_quantize_nf4), and alternates their calls; the NF4 decode step's projections are the "nf4" timer class.
 It also times the decode GEMV alone on one layer's four projections of the full 8B shape (CUDA events over 200
 launches of each) and states the share of 3.35 TB/s that their NF4 bytes (codes and absmax) reach.
+
+    python tools/bench_generate.py --shape llama-3.1-70b [--layers 80] [--tokens 32] [--json OUT]
+
+--shape llama-3.1-70b or qwen3-32b runs that shape in NF4 only, built layer by layer (BertEncoder.nf4_decoder) from
+seeded per-layer weights drawn on the device with torch's generator (one seed per layer; no full-depth copy of the
+model ever exists on the host), all layers by default.  It adds the load time (with the time spent drawing the
+weights apart), the device bytes held after the load and after the LM head (cudaMemGetInfo, against
+weights.decoder_memory_plan), and the GEMV's share of 3.35 TB/s on one layer of that shape.  The floor it states is
+the NF4 layers plus the split-plane LM head read once per token.
 """
 from __future__ import annotations
 
@@ -32,6 +41,7 @@ from dataclasses import asdict, replace
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from ragmeup_b200.weights import DecoderLayers  # noqa: E402
 
 FULL_LAYERS = 32
 PROF = {"gemm": 4, "decode_attention": 11, "lm_head": 12, "sampler": 13, "nf4": 14}
@@ -94,9 +104,77 @@ def gemv_share(cfg) -> dict:
     return out
 
 
+class SeededLayers(DecoderLayers):
+    """seeded weights drawn on the device, one torch generator per tensor group: norms 1 + N(0, 0.1), embeddings and
+    projections N(0, 0.02); ``draw_s`` sums the time spent drawing and copying to host"""
+
+    def __init__(self, cfg, seed: int = 0):
+        super().__init__(cfg)
+        self.seed, self.draw_s = seed, 0.0
+
+    def _draw(self, key: int, items):
+        import torch
+        t0 = time.perf_counter()
+        g = torch.Generator(device="cuda").manual_seed(self.seed * 1_000_003 + key)
+        out = {}
+        for name, shape in items:
+            a = torch.randn(shape, generator=g, device="cuda")
+            a = 1.0 + 0.1 * a if name.endswith("norm.weight") or name.endswith("layernorm.weight") else 0.02 * a
+            out[name] = a.cpu().numpy()
+            del a
+        torch.cuda.synchronize()
+        self.draw_s += time.perf_counter() - t0
+        return out
+
+    def globals(self):
+        c = self.cfg
+        return self._draw(0, [("embed_tokens.weight", (c.vocab_size, c.hidden)), ("norm.weight", (c.hidden,))])
+
+    def layer(self, l):
+        return self._draw(1 + l, self.layer_names(l))
+
+
+def large(args):
+    """--shape llama-3.1-70b / qwen3-32b: the NF4 handle built layer by layer, then the same timings"""
+    import torch
+    from ragmeup_b200 import _lib
+    from ragmeup_b200.encoder import BertEncoder
+    from ragmeup_b200.weights import decoder_config, decoder_memory_plan
+    cfg = replace(decoder_config("synthetic:" + args.shape), name=args.shape)
+    if args.layers:
+        cfg = replace(cfg, layers=args.layers)
+    l = _lib.lib()
+    res = {"card": card(), "shape": args.shape, "layers": cfg.layers, "weights": ["nf4"], "rows": []}
+    print(json.dumps(res["card"]))
+    plan = decoder_memory_plan(cfg, "nf4")
+    torch.cuda.synchronize()
+    free0 = torch.cuda.mem_get_info()[0]
+    src = SeededLayers(cfg, seed=0)
+    t0 = time.perf_counter()
+    enc = BertEncoder.nf4_decoder(src)
+    load_s = time.perf_counter() - t0
+    torch.cuda.empty_cache()
+    held = free0 - torch.cuda.mem_get_info()[0]
+    lm = SeededLayers(cfg, seed=1)._draw(0, [("lm_head", (cfg.vocab_size, cfg.hidden))])["lm_head"]
+    _lib.check(l.rmu_decoder_set_lm_head(enc._h, lm.ctypes.data), "rmu_decoder_set_lm_head")
+    del lm
+    torch.cuda.empty_cache()
+    held_head = free0 - torch.cuda.mem_get_info()[0]
+    res["load"] = {"load_s": round(load_s, 1), "of_which_drawing_weights_s": round(src.draw_s, 1),
+                   "device_bytes_after_load": held, "planned_without_lm_head": plan["total"] - plan["lm_head"],
+                   "device_bytes_with_lm_head": held_head, "planned_total": plan["total"],
+                   "plan_gb": {k: round(v / 1e9, 3) for k, v in plan.items()}}
+    print(json.dumps(res["load"]))
+    nbytes = plan["layers"] + cfg.vocab_size * cfg.hidden * 4
+    res["floor"] = {"bytes_per_token_computed": nbytes, "ms_per_token_at_3.35TBps_computed": round(nbytes / 3.35e9, 2)}
+    print(json.dumps(res["floor"]))
+    return cfg, {"nf4": enc}, res
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--layers", type=int, default=4)
+    ap.add_argument("--shape", choices=("llama-3.1-8b", "llama-3.1-70b", "qwen3-32b"), default="llama-3.1-8b")
+    ap.add_argument("--layers", type=int, default=None)
     ap.add_argument("--tokens", type=int, default=32)
     ap.add_argument("--calls", type=int, default=3)
     ap.add_argument("--weights", choices=("split", "nf4"), default="split")
@@ -107,25 +185,31 @@ def main():
     from ragmeup_b200.encoder import BertEncoder
     from ragmeup_b200.weights import DECODER_PRESETS, LlamaConfig, synthetic_llama_weights
 
-    cfg = replace(LlamaConfig(**asdict(DECODER_PRESETS["llama-3.1-8b"])), layers=args.layers, name="llama-3.1-8b")
     l = _lib.lib()
-    w = synthetic_llama_weights(cfg, seed=0)
-    lm = (0.02 * np.random.default_rng(1).standard_normal((cfg.vocab_size, cfg.hidden))).astype(np.float32)
-    handles = {}
-    for kind in (("split", "nf4") if args.weights == "nf4" else ("split",)):
-        enc = BertEncoder(cfg, w, with_head=False)
-        _lib.check(l.rmu_decoder_set_lm_head(enc._h, lm.ctypes.data), "rmu_decoder_set_lm_head")
-        if kind == "nf4":
-            _lib.check(l.rmu_decoder_quantize_nf4(enc._h, _lib.stream_ptr()), "rmu_decoder_quantize_nf4")
-        handles[kind] = enc
-    del lm, w
     s = _lib.SamplingC(0, 1.0, 1.0, 1.0, 50, 0, (C.c_int32 * _lib.MAX_EOS)())
-    res = {"card": card(), "shape": "llama-3.1-8b", "layers": cfg.layers, "weights": list(handles), "rows": []}
-    print(json.dumps(res["card"]))
-    full_gb = split_plane_bytes(cfg, FULL_LAYERS) / 1e9
-    res["floor"] = {"split_plane_gb_32_layers_computed": round(full_gb, 2),
-                    "ms_per_token_at_3.35TBps_computed": round(full_gb / 3.35, 2)}
-    print(json.dumps(res["floor"]))
+    if args.shape != "llama-3.1-8b":
+        cfg, handles, res = large(args)
+        full_layers = cfg.layers
+    else:
+        full_layers = FULL_LAYERS
+        cfg = replace(LlamaConfig(**asdict(DECODER_PRESETS["llama-3.1-8b"])), layers=args.layers or 4,
+                      name="llama-3.1-8b")
+        w = synthetic_llama_weights(cfg, seed=0)
+        lm = (0.02 * np.random.default_rng(1).standard_normal((cfg.vocab_size, cfg.hidden))).astype(np.float32)
+        handles = {}
+        for kind in (("split", "nf4") if args.weights == "nf4" else ("split",)):
+            enc = BertEncoder(cfg, w, with_head=False)
+            _lib.check(l.rmu_decoder_set_lm_head(enc._h, lm.ctypes.data), "rmu_decoder_set_lm_head")
+            if kind == "nf4":
+                _lib.check(l.rmu_decoder_quantize_nf4(enc._h, _lib.stream_ptr()), "rmu_decoder_quantize_nf4")
+            handles[kind] = enc
+        del lm, w
+        res = {"card": card(), "shape": "llama-3.1-8b", "layers": cfg.layers, "weights": list(handles), "rows": []}
+        print(json.dumps(res["card"]))
+        full_gb = split_plane_bytes(cfg, FULL_LAYERS) / 1e9
+        res["floor"] = {"split_plane_gb_32_layers_computed": round(full_gb, 2),
+                        "ms_per_token_at_3.35TBps_computed": round(full_gb / 3.35, 2)}
+        print(json.dumps(res["floor"]))
     rng = np.random.default_rng(0)
     for T in (1024, 4096):
         ids = np.ascontiguousarray(rng.integers(0, cfg.vocab_size, T), dtype=np.int32)
@@ -163,11 +247,12 @@ def main():
                     parts[name] = parts.get(name, 0.0) + (ms.value if k > 1 else -ms.value)
             step = {k: v / args.tokens for k, v in parts.items()}
             step["projections"] = step.pop("gemm") - step["lm_head"] + step.pop("nf4")
-            scale = FULL_LAYERS / cfg.layers
+            scale = full_layers / cfg.layers
             row = {"weights": kind, "T": T, "prefill_ms": round(one, 3), "ms_per_token": round(per_tok, 3),
-                   "step_ms": {k: round(v, 3) for k, v in step.items()},
-                   "ms_per_token_32_layers_extrapolated": round(step["lm_head"] + step["sampler"] +
-                                                                scale * (per_tok - step["lm_head"] - step["sampler"]), 3)}
+                   "step_ms": {k: round(v, 3) for k, v in step.items()}}
+            if scale != 1:
+                row[f"ms_per_token_{full_layers}_layers_extrapolated"] = round(
+                    step["lm_head"] + step["sampler"] + scale * (per_tok - step["lm_head"] - step["sampler"]), 3)
             res["rows"].append(row)
             print(json.dumps(row))
     if "nf4" in handles:
