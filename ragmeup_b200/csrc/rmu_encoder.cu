@@ -2401,6 +2401,19 @@ static int grow(DevBuf& b, size_t need, size_t alloc = 0) {
     return RMU_OK;
 }
 
+// Lays regions out back to back at 256-byte boundaries: run a layout once from a null base to size its buffer, then
+// again from the buffer to place the regions
+struct Carve {
+    uintptr_t base;
+    size_t size = 0;
+    explicit Carve(void* b) : base(reinterpret_cast<uintptr_t>(b)) {}
+    template <typename T> T* take(size_t n) {
+        T* p = reinterpret_cast<T*>(base + size);
+        size += (n * sizeof(T) + 255) / 256 * 256;
+        return p;
+    }
+};
+
 // rows of the per-token and per-sequence buffers grown for T tokens and B sequences
 static size_t token_rows(int T) { return (std::max(T, 1024) + 127) / 128 * 128; }
 static size_t seq_rows(int B) { return std::max(B + 1, 1024); }
@@ -2436,16 +2449,14 @@ struct rmu_encoder {
     bool llama = false;
     DevBuf span_ws;
     int* span_cu = nullptr;
-    // generation (rmu_decoder_set_lm_head, rmu_decoder_generate): the LM head [V, H] as split planes and a zero bias [V];
-    // the KV cache (layers x K hi | K lo | V hi | V lo [kv_heads, kv_cap, 128]); gen_ws = logits [V] | presence bits |
-    // the step's token | decode attention's partials.  Grown under mu.
+    // generation (rmu_decoder_set_lm_head, rmu_decoder_generate*): the LM head [V, H] as split planes and a zero bias
+    // [V]; the KV cache (layers x K hi | K lo | V hi | V lo [kv_heads, kv_cap, 128]); gen_ws = the scratch of one
+    // generate or generate_batch call, laid out by that call.  Grown under mu.
     SplitOperand lm_head;
     bool has_lm_head = false;
     float* lm_zero = nullptr;
     DevBuf kv_cache, gen_ws;
     int kv_cap = 0;
-    // rmu_decoder_generate_batch's own workspace (run_batch_prefill, the batched decode steps), grown under mu
-    DevBuf batch_ws;
     // NF4 weights (rmu_decoder_quantize_nf4): the layers' projections live in EncLayer::nf4; a prefill dequantises
     // each into the one scratch operand set nf4_hi | nf4_lo (lo all zero), seen through nf4_op[projection]'s tensor
     // maps.  nf4_broken: a conversion failed part-way and the handle cannot run.  nf4_peak / nf4_delta: the most the
@@ -2890,6 +2901,16 @@ static __half* kv_layer(const rmu_encoder* e, const KvView& v, int l) {
 
 static __half* kv_layer(rmu_encoder* e, int l) { return kv_layer(e, handle_kv(e), l); }
 
+// grow the handle's KV cache to hold at least cap positions
+static int ensure_kv(rmu_encoder* e, const std::string& fn, int cap) {
+    if (cap <= e->kv_cap) return RMU_OK;
+    e->kv_cap = 0;                                      // until grow succeeds: it may free the old cache first
+    const int rc = grow(e->kv_cache, static_cast<size_t>(e->cfg.layers) * 4 * e->qext.kv_heads * cap * kQwenHD * sizeof(__half));
+    if (rc != RMU_OK) set_error(fn + ": the KV cache for " + std::to_string(cap) + " positions: " + rmu_last_error());
+    else e->kv_cap = cap;
+    return rc;
+}
+
 // the rmu_decoder_* entry points run on decoder handles only
 static int check_decoder(const rmu_encoder* e, const std::string& fn) {
     if (e->qwen && !e->has_head) return RMU_OK;
@@ -2908,6 +2929,31 @@ static int check_nf4_intact(const rmu_encoder* e, const std::string& fn) {
     if (!e->nf4_broken) return RMU_OK;
     set_error(fn + ": the handle's NF4 conversion failed part-way (rmu_decoder_quantize_nf4); destroy it");
     return RMU_ERR_ARG;
+}
+
+// the generation entry points run on an intact decoder handle with an LM head
+static int check_generator(const rmu_encoder* e, const std::string& fn) {
+    int rc = check_decoder(e, fn);
+    if (rc != RMU_OK) return rc;
+    if (!e->has_lm_head) { set_error(fn + ": no LM head is attached (rmu_decoder_set_lm_head)"); return RMU_ERR_ARG; }
+    return check_nf4_intact(e, fn);
+}
+
+// the prompts b < B, ids_h[cu_h[b] .. cu_h[b + 1]), a generation entry point refuses before any CUDA call
+static int check_prompts(const rmu_encoder* e, const std::string& fn, const int32_t* ids_h, const int32_t* cu_h, int B) {
+    const rmu_bert_config& c = e->cfg;
+    for (int b = 0; b < B; ++b) {
+        const int T = cu_h[b + 1] - cu_h[b];
+        if (T <= 0 || cu_h[b] < 0) { set_error(fn + ": prompt " + std::to_string(b) + " is empty"); return RMU_ERR_ARG; }
+        if (T >= c.max_pos) {
+            set_error(fn + ": a prompt of " + std::to_string(T) + " tokens leaves no position for a new token " +
+                      "(max_position_embeddings " + std::to_string(c.max_pos) + ")");
+            return RMU_ERR_ARG;
+        }
+        for (int i = cu_h[b]; i < cu_h[b + 1]; ++i)
+            if (ids_h[i] < 0 || ids_h[i] >= c.vocab_size) { set_error(fn + ": token id out of range"); return RMU_ERR_ARG; }
+    }
+    return RMU_OK;
 }
 
 // Qwen3's layers (the header's formula): leaves the residual stream h, before the final norm, in e->PRE [T, H] fp32.
@@ -2942,17 +2988,24 @@ static int run_qwen3(rmu_encoder* e, const int32_t* ids, const int32_t* cu, int 
     return RMU_OK;
 }
 
-// reads the range flag of run_qwen3's split kernels (synchronises st): RMU_ERR_RANGE when an activation left fp16's range
-static int qwen3_check_range(rmu_encoder* e, cudaStream_t st) {
+// whether the range flag of the split kernels is raised, cleared again when it is (synchronises st)
+static int read_range(rmu_encoder* e, bool* raised, cudaStream_t st) {
     int flag = 0;
     RMU_CUDA(cudaMemcpyAsync(&flag, e->range_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
     RMU_CUDA(cudaStreamSynchronize(st));
-    if (flag) {
-        set_error(std::string(e->llama ? "Llama" : "Qwen3") + " forward: an activation entering a GEMM or attention left the fp16 range of the split planes "
-                  "(|x| > 65504); the encoder cannot compute this model's activations for this input");
-        return RMU_ERR_RANGE;
-    }
+    *raised = flag != 0;
+    if (flag) RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
     return RMU_OK;
+}
+
+// reads the range flag of run_qwen3's split kernels (synchronises st): RMU_ERR_RANGE when an activation left fp16's range
+static int qwen3_check_range(rmu_encoder* e, cudaStream_t st) {
+    bool raised = false;
+    const int rc = read_range(e, &raised, st);
+    if (rc != RMU_OK || !raised) return rc;
+    set_error(std::string(e->llama ? "Llama" : "Qwen3") + " forward: an activation entering a GEMM or attention left the fp16 range of the split planes "
+              "(|x| > 65504); the encoder cannot compute this model's activations for this input");
+    return RMU_ERR_RANGE;
 }
 
 // One prefill run of rmu_decoder_generate_batch over B sequences of T token rows in all (cu [B + 1]): each row's
@@ -2980,6 +3033,50 @@ static int run_batch_prefill(rmu_encoder* e, const KvView& kvv, const int32_t* i
     return rc;
 }
 
+// The host rows of one run_batch_prefill: tokens from .. T_b - 1 of each prompt b = seqs[i] (ids_h[cu_h[b] ..),
+// T_b = cu_h[b + 1] - cu_h[b]), token t at position t and cache row t + shift[i]; cu [seqs + 1] over the rows
+struct PrefillRows {
+    std::vector<int> ids, cu{0}, shift, pos;
+    int max_own = 0;
+};
+
+static PrefillRows prefill_rows(const int32_t* ids_h, const int32_t* cu_h, const std::vector<int>& seqs, int from,
+                                const std::vector<int>& shift) {
+    PrefillRows pr;
+    for (size_t i = 0; i < seqs.size(); ++i) {
+        const int b = seqs[i], n = cu_h[b + 1] - cu_h[b] - from;
+        for (int t = from; t < from + n; ++t) {
+            pr.ids.push_back(ids_h[cu_h[b] + t]);
+            pr.pos.push_back(t);
+            pr.shift.push_back(shift[i]);
+        }
+        pr.cu.push_back(pr.cu.back() + n);
+        pr.max_own = std::max(pr.max_own, n);
+    }
+    return pr;
+}
+
+// the last row of each sequence i of a prefill (cu) from e->PRE to row at[i] of last [., H] (at null: row i)
+static int gather_last(rmu_encoder* e, const std::vector<int>& cu, const int* at, float* last, cudaStream_t st) {
+    const size_t H = e->cfg.hidden;
+    for (size_t i = 0; i + 1 < cu.size(); ++i)
+        RMU_CUDA(cudaMemcpyAsync(last + (at ? at[i] : i) * H, e->PRE + (cu[i + 1] - 1) * H, H * 4, cudaMemcpyDeviceToDevice, st));
+    return RMU_OK;
+}
+
+// The prefill runs of B prompts of Tb tokens: an NF4 handle's one-token prompts one by one (on the GEMV their own
+// prefill takes), then the others together
+static std::vector<std::vector<int>> prefill_groups(const rmu_encoder* e, const std::vector<int>& Tb) {
+    std::vector<std::vector<int>> groups;
+    std::vector<int> rest;
+    for (int b = 0; b < static_cast<int>(Tb.size()); ++b) {
+        if (e->nf4 && Tb[b] == 1) groups.push_back({b});
+        else rest.push_back(b);
+    }
+    if (!rest.empty()) groups.push_back(rest);
+    return groups;
+}
+
 // the sampling settings rmu_decoder_generate and rmu_debug_sample refuse, before any CUDA call
 static int check_sampling(const std::string& fn, const rmu_sampling* s) {
     if (s->n_eos < 0 || s->n_eos > RMU_MAX_EOS || !(s->repetition_penalty > 0.f) || !std::isfinite(s->repetition_penalty)) {
@@ -2997,6 +3094,25 @@ static int check_sampling(const std::string& fn, const rmu_sampling* s) {
         }
     }
     return RMU_OK;
+}
+
+static SampleArgs sample_args(const rmu_sampling& s) {
+    return SampleArgs{s.do_sample ? 1 : 0, s.top_k, s.temperature, s.top_p, s.repetition_penalty};
+}
+
+// a prompt's presence bits: out [words] has bit i set for each id i among ids [n]
+static void prompt_bits(const int32_t* ids, int n, size_t words, unsigned* out) {
+    std::fill(out, out + words, 0u);
+    for (int i = 0; i < n; ++i) out[ids[i] >> 5] |= 1u << (ids[i] & 31);
+}
+
+// a reply's status after its n-th token t, for a prompt of T tokens: RMU_GEN_LIVE, or why it stops
+static int stop_status(const rmu_sampling& s, int t, int n, int max_new, int T, int max_pos) {
+    for (int i = 0; i < s.n_eos; ++i)
+        if (t == s.eos_ids[i]) return RMU_GEN_EOS;
+    if (n == max_new) return RMU_GEN_MAX_NEW;
+    if (T + n >= max_pos) return RMU_GEN_MAX_POS;
+    return RMU_GEN_LIVE;
 }
 
 // One batched decode step's layers (rmu_decoder_generate_batch's steps, a prompt-lookup verify pass): M token rows
@@ -3050,55 +3166,43 @@ using Drafter = std::function<int(const std::vector<int32_t>& seq, int k, int32_
 static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* ids_h, int T, const rmu_sampling* s,
                          uint64_t seed, int max_new_tokens, int kmax, const Drafter& draft, int32_t* out_h, int32_t* n_out,
                          float* logits_h, int32_t* n_passes, void* stream) {
-    int rc = check_decoder(e, fn);
+    const int cu_h[2] = {0, T};
+    int rc = check_generator(e, fn);
+    if (rc == RMU_OK) rc = check_prompts(e, fn, ids_h, cu_h, 1);
+    if (rc == RMU_OK) rc = check_sampling(fn, s);
     if (rc != RMU_OK) return rc;
-    if (!e->has_lm_head) { set_error(fn + ": no LM head is attached (rmu_decoder_set_lm_head)"); return RMU_ERR_ARG; }
-    rc = check_nf4_intact(e, fn);
-    if (rc != RMU_OK) return rc;
-    const rmu_bert_config& c = e->cfg;
-    if (T >= c.max_pos) {
-        set_error(fn + ": a prompt of " + std::to_string(T) + " tokens leaves no position for a new token (max_position_embeddings " +
-                  std::to_string(c.max_pos) + ")");
-        return RMU_ERR_ARG;
-    }
-    rc = check_sampling(fn, s);
-    if (rc != RMU_OK) return rc;
-    for (int i = 0; i < T; ++i)
-        if (ids_h[i] < 0 || ids_h[i] >= c.vocab_size) { set_error(fn + ": token id out of range"); return RMU_ERR_ARG; }
     std::lock_guard<std::mutex> hg(e->host_mu);
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const rmu_bert_config& c = e->cfg;
     const int V = c.vocab_size, H = c.hidden, nh = c.heads, kv = e->qext.kv_heads, L = c.layers;
     const int cap = std::min(T + max_new_tokens, c.max_pos);
-    // the KV cache: grown when a call needs more positions
-    if (cap > e->kv_cap) {
-        e->kv_cap = 0;                                  // until grow succeeds: it may free the old cache first
-        rc = grow(e->kv_cache, static_cast<size_t>(L) * 4 * kv * cap * kQwenHD * sizeof(__half));
-        if (rc != RMU_OK) {
-            set_error(fn + ": the KV cache for " + std::to_string(cap) + " positions: " + rmu_last_error());
-            return rc;
-        }
-        e->kv_cap = cap;
-    }
-    // gen_ws: logits [R, V] | presence [words] | tokens [R, at least 4] | decode partials [R rows] and, for verify
-    // passes, presence rows [R, words] | ints: ids [R] | shift [R] (zeros); R = kmax + 1
-    const int R = kmax + 1;
-    const size_t words = (static_cast<size_t>(V) + 31) / 32, ntok = 4 * ((static_cast<size_t>(R) + 3) / 4);
-    const size_t part_f = decode_part_floats(nh, cap);
-    const size_t ws = (static_cast<size_t>(R) * V + words + ntok + R * part_f + (R > 1 ? R * words + 2 * R : 0)) * sizeof(float);
-    rc = grow(e->gen_ws, ws);
+    // gen_ws: logits [R, V] | presence [words] | tokens [R] | decode partials [R rows] and, for verify passes, presence
+    // rows [R, words] | ints: ids [R] | shift [R] (zeros); R = kmax + 1
+    const int R = kmax + 1, Rv = R > 1 ? R : 0;
+    const size_t words = (static_cast<size_t>(V) + 31) / 32, part_f = decode_part_floats(nh, cap);
+    float *logits, *part;
+    unsigned *presence, *prow;
+    int *tok, *ints;
+    auto layout = [&](void* base) {
+        Carve w(base);
+        logits = w.take<float>(static_cast<size_t>(R) * V);
+        presence = w.take<unsigned>(words);
+        tok = w.take<int>(R);
+        part = w.take<float>(R * part_f);
+        prow = w.take<unsigned>(Rv * words);
+        ints = w.take<int>(2 * Rv);
+        return w.size;
+    };
+    rc = ensure_kv(e, fn, cap);
+    if (rc == RMU_OK) rc = grow(e->gen_ws, layout(nullptr));
     if (rc == RMU_OK) rc = grow(e->d_ids, T * sizeof(int32_t), token_rows(T) * sizeof(int32_t));
     if (rc == RMU_OK && R > 1) rc = ensure_tokens(e, R, 1);
     if (rc != RMU_OK) return rc;
-    float* logits = e->gen_ws.as<float>();
-    unsigned* presence = reinterpret_cast<unsigned*>(logits + static_cast<size_t>(R) * V);
-    int* tok = reinterpret_cast<int*>(presence + words);
-    float* part = reinterpret_cast<float*>(tok + ntok);
-    unsigned* prow = reinterpret_cast<unsigned*>(part + R * part_f);
-    int* ints = reinterpret_cast<int*>(prow + R * words);
-    std::vector<unsigned> bits(words, 0u);
-    for (int i = 0; i < T; ++i) bits[ids_h[i] >> 5] |= 1u << (ids_h[i] & 31);
-    const int cu_h[2] = {0, T};
+    layout(e->gen_ws.p);
+    std::vector<unsigned> bits(words);
+    prompt_bits(ids_h, T, words, bits.data());
+    RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // gen_ws is shared by all callers
     // pageable sources: each copy has taken its bytes when it returns
     RMU_CUDA(cudaMemcpyAsync(e->d_ids.p, ids_h, T * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     RMU_CUDA(cudaMemcpyAsync(e->span_cu, cu_h, sizeof(cu_h), cudaMemcpyHostToDevice, st));
@@ -3107,7 +3211,7 @@ static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* i
     if (R > 1) RMU_CUDA(cudaMemcpyAsync(ints, hints.data(), hints.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     std::vector<int32_t> seq(ids_h, ids_h + T);          // the prompt and the tokens so far: what the drafter reads
     std::vector<float> staged(logits_h && R > 1 ? static_cast<size_t>(R) * V : 0);
-    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
+    const SampleArgs sa = sample_args(*s);
     // the prefill writes the cache; its last row's hidden state gives the first token
     rc = run_qwen3(e, e->d_ids.as<int32_t>(), e->span_cu, 1, T, T, st, false, true);
     const float* last = e->PRE + static_cast<size_t>(T - 1) * H;
@@ -3177,11 +3281,8 @@ static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* i
             if (rc != RMU_OK) break;
             RMU_CUDA(cudaMemcpyAsync(t_h.data(), tok, M * sizeof(int), cudaMemcpyDeviceToHost, st));
             ++passes;
-            if (qwen3_check_range(e, st) != RMU_OK) {      // synchronises st; a rejected draft's row may be the cause
-                RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
-                redo = true;
-                continue;
-            }
+            rc = read_range(e, &redo, st);                 // synchronises st; a rejected draft's row may be the cause
+            if (rc != RMU_OK || redo) continue;
             while (acc < M && t_h[acc - 1] == hints[acc]) ++acc;
             // the last kept row's bits are the base plus every kept token: the next base
             RMU_CUDA(cudaMemcpyAsync(presence, prow + static_cast<size_t>(acc - 1) * words, words * sizeof(unsigned),
@@ -3195,9 +3296,7 @@ static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* i
                           logits_h + static_cast<size_t>(n) * V);
             out_h[n++] = t_h[j];
             seq.push_back(t_h[j]);
-            bool eos = false;
-            for (int i = 0; i < s->n_eos; ++i) eos |= t_h[j] == s->eos_ids[i];
-            stop = eos || n == max_new_tokens || T + n >= c.max_pos;
+            stop = stop_status(*s, t_h[j], n, max_new_tokens, T, c.max_pos) != RMU_GEN_LIVE;
         }
         if (stop) break;
     }
@@ -4264,27 +4363,13 @@ int rmu_decoder_generate_batch(rmu_encoder* e, const int32_t* ids_h, const int32
         set_error(fn + ": at most " + std::to_string(RMU_MAX_GENERATE_BATCH) + " prompts per call, got " + std::to_string(B));
         return RMU_ERR_ARG;
     }
-    for (int b = 0; b < B; ++b)
-        if (cu_h[b + 1] <= cu_h[b] || cu_h[b] < 0) { set_error(fn + ": prompt " + std::to_string(b) + " is empty"); return RMU_ERR_ARG; }
-    int rc = check_decoder(e, fn);
-    if (rc != RMU_OK) return rc;
-    if (!e->has_lm_head) { set_error(fn + ": no LM head is attached (rmu_decoder_set_lm_head)"); return RMU_ERR_ARG; }
-    rc = check_nf4_intact(e, fn);
+    int rc = check_generator(e, fn);
+    if (rc == RMU_OK) rc = check_prompts(e, fn, ids_h, cu_h, B);
+    if (rc == RMU_OK) rc = check_sampling(fn, s);
     if (rc != RMU_OK) return rc;
     const rmu_bert_config& c = e->cfg;
     std::vector<int> Tb(B);
-    for (int b = 0; b < B; ++b) {
-        Tb[b] = cu_h[b + 1] - cu_h[b];
-        if (Tb[b] >= c.max_pos) {
-            set_error(fn + ": a prompt of " + std::to_string(Tb[b]) + " tokens leaves no position for a new token " +
-                      "(max_position_embeddings " + std::to_string(c.max_pos) + ")");
-            return RMU_ERR_ARG;
-        }
-    }
-    rc = check_sampling(fn, s);
-    if (rc != RMU_OK) return rc;
-    for (int i = cu_h[0]; i < cu_h[B]; ++i)
-        if (ids_h[i] < 0 || ids_h[i] >= c.vocab_size) { set_error(fn + ": token id out of range"); return RMU_ERR_ARG; }
+    for (int b = 0; b < B; ++b) Tb[b] = cu_h[b + 1] - cu_h[b];
     const int32_t* prompt0 = ids_h + cu_h[0];
     int P = B > 1 ? Tb[0] - 1 : 0;
     for (int b = 1; b < B; ++b) {
@@ -4303,84 +4388,63 @@ int rmu_decoder_generate_batch(rmu_encoder* e, const int32_t* ids_h, const int32
     std::lock_guard<std::mutex> hg(e->host_mu);
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int V = c.vocab_size, H = c.hidden, nh = c.heads, kv = e->qext.kv_heads, L = c.layers;
-    const int cap = P + B * R;
-    if (cap > e->kv_cap) {
-        e->kv_cap = 0;                                  // until grow succeeds: it may free the old cache first
-        rc = grow(e->kv_cache, static_cast<size_t>(L) * 4 * kv * cap * kQwenHD * sizeof(__half));
-        if (rc != RMU_OK) {
-            set_error(fn + ": the KV cache for " + std::to_string(cap) + " positions: " + rmu_last_error());
-            return rc;
-        }
-        e->kv_cap = cap;
-    }
-    // prefill groups: the prefix, the one-token prompts of an NF4 handle one by one, the other suffixes together
-    std::vector<int> group, solo;
-    for (int b = 0; b < B; ++b) (e->nf4 && Tb[b] == 1 ? solo : group).push_back(b);
-    int suffix_rows = 0;
-    for (int b : group) suffix_rows += Tb[b] - P;
+    const int V = c.vocab_size, nh = c.heads;
+    // prefill runs: the prefix (prompt 0's first P tokens), then prefill_groups from token P of each prompt
+    const int cu_prefix[2] = {cu_h[0], cu_h[0] + P};
+    const std::vector<std::vector<int>> groups = prefill_groups(e, Tb);
+    int suffix_rows = 0;                                 // the last group's run is the longest: a solo run has one row
+    for (int b : groups.back()) suffix_rows += Tb[b] - P;
     const int rows_most = std::max({P, suffix_rows, B});
-    // batch_ws: logits [B, V] | last hidden rows [B, H] | decode partials | presence [B, words] | seeds [B] | tokens
-    // [B] | ints (ids, cu, shift of a prefill run; ids, shift, seq of a step)
+    // gen_ws: logits [B, V] | last hidden rows [B, H] | decode partials | presence [B, words] | seeds [B] | tokens [B] |
+    // ints (ids, cu, shift of a prefill run; ids, shift, seq of a step)
     const size_t words = (static_cast<size_t>(V) + 31) / 32;
-    auto al = [](size_t bytes) { return (bytes + 255) / 256 * 256; };
-    const size_t o_last = al(static_cast<size_t>(B) * V * 4), o_part = o_last + al(static_cast<size_t>(B) * H * 4);
-    const size_t o_pres = o_part + al(static_cast<size_t>(B) * decode_part_floats(nh, most) * 4);
-    const size_t o_seed = o_pres + al(static_cast<size_t>(B) * words * 4), o_tok = o_seed + al(static_cast<size_t>(B) * 8);
-    const size_t o_int = o_tok + al(static_cast<size_t>(B) * 4);
-    const size_t n_int = 2 * static_cast<size_t>(rows_most) + B + 1 + 3 * static_cast<size_t>(B);
-    rc = grow(e->batch_ws, o_int + n_int * 4);
+    float *logits, *last, *part;
+    unsigned* presence;
+    unsigned long long* seeds;
+    int *tok, *ints;
+    auto layout = [&](void* base) {
+        Carve w(base);
+        logits = w.take<float>(static_cast<size_t>(B) * V);
+        last = w.take<float>(static_cast<size_t>(B) * c.hidden);
+        part = w.take<float>(B * decode_part_floats(nh, most));
+        presence = w.take<unsigned>(B * words);
+        seeds = w.take<unsigned long long>(B);
+        tok = w.take<int>(B);
+        ints = w.take<int>(2 * static_cast<size_t>(rows_most) + B + 1 + 3 * static_cast<size_t>(B));
+        return w.size;
+    };
+    rc = ensure_kv(e, fn, P + B * R);
+    if (rc == RMU_OK) rc = grow(e->gen_ws, layout(nullptr));
     if (rc == RMU_OK) rc = ensure_tokens(e, rows_most, B);
     if (rc != RMU_OK) return rc;
-    char* base = e->batch_ws.as<char>();
-    float* logits = reinterpret_cast<float*>(base);
-    float* last = reinterpret_cast<float*>(base + o_last);
-    float* part = reinterpret_cast<float*>(base + o_part);
-    unsigned* presence = reinterpret_cast<unsigned*>(base + o_pres);
-    unsigned long long* seeds = reinterpret_cast<unsigned long long*>(base + o_seed);
-    int* tok = reinterpret_cast<int*>(base + o_tok);
-    int* ints = reinterpret_cast<int*>(base + o_int);
-    std::vector<unsigned> bits(static_cast<size_t>(B) * words, 0u);
-    for (int b = 0; b < B; ++b)
-        for (int i = cu_h[b]; i < cu_h[b + 1]; ++i) bits[b * words + (ids_h[i] >> 5)] |= 1u << (ids_h[i] & 31);
-    RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace is shared by all callers
+    layout(e->gen_ws.p);
+    std::vector<unsigned> bits(static_cast<size_t>(B) * words);
+    for (int b = 0; b < B; ++b) prompt_bits(ids_h + cu_h[b], Tb[b], words, bits.data() + b * words);
+    RMU_CUDA(cudaStreamWaitEvent(st, e->ws_done, 0));    // the activation workspace and gen_ws are shared by all callers
     RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
     // pageable sources: each copy has taken its bytes when it returns
     RMU_CUDA(cudaMemcpyAsync(presence, bits.data(), bits.size() * 4, cudaMemcpyHostToDevice, st));
     RMU_CUDA(cudaMemcpyAsync(seeds, seeds_h, static_cast<size_t>(B) * 8, cudaMemcpyHostToDevice, st));
-    // one prefill run over the sequences `seqs` from token `from` of each: ids | cu | shift into ints, positions into
-    // POSI; the last row of each goes to last[b] (gather)
-    auto prefill = [&](const std::vector<int>& seqs, int from, int p0, bool gather, bool gemv) -> int {
-        std::vector<int> hid, hcu{0}, hshift, hpos;
-        int max_own = 0;
-        for (int b : seqs) {
-            const int n = (gather ? Tb[b] : p0) - from;
-            for (int t = 0; t < n; ++t) {
-                hid.push_back(ids_h[cu_h[b] + from + t]);
-                hpos.push_back(from + t);
-                hshift.push_back(gather ? b * R : 0);
-            }
-            hcu.push_back(hcu.back() + n);
-            max_own = std::max(max_own, n);
-        }
-        const int n = hcu.back(), nb = static_cast<int>(seqs.size());
-        std::vector<int> packed(hid);
-        packed.insert(packed.end(), hcu.begin(), hcu.end());
-        packed.insert(packed.end(), hshift.begin(), hshift.end());
+    // one prefill run: ids | cu | shift into ints, positions into POSI
+    auto prefill = [&](const PrefillRows& pr, int P0, bool gemv) -> int {
+        const int n = pr.cu.back(), nb = static_cast<int>(pr.cu.size()) - 1;
+        std::vector<int> packed(pr.ids);
+        packed.insert(packed.end(), pr.cu.begin(), pr.cu.end());
+        packed.insert(packed.end(), pr.shift.begin(), pr.shift.end());
         RMU_CUDA(cudaMemcpyAsync(ints, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice, st));
-        RMU_CUDA(cudaMemcpyAsync(e->POSI, hpos.data(), hpos.size() * 4, cudaMemcpyHostToDevice, st));
-        int r = run_batch_prefill(e, handle_kv(e), ints, ints + n, ints + n + nb + 1, nb, n, max_own, gather ? P : 0, gemv, st);
-        for (int i = 0; i < nb && r == RMU_OK && gather; ++i)
-            RMU_CUDA(cudaMemcpyAsync(last + static_cast<size_t>(seqs[i]) * H, e->PRE + static_cast<size_t>(hcu[i + 1] - 1) * H,
-                                     static_cast<size_t>(H) * 4, cudaMemcpyDeviceToDevice, st));
-        return r;
+        RMU_CUDA(cudaMemcpyAsync(e->POSI, pr.pos.data(), pr.pos.size() * 4, cudaMemcpyHostToDevice, st));
+        return run_batch_prefill(e, handle_kv(e), ints, ints + n, ints + n + nb + 1, nb, n, pr.max_own, P0, gemv, st);
     };
-    if (P > 0) rc = prefill({0}, 0, P, false, false);
-    for (int b : solo)
-        if (rc == RMU_OK) rc = prefill({b}, 0, 0, true, true);
-    if (rc == RMU_OK && !group.empty()) rc = prefill(group, P, 0, true, false);
+    if (P > 0) rc = prefill(prefill_rows(ids_h, cu_prefix, {0}, 0, {0}), 0, false);
+    for (const auto& g : groups) {
+        std::vector<int> shift;
+        for (int b : g) shift.push_back(b * R);
+        const PrefillRows pr = prefill_rows(ids_h, cu_h, g, P, shift);
+        if (rc == RMU_OK) rc = prefill(pr, P, e->nf4 && g.size() == 1 && Tb[g[0]] == 1);
+        if (rc == RMU_OK) rc = gather_last(e, pr.cu, g.data(), last, st);
+    }
 
-    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
+    const SampleArgs sa = sample_args(*s);
     std::vector<int> live(B), n_b(B, 0), last_tok(B, 0);
     for (int b = 0; b < B; ++b) live[b] = b;
     const float* x_last = last;
@@ -4424,9 +4488,7 @@ int rmu_decoder_generate_batch(rmu_encoder* e, const int32_t* ids_h, const int32
             const int b = live[r];
             out_h[static_cast<size_t>(b) * max_new_tokens + n_b[b]++] = t_h[r];
             last_tok[b] = t_h[r];
-            bool eos = false;
-            for (int i = 0; i < s->n_eos; ++i) eos |= t_h[r] == s->eos_ids[i];
-            if (!(eos || n_b[b] == max_new_tokens || Tb[b] + n_b[b] >= c.max_pos)) next.push_back(b);
+            if (stop_status(*s, t_h[r], n_b[b], max_new_tokens, Tb[b], c.max_pos) == RMU_GEN_LIVE) next.push_back(b);
         }
         live.swap(next);
     }
@@ -4477,10 +4539,12 @@ struct rmu_gen_session {
     rmu_encoder* e = nullptr;
     KvRegions reg;
     void* kv = nullptr;                           // [L][4][kv_heads][reg.cap][128] halves
-    // persistent device state, one entry per row slot: presence bits [16, words] | seeds [16] | settings [16] |
-    // Philox steps [16]
+    // persistent device state, one entry per row slot: presence bits [16, words] (at state) | seeds [16] | settings
+    // [16] | Philox steps [16]
     void* state = nullptr;
-    size_t words = 0, o_seed = 0, o_args = 0, o_steps = 0;
+    size_t words = 0;
+    unsigned long long *seeds = nullptr, *steps = nullptr;
+    SampleArgs* args = nullptr;
     DevBuf ws;                                    // one call's scratch: logits, last rows, partials, tokens, ints
     struct Row {
         bool live = false;
@@ -4526,66 +4590,16 @@ int session_grow(rmu_gen_session* S, int cap, cudaStream_t st) {
     return RMU_OK;
 }
 
-// one call's scratch: logits [16, V] | last hidden rows [16, H] | decode partials | presence backup [16, words] |
-// tokens [16] | ints [n_int].  The partials are sized for 16 rows over the longest region in the session, and the
-// buffer grows with half again as much headroom, so a reply's steps do not re-grow it as its keys pass each split.
-struct SessionWs {
-    float *logits, *last, *part;
-    unsigned* backup;
-    int *tok, *ints;
-};
-
-int session_ws(rmu_gen_session* S, int M, size_t part_floats, size_t n_int, SessionWs* w) {
-    const rmu_bert_config& c = S->e->cfg;
-    auto al = [](size_t bytes) { return (bytes + 255) / 256 * 256; };
-    const size_t R = std::max(M, RMU_MAX_GENERATE_BATCH);
-    int longest = 1;
-    for (const auto& r : S->reg.used) longest = std::max(longest, r.second);
-    part_floats = std::max(part_floats, RMU_MAX_GENERATE_BATCH * decode_part_floats(c.heads, longest));
-    const size_t o_last = al(R * c.vocab_size * 4);
-    const size_t o_part = o_last + al(R * c.hidden * 4);
-    const size_t o_back = o_part + al(part_floats * 4);
-    const size_t o_tok = o_back + al(RMU_MAX_GENERATE_BATCH * S->words * 4);
-    const size_t o_int = o_tok + al(RMU_MAX_GENERATE_BATCH * 4);
-    const size_t need = o_int + n_int * 4;
-    const int rc = grow(S->ws, need, need + need / 2);
-    if (rc != RMU_OK) return rc;
-    char* b = S->ws.as<char>();
-    *w = SessionWs{reinterpret_cast<float*>(b), reinterpret_cast<float*>(b + o_last), reinterpret_cast<float*>(b + o_part),
-                   reinterpret_cast<unsigned*>(b + o_back), reinterpret_cast<int*>(b + o_tok),
-                   reinterpret_cast<int*>(b + o_int)};
-    return RMU_OK;
-}
-
 // the sampler over M rows whose slots are seq (device [M]), each with its slot's bits, seed, settings and step
 int session_sample(rmu_gen_session* S, float* logits, int M, const int* seq, int* tok, cudaStream_t st) {
-    const char* st8 = static_cast<const char*>(S->state);
     SampleRows sr;
     sr.seq = seq;
-    sr.seeds = reinterpret_cast<const unsigned long long*>(st8 + S->o_seed);
+    sr.seeds = S->seeds;
     sr.words = S->words;
-    sr.args = reinterpret_cast<const SampleArgs*>(st8 + S->o_args);
-    sr.steps = reinterpret_cast<const unsigned long long*>(st8 + S->o_steps);
+    sr.args = S->args;
+    sr.steps = S->steps;
     return launch_sample(logits, S->e->cfg.vocab_size, static_cast<unsigned*>(S->state), SampleArgs{}, -1.f, 0ull, 0ull,
                          tok, st, M, sr);
-}
-
-// upload the Philox step of every slot (its tokens so far)
-int session_upload_steps(rmu_gen_session* S, cudaStream_t st) {
-    unsigned long long h[RMU_MAX_GENERATE_BATCH];
-    for (int i = 0; i < RMU_MAX_GENERATE_BATCH; ++i) h[i] = static_cast<unsigned long long>(S->rows[i].n);
-    RMU_CUDA(cudaMemcpyAsync(static_cast<char*>(S->state) + S->o_steps, h, sizeof(h), cudaMemcpyHostToDevice, st));
-    return RMU_OK;
-}
-
-// whether the fp16 range flag is raised, cleared again when it is (synchronises st)
-int session_read_range(rmu_encoder* e, bool* raised, cudaStream_t st) {
-    int flag = 0;
-    RMU_CUDA(cudaMemcpyAsync(&flag, e->range_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-    RMU_CUDA(cudaStreamSynchronize(st));
-    *raised = flag != 0;
-    if (flag) RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
-    return RMU_OK;
 }
 
 // One pass over the slots `slots` (row r = slots[r]): with T null a decode step, each row feeding its last token at
@@ -4596,84 +4610,95 @@ int session_pass(rmu_gen_session* S, const std::vector<int>& slots, const int32_
                  const std::vector<int>* req, bool gemv, float* logits_h, int* t_h, bool* raised, cudaStream_t st) {
     rmu_encoder* e = S->e;
     const rmu_bert_config& c = e->cfg;
-    const int M = static_cast<int>(slots.size()), V = c.vocab_size, H = c.hidden;
-    std::vector<int> hid, hcu{0}, hshift, hpos;
-    int maxn = 0, max_own = 0;
-    for (int r = 0; r < M; ++r) {
+    const int M = static_cast<int>(slots.size()), V = c.vocab_size;
+    std::vector<int> base;
+    for (int q : slots) base.push_back(S->rows[q].base);
+    PrefillRows pr;                               // a decode step's rows in the same fields, with cu [0]
+    int maxn = 0;
+    if (req) pr = prefill_rows(ids_h, cu_h, *req, 0, base);
+    for (int r = 0; r < M && !req; ++r) {
         const rmu_gen_session::Row& w = S->rows[slots[r]];
-        if (req) {
-            const int b = (*req)[r], T = cu_h[b + 1] - cu_h[b];
-            for (int t = 0; t < T; ++t) {
-                hid.push_back(ids_h[cu_h[b] + t]);
-                hpos.push_back(t);
-                hshift.push_back(w.base);
-            }
-            hcu.push_back(hcu.back() + T);
-            max_own = std::max(max_own, T);
-        } else {
-            hid.push_back(w.last);
-            hpos.push_back(w.T + w.n - 1);
-            hshift.push_back(w.base);
-            maxn = std::max(maxn, w.T + w.n);
-        }
+        pr.ids.push_back(w.last);
+        pr.pos.push_back(w.T + w.n - 1);
+        pr.shift.push_back(base[r]);
+        maxn = std::max(maxn, w.T + w.n);
     }
-    const int rows = static_cast<int>(hid.size());
-    std::vector<int> packed(hid);
-    packed.insert(packed.end(), hshift.begin(), hshift.end());
+    const int rows = static_cast<int>(pr.ids.size());
+    std::vector<int> packed(pr.ids);
+    packed.insert(packed.end(), pr.shift.begin(), pr.shift.end());
     packed.insert(packed.end(), slots.begin(), slots.end());
-    packed.insert(packed.end(), hcu.begin(), hcu.end());
-    int* seq_off = nullptr;
-    SessionWs w;
-    const size_t part = req ? 0 : static_cast<size_t>(M) * decode_part_floats(c.heads, maxn);
-    int rc = session_ws(S, M, part, packed.size(), &w);
+    packed.insert(packed.end(), pr.cu.begin(), pr.cu.end());
+    // S->ws: logits [16, V] | last hidden rows [16, H] | decode partials | presence backup [16, words] | tokens [16] |
+    // ints (packed).  The partials are sized for 16 rows over the longest region in the session, and the buffer grows
+    // with half again as much headroom, so a reply's steps do not re-grow it as its keys pass each split.
+    const size_t R = std::max(M, RMU_MAX_GENERATE_BATCH);
+    int longest = 1;
+    for (const auto& u : S->reg.used) longest = std::max(longest, u.second);
+    const size_t part_f = std::max(req ? 0 : M * decode_part_floats(c.heads, maxn),
+                                   RMU_MAX_GENERATE_BATCH * decode_part_floats(c.heads, longest));
+    float *logits, *last, *part;
+    unsigned* backup;
+    int *tok, *ints;
+    auto layout = [&](void* p) {
+        Carve b(p);
+        logits = b.take<float>(R * V);
+        last = b.take<float>(R * c.hidden);
+        part = b.take<float>(part_f);
+        backup = b.take<unsigned>(RMU_MAX_GENERATE_BATCH * S->words);
+        tok = b.take<int>(RMU_MAX_GENERATE_BATCH);
+        ints = b.take<int>(packed.size());
+        return b.size;
+    };
+    const size_t need = layout(nullptr);
+    int rc = grow(S->ws, need, need + need / 2);
     if (rc == RMU_OK) rc = ensure_tokens(e, rows, M);
     if (rc != RMU_OK) return rc;
-    int* ids = w.ints;
-    int* shift = ids + rows;
-    seq_off = shift + rows;
+    layout(S->ws.p);
+    int* shift = ints + rows;
+    int* seq_off = shift + rows;
     int* cu = seq_off + M;
     RMU_CUDA(cudaMemsetAsync(e->range_flag, 0, sizeof(int), st));
     // pageable sources: each copy has taken its bytes when it returns
-    RMU_CUDA(cudaMemcpyAsync(w.ints, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice, st));
-    RMU_CUDA(cudaMemcpyAsync(e->POSI, hpos.data(), hpos.size() * 4, cudaMemcpyHostToDevice, st));
-    rc = session_upload_steps(S, st);
-    if (rc != RMU_OK) return rc;
-    RMU_CUDA(cudaMemcpyAsync(w.backup, S->state, RMU_MAX_GENERATE_BATCH * S->words * 4, cudaMemcpyDeviceToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(ints, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(e->POSI, pr.pos.data(), pr.pos.size() * 4, cudaMemcpyHostToDevice, st));
+    unsigned long long steps[RMU_MAX_GENERATE_BATCH];             // every slot's Philox step: its tokens so far
+    for (int i = 0; i < RMU_MAX_GENERATE_BATCH; ++i) steps[i] = static_cast<unsigned long long>(S->rows[i].n);
+    RMU_CUDA(cudaMemcpyAsync(S->steps, steps, sizeof(steps), cudaMemcpyHostToDevice, st));
+    RMU_CUDA(cudaMemcpyAsync(backup, S->state, RMU_MAX_GENERATE_BATCH * S->words * 4, cudaMemcpyDeviceToDevice, st));
     const KvView kvv = session_kv(S);
     const float* x = e->PRE;
     if (req) {
-        rc = run_batch_prefill(e, kvv, ids, cu, shift, M, rows, max_own, 0, gemv, st);
-        for (int r = 0; r < M && rc == RMU_OK; ++r)
-            RMU_CUDA(cudaMemcpyAsync(w.last + static_cast<size_t>(r) * H, e->PRE + static_cast<size_t>(hcu[r + 1] - 1) * H,
-                                     static_cast<size_t>(H) * 4, cudaMemcpyDeviceToDevice, st));
-        x = w.last;
+        rc = run_batch_prefill(e, kvv, ints, cu, shift, M, rows, pr.max_own, 0, gemv, st);
+        if (rc == RMU_OK) rc = gather_last(e, pr.cu, nullptr, last, st);
+        x = last;
     } else {
-        rc = run_decode_rows(e, kvv, ids, M, shift, 0, maxn, w.part, st);
+        rc = run_decode_rows(e, kvv, ints, M, shift, 0, maxn, part, st);
     }
-    if (rc == RMU_OK) rc = run_lm_head(e, x, M, w.logits, st);
+    if (rc == RMU_OK) rc = run_lm_head(e, x, M, logits, st);
     if (rc == RMU_OK && logits_h)
-        RMU_CUDA(cudaMemcpyAsync(logits_h, w.logits, static_cast<size_t>(M) * V * sizeof(float), cudaMemcpyDeviceToHost, st));
-    if (rc == RMU_OK) rc = session_sample(S, w.logits, M, seq_off, w.tok, st);
+        RMU_CUDA(cudaMemcpyAsync(logits_h, logits, static_cast<size_t>(M) * V * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (rc == RMU_OK) rc = session_sample(S, logits, M, seq_off, tok, st);
     if (rc != RMU_OK) return rc;
-    RMU_CUDA(cudaMemcpyAsync(t_h, w.tok, static_cast<size_t>(M) * sizeof(int), cudaMemcpyDeviceToHost, st));
-    rc = session_read_range(e, raised, st);       // synchronises st
+    RMU_CUDA(cudaMemcpyAsync(t_h, tok, static_cast<size_t>(M) * sizeof(int), cudaMemcpyDeviceToHost, st));
+    rc = read_range(e, raised, st);               // synchronises st
     if (rc == RMU_OK && *raised)
-        RMU_CUDA(cudaMemcpyAsync(S->state, w.backup, RMU_MAX_GENERATE_BATCH * S->words * 4, cudaMemcpyDeviceToDevice, st));
+        RMU_CUDA(cudaMemcpyAsync(S->state, backup, RMU_MAX_GENERATE_BATCH * S->words * 4, cudaMemcpyDeviceToDevice, st));
     return rc;
-}
-
-// a row's status after its n-th token t: live, or why it stopped (rmu_decoder_generate's rules)
-int row_status(const rmu_gen_session::Row& w, int t, int max_pos) {
-    for (int i = 0; i < w.s.n_eos; ++i)
-        if (t == w.s.eos_ids[i]) return RMU_GEN_EOS;
-    if (w.n == w.max_new) return RMU_GEN_MAX_NEW;
-    if (w.T + w.n >= max_pos) return RMU_GEN_MAX_POS;
-    return RMU_GEN_LIVE;
 }
 
 void release_row(rmu_gen_session* S, int slot) {
     S->reg.used.erase(S->rows[slot].base);
     S->rows[slot].live = false;
+}
+
+// the row in slot q after a pass gave it token t, or err when its own redo raised the range flag: its status, the row
+// released when it stops
+int finish_row(rmu_gen_session* S, int q, int t, int err) {
+    rmu_gen_session::Row& w = S->rows[q];
+    w.last = t;
+    const int status = err != RMU_OK ? err : stop_status(w.s, t, ++w.n, w.max_new, w.T, S->e->cfg.max_pos);
+    if (status != RMU_GEN_LIVE) release_row(S, q);
+    return status;
 }
 
 // waits on the handle's workspace and the session's last use on st
@@ -4704,12 +4729,18 @@ int rmu_decoder_session_create(rmu_encoder* e, rmu_gen_session** out) {
     rmu_gen_session* S = new rmu_gen_session();
     S->e = e;
     S->words = (static_cast<size_t>(e->cfg.vocab_size) + 31) / 32;
-    S->o_seed = (RMU_MAX_GENERATE_BATCH * S->words * 4 + 255) / 256 * 256;
-    S->o_args = S->o_seed + RMU_MAX_GENERATE_BATCH * 8;
-    S->o_steps = S->o_args + (RMU_MAX_GENERATE_BATCH * sizeof(SampleArgs) + 7) / 8 * 8;
-    const size_t bytes = S->o_steps + RMU_MAX_GENERATE_BATCH * 8;
+    auto layout = [S](void* base) {
+        Carve b(base);
+        b.take<unsigned>(RMU_MAX_GENERATE_BATCH * S->words);
+        S->seeds = b.take<unsigned long long>(RMU_MAX_GENERATE_BATCH);
+        S->args = b.take<SampleArgs>(RMU_MAX_GENERATE_BATCH);
+        S->steps = b.take<unsigned long long>(RMU_MAX_GENERATE_BATCH);
+        return b.size;
+    };
+    const size_t bytes = layout(nullptr);
     cudaError_t err = cudaSetDevice(e->device);
     if (err == cudaSuccess) err = cudaMalloc(&S->state, bytes);
+    if (err == cudaSuccess) layout(S->state);
     if (err == cudaSuccess) err = cudaEventCreateWithFlags(&S->done, cudaEventDisableTiming);
     if (err == cudaSuccess) err = cudaMemset(S->state, 0, bytes);
     if (err != cudaSuccess) {
@@ -4747,26 +4778,16 @@ int rmu_decoder_session_add(rmu_gen_session* S, const int32_t* ids_h, const int3
         return RMU_ERR_ARG;
     }
     rmu_encoder* e = S->e;
-    int rc = check_decoder(e, fn);
-    if (rc != RMU_OK) return rc;
-    if (!e->has_lm_head) { set_error(fn + ": no LM head is attached (rmu_decoder_set_lm_head)"); return RMU_ERR_ARG; }
-    rc = check_nf4_intact(e, fn);
+    int rc = check_generator(e, fn);
+    if (rc == RMU_OK) rc = check_prompts(e, fn, ids_h, cu_h, B);
     if (rc != RMU_OK) return rc;
     const rmu_bert_config& c = e->cfg;
     std::vector<int> Tb(B), nrows(B);
     for (int b = 0; b < B; ++b) {
-        if (cu_h[b + 1] <= cu_h[b] || cu_h[b] < 0) { set_error(fn + ": prompt " + std::to_string(b) + " is empty"); return RMU_ERR_ARG; }
         if (max_new_h[b] < 1) { set_error(fn + ": max_new_tokens must be at least 1"); return RMU_ERR_ARG; }
-        Tb[b] = cu_h[b + 1] - cu_h[b];
-        if (Tb[b] >= c.max_pos) {
-            set_error(fn + ": a prompt of " + std::to_string(Tb[b]) + " tokens leaves no position for a new token " +
-                      "(max_position_embeddings " + std::to_string(c.max_pos) + ")");
-            return RMU_ERR_ARG;
-        }
         rc = check_sampling(fn, s_h + b);
         if (rc != RMU_OK) return rc;
-        for (int i = cu_h[b]; i < cu_h[b + 1]; ++i)
-            if (ids_h[i] < 0 || ids_h[i] >= c.vocab_size) { set_error(fn + ": token id out of range"); return RMU_ERR_ARG; }
+        Tb[b] = cu_h[b + 1] - cu_h[b];
         nrows[b] = static_cast<int>(std::min<int64_t>(static_cast<int64_t>(Tb[b]) + max_new_h[b], c.max_pos));
     }
     std::lock_guard<std::mutex> g(e->mu);
@@ -4814,36 +4835,24 @@ int rmu_decoder_session_add(rmu_gen_session* S, const int32_t* ids_h, const int3
     // from here on a failure releases the new rows (a grown cache stays grown)
     auto settings = [&]() -> int {
         for (int b = 0; b < B; ++b) {
-            const rmu_sampling& sb = s_h[b];
-            const SampleArgs sa{sb.do_sample ? 1 : 0, sb.top_k, sb.temperature, sb.top_p, sb.repetition_penalty};
-            const unsigned long long seed = seeds_h[b];
-            char* st8 = static_cast<char*>(S->state);
-            RMU_CUDA(cudaMemcpyAsync(st8 + S->o_seed + slots[b] * 8, &seed, 8, cudaMemcpyHostToDevice, st));
-            RMU_CUDA(cudaMemcpyAsync(st8 + S->o_args + slots[b] * sizeof(SampleArgs), &sa, sizeof(SampleArgs),
-                                     cudaMemcpyHostToDevice, st));
+            const SampleArgs sa = sample_args(s_h[b]);
+            RMU_CUDA(cudaMemcpyAsync(S->seeds + slots[b], seeds_h + b, 8, cudaMemcpyHostToDevice, st));
+            RMU_CUDA(cudaMemcpyAsync(S->args + slots[b], &sa, sizeof(SampleArgs), cudaMemcpyHostToDevice, st));
         }
         return RMU_OK;
     };
     rc = settings();
     // the prompt's presence bits of request b's slot
     auto upload_bits = [&](int b) -> int {
-        std::fill(bits.begin(), bits.end(), 0u);
-        for (int i = cu_h[b]; i < cu_h[b + 1]; ++i) bits[ids_h[i] >> 5] |= 1u << (ids_h[i] & 31);
+        prompt_bits(ids_h + cu_h[b], Tb[b], S->words, bits.data());
         RMU_CUDA(cudaMemcpyAsync(session_presence(S, slots[b]), bits.data(), S->words * 4, cudaMemcpyHostToDevice, st));
         return RMU_OK;
     };
     for (int b = 0; b < B && rc == RMU_OK; ++b) rc = upload_bits(b);
-    // prefill groups as rmu_decoder_generate_batch runs them: an NF4 handle's one-token prompts alone, on the GEMV,
-    // the others as one varlen run
+    // prefill groups as rmu_decoder_generate_batch runs them
     const int V = c.vocab_size;
     std::vector<int> t_h(B, 0), err(B, RMU_OK);
-    std::vector<std::vector<int>> groups;
-    std::vector<int> group;
-    for (int b = 0; b < B; ++b) {
-        if (e->nf4 && Tb[b] == 1) groups.push_back({b});
-        else group.push_back(b);
-    }
-    if (!group.empty()) groups.push_back(group);
+    const std::vector<std::vector<int>> groups = prefill_groups(e, Tb);
     auto run = [&](const std::vector<int>& g, bool* raised) -> int {
         std::vector<int> sl, tt(g.size());
         for (int b : g) sl.push_back(slots[b]);
@@ -4878,17 +4887,9 @@ int rmu_decoder_session_add(rmu_gen_session* S, const int32_t* ids_h, const int3
         return rc;
     }
     for (int b = 0; b < B; ++b) {
-        rmu_gen_session::Row& w = S->rows[slots[b]];
         tok_h[b] = t_h[b];
-        if (err[b] != RMU_OK) {
-            status_h[b] = err[b];
-        } else {
-            w.n = 1;
-            w.last = t_h[b];
-            status_h[b] = row_status(w, t_h[b], c.max_pos);
-        }
+        status_h[b] = finish_row(S, slots[b], t_h[b], err[b]);
         slot_h[b] = status_h[b] == RMU_GEN_LIVE ? slots[b] : -1;
-        if (status_h[b] != RMU_GEN_LIVE) release_row(S, slots[b]);
     }
     return session_end(S, st);
 }
@@ -4928,17 +4929,9 @@ int rmu_decoder_session_step(rmu_gen_session* S, int32_t* slot_h, int32_t* tok_h
         return rc;
     }
     for (int r = 0; r < M; ++r) {
-        rmu_gen_session::Row& w = S->rows[slots[r]];
         slot_h[r] = slots[r];
         tok_h[r] = t_h[r];
-        if (err[r] != RMU_OK) {
-            status_h[r] = err[r];
-        } else {
-            ++w.n;
-            w.last = t_h[r];
-            status_h[r] = row_status(w, t_h[r], e->cfg.max_pos);
-        }
-        if (status_h[r] != RMU_GEN_LIVE) release_row(S, slots[r]);
+        status_h[r] = finish_row(S, slots[r], t_h[r], err[r]);
     }
     *n_h = M;
     return session_end(S, st);
@@ -5689,7 +5682,7 @@ int rmu_debug_sample(float* logits, int V, uint32_t* presence, const rmu_samplin
     }
     const int rc = check_sampling("rmu_debug_sample", s);
     if (rc != RMU_OK) return rc;
-    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
+    const SampleArgs sa = sample_args(*s);
     return launch_sample(logits, V, presence, sa, u, 0ull, 0ull, token, static_cast<cudaStream_t>(stream));
 }
 
@@ -5701,7 +5694,7 @@ int rmu_debug_sample_rows(float* logits, int V, int B, uint32_t* presence, const
     }
     const int rc = check_sampling("rmu_debug_sample_rows", s);
     if (rc != RMU_OK) return rc;
-    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
+    const SampleArgs sa = sample_args(*s);
     SampleRows sr;
     sr.seq = seq;
     sr.seeds = reinterpret_cast<const unsigned long long*>(seeds);
@@ -5719,7 +5712,7 @@ int rmu_debug_sample_verify_rows(float* logits, int V, int M, uint32_t* presence
     int rc = check_sampling("rmu_debug_sample_verify_rows", s);
     if (rc != RMU_OK) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const SampleArgs sa{s->do_sample ? 1 : 0, s->top_k, s->temperature, s->top_p, s->repetition_penalty};
+    const SampleArgs sa = sample_args(*s);
     SampleRows sr;
     sr.words = (static_cast<size_t>(V) + 31) / 32;
     sr.row_step = true;
@@ -5741,7 +5734,7 @@ int rmu_debug_sample_session_rows(float* logits, int V, int B, uint32_t* presenc
     for (int q = 0; q < n_seq; ++q) {
         const int rc = check_sampling(fn, s_h + q);
         if (rc != RMU_OK) return rc;
-        sa[q] = SampleArgs{s_h[q].do_sample ? 1 : 0, s_h[q].top_k, s_h[q].temperature, s_h[q].top_p, s_h[q].repetition_penalty};
+        sa[q] = sample_args(s_h[q]);
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SampleArgs* d_args = nullptr;

@@ -155,11 +155,7 @@ class DecoderAttention:
         same tokens, bit for bit, in fewer model passes when the reply copies the prompt."""
         if max_new_tokens < 1:
             return []
-        eos = [int(t) for t in eos_token_ids]
-        if len(eos) > _lib.MAX_EOS:
-            raise ValueError(f"{self.name}: at most {_lib.MAX_EOS} eos ids, got {len(eos)}")
-        s = _lib.SamplingC(int(bool(do_sample)), float(temperature), float(top_p), float(repetition_penalty),
-                           int(top_k or 0), len(eos), (C.c_int32 * _lib.MAX_EOS)(*eos))
+        s = self._sampling(do_sample, temperature, top_k, top_p, repetition_penalty, eos_token_ids)
         enc = self.encoder
         if not prompt_lookup_num_tokens:
             req = decode_session.Request(ids, s, seed, max_new_tokens, name=self.name)
@@ -178,6 +174,14 @@ class DecoderAttention:
                 int(prompt_lookup_num_tokens), int(max_matching_ngram_size), out.ctypes.data, C.byref(n), None, None,
                 _lib.stream_ptr()), "rmu_decoder_generate_lookup")
         return out[:n.value].tolist()
+
+    def _sampling(self, do_sample, temperature, top_k, top_p, repetition_penalty, eos_token_ids) -> "_lib.SamplingC":
+        """the C sampling settings of ``generate`` and ``generate_batch``; more than ``_lib.MAX_EOS`` eos ids raise"""
+        eos = [int(t) for t in eos_token_ids]
+        if len(eos) > _lib.MAX_EOS:
+            raise ValueError(f"{self.name}: at most {_lib.MAX_EOS} eos ids, got {len(eos)}")
+        return _lib.SamplingC(int(bool(do_sample)), float(temperature), float(top_p), float(repetition_penalty),
+                              int(top_k or 0), len(eos), (C.c_int32 * _lib.MAX_EOS)(*eos))
 
     def _attach_lm_head(self) -> None:
         """``rmu_decoder_set_lm_head`` the first time it is needed (under ``self.lock``)"""
@@ -208,11 +212,7 @@ class DecoderAttention:
             raise ValueError(f"{self.name}: one seed per prompt, got {len(seeds)} for {len(prompts)} prompts")
         if max_new_tokens < 1 or len(prompts) == 0:
             return [[] for _ in prompts]
-        eos = [int(t) for t in eos_token_ids]
-        if len(eos) > _lib.MAX_EOS:
-            raise ValueError(f"{self.name}: at most {_lib.MAX_EOS} eos ids, got {len(eos)}")
-        s = _lib.SamplingC(int(bool(do_sample)), float(temperature), float(top_p), float(repetition_penalty),
-                           int(top_k or 0), len(eos), (C.c_int32 * _lib.MAX_EOS)(*eos))
+        s = self._sampling(do_sample, temperature, top_k, top_p, repetition_penalty, eos_token_ids)
         enc = self.encoder
         result: List[List[int]] = []
         with self.lock, enc.torch.cuda.device(enc.device):
