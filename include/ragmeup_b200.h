@@ -450,6 +450,29 @@ int rmu_decoder_generate_lookup(rmu_encoder* enc, const int32_t* ids_h, int T, c
  * is not empty; that continuation goes to out and its length is returned.  0 when nothing matches or max_len == n + 1.
  * Null pointers, n < 1, k < 1 or max_ngram < 1 return RMU_ERR_ARG. */
 int rmu_prompt_lookup_draft(const int32_t* ids, int n, int k, int max_ngram, int max_len, int32_t* out);
+/* Speculative decoding with a draft model (transformers' assistant_model): rmu_decoder_generate's tokens and logits on
+ * enc, bit for bit, on any mix of split and NF4 handles, greedy and sampled, whatever the draft computes.  The draft
+ * is another decoder handle with an LM head and the same vocab_size.  Passes run as in rmu_decoder_generate_lookup,
+ * with k drafts from the draft model: its own prefill of the prompt into its own KV cache on the first pass, then per
+ * pass the rows its cache lacks (1 or 2 in steady state) and k - 1 single-row steps, each feeding the draft before it
+ * on the device, with one synchronise per pass.  Draft j samples with the target's settings, the presence bits of the
+ * tokens so far plus drafts 1 .. j - 1, and the Philox uniform of the output index it stands for, so a draft that
+ * computes the target's logits has every draft kept.  k starts at min(num_tokens, 15) and is capped as in
+ * rmu_decoder_generate_lookup and so that no draft position reaches the draft's max_pos; RMU_ASSIST_HEURISTIC then
+ * adds 2 after a pass that kept every draft and subtracts 1 (to at least 1) after any other, within this call.
+ * num_tokens 0 runs rmu_decoder_generate's steps.  A draft pass that raises the draft's fp16 range flag clears it and
+ * proposes no drafts; it never fails the call.  n_passes (target passes after the prefill), n_drafted (drafts
+ * proposed) and n_kept (drafts emitted as tokens) are host and nullable; logits_h receives the target's logits only.
+ * Both handles are held for the whole call.  Refused before any CUDA call as rmu_decoder_generate refuses, and: a null
+ * draft, the target as its own draft, num_tokens < 0 or another schedule (RMU_ERR_ARG); a draft that is not a decoder,
+ * has no LM head or is an incomplete NF4 handle, a vocab_size that differs from the target's, or a draft on another
+ * device (RMU_ERR_ARG). */
+#define RMU_ASSIST_CONSTANT 0    /* transformers' num_assistant_tokens_schedule "constant" */
+#define RMU_ASSIST_HEURISTIC 1   /* "heuristic" / "heuristic_transient": +2 after a fully kept pass, else -1 (min 1) */
+int rmu_decoder_generate_assisted(rmu_encoder* enc, rmu_encoder* draft, const int32_t* ids_h, int T,
+                                  const rmu_sampling* s, uint64_t seed, int max_new_tokens, int num_tokens,
+                                  int schedule, int32_t* out_h, int32_t* n_out, float* logits_h, int32_t* n_passes,
+                                  int32_t* n_drafted, int32_t* n_kept, void* stream);
 /* Continuous batching: a decode session of one decoder handle (with an LM head) that outlives a call.  Requests join
  * it (rmu_decoder_session_add) and leave it (when they stop, or rmu_decoder_session_cancel) between steps; each
  * rmu_decoder_session_step runs one decode step over every live row at M = live (at most RMU_MAX_GENERATE_BATCH).

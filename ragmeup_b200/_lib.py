@@ -145,6 +145,10 @@ SIGNATURES = {
                                               C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p,
                                               C.POINTER(C.c_int32), C.c_void_p]),
     "rmu_prompt_lookup_draft": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "rmu_decoder_generate_assisted": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(SamplingC),
+                                                C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int32),
+                                                C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                                C.POINTER(C.c_int32), C.c_void_p]),
     "rmu_decoder_session_create": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "rmu_decoder_session_destroy": (None, [C.c_void_p]),
     "rmu_decoder_session_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,

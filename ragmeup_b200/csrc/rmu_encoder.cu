@@ -3141,6 +3141,28 @@ static int run_decode_rows(rmu_encoder* e, const KvView& kvv, const int* ids, in
     return rc;
 }
 
+// The single-row decode step: the token id [1] (device) at position p through every layer, its k / v into cache row
+// p of the handle's cache and its attention over keys [0, p + 1); part holds decode_part_floats(heads, p + 1) floats.
+// The row's hidden state is left in e->PRE.
+static int run_decode_step(rmu_encoder* e, const int* id, int p, float* part, cudaStream_t st) {
+    const rmu_bert_config& c = e->cfg;
+    const int nh = c.heads, kv = e->qext.kv_heads;
+    set_int_kernel<<<1, 1, 0, st>>>(e->POSI, p);
+    count_launch();
+    RMU_CHECK_LAUNCH();
+    int rc = launch_embed_rows(id, 1, c.hidden, c.vocab_size, e->word, e->PRE, st);
+    for (int l = 0; l < c.layers && rc == RMU_OK; ++l) {
+        const EncLayer& Ly = e->layers[l];
+        rc = qwen3_attention_inputs(e, Ly, 1, true, st);
+        if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, 1, nh, kv, p, e->kv_cap, kv_layer(e, l), st);
+        if (rc == RMU_OK)
+            rc = launch_attention_decode(e->QKVP.hi, e->QKVP.lo, kv_layer(e, l), nh, kv, e->kv_cap, p + 1, part, e->CTX.hi,
+                                         e->CTX.lo, st);
+        if (rc == RMU_OK) rc = qwen3_layer_tail(e, Ly, 1, true, st);
+    }
+    return rc;
+}
+
 // logits [M, V] = lm_head . (w_norm RMS(x)) for M fp32 hidden rows x [M, H]
 static int run_lm_head(rmu_encoder* e, const float* x, int M, float* logits, cudaStream_t st) {
     const rmu_bert_config& c = e->cfg;
@@ -3154,28 +3176,36 @@ static int run_lm_head(rmu_encoder* e, const float* x, int M, float* logits, cud
 
 constexpr int kMaxDrafts = RMU_MAX_GENERATE_BATCH - 1;   // a verify pass feeds at most 16 rows
 
-// a prompt-lookup drafter: up to k ids that may follow seq (the prompt and the tokens so far) -> out, their count
+// a drafter (prompt lookup, a draft model): up to k ids that may follow seq (the prompt and the tokens so far) -> out,
+// their count, or a negative error code that fails the call
 using Drafter = std::function<int(const std::vector<int32_t>& seq, int k, int32_t* out)>;
 
-// The generation loop of rmu_decoder_generate and its prompt-lookup forms (DESIGN.md, "Prompt-lookup decoding").  The
-// prefill's last row gives the first token; each later pass feeds the pending token at position p = T + n - 1 plus k
-// drafts at p + 1 .. p + k, k = 0 .. kmax.  k = 0 is the single-row step.  k >= 1 is a verify pass: run_decode_rows on
-// the k + 1 rows, row j sampling as sequential step n + j would (its own presence bits: the base plus drafts 1 .. j;
-// Philox step n + j); t_0 is kept, t_j while t_{j - 1} equals draft j.  A verify pass that raises the range flag is
-// redone as a k = 0 step at the same position, so RMU_ERR_RANGE means what it means without drafts.
-static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* ids_h, int T, const rmu_sampling* s,
-                         uint64_t seed, int max_new_tokens, int kmax, const Drafter& draft, int32_t* out_h, int32_t* n_out,
-                         float* logits_h, int32_t* n_passes, void* stream) {
+// the refusals of rmu_decoder_generate and its drafting forms, before any CUDA call
+static int check_generate(rmu_encoder* e, const std::string& fn, const int32_t* ids_h, int T, const rmu_sampling* s) {
     const int cu_h[2] = {0, T};
     int rc = check_generator(e, fn);
     if (rc == RMU_OK) rc = check_prompts(e, fn, ids_h, cu_h, 1);
     if (rc == RMU_OK) rc = check_sampling(fn, s);
-    if (rc != RMU_OK) return rc;
-    std::lock_guard<std::mutex> hg(e->host_mu);
-    std::lock_guard<std::mutex> g(e->mu);
+    return rc;
+}
+
+// The generation loop of rmu_decoder_generate and its drafting forms (DESIGN.md, "Prompt-lookup decoding").  The
+// prefill's last row gives the first token; each later pass feeds the pending token at position p = T + n - 1 plus k
+// drafts at p + 1 .. p + k, k = 0 .. kmax.  k = 0 is the single-row step.  k >= 1 is a verify pass: run_decode_rows on
+// the k + 1 rows, row j sampling as sequential step n + j would (its own presence bits: the base plus drafts 1 .. j;
+// Philox step n + j); t_0 is kept, t_j while t_{j - 1} equals draft j.  A verify pass that raises the range flag is
+// redone as a k = 0 step at the same position, so RMU_ERR_RANGE means what it means without drafts.  The caller has
+// passed check_generate and holds the handle's host_mu and mu.  n_drafted / n_kept (nullable): the drafts proposed and
+// the drafts emitted as tokens.
+static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* ids_h, int T, const rmu_sampling* s,
+                         uint64_t seed, int max_new_tokens, int kmax, const Drafter& draft, int32_t* out_h, int32_t* n_out,
+                         float* logits_h, int32_t* n_passes, void* stream, int32_t* n_drafted = nullptr,
+                         int32_t* n_kept = nullptr) {
+    const int cu_h[2] = {0, T};
+    int rc = RMU_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const rmu_bert_config& c = e->cfg;
-    const int V = c.vocab_size, H = c.hidden, nh = c.heads, kv = e->qext.kv_heads, L = c.layers;
+    const int V = c.vocab_size, H = c.hidden, nh = c.heads;
     const int cap = std::min(T + max_new_tokens, c.max_pos);
     // gen_ws: logits [R, V] | presence [words] | tokens [R] | decode partials [R rows] and, for verify passes, presence
     // rows [R, words] | ints: ids [R] | shift [R] (zeros); R = kmax + 1
@@ -3215,7 +3245,7 @@ static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* i
     // the prefill writes the cache; its last row's hidden state gives the first token
     rc = run_qwen3(e, e->d_ids.as<int32_t>(), e->span_cu, 1, T, T, st, false, true);
     const float* last = e->PRE + static_cast<size_t>(T - 1) * H;
-    int n = 0, passes = 0;
+    int n = 0, passes = 0, drafted = 0, kept = 0;
     bool redo = false;                                     // the last verify pass raised the range flag
     while (rc == RMU_OK) {
         const int p = T + n - 1;
@@ -3224,15 +3254,13 @@ static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* i
             // a pass never writes past output index max_new_tokens - 1 or position max_pos - 1
             k = std::min({kmax, max_new_tokens - 1 - n, c.max_pos - 1 - T - n});
             if (k > 0) k = draft(seq, k, hints.data() + 1);
+            if (k < 0) { rc = k; break; }
+            drafted += k;
         }
         redo = false;
         int acc = 1;                                       // tokens this pass keeps: t_h[0 .. acc)
         if (k == 0) {
             if (n > 0) {
-                // the previous token at position p through every layer, its k / v into cache row p
-                set_int_kernel<<<1, 1, 0, st>>>(e->POSI, p);
-                count_launch();
-                RMU_CHECK_LAUNCH();
                 // after a verify pass the pending token is the last kept row's, not tok[0]: it goes up through ints
                 const int* pending = tok;
                 if (kmax > 0) {
@@ -3240,16 +3268,8 @@ static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* i
                     RMU_CUDA(cudaMemcpyAsync(ints, hints.data(), sizeof(int), cudaMemcpyHostToDevice, st));
                     pending = ints;
                 }
-                rc = launch_embed_rows(pending, 1, H, V, e->word, e->PRE, st);
-                for (int l = 0; l < L && rc == RMU_OK; ++l) {
-                    const EncLayer& Ly = e->layers[l];
-                    rc = qwen3_attention_inputs(e, Ly, 1, true, st);
-                    if (rc == RMU_OK) rc = launch_kv_append(e->QKVP.hi, e->QKVP.lo, 1, nh, kv, p, e->kv_cap, kv_layer(e, l), st);
-                    if (rc == RMU_OK)
-                        rc = launch_attention_decode(e->QKVP.hi, e->QKVP.lo, kv_layer(e, l), nh, kv, e->kv_cap, p + 1, part,
-                                                     e->CTX.hi, e->CTX.lo, st);
-                    if (rc == RMU_OK) rc = qwen3_layer_tail(e, Ly, 1, true, st);
-                }
+                // the previous token at position p through every layer, its k / v into cache row p
+                rc = run_decode_step(e, pending, p, part, st);
                 last = e->PRE;
             }
             if (rc == RMU_OK) rc = run_lm_head(e, last, 1, logits, st);
@@ -3296,12 +3316,15 @@ static int generate_loop(rmu_encoder* e, const std::string& fn, const int32_t* i
                           logits_h + static_cast<size_t>(n) * V);
             out_h[n++] = t_h[j];
             seq.push_back(t_h[j]);
+            kept += j > 0;
             stop = stop_status(*s, t_h[j], n, max_new_tokens, T, c.max_pos) != RMU_GEN_LIVE;
         }
         if (stop) break;
     }
     *n_out = n;
     if (n_passes) *n_passes = passes;
+    if (n_drafted) *n_drafted = drafted;
+    if (n_kept) *n_kept = kept;
     if (rc != RMU_OK) return rc;
     RMU_CUDA(cudaEventRecord(e->ws_done, st));
     return RMU_OK;
@@ -4287,6 +4310,9 @@ int rmu_decoder_generate(rmu_encoder* e, const int32_t* ids_h, int T, const rmu_
                          int max_new_tokens, int32_t* out_h, int32_t* n_out, float* logits_h, void* stream) {
     const std::string fn("rmu_decoder_generate");
     if (!e || !ids_h || !s || !out_h || !n_out || T < 1 || max_new_tokens < 1) { set_error(fn + ": bad argument"); return RMU_ERR_ARG; }
+    const int rc = check_generate(e, fn, ids_h, T, s);
+    if (rc != RMU_OK) return rc;
+    std::scoped_lock lk(e->host_mu, e->mu);
     return generate_loop(e, fn, ids_h, T, s, seed, max_new_tokens, 0, Drafter(), out_h, n_out, logits_h, nullptr, stream);
 }
 
@@ -4315,6 +4341,9 @@ int rmu_decoder_generate_lookup(rmu_encoder* e, const int32_t* ids_h, int T, con
         set_error(fn + ": bad argument");
         return RMU_ERR_ARG;
     }
+    const int rc = check_generate(e, fn, ids_h, T, s);
+    if (rc != RMU_OK) return rc;
+    std::scoped_lock lk(e->host_mu, e->mu);
     const int max_len = T + max_new_tokens;              // transformers' max_length
     const Drafter draft = [&](const std::vector<int32_t>& seq, int k, int32_t* out) {
         return std::max(0, rmu_prompt_lookup_draft(seq.data(), static_cast<int>(seq.size()), k, max_ngram, max_len, out));
@@ -4334,6 +4363,9 @@ int rmu_debug_generate_drafts(rmu_encoder* e, const int32_t* ids_h, int T, const
     if (check_decoder(e, fn) != RMU_OK) return RMU_ERR_ARG;
     for (int i = 0; i < max_new_tokens; ++i)
         if (drafts_h[i] < 0 || drafts_h[i] >= e->cfg.vocab_size) { set_error(fn + ": draft id out of range"); return RMU_ERR_ARG; }
+    const int rc = check_generate(e, fn, ids_h, T, s);
+    if (rc != RMU_OK) return rc;
+    std::scoped_lock lk(e->host_mu, e->mu);
     // the draft at output index n: drafts_h[n .. n + k)
     const Drafter draft = [&](const std::vector<int32_t>& seq, int kk, int32_t* out) {
         std::copy(drafts_h + (seq.size() - T), drafts_h + (seq.size() - T) + kk, out);
@@ -4341,6 +4373,165 @@ int rmu_debug_generate_drafts(rmu_encoder* e, const int32_t* ids_h, int T, const
     };
     return generate_loop(e, fn, ids_h, T, s, seed, max_new_tokens, std::min(k, kMaxDrafts), draft, out_h, n_out, logits_h,
                          n_passes, stream);
+}
+
+// The draft-model drafter of rmu_decoder_generate_assisted (DESIGN.md, "Speculative decoding with a draft model").  It
+// keeps dvalid, the leading positions of seq whose k / v the draft's cache holds for the right tokens.  A call with
+// the pending token at p = |seq| - 1 (output index n = |seq| - T) runs, on the draft handle: the prompt's prefill the
+// first time (dvalid = T); catch-up rows dvalid .. p through run_decode_rows, in runs of at most kRun rows, the last
+// row's logits giving draft 1; then k - 1 single-row steps, step j feeding draft j - 1, whose id the previous sampler
+// wrote on the device.  Draft j samples with the target's settings, presence bits seq + drafts 1 .. j - 1 (the sampler
+// sets each chosen bit) and Philox(seed, n + j - 1): as the target's verify row j - 1 samples.  One synchronise at the
+// end reads the drafts and the draft's range flag; a raised flag is cleared and the pass gets no drafts.  The next
+// call sets dvalid from how many drafts seq kept, and the heuristic schedule moves k from whether all of them were.
+struct ModelDrafter {
+    static constexpr int kRun = kMaxDrafts + 1;           // catch-up rows per run_decode_rows
+    rmu_encoder* d;
+    cudaStream_t st;
+    const int32_t* ids_h;
+    int T, dcap, schedule, kcur;
+    SampleArgs sa;
+    uint64_t seed;
+    float *logits = nullptr, *part = nullptr;            // the draft's gen_ws: logits [V] | presence [words] | drafts
+    unsigned* presence = nullptr;                          // [kMaxDrafts] | decode partials [kRun rows] | ints: ids
+    int *tok = nullptr, *ints = nullptr;                   // [kRun] | shift [kRun] (zeros)
+    size_t words;
+    std::vector<unsigned> bits;                            // seq[0 .. folded)'s presence bits
+    size_t folded = 0;
+    std::vector<int32_t> last;                             // the drafts the last call proposed, at last_p + 1 ..
+    int last_p = -1, dvalid = 0;
+    bool prefilled = false;
+
+    size_t layout(void* base) {
+        Carve w(base);
+        logits = w.take<float>(d->cfg.vocab_size);
+        presence = w.take<unsigned>(words);
+        tok = w.take<int>(kMaxDrafts);
+        part = w.take<float>(kRun * decode_part_floats(d->cfg.heads, dcap));
+        ints = w.take<int>(2 * kRun);
+        return w.size;
+    }
+
+    // the draft's cache, workspace and staging for this call; then st waits for the draft's last use
+    int setup(const std::string& fn) {
+        words = (static_cast<size_t>(d->cfg.vocab_size) + 31) / 32;
+        bits.assign(words, 0u);
+        int rc = ensure_kv(d, fn, dcap);
+        if (rc == RMU_OK) rc = grow(d->gen_ws, layout(nullptr));
+        if (rc == RMU_OK) rc = grow(d->d_ids, T * sizeof(int32_t), token_rows(T) * sizeof(int32_t));
+        if (rc == RMU_OK) rc = ensure_tokens(d, std::max(T, kRun), 1);
+        if (rc != RMU_OK) return rc;
+        layout(d->gen_ws.p);
+        RMU_CUDA(cudaStreamWaitEvent(st, d->ws_done, 0));
+        RMU_CUDA(cudaMemsetAsync(ints + kRun, 0, kRun * sizeof(int), st));
+        return RMU_OK;
+    }
+
+    int operator()(const std::vector<int32_t>& seq, int k, int32_t* out) {
+        const int S = static_cast<int>(seq.size()), p = S - 1, n = S - T, V = d->cfg.vocab_size;
+        if (last_p >= 0) {
+            // chain row last_p + j fed draft j: right while seq kept the drafts before it
+            const int m = static_cast<int>(last.size());
+            int kept = 0;
+            while (kept < m && last_p + 1 + kept < S && seq[last_p + 1 + kept] == last[kept]) ++kept;
+            dvalid = last_p + 1 + std::min(kept, std::max(m - 1, 0));
+            if (schedule == RMU_ASSIST_HEURISTIC && m > 0) kcur = kept == m ? std::min(kcur + 2, kMaxDrafts) : std::max(kcur - 1, 1);
+        }
+        last_p = -1;
+        last.clear();
+        // no draft position reaches the draft's max_pos: the chain feeds positions p .. p + k - 1
+        k = std::min({k, kcur, d->cfg.max_pos - p});
+        if (k <= 0) return 0;
+        const int cu_h[2] = {0, T};
+        int rc = RMU_OK;
+        if (!prefilled) {
+            RMU_CUDA(cudaMemcpyAsync(d->d_ids.p, ids_h, T * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+            RMU_CUDA(cudaMemcpyAsync(d->span_cu, cu_h, sizeof(cu_h), cudaMemcpyHostToDevice, st));
+            rc = run_qwen3(d, d->d_ids.as<int32_t>(), d->span_cu, 1, T, T, st, false, true);
+            if (rc != RMU_OK) return rc;
+            prefilled = true;
+            dvalid = T;
+        }
+        for (; folded < seq.size(); ++folded) bits[seq[folded] >> 5] |= 1u << (seq[folded] & 31);
+        RMU_CUDA(cudaMemcpyAsync(presence, bits.data(), words * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+        // catch-up: rows min(dvalid, p) .. p (the pending row always runs: its logits give draft 1)
+        int hids[kRun], hpos[kRun], M = 0;
+        for (int r0 = std::min(dvalid, p); r0 <= p && rc == RMU_OK; r0 += M) {
+            M = std::min(kRun, p + 1 - r0);
+            for (int j = 0; j < M; ++j) { hids[j] = seq[r0 + j]; hpos[j] = r0 + j; }
+            RMU_CUDA(cudaMemcpyAsync(ints, hids, M * sizeof(int), cudaMemcpyHostToDevice, st));
+            RMU_CUDA(cudaMemcpyAsync(d->POSI, hpos, M * sizeof(int), cudaMemcpyHostToDevice, st));
+            rc = run_decode_rows(d, handle_kv(d), ints, M, ints + kRun, 0, r0 + M, part, st);
+        }
+        const float* row = d->PRE + static_cast<size_t>(M - 1) * d->cfg.hidden;
+        for (int j = 1; j <= k && rc == RMU_OK; ++j) {
+            if (j > 1) rc = run_decode_step(d, tok + j - 2, p + j - 1, part, st);
+            if (rc == RMU_OK) rc = run_lm_head(d, row, 1, logits, st);
+            if (rc == RMU_OK)
+                rc = launch_sample(logits, V, presence, sa, -1.f, seed, static_cast<unsigned long long>(n + j - 1), tok + j - 1, st);
+            row = d->PRE;
+        }
+        if (rc != RMU_OK) return rc;
+        int flag = 0;
+        RMU_CUDA(cudaMemcpyAsync(out, tok, k * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        RMU_CUDA(cudaMemcpyAsync(&flag, d->range_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+        RMU_CUDA(cudaStreamSynchronize(st));
+        last_p = p;                                        // the catch-up rows stand: dvalid >= p + 1 next call
+        if (flag) {
+            RMU_CUDA(cudaMemsetAsync(d->range_flag, 0, sizeof(int), st));
+            return 0;
+        }
+        // sample_kernel writes an id of [0, V) even from NaN logits; the target never reads one outside it regardless
+        int m = 0;
+        while (m < k && out[m] >= 0 && out[m] < V) ++m;
+        last.assign(out, out + m);
+        return m;
+    }
+};
+
+int rmu_decoder_generate_assisted(rmu_encoder* e, rmu_encoder* draft, const int32_t* ids_h, int T, const rmu_sampling* s,
+                                  uint64_t seed, int max_new_tokens, int num_tokens, int schedule, int32_t* out_h,
+                                  int32_t* n_out, float* logits_h, int32_t* n_passes, int32_t* n_drafted, int32_t* n_kept,
+                                  void* stream) {
+    const std::string fn("rmu_decoder_generate_assisted");
+    if (!e || !draft || !ids_h || !s || !out_h || !n_out || T < 1 || max_new_tokens < 1 || num_tokens < 0) {
+        set_error(fn + ": bad argument");
+        return RMU_ERR_ARG;
+    }
+    if (schedule != RMU_ASSIST_CONSTANT && schedule != RMU_ASSIST_HEURISTIC) {
+        set_error(fn + ": unknown schedule " + std::to_string(schedule) + " (RMU_ASSIST_CONSTANT or RMU_ASSIST_HEURISTIC)");
+        return RMU_ERR_ARG;
+    }
+    if (draft == e) { set_error(fn + ": the draft must be another handle than the target"); return RMU_ERR_ARG; }
+    int rc = check_generate(e, fn, ids_h, T, s);
+    if (rc == RMU_OK) rc = check_generator(draft, fn + " (draft)");
+    if (rc != RMU_OK) return rc;
+    if (draft->cfg.vocab_size != e->cfg.vocab_size) {
+        set_error(fn + ": the draft's vocab_size " + std::to_string(draft->cfg.vocab_size) + " differs from the target's " +
+                  std::to_string(e->cfg.vocab_size) + ": the two models must share a tokenizer");
+        return RMU_ERR_ARG;
+    }
+    if (draft->device != e->device) {
+        set_error(fn + ": the draft is on device " + std::to_string(draft->device) + ", the target on device " +
+                  std::to_string(e->device));
+        return RMU_ERR_ARG;
+    }
+    std::scoped_lock lk(e->host_mu, e->mu, draft->host_mu, draft->mu);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int k0 = std::min(num_tokens, kMaxDrafts);
+    ModelDrafter md{draft, st, ids_h, T, std::min(T + max_new_tokens, draft->cfg.max_pos), schedule, k0, sample_args(*s), seed};
+    if (k0 > 0) rc = md.setup(fn);
+    if (rc != RMU_OK) return rc;
+    const Drafter dr = [&](const std::vector<int32_t>& seq, int k, int32_t* out) { return md(seq, k, out); };
+    // the heuristic schedule may grow k to 15: the loop's workspace is laid out for it
+    const int kmax = k0 > 0 && schedule == RMU_ASSIST_HEURISTIC ? kMaxDrafts : k0;
+    rc = generate_loop(e, fn, ids_h, T, s, seed, max_new_tokens, kmax, dr, out_h, n_out, logits_h, n_passes, stream,
+                       n_drafted, n_kept);
+    if (k0 > 0) {
+        const cudaError_t err = cudaEventRecord(draft->ws_done, st);
+        if (rc == RMU_OK && err != cudaSuccess) { set_error(fn + ": " + cudaGetErrorString(err)); rc = RMU_ERR_CUDA; }
+    }
+    return rc;
 }
 
 // The batch layout.  P = the prompts' longest common prefix, capped so that every prompt keeps one own token (0 when

@@ -33,7 +33,7 @@ REFUSED_FIELDS = ("num_beams", "num_beam_groups", "num_return_sequences", "min_p
                   "forced_eos_token_id", "min_new_tokens", "min_length", "stop_strings", "epsilon_cutoff", "eta_cutoff",
                   "guidance_scale", "encoder_repetition_penalty", "encoder_no_repeat_ngram_size", "diversity_penalty",
                   "exponential_decay_length_penalty", "renormalize_logits", "constraints", "force_words_ids",
-                  "penalty_alpha", "watermarking_config", "top_h", "assistant_model", "dola_layers")
+                  "penalty_alpha", "watermarking_config", "top_h", "dola_layers")
 # unset fields hold None in a GenerationConfig built from scratch and False / 0 / [] in one built from a model's config:
 # these values all mean "off"
 
@@ -49,6 +49,11 @@ def resolve_settings(generation_config: Any, generate_kwargs: dict, prompt_len: 
     sampler does not compute"""
     from transformers import GenerationConfig
     gc = copy.deepcopy(generation_config) if generation_config is not None else GenerationConfig()
+    generate_kwargs = dict(generate_kwargs)
+    assistant = generate_kwargs.pop("assistant_model", None)
+    if generate_kwargs.pop("assistant_tokenizer", None) is not None:
+        raise ValueError("generate kwarg 'assistant_tokenizer' is not supported by the GPU decoder: the draft model must "
+                         "share the target's tokenizer (universal assisted decoding is not computed)")
     unused = gc.update(**generate_kwargs)
     if unused:
         raise ValueError(f"generate kwarg {sorted(unused)[0]!r} is not supported by the GPU decoder")
@@ -77,7 +82,32 @@ def resolve_settings(generation_config: Any, generate_kwargs: dict, prompt_len: 
     if not _off(lookup):
         # prompt-lookup decoding changes how many passes a reply takes, never its tokens
         out.update(prompt_lookup_num_tokens=int(lookup), max_matching_ngram_size=int(get("max_matching_ngram_size") or 2))
+    if assistant is not None:
+        out.update(assistant_settings(assistant))
     return out
+
+
+def assistant_settings(assistant: Any) -> dict:
+    """``assistant_model`` (a transformers model with ``name_or_path``, or a ``provenance.DecoderAttention``) -> the
+    draft settings ``HuggingFacePipeline`` passes on: the model itself and, as transformers reads them, the drafts per
+    pass and their schedule from the assistant's own ``generation_config`` (transformers' defaults, 20 and
+    ``"constant"``, without one).  Speculative decoding changes how many passes a reply takes, never its tokens.
+    ``assistant_confidence_threshold`` only ends drafting early, so it is accepted and not computed.  ValueError naming
+    ``assistant_model`` for anything else, and naming the setting for a count or schedule the drafter does not take."""
+    if not isinstance(assistant, provenance.DecoderAttention) and not getattr(assistant, "name_or_path", None):
+        raise ValueError(f"generation setting assistant_model = {assistant!r} is not supported by the GPU decoder: "
+                         f"pass a transformers model with name_or_path or a DecoderAttention")
+    gc = getattr(assistant, "generation_config", None)
+    num = getattr(gc, "num_assistant_tokens", None)
+    schedule = getattr(gc, "num_assistant_tokens_schedule", None)
+    num = 20 if num is None else num
+    schedule = "constant" if schedule is None else schedule
+    if isinstance(num, bool) or not isinstance(num, (int, float)) or num < 0 or int(num) != num:
+        raise ValueError(f"generation setting num_assistant_tokens = {num!r}: expected a non-negative integer")
+    if schedule not in provenance.ASSIST_SCHEDULES:
+        raise ValueError(f"generation setting num_assistant_tokens_schedule = {schedule!r} is not supported by the GPU "
+                         f"decoder (one of {tuple(provenance.ASSIST_SCHEDULES)})")
+    return dict(assistant_model=assistant, num_assistant_tokens=int(num), num_assistant_tokens_schedule=schedule)
 
 
 PROMPT_LOOKUP_ENV = "RMU_PROMPT_LOOKUP_TOKENS"
@@ -99,6 +129,39 @@ def prompt_lookup_tokens() -> int:
     return v
 
 
+ASSISTANT_ENV = "RMU_ASSISTANT_MODEL"
+
+
+def assistant_model_name() -> Optional[str]:
+    """``$RMU_ASSISTANT_MODEL``: the draft model (a snapshot name or ``synthetic:<preset>``) HuggingFacePipeline drafts
+    with when neither its generate kwargs nor its generation_config set ``assistant_model``, as
+    ``RMU_PROMPT_LOOKUP_TOKENS`` does for prompt lookup; unset or empty: none"""
+    return os.environ.get(ASSISTANT_ENV, "").strip() or None
+
+
+class _EnvAssistant:
+    """the draft model ``$RMU_ASSISTANT_MODEL`` names, as ``assistant_settings`` takes one: no generation_config, so
+    transformers' defaults apply"""
+
+    def __init__(self, name: str):
+        self.name_or_path = name
+
+
+def pipeline_settings(generation_config: Any, generate_kwargs: dict, prompt_len: int) -> dict:
+    """``resolve_settings`` with the ``.env`` keys filled in where neither the kwargs nor the generation config set
+    their field: ``RMU_PROMPT_LOOKUP_TOKENS`` and ``RMU_ASSISTANT_MODEL``.  Prompt lookup and a draft model both on,
+    from any source, raise ValueError naming both."""
+    settings = resolve_settings(generation_config, generate_kwargs, prompt_len)
+    if "prompt_lookup_num_tokens" not in settings and prompt_lookup_tokens():
+        settings.update(prompt_lookup_num_tokens=prompt_lookup_tokens(), max_matching_ngram_size=2)
+    if "assistant_model" not in settings and assistant_model_name():
+        settings.update(assistant_settings(_EnvAssistant(assistant_model_name())))
+    if "prompt_lookup_num_tokens" in settings and "assistant_model" in settings:
+        raise ValueError(f"prompt_lookup_num_tokens ({PROMPT_LOOKUP_ENV}) and assistant_model ({ASSISTANT_ENV}) are both "
+                         f"set: the GPU decoder drafts from one source per reply")
+    return settings
+
+
 class _PipelineGenerator:
     """the parts shared by both forms of HuggingFacePipeline"""
 
@@ -108,6 +171,15 @@ class _PipelineGenerator:
 
     def _decoder(self):
         return provenance._decoder(self._pipe.model)
+
+    def _assistant(self, model: Any, target: Any):
+        """the draft handle of ``model``, found as the target's is (``provenance._decoder``: the same
+        ``RMU_DECODER_WEIGHTS``, memory plan and release rule); ValueError when it is the target's own handle"""
+        draft = provenance._decoder(model)
+        if draft is target:
+            raise ValueError(f"assistant_model {getattr(model, 'name_or_path', model)!r} resolves to the target's own "
+                             f"decoder: the draft must be another model")
+        return draft
 
     def _call(self, prompt: str, seed: Optional[int] = None) -> str:
         import torch
@@ -122,12 +194,13 @@ class _PipelineGenerator:
             fwd = {k: v for k, v in pipe._forward_params.items() if k not in ("generation_config",)}
             gen_cfg = pipe._forward_params.get("generation_config", getattr(pipe, "generation_config", None) or
                                                pipe.model.generation_config)
-            settings = resolve_settings(gen_cfg, fwd, ids.shape[1])
-            if "prompt_lookup_num_tokens" not in settings and prompt_lookup_tokens():
-                settings.update(prompt_lookup_num_tokens=prompt_lookup_tokens(), max_matching_ngram_size=2)
+            settings = pipeline_settings(gen_cfg, fwd, ids.shape[1])
             if seed is None:
                 seed = int(torch.randint(0, 2 ** 63 - 1, (1,)).item())
-        new = self._decoder().generate(ids[0].tolist(), seed=seed, **settings)
+        dec = self._decoder()
+        if "assistant_model" in settings:
+            settings["assistant"] = self._assistant(settings.pop("assistant_model"), dec)
+        new = dec.generate(ids[0].tolist(), seed=seed, **settings)
         with self._lock:
             seq = torch.cat([ids[0].cpu(), torch.as_tensor(new, dtype=ids.dtype)])
             model_outputs = {"generated_sequence": seq.view(1, 1, -1), "input_ids": ids,

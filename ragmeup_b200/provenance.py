@@ -146,17 +146,28 @@ class DecoderAttention:
 
     def generate(self, ids: Sequence[int], max_new_tokens: int, do_sample: bool = False, temperature: float = 1.0,
                  top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.0, eos_token_ids=(),
-                 seed: int = 0, prompt_lookup_num_tokens: int = 0, max_matching_ngram_size: int = 2) -> List[int]:
+                 seed: int = 0, prompt_lookup_num_tokens: int = 0, max_matching_ngram_size: int = 2,
+                 assistant: Optional["DecoderAttention"] = None, num_assistant_tokens: int = 20,
+                 num_assistant_tokens_schedule: str = "constant") -> List[int]:
         """the new token ids after the prompt ``ids`` (``rmu_decoder_generate``'s tokens), the eos token included when
         one ends the run.  Concurrent calls share the handle's decode session (``decode_session``): a call joins it at
         the next step boundary, so a second caller's reply starts before the first one's ends, and each reply is bit for
         bit its solo run.  ``prompt_lookup_num_tokens`` > 0 drafts that many tokens (at most 15) per pass from earlier
         matches of the last ``max_matching_ngram_size``-gram (``rmu_decoder_generate_lookup``, one whole call): the
-        same tokens, bit for bit, in fewer model passes when the reply copies the prompt."""
+        same tokens, bit for bit, in fewer model passes when the reply copies the prompt.  ``assistant``, another
+        DecoderAttention sharing this one's vocabulary, drafts ``num_assistant_tokens`` tokens (at most 15) per pass
+        with its own model, the count moving per pass with ``num_assistant_tokens_schedule`` ``"heuristic"`` or
+        ``"heuristic_transient"`` (``rmu_decoder_generate_assisted``, one whole call): the same tokens again, bit for
+        bit, whatever the draft computes."""
+        if assistant is not None and prompt_lookup_num_tokens:
+            raise ValueError(f"{self.name}: prompt_lookup_num_tokens and assistant are both set: one drafter per reply")
         if max_new_tokens < 1:
             return []
         s = self._sampling(do_sample, temperature, top_k, top_p, repetition_penalty, eos_token_ids)
         enc = self.encoder
+        if assistant is not None:
+            return self._generate_assisted(ids, s, seed, max_new_tokens, assistant, num_assistant_tokens,
+                                           num_assistant_tokens_schedule)
         if not prompt_lookup_num_tokens:
             req = decode_session.Request(ids, s, seed, max_new_tokens, name=self.name)
             with enc.torch.cuda.device(enc.device):
@@ -173,6 +184,31 @@ class DecoderAttention:
                 enc._h, prompt.ctypes.data, len(prompt), C.byref(s), int(seed) & (2 ** 64 - 1), int(max_new_tokens),
                 int(prompt_lookup_num_tokens), int(max_matching_ngram_size), out.ctypes.data, C.byref(n), None, None,
                 _lib.stream_ptr()), "rmu_decoder_generate_lookup")
+        return out[:n.value].tolist()
+
+    def _generate_assisted(self, ids, s, seed, max_new_tokens, assistant, num_tokens, schedule) -> List[int]:
+        """``generate`` with the draft model ``assistant``: each LM head is attached under its own handle's lock, then
+        the C call (which holds both handles) runs under neither Python lock, so two calls with swapped roles cannot
+        deadlock"""
+        if not isinstance(assistant, DecoderAttention):
+            raise ValueError(f"{self.name}: assistant must be a DecoderAttention, got {type(assistant).__name__}")
+        if assistant is self:
+            raise ValueError(f"{self.name}: assistant is the target's own decoder: the draft must be another handle")
+        if schedule not in ASSIST_SCHEDULES:
+            raise ValueError(f"{self.name}: num_assistant_tokens_schedule must be one of {tuple(ASSIST_SCHEDULES)}, "
+                             f"got {schedule!r}")
+        for dec in (self, assistant):
+            with dec.lock, dec.encoder.torch.cuda.device(dec.encoder.device):
+                dec._attach_lm_head()
+        enc = self.encoder
+        prompt = np.ascontiguousarray(list(ids), dtype=np.int32)
+        out = np.zeros(int(max_new_tokens), dtype=np.int32)
+        n = C.c_int32(0)
+        with enc.torch.cuda.device(enc.device):
+            enc._check(_lib.lib().rmu_decoder_generate_assisted(
+                enc._h, assistant.encoder._h, prompt.ctypes.data, len(prompt), C.byref(s), int(seed) & (2 ** 64 - 1),
+                int(max_new_tokens), int(num_tokens), ASSIST_SCHEDULES[schedule], out.ctypes.data, C.byref(n), None,
+                None, None, None, _lib.stream_ptr()), "rmu_decoder_generate_assisted")
         return out[:n.value].tolist()
 
     def _sampling(self, do_sample, temperature, top_k, top_p, repetition_penalty, eos_token_ids) -> "_lib.SamplingC":
@@ -232,6 +268,10 @@ class DecoderAttention:
                 result += [out[b, :n[b]].tolist() for b in range(B)]
         return result
 
+
+# transformers' num_assistant_tokens_schedule -> rmu_decoder_generate_assisted's schedule; both heuristics move k
+# within one call (the assistant's config is not updated)
+ASSIST_SCHEDULES = {"constant": 0, "heuristic": 1, "heuristic_transient": 1}
 
 DECODER_WEIGHTS = ("split", "nf4")
 DECODER_WEIGHTS_ENV = "RMU_DECODER_WEIGHTS"
@@ -420,6 +460,8 @@ def compute_llm_provenance(tokenizer: Any, model: Any, query: str, context: Sequ
     max_new = settings.pop("max_new_tokens")
     settings.pop("prompt_lookup_num_tokens", None)     # the batched path does not draft; its tokens are the same
     settings.pop("max_matching_ngram_size", None)
+    for key in ("assistant_model", "num_assistant_tokens", "num_assistant_tokens_schedule"):
+        settings.pop(key, None)
     seeds = [int(torch.randint(0, 2 ** 63 - 1, (1,)).item()) for _ in prompts]
     new = dec.generate_batch(prompts, max_new, seeds, **settings)
     return [_llm_score(tokenizer, p, n) for p, n in zip(prompts, new)]

@@ -656,9 +656,21 @@ def synthetic_llama_weights(cfg: LlamaConfig, seed: int = 0, scale: float = 1.0)
 # llama-3.1-8b: Meta-Llama-3.1-8B-Instruct's shape [3P-recall: its config.json is not read here].
 # llama-3.1-70b: Llama-3.1-70B-Instruct's (and Llama-3.3-70B-Instruct's) shape, and qwen3-32b: Qwen3-32B's
 # [3P-recall: their config.json files are not read here]; both run in NF4 only (hidden above 4096).
+# Draft models for speculative decoding (DecoderAttention.generate's assistant), sharing their targets' vocabularies:
+# llama-3.2-3b: Llama-3.2-3B-Instruct's shape, tied embeddings and llama3 rope scaling factor 32, the draft of
+# Llama-3.1-8B / 70B and Llama-3.3-70B; qwen3-0.6b: Qwen3-0.6B's shape as a chat decoder (vocabulary 151936, tied
+# embeddings), the draft of Qwen3-8B / 14B / 32B [3P-recall: their config.json files are not read here].  A synthetic
+# preset's LM head is drawn on its own, so the tie only matters for snapshots (decoder_lm_head reads it there).
+# tiny-llama-draft: one layer, two query heads over one kv head, with tiny-llama's vocabulary and rope.
 DECODER_PRESETS: Dict[str, BertConfig] = {
     "tiny-llama": LlamaConfig(vocab_size=1000, hidden=256, layers=3, heads=4, ffn=384, max_pos=8192, kv_heads=2,
                               rope_theta=10000.0, rope_scaling=(8.0, 1.0, 4.0, 64)),
+    "tiny-llama-draft": LlamaConfig(vocab_size=1000, hidden=256, layers=1, heads=2, ffn=384, max_pos=8192, kv_heads=1,
+                                    rope_theta=10000.0, rope_scaling=(8.0, 1.0, 4.0, 64)),
+    "llama-3.2-3b": LlamaConfig(hidden=3072, layers=28, heads=24, ffn=8192, kv_heads=8,
+                                rope_scaling=(32.0, 1.0, 4.0, 8192)),
+    "qwen3-0.6b": Qwen3Config(vocab_size=151936, hidden=1024, layers=28, heads=16, ffn=3072, kv_heads=8,
+                              tie_word_embeddings=True, num_labels=1),
     "llama-3.1-8b": LlamaConfig(),
     "llama-3.1-70b": LlamaConfig(hidden=8192, layers=80, heads=64, ffn=28672),
     "qwen3-32b": Qwen3Config(vocab_size=151936, hidden=5120, layers=64, heads=64, ffn=25600, kv_heads=8,
